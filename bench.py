@@ -7,7 +7,7 @@ transformers, sampling) -> ``MimiModel.decode`` (8 codes -> PCM).  Sessions are 
 with N GPUs every rank runs a replica with its own shard of sessions (no data-path collective),
 so scaling is weak and ``value`` sums the sessions of all ranks.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--sessions B_per_gpu]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--sessions B_per_gpu] [--dump-outputs DIR]
 
 Prints ONE JSON line (rank 0).  See DESIGN.md "Measurement" for the definition of every field.
 """
@@ -41,7 +41,7 @@ def sessions_sustained(total_sessions: float, ms_per_step: float) -> float:
 
 
 # ---------------------------------------------------------------------------------------------
-# clocks (B200_PROFILING.md recipe)
+# clocks
 # ---------------------------------------------------------------------------------------------
 class ClockSampler:
     FIELDS = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
@@ -172,13 +172,13 @@ def reference_arm(args) -> None:
 
 
 # ---------------------------------------------------------------------------------------------
-# B200 arm
+# GPU arm
 # ---------------------------------------------------------------------------------------------
 def _peaks() -> tuple[float, str]:
     p = ROOT / "MEASURED_PEAKS.json"
     if p.exists():
         return float(json.loads(p.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 def _event_time(fn, iters: int = 10, warm: int = 3) -> float:
@@ -196,7 +196,7 @@ def _event_time(fn, iters: int = 10, warm: int = 3) -> float:
 
 def _dominant_kernel_roofline(B: int, kv_fill: int, device, fp8: int = 0) -> dict:
     """The dominant kernel of the step at serving batch is the temporal ring-attention decode (32 launches per
-    step, each streaming 2*B*32*fill*128 bf16 of K/V; profiles/ has its share of the step).  Timed here alone
+    step, each streaming 2*B*32*fill*128 bf16 of K/V).  Timed here alone
     with CUDA events on the launching stream, on K/V rings of the bench's own shape (4.7 GB at B=96: far
     larger than L2, so every launch streams from HBM), same split-KV configuration the LM uses."""
     import ctypes as C
@@ -233,25 +233,14 @@ def _dominant_kernel_roofline(B: int, kv_fill: int, device, fp8: int = 0) -> dic
     peak, src = _peaks()
     gbs = alg / (ms * 1e-3) / 1e9
     del k, v
-    # DRAM traffic of this kernel from the committed `ncu --set full` capture (profiles/attn_step_ncu.json: B = 96, full ring);
-    # the kernel reads every session's K/V exactly once, so bytes per launch scale with sessions x keys
-    traffic, traffic_src = None, None
-    cap_file = ROOT / "profiles" / "attn_step_ncu.json"
-    if cap_file.exists() and not fp8:
-        cap_d = json.loads(cap_file.read_text())
-        per_key_session = (cap_d["dram_bytes_read"] + cap_d["dram_bytes_write"]) / (cap_d["B"] * cap_d["keys"])
-        traffic = per_key_session * B * n_keys
-        traffic_src = ("ncu --set full at B=%d, %d keys (%s): dram read+write / launch scaled by sessions x keys"
-                       % (cap_d["B"], cap_d["keys"], cap_d["source"]))
-    return {"traffic": traffic, "traffic_source": traffic_src, "kernel": "lm::attn_step%s_kernel (RoPE + ring append + split-KV attention + merge), B=%d H=32 keys=%d D=128 %s" % (("", "_f8", "_i8")[fp8], B, n_keys, ("bf16", "e4m3 + fp32 scale per key", "int8 + fp32 scale per key")[fp8]),
+    return {"kernel": "lm::attn_step%s_kernel (RoPE + ring append + split-KV attention + merge), B=%d H=32 keys=%d D=128 %s" % (("", "_f8", "_i8")[fp8], B, n_keys, ("bf16", "e4m3 + fp32 scale per key", "int8 + fp32 scale per key")[fp8]),
             "bound": "hbm", "achieved": gbs, "peak": peak, "peak_source": src, "unit": "GB/s", "frac": gbs / peak,
-            "peak_note": "the measured peak is a device-to-device copy (half reads, half writes); this kernel is a pure read "
-                         "stream, which HBM3e serves slightly faster, so frac can exceed 1 (nominal 8 TB/s: %.2f)" % (gbs / 8000.0),
+            "peak_note": "fraction of %s; this kernel is a pure read stream" % src,
             "ms_per_launch": ms, "algorithmic_bytes": alg, "launches_per_step": 32}
 
 
 def _gemm_roofline(B: int, device) -> dict:
-    """Second kernel by time: the tcgen05 GEMM of the gated-MLP input projection (184.5 MB of weights) as the LM launches it at this
+    """Second kernel by time: the wgmma GEMM of the gated-MLP input projection (184.5 MB of weights) as the LM launches it at this
     batch size (non-swapped N = 256 kernel for 33..256 sessions, swap-AB stream-K otherwise)."""
     import ctypes as C
     from moshi_b200 import _lib
@@ -393,6 +382,18 @@ def _kv_fill_sweep(lm, mimi, device, free_bytes: int, fills=(2250, 1500, 750), s
     return out
 
 
+def _dump_outputs(out_dir: str, last) -> None:
+    """What the timed step returned in its last iteration: the sampled tokens [B, 9, 1] (text + 8 audio; -1 while the
+    delays are still filling, as float64) and the decoded PCM [B, 1, 1920] (float32), one .npy file each."""
+    import numpy as np
+    toks, pcm = last
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    if toks is not None:
+        np.save(d / "tokens.npy", toks.detach().cpu().double().numpy())
+    np.save(d / "pcm.npy", pcm.detach().float().cpu().numpy())
+
+
 def b200_arm(args) -> None:
     from moshi_b200 import _lib
     from moshi_b200.config import MOSHI_7B
@@ -400,6 +401,7 @@ def b200_arm(args) -> None:
     from moshi_b200.serving import DialogueService, barrier, init_distributed, max_over_ranks, sum_over_ranks
 
     rank, world = init_distributed()
+    torch.manual_seed(1234 + rank)      # seeds the sessions' sampling noise: the same arguments give the same outputs
     local = int(os.environ.get("LOCAL_RANK", "0"))
     device = torch.device("cuda", local)
     torch.cuda.set_device(device)
@@ -411,7 +413,7 @@ def b200_arm(args) -> None:
     lm = loaders.get_moshi_lm(None, lm_kwargs, device=device, synth_device=device)
     torch.cuda.synchronize(device)
 
-    # sessions per GPU: the full-context bf16 KV ring (1.573 GB/session) is what bounds it
+    # sessions per GPU: the full-context bf16 KV ring (1.573 GB/session) is what bounds it (about 35 in 80 GB)
     free, total = torch.cuda.mem_get_info(device)
     fp8 = {"bf16": 0, "fp8_e4m3": 1, "int8": 2}[args.kv_dtype]
     kv_step = (32 * 2 * (4096 + 32 * 4)) if fp8 else KV_BYTES_PER_SESSION_STEP     # e4m3 bytes + one fp32 scale per head
@@ -457,11 +459,13 @@ def b200_arm(args) -> None:
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
             for i in range(args.steps):
-                frame(pcm_dev[i % n_buf], timed_lm=True)
+                last = frame(pcm_dev[i % n_buf], timed_lm=True)
             e1.record()
             torch.cuda.synchronize(device)
             barrier()
         launches = lib.b200_launch_count() - launches0
+        if args.dump_outputs and rank == 0:
+            _dump_outputs(args.dump_outputs, last)
         ms_dev = max_over_ranks(e0.elapsed_time(e1) / args.steps)
         lm_ms = sum(a.elapsed_time(b) for a, b in lm_ev) / len(lm_ev)
 
@@ -493,7 +497,7 @@ def b200_arm(args) -> None:
     peak, peak_src = _peaks()
     roof = gemm_roof = None
     if rank == 0:
-        # release the sessions' state (150+ GB of KV rings) before allocating the stand-alone kernel operands
+        # release the sessions' state (most of HBM is KV rings) before allocating the stand-alone kernel operands
         svc.close()
         torch.cuda.empty_cache()
         roof = _dominant_kernel_roofline(B, kv_fill, device, fp8)
@@ -548,7 +552,7 @@ def b200_arm(args) -> None:
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--steps", type=int, default=20, help="timed steps")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", choices=["b200", "reference"], default="b200")
     ap.add_argument("--sessions", type=int, default=0, help="sessions per GPU (default: as many as the full-context bf16 KV rings fit in HBM)")
@@ -559,6 +563,9 @@ def main() -> None:
                     help="storage of the temporal KV rings; fp8_e4m3 / int8 are opt-in extensions outside the reference's numerics "
                          "(half the ring, twice the sessions per GPU; logit error in tests/test_gpu_zv_kv_q8.py)")
     ap.add_argument("--quantize", action="store_true", help="BASELINE config 5: int8 (W8A8 QLinear) Moshi 7B instead of bf16")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's tokens and PCM as DIR/<name>.npy (seeded inputs: "
+                         "two builds run with the same arguments can be compared output for output)")
     args = ap.parse_args()
     if args.impl == "reference":
         reference_arm(args)

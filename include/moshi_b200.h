@@ -1,5 +1,5 @@
 /*
- * moshi_b200 — C ABI of the B200-native (sm_100a) streaming inference path for
+ * moshi_b200 — C ABI of the H100-native (sm_90a) streaming inference path for
  * Mimi (SEANet + transformer bottleneck + split RVQ) and the Moshi LM decode step.
  *
  * The reference (kyutai-labs/moshi) has no native boundary on this path: its Python classes call
@@ -325,10 +325,10 @@ int b200_frame_read_buffer(b200_frame* f, const char* name, void* dst_dev, int64
 /* ------------------------------------------------------------------------------------------ */
 
 /* y[M,N] = x[M,K] * w[N,K]^T, bf16 in, fp32 accumulate, bf16 out, on row-major weights: packs them into tiles and runs
- * the LM's linear for this shape (GEMV kernel up to 2 rows, tcgen05 stream-K / whole-tile / cluster split-K kernels above);
+ * the LM's linear for this shape (GEMV kernel up to 2 rows, wgmma stream-K / whole-tile / cluster split-K kernels above);
  * synchronises the stream (test helper).  Reference op: every nn.Linear of the LM (transformer.py:304-305,554-555,588-589). */
 int b200_op_linear_bf16(const void* x_dev, const void* w_dev, void* y_dev, int M, int N, int K, void* stream);
-/* Stream-K tcgen05 GEMM over pre-tiled weights (the LM's linear kernel; csrc/gemm_sk.cu).
+/* Stream-K wgmma GEMM over pre-tiled weights (the LM's linear kernel; csrc/gemm_sk.cu).
  *   b200_op_packed_bytes / b200_op_pack_tiles: repack w bf16 [N,K] (epi 2: [2*gate_rows,K], rows gate|value,
  *   gating.py:18-20) into 16 KB SWIZZLE_128B tiles.
  *   b200_op_linear_sk: y = epi(x . W^T); epi 0 store [M,N], 1 residual add (y = res + .), 2 silu(gate)*value
@@ -337,8 +337,8 @@ int64_t b200_op_packed_bytes(int N, int K, int epi, int gate_rows);
 int b200_op_pack_tiles(const void* w_dev, void* out_dev, int N, int K, int epi, int gate_rows, void* stream);
 int b200_op_linear_sk(const void* x_dev, const void* w_tiles_dev, void* y_dev, const void* res_dev, int M, int N,
                       int K, int epi, int gate_rows, int grid, int smem_budget, int stream_only, void* stream);
-/* The LM's linear kernel for 33..256 sessions (csrc/gemm_ns.cu): activations as the UMMA A operand, two pre-tiled weight tiles
- * as B (N = 256 per tcgen05.mma), K cut over a cluster of `cluster` CTAs and reduced over distributed shared memory
+/* The LM's linear kernel for 33..256 sessions (csrc/gemm_ns.cu): activations as the wgmma A operand, two pre-tiled weight tiles
+ * as B (N = 256 per wgmma), K cut over a cluster of `cluster` CTAs and reduced over distributed shared memory
  * (0 = the LM's own choice; 100 + n = single-tile units, N = 128 per instruction, n K-splits); same packed weights and
  * epilogues as b200_op_linear_sk, any M <= 256.
  * (b200_op_linear_sk with smem_budget = -1 keeps the swap-AB kernels at every M: the comparison row of tools/kbench.py.) */
@@ -348,7 +348,7 @@ int b200_op_linear_ns(const void* x_dev, const void* w_tiles_dev, void* y_dev, c
  * tensor-core GEMM; csrc/gemm_sk.cu): 0..4, default 2 (or B200_GEMV_MAX_M).  Returns the previous value. */
 int b200_op_set_gemv_max_rows(int max_rows);
 /* int8 x int8 linear (QLinear, utils/quantize.py:13-40: bitsandbytes row-wise absmax quantisation of weights and
- * activations, int32 accumulation, dequantisation by both row scales / 127^2), on tcgen05 kind::i8.
+ * activations, int32 accumulation, dequantisation by both row scales / 127^2), on wgmma s8 x s8 -> s32.
  *   b200_op_quant_pack_tiles: w bf16 [N,K] -> int8 SWIZZLE_128B tiles (b200_op_packed_bytes_i8 bytes) + scales f32 [N]
  *   b200_op_quantize_rows:    x bf16 [M,K] -> xq int8 [M,K] + scales f32 [M]
  *   b200_op_linear_i8:        y bf16 = epi(dequant(xq . Wq^T)), epilogues as b200_op_linear_sk */
@@ -363,7 +363,7 @@ int b200_op_linear_i8(const void* xq_dev, const float* sa_dev, const void* w_til
 int b200_op_conv1d(const float* x_dev, const float* w_dev, const float* bias_dev, float* prev_dev,
                    const uint8_t* exec_mask_dev, float* y_dev, int B, int Cin, int Cout, int T,
                    int K, int stride, int dilation, int elu_in, void* stream);
-/* mimi_tc_kernel (TMA + tcgen05 kind::tf32, 3xTF32 split products: fp32-equivalent accuracy) on the reference's layouts;
+/* mimi_tc_kernel (TMA + wgmma tf32, 3xTF32 split products: fp32-equivalent accuracy) on the reference's layouts;
  * test scaffolding around the kernel the Mimi handle launches for every conv / convtr / linear (the handle itself keeps all
  * activations token-major and never transposes).
  *   b200_op_tc_linear_f32: y[M,N] = x[M,K] . w[N,K]^T  (K % 32 == 0, N % 16 == 0)

@@ -1,4 +1,4 @@
-"""moshi_b200 — B200-native (sm_100a) streaming inference path for Mimi + the Moshi LM decode step.
+"""moshi_b200 — H100-native (sm_90a) streaming inference path for Mimi + the Moshi LM decode step.
 
 Public surface mirrors the reference package on this path::
 

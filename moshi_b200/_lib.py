@@ -1,6 +1,6 @@
 """ctypes binding of ``include/moshi_b200.h``.
 
-There is no CPU fallback: if the sm_100a library has not been built, importing a model class raises
+There is no CPU fallback: if the sm_90a library has not been built, importing a model class raises
 with the build command.  ``__graft_entry__.build()`` / ``python -m moshi_b200.build`` produce it
 in-tree (``moshi_b200/_C/libmoshi_b200.so``).
 """
@@ -149,8 +149,8 @@ def lib() -> C.CDLL:
     if _lib is None:
         if not LIB_PATH.exists():
             raise RuntimeError(
-                f"{LIB_PATH} is missing: the B200 path has no CPU fallback. Build it with "
-                "`python -m moshi_b200.build` (needs nvcc; cross-compiles for sm_100a).")
+                f"{LIB_PATH} is missing: the GPU path has no CPU fallback. Build it with "
+                "`python -m moshi_b200.build` (needs nvcc; cross-compiles for sm_90a).")
         handle = C.CDLL(str(LIB_PATH))
         for name, (res, args) in _PROTOTYPES.items():
             fn = getattr(handle, name)

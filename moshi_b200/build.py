@@ -1,4 +1,4 @@
-"""Builds ``moshi_b200/_C/libmoshi_b200.so`` in-tree with nvcc for sm_100a (cross-compiles on a CPU box)."""
+"""Builds ``moshi_b200/_C/libmoshi_b200.so`` in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import hashlib
@@ -14,7 +14,7 @@ OUT_DIR = HERE / "_C"
 LIB = OUT_DIR / "libmoshi_b200.so"
 SOURCES = ["common.cu", "mimi.cu", "lm.cu", "ops.cu", "gemm_sk.cu", "gemm_ns.cu", "dep_fused.cu", "frame.cu", "mimi_tc.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v",
 ]
 
@@ -23,7 +23,7 @@ def _nvcc() -> str:
     for cand in (os.environ.get("NVCC"), shutil.which("nvcc"), "/usr/local/cuda/bin/nvcc"):
         if cand and Path(cand).exists():
             return cand
-    raise RuntimeError("nvcc not found; cannot build the sm_100a extension")
+    raise RuntimeError("nvcc not found; cannot build the sm_90a extension")
 
 
 def _digest(files: list[Path]) -> str:
@@ -59,7 +59,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
         objs.append(str(obj))
     if failed:
         raise RuntimeError(f"nvcc failed on {failed}")
-    cmd = [nvcc, "-shared", "-o", str(LIB), *objs, "-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [nvcc, "-shared", "-o", str(LIB), *objs, "-gencode", "arch=compute_90a,code=sm_90a"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         sys.stderr.write(r.stdout + r.stderr)

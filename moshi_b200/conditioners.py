@@ -143,7 +143,7 @@ class ConditionFuser:
         assert all(k in self.FUSING_METHODS for k in fuse2cond), f"Got invalid fuse method, allowed methods: {self.FUSING_METHODS}"
         self.fuse2cond = {k: list(fuse2cond.get(k, [])) for k in self.FUSING_METHODS}
         if self.fuse2cond["cross"] or self.fuse2cond["prepend"]:
-            raise ValueError("cross-attention / prepend conditioning is outside the B200 hot path (SURVEY.md 8f)")
+            raise ValueError("cross-attention / prepend conditioning is outside the GPU hot path (SURVEY.md 8f)")
 
     @property
     def has_conditions(self) -> bool:

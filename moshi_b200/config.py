@@ -93,7 +93,7 @@ class MimiConfig:
         if not tr.get("conv_layout", True):
             unsupported.append("transformer.conv_layout=False")
         if unsupported:
-            raise ValueError(f"Mimi options outside the B200 hot path: {unsupported}")
+            raise ValueError(f"Mimi options outside the GPU hot path: {unsupported}")
         return MimiConfig(
             sample_rate=cfg["sample_rate"], frame_rate=cfg["frame_rate"], channels=cfg["channels"],
             dimension=sea["dimension"], n_filters=sea["n_filters"],
@@ -197,7 +197,7 @@ class LMConfig:
         known = {f.name for f in dataclasses.fields(LMConfig)}
         extra = sorted(set(d) - known)
         if extra:
-            raise ValueError(f"LM options outside the B200 hot path: {extra}")
+            raise ValueError(f"LM options outside the GPU hot path: {extra}")
         cfg = LMConfig(**d)
         cfg.check_supported()
         return cfg
@@ -245,7 +245,7 @@ class LMConfig:
         if self.quantize and any(k % 16 for k in (self.dim, self.ffn_hidden, self.depformer_dim, self.depformer_ffn_hidden)):
             bad.append("quantize (int8 k-extents must be multiples of 16)")
         if bad:
-            raise ValueError(f"LM options outside the B200 hot path: {bad}")
+            raise ValueError(f"LM options outside the GPU hot path: {bad}")
 
 
 def _gated_hidden(dim: int, dim_feedforward: int) -> int:

@@ -1,4 +1,4 @@
-// Shared helpers for the moshi_b200 CUDA library (sm_100a only).
+// Shared helpers for the moshi_b200 CUDA library (sm_90a only).
 #pragma once
 
 #include <cuda_bf16.h>

@@ -7,7 +7,7 @@
 // grid barriers (all CTAs are co-resident: cooperative launch, 1 CTA/SM by shared-memory size, grid <= #SMs):
 //
 //   per sub-step k:   [row phase]   x = depformer_in[k](transformer_out) + emb_k(prev token); xn = rmsnorm(x)
-//     per layer l:    [GEMM]        in_proj partials            (tcgen05, split-K units over all CTAs)
+//     per layer l:    [GEMM]        in_proj partials            (wgmma, split-K units over all CTAs)
 //                     [warp phase]  q,k,v = bf16(sum partials); KV append; attention over k+1 keys -> ao
 //                     [GEMM]        out_proj partials
 //                     [row phase]   x = bf16(x + bf16(sum)); xn = rmsnorm(x)
@@ -20,8 +20,9 @@
 //                     [row phase]   logits = bf16(sum) ; token = sample(logits) ; next sub-step's input row
 //
 // GEMM phases use the same machinery as gemm_sk.cu (pre-tiled SWIZZLE_128B weights streamed by cp.async.bulk, the
-// activation box by 2-D TMA, single-thread tcgen05.mma into TMEM, tcgen05.ld epilogue); a unit = (128-row weight
-// tile, k-split) and every unit writes its fp32 partial [M x 128] to an L2-resident workspace; the consumer phase
+// activation box by 2-D TMA, wgmma into register accumulators of one consumer warpgroup, epilogue from the fragments); a
+// unit = (128-row weight tile, k-split, block of 64 sessions) and every unit writes its fp32 partial [64 x 128] to an
+// L2-resident workspace; the consumer phase
 // sums the splits in split order (deterministic, independent of the batch) and applies the reference's cast points.
 #include "gemm_sk.cuh"
 #include "tc_prims.cuh"
@@ -35,7 +36,8 @@ namespace {
 using lm::bf16;
 
 constexpr int BLOCK_ROWS = 128, BLOCK_K = 64, UMMA_K = 16;
-constexpr int THREADS = 256;                 // warp 0 producer, 1 MMA, 2-5 epilogue, 6-7 extra hands in the SIMT phases
+constexpr int THREADS = 256;                 // GEMM phases: warp 0 producer, warps 4-7 the consumer warpgroup; all in the SIMT phases
+constexpr int MC = 64;                       // sessions per GEMM unit (wgmma N): the warpgroup holds 128 rows x MC x 2 accumulators
 constexpr int TILE_BYTES = BLOCK_ROWS * BLOCK_K * 2;
 constexpr int MAX_STAGES = 8;
 constexpr int DD = 64;                       // depformer head dim
@@ -59,7 +61,7 @@ struct DepLayerW { const uint8_t *in_w, *out_w, *lin_in, *lin_out; };
 struct DepParams {
   int B, Mpad, dd, H, F, card, text_card, dep_q, L, n_tables;
   int* err;                                                  // device error flags (lm::ERR_*)
-  int stages; uint32_t stage_bytes, tmem_cols, acc_cols; int n_acc;
+  int stages; uint32_t stage_bytes;
   Gemm g_in, g_out, g_lin_in, g_lin_out, g_head;              // shapes (wt filled per (k, l) from the tables below)
   const DepLayerW* w;                                        // [dep_q][L] packed weight pointers (device)
   const uint8_t* const* heads;                               // [dep_q]
@@ -80,7 +82,7 @@ struct DepParams {
 
 namespace {
 
-struct Pipe { int s; uint32_t ph; int acc; uint32_t acc_bits; int pre; };   // per-role pipeline cursor, carried across phases
+struct Pipe { int s; uint32_t ph; int pre; };   // per-role pipeline cursor, carried across phases
 // (pre: producer only — stages of the upcoming GEMM phase whose weight copy is already in flight)
 
 // Grid barrier: one release-reduction per CTA and acquire polling by one thread (all CTAs are co-resident).
@@ -240,20 +242,31 @@ __device__ void sample_phase(const DepParams& p, int S, int k) {
   }
 }
 
-// One GEMM phase: units u = blockIdx.x, += gridDim.x; unit = (tile, split); partial [M x 128] -> part[split][m][tile*128 + row]
+// One GEMM phase: units u = blockIdx.x, += gridDim.x; unit = (tile, split, block of MC sessions), the session block fastest
+// (the CTAs that share a weight slice run side by side, so all but the first read it from L2);
+// partial [MC x 128] -> part[split][m][tile*128 + row]
+__device__ __forceinline__ void unit_at(const Gemm& g, int mch, int u, int& tile, int& sp, int& mc) {
+  mc = u % mch;
+  const int ts = u / mch;
+  tile = ts / g.S;
+  sp = ts - tile * g.S;
+}
+
 template <class P>
 __device__ void gemm_phase(const P& p, const Gemm& g, const Gemm* next, const CUtensorMap* xmap, uint32_t base, uint32_t full0,
-                           uint32_t empty0, uint32_t tfull0, uint32_t tempty0, uint32_t tmem_base, Pipe& pipe) {
+                           uint32_t empty0, Pipe& pipe) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int units = g.n_tiles * g.S;
+  const int mch = (p.B + MC - 1) / MC;
+  const int units = g.n_tiles * g.S * mch;
   const uint32_t a_bytes = (uint32_t)g.A * TILE_BYTES;
-  const uint32_t x_bytes = (uint32_t)p.Mpad * BLOCK_K * 2;
+  constexpr uint32_t x_bytes = (uint32_t)MC * BLOCK_K * 2;
   if (warp == 0) {
     if (lane == 0) {
       asm volatile("fence.proxy.async;" ::: "memory");        // activations were written with generic stores by other CTAs
       int item = 0;
       for (int u = blockIdx.x; u < units; u += gridDim.x) {
-        const int tile = u / g.S, sp = u - tile * g.S;
+        int tile, sp, mc;
+        unit_at(g, mch, u, tile, sp, mc);
         const int kb0 = sp * g.kbps, kb1 = min(g.num_kb, kb0 + g.kbps);
         const uint8_t* src = g.wt + ((size_t)tile * g.num_kb + kb0) * a_bytes;
         for (int kb = kb0; kb < kb1; ++kb, src += a_bytes, ++item) {
@@ -263,7 +276,7 @@ __device__ void gemm_phase(const P& p, const Gemm& g, const Gemm* next, const CU
             mbar_expect_tx(full0 + 8 * pipe.s, a_bytes + x_bytes);
             bulk_load(sa, src, a_bytes, full0 + 8 * pipe.s);
           }
-          tma_load_2d(sa + 2 * TILE_BYTES, xmap, full0 + 8 * pipe.s, kb * BLOCK_K, 0);
+          tma_load_2d(sa + 2 * TILE_BYTES, xmap, full0 + 8 * pipe.s, kb * BLOCK_K, mc * MC);
           if (++pipe.s == p.stages) { pipe.s = 0; pipe.ph ^= 1u; }
         }
       }
@@ -273,9 +286,10 @@ __device__ void gemm_phase(const P& p, const Gemm& g, const Gemm* next, const CU
       if (next != nullptr) {
         const uint32_t nb = (uint32_t)next->A * TILE_BYTES;
         int s2 = pipe.s; uint32_t ph2 = pipe.ph;
-        const int nunits = next->n_tiles * next->S;
+        const int nunits = next->n_tiles * next->S * mch;
         for (int u = blockIdx.x; u < nunits && pipe.pre < p.stages; u += gridDim.x) {
-          const int tile = u / next->S, sp = u - tile * next->S;
+          int tile, sp, mc;
+          unit_at(*next, mch, u, tile, sp, mc);
           const int kb0 = sp * next->kbps, kb1 = min(next->num_kb, kb0 + next->kbps);
           const uint8_t* src = next->wt + ((size_t)tile * next->num_kb + kb0) * nb;
           for (int kb = kb0; kb < kb1 && pipe.pre < p.stages; ++kb, src += nb, ++pipe.pre) {
@@ -287,69 +301,56 @@ __device__ void gemm_phase(const P& p, const Gemm& g, const Gemm* next, const CU
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc(BLOCK_ROWS, p.Mpad);
-      for (int u = blockIdx.x; u < units; u += gridDim.x) {
-        const int tile = u / g.S, sp = u - tile * g.S;
-        const int kb0 = sp * g.kbps, kb1 = min(g.num_kb, kb0 + g.kbps);
-        mbar_wait(tempty0 + 8 * pipe.acc, ((pipe.acc_bits >> pipe.acc) & 1u) ^ 1u);
-        tc_fence_after();
-        const uint32_t d0 = tmem_base + (uint32_t)(pipe.acc * p.acc_cols);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(full0 + 8 * pipe.s, pipe.ph);
-          tc_fence_after();
-          const uint32_t sa = base + (uint32_t)pipe.s * p.stage_bytes;
-          const uint32_t sb = sa + 2 * TILE_BYTES;
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-            const uint64_t db = make_desc(sb + k * UMMA_K * 2);
-            const uint32_t accum = (kb == kb0 && k == 0) ? 0u : 1u;
-            umma_bf16(d0, make_desc(sa + k * UMMA_K * 2), db, idesc, accum);
-            if (g.A == 2) umma_bf16(d0 + (uint32_t)p.Mpad, make_desc(sa + TILE_BYTES + k * UMMA_K * 2), db, idesc, accum);
-          }
-          umma_commit(empty0 + 8 * pipe.s);
-          if (++pipe.s == p.stages) { pipe.s = 0; pipe.ph ^= 1u; }
-        }
-        umma_commit(tfull0 + 8 * pipe.acc);
-        pipe.acc_bits ^= 1u << pipe.acc;
-        if (p.n_acc == 2) pipe.acc ^= 1;
-      }
-    }
-    __syncwarp();
-  } else if (warp < 6) {
-    const int q = warp & 3;                    // TMEM lane quadrant this warp may access
-    const int row = q * 32 + lane;
+  } else if (warp >= 4) {
+    // the consumer warpgroup: weight rows 0..63 and 64..127 of the tile (h), one accumulator per weight tile (a)
+    const int t = threadIdx.x & 127;
     for (int u = blockIdx.x; u < units; u += gridDim.x) {
-      const int tile = u / g.S, sp = u - tile * g.S;
-      const int n = tile * BLOCK_ROWS + row;
-      mbar_wait(tfull0 + 8 * pipe.acc, (pipe.acc_bits >> pipe.acc) & 1u);
-      tc_fence_after();
-      const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(pipe.acc * p.acc_cols);
-      float* o0 = p.part0 + (long long)sp * p.B * g.N + n;
-      float* o1 = p.part1 + (long long)sp * p.B * g.N + n;
-      for (int c0 = 0; c0 < p.Mpad; c0 += 16) {
-        if (c0 >= p.B) break;
-        uint32_t r0[16], r1[16];
-        tmem_ld16(lane_addr + (uint32_t)c0, r0);
-        if (g.A == 2) tmem_ld16(lane_addr + (uint32_t)(p.Mpad + c0), r1);
-        tmem_ld_wait();
-        if (n < g.N) {
+      int tile, sp, mc;
+      unit_at(g, mch, u, tile, sp, mc);
+      const int kb0 = sp * g.kbps, kb1 = min(g.num_kb, kb0 + g.kbps);
+      uint32_t d00[MC / 2], d01[MC / 2], d10[MC / 2], d11[MC / 2];    // d<h><a>
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(full0 + 8 * pipe.s, pipe.ph);
+        const uint32_t sa = base + (uint32_t)pipe.s * p.stage_bytes;
+        const uint32_t sb = sa + 2 * TILE_BYTES;
+        wg_fence();
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const int m = c0 + j;
-            if (m < p.B) {
-              __stcg(o0 + (long long)m * g.N, __uint_as_float(r0[j]));
-              if (g.A == 2) __stcg(o1 + (long long)m * g.N, __uint_as_float(r1[j]));
-            }
+        for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
+          const uint64_t db = make_desc(sb + k * UMMA_K * 2);
+          const uint32_t accum = (kb == kb0 && k == 0) ? 0u : 1u;
+          const uint32_t a0 = sa + k * UMMA_K * 2;
+          Wgmma<MC>::bf16(d00, make_desc(a0), db, accum);
+          Wgmma<MC>::bf16(d10, make_desc(a0 + TILE_BYTES / 2), db, accum);
+          if (g.A == 2) {
+            Wgmma<MC>::bf16(d01, make_desc(a0 + TILE_BYTES), db, accum);
+            Wgmma<MC>::bf16(d11, make_desc(a0 + TILE_BYTES + TILE_BYTES / 2), db, accum);
+          }
+        }
+        wg_commit();
+        wg_wait<0>();
+        wg_hold(d00); wg_hold(d10);
+        if (g.A == 2) { wg_hold(d01); wg_hold(d11); }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty0 + 8 * pipe.s);
+        if (++pipe.s == p.stages) { pipe.s = 0; pipe.ph ^= 1u; }
+      }
+      float* o0 = p.part0 + (long long)sp * p.B * g.N;
+      float* o1 = p.part1 + (long long)sp * p.B * g.N;
+#pragma unroll
+      for (int i = 0; i < MC / 2; ++i) {
+        const int m = mc * MC + frag_col(t, i);
+        const int n0 = tile * BLOCK_ROWS + frag_row(t, i), n1 = n0 + 64;
+        if (m < p.B) {
+          if (n0 < g.N) {
+            __stcg(o0 + (long long)m * g.N + n0, __uint_as_float(d00[i]));
+            if (g.A == 2) __stcg(o1 + (long long)m * g.N + n0, __uint_as_float(d01[i]));
+          }
+          if (n1 < g.N) {
+            __stcg(o0 + (long long)m * g.N + n1, __uint_as_float(d10[i]));
+            if (g.A == 2) __stcg(o1 + (long long)m * g.N + n1, __uint_as_float(d11[i]));
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty0 + 8 * pipe.acc);
-      pipe.acc_bits ^= 1u << pipe.acc;
-      if (p.n_acc == 2) pipe.acc ^= 1;
     }
   }
 }
@@ -362,9 +363,7 @@ dep_fused_kernel(const __grid_constant__ CUtensorMap map_xn, const __grid_consta
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
   const uint32_t bars = base + (uint32_t)p.stages * p.stage_bytes;
-  const uint32_t full0 = bars, empty0 = bars + 8 * MAX_STAGES, tfull0 = bars + 16 * MAX_STAGES, tempty0 = tfull0 + 16;
-  const uint32_t tptr = tempty0 + 16;
-  uint32_t* tptr_generic = reinterpret_cast<uint32_t*>(smem_raw + (tptr - raw));
+  const uint32_t full0 = bars, empty0 = bars + 8 * MAX_STAGES;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (warp == 0 && lane == 0) {
@@ -374,21 +373,13 @@ dep_fused_kernel(const __grid_constant__ CUtensorMap map_xn, const __grid_consta
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_x) : "memory");
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(full0 + 8 * s, 1);
-      mbar_init(empty0 + 8 * s, 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull0 + 8 * a, 1);
-      mbar_init(tempty0 + 8 * a, 4);
+      mbar_init(empty0 + 8 * s, 4);          // one arrival per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) tmem_alloc(tptr, p.tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tptr_generic;
 
-  Pipe pipe{0, 0u, 0, 0u, 0};
+  Pipe pipe{0, 0u, 0};
   unsigned epoch = 0;
   if (p.trace != nullptr && blockIdx.x == 0 && threadIdx.x == 0) p.trace[0] = global_timer_ns();
   // GEMM phases in execution order: per sub-step k, per layer l: in_proj, out_proj, linear_in, linear_out; then the head
@@ -409,22 +400,22 @@ dep_fused_kernel(const __grid_constant__ CUtensorMap map_xn, const __grid_consta
     grid_sync(p.bar, epoch, p.trace);
     for (int l = 0; l < p.L; ++l) {
       Gemm nxt = gemm_at(k, l, 1);
-      gemm_phase(p, cur, &nxt, &map_xn, base, full0, empty0, tfull0, tempty0, tmem_base, pipe);
+      gemm_phase(p, cur, &nxt, &map_xn, base, full0, empty0, pipe);
       grid_sync(p.bar, epoch, p.trace);
       attn_phase(p, cur.S, l, k);
       grid_sync(p.bar, epoch, p.trace);
       cur = nxt; nxt = gemm_at(k, l, 2);
-      gemm_phase(p, cur, &nxt, &map_ao, base, full0, empty0, tfull0, tempty0, tmem_base, pipe);
+      gemm_phase(p, cur, &nxt, &map_ao, base, full0, empty0, pipe);
       grid_sync(p.bar, epoch, p.trace);
       row_phase<4>(p, p.dd, cur.S, p.part0, cur.N, true, p.n2[l], red);
       grid_sync(p.bar, epoch, p.trace);
       cur = nxt; nxt = gemm_at(k, l, 3);
-      gemm_phase(p, cur, &nxt, &map_xn, base, full0, empty0, tfull0, tempty0, tmem_base, pipe);
+      gemm_phase(p, cur, &nxt, &map_xn, base, full0, empty0, pipe);
       grid_sync(p.bar, epoch, p.trace);
       gate_phase(p, cur.S);
       grid_sync(p.bar, epoch, p.trace);
       cur = nxt; nxt = l + 1 < p.L ? gemm_at(k, l + 1, 0) : gemm_at(k, 0, 4);
-      gemm_phase(p, cur, &nxt, &map_h, base, full0, empty0, tfull0, tempty0, tmem_base, pipe);
+      gemm_phase(p, cur, &nxt, &map_h, base, full0, empty0, pipe);
       grid_sync(p.bar, epoch, p.trace);
       // depformer_norms is Identity (lm.py:197-198): after the last layer the head reads x itself
       row_phase<4>(p, p.dd, cur.S, p.part0, cur.N, true, l + 1 < p.L ? p.n1[l + 1] : nullptr, red);
@@ -433,14 +424,11 @@ dep_fused_kernel(const __grid_constant__ CUtensorMap map_xn, const __grid_consta
     }
     const bool last = k + 1 == p.dep_q;
     Gemm nxt = last ? cur : gemm_at(k + 1, 0, 0);
-    gemm_phase(p, cur, last ? nullptr : &nxt, &map_x, base, full0, empty0, tfull0, tempty0, tmem_base, pipe);
+    gemm_phase(p, cur, last ? nullptr : &nxt, &map_x, base, full0, empty0, pipe);
     grid_sync(p.bar, epoch, p.trace);
     sample_phase(p, cur.S, k);       // the next sub-step's input rows are the same rows of the same CTA: no barrier needed
     cur = nxt;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, p.tmem_cols);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -512,16 +500,11 @@ int dep_fused_create(const DepFusedConfig& c, DepFused** out) {
   memset(&p, 0, sizeof(p));
   d->grid = sk_num_sms();
   p.B = c.B; p.Mpad = ((c.B + 15) / 16) * 16; p.dd = c.dd; p.H = c.H; p.F = c.F; p.card = c.card; p.text_card = c.text_card; p.err = c.err; p.dep_q = c.dep_q; p.L = c.L;
-  p.stage_bytes = (uint32_t)(2 * TILE_BYTES + p.Mpad * BLOCK_K * 2);
+  p.stage_bytes = (uint32_t)(2 * TILE_BYTES + MC * BLOCK_K * 2);
   int stages = (200 * 1024) / (int)p.stage_bytes;
   if (stages > MAX_STAGES) stages = MAX_STAGES;
   if (stages < 2) { delete d; B200_FAIL(B200_ERR_INVALID, "fused depformer: batch too large for the stage ring"); }
   p.stages = stages;
-  p.acc_cols = 2 * p.Mpad;
-  p.n_acc = 2 * p.acc_cols <= 512 ? 2 : 1;
-  uint32_t cols = (uint32_t)(p.n_acc * p.acc_cols), pow2 = 32;
-  while (pow2 < cols) pow2 <<= 1;
-  p.tmem_cols = pow2;
   p.g_in = plan(3 * c.dd, c.dd, 1, c.B, d->grid);
   p.g_out = plan(c.dd, c.dd, 1, c.B, d->grid);
   p.g_lin_in = plan(c.F, c.dd, 2, c.B, d->grid);
@@ -561,10 +544,10 @@ int dep_fused_create(const DepFusedConfig& c, DepFused** out) {
   p.noise = c.noise; p.noise_ld = c.noise_ld; p.noise_off = c.noise_off; p.ka = c.ka;
   p.use_sampling = c.use_sampling; p.top_k = c.top_k; p.temp = c.temp;
   p.bar = c.bar; p.trace = c.trace;
-  B200_TRY(make_map(enc, &d->map_xn, c.xn, c.B, c.dd, p.Mpad));
-  B200_TRY(make_map(enc, &d->map_ao, c.ao, c.B, c.dd, p.Mpad));
-  B200_TRY(make_map(enc, &d->map_h, c.hbuf, c.B, c.F, p.Mpad));
-  B200_TRY(make_map(enc, &d->map_x, c.x, c.B, c.dd, p.Mpad));
+  B200_TRY(make_map(enc, &d->map_xn, c.xn, c.B, c.dd, MC));
+  B200_TRY(make_map(enc, &d->map_ao, c.ao, c.B, c.dd, MC));
+  B200_TRY(make_map(enc, &d->map_h, c.hbuf, c.B, c.F, MC));
+  B200_TRY(make_map(enc, &d->map_x, c.x, c.B, c.dd, MC));
   d->smem = (size_t)stages * p.stage_bytes + 1024 + 16 * MAX_STAGES + 64;
   B200_CUDA(cudaFuncSetAttribute(dep_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
   int per_sm = 0, coop = 0, dev = 0;

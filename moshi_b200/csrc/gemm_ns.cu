@@ -1,22 +1,21 @@
-// tcgen05 GEMM for the LM linears at 33..256 sessions:  y[M][N] = epi(x[M][K] . w[N][K]^T), bf16 in, fp32 in TMEM, bf16 out.
+// wgmma GEMM for the LM linears at 33..256 sessions:  y[M][N] = epi(x[M][K] . w[N][K]^T), bf16 in, fp32 in registers, bf16 out.
 //
-// gemm_sk.cu feeds the 128-row weight tile as the UMMA *A* operand and the sessions as N ("swap-AB"): right while the batch is
-// tiny, but a tcgen05.mma with M = 128 occupies the tensor pipe for ~120-140 cycles whatever N <= 128 is (measured: the stream-K
-// kernel runs the same copy pipeline 1.8x slower with its MMAs switched on than with them off, and cuBLAS beats it on every LM
-// shape from 48 sessions up, profiles/r02_a_kbench_gemm_vs_cublas_mimi.jsonl).  Here the operands keep their textbook roles:
+// gemm_sk.cu feeds the 128-row weight tile as the MMA *A* operand and the sessions as N ("swap-AB"): right while the batch is
+// tiny.  From 33 sessions on the operands keep their textbook roles here:
 //
-//   * A = the activations, one [128 sessions x 64 k] SWIZZLE_128B box per k-block (2-D TMA, rows beyond M zero-filled; two such
-//     blocks and two accumulators above 128 sessions);
-//   * B = TWO pre-tiled 128-row weight tiles side by side (N = 256 per instruction: twice the weight bytes per tensor-pipe
-//     cycle); for the gated MLP the pair is (gate rows, value rows) of the same outputs, already stored back to back, so the
+//   * A = the activations, one [128 sessions x 64 k] SWIZZLE_128B box per k-block (2-D TMA, rows beyond M zero-filled);
+//     consumer warpgroup w multiplies sessions 64w..64w+63 (a warpgroup without sessions skips its MMAs).  Above 128
+//     sessions ns_linear runs two launches, one per block of 128 sessions;
+//   * B = TWO pre-tiled 128-row weight tiles side by side (N = 256 per instruction: twice the weight bytes per MMA);
+//     for the gated MLP the pair is (gate rows, value rows) of the same outputs, already stored back to back, so the
 //     accumulator holds gate in columns 0..127 and value in 128..255 of the SAME thread and silu(g) * u needs no exchange;
-//   * D = [128 sessions (TMEM lanes) x 256 weight rows (columns)] fp32: an epilogue thread owns one session and writes 16
-//     consecutive outputs (32 bytes) per TMEM load.
+//   * D = [64 sessions x 256 weight rows] fp32 per warpgroup in registers; the epilogue runs straight from the fragments
+//     (two consecutive outputs of one session per store).
 //   * shapes with fewer units than SMs are cut along K over a cluster of 2..4 CTAs (in_proj: 48 pairs x 2; out_proj / linear_out:
 //     32 single tiles x 4, N = 128 per instruction there so that 128 SMs pull on the weights); the partial accumulators are
 //     reduce-scattered over distributed shared memory by output columns (the stage ring is dead by then and serves as the
 //     receive buffer), summed in rank order (deterministic) and stored by the owning rank: no workspace, no atomics.
-//     ns_default_plan() holds the measured choice per shape.
+//     ns_default_plan() holds the choice per shape.
 //
 // Same packed weights, same epilogues and cast points as gemm_sk.cu (residual add bf16(res + bf16(acc)), gated SiLU
 // bf16(bf16(silu(g)) * u), gating.py:18-20); same PDL protocol (weights requested before griddepcontrol.wait).
@@ -32,14 +31,16 @@ using namespace tcp;
 
 constexpr int EPI_STORE = 0, EPI_RESADD = 1, EPI_GATE = 2;
 constexpr int BLOCK_ROWS = 128, BLOCK_K = 64, UMMA_K = 16;
-constexpr int NUM_THREADS = 192;             // warp 0 producer, warp 1 MMA, warps 2-5 epilogue
+constexpr int NUM_THREADS = 288;             // warps 0-7: two consumer warpgroups (MMA + epilogue), warp 8: producer
+constexpr int PRODUCER_WARP = 8;
+constexpr int CONSUMERS = 256;
 constexpr int TILE_BYTES = BLOCK_ROWS * BLOCK_K * 2;
 constexpr int A_BYTES = 128 * BLOCK_K * 2;   // one activation box: 128 session rows x 64 k
 constexpr int MAX_STAGES = 8;
 constexpr int MAX_CS = 8;
 
 struct NsParams {
-  int M, N, K, out_rows, gate_rows, CS, num_kb, kb_per, stages, n_tiles, ldw, unit_tiles, mblocks;
+  int M, N, K, out_rows, gate_rows, CS, num_kb, kb_per, stages, n_tiles, ldw;
   const uint8_t* wt;
   __nv_bfloat16* y; long long ldy;
   const __nv_bfloat16* res; long long ldr;
@@ -50,8 +51,8 @@ __device__ __forceinline__ uint32_t ns_map_to_rank(uint32_t local_smem_addr, uin
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_smem_addr), "r"(rank));
   return r;
 }
-__device__ __forceinline__ void ns_st_cluster_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared::cluster.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+__device__ __forceinline__ void ns_st_cluster_v2(uint32_t addr, uint32_t a, uint32_t b) {
+  asm volatile("st.shared::cluster.v2.b32 [%0], {%1, %2};" ::"r"(addr), "r"(a), "r"(b) : "memory");
 }
 __device__ __forceinline__ void ns_cluster_sync() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
@@ -62,6 +63,19 @@ __device__ __forceinline__ float ns_bf16_round(float v) { return __bfloat162floa
 // first accumulator column of rank q's share of `width` columns (multiples of 16; the last rank takes the remainder)
 __device__ __forceinline__ int col_begin(int width, int cs, int q) { return q >= cs ? width : ((width * q / cs) >> 4) << 4; }
 
+// two consecutive outputs of one session row -> y (one 4-byte store; `valid` outputs remain in the row)
+__device__ __forceinline__ void store2(__nv_bfloat16* dst, const float* v, int valid) {
+  if (valid >= 2) *reinterpret_cast<__nv_bfloat162*>(dst) = __floats2bfloat162_rn(v[0], v[1]);
+  else dst[0] = __float2bfloat16_rn(v[0]);
+}
+__device__ __forceinline__ void load2(const __nv_bfloat16* src, float* v, int valid) {
+  if (valid >= 2) {
+    const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(src));
+    v[0] = f.x; v[1] = f.y;
+  } else {
+    v[0] = __bfloat162float(src[0]); v[1] = 0.f;
+  }
+}
 // 16 consecutive outputs of one session row -> y (two 16-byte stores)
 __device__ __forceinline__ void store16(__nv_bfloat16* dst, const float* v, int valid) {
   if (valid >= 16) {
@@ -92,19 +106,17 @@ __device__ __forceinline__ void load16(const __nv_bfloat16* src, float* v, int v
   }
 }
 
-template <int EPI>
+template <int EPI, int UT>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_ns_kernel(const __grid_constant__ CUtensorMap tmap_x, const NsParams p) {
+  constexpr int NW = 128 * UT;                                            // wgmma width: the weight rows of a unit
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
-  const uint32_t a_off = (uint32_t)p.unit_tiles * TILE_BYTES;             // stage = B (one or two weight tiles) | A (activation box)
-  const uint32_t a_bytes = (uint32_t)p.mblocks * A_BYTES;                // one or two blocks of 128 sessions (M <= 256)
-  const uint32_t stage_bytes = a_off + a_bytes;
+  constexpr uint32_t a_off = (uint32_t)UT * TILE_BYTES;                   // stage = B (one or two weight tiles) | A (activation box)
+  constexpr uint32_t stage_bytes = a_off + A_BYTES;
   const uint32_t bars = base + (uint32_t)p.stages * stage_bytes;
-  const uint32_t full0 = bars, empty0 = bars + 8 * MAX_STAGES, tfull = bars + 16 * MAX_STAGES;
-  const uint32_t tptr = tfull + 8;
-  uint32_t* tptr_generic = reinterpret_cast<uint32_t*>(smem_raw + (tptr - raw));
+  const uint32_t full0 = bars, empty0 = bars + 8 * MAX_STAGES;
   const float* recv_generic = reinterpret_cast<const float*>(smem_raw + (base - raw));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -112,28 +124,27 @@ gemm_ns_kernel(const __grid_constant__ CUtensorMap tmap_x, const NsParams p) {
   const int kb0 = me * p.kb_per, kb1 = min(p.num_kb, kb0 + p.kb_per);
   const int n_items = kb1 > kb0 ? kb1 - kb0 : 0;
   // weight tiles of this unit: the (gate, value) pair, or row tiles 2u and 2u+1 (the last unit of an odd count has one)
-  const bool two = EPI == EPI_GATE || (p.unit_tiles == 2 && 2 * unit + 1 < p.n_tiles);
-  const int tile0 = EPI == EPI_GATE ? unit : unit * p.unit_tiles;
+  const bool two = EPI == EPI_GATE || (UT == 2 && 2 * unit + 1 < p.n_tiles);
+  const int tile0 = EPI == EPI_GATE ? unit : unit * UT;
   const int width = two ? 256 : 128;                                      // accumulator columns in use
   const uint32_t b_bytes = two ? 2u * TILE_BYTES : (uint32_t)TILE_BYTES;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == PRODUCER_WARP && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_x) : "memory");
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(full0 + 8 * s, 1);
-      mbar_init(empty0 + 8 * s, 1);
+      mbar_init(empty0 + 8 * s, CONSUMERS / 32);
     }
-    mbar_init(tfull, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) tmem_alloc(tptr, 256u * p.mblocks);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tptr_generic;
   pdl_trigger();
 
-  if (warp == 0) {
+  uint32_t d[NW / 2];
+#pragma unroll
+  for (int i = 0; i < NW / 2; ++i) d[i] = 0u;    // a rank without k-blocks contributes zeros
+  const int wg = warp >> 2, t = threadIdx.x & 127;
+  if (warp == PRODUCER_WARP) {
     if (lane == 0) {
       auto load_b = [&](int i, int s) {
         const int kb = kb0 + i;
@@ -148,7 +159,7 @@ gemm_ns_kernel(const __grid_constant__ CUtensorMap tmap_x, const NsParams p) {
       // weights first (they do not depend on the preceding kernel), activations after the dependency wait
       const int pre = n_items < p.stages ? n_items : p.stages;
       for (int i = 0; i < pre; ++i) {
-        mbar_expect_tx(full0 + 8 * i, b_bytes + a_bytes);
+        mbar_expect_tx(full0 + 8 * i, b_bytes + A_BYTES);
         load_b(i, i);
       }
       pdl_wait();
@@ -156,7 +167,7 @@ gemm_ns_kernel(const __grid_constant__ CUtensorMap tmap_x, const NsParams p) {
       for (int i = 0; i < n_items; ++i) {
         if (i >= pre) {
           mbar_wait(empty0 + 8 * s, ph ^ 1u);
-          mbar_expect_tx(full0 + 8 * s, b_bytes + a_bytes);
+          mbar_expect_tx(full0 + 8 * s, b_bytes + A_BYTES);
           load_b(i, s);
         }
         tma_load_2d(base + (uint32_t)s * stage_bytes + a_off, &tmap_x, full0 + 8 * s, (kb0 + i) * BLOCK_K, 0);
@@ -164,131 +175,112 @@ gemm_ns_kernel(const __grid_constant__ CUtensorMap tmap_x, const NsParams p) {
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc(128, width);
-      int s = 0; uint32_t ph = 0;
-      for (int i = 0; i < n_items; ++i) {
-        mbar_wait(full0 + 8 * s, ph);
-        tc_fence_after();
+  } else {
+    // warpgroup wg: sessions 64 wg .. 64 wg + 63 (a warpgroup without sessions only keeps the ring moving)
+    const bool active = 64 * wg < p.M;
+    int s = 0; uint32_t ph = 0;
+    for (int i = 0; i < n_items; ++i) {
+      mbar_wait(full0 + 8 * s, ph);
+      if (active) {
         const uint32_t sb = base + (uint32_t)s * stage_bytes;
-        const uint32_t sa = sb + a_off;
-        for (int mb = 0; mb < p.mblocks; ++mb) {
+        const uint32_t sa = sb + a_off + (uint32_t)wg * (A_BYTES / 2);
+        wg_fence();
 #pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-            umma_bf16(tmem_base + (uint32_t)(mb * 256), make_desc(sa + mb * A_BYTES + k * UMMA_K * 2), make_desc(sb + k * UMMA_K * 2), idesc,
-                      (i == 0 && k == 0) ? 0u : 1u);
-        }
-        umma_commit(empty0 + 8 * s);
-        if (++s == p.stages) { s = 0; ph ^= 1u; }
+        for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
+          Wgmma<NW>::bf16(d, make_desc(sa + k * UMMA_K * 2), make_desc(sb + k * UMMA_K * 2), (i == 0 && k == 0) ? 0u : 1u);
+        wg_commit();
+        wg_wait<0>();
+        wg_hold(d);
       }
-      umma_commit(tfull);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty0 + 8 * s);
+      if (++s == p.stages) { s = 0; ph ^= 1u; }
     }
-    __syncwarp();
+    pdl_wait();                                 // y / res may still be in use by the predecessor
   }
 
-  const int q4 = warp & 3;
-  const int my_c0 = col_begin(width, p.CS, me), my_c1 = col_begin(width, p.CS, me + 1);
-  if (warp >= 2) {
-    mbar_wait(tfull, 0);
-    tc_fence_after();
-  }
-  bool waited = false;
-  for (int mb = 0; mb < p.mblocks; ++mb) {      // blocks of 128 sessions: one accumulator each, the receive buffer is reused
-    const int m = mb * 128 + q4 * 32 + lane;    // session row of an epilogue thread (TMEM lane q4*32 + lane of accumulator mb)
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(q4 * 32) << 16) + (uint32_t)(mb * 256);
-    const bool m_ok = m < p.M;
-    if (p.CS > 1) {
-      ns_cluster_sync();                        // every rank's MMAs have retired / has read the previous block: the rings are free to receive
-      if (warp >= 2) {
-        for (int q = 0; q < p.CS; ++q) {
-          if (q == me) continue;
-          const int c0q = col_begin(width, p.CS, q), c1q = col_begin(width, p.CS, q + 1);
-          const int slot = me < q ? me : me - 1;
-          const uint32_t dst = ns_map_to_rank(base + (uint32_t)((slot * 128 + q4 * 32 + lane) * p.ldw) * 4u, (uint32_t)q);
-          for (int c = c0q; c < c1q; c += 16) {
-            uint32_t r[16];
-            if (n_items > 0) {
-              tmem_ld16(lane_addr + (uint32_t)c, r);
-              tmem_ld_wait();
-            } else {
+  if (p.CS == 1) {
+    if (warp == PRODUCER_WARP) return;
+    // straight from the fragments: element pair (i, i + 1) is outputs n, n + 1 of session m
+    if (EPI == EPI_GATE) {
+      // columns j (gate) and 128 + j (value) of the same output sit in registers i and i + 64 of the same thread
+      const int nb = unit * BLOCK_ROWS;
 #pragma unroll
-              for (int j = 0; j < 16; ++j) r[j] = 0u;
-            }
-            if (m_ok) {
+      for (int i = 0; i < 64; i += 2) {
+        const int m = 64 * wg + frag_row(t, i), n = nb + frag_col(t, i);
+        if (m < p.M && n < p.out_rows) {
+          float v[2];
 #pragma unroll
-              for (int j = 0; j < 16; j += 4) ns_st_cluster_v4(dst + (uint32_t)(c - c0q + j) * 4u, r[j], r[j + 1], r[j + 2], r[j + 3]);
-            }
+          for (int j = 0; j < 2; ++j) {
+            const float gt = ns_bf16_round(__uint_as_float(d[i + j])), ut = ns_bf16_round(__uint_as_float(d[64 + i + j]));
+            v[j] = ns_bf16_round(gt / (1.f + expf(-gt))) * ut;
           }
-        }
-        tc_fence_before();
-      }
-      ns_cluster_sync();                        // every partial has landed in its owner's receive buffer
-    }
-    if (warp >= 2) {
-      if (!waited) { pdl_wait(); waited = true; }   // y / res may still be in use by the predecessor
-      if (EPI == EPI_GATE) {
-        // columns j (gate) and 128 + j (value) of the same output; CS == 1 (the pair never needs a split: 88 units at 7B)
-        const int nb = unit * BLOCK_ROWS;
-        for (int c = 0; c < 128; c += 16) {
-          uint32_t g[16], u[16];
-          tmem_ld16(lane_addr + (uint32_t)c, g);
-          tmem_ld16(lane_addr + (uint32_t)(128 + c), u);
-          tmem_ld_wait();
-          const int valid = p.out_rows - (nb + c);
-          if (m_ok && valid > 0) {
-            float v[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              const float gt = ns_bf16_round(__uint_as_float(g[j])), ut = ns_bf16_round(__uint_as_float(u[j]));
-              v[j] = ns_bf16_round(gt / (1.f + expf(-gt))) * ut;
-            }
-            store16(p.y + (long long)m * p.ldy + nb + c, v, valid);
-          }
-        }
-      } else {
-        const int nb = tile0 * BLOCK_ROWS;
-        for (int c = my_c0; c < my_c1; c += 16) {
-          float acc[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) acc[j] = 0.f;
-          const int valid = p.out_rows - (nb + c);
-          float rv[16];
-          if (EPI == EPI_RESADD && m_ok && valid > 0) load16(p.res + (long long)m * p.ldr + nb + c, rv, valid);
-          for (int r = 0; r < p.CS; ++r) {      // rank order: the sum does not depend on which rank does it
-            if (r == me) {
-              if (n_items > 0) {
-                uint32_t t[16];
-                tmem_ld16(lane_addr + (uint32_t)c, t);
-                tmem_ld_wait();
-#pragma unroll
-                for (int j = 0; j < 16; ++j) acc[j] += __uint_as_float(t[j]);
-              }
-            } else if (m_ok) {
-              const int slot = r < me ? r : r - 1;
-              const float4* src = reinterpret_cast<const float4*>(recv_generic + (size_t)(slot * 128 + q4 * 32 + lane) * p.ldw + (c - my_c0));
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                const float4 t = src[j];
-                acc[4 * j] += t.x; acc[4 * j + 1] += t.y; acc[4 * j + 2] += t.z; acc[4 * j + 3] += t.w;
-              }
-            }
-          }
-          if (m_ok && valid > 0) {
-            if (EPI == EPI_RESADD) {
-#pragma unroll
-              for (int j = 0; j < 16; ++j) acc[j] = rv[j] + ns_bf16_round(acc[j]);
-            }
-            store16(p.y + (long long)m * p.ldy + nb + c, acc, valid);
-          }
+          store2(p.y + (long long)m * p.ldy + n, v, p.out_rows - n);
         }
       }
-      tc_fence_before();
+    } else {
+      const int nb = tile0 * BLOCK_ROWS;
+#pragma unroll
+      for (int i = 0; i < NW / 2; i += 2) {
+        const int m = 64 * wg + frag_row(t, i), c = frag_col(t, i), n = nb + c;
+        if (c < width && m < p.M && n < p.out_rows) {
+          float v[2] = {__uint_as_float(d[i]), __uint_as_float(d[i + 1])};
+          if (EPI == EPI_RESADD) {
+            float rv[2];
+            load2(p.res + (long long)m * p.ldr + n, rv, p.out_rows - n);
+            v[0] = rv[0] + ns_bf16_round(v[0]); v[1] = rv[1] + ns_bf16_round(v[1]);
+          }
+          store2(p.y + (long long)m * p.ldy + n, v, p.out_rows - n);
+        }
+      }
+    }
+    return;
+  }
+  // K split over the cluster: column c of every rank's accumulator goes to the rank that owns c, slot = sender rank
+  ns_cluster_sync();                            // every rank's MMAs have retired: the rings are free to receive
+  if (warp != PRODUCER_WARP) {
+#pragma unroll
+    for (int i = 0; i < NW / 2; i += 2) {
+      const int m = 64 * wg + frag_row(t, i), c = frag_col(t, i);
+      if (c < width && m < p.M) {
+        int q = 0;
+        while (c >= col_begin(width, p.CS, q + 1)) ++q;
+        const uint32_t dst = ns_map_to_rank(base + (uint32_t)((me * 128 + m) * p.ldw + (c - col_begin(width, p.CS, q))) * 4u, (uint32_t)q);
+        ns_st_cluster_v2(dst, d[i], d[i + 1]);
+      }
     }
   }
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 256u * p.mblocks);
-  if (p.CS > 1) ns_cluster_sync();              // no CTA exits while a peer could still address its shared memory
+  ns_cluster_sync();                            // every partial has landed in its owner's receive buffer
+  if (warp != PRODUCER_WARP) {
+    const int my_c0 = col_begin(width, p.CS, me), my_c1 = col_begin(width, p.CS, me + 1);
+    const int et = threadIdx.x, m = et & 127;
+    const int nb = tile0 * BLOCK_ROWS;
+    if (m < p.M) {
+      for (int c = my_c0 + (et >> 7) * 16; c < my_c1; c += 32) {
+        const int valid = p.out_rows - (nb + c);
+        if (valid <= 0) break;
+        float acc[16];
+#pragma unroll
+        for (int j = 0; j < 16; ++j) acc[j] = 0.f;
+        float rv[16];
+        if (EPI == EPI_RESADD) load16(p.res + (long long)m * p.ldr + nb + c, rv, valid);
+        for (int r = 0; r < p.CS; ++r) {        // rank order: the sum does not depend on which rank does it
+          const float4* src = reinterpret_cast<const float4*>(recv_generic + (size_t)(r * 128 + m) * p.ldw + (c - my_c0));
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const float4 v = src[j];
+            acc[4 * j] += v.x; acc[4 * j + 1] += v.y; acc[4 * j + 2] += v.z; acc[4 * j + 3] += v.w;
+          }
+        }
+        if (EPI == EPI_RESADD) {
+#pragma unroll
+          for (int j = 0; j < 16; ++j) acc[j] = rv[j] + ns_bf16_round(acc[j]);
+        }
+        store16(p.y + (long long)m * p.ldy + nb + c, acc, valid);
+      }
+    }
+  }
+  ns_cluster_sync();                            // no CTA exits while a peer could still address its shared memory
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -308,9 +300,11 @@ int ns_init() {
   }
   if (!g_ns_attr) {
     const int max_smem = 220 * 1024;
-    B200_CUDA(cudaFuncSetAttribute(gemm_ns_kernel<EPI_STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-    B200_CUDA(cudaFuncSetAttribute(gemm_ns_kernel<EPI_RESADD>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-    B200_CUDA(cudaFuncSetAttribute(gemm_ns_kernel<EPI_GATE>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+    B200_CUDA(cudaFuncSetAttribute(gemm_ns_kernel<EPI_STORE, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+    B200_CUDA(cudaFuncSetAttribute(gemm_ns_kernel<EPI_RESADD, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+    B200_CUDA(cudaFuncSetAttribute(gemm_ns_kernel<EPI_STORE, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+    B200_CUDA(cudaFuncSetAttribute(gemm_ns_kernel<EPI_RESADD, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+    B200_CUDA(cudaFuncSetAttribute(gemm_ns_kernel<EPI_GATE, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
     int dev = 0;
     B200_CUDA(cudaGetDevice(&dev));
     B200_CUDA(cudaDeviceGetAttribute(&g_ns_sms, cudaDevAttrMultiProcessorCount, dev));
@@ -328,13 +322,11 @@ bool ns_supported(int M, int N, int K, int epi) {
 
 int ns_prepare() { return ns_init(); }
 
-// The LM's choice of unit and K-split for a shape, from measurements on B200 at 48 / 104 sessions
-// (profiles/r02_c_kbench_ns_sweep.jsonl, profiles/r02_d_kbench_ns_sweep_m104.jsonl):
+// The LM's choice of unit and K-split for a shape:
 //   * >= 40 pairs of tiles (in_proj 48, the gated MLP's input 88, the text head 125): N = 256 units, two K-splits while both CTAs
 //     of every unit are resident at once (in_proj: 96 CTAs), else one;
 //   * fewer (out_proj / linear_out: 32 tiles, depformer_in: 64): single-tile units (N = 128) so that more SMs pull on the
 //     weights, K cut over the largest power of two <= 4 that keeps the grid resident (32 x 4, 64 x 2 = 128 CTAs).
-// Wider clusters lose more to the receive traffic (~10 B/clk per SM over DSMEM) and to cluster placement than they gain.
 static void ns_default_plan(int n_tiles, int num_kb, int epi, int* unit_tiles, int* cs) {
   if (epi == EPI_GATE) { *unit_tiles = 2; *cs = 1; return; }
   const int pairs = (n_tiles + 1) / 2;
@@ -357,6 +349,13 @@ int ns_linear(GemmPlanCache& cache, const __nv_bfloat16* x, long long ldx, const
     B200_FAIL(B200_ERR_SHAPE, "ns GEMM: operands must be 16-byte aligned");
   if ((ldy % 8) || (res && ldr % 8)) B200_FAIL(B200_ERR_SHAPE, "ns GEMM: row strides must be multiples of 8");
   B200_TRY(ns_init());
+  // the accumulator [128 sessions x 256 weight rows] lives in the registers of the two consumer warpgroups: above 128
+  // sessions the batch runs as two launches (each streams the weights again)
+  if (M > 128) {
+    B200_TRY(ns_linear(cache, x, ldx, w_tiles, y, ldy, res, ldr, 128, N, K, epi, gate_rows, cluster, pdl, stream, unit_tiles));
+    return ns_linear(cache, x + 128 * ldx, ldx, w_tiles, y + 128 * ldy, ldy, res ? res + 128 * ldr : nullptr, ldr, M - 128, N, K, epi,
+                     gate_rows, cluster, pdl, stream, unit_tiles);
+  }
   NsParams p;
   p.M = M; p.N = N; p.K = K; p.gate_rows = gate_rows;
   p.out_rows = epi == EPI_GATE ? gate_rows : N;
@@ -365,10 +364,9 @@ int ns_linear(GemmPlanCache& cache, const __nv_bfloat16* x, long long ldx, const
   int def_ut = 2, def_cs = 1;
   ns_default_plan(p.n_tiles, p.num_kb, epi, &def_ut, &def_cs);
   if (unit_tiles == 0) unit_tiles = cluster > 0 ? 2 : def_ut;
-  p.unit_tiles = (unit_tiles == 1 && epi != EPI_GATE) ? 1 : 2;
-  p.mblocks = M > 128 ? 2 : 1;
-  const uint32_t stage_bytes = (uint32_t)p.unit_tiles * TILE_BYTES + (uint32_t)p.mblocks * A_BYTES;
-  const int n_units = (epi == EPI_GATE || p.unit_tiles == 1) ? p.n_tiles : (p.n_tiles + 1) / 2;
+  const int ut = (unit_tiles == 1 && epi != EPI_GATE) ? 1 : 2;
+  const uint32_t stage_bytes = (uint32_t)ut * TILE_BYTES + (uint32_t)A_BYTES;
+  const int n_units = (epi == EPI_GATE || ut == 1) ? p.n_tiles : (p.n_tiles + 1) / 2;
   int cs = cluster > 0 ? cluster : def_cs;
   if (epi == EPI_GATE) cs = 1;
   if (cs > MAX_CS) cs = MAX_CS;
@@ -387,7 +385,7 @@ int ns_linear(GemmPlanCache& cache, const __nv_bfloat16* x, long long ldx, const
   if (stages > MAX_STAGES) stages = MAX_STAGES;
   if (stages > p.kb_per && p.kb_per >= 2) stages = p.kb_per;
   if (stages < 2) stages = 2;
-  const size_t recv_bytes = cs > 1 ? (size_t)(cs - 1) * 128 * p.ldw * 4 : 0;
+  const size_t recv_bytes = cs > 1 ? (size_t)cs * 128 * p.ldw * 4 : 0;
   while ((size_t)stages * stage_bytes < recv_bytes) ++stages;          // the ring doubles as the receive buffer
   if (stages > MAX_STAGES || (size_t)stages * stage_bytes > 204 * 1024)
     B200_FAIL(B200_ERR_SHAPE, "ns GEMM: the receive buffer of a %d-way split does not fit", cs);
@@ -395,13 +393,13 @@ int ns_linear(GemmPlanCache& cache, const __nv_bfloat16* x, long long ldx, const
   p.wt = static_cast<const uint8_t*>(w_tiles);
   p.y = y; p.ldy = ldy; p.res = res; p.ldr = ldr;
   // activations x [M][K]: boxes of [128 rows x 64 k]; rows >= M are zero-filled by the TMA unit
-  PlanKey key{x, ldx, M, K, 128 * p.mblocks};
+  PlanKey key{x, ldx, M, K, 128};
   auto it = cache.maps.find(key);
   if (it == cache.maps.end()) {
     CUtensorMap mp;
     cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)M};
     cuuint64_t strides[1] = {(cuuint64_t)ldx * 2};
-    cuuint32_t box[2] = {(cuuint32_t)BLOCK_K, (cuuint32_t)(128 * p.mblocks)};
+    cuuint32_t box[2] = {(cuuint32_t)BLOCK_K, 128u};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = g_ns_encode(&mp, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<__nv_bfloat16*>(x), dims, strides, box, estr,
                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -427,9 +425,11 @@ int ns_linear(GemmPlanCache& cache, const __nv_bfloat16* x, long long ldx, const
   }
   cfg.attrs = attr; cfg.numAttrs = na;
   cudaError_t le;
-  if (epi == EPI_STORE) le = cudaLaunchKernelEx(&cfg, gemm_ns_kernel<EPI_STORE>, it->second, p);
-  else if (epi == EPI_RESADD) le = cudaLaunchKernelEx(&cfg, gemm_ns_kernel<EPI_RESADD>, it->second, p);
-  else le = cudaLaunchKernelEx(&cfg, gemm_ns_kernel<EPI_GATE>, it->second, p);
+  if (epi == EPI_GATE) le = cudaLaunchKernelEx(&cfg, gemm_ns_kernel<EPI_GATE, 2>, it->second, p);
+  else if (ut == 1) le = epi == EPI_STORE ? cudaLaunchKernelEx(&cfg, gemm_ns_kernel<EPI_STORE, 1>, it->second, p)
+                                         : cudaLaunchKernelEx(&cfg, gemm_ns_kernel<EPI_RESADD, 1>, it->second, p);
+  else le = epi == EPI_STORE ? cudaLaunchKernelEx(&cfg, gemm_ns_kernel<EPI_STORE, 2>, it->second, p)
+                             : cudaLaunchKernelEx(&cfg, gemm_ns_kernel<EPI_RESADD, 2>, it->second, p);
   if (le != cudaSuccess) B200_FAIL(B200_ERR_CUDA, "gemm_ns launch failed: %s", cudaGetErrorString(le));
   g_launches.fetch_add(1, std::memory_order_relaxed);
   return check_launch("gemm_ns");

@@ -1,8 +1,8 @@
-// Stream-K tcgen05 GEMM for the LM linears (see gemm_sk.cuh):  y[M][N] = epi(x[M][K] . w[N][K]^T), bf16 in,
-// fp32 accumulate in TMEM, bf16 out.  M = concurrent sessions (<= 256), so the kernel is a weight
-// streamer: every weight byte crosses HBM -> SMEM exactly once and the whole chip pulls on it.
+// Stream-K wgmma GEMM for the LM linears (see gemm_sk.cuh):  y[M][N] = epi(x[M][K] . w[N][K]^T), bf16 in,
+// fp32 accumulate in registers, bf16 out.  M = concurrent sessions (<= 256), so the kernel is a weight
+// streamer: every weight byte crosses HBM -> SMEM exactly once per launch and the whole chip pulls on it.
 //
-//   * Weights are repacked once at load into UMMA-ready tiles: [n_tile][k_block][A][128 rows x 64 k] bf16,
+//   * Weights are repacked once at load into MMA-ready tiles: [n_tile][k_block][A][128 rows x 64 k] bf16,
 //     each 16 KB tile already in the SWIZZLE_128B K-major shared-memory layout.  A pipeline stage is
 //     therefore ONE contiguous `cp.async.bulk` (16 KB, or 32 KB for the gated MLP's gate+value pair).
 //   * Work = the linear sequence of (n_tile, k_block) items, cut into equal contiguous ranges, one per
@@ -10,9 +10,10 @@
 //     (out_proj has 32 n-tiles, the text head 250).  A tile whose k-range is cut across CTAs is
 //     finished by whichever CTA arrives last: partial accumulators go to an L2-resident workspace and
 //     are summed in CTA order, so the result is bit-reproducible and independent of arrival order.
-//   * Warp roles (192 threads): warp 0 = bulk-copy/TMA producer, warp 1 = TMEM owner + single-thread
-//     tcgen05.mma issuer, warps 2..5 = epilogue (TMEM lane quadrant = warp % 4).  Two TMEM accumulator
-//     stages let the epilogue of one segment overlap the MMAs of the next.
+//   * Warp roles (288 threads): warp 8 = bulk-copy/TMA producer, warps 0-7 = two consumer warpgroups
+//     (wgmma with the weight tile as A, warpgroup w taking rows 64w..64w+63, the sessions as N), each running
+//     the epilogue of its rows straight from the accumulator fragments.  The register accumulator bounds a
+//     launch to 128 sessions (64 for the gated pair); sk_linear runs larger batches as consecutive launches.
 #include "gemm_sk.cuh"
 #include "tc_prims.cuh"
 
@@ -23,20 +24,24 @@ namespace {
 
 constexpr int EPI_STORE = 0, EPI_RESADD = 1, EPI_GATE = 2;   // == lm::LIN_*
 constexpr int BLOCK_ROWS = 128, BLOCK_K = 64, UMMA_K = 16;
-constexpr int NUM_THREADS = 192;
+constexpr int SK_MAX_NP = 128;     // sessions per launch of the stream-K kernel (register accumulators)
+constexpr int SK_MAX_NP_GATE = 64; // ... of the gated MLP input (two accumulators)
+constexpr int NUM_THREADS = 288;   // two consumer warpgroups + one producer warp
+constexpr int PRODUCER_WARP = 8;
 constexpr int TILE_BYTES = BLOCK_ROWS * BLOCK_K * 2;   // 16 KB
 constexpr int MAX_STAGES = 12;
+constexpr int MAX_DYN_SMEM = 220 * 1024;   // of the 227 KB a block may use; the kernels also have a few bytes of static shared memory
 
 struct SkParams {
   int M, N, K, Mpad, gate_rows, out_rows;
-  int stages, num_kb, n_tiles, n_acc, acc_cols;
+  int stages, num_kb, n_tiles;
   int grid, whole_rounds, sk_tile0, sk_items;   // schedule: tiles [0, sk_tile0) whole, the rest stream-K items
   const uint8_t* wt;            // pre-tiled weights
   __nv_bfloat16* y; long long ldy;
   const __nv_bfloat16* res; long long ldr;
   float* ws;                    // partial slots: [2 * grid][A][Mpad][128] fp32
   int* counters;                // [n_tiles], zero between launches
-  uint32_t tmem_cols, stage_bytes;
+  uint32_t stage_bytes;
   int stream_only;              // diagnostics: skip the MMAs (measures the copy pipeline alone)
   // int8 x int8 -> int32 (QLinear, utils/quantize.py:13-40): activations / weights are row-wise absmax int8, the
   // accumulator is dequantised as acc * sa[m] * sw[n] / 127^2; whole tiles only (exact integer sums)
@@ -106,7 +111,37 @@ __device__ __forceinline__ float epilogue_value(const SkParams& p, float a, floa
   return bf16_round(g / (1.f + expf(-g))) * u;     // bf16(silu(gate)) * value   (gating.py:18-20)
 }
 
-template <int EPI>
+// The kernels below run 288 threads: warps 0-7 are two consumer warpgroups (wgmma into register accumulators, then the
+// epilogue straight from the fragments; warpgroup w owns weight rows 64w..64w+63 of the 128-row tile), warp 8 is the
+// bulk-copy / TMA producer.  NP = the session count padded to the wgmma width (the activation box has NP rows, rows beyond
+// M are zero-filled by the TMA unit).
+constexpr int CONSUMERS = 256;
+
+// one k-block of MMAs of a consumer warpgroup: 4 k-steps of 32 bytes per row (16 bf16 or 32 int8)
+template <int NP, int A>
+__device__ __forceinline__ void sk_mma_kblock(uint32_t sa, uint32_t sb, int wg, bool i8, bool first, uint32_t (&d0)[NP / 2],
+                                              uint32_t (&d1)[NP / 2]) {
+  wg_fence();
+#pragma unroll
+  for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
+    const uint64_t db = make_desc(sb + k * UMMA_K * 2);
+    const uint32_t accum = (first && k == 0) ? 0u : 1u;
+    const uint32_t a0 = sa + (uint32_t)wg * (TILE_BYTES / 2) + k * UMMA_K * 2;
+    if (i8) {
+      Wgmma<NP>::s8(d0, make_desc(a0), db, accum);
+      if (A == 2) Wgmma<NP>::s8(d1, make_desc(a0 + TILE_BYTES), db, accum);
+    } else {
+      Wgmma<NP>::bf16(d0, make_desc(a0), db, accum);
+      if (A == 2) Wgmma<NP>::bf16(d1, make_desc(a0 + TILE_BYTES), db, accum);
+    }
+  }
+  wg_commit();
+  wg_wait<0>();
+  wg_hold(d0);
+  if (A == 2) wg_hold(d1);
+}
+
+template <int EPI, int NP>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_sk_kernel(const __grid_constant__ CUtensorMap tmap_x, const SkParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -114,9 +149,7 @@ gemm_sk_kernel(const __grid_constant__ CUtensorMap tmap_x, const SkParams p) {
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;                 // SWIZZLE_128B tiles need 1024 B alignment
   const uint32_t bars = base + (uint32_t)p.stages * p.stage_bytes;
-  const uint32_t full0 = bars, empty0 = bars + 8 * MAX_STAGES, tfull0 = bars + 16 * MAX_STAGES, tempty0 = tfull0 + 16;
-  const uint32_t tptr = tempty0 + 16;
-  uint32_t* tptr_generic = reinterpret_cast<uint32_t*>(smem_raw + (tptr - raw));
+  const uint32_t full0 = bars, empty0 = bars + 8 * MAX_STAGES;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   constexpr int A_TILES = EPI == EPI_GATE ? 2 : 1;
@@ -125,26 +158,18 @@ gemm_sk_kernel(const __grid_constant__ CUtensorMap tmap_x, const SkParams p) {
   int n_sk = 0;
   const int n_seg = seg_count(p, c, n_sk);
 
-  if (warp == 0 && lane == 0) {
+  if (warp == PRODUCER_WARP && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_x) : "memory");
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(full0 + 8 * s, 1);
-      mbar_init(empty0 + 8 * s, 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull0 + 8 * a, 1);
-      mbar_init(tempty0 + 8 * a, 4);       // one arrival per epilogue warp
+      mbar_init(empty0 + 8 * s, CONSUMERS / 32);   // one arrival per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) tmem_alloc(tptr, p.tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tptr_generic;
   pdl_trigger();
 
-  if (warp == 0) {
+  if (warp == PRODUCER_WARP) {
     if (lane == 0) {
       // ===== producer: one contiguous bulk copy of the weight tile(s) + one TMA box of activations per k-block =====
       // Weights do not depend on the preceding kernel: the first `stages` weight tiles are requested before the
@@ -180,183 +205,119 @@ gemm_sk_kernel(const __grid_constant__ CUtensorMap tmap_x, const SkParams p) {
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ===== MMA issuer =====
-      const uint32_t idesc = p.i8 ? make_idesc_i8(BLOCK_ROWS, p.Mpad) : make_idesc(BLOCK_ROWS, p.Mpad);
-      int s = 0; uint32_t ph = 0;
-      int acc = 0; uint32_t acc_bits = 0u;       // bit a = phase parity of accumulator stage a
-      for (int si = 0; si < n_seg; ++si) {
-        const Seg sg = seg_get(p, c, n_sk, si);
-        mbar_wait(tempty0 + 8 * acc, ((acc_bits >> acc) & 1u) ^ 1u);        // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t d0 = tmem_base + (uint32_t)(acc * p.acc_cols);
-        for (int kb = sg.kb0; kb < sg.kb1; ++kb) {
-          mbar_wait(full0 + 8 * s, ph);
-          tc_fence_after();
-          if (!p.stream_only) {
-            const uint32_t sa = base + (uint32_t)s * p.stage_bytes;
-            const uint32_t sb = sa + a_bytes;
-#pragma unroll
-            for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-              const uint64_t db = make_desc(sb + k * UMMA_K * 2);
-              const uint32_t accum = (kb == sg.kb0 && k == 0) ? 0u : 1u;
-              // one MMA consumes 32 bytes of K per row either way: 16 bf16 or 32 int8
-              if (p.i8) {
-                umma_i8(d0, make_desc(sa + k * UMMA_K * 2), db, idesc, accum);
-                if (EPI == EPI_GATE) umma_i8(d0 + (uint32_t)p.Mpad, make_desc(sa + TILE_BYTES + k * UMMA_K * 2), db, idesc, accum);
-              } else {
-                umma_bf16(d0, make_desc(sa + k * UMMA_K * 2), db, idesc, accum);
-                if (EPI == EPI_GATE) umma_bf16(d0 + (uint32_t)p.Mpad, make_desc(sa + TILE_BYTES + k * UMMA_K * 2), db, idesc, accum);
-              }
-            }
-          }
-          umma_commit(empty0 + 8 * s);           // frees the smem stage once these MMAs have read it
-          if (++s == p.stages) { s = 0; ph ^= 1u; }
-        }
-        umma_commit(tfull0 + 8 * acc);           // segment accumulated
-        acc_bits ^= 1u << acc;
-        if (p.n_acc == 2) acc ^= 1;
-      }
+    return;
+  }
+  // ===== consumers: MMAs of a segment, then its epilogue from the accumulator fragments =====
+  const int wg = warp >> 2, t = threadIdx.x & 127;
+  const int et = threadIdx.x;                    // 0..255
+  const size_t slot_floats = (size_t)A_TILES * BLOCK_ROWS * p.Mpad;
+  uint32_t d0[NP / 2], d1[NP / 2];
+  int s = 0; uint32_t ph = 0;
+  pdl_wait();                                    // y / res / workspace / counters may still be in use by the predecessor
+  for (int si = 0; si < n_seg; ++si) {
+    const Seg sg = seg_get(p, c, n_sk, si);
+    for (int kb = sg.kb0; kb < sg.kb1; ++kb) {
+      mbar_wait(full0 + 8 * s, ph);
+      const uint32_t sa = base + (uint32_t)s * p.stage_bytes;
+      if (!p.stream_only) sk_mma_kblock<NP, A_TILES>(sa, sa + a_bytes, wg, p.i8 != 0, kb == sg.kb0, d0, d1);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty0 + 8 * s);  // the smem stage is free once this warp's MMAs have read it
+      if (++s == p.stages) { s = 0; ph ^= 1u; }
     }
-    __syncwarp();
-  } else {
-    // ===== epilogue: TMEM -> registers -> (global | workspace + last-arriver reduction) =====
-    const int q = warp & 3;                    // TMEM lane quadrant this warp may access
-    const int row = q * 32 + lane;
-    const int et = threadIdx.x - 64;           // 0..127
-    const size_t slot_floats = (size_t)A_TILES * BLOCK_ROWS * p.Mpad;
-    int acc = 0; uint32_t acc_bits = 0u;
-    pdl_wait();                                // y / res / workspace / counters may still be in use by the predecessor
-    for (int si = 0; si < n_seg; ++si) {
-      const Seg sg = seg_get(p, c, n_sk, si);
-      const int n = sg.tile * BLOCK_ROWS + row;
-      const bool n_ok = n < p.out_rows;
-      mbar_wait(tfull0 + 8 * acc, (acc_bits >> acc) & 1u);
-      tc_fence_after();
-      const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * p.acc_cols);
-      if (sg.slot < 0) {
-        for (int c0 = 0; c0 < p.Mpad; c0 += 16) {
-          uint32_t r0[16], r1[16];
-          // the 16 residual reads of this column chunk are issued together, ahead of the TMEM load they are added to
-          // (one dependent global load per element would cost a DRAM/L2 latency each: 96 of them per thread at B=96)
-          float rv[16];
-          if (EPI == EPI_RESADD && !p.stream_only) {
+    if (p.stream_only) continue;
+    if (sg.slot < 0) {
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              const int m = c0 + j;
-              rv[j] = (m < p.M && n_ok) ? __bfloat162float(p.res[(long long)m * p.ldr + n]) : 0.f;
-            }
-          }
-          tmem_ld16(lane_addr + (uint32_t)c0, r0);
-          if (EPI == EPI_GATE) tmem_ld16(lane_addr + (uint32_t)(p.Mpad + c0), r1);
-          tmem_ld_wait();
-          if (!p.stream_only) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              const int m = c0 + j;
-              if (m < p.M && n_ok) {
-                float v;
-                if (EPI == EPI_RESADD) v = rv[j] + bf16_round(acc_value(p, r0[j], m, n));
-                else v = epilogue_value<EPI>(p, acc_value(p, r0[j], m, n), EPI == EPI_GATE ? acc_value(p, r1[j], m, p.gate_rows + n) : 0.f, m, n);
-                p.y[(long long)m * p.ldy + n] = __float2bfloat16_rn(v);
-              }
-            }
-          }
+      for (int i = 0; i < NP / 2; ++i) {
+        const int row = 64 * wg + frag_row(t, i), m = frag_col(t, i);
+        const int n = sg.tile * BLOCK_ROWS + row;
+        if (m < p.M && n < p.out_rows) {
+          float v;
+          if (EPI == EPI_RESADD) v = __bfloat162float(p.res[(long long)m * p.ldr + n]) + bf16_round(acc_value(p, d0[i], m, n));
+          else v = epilogue_value<EPI>(p, acc_value(p, d0[i], m, n), EPI == EPI_GATE ? acc_value(p, d1[i], m, p.gate_rows + n) : 0.f, m, n);
+          p.y[(long long)m * p.ldy + n] = __float2bfloat16_rn(v);
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(tempty0 + 8 * acc);
-      } else {
-        // partial accumulator -> workspace slot, layout [A][128 rows][Mpad] (a thread owns one contiguous row)
-        float* wrow = p.ws + (size_t)sg.slot * slot_floats + (size_t)row * p.Mpad;
-        for (int c0 = 0; c0 < p.Mpad; c0 += 16) {
-          uint32_t r0[16], r1[16];
-          tmem_ld16(lane_addr + (uint32_t)c0, r0);
-          if (EPI == EPI_GATE) tmem_ld16(lane_addr + (uint32_t)(p.Mpad + c0), r1);
-          tmem_ld_wait();
+      }
+    } else {
+      // partial accumulator -> workspace slot, layout [A][128 rows][Mpad]
+      float* ws = p.ws + (size_t)sg.slot * slot_floats;
 #pragma unroll
-          for (int j = 0; j < 16; j += 4) {
-            __stcg(reinterpret_cast<float4*>(wrow + c0 + j),
-                   make_float4(__uint_as_float(r0[j]), __uint_as_float(r0[j + 1]), __uint_as_float(r0[j + 2]), __uint_as_float(r0[j + 3])));
-            if (EPI == EPI_GATE)
-              __stcg(reinterpret_cast<float4*>(wrow + (size_t)BLOCK_ROWS * p.Mpad + c0 + j),
-                     make_float4(__uint_as_float(r1[j]), __uint_as_float(r1[j + 1]), __uint_as_float(r1[j + 2]), __uint_as_float(r1[j + 3])));
-          }
+      for (int i = 0; i < NP / 2; i += 2) {
+        const int row = 64 * wg + frag_row(t, i), m = frag_col(t, i);
+        if (m < p.Mpad) {
+          __stcg(reinterpret_cast<float2*>(ws + (size_t)row * p.Mpad + m), make_float2(__uint_as_float(d0[i]), __uint_as_float(d0[i + 1])));
+          if (EPI == EPI_GATE)
+            __stcg(reinterpret_cast<float2*>(ws + (size_t)(BLOCK_ROWS + row) * p.Mpad + m),
+                   make_float2(__uint_as_float(d1[i]), __uint_as_float(d1[i + 1])));
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(tempty0 + 8 * acc);
-        // publish, count arrivals; the last arriver of this tile reduces all partials in CTA order
+      }
+      // publish, count arrivals; the last arriver of this tile reduces all partials in CTA order
+      __threadfence();
+      named_bar(1, CONSUMERS);
+      const int rel = sg.tile - p.sk_tile0;
+      const int first_c = sk_owner(p, rel * p.num_kb), last_c = sk_owner(p, (rel + 1) * p.num_kb - 1);
+      if (et == 0) {
+        const int old = atomicAdd(p.counters + sg.tile, 1);
+        const int last = old == last_c - first_c;
+        s_last = last;
+        if (last) p.counters[sg.tile] = 0;                     // ready for the next launch
+      }
+      named_bar(1, CONSUMERS);
+      if (s_last) {
         __threadfence();
-        epi_bar_sync();
-        const int rel = sg.tile - p.sk_tile0;
-        const int first_c = sk_owner(p, rel * p.num_kb), last_c = sk_owner(p, (rel + 1) * p.num_kb - 1);
-        if (et == 0) {
-          const int old = atomicAdd(p.counters + sg.tile, 1);
-          const int last = old == last_c - first_c;
-          s_last = last;
-          if (last) p.counters[sg.tile] = 0;                     // ready for the next launch
-        }
-        epi_bar_sync();
-        if (s_last) {
-          __threadfence();
-          // 16 columns per pass: every contribution's 4 (gate: 8) 16-byte loads are issued before the adds
-          for (int m0 = 0; m0 < p.M; m0 += 16) {
-            float av[16], bv[16];
+        const int row = et & 127, n = sg.tile * BLOCK_ROWS + row;
+        const bool n_ok = n < p.out_rows;
+        // 16 columns per pass (the two halves of the consumers take alternate passes): every contribution's 4 (gate: 8)
+        // 16-byte loads are issued before the adds
+        for (int m0 = (et >> 7) * 16; m0 < p.M; m0 += 32) {
+          float av[16], bv[16];
 #pragma unroll
-            for (int j = 0; j < 16; ++j) { av[j] = 0.f; bv[j] = 0.f; }
+          for (int j = 0; j < 16; ++j) { av[j] = 0.f; bv[j] = 0.f; }
 #pragma unroll 2
-            for (int cc = first_c; cc <= last_c; ++cc) {
-              const int sl = 2 * cc + ((sk_begin(p, cc) / p.num_kb == rel) ? 0 : 1);
-              const float4* w2 = reinterpret_cast<const float4*>(p.ws + (size_t)sl * slot_floats + (size_t)row * p.Mpad + m0);
-              float4 v[4], u[4];
+          for (int cc = first_c; cc <= last_c; ++cc) {
+            const int sl = 2 * cc + ((sk_begin(p, cc) / p.num_kb == rel) ? 0 : 1);
+            const float4* w2 = reinterpret_cast<const float4*>(p.ws + (size_t)sl * slot_floats + (size_t)row * p.Mpad + m0);
+            float4 v[4], u[4];
 #pragma unroll
-              for (int j = 0; j < 4; ++j) v[j] = __ldcg(w2 + j);
+            for (int j = 0; j < 4; ++j) v[j] = __ldcg(w2 + j);
+            if (EPI == EPI_GATE) {
+#pragma unroll
+              for (int j = 0; j < 4; ++j) u[j] = __ldcg(w2 + (size_t)BLOCK_ROWS * p.Mpad / 4 + j);
+            }
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              const bool q8 = p.i8 != 0;
+              av[4 * j] = part_add(q8, av[4 * j], v[j].x); av[4 * j + 1] = part_add(q8, av[4 * j + 1], v[j].y);
+              av[4 * j + 2] = part_add(q8, av[4 * j + 2], v[j].z); av[4 * j + 3] = part_add(q8, av[4 * j + 3], v[j].w);
               if (EPI == EPI_GATE) {
-#pragma unroll
-                for (int j = 0; j < 4; ++j) u[j] = __ldcg(w2 + (size_t)BLOCK_ROWS * p.Mpad / 4 + j);
-              }
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                const bool q8 = p.i8 != 0;
-                av[4 * j] = part_add(q8, av[4 * j], v[j].x); av[4 * j + 1] = part_add(q8, av[4 * j + 1], v[j].y);
-                av[4 * j + 2] = part_add(q8, av[4 * j + 2], v[j].z); av[4 * j + 3] = part_add(q8, av[4 * j + 3], v[j].w);
-                if (EPI == EPI_GATE) {
-                  bv[4 * j] = part_add(q8, bv[4 * j], u[j].x); bv[4 * j + 1] = part_add(q8, bv[4 * j + 1], u[j].y);
-                  bv[4 * j + 2] = part_add(q8, bv[4 * j + 2], u[j].z); bv[4 * j + 3] = part_add(q8, bv[4 * j + 3], u[j].w);
-                }
+                bv[4 * j] = part_add(q8, bv[4 * j], u[j].x); bv[4 * j + 1] = part_add(q8, bv[4 * j + 1], u[j].y);
+                bv[4 * j + 2] = part_add(q8, bv[4 * j + 2], u[j].z); bv[4 * j + 3] = part_add(q8, bv[4 * j + 3], u[j].w);
               }
             }
-            if (n_ok && !p.stream_only) {
+          }
+          if (n_ok) {
 #pragma unroll
-              for (int j = 0; j < 16; ++j) {
-                const int m = m0 + j;
-                if (m < p.M) {
-                  // fp32 zero and int32 zero share a bit pattern, so the accumulators start right on both paths
-                  const float a = acc_value(p, __float_as_uint(av[j]), m, n);
-                  const float b = EPI == EPI_GATE ? acc_value(p, __float_as_uint(bv[j]), m, p.gate_rows + n) : 0.f;
-                  p.y[(long long)m * p.ldy + n] = __float2bfloat16_rn(epilogue_value<EPI>(p, a, b, m, n));
-                }
+            for (int j = 0; j < 16; ++j) {
+              const int m = m0 + j;
+              if (m < p.M) {
+                // fp32 zero and int32 zero share a bit pattern, so the accumulators start right on both paths
+                const float a = acc_value(p, __float_as_uint(av[j]), m, n);
+                const float b = EPI == EPI_GATE ? acc_value(p, __float_as_uint(bv[j]), m, p.gate_rows + n) : 0.f;
+                p.y[(long long)m * p.ldy + n] = __float2bfloat16_rn(epilogue_value<EPI>(p, a, b, m, n));
               }
             }
           }
         }
       }
-      acc_bits ^= 1u << acc;
-      if (p.n_acc == 2) acc ^= 1;
+      named_bar(1, CONSUMERS);                   // s_last is reused by the next segment
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, p.tmem_cols);
 }
 
 // ---------------------------------------------------------------------------------------------
 // Cluster split-K ("ck") for the few-tile GEMMs at more than 32 sessions (out_proj / linear_out: 32 row tiles).
-// A cluster of CS CTAs owns one 128-row tile; rank r streams k-blocks [r*kb_per, (r+1)*kb_per) into its own TMEM
+// A cluster of CS CTAs owns one 128-row tile; rank r streams k-blocks [r*kb_per, (r+1)*kb_per) into its own register
 // accumulator.  The partials are then reduce-scattered over distributed shared memory: rank q is sent columns
-// [q*Wc, (q+1)*Wc) of everybody's accumulator (st.shared::cluster into its receive buffer), one cluster barrier,
+// [q*Wc, (q+1)*Wc) of everybody's accumulator (st.shared::cluster into slot r of its receive buffer), one cluster barrier,
 // and every rank sums its column block in rank order (deterministic) and runs the epilogue for it.  No global
 // workspace, no atomics; CS x more SMs pull on the weights and the epilogue is spread over the cluster too.
 // ---------------------------------------------------------------------------------------------
@@ -365,7 +326,7 @@ struct CkParams {
   const uint8_t* wt;
   __nv_bfloat16* y; long long ldy;
   const __nv_bfloat16* res; long long ldr;
-  uint32_t tmem_cols, stage_bytes;
+  uint32_t stage_bytes;
   int i8; const float* sa; const float* sw;      // int8 operands: partials are exact int32, scaled once after the reduction
 };
 
@@ -374,50 +335,47 @@ __device__ __forceinline__ uint32_t map_to_rank(uint32_t local_smem_addr, uint32
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_smem_addr), "r"(rank));
   return r;
 }
-__device__ __forceinline__ void st_cluster_v4(uint32_t addr, float a, float b, float c, float d) {
-  asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+__device__ __forceinline__ void st_cluster_v2(uint32_t addr, uint32_t a, uint32_t b) {
+  asm volatile("st.shared::cluster.v2.b32 [%0], {%1, %2};" ::"r"(addr), "r"(a), "r"(b) : "memory");
 }
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
-template <int EPI>      // EPI_STORE or EPI_RESADD
+template <int EPI, int NP>      // EPI_STORE or EPI_RESADD
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_ck_kernel(const __grid_constant__ CUtensorMap tmap_x, const CkParams p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
   const uint32_t bars = base + (uint32_t)p.stages * p.stage_bytes;
-  const uint32_t full0 = bars, empty0 = bars + 8 * MAX_STAGES, tfull = bars + 16 * MAX_STAGES;
-  const uint32_t tptr = tfull + 8;
-  uint32_t* tptr_generic = reinterpret_cast<uint32_t*>(smem_raw + (tptr - raw));
+  const uint32_t full0 = bars, empty0 = bars + 8 * MAX_STAGES;
   // receive buffer [CS][128 rows][Wc + 4] fp32 (rows padded against bank conflicts), after the barrier block
   const int ldw = p.Wc + 4;
-  const uint32_t recv = (tptr + 8 + 15u) & ~15u;
-  float* recv_generic = reinterpret_cast<float*>(smem_raw + (recv - raw));
+  const uint32_t recv = (bars + 16 * MAX_STAGES + 15u) & ~15u;
+  const float* recv_generic = reinterpret_cast<const float*>(smem_raw + (recv - raw));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tile = blockIdx.x / p.CS, me = blockIdx.x - tile * p.CS;
   const int kb0 = me * p.kb_per, kb1 = min(p.num_kb, kb0 + p.kb_per);
 
-  if (warp == 0 && lane == 0) {
+  if (warp == PRODUCER_WARP && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_x) : "memory");
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(full0 + 8 * s, 1);
-      mbar_init(empty0 + 8 * s, 1);
+      mbar_init(empty0 + 8 * s, CONSUMERS / 32);
     }
-    mbar_init(tfull, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) tmem_alloc(tptr, p.tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tptr_generic;
+  asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory");   // waited for before the first remote store
   pdl_trigger();
 
-  if (warp == 0) {
+  uint32_t d[NP / 2], dummy[NP / 2];
+#pragma unroll
+  for (int i = 0; i < NP / 2; ++i) d[i] = 0u;    // a rank without k-blocks contributes zeros
+  if (warp == PRODUCER_WARP) {
     if (lane == 0) {
       // weights first (they do not depend on the preceding kernel), activations after the dependency wait
       const uint8_t* src = p.wt + ((size_t)tile * p.num_kb + kb0) * TILE_BYTES;
@@ -440,140 +398,95 @@ gemm_ck_kernel(const __grid_constant__ CUtensorMap tmap_x, const CkParams p) {
         if (++s == p.stages) { s = 0; ph ^= 1u; }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc = p.i8 ? make_idesc_i8(BLOCK_ROWS, p.Mpad) : make_idesc(BLOCK_ROWS, p.Mpad);
-      int s = 0; uint32_t ph = 0;
-      for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(full0 + 8 * s, ph);
-        tc_fence_after();
-        const uint32_t sa = base + (uint32_t)s * p.stage_bytes;
-        const uint32_t sb = sa + TILE_BYTES;
-#pragma unroll
-        for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-          const uint32_t accum = (kb == kb0 && k == 0) ? 0u : 1u;
-          if (p.i8) umma_i8(tmem_base, make_desc(sa + k * UMMA_K * 2), make_desc(sb + k * UMMA_K * 2), idesc, accum);
-          else umma_bf16(tmem_base, make_desc(sa + k * UMMA_K * 2), make_desc(sb + k * UMMA_K * 2), idesc, accum);
-        }
-        umma_commit(empty0 + 8 * s);
-        if (++s == p.stages) { s = 0; ph ^= 1u; }
-      }
-      umma_commit(tfull);
-    }
     __syncwarp();
-  }
-  float own[64];                               // this rank's column block of its own accumulator (Wc <= 64)
-  const int q4 = warp & 3;
-  const int row = q4 * 32 + lane;
-  if (warp >= 2) {
+    asm volatile("barrier.cluster.wait.aligned;" ::: "memory");
+  } else {
+    const int wg = warp >> 2, t = threadIdx.x & 127;
+    int s = 0; uint32_t ph = 0;
+    for (int kb = kb0; kb < kb1; ++kb) {
+      mbar_wait(full0 + 8 * s, ph);
+      const uint32_t sa = base + (uint32_t)s * p.stage_bytes;
+      sk_mma_kblock<NP, 1>(sa, sa + TILE_BYTES, wg, p.i8 != 0, kb == kb0, d, dummy);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty0 + 8 * s);
+      if (++s == p.stages) { s = 0; ph ^= 1u; }
+    }
     pdl_wait();
-    mbar_wait(tfull, 0);
-    tc_fence_after();
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(q4 * 32) << 16);
-    for (int q = 0; q < p.CS; ++q) {
-      const uint32_t dst = map_to_rank(recv + (uint32_t)((me * BLOCK_ROWS + row) * ldw) * 4u, (uint32_t)q);
+    asm volatile("barrier.cluster.wait.aligned;" ::: "memory");   // every rank's receive buffer exists
+    // column m of the accumulator goes to rank m / Wc, slot `me`, row `row`
 #pragma unroll
-      for (int c0 = 0; c0 < 64; c0 += 8) {
-        if (c0 < p.Wc) {
-          uint32_t r[8];
-          tmem_ld8(lane_addr + (uint32_t)(q * p.Wc + c0), r);
-          tmem_ld_wait();
-          if (kb1 <= kb0) {                    // a rank without k-blocks contributes zeros
-#pragma unroll
-            for (int j = 0; j < 8; ++j) r[j] = 0u;
-          }
-          if (q == me) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) own[c0 + j] = __uint_as_float(r[j]);
-          } else {
-            st_cluster_v4(dst + (uint32_t)c0 * 4u, __uint_as_float(r[0]), __uint_as_float(r[1]), __uint_as_float(r[2]), __uint_as_float(r[3]));
-            st_cluster_v4(dst + (uint32_t)(c0 + 4) * 4u, __uint_as_float(r[4]), __uint_as_float(r[5]), __uint_as_float(r[6]), __uint_as_float(r[7]));
-          }
-        }
+    for (int i = 0; i < NP / 2; i += 2) {
+      const int row = 64 * wg + frag_row(t, i), m = frag_col(t, i);
+      if (m < p.Mpad) {
+        const int q = m / p.Wc;
+        const uint32_t dst = map_to_rank(recv + (uint32_t)(((me * BLOCK_ROWS + row) * ldw) + (m - q * p.Wc)) * 4u, (uint32_t)q);
+        st_cluster_v2(dst, d[i], d[i + 1]);
       }
     }
-    tc_fence_before();
   }
   cluster_sync_all();                          // every partial has landed in its owner's receive buffer
-  if (warp >= 2) {
+  if (warp != PRODUCER_WARP) {
+    const int et = threadIdx.x, row = et & 127;
     const int n = tile * BLOCK_ROWS + row;
     const bool n_ok = n < p.N;
-#pragma unroll
-    for (int c0 = 0; c0 < 64; c0 += 8) {
-      if (c0 < p.Wc) {
-        float rv[8];
-        if (EPI == EPI_RESADD) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const int m = me * p.Wc + c0 + j;
-            rv[j] = (m < p.M && n_ok) ? __bfloat162float(p.res[(long long)m * p.ldr + n]) : 0.f;
-          }
-        }
-        float acc[8];
-        if (p.i8) {                            // exact: the partials are int32 bit patterns
-          int isum[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) isum[j] = 0;
-          for (int r = 0; r < p.CS; ++r) {
-            if (r == me) {
-#pragma unroll
-              for (int j = 0; j < 8; ++j) isum[j] += __float_as_int(own[c0 + j]);
-            } else {
-              const int4 a = *reinterpret_cast<const int4*>(recv_generic + (size_t)(r * BLOCK_ROWS + row) * ldw + c0);
-              const int4 b = *reinterpret_cast<const int4*>(recv_generic + (size_t)(r * BLOCK_ROWS + row) * ldw + c0 + 4);
-              isum[0] += a.x; isum[1] += a.y; isum[2] += a.z; isum[3] += a.w;
-              isum[4] += b.x; isum[5] += b.y; isum[6] += b.z; isum[7] += b.w;
-            }
-          }
-          const float swn = n_ok ? p.sw[n] : 0.f;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const int m = me * p.Wc + c0 + j;
-            acc[j] = m < p.M ? (float)isum[j] * (p.sa[m] * swn * (1.f / 16129.f)) : 0.f;     // same expression as acc_value()
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) acc[j] = 0.f;
-          for (int r = 0; r < p.CS; ++r) {       // rank order: the sum does not depend on which rank does it
-            if (r == me) {
-#pragma unroll
-              for (int j = 0; j < 8; ++j) acc[j] += own[c0 + j];
-            } else {
-              const float4 a = *reinterpret_cast<const float4*>(recv_generic + (size_t)(r * BLOCK_ROWS + row) * ldw + c0);
-              const float4 b = *reinterpret_cast<const float4*>(recv_generic + (size_t)(r * BLOCK_ROWS + row) * ldw + c0 + 4);
-              acc[0] += a.x; acc[1] += a.y; acc[2] += a.z; acc[3] += a.w;
-              acc[4] += b.x; acc[5] += b.y; acc[6] += b.z; acc[7] += b.w;
-            }
-          }
-        }
+    for (int c0 = (et >> 7) * 8; c0 < p.Wc; c0 += 16) {
+      float rv[8];
+      if (EPI == EPI_RESADD) {
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           const int m = me * p.Wc + c0 + j;
-          if (m < p.M && n_ok) {
-            const float v = EPI == EPI_RESADD ? rv[j] + bf16_round(acc[j]) : acc[j];
-            p.y[(long long)m * p.ldy + n] = __float2bfloat16_rn(v);
-          }
+          rv[j] = (m < p.M && n_ok) ? __bfloat162float(p.res[(long long)m * p.ldr + n]) : 0.f;
+        }
+      }
+      float acc[8];
+      if (p.i8) {                            // exact: the partials are int32 bit patterns
+        int isum[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) isum[j] = 0;
+        for (int r = 0; r < p.CS; ++r) {
+          const int4 a = *reinterpret_cast<const int4*>(recv_generic + (size_t)(r * BLOCK_ROWS + row) * ldw + c0);
+          const int4 b = *reinterpret_cast<const int4*>(recv_generic + (size_t)(r * BLOCK_ROWS + row) * ldw + c0 + 4);
+          isum[0] += a.x; isum[1] += a.y; isum[2] += a.z; isum[3] += a.w;
+          isum[4] += b.x; isum[5] += b.y; isum[6] += b.z; isum[7] += b.w;
+        }
+        const float swn = n_ok ? p.sw[n] : 0.f;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int m = me * p.Wc + c0 + j;
+          acc[j] = m < p.M ? (float)isum[j] * (p.sa[m] * swn * (1.f / 16129.f)) : 0.f;     // same expression as acc_value()
+        }
+      } else {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) acc[j] = 0.f;
+        for (int r = 0; r < p.CS; ++r) {       // rank order: the sum does not depend on which rank does it
+          const float4 a = *reinterpret_cast<const float4*>(recv_generic + (size_t)(r * BLOCK_ROWS + row) * ldw + c0);
+          const float4 b = *reinterpret_cast<const float4*>(recv_generic + (size_t)(r * BLOCK_ROWS + row) * ldw + c0 + 4);
+          acc[0] += a.x; acc[1] += a.y; acc[2] += a.z; acc[3] += a.w;
+          acc[4] += b.x; acc[5] += b.y; acc[6] += b.z; acc[7] += b.w;
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int m = me * p.Wc + c0 + j;
+        if (m < p.M && n_ok) {
+          const float v = EPI == EPI_RESADD ? rv[j] + bf16_round(acc[j]) : acc[j];
+          p.y[(long long)m * p.ldy + n] = __float2bfloat16_rn(v);
         }
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, p.tmem_cols);
 }
 
 // ---------------------------------------------------------------------------------------------
 // GEMV path for one or two sessions (up to four compiled).  With so few activation rows there is nothing for a tensor core to reuse: the GEMM
-// above is then just a weight stream, and its bulk-copy engine tops out at ~36 GB/s per SM (5.3 TB/s chip-wide, measured).
-// Plain 16-byte loads do not have that ceiling (the attention kernel streams 6.7 TB/s with them), so the same pre-tiled
-// weights are read with LDG.128 here: a CTA owns one 128-row tile (tile pair for the gated MLP) over a k-range, a thread
+// above is then just a weight stream through the bulk-copy engine, so the same pre-tiled weights are read with LDG.128 here: a CTA owns one 128-row tile (tile pair for the gated MLP) over a k-range, a thread
 // owns one 16-byte chunk position of four rows (the SWIZZLE_128B layout puts logical k-chunk (pos ^ (row & 7)) at position
 // pos, and row & 7 is the same for a thread's four rows, so it multiplies all of them with the same 8 activations), two
 // k-blocks of weights are in flight per thread (register double buffering), fp32 accumulation, 8-lane tree reduction at the
 // end, split partials summed in split order by the last CTA to arrive (deterministic), same epilogues as the GEMM.
 // ---------------------------------------------------------------------------------------------
 constexpr int GV_THREADS = 256;
-constexpr int GV_MAX_M = 4;                // compiled for up to 4 rows; used for <= 2 by default (measured: B=1 -14 %, B=2 -11 %, B=4 +1 %)
+constexpr int GV_MAX_M = 4;                // compiled for up to 4 rows; used for <= 2 by default (B200_GEMV_MAX_M)
 constexpr int GV_MAX_KBPS = 44;            // k-blocks per split: M * 44 * 64 bf16 of activations in shared memory (<= 22.5 KB)
 
 struct GvParams {
@@ -940,6 +853,31 @@ int g_sms = 0;
 int g_gemv_max_m = 2;            // B200_GEMV_MAX_M (0..4): 0 sends every batch size through the tensor-core GEMM
 int g_use_ns = 1;                // B200_GEMM_NS=0: keep the swap-AB kernels above 32 sessions (A/B measurements)
 
+template <class F>
+static cudaError_t smem_attr(F* kernel) {
+  return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_DYN_SMEM);
+}
+template <int NP>
+static int set_smem_attrs_np() {
+  B200_CUDA(smem_attr(gemm_sk_kernel<EPI_STORE, NP>));
+  B200_CUDA(smem_attr(gemm_sk_kernel<EPI_RESADD, NP>));
+  B200_CUDA(smem_attr(gemm_sk_kernel<EPI_GATE, (NP < SK_MAX_NP_GATE ? NP : SK_MAX_NP_GATE)>));
+  return B200_OK;
+}
+static int set_smem_attrs() {
+  B200_TRY(set_smem_attrs_np<16>());
+  B200_TRY(set_smem_attrs_np<32>());
+  B200_TRY(set_smem_attrs_np<64>());
+  B200_TRY(set_smem_attrs_np<128>());
+  B200_CUDA(smem_attr(gemm_ck_kernel<EPI_STORE, 64>));
+  B200_CUDA(smem_attr(gemm_ck_kernel<EPI_STORE, 128>));
+  B200_CUDA(smem_attr(gemm_ck_kernel<EPI_STORE, 256>));
+  B200_CUDA(smem_attr(gemm_ck_kernel<EPI_RESADD, 64>));
+  B200_CUDA(smem_attr(gemm_ck_kernel<EPI_RESADD, 128>));
+  B200_CUDA(smem_attr(gemm_ck_kernel<EPI_RESADD, 256>));
+  return B200_OK;
+}
+
 int init_once() {
   if (!g_encode) {
     void* fn = nullptr;
@@ -949,12 +887,7 @@ int init_once() {
     g_encode = reinterpret_cast<EncodeTiledFn>(fn);
   }
   if (!g_attr_set) {
-    const int max_smem = 220 * 1024;     // the kernel also has a few bytes of static shared memory
-    B200_CUDA(cudaFuncSetAttribute(gemm_sk_kernel<EPI_STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-    B200_CUDA(cudaFuncSetAttribute(gemm_sk_kernel<EPI_RESADD>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-    B200_CUDA(cudaFuncSetAttribute(gemm_sk_kernel<EPI_GATE>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-    B200_CUDA(cudaFuncSetAttribute(gemm_ck_kernel<EPI_STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-    B200_CUDA(cudaFuncSetAttribute(gemm_ck_kernel<EPI_RESADD>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+    B200_TRY(set_smem_attrs());
     int dev = 0;
     B200_CUDA(cudaGetDevice(&dev));
     B200_CUDA(cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, dev));
@@ -1078,6 +1011,13 @@ static int x_map(GemmPlanCache& cache, const void* x, long long ldx, int M, int 
   return B200_OK;
 }
 
+template <int NP>
+static cudaError_t sk_launch(const cudaLaunchConfig_t& cfg, int epi, const CUtensorMap& mx, const SkParams& p) {
+  if (epi == EPI_STORE) return cudaLaunchKernelEx(&cfg, gemm_sk_kernel<EPI_STORE, NP>, mx, p);
+  if (epi == EPI_RESADD) return cudaLaunchKernelEx(&cfg, gemm_sk_kernel<EPI_RESADD, NP>, mx, p);
+  return cudaLaunchKernelEx(&cfg, gemm_sk_kernel<EPI_GATE, (NP < SK_MAX_NP_GATE ? NP : SK_MAX_NP_GATE)>, mx, p);
+}
+
 // y = epi(x . W^T) with W given as packed tiles.  ws / counters: sk_workspace_bytes(M) and >= 1024 ints, zeroed once.
 int sk_linear(GemmPlanCache& cache, const __nv_bfloat16* x, long long ldx, const void* w_tiles, __nv_bfloat16* y,
               long long ldy, const __nv_bfloat16* res, long long ldr, int M, int N, int K, int epi, int gate_rows,
@@ -1125,7 +1065,7 @@ int sk_linear(GemmPlanCache& cache, const __nv_bfloat16* x, long long ldx, const
     }
   }
   if (tune.norm_alpha) B200_FAIL(B200_ERR_STATE, "sk GEMM: a fused RMSNorm input is only available on the GEMV path (M=%d)", M);
-  // 33..256 sessions: activations as the A operand, two weight tiles (N = 256) per tcgen05.mma (gemm_ns.cu)
+  // 33..256 sessions: activations as the A operand, two weight tiles (N = 256) per wgmma (gemm_ns.cu)
   if (!i8 && tune.ns >= 0 && (tune.ns > 0 || (g_use_ns && M > 32)) && M <= 256 && tune.grid == 0 && tune.cluster == 0 && !tune.stream_only &&
       !tune.force_split && ns_supported(M, N, K, epi) && ldy % 8 == 0 && (!res || ldr % 8 == 0))
     return ns_linear(cache, x, ldx, w_tiles, y, ldy, res, ldr, M, N, K, epi, gate_rows, 0, tune.pdl, stream);
@@ -1139,28 +1079,27 @@ int sk_linear(GemmPlanCache& cache, const __nv_bfloat16* x, long long ldx, const
     if (cs > 1) {
       CkParams p;
       p.M = M; p.N = N; p.K = K; p.CS = cs;
-      const int quantum = 8 * cs < 16 ? 16 : 8 * cs;       // UMMA N is a multiple of 16; every rank owns whole 8-column groups
+      const int quantum = 8 * cs < 16 ? 16 : 8 * cs;       // wgmma N is a multiple of 16; every rank owns whole 8-column groups
       p.Mpad = ((M + quantum - 1) / quantum) * quantum;
       p.Wc = p.Mpad / cs;
+      int np = 64;                                          // wgmma width: the padded session count (M > 32 here)
+      while (np < p.Mpad) np <<= 1;
       if (p.Mpad <= 256 && p.Wc <= 64) {
         p.num_kb = num_kb; p.kb_per = (num_kb + cs - 1) / cs;
         p.wt = static_cast<const uint8_t*>(w_tiles);
         p.y = y; p.ldy = ldy; p.res = res; p.ldr = ldr;
         p.i8 = i8 ? 1 : 0; p.sa = tune.sa; p.sw = tune.sw;
-        p.stage_bytes = (uint32_t)(TILE_BYTES + p.Mpad * BLOCK_K * 2);      // 128 bytes of K per row, bf16 or int8
+        p.stage_bytes = (uint32_t)(TILE_BYTES + np * BLOCK_K * 2);          // 128 bytes of K per row, bf16 or int8
         const size_t recv_bytes = (size_t)cs * BLOCK_ROWS * (p.Wc + 4) * 4;
         int stages = (int)((200 * 1024 - recv_bytes) / p.stage_bytes);
         if (stages > MAX_STAGES) stages = MAX_STAGES;
         if (stages > p.kb_per) stages = p.kb_per;
         if (stages >= 2) {
           p.stages = stages;
-          uint32_t pow2 = 32;
-          while (pow2 < (uint32_t)p.Mpad) pow2 <<= 1;
-          p.tmem_cols = pow2;
           const CUtensorMap* mx = nullptr;
-          if (i8) B200_TRY(x_map(cache, tune.xq, K, M, K, p.Mpad, 1, &mx));
-          else B200_TRY(x_map(cache, x, ldx, M, K, p.Mpad, 2, &mx));
-          const size_t smem = (size_t)stages * p.stage_bytes + 1024 + 16 * MAX_STAGES + 64 + recv_bytes + 64;
+          if (i8) B200_TRY(x_map(cache, tune.xq, K, M, K, np, 1, &mx));
+          else B200_TRY(x_map(cache, x, ldx, M, K, np, 2, &mx));
+          const size_t smem = (size_t)stages * p.stage_bytes + 1024 + 16 * MAX_STAGES + 16 + recv_bytes;
           cudaLaunchConfig_t cfg;
           memset(&cfg, 0, sizeof(cfg));
           cfg.gridDim = dim3(n_tiles * cs); cfg.blockDim = dim3(NUM_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
@@ -1170,14 +1109,33 @@ int sk_linear(GemmPlanCache& cache, const __nv_bfloat16* x, long long ldx, const
           attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
           attr[1].val.programmaticStreamSerializationAllowed = 1;
           cfg.attrs = attr; cfg.numAttrs = tune.pdl ? 2 : 1;
-          cudaError_t le = epi == EPI_STORE ? cudaLaunchKernelEx(&cfg, gemm_ck_kernel<EPI_STORE>, *mx, p)
-                                            : cudaLaunchKernelEx(&cfg, gemm_ck_kernel<EPI_RESADD>, *mx, p);
+          cudaError_t le;
+          if (np == 64) le = epi == EPI_STORE ? cudaLaunchKernelEx(&cfg, gemm_ck_kernel<EPI_STORE, 64>, *mx, p)
+                                              : cudaLaunchKernelEx(&cfg, gemm_ck_kernel<EPI_RESADD, 64>, *mx, p);
+          else if (np == 128) le = epi == EPI_STORE ? cudaLaunchKernelEx(&cfg, gemm_ck_kernel<EPI_STORE, 128>, *mx, p)
+                                                    : cudaLaunchKernelEx(&cfg, gemm_ck_kernel<EPI_RESADD, 128>, *mx, p);
+          else le = epi == EPI_STORE ? cudaLaunchKernelEx(&cfg, gemm_ck_kernel<EPI_STORE, 256>, *mx, p)
+                                     : cudaLaunchKernelEx(&cfg, gemm_ck_kernel<EPI_RESADD, 256>, *mx, p);
           if (le != cudaSuccess) B200_FAIL(B200_ERR_CUDA, "gemm_ck launch failed: %s", cudaGetErrorString(le));
           g_launches.fetch_add(1, std::memory_order_relaxed);
           return check_launch("gemm_ck");
         }
       }
     }
+  }
+  // The accumulator of a CTA lives in the registers of its two consumer warpgroups: at most 128 sessions per launch (64 for
+  // the gated MLP's two accumulators).  Larger batches run as consecutive launches over blocks of sessions, each streaming
+  // the weights again.
+  const int max_np = epi == EPI_GATE ? SK_MAX_NP_GATE : SK_MAX_NP;
+  if (M > max_np) {
+    for (int m0 = 0; m0 < M; m0 += max_np) {
+      const int mc = M - m0 < max_np ? M - m0 : max_np;
+      SkTuning t2 = tune;
+      if (i8) { t2.xq = static_cast<const int8_t*>(tune.xq) + (long long)m0 * K; t2.sa = tune.sa + m0; }
+      B200_TRY(sk_linear(cache, x + (long long)m0 * ldx, ldx, w_tiles, y + (long long)m0 * ldy, ldy, res ? res + (long long)m0 * ldr : nullptr,
+                         ldr, mc, N, K, epi, gate_rows, ws, counters, t2, stream));
+    }
+    return B200_OK;
   }
   SkParams p;
   p.M = M; p.N = N; p.K = K; p.gate_rows = gate_rows;
@@ -1198,7 +1156,7 @@ int sk_linear(GemmPlanCache& cache, const __nv_bfloat16* x, long long ldx, const
   // Cutting a tile into S pieces moves S fp32 partials of [128 x Mpad] through L2 (written + read back): allow it
   // only while that stays under half of the tile's weight bytes, i.e. S <= 8 * num_kb / Mpad.
   int s_max = tune.no_split ? 1 : (8 * p.num_kb) / p.Mpad;      // int8 partials are int32 and add exactly
-  // measured on B200 (profiles/r01_c_kbench.jsonl): with more than 32 sessions the publish / count / re-read protocol
+  // with more than 32 sessions the publish / count / re-read protocol
   // costs more than the idle SMs it recovers, so tiles stay whole there
   if (p.Mpad > 32 && tune.force_split == 0) s_max = 1;
   if (s_max < 1) s_max = 1;
@@ -1212,20 +1170,17 @@ int sk_linear(GemmPlanCache& cache, const __nv_bfloat16* x, long long ldx, const
   p.sk_tile0 = p.n_tiles - rem;
   p.sk_items = rem * p.num_kb;
   const int a_tiles = epi == EPI_GATE ? 2 : 1;
-  p.stage_bytes = (uint32_t)(a_tiles * TILE_BYTES + p.Mpad * BLOCK_K * 2);
+  int np = 16;                                                        // wgmma width: the padded session count
+  while (np < p.Mpad) np <<= 1;
+  p.stage_bytes = (uint32_t)(a_tiles * TILE_BYTES + np * BLOCK_K * 2);
   int stages = (tune.smem_budget > 0 ? tune.smem_budget : 200 * 1024) / (int)p.stage_bytes;
   if (stages > MAX_STAGES) stages = MAX_STAGES;
   if (stages < 2) stages = 2;
   p.stages = stages;
-  p.acc_cols = a_tiles * p.Mpad;
-  p.n_acc = 2 * p.acc_cols <= 512 ? 2 : 1;
-  uint32_t cols = (uint32_t)(p.n_acc * p.acc_cols), pow2 = 32;
-  while (pow2 < cols) pow2 <<= 1;
-  p.tmem_cols = pow2;
   p.stream_only = tune.stream_only;
   const CUtensorMap* mx = nullptr;
-  if (i8) B200_TRY(x_map(cache, tune.xq, K, M, K, p.Mpad, 1, &mx));
-  else B200_TRY(x_map(cache, x, ldx, M, K, p.Mpad, 2, &mx));
+  if (i8) B200_TRY(x_map(cache, tune.xq, K, M, K, np, 1, &mx));
+  else B200_TRY(x_map(cache, x, ldx, M, K, np, 2, &mx));
   const size_t smem = (size_t)stages * p.stage_bytes + 1024 + 16 * MAX_STAGES + 64;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
@@ -1235,9 +1190,10 @@ int sk_linear(GemmPlanCache& cache, const __nv_bfloat16* x, long long ldx, const
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr; cfg.numAttrs = tune.pdl ? 1 : 0;
   cudaError_t le;
-  if (epi == EPI_STORE) le = cudaLaunchKernelEx(&cfg, gemm_sk_kernel<EPI_STORE>, *mx, p);
-  else if (epi == EPI_RESADD) le = cudaLaunchKernelEx(&cfg, gemm_sk_kernel<EPI_RESADD>, *mx, p);
-  else le = cudaLaunchKernelEx(&cfg, gemm_sk_kernel<EPI_GATE>, *mx, p);
+  if (np == 16) le = sk_launch<16>(cfg, epi, *mx, p);
+  else if (np == 32) le = sk_launch<32>(cfg, epi, *mx, p);
+  else if (np == 64) le = sk_launch<64>(cfg, epi, *mx, p);
+  else le = sk_launch<128>(cfg, epi, *mx, p);
   if (le != cudaSuccess) B200_FAIL(B200_ERR_CUDA, "gemm_sk launch failed: %s", cudaGetErrorString(le));
   g_launches.fetch_add(1, std::memory_order_relaxed);
   return check_launch("gemm_sk");

@@ -1,10 +1,10 @@
-// tcgen05 / TMA weight-streaming GEMM for the LM linears:  y[M][N] = epi(x[M][K] . w[N][K]^T)
+// wgmma / TMA weight-streaming GEMM for the LM linears:  y[M][N] = epi(x[M][K] . w[N][K]^T)
 //
 // Skinny-M decode GEMMs are HBM-bound on the weights, so the kernel is organised around streaming
-// each weight row exactly once ("swap-AB"): the 128-row weight tile is the UMMA A operand (M_umma =
-// 128), the B <= 256 sessions are the UMMA N dimension, and the fp32 accumulator [128 x Mpad] lives
-// in TMEM.  Both operands are K-major in HBM, which is the native TMA / UMMA SWIZZLE_128B layout, so
-// no repacking of the reference's [out, in] weight layout is needed.
+// each weight row exactly once ("swap-AB"): the 128-row weight tile is the MMA A operand (two m64
+// halves, one per consumer warpgroup), the sessions are the MMA N dimension, and the fp32 accumulator
+// lives in registers.  Both operands are K-major in HBM, which is the native TMA / wgmma SWIZZLE_128B
+// layout, so no repacking of the reference's [out, in] weight layout is needed.
 #pragma once
 
 #include <cuda.h>
@@ -72,7 +72,7 @@ int sk_linear(GemmPlanCache& cache, const __nv_bfloat16* x, long long ldx, const
 // ---- non-swapped kernel for 33..256 sessions (gemm_ns.cu): A = activations, B = two weight tiles (N = 256) ------------
 bool ns_supported(int M, int N, int K, int epi);
 int ns_prepare();
-// cluster: K-splits (0 = the measured choice for the shape); same packed weights and epilogues as sk_linear
+// cluster: K-splits (0 = the default plan for the shape); same packed weights and epilogues as sk_linear
 // unit_tiles: weight tiles per CTA as the B operand (2 = N 256; 1 = N 128: twice the units for few-tile shapes; 0 = the LM's choice)
 int ns_linear(GemmPlanCache& cache, const __nv_bfloat16* x, long long ldx, const void* w_tiles, __nv_bfloat16* y, long long ldy,
               const __nv_bfloat16* res, long long ldr, int M, int N, int K, int epi, int gate_rows, int cluster, int pdl,

@@ -674,7 +674,7 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
     B200_TRY(A.alloc_t(&h->xq_scale, (size_t)MB, false));
   }
   // One or two sessions: the depformer's linears take the GEMV path and the PDL-chained launches beat the persistent kernel
-  // (B=1: 5.5 vs 6.4 ms per LM step, B=2: 6.2 vs 7.1; profiles/r01_r_*).  B200_DEP_FUSED=2 forces the kernel at any batch.
+  // (a grid barrier per phase costs more than the launch it saves).  B200_DEP_FUSED=2 forces the kernel at any batch.
   // Under classifier-free guidance the two halves of the batch meet before every sampler (lm.py:828-833): launch chain.
   const bool dep_small = B <= tc::sk_gemv_max_m() && h->dep_fused != 2;
   h->depf = nullptr;

@@ -274,7 +274,7 @@ inline int attn_group_keys() {
   return u;
 }
 
-// split-KV so that B*H*nsplit CTAs cover the 148 SMs a few times over even at B = 1
+// split-KV so that B*H*nsplit CTAs cover the 132 SMs a few times over even at B = 1
 inline int attn_pick_splits(int B, int H, int cap) {
   int ns = (148 * 4 + B * H - 1) / (B * H);
   if (ns < 1) ns = 1;

@@ -2,7 +2,7 @@
 // Reference orchestration: moshi/moshi/models/compression.py:338-433.
 //
 // Everything between the PCM frame and the latent is TOKEN-MAJOR ([session][step][channel]): every SEANet conv / transposed
-// conv and every transformer linear is one launch of mimi_tc_kernel (TMA + tcgen05 kind::tf32 with 3xTF32 split products,
+// conv and every transformer linear is one launch of mimi_tc_kernel (TMA + wgmma tf32 with 3xTF32 split products,
 // mimi_tc.cuh); a layer's epilogue writes its consumer's activation (ELU applied, hi / lo pair) straight behind the
 // consumer's carried left context, so that `cat(previous, x)` (conv.py:261) is an address, the streaming-state update
 // (conv.py:263-267) is a P-row shift inside that buffer, and ProjectedTransformer.conv_layout (transformer.py:972-981)

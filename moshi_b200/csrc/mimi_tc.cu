@@ -1,4 +1,4 @@
-// mimi_tc_kernel: persistent TMA + tcgen05 kind::tf32 implicit GEMM with 3xTF32 split products (see mimi_tc.cuh).
+// mimi_tc_kernel: persistent TMA + wgmma tf32 implicit GEMM with 3xTF32 split products (see mimi_tc.cuh).
 #include <cstdlib>
 #include <cstring>
 
@@ -40,10 +40,10 @@ __device__ __forceinline__ void store_row_chunk(const TcParams& p, int b, int t,
   } else if (p.epi == TC_EPI_RES_SCALE) {                       // x + layer_scale * update (transformer.py:769,777)
     const float* r = p.res + (long long)b * p.r_sb + (long long)t * p.r_row + n0;
 #pragma unroll
-    for (int i = 0; i < V; i += 4) {
-      const float4 rv = *reinterpret_cast<const float4*>(r + i);
-      const float4 sv = *reinterpret_cast<const float4*>(p.scale + n0 + i);
-      v[i] = rv.x + sv.x * v[i]; v[i + 1] = rv.y + sv.y * v[i + 1]; v[i + 2] = rv.z + sv.z * v[i + 2]; v[i + 3] = rv.w + sv.w * v[i + 3];
+    for (int i = 0; i < V; i += 2) {
+      const float2 rv = *reinterpret_cast<const float2*>(r + i);
+      const float2 sv = *reinterpret_cast<const float2*>(p.scale + n0 + i);
+      v[i] = rv.x + sv.x * v[i]; v[i + 1] = rv.y + sv.y * v[i + 1];
     }
   } else {
     if (p.bias != nullptr) {
@@ -53,16 +53,16 @@ __device__ __forceinline__ void store_row_chunk(const TcParams& p, int b, int t,
     if (p.res != nullptr) {                                     // SEANetResnetBlock: u + v (seanet.py:90-93)
       const float* r = p.res + (long long)b * p.r_sb + (long long)t * p.r_row + n0;
 #pragma unroll
-      for (int i = 0; i < V; i += 4) {
-        const float4 rv = *reinterpret_cast<const float4*>(r + i);
-        v[i] += rv.x; v[i + 1] += rv.y; v[i + 2] += rv.z; v[i + 3] += rv.w;
+      for (int i = 0; i < V; i += 2) {
+        const float2 rv = *reinterpret_cast<const float2*>(r + i);
+        v[i] += rv.x; v[i + 1] += rv.y;
       }
     }
   }
   if (p.y != nullptr) {
     float* y = p.y + (long long)b * p.y_sb + (long long)t * p.y_row + n0;
 #pragma unroll
-    for (int i = 0; i < V; i += 4) *reinterpret_cast<float4*>(y + i) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
+    for (int i = 0; i < V; i += 2) *reinterpret_cast<float2*>(y + i) = make_float2(v[i], v[i + 1]);
   }
   if (p.act_mode != TC_ACT_NONE) {
     if (p.act_elu) {
@@ -72,55 +72,49 @@ __device__ __forceinline__ void store_row_chunk(const TcParams& p, int b, int t,
     const long long o = (long long)b * p.a_sb + (long long)t * p.a_row + n0;
     if (p.act_mode == TC_ACT_FULL) {
 #pragma unroll
-      for (int i = 0; i < V; i += 4) *reinterpret_cast<float4*>(p.a_hi + o + i) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
+      for (int i = 0; i < V; i += 2) *reinterpret_cast<float2*>(p.a_hi + o + i) = make_float2(v[i], v[i + 1]);
     } else {
       float lo[V];
 #pragma unroll
       for (int i = 0; i < V; ++i) split_tf32(v[i], v[i], lo[i]);
 #pragma unroll
-      for (int i = 0; i < V; i += 4) {
-        *reinterpret_cast<float4*>(p.a_hi + o + i) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-        *reinterpret_cast<float4*>(p.a_lo + o + i) = make_float4(lo[i], lo[i + 1], lo[i + 2], lo[i + 3]);
+      for (int i = 0; i < V; i += 2) {
+        *reinterpret_cast<float2*>(p.a_hi + o + i) = make_float2(v[i], v[i + 1]);
+        *reinterpret_cast<float2*>(p.a_lo + o + i) = make_float2(lo[i], lo[i + 1]);
       }
     }
   }
 }
 
+// NC: wgmma width; NT = nch * NC output features per tile (NC = 128 for full tiles, 16 for the narrow layers)
+template <int NC>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 mimi_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo, const TcParams p) {
+  constexpr int MAXC = TC_MAX_NT / NC;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;                 // SWIZZLE_128B tiles need 1024 B alignment
   const uint32_t bars = base + (uint32_t)p.stages * p.stage_bytes;
-  const uint32_t full0 = bars, empty0 = bars + 8 * TC_MAX_STAGES, tfull0 = bars + 16 * TC_MAX_STAGES, tempty0 = tfull0 + 16;
-  const uint32_t tptr = tempty0 + 16;
-  uint32_t* tptr_generic = reinterpret_cast<uint32_t*>(smem_raw + (tptr - raw));
+  const uint32_t full0 = bars, empty0 = bars + 8 * TC_MAX_STAGES;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_tiles = p.m_tiles * p.n_tiles_n * p.ksplit;
   const uint32_t w_bytes = (uint32_t)p.NT * 128u;               // one weight tile (hi or lo)
   const int cb_per_tap = p.Cin / TC_KB;
+  const int nch = p.NT / NC;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == TC_PRODUCER_WARP && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_hi) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_lo) : "memory");
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(full0 + 8 * s, 1);
-      mbar_init(empty0 + 8 * s, 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull0 + 8 * a, 1);
-      mbar_init(tempty0 + 8 * a, 4);           // one arrival per epilogue warp
+      mbar_init(empty0 + 8 * s, TC_CONSUMERS / 32);   // one arrival per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) tmem_alloc(tptr, p.tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tptr_generic;
   pdl_trigger();                                 // the next kernel of the frame may begin its own prologue and weight prefetch
 
-  if (warp == 0) {
+  if (warp == TC_PRODUCER_WARP) {
     if (lane == 0) {
       // ===== producer =====
       // Programmatic dependent launch: the weights do not depend on the preceding kernel, so the first `stages` weight pairs of
@@ -156,79 +150,64 @@ mimi_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ===== MMA issuer: per k-block 4 k-steps x (hi*hi + hi*lo + lo*hi) =====
-      const uint32_t idesc = make_idesc_tf32(TC_ROWS, p.NT);
-      int s = 0; uint32_t ph = 0;
-      int acc = 0; uint32_t acc_bits = 0u;
-      for (int id = blockIdx.x; id < n_tiles; id += gridDim.x) {
-        const Tile tl = tile_at(p, id);
-        mbar_wait(tempty0 + 8 * acc, ((acc_bits >> acc) & 1u) ^ 1u);
-        tc_fence_after();
-        const uint32_t d0 = tmem_base + (uint32_t)(acc * p.NT);
-        for (int kb = tl.kb0; kb < tl.kb1; ++kb) {
-          mbar_wait(full0 + 8 * s, ph);
-          tc_fence_after();
-          const uint32_t a_hi = base + (uint32_t)s * p.stage_bytes, a_lo = a_hi + A_TILE_BYTES;
-          const uint32_t w_hi = a_lo + A_TILE_BYTES, w_lo = w_hi + w_bytes;
+    return;
+  }
+  // ===== consumers: warpgroup wg owns GEMM rows 64 wg .. 64 wg + 63 (one (session, step) each) of every tile =====
+  const int wg = warp >> 2, t = threadIdx.x & 127;
+  uint32_t d[MAXC][NC / 2];
+  int s = 0; uint32_t ph = 0;
+  pdl_wait();                                    // outputs / residuals / the split-K workspace may still be in use by the predecessor
+  for (int id = blockIdx.x; id < n_tiles; id += gridDim.x) {
+    const Tile tl = tile_at(p, id);
+    for (int kb = tl.kb0; kb < tl.kb1; ++kb) {
+      mbar_wait(full0 + 8 * s, ph);
+      const uint32_t a_hi = base + (uint32_t)s * p.stage_bytes + (uint32_t)wg * (A_TILE_BYTES / 2), a_lo = a_hi + A_TILE_BYTES;
+      const uint32_t w_hi = base + (uint32_t)s * p.stage_bytes + 2 * A_TILE_BYTES, w_lo = w_hi + w_bytes;
+      // per k-block 4 k-steps x (lo*hi + hi*lo + hi*hi): small terms first
+      wg_fence();
 #pragma unroll
-          for (int k = 0; k < TC_KB / 8; ++k) {
-            const uint32_t off = (uint32_t)k * 32u;          // 8 tf32 = 32 bytes of K per MMA
-            const uint32_t first = (kb == tl.kb0 && k == 0) ? 0u : 1u;
-            umma_tf32(d0, make_desc(a_lo + off), make_desc(w_hi + off), idesc, first);      // small terms first
-            umma_tf32(d0, make_desc(a_hi + off), make_desc(w_lo + off), idesc, 1u);
-            umma_tf32(d0, make_desc(a_hi + off), make_desc(w_hi + off), idesc, 1u);
+      for (int k = 0; k < TC_KB / 8; ++k) {
+        const uint32_t off = (uint32_t)k * 32u;          // 8 tf32 = 32 bytes of K per MMA
+        const uint32_t first = (kb == tl.kb0 && k == 0) ? 0u : 1u;
+#pragma unroll
+        for (int c = 0; c < MAXC; ++c) {
+          if (c < nch) {
+            const uint32_t wc = (uint32_t)(c * NC) * 128u + off;
+            Wgmma<NC>::tf32(d[c], make_desc(a_lo + off), make_desc(w_hi + wc), first);
+            Wgmma<NC>::tf32(d[c], make_desc(a_hi + off), make_desc(w_lo + wc), 1u);
+            Wgmma<NC>::tf32(d[c], make_desc(a_hi + off), make_desc(w_hi + wc), 1u);
           }
-          umma_commit(empty0 + 8 * s);
-          if (++s == p.stages) { s = 0; ph ^= 1u; }
-        }
-        umma_commit(tfull0 + 8 * acc);
-        acc_bits ^= 1u << acc;
-        acc ^= 1;
-      }
-    }
-    __syncwarp();
-  } else {
-    // ===== epilogue: TMEM lane = GEMM row = one (session, step) =====
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    const int bi = row / p.tt, ti = row - bi * p.tt;
-    int acc = 0; uint32_t acc_bits = 0u;
-    pdl_wait();                                  // outputs / residuals / the split-K workspace may still be in use by the predecessor
-    for (int id = blockIdx.x; id < n_tiles; id += gridDim.x) {
-      const Tile tl = tile_at(p, id);
-      const int b = tl.b0 + bi, t = tl.t0 + ti;
-      const bool valid = b < p.n_sessions && t < p.T;
-      mbar_wait(tfull0 + 8 * acc, (acc_bits >> acc) & 1u);
-      tc_fence_after();
-      const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * p.NT);
-      const int n_base = tl.n * p.NT;
-      for (int c0 = 0; c0 < p.NT; c0 += 16) {
-        uint32_t r[16];
-        tmem_ld16(lane_addr + (uint32_t)c0, r);
-        tmem_ld_wait();
-        float v[16];
-#pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(r[j]);
-        if (p.ksplit > 1) {
-          float* w = p.ws + ((size_t)tl.split * p.m_tiles * TC_ROWS + (size_t)tl.m * TC_ROWS + row) * (size_t)p.N + n_base + c0;
-#pragma unroll
-          for (int j = 0; j < 16; j += 4) __stcg(reinterpret_cast<float4*>(w + j), make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]));
-        } else if (valid) {
-          store_row_chunk<16>(p, b, t, n_base + c0, v);
         }
       }
-      tc_fence_before();
+      wg_commit();
+      wg_wait<0>();
+#pragma unroll
+      for (int c = 0; c < MAXC; ++c) wg_hold(d[c]);
       __syncwarp();
-      if (lane == 0) mbar_arrive(tempty0 + 8 * acc);
-      acc_bits ^= 1u << acc;
-      acc ^= 1;
+      if (lane == 0) mbar_arrive(empty0 + 8 * s);
+      if (++s == p.stages) { s = 0; ph ^= 1u; }
+    }
+    // epilogue straight from the fragments: element pair (i, i + 1) = features n, n + 1 of GEMM row `row`
+    const int n_base = tl.n * p.NT;
+#pragma unroll
+    for (int c = 0; c < MAXC; ++c) {
+      if (c < nch) {
+#pragma unroll
+        for (int i = 0; i < NC / 2; i += 2) {
+          const int row = 64 * wg + frag_row(t, i), n = n_base + c * NC + frag_col(t, i);
+          const int bi = row / p.tt, ti = row - bi * p.tt;
+          const int b = tl.b0 + bi, tt = tl.t0 + ti;
+          float v[2] = {__uint_as_float(d[c][i]), __uint_as_float(d[c][i + 1])};
+          if (p.ksplit > 1) {
+            float* w = p.ws + ((size_t)tl.split * p.m_tiles * TC_ROWS + (size_t)tl.m * TC_ROWS + row) * (size_t)p.N + n;
+            __stcg(reinterpret_cast<float2*>(w), make_float2(v[0], v[1]));
+          } else if (b < p.n_sessions && tt < p.T) {
+            store_row_chunk<2>(p, b, tt, n, v);
+          }
+        }
+      }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, p.tmem_cols);
 }
 
 // split-K: sum the partials in split order (deterministic) and run the epilogue; one thread per (row, 4 features)
@@ -296,7 +275,8 @@ int tc_init() {
     g_encode = reinterpret_cast<EncodeTiledFn>(fn);
   }
   if (!g_attr) {
-    B200_CUDA(cudaFuncSetAttribute(mimi_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+    B200_CUDA(cudaFuncSetAttribute(mimi_tc_kernel<TC_MAX_NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+    B200_CUDA(cudaFuncSetAttribute(mimi_tc_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
     g_attr = true;
   }
   return B200_OK;
@@ -362,9 +342,6 @@ int tc_plan(TcLayer& L, int n_sessions, int T, int sms, size_t ws_bytes) {
   int stages = (200 * 1024) / (int)p.stage_bytes;
   if (stages > TC_MAX_STAGES) stages = TC_MAX_STAGES;
   p.stages = stages;
-  uint32_t cols = 32;
-  while (cols < (uint32_t)(2 * p.NT)) cols <<= 1;
-  p.tmem_cols = cols;
   const long long tiles = mn * p.ksplit;
   L.grid = (int)(tiles < sms ? tiles : sms);
   L.smem = (size_t)stages * p.stage_bytes + 1024 + 16 * TC_MAX_STAGES + 64;
@@ -382,7 +359,8 @@ int tc_launch(const TcLayer& L, cudaStream_t st) {
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
-  const cudaError_t le = cudaLaunchKernelEx(&cfg, mimi_tc_kernel, L.map_hi, L.map_lo, L.p);
+  const cudaError_t le = L.p.NT == TC_MAX_NT ? cudaLaunchKernelEx(&cfg, mimi_tc_kernel<TC_MAX_NT>, L.map_hi, L.map_lo, L.p)
+                                             : cudaLaunchKernelEx(&cfg, mimi_tc_kernel<16>, L.map_hi, L.map_lo, L.p);
   if (le != cudaSuccess) B200_FAIL(B200_ERR_CUDA, "mimi_tc launch failed: %s", cudaGetErrorString(le));
   g_launches.fetch_add(1, std::memory_order_relaxed);
   if (L.p.ksplit > 1) {

@@ -1,6 +1,6 @@
-// Mimi's contractions on the 5th-generation tensor cores: every StreamingConv1d / StreamingConvTranspose1d of the SEANet
+// Mimi's contractions on the Hopper tensor cores: every StreamingConv1d / StreamingConvTranspose1d of the SEANet
 // (conv.py:245-274, 340-362; seanet.py:90-93) and every nn.Linear of the two bottleneck transformers (transformer.py:752-777)
-// is one launch of mimi_tc_kernel, a persistent TMA + tcgen05 (kind::tf32) implicit GEMM with fp32-equivalent accuracy:
+// is one launch of mimi_tc_kernel, a persistent TMA + wgmma (tf32) implicit GEMM with fp32-equivalent accuracy:
 //
 //     out[token][n] = epi( sum_{tap, ci} act[session][row0 + t * stride + tap * dil][ci] * w[n][tap][ci] )
 //
@@ -15,13 +15,14 @@
 //     overlap-add carry of conv.py:349-361 becomes one carried input row (x[-1] of the next frame).
 //   * 3xTF32: a = a_hi + a_lo with a_hi = tf32(a) and a_lo = tf32(a - a_hi) (both round-to-nearest, written by the producing
 //     epilogue), likewise for the weights at load; the product is a_hi*w_hi + a_hi*w_lo + a_lo*w_hi with fp32 accumulation
-//     in TMEM (dropped terms <= 2^-22 relative).  The RVQ indices downstream stay exact up to the margin the parity tests
+//     in registers (dropped terms <= 2^-22 relative).  The RVQ indices downstream stay exact up to the margin the parity tests
 //     define (tests/util.py).
-//   * Warp roles (192 threads): warp 0 = TMA producer (A hi + A lo boxes, one contiguous bulk copy of the pre-tiled weight
-//     pair per k-block), warp 1 = TMEM owner + single-thread MMA issuer, warps 2-5 = epilogue (TMEM lane = GEMM row = one
-//     token: bias, residual, ELU / GELU / layer-scale, hi/lo split, 64-byte contiguous stores).  Persistent grid, two TMEM
-//     accumulator stages: the epilogue of a tile overlaps the MMAs of the next.  Deep-and-skinny layers are cut along K into
-//     fp32 partials reduced in split order by mimi_tc_reduce_kernel (deterministic).
+//   * Warp roles (288 threads): warp 8 = TMA producer (A hi + A lo boxes, one contiguous bulk copy of the pre-tiled weight
+//     pair per k-block), warps 0-7 = two consumer warpgroups, each owning 64 GEMM rows (tokens) of the tile: wgmma into
+//     register accumulators, then the epilogue straight from the fragments (bias, residual, ELU / GELU / layer-scale, hi/lo
+//     split).  Persistent grid; the producer runs ahead through the stage ring while the consumers finish a tile.
+//     Deep-and-skinny layers are cut along K into fp32 partials reduced in split order by mimi_tc_reduce_kernel
+//     (deterministic).
 #pragma once
 
 #include <cuda.h>
@@ -31,10 +32,12 @@
 namespace b200 {
 namespace mtc {
 
-constexpr int TC_ROWS = 128;            // GEMM rows (tokens) per tile = UMMA M
+constexpr int TC_ROWS = 128;            // GEMM rows (tokens) per tile: 64 per consumer warpgroup
 constexpr int TC_KB = 32;               // fp32 elements per k-block row: 128 bytes = one SWIZZLE_128B row
-constexpr int TC_MAX_NT = 128;          // output features per tile = UMMA N (<= 128: 64 KB per stage, 3 stages)
-constexpr int TC_THREADS = 192;
+constexpr int TC_MAX_NT = 128;          // output features per tile = wgmma N (<= 128: 64 KB per stage, 3 stages)
+constexpr int TC_THREADS = 288;         // warps 0-7: two consumer warpgroups (MMA + epilogue), warp 8: producer
+constexpr int TC_PRODUCER_WARP = 8;
+constexpr int TC_CONSUMERS = 256;
 constexpr int TC_MAX_STAGES = 6;
 
 enum { TC_EPI_CONV = 0, TC_EPI_GELU = 1, TC_EPI_RES_SCALE = 2 };
@@ -59,7 +62,7 @@ struct TcParams {
   const float* scale;                              // lin RES_SCALE: per-feature layer scale
   int act_mode, act_elu;
   float *a_hi, *a_lo; long long a_sb, a_row;       // activated copy for the consumer: a[b * a_sb + t * a_row + n]
-  uint32_t stage_bytes, tmem_cols; int stages;
+  uint32_t stage_bytes; int stages;
 };
 
 // y = hi + lo with hi = tf32(y) and lo = tf32(y - hi), both round-to-nearest (cvt.rna): |y - hi - lo| <= 2^-23 |y|

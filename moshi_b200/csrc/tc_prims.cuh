@@ -1,9 +1,12 @@
-// sm_100a primitives shared by the tensor-core kernels (gemm_sk.cu, dep_fused.cu, mimi_tc.cu): mbarriers, bulk / tensor
-// TMA copies, TMEM allocation, tcgen05.mma / commit / ld, UMMA descriptors, programmatic dependent launch.
+// sm_90a primitives shared by the tensor-core kernels (gemm_sk.cu, gemm_ns.cu, dep_fused.cu, mimi_tc.cu): mbarriers, bulk /
+// tensor TMA copies, warpgroup MMA (wgmma) fences and fragment coordinates, shared-memory matrix descriptors, programmatic
+// dependent launch.
 #pragma once
 
 #include <cuda.h>
 #include <stdint.h>
+
+#include "wgmma_ops.cuh"
 
 namespace b200 {
 namespace tcp {
@@ -56,77 +59,38 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
   asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
                ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// Warpgroup MMA (wgmma): the four warps of a warpgroup issue together; `wg_fence` orders register / shared-memory writes
+// before the MMAs that read them, `wg_commit` closes a group of issued MMAs, `wg_wait<n>` waits until at most n groups are
+// still in flight (their accumulator registers and the shared-memory operands they read are then free).
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of an accumulator across the asynchronous MMAs that own it
+template <int R>
+__device__ __forceinline__ void wg_hold(uint32_t (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+r"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_i8(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t* r) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// (row, column) of accumulator element i of an m64nN fragment, for thread t (0..127) of its warpgroup
+__device__ __forceinline__ int frag_row(int t, int i) { return 16 * (t >> 5) + ((t & 31) >> 2) + 8 * ((i >> 1) & 1); }
+__device__ __forceinline__ int frag_col(int t, int i) { return 8 * (i >> 2) + 2 * (t & 3) + (i & 1); }
+// named barrier over `count` threads (ids 1..15; 0 is __syncthreads)
+__device__ __forceinline__ void named_bar(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 // Programmatic dependent launch: `pdl_wait` blocks until the preceding kernel in the stream has completed and its
 // writes are visible; `pdl_trigger` lets the following kernel start its own prologue (and weight prefetch) early.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-// K-major SWIZZLE_128B shared-memory matrix descriptor: start address >> 4, LBO = 1 (unused for swizzled K-major), SBO = 1024 B
-// (8 rows x 128 B), descriptor version 1 (bit 46), layout type 2 = SWIZZLE_128B (bits 61-63).
+// K-major SWIZZLE_128B shared-memory matrix descriptor (sm_90): start address >> 4 (bits 0-13), leading byte offset 1 (unused
+// for swizzled K-major), stride byte offset 1024 B >> 4 (8 rows x 128 B, bits 32-45), layout type 1 = SWIZZLE_128B (bits 62-63).
+// Tiles are 1024-byte aligned, so the base offset (bits 49-51) is 0; a K step inside the 128-byte row adds its byte offset.
 __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
   uint64_t d = (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
-}
-// instruction descriptors: D format at bit 4 (1 = f32, 2 = s32), A / B formats at bits 7 / 10, N >> 3 at bit 17, M >> 4 at bit 24;
-// both operands K-major.  kind::f16: A = B = bf16 (1); kind::tf32: A = B = tf32 (2); kind::i8: A = B = signed 8 bit (1).
-__device__ __forceinline__ uint32_t make_idesc(int umma_m, int umma_n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(umma_n >> 3) << 17) | ((uint32_t)(umma_m >> 4) << 24);
-}
-__device__ __forceinline__ uint32_t make_idesc_tf32(int umma_m, int umma_n) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(umma_n >> 3) << 17) | ((uint32_t)(umma_m >> 4) << 24);
-}
-__device__ __forceinline__ uint32_t make_idesc_i8(int umma_m, int umma_n) {
-  return (2u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(umma_n >> 3) << 17) | ((uint32_t)(umma_m >> 4) << 24);
 }
 
 }  // namespace tcp

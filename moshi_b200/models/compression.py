@@ -1,4 +1,4 @@
-"""``MimiModel`` with the reference's public surface, backed by the sm_100a library.
+"""``MimiModel`` with the reference's public surface, backed by the sm_90a library.
 
 Mirrors ``moshi/moshi/models/compression.py:97-433`` (properties, ``encode`` / ``decode`` /
 ``encode_to_latent`` / ``decode_latent``) and the ``StreamingModule`` protocol of
@@ -37,7 +37,7 @@ def _config_struct(cfg: MimiConfig) -> _lib.MimiConfigC:
 
 
 class MimiModel:
-    """Mimi on one B200.  Construct through ``loaders.get_mimi``."""
+    """Mimi on one GPU.  Construct through ``loaders.get_mimi``."""
 
     def __init__(self, cfg: MimiConfig, state_dict: tp.Mapping[str, torch.Tensor],
                  device: torch.device | str = "cuda"):

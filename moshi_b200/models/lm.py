@@ -1,4 +1,4 @@
-"""``LMModel`` / ``LMGen`` with the reference's public surface, backed by the sm_100a library.
+"""``LMModel`` / ``LMGen`` with the reference's public surface, backed by the sm_90a library.
 
 Mirrors ``moshi/moshi/models/lm.py``: ``LMModel`` exposes the attributes callers read
 (``dep_q, n_q, card, text_card, delays, device, dtype, num_codebooks, condition_provider, fuser, ...``,
@@ -44,13 +44,13 @@ def _config_struct(cfg: LMConfig) -> _lib.LMConfigC:
 
 
 class LMModel:
-    """Moshi Temporal + Depth transformer weights on one B200.  Construct via ``loaders.get_moshi_lm``."""
+    """Moshi Temporal + Depth transformer weights on one GPU.  Construct via ``loaders.get_moshi_lm``."""
 
     def __init__(self, cfg: LMConfig, tensors: tp.Iterable[tuple[str, torch.Tensor]] | tp.Mapping[str, torch.Tensor],
                  device: torch.device | str = "cuda", dtype: torch.dtype = torch.bfloat16):
         cfg.check_supported()
         if dtype != torch.bfloat16:
-            raise ValueError("the B200 LM path computes in bfloat16 (reference default, loaders.py:370)")
+            raise ValueError("the GPU LM path computes in bfloat16 (reference default, loaders.py:370)")
         self.cfg = cfg
         self.device = torch.device(device)
         if self.device.type != "cuda":

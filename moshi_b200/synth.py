@@ -4,7 +4,7 @@ There are no real weights in the build/bench environment (no network), so parity
 fixture generator and both bench arms use these.  Key names and tensor shapes follow what
 ``loaders.get_mimi(None)`` / ``LMModel(**cfg)`` produce in the reference (SURVEY.md appendix A;
 ``moshi/moshi/models/loaders.py:323-361``, ``lm.py:140-252``), so the same dict loads into the
-reference modules (``load_state_dict``), into the CPU oracle and into the B200 handles.
+reference modules (``load_state_dict``), into the CPU oracle and into the GPU handles.
 
 Values are drawn from a ``torch.Generator`` on the requested device.  Parity work always draws on
 the CPU (bit-reproducible across machines for a given torch build) and copies; the 7B bench draws on

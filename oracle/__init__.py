@@ -7,6 +7,6 @@ TEST INFRASTRUCTURE ONLY.  Nothing under ``moshi_b200/`` imports this package; i
 The oracle restates, as plain functional PyTorch-on-CPU code with explicit state, the algorithms of
 the reference's PyTorch path (each function cites the reference ``file:line`` it follows).  It is
 pinned against the unmodified reference by ``oracle/gen_golden.py`` (run in the build container,
-where ``/root/reference`` exists) — see ``tests/golden/MANIFEST.json`` for what was compared and the
+where ``$MOSHI_REFERENCE`` exists) — see ``tests/golden/MANIFEST.json`` for what was compared and the
 fixtures that travel to the GPU box.
 """

@@ -1,6 +1,6 @@
-"""Generates ``tests/golden/*`` by running the UNMODIFIED reference (``/root/reference/moshi``, CPU).
+"""Generates ``tests/golden/*`` by running the UNMODIFIED reference (``$MOSHI_REFERENCE/moshi``, CPU).
 
-Run in the build container only (the GPU box has no ``/root/reference``):
+Run in the build container only (needs a checkout of the reference, ``MOSHI_REFERENCE``):
 
     python -m oracle.gen_golden
 
@@ -20,7 +20,7 @@ from pathlib import Path
 os.environ["NO_TORCH_COMPILE"] = "1"
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
-sys.path.insert(0, "/root/reference/moshi")
+sys.path.insert(0, os.path.join(os.environ.get("MOSHI_REFERENCE", ""), "moshi"))   # a checkout of kyutai-labs/moshi
 
 import torch  # noqa: E402
 from safetensors.torch import save_file  # noqa: E402
@@ -139,8 +139,8 @@ def main() -> None:
     GOLDEN.mkdir(parents=True, exist_ok=True)
     manifest: dict = {
         "generated_by": "oracle/gen_golden.py", "torch": torch.__version__,
-        "reference": "/root/reference/moshi (moshi 0.2.x, unmodified, CPU, NO_TORCH_COMPILE=1)",
-        "reference_test_lm": "copied verbatim from /root/reference/moshi/tests/assets (KAT of tests/test_lm.py)",
+        "reference": "kyutai-labs/moshi python package (moshi 0.2.x, unmodified, CPU, NO_TORCH_COMPILE=1)",
+        "reference_test_lm": "copied verbatim from the reference's moshi/tests/assets (KAT of tests/test_lm.py)",
     }
     mimi_fixtures(manifest)
     lm_fixtures(manifest)

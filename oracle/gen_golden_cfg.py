@@ -1,6 +1,6 @@
 """Generates ``tests/golden/lm_tiny_cfg.safetensors``: classifier-free guidance without a conditioner (``LMGen(cfg_coef != 1,
 cfg_is_no_text / cfg_is_masked_until)``, lm.py:596-604, 646-662, 714-732, 820-833) on the tiny LM, run through the UNMODIFIED
-reference (CPU); records whether the oracle agrees bit for bit.  Build container only (needs /root/reference):
+reference (CPU); records whether the oracle agrees bit for bit.  Build container only (needs $MOSHI_REFERENCE):
 
     python -m oracle.gen_golden_cfg
 
@@ -16,7 +16,7 @@ from pathlib import Path
 os.environ["NO_TORCH_COMPILE"] = "1"
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
-sys.path.insert(0, "/root/reference/moshi")
+sys.path.insert(0, os.path.join(os.environ.get("MOSHI_REFERENCE", ""), "moshi"))   # a checkout of kyutai-labs/moshi
 
 import torch  # noqa: E402
 from safetensors.torch import save_file  # noqa: E402

@@ -4,7 +4,7 @@ UNMODIFIED reference (CPU).  The conditioners run once per session outside the s
 what reaches the hot path is ``condition_sum`` [B or 2B, 1, dim], added to the summed input embeddings every step
 (lm.py:398-399).  The fixture stores the reference's ``condition_sum`` and its tokens; the oracle restates the step.
 
-    python -m oracle.gen_golden_cond          # build container only: needs /root/reference
+    python -m oracle.gen_golden_cond          # build container only: needs $MOSHI_REFERENCE
 """
 from __future__ import annotations
 
@@ -16,7 +16,7 @@ from pathlib import Path
 os.environ["NO_TORCH_COMPILE"] = "1"
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
-sys.path.insert(0, "/root/reference/moshi")
+sys.path.insert(0, os.path.join(os.environ.get("MOSHI_REFERENCE", ""), "moshi"))   # a checkout of kyutai-labs/moshi
 
 import torch  # noqa: E402
 from safetensors.torch import save_file  # noqa: E402

@@ -1,6 +1,6 @@
 """Generates ``tests/golden/lm_tiny_delay2.safetensors``: a member of the family with the acoustic delay pattern of the 2B
 configuration (``configs/moshi_dev_2b.json``: delays up to 2) run through the UNMODIFIED reference (CPU), and records whether
-the oracle agrees bit for bit.  Build container only (needs /root/reference):
+the oracle agrees bit for bit.  Build container only (needs $MOSHI_REFERENCE):
 
     python -m oracle.gen_golden_delay2
 """
@@ -14,7 +14,7 @@ from pathlib import Path
 os.environ["NO_TORCH_COMPILE"] = "1"
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
-sys.path.insert(0, "/root/reference/moshi")
+sys.path.insert(0, os.path.join(os.environ.get("MOSHI_REFERENCE", ""), "moshi"))   # a checkout of kyutai-labs/moshi
 
 import torch  # noqa: E402
 from safetensors.torch import save_file  # noqa: E402

@@ -1,7 +1,7 @@
 """Generates ``tests/golden/lm_tiny_sampled_peaked.safetensors``: 30 sampled ``LMGen.step`` calls of the UNMODIFIED reference
 (CPU, global Philox generator seeded with ``scenarios.LM_NOISE_SEED``) on the tiny LM with peaked output distributions
 (``scenarios.peaked_state_dict``), with the exec-mask / reset events of ``scenarios.lm_mask_events``; records whether the oracle,
-fed the same Exp(1) draws explicitly, reproduces every token.  Build container only (needs /root/reference):
+fed the same Exp(1) draws explicitly, reproduces every token.  Build container only (needs $MOSHI_REFERENCE):
 
     python -m oracle.gen_golden_peaked
 """
@@ -15,7 +15,7 @@ from pathlib import Path
 os.environ["NO_TORCH_COMPILE"] = "1"
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
-sys.path.insert(0, "/root/reference/moshi")
+sys.path.insert(0, os.path.join(os.environ.get("MOSHI_REFERENCE", ""), "moshi"))   # a checkout of kyutai-labs/moshi
 
 import torch  # noqa: E402
 from safetensors.torch import save_file  # noqa: E402

@@ -2,7 +2,7 @@
 ``oracle/scenarios.py`` (no depformer, ``extra_heads``; ``LMGen.step_with_extra_heads``, lm.py:793-807 — what
 ``rust/moshi-server/batched_asr.py:197`` calls), and records whether the oracle agrees bit for bit.
 
-    python -m oracle.gen_golden_stt          # build container only: needs /root/reference
+    python -m oracle.gen_golden_stt          # build container only: needs $MOSHI_REFERENCE
 
 Test infrastructure for the next row of SURVEY.md 8(f) item 2; the CUDA path does not implement this configuration yet.
 """
@@ -16,7 +16,7 @@ from pathlib import Path
 os.environ["NO_TORCH_COMPILE"] = "1"
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
-sys.path.insert(0, "/root/reference/moshi")
+sys.path.insert(0, os.path.join(os.environ.get("MOSHI_REFERENCE", ""), "moshi"))   # a checkout of kyutai-labs/moshi
 
 import torch  # noqa: E402
 from safetensors.torch import save_file  # noqa: E402

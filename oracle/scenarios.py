@@ -1,7 +1,7 @@
 """Seeded inputs and mask/reset schedules shared by the golden generator and the tests.
 
 Any object with ``set_exec_mask`` / ``reset_streaming`` works (reference modules, the oracle, the
-B200 shims): the same schedule drives all three.
+GPU shims): the same schedule drives all three.
 """
 from __future__ import annotations
 

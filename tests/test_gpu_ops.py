@@ -24,7 +24,7 @@ def _stream():
 @pytest.mark.parametrize("M,N,K", [(1, 512, 256), (3, 1024, 4096), (8, 12288, 4096), (17, 4096, 11264),
                                    (96, 4096, 4096), (128, 2048, 1024), (200, 1024, 2816), (5, 200, 72)])
 def test_linear_bf16(lib, M, N, K):
-    """The LM's linear on row-major weights (packed on the fly): GEMV kernel at M <= 2, tcgen05 kernels above."""
+    """The LM's linear on row-major weights (packed on the fly): GEMV kernel at M <= 2, wgmma kernels above."""
     from moshi_b200 import _lib
     g = torch.Generator().manual_seed(M * 7 + N)
     x = torch.randn(M, K, generator=g).bfloat16().cuda()

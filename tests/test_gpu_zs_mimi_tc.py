@@ -1,4 +1,4 @@
-"""GPU: mimi_tc_kernel (TMA + tcgen05 kind::tf32 with 3xTF32 split products) at the op level: accuracy against float64, and
+"""GPU: mimi_tc_kernel (TMA + wgmma tf32 with 3xTF32 split products) at the op level: accuracy against float64, and
 the conv / strided conv / dilated conv / transposed-conv geometry against torch on the reference's layouts."""
 import ctypes as C
 

@@ -1,4 +1,4 @@
-"""GPU: the int8 x int8 linear (tcgen05 kind::i8) against the CPU restatement of the reference's QLinear
+"""GPU: the int8 x int8 linear (wgmma s8 x s8 -> s32) against the CPU restatement of the reference's QLinear
 (oracle/quant.py; parity unpinned: bitsandbytes is absent, see that file).  Integer accumulation is exact, so the
 comparison is bit for bit: quantised weights, weight scales, quantised activations, activation scales, outputs."""
 import ctypes as C

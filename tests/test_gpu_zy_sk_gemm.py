@@ -1,4 +1,4 @@
-"""GPU: the stream-K tcgen05 GEMM over pre-tiled weights (csrc/gemm_sk.cu) against fp32 math.
+"""GPU: the stream-K wgmma GEMM over pre-tiled weights (csrc/gemm_sk.cu) against fp32 math.
 
 Covers the three epilogues of the LM (store, residual add, gated SiLU), ragged shapes, and work
 partitions that cut tiles into many / few / no partial segments; the partition must not change the
@@ -184,11 +184,11 @@ def _run_ns(lib, x, wt, res, M, N, K, epi, gate_rows, cluster=0):
                                         (128, 2048, 1024, STORE), (48, 32000, 4096, STORE), (104, 22528, 4096, GATE),
                                         (64, 5632, 1024, GATE), (40, 200, 520, RESADD), (5, 384, 72, STORE), (77, 608, 136, GATE),
                                         (104, 8192, 4096, STORE), (1, 256, 512, STORE),
-                                        # above 128 sessions: two blocks of 128 rows, two TMEM accumulators
+                                        # above 128 sessions: two launches of up to 128 rows
                                         (130, 1024, 1024, STORE), (200, 4096, 4096, RESADD), (256, 2048, 1024, STORE), (197, 5632, 1024, GATE),
                                         (197, 12288, 4096, STORE)])
 def test_ns_gemm(M, N, K, epi):
-    """The non-swapped kernel (csrc/gemm_ns.cu; the LM's linears at 33..128 sessions: activations = UMMA A, two weight tiles = B,
+    """The non-swapped kernel (csrc/gemm_ns.cu; the LM's linears at 33..128 sessions: activations = wgmma A, two weight tiles = B,
     N = 256; two 128-session blocks above 128) against fp32 math for the three epilogues, odd tile counts, ragged N / K, every cluster size (K cut over 1..8 CTAs,
     DSMEM reduce-scatter by output columns), bit-identical repeats, and against the swap-AB kernels (same weights, same cast
     points: a bf16 ulp apart now and then from the fp32 summation order)."""

@@ -74,9 +74,9 @@ def bench_gemm(lib, Ms, legacy=True, only="", ns_sweep=False):
             variants = [("lm", 0, 0, 0), ("swapAB", 0, -1, 0), ("swapAB.stream_only", 0, -1, 1)]
             if ns_sweep and M <= 128:
                 n_units = -(-(gr if epi == 2 else N) // 128) if epi == 2 else -(-N // 256)
-                variants += [(f"ns.cs{c}", -c, 0, 0) for c in ((1,) if epi == 2 else (1, 2, 3, 4, 8)) if n_units * c <= 148]
+                variants += [(f"ns.cs{c}", -c, 0, 0) for c in ((1,) if epi == 2 else (1, 2, 3, 4, 8)) if n_units * c <= torch.cuda.get_device_properties(0).multi_processor_count]
                 if epi != 2:
-                    variants += [(f"ns.n128.cs{c}", -(100 + c), 0, 0) for c in (1, 2, 4) if -(-N // 128) * c <= 148]
+                    variants += [(f"ns.n128.cs{c}", -(100 + c), 0, 0) for c in (1, 2, 4) if -(-N // 128) * c <= torch.cuda.get_device_properties(0).multi_processor_count]
             for vname, grid, smem, so in variants:
                 def fn(i):
                     if vname.startswith("ns."):
