@@ -359,7 +359,8 @@ int b200_op_quantize_rows(const void* x_dev, void* xq_dev, float* sa_dev, int M,
 int b200_op_linear_i8(const void* xq_dev, const float* sa_dev, const void* w_tiles_dev, const float* sw_dev, void* y_dev,
                       const void* res_dev, int M, int N, int K, int epi, int gate_rows, void* stream);
 /* StreamingConv1d.forward on one layer (conv.py:245-274): x [B,Cin,T], w [Cout,Cin,K], state
- * previous [B,Cin,Keff-S] (updated in place where exec_mask), y [B,Cout,T/S]. elu_in applies ELU to x. */
+ * previous [B,Cin,Keff-S] (updated in place where exec_mask), y [B,Cout,T/S]. elu_in applies ELU to x.
+ * Runs the kernels of the Mimi handle's down-sampling conv: split-K fp32 GEMM, in-order reduction, state commit. */
 int b200_op_conv1d(const float* x_dev, const float* w_dev, const float* bias_dev, float* prev_dev,
                    const uint8_t* exec_mask_dev, float* y_dev, int B, int Cin, int Cout, int T,
                    int K, int stride, int dilation, int elu_in, void* stream);

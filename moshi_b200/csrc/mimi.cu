@@ -17,6 +17,8 @@ using namespace b200::mimi;
 
 namespace {
 
+constexpr size_t kTcSplitBytes = (size_t)64 << 20;   // split-K partials budget of a tensor-core layer (tc_plan)
+
 struct SeaLayer {
   int kind = 0;              // 0 = StreamingConv1d, 1 = StreamingConvTranspose1d
   std::string key;           // state-dict prefix of the nn.Conv1d / nn.ConvTranspose1d
@@ -49,7 +51,7 @@ struct Transformer {
   long long* offset = nullptr;   // [B] tokens seen (== RingKVCache.end_offset == _MHAState.offset)
 };
 
-struct Tap { const float* p; int C, T; bool transpose; };
+struct Tap { const float* p; int C, T; bool transpose; };   // transpose: stored [B][T][C], reported [B][C][T]
 
 struct DownLayer {             // ConvDownsample1d (resample.py:14-65): k = 2 * stride, no bias, replicate padding
   std::string key;
@@ -58,7 +60,7 @@ struct DownLayer {             // ConvDownsample1d (resample.py:14-65): k = 2 * 
   float* w = nullptr;          // [Cout][K * Cin]
   float* state = nullptr;      // previous [B][Cin][P]
   uint8_t* first = nullptr;    // replicate flags [B]
-};     // transpose: stored [B][T][C], reported [B][C][T]
+};
 
 }  // namespace
 
@@ -75,7 +77,7 @@ struct b200_mimi {
   int sms = 148;
 
   std::vector<SeaLayer> enc, dec;
-  DownLayer down;                            // learnt down-sampling conv (replicate padding): first-generation SIMT kernel
+  DownLayer down;                            // learnt down-sampling conv (replicate padding): split-K fp32 SIMT kernels
   // up-sampling (depth-wise convtr)
   float *up_w = nullptr, *up_partial = nullptr, *up_scratch = nullptr;
   Transformer enc_tr, dec_tr;
@@ -89,16 +91,13 @@ struct b200_mimi {
   float *tr_xn_hi = nullptr, *tr_xn_lo = nullptr, *tr_qkv = nullptr, *tr_ao_hi = nullptr,
         *tr_ao_lo = nullptr, *tr_h_hi = nullptr, *tr_h_lo = nullptr;
   uint8_t* exec_mask = nullptr;
-  uint8_t* first_flags = nullptr; int n_first = 0;
-  ConvCommit* enc_commits = nullptr; int n_enc_commits = 0, max_enc_rows = 0;
-  ConvTrCommit* dec_tr_commits = nullptr; int n_dec_tr_commits = 0; long long max_tr_rows = 0;
   TmCommit *enc_tm = nullptr, *dec_tm = nullptr; int n_enc_tm = 0, n_dec_tm = 0; long long max_enc_tm = 0, max_dec_tm = 0;
   long long* scratch_codes = nullptr;          // [B][K][1] for the host variants
   float* rvq_res[2] = {nullptr, nullptr};      // RVQ workspace: residuals, per-chunk partial argmin
   float* rvq_best[2] = {nullptr, nullptr};
   int* rvq_idx[2] = {nullptr, nullptr};
   int rvq_cap = 0;
-  float* splitk_ws = nullptr; size_t splitk_bytes = 0;   // split-K partial sums of the deep / skinny layers
+  float* splitk_ws = nullptr;                            // split-K partial sums of the deep / skinny layers
   int* err = nullptr;                                     // device error flags (B200_FLAG_CODE_RANGE)
   // one-frame encode / decode as CUDA graphs over static buffers (frame in enc[0].ext -> enc_codes, dec_codes -> out_frame)
   cudaStream_t body = nullptr;                 // stream the kernels are being enqueued on (caller's, or gstream in capture)
@@ -217,6 +216,7 @@ void plan_seanet(b200_mimi* h) {
   h->down = DownLayer();
   h->down.key = "downsample.conv.conv.conv"; h->down.cin = c.dimension; h->down.cout = c.dimension;
   h->down.k = 2 * h->rs; h->down.stride = h->rs;
+  h->down.t_in = h->rs; h->down.t_out = 1; h->down.P = h->down.k - h->down.stride;   // the encoder transformer's rs tokens -> one frame
 }
 
 int get_f32(b200_mimi* h, const std::string& name, std::vector<int64_t> shape, const float** out) {
@@ -238,14 +238,11 @@ struct ScratchFree { void* p = nullptr; ~ScratchFree() { if (p) cudaFree(p); } }
 int pack_tc(b200_mimi* h, mtc::TcLayer& L, const float* w_ntc, int N, int Cin, int n_taps) {
   if (Cin % mtc::TC_KB || N % 16 || (N > mtc::TC_MAX_NT && N % mtc::TC_MAX_NT))
     B200_FAIL(B200_ERR_INVALID, "mimi: a %d x %d (x %d taps) contraction does not tile on the tensor-core kernel", N, Cin, n_taps);
-  L.Cin = Cin; L.N = N; L.n_taps = n_taps;
-  L.NT = N >= mtc::TC_MAX_NT ? mtc::TC_MAX_NT : N;
-  L.n_tiles_n = (N + L.NT - 1) / L.NT;
-  L.num_kb = n_taps * (Cin / mtc::TC_KB);
-  const size_t bytes = mtc::tc_packed_bytes(N, Cin, n_taps);
+  mtc::tc_set_shape(L, N, Cin, n_taps);
+  const size_t bytes = mtc::tc_packed_bytes(L);
   void* out = nullptr;
   B200_TRY(h->weights.alloc(&out, bytes, false));
-  B200_TRY(mtc::tc_pack_weights(w_ntc, out, N, Cin, n_taps, nullptr));
+  B200_TRY(mtc::tc_pack_weights(w_ntc, out, L, nullptr));
   L.wt = static_cast<uint8_t*>(out);
   h->weight_bytes += (int64_t)bytes;
   return B200_OK;
@@ -292,13 +289,13 @@ int pack_sea(b200_mimi* h, SeaLayer& l) {
   return check_launch("pack_sea");
 }
 
-// the down-sampling conv keeps the first-generation kernel and weight layout ([Cout][K*Cin])
+// the down-sampling conv's weights for conv_splitk_kernel: [Cout][K * Cin]
 int pack_down(b200_mimi* h, DownLayer& l) {
   const float* w = nullptr;
   B200_TRY(get_f32(h, l.key + ".weight", {l.cout, l.cin, l.k}, &w));
   const long long n = (long long)l.cout * l.cin * l.k;
   B200_TRY(h->weights.alloc_t(&l.w, n, false));
-  B200_LAUNCH(pack_conv_w_kernel, (unsigned)ceil_div64(n, 256), 256, 0, 0, w, l.w, l.cout, l.cin, l.k);
+  B200_LAUNCH(tm_weight_conv_kernel, (unsigned)ceil_div64(n, 256), 256, 0, 0, w, l.w, l.cout, l.cin, l.k);
   h->weight_bytes += n * 4;
   B200_CUDA(cudaDeviceSynchronize());
   h->store.release(l.key + ".weight");
@@ -449,15 +446,24 @@ int run_seanet(b200_mimi* h, std::vector<SeaLayer>& layers) {
   return check_launch("mimi seanet");
 }
 
+// the down-sampling conv reads tok_enc token-major and writes latent [B][C] (replicate padding on a session's first frame)
+ConvSplitK down_conv(b200_mimi* h) {
+  const DownLayer& l = h->down;
+  const int d = h->cfg.dimension;
+  ConvSplitK p;
+  p.x = h->tok_enc; p.xb = (long long)l.t_in * d; p.xc = 1; p.xt = d; p.Tin = l.t_in;
+  p.st = l.state; p.P = l.P; p.first = l.first;
+  p.w = l.w; p.bias = nullptr;
+  p.y = h->latent; p.yb = d; p.yc = 1; p.yt = 1;
+  p.Cin = l.cin; p.stride = l.stride; p.dil = 1; p.Tout = l.t_out; p.elu_in = 0;
+  p.M = l.cout; p.N = h->batch * l.t_out; p.Kd = l.cin * l.k;
+  return p;
+}
+
 int commit_states(b200_mimi* h, bool encoder) {
   const int B = h->batch;
   if (encoder) {
-    if (h->n_enc_commits) {      // the down-sampling conv (first-generation state layout + replicate flags)
-      dim3 grid(ceil_div(h->max_enc_rows, 128), h->n_enc_commits);
-      B200_LAUNCH(conv_commit_kernel, grid, 128, 0, h->body, h->enc_commits, h->n_enc_commits, h->exec_mask, B);
-      B200_LAUNCH(conv_clear_first_kernel, ceil_div(h->n_enc_commits * B, 128), 128, 0, h->body, h->enc_commits,
-                  h->n_enc_commits, h->exec_mask, B);
-    }
+    B200_LAUNCH(conv_commit_kernel, B, 128, 0, h->body, down_conv(h), h->exec_mask);   // the down-sampling conv
     if (h->n_enc_tm) {
       dim3 grid((unsigned)ceil_div64(h->max_enc_tm, 128), h->n_enc_tm);
       B200_LAUNCH(tm_commit_kernel, grid, 128, 0, h->body, h->enc_tm, h->exec_mask, B);
@@ -467,39 +473,25 @@ int commit_states(b200_mimi* h, bool encoder) {
       dim3 grid((unsigned)ceil_div64(h->max_dec_tm, 128), h->n_dec_tm);
       B200_LAUNCH(tm_commit_kernel, grid, 128, 0, h->body, h->dec_tm, h->exec_mask, B);
     }
-    dim3 g2((unsigned)ceil_div64(h->max_tr_rows, 256), h->n_dec_tr_commits);      // the depth-wise up-sampling's overlap-add carry
-    B200_LAUNCH(convtr_commit_kernel, g2, 256, 0, h->body, h->dec_tr_commits, h->exec_mask, B);
+    const int per_row = h->cfg.dimension * h->rs;                                 // the depth-wise up-sampling's overlap-add carry
+    B200_LAUNCH(convtr_commit_kernel, (unsigned)ceil_div64((long long)B * per_row, 256), 256, 0, h->body, h->up_partial, h->up_scratch,
+                per_row, h->exec_mask, B);
   }
   return check_launch("commit_states");
 }
 
 // frame in enc[0].ext -> latent [B][C]   (static buffers only: this is what gets captured into a graph)
 int encode_body(b200_mimi* h) {
-  const int d = h->cfg.dimension;
   const int T = h->frame_size / h->hop;   // encoder tokens per frame (2)
   B200_TRY(run_seanet(h, h->enc));        // the last conv's raw output is tok_in_enc, token-major [B][T][C]
   B200_TRY(run_transformer(h, h->enc_tr, h->tok_in_enc, h->tok_enc, T));
-  {                                       // learnt down-sampling conv reads token-major, writes latent [B][C][1]
-    const DownLayer& l = h->down;
-    ConvP p;
-    p.x = h->tok_enc; p.xb = (long long)T * d; p.xc = 1; p.xt = d; p.Tin = l.t_in;
-    p.st = l.state; p.P = l.P; p.first = l.first;
-    p.w = l.w; p.bias = nullptr;
-    p.y = h->latent; p.yb = d; p.yc = 1; p.yt = 1;
-    p.res = nullptr; p.rb = p.rc = p.rt = 0;
-    p.B = h->batch; p.Cin = l.cin; p.Cout = l.cout; p.K = l.k; p.stride = l.stride; p.dil = 1; p.Tout = l.t_out;
-    p.elu_in = 0;
-    p.M = l.cout; p.N = h->batch * l.t_out; p.Kd = l.cin * l.k; p.cin_aligned = (l.cin % BK) == 0;
+  {
+    // deep and skinny (2048 reduction steps, N = sessions): the reduction cut over KS CTAs per 64 outputs, slices added in order
+    const ConvSplitK p = down_conv(h);
     const int KS = ceil_div(p.Kd, DS_KP);
-    if ((size_t)KS * p.N * p.M * 4 <= h->splitk_bytes) {
-      // deep and skinny (2048 reduction steps, N = sessions): the reduction cut over KS CTAs per 64 outputs, slices added in order
-      dim3 g1(ceil_div(p.M, DS_CO), KS);
-      B200_LAUNCH(conv_splitk_kernel, g1, 256, 0, h->body, p, h->splitk_ws, KS);
-      B200_LAUNCH(conv_splitk_reduce_kernel, (unsigned)ceil_div64((long long)p.N * p.M, 256), 256, 0, h->body, p, h->splitk_ws, KS);
-    } else {
-      dim3 grid(ceil_div(p.N, BN), ceil_div(p.M, BM));
-      B200_LAUNCH((igemm_f32_kernel<ConvP, false>), grid, 256, 0, h->body, p);
-    }
+    dim3 g1(ceil_div(p.M, DS_CO), KS);
+    B200_LAUNCH(conv_splitk_kernel, g1, 256, 0, h->body, p, h->splitk_ws, KS);
+    B200_LAUNCH(conv_splitk_reduce_kernel, (unsigned)ceil_div64((long long)p.N * p.M, 256), 256, 0, h->body, p, h->splitk_ws, KS);
   }
   B200_TRY(commit_states(h, true));
   return B200_OK;
@@ -650,27 +642,17 @@ int ensure_streaming(b200_mimi* h, const char* what) {
 
 void register_tap(b200_mimi* h, const std::string& name, const float* p, int C, int T, bool transpose) { h->taps[name] = Tap{p, C, T, transpose}; }
 
-// Tile shape of a layer whose sessions produce T GEMM rows per frame: the largest power of two that divides T (<= 128) steps
-// of bb = 128 / tt sessions; strided convolutions also keep the TMA box (tt * stride rows) within 256.
-int tile_shape(int T, int stride, int* tt, int* bb) {
-  int t = 128;
-  while (t > 1 && (T % t || t * stride > 256)) t >>= 1;
-  if (T % t) return B200_ERR_SHAPE;
-  *tt = t; *bb = 128 / t;
-  return B200_OK;
-}
-
 // Plans one tensor-core layer for B sessions of T GEMM rows: A maps over `in_hi / in_lo` ([B][rows][Cin]), epilogue pointers set
 // by the caller in L.p beforehand (y / res / act); this fills geometry, schedule and tensor maps.
 int plan_layer(b200_mimi* h, mtc::TcLayer& L, const float* in_hi, const float* in_lo, int rows_per_session, int row0, int T) {
   const int B = h->batch;
   int tt = 0, bb = 0;
-  if (tile_shape(T, L.stride, &tt, &bb) != B200_OK) B200_FAIL(B200_ERR_INVALID, "mimi: %d steps per frame do not tile", T);
+  if (mtc::tc_tile_shape(T, L.stride, &tt, &bb) != B200_OK) B200_FAIL(B200_ERR_INVALID, "mimi: %d steps per frame do not tile", T);
   L.p.tt = tt; L.p.bb = bb; L.p.row0 = row0;
   L.p.ws = h->splitk_ws;
   B200_TRY(mtc::tc_make_map(&L.map_hi, in_hi, L.Cin, rows_per_session, (long long)rows_per_session * L.Cin, B, tt, bb, L.stride));
   B200_TRY(mtc::tc_make_map(&L.map_lo, in_lo, L.Cin, rows_per_session, (long long)rows_per_session * L.Cin, B, tt, bb, L.stride));
-  return mtc::tc_plan(L, B, T, h->sms, h->splitk_bytes);
+  return mtc::tc_plan(L, B, T, h->sms, kTcSplitBytes);
 }
 
 }  // namespace
@@ -783,13 +765,12 @@ int b200_mimi_streaming_begin(b200_mimi* h, int batch, void* stream) {
   B200_TRY(A.alloc_t(&h->exec_mask, B, false));
   B200_CUDA(cudaMemset(h->exec_mask, 1, B));
   B200_TRY(A.alloc_t(&h->err, 1));
-  h->splitk_bytes = (size_t)64 << 20;
-  B200_TRY(A.alloc(reinterpret_cast<void**>(&h->splitk_ws), h->splitk_bytes, false));
-
-  // flags for replicate-padded convs (only the down-sampling conv in Mimi)
-  h->n_first = 1;
-  B200_TRY(A.alloc_t(&h->first_flags, (size_t)h->n_first * B, false));
-  B200_CUDA(cudaMemset(h->first_flags, 1, (size_t)h->n_first * B));
+  {
+    // the tensor-core layers plan their splits within kTcSplitBytes; the down-sampling conv's partials outgrow it above 1024 sessions
+    const DownLayer& l = h->down;
+    const size_t down_bytes = (size_t)ceil_div(l.cin * l.k, DS_KP) * B * l.t_out * l.cout * 4;
+    B200_TRY(A.alloc(reinterpret_cast<void**>(&h->splitk_ws), down_bytes > kTcSplitBytes ? down_bytes : kTcSplitBytes, false));
+  }
 
   const int T = h->rs;   // transformer tokens per frame on both sides
   B200_TRY(A.alloc_t(&h->tok_in_enc, (size_t)B * T * d));   // written by the last encoder conv
@@ -876,39 +857,17 @@ int b200_mimi_streaming_begin(b200_mimi* h, int batch, void* stream) {
   register_tap(h, "dec.up", h->tok_in_dec, d, T, false);
   register_tap(h, "dec.tr", h->tok_dec, d, T, false);
 
-  // down-sampling conv (replicate pad): reads tok_enc token-major
-  std::vector<ConvCommit> enc_c;
-  {
-    DownLayer& l = h->down;
-    l.t_in = T; l.t_out = T / l.stride; l.P = l.k - l.stride;
-    B200_TRY(A.alloc_t(&l.state, (size_t)B * l.cin * l.P));
-    l.first = h->first_flags;
-    ConvCommit cc;
-    cc.x = h->tok_enc; cc.xb = (long long)T * d; cc.xc = 1; cc.xt = d; cc.Tin = T; cc.st = l.state; cc.P = l.P;
-    cc.Cin = l.cin; cc.elu_in = 0; cc.first = l.first;
-    enc_c.push_back(cc);
-    h->max_enc_rows = B * l.cin;
-  }
+  // down-sampling conv (replicate pad): carried input and first-frame flags
+  B200_TRY(A.alloc_t(&h->down.state, (size_t)B * h->down.cin * h->down.P));
+  B200_TRY(A.alloc_t(&h->down.first, B, false));
+  B200_CUDA(cudaMemset(h->down.first, 1, B));
   // up-sampling depth-wise convtr
-  std::vector<ConvTrCommit> dec_t;
   B200_TRY(A.alloc_t(&h->up_partial, (size_t)B * d * h->rs));
   B200_TRY(A.alloc_t(&h->up_scratch, (size_t)B * d * h->rs));
-  {
-    ConvTrCommit tc;
-    tc.partial = h->up_partial; tc.scratch = h->up_scratch; tc.per_row = d * h->rs;
-    dec_t.push_back(tc);
-    h->max_tr_rows = (long long)B * tc.per_row;
-  }
-  h->n_enc_commits = (int)enc_c.size();
-  h->n_dec_tr_commits = (int)dec_t.size();
   h->n_enc_tm = (int)enc_tm.size();
   h->n_dec_tm = (int)dec_tm.size();
-  B200_TRY(A.alloc_t(&h->enc_commits, enc_c.size(), false));
-  B200_TRY(A.alloc_t(&h->dec_tr_commits, dec_t.size(), false));
   B200_TRY(A.alloc_t(&h->enc_tm, enc_tm.size() ? enc_tm.size() : 1, false));
   B200_TRY(A.alloc_t(&h->dec_tm, dec_tm.size() ? dec_tm.size() : 1, false));
-  B200_CUDA(cudaMemcpy(h->enc_commits, enc_c.data(), enc_c.size() * sizeof(ConvCommit), cudaMemcpyHostToDevice));
-  B200_CUDA(cudaMemcpy(h->dec_tr_commits, dec_t.data(), dec_t.size() * sizeof(ConvTrCommit), cudaMemcpyHostToDevice));
   if (!enc_tm.empty()) B200_CUDA(cudaMemcpy(h->enc_tm, enc_tm.data(), enc_tm.size() * sizeof(TmCommit), cudaMemcpyHostToDevice));
   if (!dec_tm.empty()) B200_CUDA(cudaMemcpy(h->dec_tm, dec_tm.data(), dec_tm.size() * sizeof(TmCommit), cudaMemcpyHostToDevice));
 
@@ -932,28 +891,26 @@ int b200_mimi_streaming_begin(b200_mimi* h, int batch, void* stream) {
       B200_TRY(A.alloc_t(&L.kc, (size_t)B * H * c.tr_context * D));
       B200_TRY(A.alloc_t(&L.vc, (size_t)B * H * c.tr_context * D));
       const float* cur = li == 0 ? x_in : x;
-      auto lin = [&](mtc::TcLayer& G, const float* in_hi, const float* in_lo, int K, float* y, int N) -> int {
+      auto lin = [&](mtc::TcLayer& G, float* y, int N) {
         memset(&G.p, 0, sizeof(G.p));
         G.p.epi = mtc::TC_EPI_CONV;
         G.p.y = y; G.p.y_sb = (long long)T * N; G.p.y_row = N;
-        (void)K;
-        return B200_OK;
       };
       // in_proj: qkv = W_in xn
-      B200_TRY(lin(L.in_proj, h->tr_xn_hi, h->tr_xn_lo, d, h->tr_qkv, 3 * d));
+      lin(L.in_proj, h->tr_qkv, 3 * d);
       B200_TRY(plan_layer(h, L.in_proj, h->tr_xn_hi, h->tr_xn_lo, T, 0, T));
       // out_proj: x = cur + layer_scale_1 * (W_out ao)   (transformer.py:769)
-      B200_TRY(lin(L.out_proj, h->tr_ao_hi, h->tr_ao_lo, d, x, d));
+      lin(L.out_proj, x, d);
       L.out_proj.p.epi = mtc::TC_EPI_RES_SCALE; L.out_proj.p.res = cur; L.out_proj.p.r_sb = (long long)T * d; L.out_proj.p.r_row = d;
       L.out_proj.p.scale = L.ls1;
       B200_TRY(plan_layer(h, L.out_proj, h->tr_ao_hi, h->tr_ao_lo, T, 0, T));
       // linear1 + GELU -> h as a hi / lo pair (never stored raw)
-      B200_TRY(lin(L.l1, h->tr_xn_hi, h->tr_xn_lo, d, nullptr, ff));
+      lin(L.l1, nullptr, ff);
       L.l1.p.epi = mtc::TC_EPI_GELU; L.l1.p.act_mode = mtc::TC_ACT_SPLIT; L.l1.p.act_elu = 0;
       L.l1.p.a_hi = h->tr_h_hi; L.l1.p.a_lo = h->tr_h_lo; L.l1.p.a_sb = (long long)T * ff; L.l1.p.a_row = ff;
       B200_TRY(plan_layer(h, L.l1, h->tr_xn_hi, h->tr_xn_lo, T, 0, T));
       // linear2: x = x + layer_scale_2 * (W_2 h)   (transformer.py:777); the decoder's last layer also feeds dec[0]
-      B200_TRY(lin(L.l2, h->tr_h_hi, h->tr_h_lo, ff, x, d));
+      lin(L.l2, x, d);
       L.l2.p.epi = mtc::TC_EPI_RES_SCALE; L.l2.p.res = x; L.l2.p.r_sb = (long long)T * d; L.l2.p.r_row = d; L.l2.p.scale = L.ls2;
       if (which == 1 && li + 1 == tr->layers.size()) {
         const SeaLayer& nx = h->dec[0];
@@ -974,7 +931,7 @@ int b200_mimi_streaming_begin(b200_mimi* h, int batch, void* stream) {
   // what a streaming-state snapshot holds (streaming.py:158-181): masks, carried conv rows (the transposed convs' carry is
   // their previous input step), both transformers' KV rings and offsets
   A.mark_state(h->exec_mask, B, "exec_mask", B200_U8, {B});
-  A.mark_state(h->first_flags, (size_t)h->n_first * B, "downsample.first", B200_U8, {B});
+  A.mark_state(h->down.first, B, "downsample.first", B200_U8, {B});
   for (int which = 0; which < 2; ++which)
     for (auto& l : which == 0 ? h->enc : h->dec) {
       const std::string nm = (which == 0 ? "encoder." : "decoder.") + l.key.substr(l.key.find("model."));
@@ -1038,8 +995,8 @@ int b200_mimi_reset(b200_mimi* h, const uint8_t* reset_mask_dev) {
                     l.cin, (long long)(l.P + l.t_in) * l.cin, reset_mask_dev, B);
   zero(h->down.state, (long long)h->down.cin * h->down.P);
   zero(h->up_partial, (long long)h->cfg.dimension * h->rs);
-  B200_LAUNCH(reset_flags_kernel, ceil_div(B, 128), 128, 0, h->stream, h->first_flags, h->n_first, h->enc_tr.offset,
-              h->dec_tr.offset, h->exec_mask, reset_mask_dev, B);
+  B200_LAUNCH(reset_flags_kernel, ceil_div(B, 128), 128, 0, h->stream, h->down.first, h->enc_tr.offset, h->dec_tr.offset,
+              h->exec_mask, reset_mask_dev, B);
   return check_launch("mimi_reset");
 }
 

@@ -1,15 +1,10 @@
-// fp32 kernels of the Mimi codec path.  Everything on the encode side stays in exact fp32 FMA
-// arithmetic (no TF32 / bf16) because the RVQ indices downstream must match the reference's.
+// SIMT fp32 kernels of the Mimi codec: the learnt down-sampling conv, the depth-wise up-sampling, state commits and resets,
+// the residual VQ and load-time re-layouts.  Every other contraction of the codec is on the tensor cores (mimi_tc.cuh).
+// The down-sampling conv and the RVQ run in plain fp32 FMA arithmetic (no TF32 / bf16) because the RVQ indices must match
+// the reference's.
 //
-// Layout conventions
-//   * activations are addressed through explicit (batch, channel, time) strides, so a layer can
-//     read / write either the reference's [B, C, T] layout or the token-major [B, T, C] layout the
-//     transformer kernels use — no transposition kernels (ProjectedTransformer.conv_layout,
-//     transformer.py:972-981, is folded into the neighbouring conv's addressing).
-//   * conv weights are repacked once at load: Conv1d  [Cout][Cin][K] -> [Cout][K*Cin] (tap-major,
-//     channel fastest) so a K-chunk of the implicit GEMM shares one tap.
-// Since round 2 only the learnt down-sampling conv (replicate padding) still runs on igemm_f32_kernel; every other
-// contraction of the codec is on the tensor cores (mimi_tc.cuh).
+// Activations are addressed through explicit (batch, channel, time) strides, so a kernel can read / write either the
+// reference's [B, C, T] layout or the token-major [B, T, C] layout of the transformer kernels without a transposition.
 #pragma once
 
 #include "common.cuh"
@@ -18,26 +13,18 @@ namespace b200 {
 namespace mimi {
 
 // ---------------------------------------------------------------------------------------------
-// Tiled fp32 implicit GEMM:  C[m][n] = sum_k A[m][k] * B[k][n]   (64x64 tile, 256 threads, 4x4/thread)
-// A = packed weights (row-major [M][Kd]); B is gathered by the policy; the policy owns the epilogue.
+// StreamingConv1d (conv.py:245-274) as a split-K fp32 GEMM over packed weights [M = Cout][Kd = K * Cin] (tap-major, channel
+// fastest) and N = sessions x Tout output columns.
 // ---------------------------------------------------------------------------------------------
-constexpr int BM = 64, BN = 64, BK = 16;
-
-struct ConvP {
-  const float* x; long long xb, xc, xt; int Tin;
-  const float* st; int P;            // carried left context [B][Cin][P]
-  const uint8_t* first;              // replicate-pad flags or nullptr
-  const float* w; const float* bias;
+struct ConvSplitK {
+  const float* x; long long xb, xc, xt; int Tin;   // input x[b][ci][t] through strides, Tin steps
+  float* st; int P;                  // carried left context [B][Cin][P]
+  uint8_t* first;                    // replicate-pad flags [B] or nullptr
+  const float* w; const float* bias; // [M][Kd]; [M] or nullptr
   float* y; long long yb, yc, yt;
-  const float* res; long long rb, rc, rt;
-  float* a = nullptr; long long ab = 0, ac = 0, at = 0; int a_elu = 0;   // activated copy for a following layer (unused by the down-sampling conv)
-  int B, Cin, Cout, K, stride, dil, Tout, elu_in;
-  int M, N, Kd, cin_aligned;
+  int Cin, stride, dil, Tout, elu_in;
+  int M, N, Kd;
 
-  struct Ctx { int valid, b, t; };
-  __device__ __forceinline__ Ctx prepare(int n) const {
-    Ctx c; c.valid = n < N; c.b = c.valid ? n / Tout : 0; c.t = n - c.b * Tout; return c;
-  }
   __device__ __forceinline__ float ext(int b, int ci, int j) const {
     // sample j of cat(previous, x) for row b, channel ci   (conv.py:261)
     if (j < P) {
@@ -50,22 +37,6 @@ struct ConvP {
     float v = x[b * xb + ci * xc + (long long)(j - P) * xt];
     return elu_in ? elu1(v) : v;
   }
-  __device__ __forceinline__ float loadB(const Ctx& c, int kk, int kw_hint) const {
-    if (!c.valid || kk >= Kd) return 0.f;
-    int kw = cin_aligned ? kw_hint : kk / Cin;
-    int ci = kk - kw * Cin;
-    return ext(c.b, ci, c.t * stride + kw * dil);
-  }
-  __device__ __forceinline__ int chunk_hint(int k0) const { return cin_aligned ? k0 / Cin : 0; }
-  __device__ __forceinline__ float loadBk(int, int) const { return 0.f; }
-  __device__ __forceinline__ void store(int m, int n, float acc) const {
-    if (m >= M || n >= N) return;
-    int b = n / Tout, t = n - b * Tout;
-    float v = acc + (bias ? bias[m] : 0.f);
-    if (res) v = res[b * rb + m * rc + t * rt] + v;   // SEANetResnetBlock: u + v (seanet.py:90-93)
-    y[b * yb + m * yc + t * yt] = v;
-    if (a) a[b * ab + m * ac + t * at] = a_elu ? elu1(v) : v;
-  }
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -73,10 +44,10 @@ struct ConvP {
 // per frame): N = sessions x T_out columns against K * Cin = 2048 reduction steps and 4 MB of weights.  As a plain tile
 // GEMM that is 16 CTAs walking 2048 k each (249 us at 104 sessions, 209 us at one); here the reduction is cut into KS
 // slices so that (Cout / 64) x KS CTAs stream the weights once, and a second pass adds the slices in slice order
-// (deterministic).  Same ext() semantics as ConvP (carried left context, replicate padding on a session's first frame).
+// (deterministic).  The partials take KS * N * M floats.
 // ---------------------------------------------------------------------------------------------
 constexpr int DS_CO = 64, DS_KP = 64, DS_NC = 32;
-static __global__ void __launch_bounds__(256) conv_splitk_kernel(const ConvP p, float* __restrict__ part, int KS) {
+static __global__ void __launch_bounds__(256) conv_splitk_kernel(const ConvSplitK p, float* __restrict__ part, int KS) {
   __shared__ float ws[DS_KP][DS_CO + 1];
   __shared__ float xs[DS_KP][DS_NC + 1];
   const int tid = threadIdx.x;
@@ -118,7 +89,7 @@ static __global__ void __launch_bounds__(256) conv_splitk_kernel(const ConvP p, 
   }
   (void)KS;
 }
-static __global__ void __launch_bounds__(256) conv_splitk_reduce_kernel(const ConvP p, const float* __restrict__ part, int KS) {
+static __global__ void __launch_bounds__(256) conv_splitk_reduce_kernel(const ConvSplitK p, const float* __restrict__ part, int KS) {
   const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
   if (i >= (long long)p.N * p.M) return;
   const int n = (int)(i / p.M), m = (int)(i - (long long)n * p.M);
@@ -130,136 +101,31 @@ static __global__ void __launch_bounds__(256) conv_splitk_reduce_kernel(const Co
 #pragma unroll
     for (int j = 0; j < 8; ++j) a += v[j];
   }
-  p.store(m, n, a);
-}
-
-template <class P, bool B_K_FAST>
-static __global__ void __launch_bounds__(256) igemm_f32_kernel(const P p) {
-  __shared__ float As[2][BK][BM + 4];
-  __shared__ float Bs[2][BK][BN + 4];
-  const int tid = threadIdx.x;
-  const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
-  const int tx = tid & 15, ty = tid >> 4;
-
-  // A loader: 16 consecutive k per row -> coalesced 64 B segments
-  const int a_k = tid & 15, a_m = tid >> 4;               // rows a_m + 16*i
-  // B loader, n-fast (gathers): one column per thread, rows b_k + 4*i
-  const int bn_n = tid & 63, bn_k = tid >> 6;
-  // B loader, k-fast (row-major activations): 16 consecutive k per token
-  const int bk_k = tid & 15, bk_n = tid >> 4;             // cols bk_n + 16*i
-
-  const typename P::Ctx ctx = p.prepare(n0 + bn_n);
-
-  float acc[4][4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-
-  float ra[4], rb[4];
-  auto fetch = [&](int k0) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      int m = m0 + a_m + 16 * i, kk = k0 + a_k;
-      ra[i] = (m < p.M && kk < p.Kd) ? p.w[(long long)m * p.Kd + kk] : 0.f;
-    }
-    if constexpr (B_K_FAST) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) rb[i] = p.loadBk(k0 + bk_k, n0 + bk_n + 16 * i);
-    } else {
-      int hint = p.chunk_hint(k0);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) rb[i] = p.loadB(ctx, k0 + bn_k + 4 * i, hint);
-    }
-  };
-  auto stash = [&](int buf) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) As[buf][a_k][a_m + 16 * i] = ra[i];
-    if constexpr (B_K_FAST) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) Bs[buf][bk_k][bk_n + 16 * i] = rb[i];
-    } else {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) Bs[buf][bn_k + 4 * i][bn_n] = rb[i];
-    }
-  };
-
-  const int nk = (p.Kd + BK - 1) / BK;
-  fetch(0);
-  stash(0);
-  __syncthreads();
-  for (int it = 0; it < nk; ++it) {
-    const int cur = it & 1;
-    if (it + 1 < nk) fetch((it + 1) * BK);
-#pragma unroll
-    for (int kk = 0; kk < BK; ++kk) {
-      float a[4], b[4];
-      const float4 av = *reinterpret_cast<const float4*>(&As[cur][kk][ty * 4]);
-      a[0] = av.x; a[1] = av.y; a[2] = av.z; a[3] = av.w;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) b[j] = Bs[cur][kk][tx + 16 * j];
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
-    }
-    if (it + 1 < nk) stash(cur ^ 1);
-    __syncthreads();
-  }
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) p.store(m0 + ty * 4 + i, n0 + tx + 16 * j, acc[i][j]);
+  const int b = n / p.Tout, t = n - b * p.Tout;
+  p.y[b * p.yb + m * p.yc + t * p.yt] = a + (p.bias ? p.bias[m] : 0.f);
 }
 
 // ---------------------------------------------------------------------------------------------
 // state commits (run after the layer kernels of a step; only rows with exec_mask change)
 // ---------------------------------------------------------------------------------------------
-struct ConvCommit {   // previous <- last P samples of cat(previous, act(x))   (conv.py:263-267)
-  const float* x; long long xb, xc, xt; int Tin;
-  float* st; int P, Cin, elu_in;
-  uint8_t* first;     // replicate flags (cleared where exec_mask) or nullptr
-};
-struct ConvTrCommit { // partial <- scratch   (conv.py:357-360)
-  float* partial; const float* scratch; int per_row;   // Cout * S
-};
-
-static __global__ void conv_commit_kernel(const ConvCommit* descs, int n_desc, const uint8_t* exec_mask, int B) {
-  const ConvCommit d = descs[blockIdx.y];
-  const int row = blockIdx.x * blockDim.x + threadIdx.x;   // (b, ci)
-  if (row >= B * d.Cin) return;
-  const int b = row / d.Cin, ci = row - b * d.Cin;
+// previous <- last P samples of cat(previous, act(x)) (conv.py:263-267), then the session's replicate flag is cleared.
+// One CTA per session; the flag is cleared after every thread of the CTA has read it.
+static __global__ void conv_commit_kernel(const ConvSplitK p, const uint8_t* exec_mask) {
+  const int b = blockIdx.x;
   if (!exec_mask[b]) return;
-  const bool rep = d.first != nullptr && d.first[b];
-  float* s = d.st + (long long)row * d.P;
-  for (int j = 0; j < d.P; ++j) {
-    const int e = d.Tin + j;          // index into cat(previous, x); reads run ahead of writes
-    float v;
-    if (e < d.P) {
-      if (rep) { v = d.x[b * d.xb + ci * d.xc]; v = d.elu_in ? elu1(v) : v; }
-      else v = s[e];
-    } else {
-      v = d.x[b * d.xb + ci * d.xc + (long long)(e - d.P) * d.xt];
-      v = d.elu_in ? elu1(v) : v;
-    }
-    s[j] = v;
+  for (int ci = threadIdx.x; ci < p.Cin; ci += blockDim.x) {
+    float* s = p.st + ((long long)b * p.Cin + ci) * p.P;
+    for (int j = 0; j < p.P; ++j) s[j] = p.ext(b, ci, p.Tin + j);   // reads run ahead of writes
   }
+  __syncthreads();
+  if (threadIdx.x == 0 && p.first != nullptr) p.first[b] = 0;
 }
 
-// `first` flags are cleared in a second tiny pass so that every (b, ci) thread above saw the old value.
-static __global__ void conv_clear_first_kernel(const ConvCommit* descs, int n_desc, const uint8_t* exec_mask, int B) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n_desc * B) return;
-  const ConvCommit d = descs[i / B];
-  const int b = i % B;
-  if (d.first != nullptr && exec_mask[b]) d.first[b] = 0;
-}
-
-static __global__ void convtr_commit_kernel(const ConvTrCommit* descs, const uint8_t* exec_mask, int B) {
-  const ConvTrCommit d = descs[blockIdx.y];
+// partial <- scratch (conv.py:357-360), per_row = Cout * S
+static __global__ void convtr_commit_kernel(float* partial, const float* scratch, int per_row, const uint8_t* exec_mask, int B) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (long long)B * d.per_row) return;
-  if (exec_mask[i / d.per_row]) d.partial[i] = d.scratch[i];
+  if (i >= (long long)B * per_row) return;
+  if (exec_mask[i / per_row]) partial[i] = scratch[i];
 }
 
 // reset: zero the state of the rows in reset_mask (conv.py:166-169, 281-286)
@@ -268,13 +134,13 @@ static __global__ void zero_rows_kernel(float* buf, long long per_row, const uin
   if (i >= (long long)B * per_row) return;
   if (mask == nullptr || mask[i / per_row]) buf[i] = 0.f;
 }
-static __global__ void reset_flags_kernel(uint8_t* first /*[n_first][B]*/, int n_first, long long* off_a, long long* off_b,
-                                   uint8_t* exec_mask, const uint8_t* mask, int B) {
+static __global__ void reset_flags_kernel(uint8_t* first, long long* off_a, long long* off_b, uint8_t* exec_mask,
+                                          const uint8_t* mask, int B) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
   if (mask != nullptr && !mask[b]) return;
   exec_mask[b] = 1;                                       // State.reset (streaming.py:41-42)
-  for (int i = 0; i < n_first; ++i) first[(long long)i * B + b] = 1;
+  first[b] = 1;
   if (off_a) off_a[b] = 0;                                // _MHAState.reset / RingKVCache.reset
   if (off_b) off_b[b] = 0;
 }
@@ -525,13 +391,6 @@ static __global__ void __launch_bounds__(256) rvq_decode_kernel(const RvqDecArgs
 // ---------------------------------------------------------------------------------------------
 // load-time repacking
 // ---------------------------------------------------------------------------------------------
-static __global__ void pack_conv_w_kernel(const float* w /*[Cout][Cin][K]*/, float* out /*[Cout][K*Cin]*/, int Cout, int Cin, int K) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (long long)Cout * Cin * K) return;
-  const int kw = i % K; long long r = i / K;
-  const int ci = r % Cin; const int co = r / Cin;
-  out[((long long)co * K + kw) * Cin + ci] = w[i];
-}
 static __global__ void transpose_kernel(const float* in /*[R][C]*/, float* out /*[C][R]*/, int R, int C) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long long)R * C) return;

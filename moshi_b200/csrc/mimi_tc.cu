@@ -282,19 +282,29 @@ int tc_init() {
   return B200_OK;
 }
 
-static int pick_nt(int N) { return N >= TC_MAX_NT ? TC_MAX_NT : N; }
-
-size_t tc_packed_bytes(int N, int Cin, int n_taps) {
-  const int NT = pick_nt(N), n_tiles = (N + NT - 1) / NT, num_kb = n_taps * (Cin / TC_KB);
-  return (size_t)n_tiles * num_kb * 2 * NT * 128;
+void tc_set_shape(TcLayer& L, int N, int Cin, int n_taps) {
+  L.Cin = Cin; L.N = N; L.n_taps = n_taps;
+  L.NT = N >= TC_MAX_NT ? TC_MAX_NT : N;
+  L.n_tiles_n = (N + L.NT - 1) / L.NT;
+  L.num_kb = n_taps * (Cin / TC_KB);
 }
 
-int tc_pack_weights(const float* w_dev, void* out_dev, int N, int Cin, int n_taps, cudaStream_t st) {
-  if (Cin % TC_KB || N % 16 || (N > TC_MAX_NT && N % TC_MAX_NT))
-    B200_FAIL(B200_ERR_SHAPE, "tc_pack_weights: Cin %d must be a multiple of 32, N %d a multiple of 16 (of 128 above 128)", Cin, N);
-  const int NT = pick_nt(N), n_tiles = (N + NT - 1) / NT, num_kb = n_taps * (Cin / TC_KB);
-  const long long total = (long long)n_tiles * num_kb * NT * 8;
-  tc_pack_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(w_dev, static_cast<float4*>(out_dev), N, n_taps * Cin, NT, n_tiles, num_kb);
+int tc_tile_shape(int T, int stride, int* tt, int* bb) {
+  int t = TC_ROWS;
+  while (t > 1 && (T % t || t * stride > 256)) t >>= 1;
+  if (T % t) return B200_ERR_SHAPE;
+  *tt = t; *bb = TC_ROWS / t;
+  return B200_OK;
+}
+
+size_t tc_packed_bytes(const TcLayer& L) { return (size_t)L.n_tiles_n * L.num_kb * 2 * L.NT * 128; }
+
+int tc_pack_weights(const float* w_dev, void* out_dev, const TcLayer& L, cudaStream_t st) {
+  if (L.Cin % TC_KB || L.N % 16 || (L.N > TC_MAX_NT && L.N % TC_MAX_NT))
+    B200_FAIL(B200_ERR_SHAPE, "tc_pack_weights: Cin %d must be a multiple of 32, N %d a multiple of 16 (of 128 above 128)", L.Cin, L.N);
+  const long long total = (long long)L.n_tiles_n * L.num_kb * L.NT * 8;
+  tc_pack_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(w_dev, static_cast<float4*>(out_dev), L.N, L.n_taps * L.Cin, L.NT,
+                                                                 L.n_tiles_n, L.num_kb);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   return check_launch("tc_pack");
 }

@@ -90,9 +90,14 @@ struct TcLayer {
   int grid = 0; size_t smem = 0;
 };
 
-size_t tc_packed_bytes(int N, int Cin, int n_taps);
-// w: fp32 [N][n_taps * Cin] (k = tap * Cin + ci) -> tiles
-int tc_pack_weights(const float* w_dev, void* out_dev, int N, int Cin, int n_taps, cudaStream_t st);
+// static shape of a layer of N output features over n_taps * Cin inputs: Cin, N, n_taps and the weight tiling NT / n_tiles_n / num_kb
+void tc_set_shape(TcLayer& L, int N, int Cin, int n_taps);
+// Tile shape of a layer whose sessions produce T GEMM rows: the largest power of two that divides T (<= 128) steps of
+// bb = 128 / tt sessions; strided convolutions also keep the TMA box (tt * stride rows) within 256.
+int tc_tile_shape(int T, int stride, int* tt, int* bb);
+size_t tc_packed_bytes(const TcLayer& L);
+// w: fp32 [N][n_taps * Cin] (k = tap * Cin + ci) -> tiles, for a layer whose shape tc_set_shape filled
+int tc_pack_weights(const float* w_dev, void* out_dev, const TcLayer& L, cudaStream_t st);
 int tc_init();
 // 3-D tensor map over a token-major activation buffer base[b][row][Cin] (session stride sb elements, row stride = Cin)
 int tc_make_map(CUtensorMap* m, const float* base, int Cin, long long rows_per_session, long long sb_elems, int n_sessions, int tt,

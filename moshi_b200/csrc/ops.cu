@@ -3,6 +3,7 @@
 #include "lm_kernels.cuh"
 #include "mimi_kernels.cuh"
 #include "mimi_tc.cuh"
+#include "mimi_tm_kernels.cuh"
 
 using namespace b200;
 
@@ -19,6 +20,27 @@ static int sk_scratch(float** ws, int** counters, int which = 0) {
     B200_CUDA(cudaMemset(g_counters[which], 0, tc::SK_MAX_TILES * sizeof(int)));
   }
   *ws = g_ws[which]; *counters = g_counters[which];
+  return B200_OK;
+}
+
+// split-KV partials + merge counters of the attention entry points, grown on demand; separate sets for the bf16 and the 8-bit rings
+static int attn_scratch(int B, int H, int nsplit, float** part, int** counters, int which) {
+  static float* g_part[2] = {nullptr, nullptr};
+  static int* g_counters[2] = {nullptr, nullptr};
+  static size_t part_n[2] = {0, 0}, cnt_n[2] = {0, 0};
+  const size_t need = (size_t)B * H * nsplit * (lm::ATT_D + 2);
+  if (need > part_n[which]) {
+    if (g_part[which]) cudaFree(g_part[which]);
+    B200_CUDA(cudaMalloc(&g_part[which], need * sizeof(float)));
+    part_n[which] = need;
+  }
+  if ((size_t)B * H > cnt_n[which]) {
+    if (g_counters[which]) cudaFree(g_counters[which]);
+    B200_CUDA(cudaMalloc(&g_counters[which], (size_t)B * H * sizeof(int)));
+    B200_CUDA(cudaMemset(g_counters[which], 0, (size_t)B * H * sizeof(int)));
+    cnt_n[which] = (size_t)B * H;
+  }
+  *part = g_part[which]; *counters = g_counters[which];
   return B200_OK;
 }
 
@@ -114,64 +136,15 @@ int b200_op_linear_i8(const void* xq_dev, const float* sa_dev, const void* w_til
                        static_cast<cudaStream_t>(stream));
 }
 
-int b200_op_conv1d(const float* x_dev, const float* w_dev, const float* bias_dev, float* prev_dev,
-                   const uint8_t* exec_mask_dev, float* y_dev, int B, int Cin, int Cout, int T, int K, int stride,
-                   int dilation, int elu_in, void* stream) {
-  using namespace b200::mimi;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int keff = (K - 1) * dilation + 1, P = keff - stride;
-  if (T % stride || P < 0) B200_FAIL(B200_ERR_SHAPE, "op_conv1d: T %% stride != 0");
-  float* wp = nullptr;
-  ConvCommit* desc = nullptr;
-  B200_CUDA(cudaMalloc(&wp, (size_t)Cout * Cin * K * 4));
-  const long long n = (long long)Cout * Cin * K;
-  B200_LAUNCH(pack_conv_w_kernel, (unsigned)ceil_div64(n, 256), 256, 0, st, w_dev, wp, Cout, Cin, K);
-  ConvP p;
-  p.x = x_dev; p.xb = (long long)Cin * T; p.xc = T; p.xt = 1; p.Tin = T;
-  p.st = prev_dev; p.P = P; p.first = nullptr; p.w = wp; p.bias = bias_dev;
-  p.y = y_dev; p.yb = (long long)Cout * (T / stride); p.yc = T / stride; p.yt = 1;
-  p.res = nullptr; p.rb = p.rc = p.rt = 0;
-  p.B = B; p.Cin = Cin; p.Cout = Cout; p.K = K; p.stride = stride; p.dil = dilation; p.Tout = T / stride; p.elu_in = elu_in;
-  p.M = Cout; p.N = B * (T / stride); p.Kd = Cin * K; p.cin_aligned = (Cin % BK) == 0;
-  auto kern = igemm_f32_kernel<ConvP, false>;
-  dim3 grid(ceil_div(p.N, BN), ceil_div(p.M, BM));
-  B200_LAUNCH(kern, grid, 256, 0, st, p);
-  if (P > 0) {
-    ConvCommit cc;
-    cc.x = x_dev; cc.xb = p.xb; cc.xc = p.xc; cc.xt = 1; cc.Tin = T; cc.st = prev_dev; cc.P = P; cc.Cin = Cin;
-    cc.elu_in = elu_in; cc.first = nullptr;
-    B200_CUDA(cudaMalloc(&desc, sizeof(ConvCommit)));
-    B200_CUDA(cudaMemcpyAsync(desc, &cc, sizeof(cc), cudaMemcpyHostToDevice, st));
-    dim3 g2(ceil_div(B * Cin, 128), 1);
-    B200_LAUNCH(conv_commit_kernel, g2, 128, 0, st, desc, 1, exec_mask_dev, B);
-  }
-  B200_CUDA(cudaStreamSynchronize(st));
-  cudaFree(wp);
-  if (desc) cudaFree(desc);
-  return check_launch("op_conv1d");
-}
-
 int b200_op_attn_step(const void* qkv_dev, void* k_dev, void* v_dev, void* out_dev, const int64_t* pos_dev,
                       const uint8_t* exec_mask_dev, int B, int H, int cap, int nsplit, float max_period, void* stream) {
   using namespace b200::lm;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (B < 1 || H < 1 || cap < 1) B200_FAIL(B200_ERR_SHAPE, "op_attn_step: bad shape");
   if (nsplit <= 0) nsplit = attn_pick_splits(B, H, cap);
-  static float* part = nullptr;
-  static int* counters = nullptr;
-  static size_t part_n = 0, cnt_n = 0;
-  const size_t need = (size_t)B * H * nsplit * (ATT_D + 2);
-  if (need > part_n) {
-    if (part) cudaFree(part);
-    B200_CUDA(cudaMalloc(&part, need * sizeof(float)));
-    part_n = need;
-  }
-  if ((size_t)B * H > cnt_n) {
-    if (counters) cudaFree(counters);
-    B200_CUDA(cudaMalloc(&counters, (size_t)B * H * sizeof(int)));
-    B200_CUDA(cudaMemset(counters, 0, (size_t)B * H * sizeof(int)));
-    cnt_n = (size_t)B * H;
-  }
+  float* part = nullptr;
+  int* counters = nullptr;
+  B200_TRY(attn_scratch(B, H, nsplit, &part, &counters, 0));
   AttnStep a;
   a.qkv = static_cast<const bf16*>(qkv_dev); a.kc = static_cast<bf16*>(k_dev); a.vc = static_cast<bf16*>(v_dev);
   a.out = static_cast<bf16*>(out_dev); a.part = part; a.counters = counters;
@@ -191,21 +164,9 @@ int b200_op_attn_step_q8(const void* qkv_dev, void* k8_dev, void* v8_dev, float*
   if (B < 1 || H < 1 || cap < 1) B200_FAIL(B200_ERR_SHAPE, "op_attn_step_q8: bad shape");
   if (kv_dtype != B200_KV_FP8_E4M3 && kv_dtype != B200_KV_INT8) B200_FAIL(B200_ERR_INVALID, "op_attn_step_q8: kv_dtype %d", kv_dtype);
   if (nsplit <= 0) nsplit = attn_pick_splits(B, H, cap);
-  static float* part = nullptr;
-  static int* counters = nullptr;
-  static size_t part_n = 0, cnt_n = 0;
-  const size_t need = (size_t)B * H * nsplit * (ATT_D + 2);
-  if (need > part_n) {
-    if (part) cudaFree(part);
-    B200_CUDA(cudaMalloc(&part, need * sizeof(float)));
-    part_n = need;
-  }
-  if ((size_t)B * H > cnt_n) {
-    if (counters) cudaFree(counters);
-    B200_CUDA(cudaMalloc(&counters, (size_t)B * H * sizeof(int)));
-    B200_CUDA(cudaMemset(counters, 0, (size_t)B * H * sizeof(int)));
-    cnt_n = (size_t)B * H;
-  }
+  float* part = nullptr;
+  int* counters = nullptr;
+  B200_TRY(attn_scratch(B, H, nsplit, &part, &counters, 1));
   AttnStepQ8 a;
   a.qkv = static_cast<const bf16*>(qkv_dev); a.kc = static_cast<uint8_t*>(k8_dev); a.vc = static_cast<uint8_t*>(v8_dev);
   a.ks = ks_dev; a.vs = vs_dev; a.out = static_cast<bf16*>(out_dev); a.part = part; a.counters = counters;
@@ -219,7 +180,7 @@ int b200_op_attn_step_q8(const void* qkv_dev, void* k8_dev, void* v8_dev, float*
 
 }  // extern "C"
 
-// ---- mimi_tc_kernel on the reference's [B, C, T] layout (test scaffolding: the handle keeps everything token-major) --------
+// ---- Mimi's conv kernels on the reference's [B, C, T] layout (test scaffolding: the handle keeps everything token-major) ----
 namespace {
 
 // ext[b][j][ci] (hi / lo) = cat(previous, act(x))[b][ci][j]  for j < P + T
@@ -238,18 +199,9 @@ __global__ void tm_pack_in_kernel(const float* __restrict__ x, const float* __re
   b200::mtc::split_tf32(v, h, l);
   hi[i] = h; lo[i] = l;
 }
-// y[b][c][t] = ytm[b][t][c]
-__global__ void tm_unpack_out_kernel(const float* __restrict__ ytm, float* __restrict__ y, int B, int C, int T) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (long long)B * C * T) return;
-  const int t = (int)(i % T);
-  const long long r = i / T;
-  const int c = (int)(r % C), b = (int)(r / C);
-  y[i] = ytm[((long long)b * T + t) * C + c];
-}
 // previous[b][ci][j] <- (hi + lo)[b][T + j][ci] for rows with exec_mask (conv.py:263-267)
-__global__ void tm_commit_kernel(const float* __restrict__ hi, const float* __restrict__ lo, float* __restrict__ prev,
-                                 const uint8_t* __restrict__ exec_mask, int B, int Cin, int T, int P) {
+__global__ void tm_commit_bct_kernel(const float* __restrict__ hi, const float* __restrict__ lo, float* __restrict__ prev,
+                                     const uint8_t* __restrict__ exec_mask, int B, int Cin, int T, int P) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long long)B * Cin * P) return;
   const int j = (int)(i % P);
@@ -259,26 +211,6 @@ __global__ void tm_commit_kernel(const float* __restrict__ hi, const float* __re
   const long long o = ((long long)b * (P + T) + T + j) * Cin + ci;
   prev[i] = hi[o] + lo[o];
 }
-// conv [Cout][Cin][K] -> [Cout][K][Cin];  convtr [Cin][Cout][2S] -> [(r, co)][tap'][ci] with tap' = 0: x[t-1] (kernel taps S + r), 1: x[t]
-__global__ void tm_weight_conv_kernel(const float* __restrict__ w, float* __restrict__ out, int Cout, int Cin, int K) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (long long)Cout * Cin * K) return;
-  const int kw = (int)(i % K);
-  const long long r = i / K;
-  const int ci = (int)(r % Cin), co = (int)(r / Cin);
-  out[((long long)co * K + kw) * Cin + ci] = w[i];
-}
-__global__ void tm_weight_convtr_kernel(const float* __restrict__ w, float* __restrict__ out, int Cin, int Cout, int S) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (long long)Cin * Cout * 2 * S) return;
-  const int k = (int)(i % (2 * S));
-  const long long r = i / (2 * S);
-  const int co = (int)(r % Cout), ci = (int)(r / Cout);
-  const int tap = k / S, ph = k - tap * S;            // tap 0 multiplies x[t], tap 1 multiplies x[t-1]
-  const int n = ph * Cout + co, slot = 1 - tap;       // rows of the A operand: slot 0 = x[t-1], slot 1 = x[t]
-  out[((long long)n * 2 + slot) * Cin + ci] = w[i];
-}
-
 struct DevBufs {
   std::vector<void*> p;
   ~DevBufs() { for (void* q : p) cudaFree(q); }
@@ -291,35 +223,59 @@ struct DevBufs {
   }
 };
 
-int tc_tile_shape(int T, int* tt, int* bb) {
-  for (int c = 128; c >= 1; c >>= 1)
-    if (T % c == 0) { *tt = c; *bb = 128 / c; return B200_OK; }
-  return B200_ERR_SHAPE;
-}
-
 }  // namespace
 
 extern "C" {
+
+// StreamingConv1d on the down-sampling conv's kernels: weight re-layout, split-K GEMM + in-order reduction, state commit
+int b200_op_conv1d(const float* x_dev, const float* w_dev, const float* bias_dev, float* prev_dev,
+                   const uint8_t* exec_mask_dev, float* y_dev, int B, int Cin, int Cout, int T, int K, int stride,
+                   int dilation, int elu_in, void* stream) {
+  using namespace b200::mimi;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int keff = (K - 1) * dilation + 1, P = keff - stride;
+  if (T % stride || P < 0) B200_FAIL(B200_ERR_SHAPE, "op_conv1d: T %% stride != 0");
+  ConvSplitK p;
+  p.x = x_dev; p.xb = (long long)Cin * T; p.xc = T; p.xt = 1; p.Tin = T;
+  p.st = prev_dev; p.P = P; p.first = nullptr; p.bias = bias_dev;
+  p.y = y_dev; p.yb = (long long)Cout * (T / stride); p.yc = T / stride; p.yt = 1;
+  p.Cin = Cin; p.stride = stride; p.dil = dilation; p.Tout = T / stride; p.elu_in = elu_in;
+  p.M = Cout; p.N = B * (T / stride); p.Kd = Cin * K;
+  const int KS = ceil_div(p.Kd, DS_KP);
+  DevBufs d;
+  float *wp, *part;
+  B200_TRY(d.get(&wp, (size_t)Cout * Cin * K * 4));
+  B200_TRY(d.get(&part, (size_t)KS * p.N * p.M * 4));
+  p.w = wp;
+  const long long n = (long long)Cout * Cin * K;
+  B200_LAUNCH(tm_weight_conv_kernel, (unsigned)ceil_div64(n, 256), 256, 0, st, w_dev, wp, Cout, Cin, K);
+  B200_LAUNCH(conv_splitk_kernel, dim3(ceil_div(p.M, DS_CO), KS), 256, 0, st, p, part, KS);
+  B200_LAUNCH(conv_splitk_reduce_kernel, (unsigned)ceil_div64((long long)p.N * p.M, 256), 256, 0, st, p, part, KS);
+  if (P > 0) B200_LAUNCH(conv_commit_kernel, B, 128, 0, st, p, exec_mask_dev);
+  B200_CUDA(cudaStreamSynchronize(st));
+  return check_launch("op_conv1d");
+}
 
 int b200_op_tc_linear_f32(const float* x_dev, const float* w_dev, float* y_dev, int M, int N, int K, void* stream) {
   using namespace b200::mtc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (!x_dev || !w_dev || !y_dev || M < 1 || K % 32 || N % 16) B200_FAIL(B200_ERR_SHAPE, "op_tc_linear_f32: bad shape");
   B200_TRY(tc_init());
+  TcLayer L;
+  tc_set_shape(L, N, K, 1);
+  L.kind = 2;
   DevBufs d;
   float *hi, *lo, *ws; uint8_t* wt;
   B200_TRY(d.get(&hi, (size_t)M * K * 4));
   B200_TRY(d.get(&lo, (size_t)M * K * 4));
-  B200_TRY(d.get(&wt, tc_packed_bytes(N, K, 1)));
+  B200_TRY(d.get(&wt, tc_packed_bytes(L)));
   const size_t ws_bytes = (size_t)64 << 20;
   B200_TRY(d.get(&ws, ws_bytes));
   const long long n = (long long)M * K;
   // x is already [M][K] token-major: a flat hi/lo split is tm_pack_in with B = M "sessions" of Cin = K, T = 1, P = 0
   B200_LAUNCH(tm_pack_in_kernel, (unsigned)ceil_div64(n, 256), 256, 0, st, x_dev, (const float*)nullptr, hi, lo, M, K, 1, 0, 0);
-  B200_TRY(tc_pack_weights(w_dev, wt, N, K, 1, st));
-  TcLayer L;
-  L.kind = 2; L.Cin = K; L.N = N; L.n_taps = 1; L.wt = wt;
-  L.NT = N >= TC_MAX_NT ? TC_MAX_NT : N; L.n_tiles_n = (N + L.NT - 1) / L.NT; L.num_kb = K / TC_KB;
+  B200_TRY(tc_pack_weights(w_dev, wt, L, st));
+  L.wt = wt;
   memset(&L.p, 0, sizeof(L.p));
   L.p.tt = 128; L.p.bb = 1; L.p.row0 = 0;
   L.p.epi = TC_EPI_CONV; L.p.y = y_dev; L.p.y_sb = 0; L.p.y_row = N; L.p.ws = ws;
@@ -346,28 +302,28 @@ int b200_op_tc_conv1d(const float* x_dev, const float* w_dev, const float* bias_
   const int N = transposed ? S * Cout : Cout;
   if (Cin % 32 || N % 16 || (N > 128 && N % 128) || P < 0 || (!transposed && T % stride) || (transposed && K != 2 * S))
     B200_FAIL(B200_ERR_SHAPE, "op_tc_conv1d: unsupported shape");
+  TcLayer L;
+  tc_set_shape(L, N, Cin, n_taps);
+  L.kind = transposed ? 1 : 0; L.dil = transposed ? 1 : dilation; L.stride = transposed ? 1 : stride;
+  L.bias = bias_dev; L.bias_mod = Cout;
   DevBufs d;
   float *hi, *lo, *ws, *wk, *ytm; uint8_t* wt;
   const size_t E = (size_t)P + T;
   B200_TRY(d.get(&hi, (size_t)B * E * Cin * 4));
   B200_TRY(d.get(&lo, (size_t)B * E * Cin * 4));
   B200_TRY(d.get(&wk, (size_t)N * n_taps * Cin * 4));
-  B200_TRY(d.get(&wt, tc_packed_bytes(N, Cin, n_taps)));
+  B200_TRY(d.get(&wt, tc_packed_bytes(L)));
   B200_TRY(d.get(&ytm, (size_t)B * Tout * N * 4));
   const size_t ws_bytes = (size_t)64 << 20;
   B200_TRY(d.get(&ws, ws_bytes));
   const long long n_in = (long long)B * E * Cin, n_w = (long long)N * n_taps * Cin;
   B200_LAUNCH(tm_pack_in_kernel, (unsigned)ceil_div64(n_in, 256), 256, 0, st, x_dev, (const float*)prev_dev, hi, lo, B, Cin, T, P, elu_in);
-  if (transposed) B200_LAUNCH(tm_weight_convtr_kernel, (unsigned)ceil_div64(n_w, 256), 256, 0, st, w_dev, wk, Cin, Cout, S);
-  else B200_LAUNCH(tm_weight_conv_kernel, (unsigned)ceil_div64(n_w, 256), 256, 0, st, w_dev, wk, Cout, Cin, K);
-  B200_TRY(tc_pack_weights(wk, wt, N, Cin, n_taps, st));
-  TcLayer L;
-  L.kind = transposed ? 1 : 0; L.Cin = Cin; L.N = N; L.n_taps = n_taps; L.dil = transposed ? 1 : dilation; L.stride = transposed ? 1 : stride;
-  L.wt = wt; L.bias = bias_dev; L.bias_mod = Cout;
-  L.NT = N >= TC_MAX_NT ? TC_MAX_NT : N; L.n_tiles_n = (N + L.NT - 1) / L.NT; L.num_kb = n_taps * (Cin / TC_KB);
+  if (transposed) B200_LAUNCH(mimi::tm_weight_convtr_kernel, (unsigned)ceil_div64(n_w, 256), 256, 0, st, w_dev, wk, Cin, Cout, S);
+  else B200_LAUNCH(mimi::tm_weight_conv_kernel, (unsigned)ceil_div64(n_w, 256), 256, 0, st, w_dev, wk, Cout, Cin, K);
+  B200_TRY(tc_pack_weights(wk, wt, L, st));
+  L.wt = wt;
   memset(&L.p, 0, sizeof(L.p));
-  if (tc_tile_shape(Tout, &L.p.tt, &L.p.bb) != B200_OK) B200_FAIL(B200_ERR_SHAPE, "op_tc_conv1d: T");
-  while (L.p.tt * L.stride > 256) { L.p.tt /= 2; L.p.bb *= 2; }
+  if (tc_tile_shape(Tout, L.stride, &L.p.tt, &L.p.bb) != B200_OK) B200_FAIL(B200_ERR_SHAPE, "op_tc_conv1d: T");
   L.p.row0 = 0;
   L.p.epi = TC_EPI_CONV; L.p.y = ytm; L.p.y_sb = (long long)Tout * N; L.p.y_row = N; L.p.ws = ws;
   B200_TRY(tc_make_map(&L.map_hi, hi, Cin, (long long)E, (long long)E * Cin, B, L.p.tt, L.p.bb, L.stride));
@@ -378,9 +334,9 @@ int b200_op_tc_conv1d(const float* x_dev, const float* w_dev, const float* bias_
   B200_TRY(tc_launch(L, st));
   // token-major [B][Tout][N] -> the reference layout: conv [B][Cout][Tout]; convtr [B][Cout][Tout * S] (row t holds S steps of Cout)
   const int Tr = transposed ? Tout * S : Tout;
-  B200_LAUNCH(tm_unpack_out_kernel, (unsigned)ceil_div64((long long)B * Cout * Tr, 256), 256, 0, st, ytm, y_dev, B, Cout, Tr);
+  B200_LAUNCH(mimi::tm_to_bct_kernel, (unsigned)ceil_div64((long long)B * Cout * Tr, 256), 256, 0, st, ytm, y_dev, B, Cout, Tr);
   if (P > 0 && prev_dev)
-    B200_LAUNCH(tm_commit_kernel, (unsigned)ceil_div64((long long)B * Cin * P, 256), 256, 0, st, hi, lo, prev_dev, exec_mask_dev, B, Cin, T, P);
+    B200_LAUNCH(tm_commit_bct_kernel, (unsigned)ceil_div64((long long)B * Cin * P, 256), 256, 0, st, hi, lo, prev_dev, exec_mask_dev, B, Cin, T, P);
   B200_CUDA(cudaStreamSynchronize(st));
   return check_launch("op_tc_conv1d");
 }
