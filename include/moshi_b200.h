@@ -262,13 +262,17 @@ int b200_lm_set_offset_cpu(b200_lm* h, int64_t value);
 #define B200_FLAG_TOKEN_RANGE 1
 #define B200_FLAG_CODE_RANGE 2
 #define B200_FLAG_KV_CAPACITY 4
+/* A row of a paged handle (b200_lm_set_kv_pool) did not get a page because the pool was full: that row's output is garbage
+ * until it is reset; no other row is affected.  b200_lm_step_host and b200_frame_step return B200_ERR_STATE on it. */
+#define B200_FLAG_KV_POOL 8
 int b200_lm_error_flags(b200_lm* h, int* flags_out);
 /* Algorithmic HBM bytes of one step at the current batch and ring fill (DESIGN.md): weights once
  * + per-row KV read/append + embeddings + logits. */
 int64_t b200_lm_algorithmic_bytes(b200_lm* h, int kv_fill);
 /* Test/bench helper: declare that every row already holds `fill` steps of history (positions and
  * ring offsets are advanced; ring contents are whatever is in memory) so that the steady-state
- * full-ring step can be timed without running 3000 warm-up steps. */
+ * full-ring step can be timed without running 3000 warm-up steps.  On a paged handle (b200_lm_set_kv_pool) every row then
+ * holds the pages of that fill (B200_ERR_STATE, nothing changed, if they do not fit). */
 int b200_lm_assume_fill(b200_lm* h, int fill);
 /* 0 = one launch per kernel, 1 = replay the whole step as one CUDA graph (default 1): the reference graphs forward_text and
  * depformer_step separately (lm.py:628-634, utils/compile.py:190-280). */
@@ -287,6 +291,18 @@ int b200_lm_set_kv_dtype(b200_lm* h, int kv_dtype);
  * (SURVEY.md 8f item 3, "rings sized to live fill").  A row that steps past the capacity raises B200_FLAG_KV_CAPACITY; the
  * caller moves such a session to a full-size handle (get / set streaming state) before that. */
 int b200_lm_set_kv_capacity(b200_lm* h, int slots);
+/* Paged temporal KV rings, chosen before b200_lm_streaming_begin (frames = 0: off, the default).  The rings of all model
+ * rows share one pool of `frames` slots, rounded up to whole pages of `page_slots` slots (a power of two in [4, 256]) and
+ * capped at what every row's full ring needs.  A row takes pages as its fill grows (inside the step) and returns them on
+ * b200_lm_reset, so young and old sessions share one handle.  Keys are only stored elsewhere: the numerics are those of the
+ * contiguous ring, bit for bit.  The streaming state keeps the contiguous layout (entries layers.<i>.k / .v [MB,H,context,128];
+ * slots past a row's fill read as zeros), so snapshots move between paged and contiguous handles; writing model.offset (or a
+ * whole snapshot) maps exactly the pages of the new fill, and returns B200_ERR_STATE, changing nothing, if they do not fit.
+ * A row the step cannot serve raises B200_FLAG_KV_POOL.  Bf16 rings of the full context only: with b200_lm_set_kv_dtype
+ * other than B200_KV_BF16 or with b200_lm_set_kv_capacity it returns B200_ERR_INVALID (here or at streaming_begin). */
+int b200_lm_set_kv_pool(b200_lm* h, int64_t frames, int page_slots);
+/* Pages held by rows and pages in the pool (0 / 0 without a pool).  Synchronises the handle's stream. */
+int b200_lm_kv_pool_usage(b200_lm* h, int* pages_used, int* pages_total);
 
 /* ------------------------------------------------------------------------------------------ */
 /* One dialogue frame for every session slot: host PCM in, host PCM + tokens out, one host wait  */
@@ -381,6 +397,13 @@ int b200_op_tc_conv1d(const float* x_dev, const float* w_dev, const float* bias_
  * the min(pos + exec, cap) valid slots, out bf16 [B,H*128].  One kernel (rope + append + split-KV + merge). */
 int b200_op_attn_step(const void* qkv_dev, void* k_dev, void* v_dev, void* out_dev, const int64_t* pos_dev,
                       const uint8_t* exec_mask_dev, int B, int H, int cap, int nsplit, float max_period, void* stream);
+/* The same step over paged rings (b200_lm_set_kv_pool): k_pool / v_pool bf16 [n_pages,H,page_slots,128], page_table int32
+ * [B,ceil(cap / page_slots)]; slot s of row b is page page_table[b][s / page_slots], offset s % page_slots.  Every slot the
+ * step reads or writes (those below min(pos + exec, cap)) must be mapped.  Bit-identical to b200_op_attn_step on a ring
+ * holding the same keys, for the same nsplit (<= 0: the LM's choice for (B, H, cap)). */
+int b200_op_attn_step_paged(const void* qkv_dev, void* k_pool_dev, void* v_pool_dev, const int32_t* page_table_dev, void* out_dev,
+                            const int64_t* pos_dev, const uint8_t* exec_mask_dev, int B, int H, int cap, int page_slots, int nsplit,
+                            float max_period, void* stream);
 /* sample_token (sampling.py:86-106): logits bf16 [B,card], noise f32 [B,min(k,card)] -> i64 [B]. */
 /* The same step over an opt-in 8-bit ring (b200_lm_set_kv_dtype): k8 / v8 u8 [B,H,cap,128] (e4m3 bytes, or
  * round(x * 127 / absmax) + 128), ks / vs f32 [B,H,cap] = absmax / 448 (or / 127) of the row. */

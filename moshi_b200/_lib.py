@@ -98,6 +98,8 @@ _PROTOTYPES: dict[str, tuple[tp.Any, list]] = {
     "b200_lm_set_graph": (_I, [_P, _I]),
     "b200_lm_set_kv_dtype": (_I, [_P, _I]),
     "b200_lm_set_kv_capacity": (_I, [_P, _I]),
+    "b200_lm_set_kv_pool": (_I, [_P, C.c_int64, _I]),
+    "b200_lm_kv_pool_usage": (_I, [_P, C.POINTER(_I), C.POINTER(_I)]),
     "b200_lm_set_cfg": (_I, [_P, C.c_float, _I, _P, _I]),
     "b200_lm_set_condition_sum": (_I, [_P, _P, _I]),
     "b200_lm_seed_noise": (_I, [_P, C.c_uint64]),
@@ -129,6 +131,7 @@ _PROTOTYPES: dict[str, tuple[tp.Any, list]] = {
     "b200_op_tc_linear_f32": (_I, [_P, _P, _P, _I, _I, _I, _P]),
     "b200_op_tc_conv1d": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
     "b200_op_attn_step": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, C.c_float, _P]),
+    "b200_op_attn_step_paged": (_I, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, C.c_float, _P]),
     "b200_op_attn_step_q8": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, C.c_float, _I, _P]),
     "b200_op_sample": (_I, [_P, _P, _P, _I, _I, _I, C.c_float, _I, _P]),
 }

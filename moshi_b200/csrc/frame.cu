@@ -13,6 +13,7 @@
 #include "common.cuh"
 
 namespace b200 {
+int lm_check_kv_pool(b200_lm* h);      // lm.cu: B200_ERR_STATE (and clears the flag) if B200_FLAG_KV_POOL was raised; no-op without a pool
 namespace {
 
 // Slot updates -> reset / exec masks (batched_asr.py:146-177 builds them on the host and copies three tensors).
@@ -201,7 +202,7 @@ int b200_frame_step(b200_frame* f, const float* pcm_in_host, const int32_t* upda
   memcpy(tokens_out_host, f->h_tokens, B * (f->dep_q + 1) * 8);
   memcpy(pcm_out_host, f->h_pcm_out, B * f->frame * 4);
   if (ready_out_host) memcpy(ready_out_host, f->h_ready, B);
-  return B200_OK;
+  return lm_check_kv_pool(f->lm);
 }
 
 }  // extern "C"

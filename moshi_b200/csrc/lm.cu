@@ -85,6 +85,12 @@ struct b200_lm {
   int fuse_norm = 1;                           // B200_FUSE_NORM=0: keep rmsnorm_kernel in front of the GEMV path too (diagnostics)
   int kv_cap = 0;                              // b200_lm_set_kv_capacity: slots per ring (0 = cfg.context, the reference's ring)
   int kv_fp8 = 0;                              // b200_lm_set_kv_dtype / B200_KV_DTYPE: opt-in 8-bit KV ring (B200_KV_FP8_E4M3 or B200_KV_INT8; 0 = bf16)
+  // b200_lm_set_kv_pool: the temporal rings live in pages of page_slots slots (TLayer kc / vc are then the pools
+  // [n_pages + 1][H][page_slots][D], the last page a sink); n_pages = 0: contiguous rings
+  int64_t pool_frames = 0; int page_slots = 64;
+  int n_pages = 0, tab_ld = 0, page_shift = 0;
+  int *page_table = nullptr, *page_held = nullptr;     // [MB][tab_ld] (-1 = unmapped), [MB]
+  int *free_stack = nullptr, *free_top = nullptr;      // [n_pages], [1]
   float *dep_part0 = nullptr, *dep_part1 = nullptr;
   unsigned* dep_bar = nullptr;
   unsigned long long* dep_trace = nullptr;     // B200_DEP_TRACE=1: barrier timestamps of the fused depformer (diagnostics)
@@ -261,6 +267,9 @@ int step_body(b200_lm* h) {
   }
   if (ring_cap(h) < c.context)      // a shortened ring serves a session only until it is full: flag instead of silently forgetting
     B200_LAUNCH(kv_capacity_check_kernel, ceil_div(MB, 128), 128, 0, st, h->pos, h->exec_mask_m, MB, ring_cap(h), h->err);
+  if (h->n_pages)                   // map the page of this step's slot (all layers share the table)
+    B200_LAUNCH(kv_page_alloc_kernel, 1, KV_PAGE_THREADS, 0, st, h->page_table, h->page_held, h->free_stack, h->free_top, h->pos,
+                h->exec_mask_m, MB, h->tab_ld, h->page_shift, c.context, h->n_pages, h->err);
   for (auto& L : h->layers) {
     B200_TRY(norm_linear(h, h->x, L.n1, h->xn, L.in_w, h->qkv, 3 * d, MB, 3 * d, d, LIN_STORE, 0, L.in_s));
     if (h->kv_fp8) {
@@ -276,8 +285,10 @@ int step_body(b200_lm* h) {
       a.qkv = h->qkv; a.kc = L.kc; a.vc = L.vc; a.out = h->ao; a.part = h->attn_part; a.counters = h->attn_counters;
       a.pos = h->pos; a.exec_mask = h->exec_mask_m; a.H = H; a.cap = ring_cap(h); a.nsplit = h->nsplit;
       a.neg_log_period_2_over_d = nl;
+      a.table = h->page_table; a.tab_ld = h->tab_ld; a.page_shift = h->page_shift;
       dim3 grid(MB * H, h->nsplit);
-      if (attn_group_keys() == 2) B200_LAUNCH(attn_step_kernel<2>, grid, ATT_THREADS, 0, st, a);
+      if (h->n_pages) B200_LAUNCH(attn_step_paged_kernel, grid, ATT_THREADS, 0, st, a);
+      else if (attn_group_keys() == 2) B200_LAUNCH(attn_step_kernel<2>, grid, ATT_THREADS, 0, st, a);
       else B200_LAUNCH(attn_step_kernel<4>, grid, ATT_THREADS, 0, st, a);
     }
     B200_TRY(linear(h, h->ao, d, L.out_w, h->x, d, h->x, d, MB, d, d, LIN_RESADD, 0, L.out_s));
@@ -345,7 +356,100 @@ void drop_graph(b200_lm* h) {
   }
 }
 
+// pages a row holds at model position `pos`: those of slots [0, min(pos, context))
+int pages_for(const b200_lm* h, long long pos) {
+  const long long n = std::min(std::max(pos, 0LL), (long long)h->cfg.context);
+  return (int)((n + h->page_slots - 1) / h->page_slots);
+}
+
+// Paged handle, synchronous: every row holds exactly pages_for(pos[b]) pages.  Excess pages are pushed back first (row and table
+// order), then missing ones are popped (row order).  Fails with B200_ERR_STATE, changing nothing, when they do not all fit.
+int pool_map(b200_lm* h, const std::vector<long long>& pos, const char* what) {
+  const int MB = h->MB, T = h->tab_ld;
+  int64_t want_total = 0;
+  for (int b = 0; b < MB; ++b) want_total += pages_for(h, pos[b]);
+  if (want_total > h->n_pages)
+    B200_FAIL(B200_ERR_STATE, "%s: the rows' fill needs %lld KV pages, the pool has %d", what, (long long)want_total, h->n_pages);
+  std::vector<int> table((size_t)MB * T), held(MB), stack(h->n_pages);
+  int top = 0;
+  B200_CUDA(cudaStreamSynchronize(h->stream));
+  B200_CUDA(cudaMemcpy(table.data(), h->page_table, table.size() * 4, cudaMemcpyDeviceToHost));
+  B200_CUDA(cudaMemcpy(held.data(), h->page_held, held.size() * 4, cudaMemcpyDeviceToHost));
+  B200_CUDA(cudaMemcpy(stack.data(), h->free_stack, stack.size() * 4, cudaMemcpyDeviceToHost));
+  B200_CUDA(cudaMemcpy(&top, h->free_top, 4, cudaMemcpyDeviceToHost));
+  for (int b = 0; b < MB; ++b) {
+    const int want = pages_for(h, pos[b]);
+    int* row = table.data() + (size_t)b * T;
+    for (int i = want; i < T; ++i) {
+      if (i < held[b]) stack[top++] = row[i];
+      row[i] = -1;
+    }
+    held[b] = std::min(held[b], want);
+  }
+  for (int b = 0; b < MB; ++b) {
+    const int want = pages_for(h, pos[b]);
+    for (int i = held[b]; i < want; ++i) table[(size_t)b * T + i] = stack[--top];
+    held[b] = want;
+  }
+  B200_CUDA(cudaMemcpy(h->page_table, table.data(), table.size() * 4, cudaMemcpyHostToDevice));
+  B200_CUDA(cudaMemcpy(h->page_held, held.data(), held.size() * 4, cudaMemcpyHostToDevice));
+  B200_CUDA(cudaMemcpy(h->free_stack, stack.data(), stack.size() * 4, cudaMemcpyHostToDevice));
+  B200_CUDA(cudaMemcpy(h->free_top, &top, 4, cudaMemcpyHostToDevice));
+  return B200_OK;
+}
+
+// The K / V state entry of a paged layer: its ring view is gathered from / scattered into the pool.  Other entries: nullptr.
+bf16* paged_pool_of(const b200_lm* h, const StateEntry& e) {
+  if (!h->n_pages) return nullptr;
+  for (auto& L : h->layers)
+    if (e.ptr == L.kc || e.ptr == L.vc) return static_cast<bf16*>(e.ptr);
+  return nullptr;
+}
+
+// One state entry between the handle and a device buffer (exactly one of dst / src is non-null), on the handle's stream.
+int state_copy(b200_lm* h, const StateEntry& e, void* dst, const void* src) {
+  bf16* pool = paged_pool_of(h, e);
+  if (!pool) {
+    if (dst) B200_CUDA(cudaMemcpyAsync(dst, e.ptr, e.bytes, cudaMemcpyDeviceToDevice, h->stream));
+    else B200_CUDA(cudaMemcpyAsync(e.ptr, src, e.bytes, cudaMemcpyDeviceToDevice, h->stream));
+    return B200_OK;
+  }
+  const long long n_vec = (long long)(e.bytes / 16);
+  const unsigned grid = (unsigned)ceil_div64(n_vec, 256);
+  const int H = h->cfg.num_heads, cap = h->cfg.context;
+  if (dst) B200_LAUNCH(kv_page_copy_kernel<true>, grid, 256, 0, h->stream, pool, static_cast<bf16*>(dst), h->page_table, h->pos, H, cap,
+                       h->tab_ld, h->page_shift, h->n_pages, n_vec);
+  else B200_LAUNCH(kv_page_copy_kernel<false>, grid, 256, 0, h->stream, pool, const_cast<bf16*>(static_cast<const bf16*>(src)),
+                   h->page_table, h->pos, H, cap, h->tab_ld, h->page_shift, h->n_pages, n_vec);
+  return check_launch("kv_page_copy");
+}
+
+// the model positions a write of `model.offset` from `src_dev` would set, on the host
+int read_positions(b200_lm* h, const void* src_dev, std::vector<long long>* pos) {
+  pos->assign(h->MB, 0);
+  B200_CUDA(cudaStreamSynchronize(h->stream));
+  B200_CUDA(cudaMemcpy(pos->data(), src_dev, (size_t)h->MB * 8, cudaMemcpyDeviceToHost));
+  return B200_OK;
+}
+
 }  // namespace
+
+namespace b200 {
+// b200_frame_step: a row the KV pool could not serve fails the frame (B200_ERR_STATE), as b200_lm_step_host does.  Synchronises;
+// clears that flag only, the others stay for b200_lm_error_flags.
+int lm_check_kv_pool(b200_lm* h) {
+  if (!h || !h->n_pages || h->batch <= 0) return B200_OK;
+  DeviceGuard g(h->device);
+  int v = 0;
+  B200_CUDA(cudaMemcpyAsync(&v, h->err, 4, cudaMemcpyDeviceToHost, h->stream));
+  B200_CUDA(cudaStreamSynchronize(h->stream));
+  if (!(v & ERR_KV_POOL)) return B200_OK;
+  const int rest = v & ~ERR_KV_POOL;
+  B200_CUDA(cudaMemcpyAsync(h->err, &rest, 4, cudaMemcpyHostToDevice, h->stream));
+  B200_CUDA(cudaStreamSynchronize(h->stream));
+  B200_FAIL(B200_ERR_STATE, "frame_step: a session's KV ring did not get a page: the KV pool of %d pages is full (flags %d)", h->n_pages, v);
+}
+}  // namespace b200
 
 extern "C" {
 
@@ -576,11 +680,20 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
     B200_FAIL(B200_ERR_SHAPE, "lm_streaming_begin: cfg_is_masked_until has %zu entries for %d sessions", h->cfg_until_host.size(), B);
   h->stream = static_cast<cudaStream_t>(stream);
   Arena& A = h->state;
-  struct Cleanup { b200_lm* h; bool armed = true; ~Cleanup() { if (armed) { h->state.free_all(); h->cfg_until = nullptr; h->noise_ctr = nullptr; } } } cleanup{h};
+  struct Cleanup { b200_lm* h; bool armed = true; ~Cleanup() { if (armed) { h->state.free_all(); h->cfg_until = nullptr; h->noise_ctr = nullptr; h->n_pages = 0; } } } cleanup{h};
   size_t free_b = 0, total_b = 0;
   cudaMemGetInfo(&free_b, &total_b);
   const int cap = ring_cap(h);
-  const size_t kv_bytes = (size_t)c.num_layers * 2 * MB * H * cap * (h->kv_fp8 ? (size_t)D + 4 : (size_t)D * 2);
+  if (h->pool_frames > 0 && (h->kv_fp8 || cap < c.context))
+    B200_FAIL(B200_ERR_INVALID, "lm_streaming_begin: the KV pool holds bf16 rings of the model's context (no kv_dtype or kv_capacity)");
+  h->n_pages = 0;
+  if (h->pool_frames > 0) {
+    h->tab_ld = ceil_div(c.context, h->page_slots);
+    h->page_shift = __builtin_ctz(h->page_slots);
+    h->n_pages = (int)std::min(ceil_div64(h->pool_frames, h->page_slots), (int64_t)MB * h->tab_ld);
+  }
+  const size_t ring_slots = h->n_pages ? (size_t)(h->n_pages + 1) * h->page_slots : (size_t)MB * cap;   // per layer and head
+  const size_t kv_bytes = (size_t)c.num_layers * 2 * ring_slots * H * (h->kv_fp8 ? (size_t)D + 4 : (size_t)D * 2);
   if (kv_bytes + (1ull << 30) > free_b)
     B200_FAIL(B200_ERR_INVALID, "lm_streaming_begin: %d sessions need %.1f GB of KV ring, %.1f GB free", B, kv_bytes / 1e9,
               free_b / 1e9);
@@ -614,9 +727,20 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
       B200_TRY(A.alloc_t(&L.ks, (size_t)MB * H * cap));
       B200_TRY(A.alloc_t(&L.vs, (size_t)MB * H * cap));
     } else {
-      B200_TRY(A.alloc_t(&L.kc, (size_t)MB * H * cap * D));
-      B200_TRY(A.alloc_t(&L.vc, (size_t)MB * H * cap * D));
+      B200_TRY(A.alloc_t(&L.kc, ring_slots * H * D));
+      B200_TRY(A.alloc_t(&L.vc, ring_slots * H * D));
     }
+  }
+  if (h->n_pages) {
+    B200_TRY(A.alloc_t(&h->page_table, (size_t)MB * h->tab_ld, false));
+    B200_CUDA(cudaMemset(h->page_table, 0xFF, (size_t)MB * h->tab_ld * 4));      // -1: unmapped
+    B200_TRY(A.alloc_t(&h->page_held, MB));
+    B200_TRY(A.alloc_t(&h->free_stack, h->n_pages, false));
+    B200_TRY(A.alloc_t(&h->free_top, 1, false));
+    std::vector<int> stack(h->n_pages);
+    for (int i = 0; i < h->n_pages; ++i) stack[i] = h->n_pages - 1 - i;        // page 0 is popped first
+    B200_CUDA(cudaMemcpy(h->free_stack, stack.data(), stack.size() * 4, cudaMemcpyHostToDevice));
+    B200_CUDA(cudaMemcpy(h->free_top, &h->n_pages, 4, cudaMemcpyHostToDevice));
   }
   for (auto& L : h->dlayers) {
     B200_TRY(A.alloc_t(&L.kc, (size_t)MB * dd * c.dep_q));
@@ -746,7 +870,15 @@ int b200_lm_get_state(b200_lm* h, void* dst_dev, int64_t capacity) {
   DeviceGuard g(h->device);
   const size_t n = h->state.state_bytes();
   if (!dst_dev || capacity < (int64_t)n + 256) B200_FAIL(B200_ERR_SHAPE, "lm_get_state: destination too small");
-  B200_TRY(h->state.save(dst_dev, h->stream));
+  if (h->n_pages) {          // the same blob as a contiguous handle's: the K / V entries are gathered into ring layout
+    size_t off = 0;
+    for (auto& e : h->state.snap) {
+      B200_TRY(state_copy(h, e, static_cast<char*>(dst_dev) + off, nullptr));
+      off += (e.bytes + 255) / 256 * 256;
+    }
+  } else {
+    B200_TRY(h->state.save(dst_dev, h->stream));
+  }
   B200_CUDA(cudaMemcpyAsync(static_cast<char*>(dst_dev) + n, &h->offset_cpu, 8, cudaMemcpyHostToDevice, h->stream));
   B200_CUDA(cudaStreamSynchronize(h->stream));
   return B200_OK;
@@ -757,7 +889,23 @@ int b200_lm_set_state(b200_lm* h, const void* src_dev, int64_t nbytes) {
   DeviceGuard g(h->device);
   const size_t n = h->state.state_bytes();
   if (!src_dev || nbytes != (int64_t)n + 256) B200_FAIL(B200_ERR_SHAPE, "lm_set_state: snapshot does not fit this session layout");
-  B200_TRY(h->state.load(src_dev, h->stream));
+  if (h->n_pages) {          // map the snapshot's fill first (nothing changes if it does not fit), then scatter its K / V
+    size_t off = 0, off_pos = 0;
+    for (auto& e : h->state.snap) {
+      if (e.name == "model.offset") off_pos = off;
+      off += (e.bytes + 255) / 256 * 256;
+    }
+    std::vector<long long> pos;
+    B200_TRY(read_positions(h, static_cast<const char*>(src_dev) + off_pos, &pos));
+    B200_TRY(pool_map(h, pos, "lm_set_state"));
+    off = 0;
+    for (auto& e : h->state.snap) {
+      B200_TRY(state_copy(h, e, nullptr, static_cast<const char*>(src_dev) + off));
+      off += (e.bytes + 255) / 256 * 256;
+    }
+  } else {
+    B200_TRY(h->state.load(src_dev, h->stream));
+  }
   B200_CUDA(cudaMemcpyAsync(&h->offset_cpu, static_cast<const char*>(src_dev) + n, 8, cudaMemcpyDeviceToHost, h->stream));
   B200_CUDA(cudaStreamSynchronize(h->stream));
   return B200_OK;
@@ -773,13 +921,26 @@ int b200_lm_state_read(b200_lm* h, const char* name, void* dst_dev, int64_t nbyt
   B200_TRY(ensure_streaming(h, "lm_state_read"));
   DeviceGuard g(h->device);
   if (!dst_dev) B200_FAIL(B200_ERR_INVALID, "lm_state_read: null destination");
-  return state_entry_copy(h->state, name, dst_dev, nullptr, nbytes, h->stream);
+  if (!h->n_pages) return state_entry_copy(h->state, name, dst_dev, nullptr, nbytes, h->stream);
+  const StateEntry* e = h->state.find_state(name ? name : "");
+  if (!e) B200_FAIL(B200_ERR_INVALID, "state entry '%s' does not exist", name ? name : "(null)");
+  if (nbytes != (int64_t)e->bytes) B200_FAIL(B200_ERR_SHAPE, "state entry '%s' holds %zu bytes, caller passed %lld", name, e->bytes, (long long)nbytes);
+  return state_copy(h, *e, dst_dev, nullptr);
 }
 int b200_lm_state_write(b200_lm* h, const char* name, const void* src_dev, int64_t nbytes) {
   B200_TRY(ensure_streaming(h, "lm_state_write"));
   DeviceGuard g(h->device);
   if (!src_dev) B200_FAIL(B200_ERR_INVALID, "lm_state_write: null source");
-  return state_entry_copy(h->state, name, nullptr, src_dev, nbytes, h->stream);
+  if (!h->n_pages) return state_entry_copy(h->state, name, nullptr, src_dev, nbytes, h->stream);
+  const StateEntry* e = h->state.find_state(name ? name : "");
+  if (!e) B200_FAIL(B200_ERR_INVALID, "state entry '%s' does not exist", name ? name : "(null)");
+  if (nbytes != (int64_t)e->bytes) B200_FAIL(B200_ERR_SHAPE, "state entry '%s' holds %zu bytes, caller passed %lld", name, e->bytes, (long long)nbytes);
+  if (e->name == "model.offset") {     // each row then holds exactly the pages of its new fill
+    std::vector<long long> pos;
+    B200_TRY(read_positions(h, src_dev, &pos));
+    B200_TRY(pool_map(h, pos, "lm_state_write"));
+  }
+  return state_copy(h, *e, nullptr, src_dev);
 }
 int64_t b200_lm_get_offset_cpu(b200_lm* h) { return h ? h->offset_cpu : 0; }
 int b200_lm_set_offset_cpu(b200_lm* h, int64_t v) {
@@ -805,6 +966,8 @@ int b200_lm_streaming_end(b200_lm* h) {
   h->depf = nullptr;
   h->state.free_all();
   h->cfg_until = nullptr; h->noise_ctr = nullptr; h->err = nullptr; h->cond_sum = nullptr; h->cond_on = 0;
+  h->n_pages = 0;
+  h->page_table = h->page_held = h->free_stack = h->free_top = nullptr;
   if (h->pin_in) cudaFreeHost(h->pin_in);
   if (h->pin_out) cudaFreeHost(h->pin_out);
   if (h->pin_noise) cudaFreeHost(h->pin_noise);
@@ -819,6 +982,9 @@ int b200_lm_reset(b200_lm* h, const uint8_t* reset_mask_dev) {
   B200_TRY(ensure_streaming(h, "lm_reset"));
   DeviceGuard g(h->device);
   const int B = h->batch;
+  if (h->n_pages)         // a reset row's pages return to the pool
+    B200_LAUNCH(kv_page_free_kernel, 1, KV_PAGE_THREADS, 0, h->stream, h->page_table, h->page_held, h->free_stack, h->free_top,
+                reset_mask_dev, B, h->MB, h->tab_ld);
   // per-row device offsets (lm.py:539, transformer.py:229-234, 331-333) ...
   B200_LAUNCH(lm_reset_kernel, ceil_div(B, 128), 128, 0, h->stream, h->offsets, h->pos, h->exec_mask, h->exec_mask_m,
               reset_mask_dev, B, cfg_on(h) ? 1 : 0);
@@ -868,11 +1034,40 @@ int b200_lm_set_kv_capacity(b200_lm* h, int slots) {
   return B200_OK;
 }
 
+int b200_lm_set_kv_pool(b200_lm* h, int64_t frames, int page_slots) {
+  if (!h) B200_FAIL(B200_ERR_INVALID, "lm_set_kv_pool: null handle");
+  if (h->batch > 0) B200_FAIL(B200_ERR_STATE, "lm_set_kv_pool: the pool is allocated at streaming_begin; set it before it");
+  if (frames < 0) B200_FAIL(B200_ERR_INVALID, "lm_set_kv_pool: negative size");
+  if (frames > 0) {
+    if (page_slots < 4 || page_slots > 256 || (page_slots & (page_slots - 1)))
+      B200_FAIL(B200_ERR_INVALID, "lm_set_kv_pool: page_slots %d (a power of two in [4, 256])", page_slots);
+    if (h->kv_fp8 || h->kv_cap > 0)
+      B200_FAIL(B200_ERR_INVALID, "lm_set_kv_pool: the pool holds bf16 rings of the model's context (no kv_dtype or kv_capacity)");
+    h->page_slots = page_slots;
+  }
+  h->pool_frames = frames;
+  return B200_OK;
+}
+
+int b200_lm_kv_pool_usage(b200_lm* h, int* pages_used, int* pages_total) {
+  B200_TRY(ensure_streaming(h, "lm_kv_pool_usage"));
+  DeviceGuard g(h->device);
+  int top = 0;
+  if (h->n_pages) {
+    B200_CUDA(cudaMemcpyAsync(&top, h->free_top, 4, cudaMemcpyDeviceToHost, h->stream));
+    B200_CUDA(cudaStreamSynchronize(h->stream));
+  }
+  if (pages_used) *pages_used = h->n_pages - top;
+  if (pages_total) *pages_total = h->n_pages;
+  return B200_OK;
+}
+
 int b200_lm_assume_fill(b200_lm* h, int fill) {
   B200_TRY(ensure_streaming(h, "lm_assume_fill"));
   DeviceGuard g(h->device);
   if (fill < 0) B200_FAIL(B200_ERR_INVALID, "lm_assume_fill: negative fill");
   std::vector<long long> v(h->MB, fill);
+  if (h->n_pages) B200_TRY(pool_map(h, v, "lm_assume_fill"));
   B200_CUDA(cudaMemcpyAsync(h->offsets, v.data(), (size_t)h->batch * 8, cudaMemcpyHostToDevice, h->stream));
   B200_CUDA(cudaMemcpyAsync(h->pos, v.data(), v.size() * 8, cudaMemcpyHostToDevice, h->stream));
   B200_CUDA(cudaStreamSynchronize(h->stream));
@@ -989,6 +1184,8 @@ int b200_lm_step_host(b200_lm* h, const int64_t* in_codes_host, int n_in, const 
     cudaMemsetAsync(h->err, 0, 4, h->stream);
     if (flags & lm::ERR_KV_CAPACITY)
       B200_FAIL(B200_ERR_STATE, "lm_step_host: a session stepped past its %d-slot KV ring (b200_lm_set_kv_capacity; flags %d)", ring_cap(h), flags);
+    if (flags & lm::ERR_KV_POOL)
+      B200_FAIL(B200_ERR_STATE, "lm_step_host: a session's KV ring did not get a page: the KV pool of %d pages is full (flags %d)", h->n_pages, flags);
     B200_FAIL(B200_ERR_INVALID, "lm_step_host: a token id outside its embedding table reached the model (flags %d)", flags);
   }
   return B200_OK;

@@ -48,7 +48,7 @@ struct TokenRing {
 
 // device error flags: raised instead of reading out of bounds; surfaced by b200_lm_error_flags / b200_mimi_error_flags and by
 // the host-synchronising entry points
-enum { ERR_TOKEN_RANGE = 1, ERR_CODE_RANGE = 2, ERR_KV_CAPACITY = 4 };
+enum { ERR_TOKEN_RANGE = 1, ERR_CODE_RANGE = 2, ERR_KV_CAPACITY = 4, ERR_KV_POOL = 8 };
 
 // One thread per (b, k): write the user's codes, then build the model input row(s) [MB][Kc].
 static __global__ void lm_prepare_kernel(const TokenRing r, const long long* __restrict__ in_codes, int n_in,
@@ -293,15 +293,20 @@ inline int attn_pick_splits(int B, int H, int cap) {
 //     append needs no separate kernel and the oldest key it replaces is never attended;
 //   * q is rotated in registers (rounded to bf16 like the reference's apply_rope output);
 //   * with nsplit > 1 the last CTA to arrive for a (b, h) merges the partials in split order.
+// PAGED: kc / vc are page pools [n_pages + 1][H][page_slots][ATT_D] (b200_lm_set_kv_pool) and slot s of row b lives at
+// page table[b * tab_ld + (s >> page_shift)], offset s & (page_slots - 1).  Only the key address changes: the split
+// boundaries, the per-key arithmetic and the merge order are those of the contiguous ring, so the output is bit-identical.
+// The table must map every slot the step reads or writes (kv_page_alloc_kernel does, with the sink page when the pool is dry).
 // ---------------------------------------------------------------------------------------------
 struct AttnStep {
   const bf16* qkv; bf16* kc; bf16* vc; bf16* out;
   float* part; int* counters;                  // [B*H][nsplit][ATT_D + 2], [B*H] (zero between launches)
   const long long* pos; const uint8_t* exec_mask;
   int H, cap, nsplit; float neg_log_period_2_over_d;
+  const int* table; int tab_ld, page_shift;    // PAGED only: page table [B][tab_ld], log2(page_slots)
 };
 
-template <int ATT_U>       // keys per half-warp per register buffer
+template <int ATT_U, bool PAGED = false>       // keys per half-warp per register buffer; paged rings
 static __global__ void __launch_bounds__(ATT_THREADS) attn_step_kernel(const AttnStep a) {
   pdl_trigger();
   const int bh = blockIdx.x, split = blockIdx.y;
@@ -319,6 +324,11 @@ static __global__ void __launch_bounds__(ATT_THREADS) attn_step_kernel(const Att
   const int slot_new = (int)(p % a.cap);
   const bf16* base = a.qkv + (long long)b * 3 * C + h * ATT_D;
   const float fpos = (float)p;
+  // PAGED: element offset of slot s of this (b, h) in the pool
+  auto paged_off = [&](int s) -> long long {
+    const int pg = __ldg(a.table + (long long)b * a.tab_ld + (s >> a.page_shift));
+    return ((((long long)pg * a.H + h) << a.page_shift) + (s & ((1 << a.page_shift) - 1))) * ATT_D;
+  };
 
   if (exec && slot_new >= s0 && slot_new < s1) {    // CTA-uniform: this CTA owns the new key's slot
     if (tid < ATT_D / 2) {
@@ -328,7 +338,9 @@ static __global__ void __launch_bounds__(ATT_THREADS) attn_step_kernel(const Att
       float sn, cs;
       sincosf(freq * fpos, &sn, &cs);
       const float c2 = kr * cs - ki * sn, d2 = kr * sn + ki * cs;
-      const long long o = ((long long)bh * a.cap + slot_new) * ATT_D + 2 * pr;
+      long long o;
+      if constexpr (PAGED) o = paged_off(slot_new) + 2 * pr;
+      else o = ((long long)bh * a.cap + slot_new) * ATT_D + 2 * pr;
       *reinterpret_cast<__nv_bfloat162*>(a.kc + o) = __floats2bfloat162_rn(c2, d2);
       *reinterpret_cast<__nv_bfloat162*>(a.vc + o) = *reinterpret_cast<const __nv_bfloat162*>(base + 2 * C + 2 * pr);
     }
@@ -352,8 +364,9 @@ static __global__ void __launch_bounds__(ATT_THREADS) attn_step_kernel(const Att
     }
   }
 
-  const bf16* kb = a.kc + (long long)bh * a.cap * ATT_D + l16 * 8;
-  const bf16* vb = a.vc + (long long)bh * a.cap * ATT_D + l16 * 8;
+  const long long row0 = PAGED ? 0 : (long long)bh * a.cap * ATT_D;
+  const bf16* kb = a.kc + row0 + l16 * 8;
+  const bf16* vb = a.vc + row0 + l16 * 8;
   float m = -INFINITY, l = 0.f, acc[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) acc[i] = 0.f;
@@ -367,8 +380,11 @@ static __global__ void __launch_bounds__(ATT_THREADS) attn_step_kernel(const Att
 #pragma unroll
     for (int u = 0; u < U; ++u) {
       const int ss = s + u < s1 ? s + u : s1 - 1;
-      gp.k[u] = *reinterpret_cast<const uint4*>(kb + (long long)ss * ATT_D);
-      gp.v[u] = *reinterpret_cast<const uint4*>(vb + (long long)ss * ATT_D);
+      long long o;
+      if constexpr (PAGED) o = paged_off(ss);
+      else o = (long long)ss * ATT_D;
+      gp.k[u] = *reinterpret_cast<const uint4*>(kb + o);
+      gp.v[u] = *reinterpret_cast<const uint4*>(vb + o);
     }
   };
   auto reduce_group = [&](int kb0, const Group& gp) {
@@ -453,6 +469,8 @@ static __global__ void __launch_bounds__(ATT_THREADS) attn_step_kernel(const Att
   }
   a.out[(long long)bh * ATT_D + tid] = f2bf(LL > 0.f ? AA / LL : 0.f);
 }
+// the paged rings run the default register-buffer depth only
+static void (*const attn_step_paged_kernel)(const AttnStep) = attn_step_kernel<4, true>;
 
 // ---------------------------------------------------------------------------------------------
 // Opt-in 8-bit KV rings (SURVEY.md 8f item 3; NOT the reference's numerics): the same fused step as attn_step_kernel
@@ -777,6 +795,104 @@ static __global__ void kv_capacity_check_kernel(const long long* __restrict__ po
   pdl_trigger();
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b < B && exec_mask[b] && pos[b] >= cap && err != nullptr) atomicOr(err, ERR_KV_CAPACITY);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Paged temporal KV pool (b200_lm_set_kv_pool): one page table [MB][tab_ld] shared by all layers (-1 = unmapped), a stack of
+// free page ids and its top, all on the device.  A row holds its pages as a prefix of its table (held[b] of them); entries
+// past that prefix are unmapped, or the sink page n_pages while the pool is dry.  One CTA of KV_PAGE_THREADS >= MB threads
+// scans the rows in row order, so which row gets which page is deterministic.
+// ---------------------------------------------------------------------------------------------
+constexpr int KV_PAGE_THREADS = 256;
+
+__device__ __forceinline__ int block_inclusive_scan(int v, int* s) {
+  const int t = threadIdx.x;
+  s[t] = v;
+  __syncthreads();
+  for (int o = 1; o < KV_PAGE_THREADS; o <<= 1) {
+    const int w = t >= o ? s[t - o] : 0;
+    __syncthreads();
+    s[t] += w;
+    __syncthreads();
+  }
+  return s[t];
+}
+
+// Before the first layer of a step: every executing row gets pages until slots [0, min(pos + 1, cap)) are mapped.  A row the
+// pool cannot serve maps its missing entries to the sink page and raises ERR_KV_POOL; it keeps asking every step.
+static __global__ void __launch_bounds__(KV_PAGE_THREADS) kv_page_alloc_kernel(int* __restrict__ table, int* __restrict__ held,
+    const int* __restrict__ free_stack, int* __restrict__ top, const long long* __restrict__ pos, const uint8_t* __restrict__ exec_mask,
+    int B, int tab_ld, int page_shift, int cap, int sink, int* err) {
+  __shared__ int s[KV_PAGE_THREADS];
+  pdl_trigger();
+  const int b = threadIdx.x;
+  int have = 0, need = 0;
+  if (b < B && exec_mask[b]) {
+    const long long n = min(pos[b] + 1, (long long)cap);
+    const int want = (int)((n + (1 << page_shift) - 1) >> page_shift);
+    have = held[b];
+    need = max(want - have, 0);
+  }
+  const int end = block_inclusive_scan(need, s), start = end - need;
+  const int avail = *top;
+  const int total = s[KV_PAGE_THREADS - 1];
+  __syncthreads();                     // every thread has read the top before it moves
+  if (need > 0) {
+    int* row = table + (long long)b * tab_ld;
+    int got = 0;
+    for (int i = 0; i < need; ++i) {
+      const int k = start + i;         // this row's i-th page is the k-th pop of this step
+      if (k < avail) { row[have + i] = free_stack[avail - 1 - k]; ++got; }
+      else row[have + i] = sink;
+    }
+    held[b] = have + got;
+    if (got < need && err != nullptr) atomicOr(err, ERR_KV_POOL);
+  }
+  if (b == 0) *top = avail - min(total, avail);
+}
+
+// b200_lm_reset: the masked sessions' rows (b and b + B under CFG, lm.py:653-656; null mask = all) push their pages back in row
+// and table order and become unmapped.
+static __global__ void __launch_bounds__(KV_PAGE_THREADS) kv_page_free_kernel(int* __restrict__ table, int* __restrict__ held,
+    int* __restrict__ free_stack, int* __restrict__ top, const uint8_t* __restrict__ mask, int B, int MB, int tab_ld) {
+  __shared__ int s[KV_PAGE_THREADS];
+  const int r = threadIdx.x;
+  const bool f = r < MB && (mask == nullptr || mask[r < B ? r : r - B]);
+  const int n = f ? held[r] : 0;
+  const int end = block_inclusive_scan(n, s), start = end - n;
+  const int t0 = *top;
+  const int total = s[KV_PAGE_THREADS - 1];
+  __syncthreads();
+  if (f) {
+    int* row = table + (long long)r * tab_ld;
+    for (int i = 0; i < n; ++i) free_stack[t0 + start + i] = row[i];
+    for (int i = 0; i < tab_ld; ++i) row[i] = -1;
+    held[r] = 0;
+  }
+  if (r == 0) *top = t0 + total;
+}
+
+// Streaming-state view of a paged layer as the contiguous ring [MB][H][cap][ATT_D]: GATHER reads the pool (slots at or past the
+// row's fill min(pos, cap), and unmapped or sink pages, read as zeros); otherwise the fill's slots are scattered into the pool.
+template <bool GATHER>
+static __global__ void kv_page_copy_kernel(bf16* __restrict__ pool, bf16* __restrict__ ring, const int* __restrict__ table,
+                                           const long long* __restrict__ pos, int H, int cap, int tab_ld, int page_shift, int sink,
+                                           long long n_vec) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;   // one 16-byte vector of 8 elements
+  if (i >= n_vec) return;
+  constexpr int V = ATT_D / 8;
+  const int c = (int)(i % V);
+  const long long rs = i / V;
+  const int s = (int)(rs % cap);
+  const long long bh = rs / cap;
+  const int b = (int)(bh / H), h = (int)(bh % H);
+  const int pg = table[(long long)b * tab_ld + (s >> page_shift)];
+  const bool valid = s < min(pos[b], (long long)cap) && pg >= 0 && pg < sink;
+  uint4* rv = reinterpret_cast<uint4*>(ring) + i;
+  uint4* pv = reinterpret_cast<uint4*>(pool) +
+              ((((long long)pg * H + h) << page_shift) + (s & ((1 << page_shift) - 1))) * V + c;
+  if (GATHER) *rv = valid ? *pv : make_uint4(0, 0, 0, 0);
+  else if (valid) *pv = *rv;
 }
 
 static __global__ void advance_pos_kernel(long long* pos, const uint8_t* exec_mask, int B) {

@@ -156,6 +156,30 @@ int b200_op_attn_step(const void* qkv_dev, void* k_dev, void* v_dev, void* out_d
   return check_launch("op_attn_step");
 }
 
+int b200_op_attn_step_paged(const void* qkv_dev, void* k_pool_dev, void* v_pool_dev, const int32_t* page_table_dev, void* out_dev,
+                            const int64_t* pos_dev, const uint8_t* exec_mask_dev, int B, int H, int cap, int page_slots, int nsplit,
+                            float max_period, void* stream) {
+  using namespace b200::lm;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (B < 1 || H < 1 || cap < 1) B200_FAIL(B200_ERR_SHAPE, "op_attn_step_paged: bad shape");
+  if (page_slots < 4 || page_slots > 256 || (page_slots & (page_slots - 1)))
+    B200_FAIL(B200_ERR_INVALID, "op_attn_step_paged: page_slots %d (a power of two in [4, 256])", page_slots);
+  if (!page_table_dev) B200_FAIL(B200_ERR_INVALID, "op_attn_step_paged: null page table");
+  if (nsplit <= 0) nsplit = attn_pick_splits(B, H, cap);
+  float* part = nullptr;
+  int* counters = nullptr;
+  B200_TRY(attn_scratch(B, H, nsplit, &part, &counters, 0));
+  AttnStep a;
+  a.qkv = static_cast<const bf16*>(qkv_dev); a.kc = static_cast<bf16*>(k_pool_dev); a.vc = static_cast<bf16*>(v_pool_dev);
+  a.out = static_cast<bf16*>(out_dev); a.part = part; a.counters = counters;
+  a.pos = reinterpret_cast<const long long*>(pos_dev); a.exec_mask = exec_mask_dev; a.H = H; a.cap = cap; a.nsplit = nsplit;
+  a.neg_log_period_2_over_d = -logf(max_period) * 2.f / (float)ATT_D;
+  a.table = page_table_dev; a.tab_ld = (cap + page_slots - 1) / page_slots; a.page_shift = __builtin_ctz(page_slots);
+  dim3 grid(B * H, nsplit);
+  B200_LAUNCH(attn_step_paged_kernel, grid, ATT_THREADS, 0, st, a);
+  return check_launch("op_attn_step_paged");
+}
+
 int b200_op_attn_step_q8(const void* qkv_dev, void* k8_dev, void* v8_dev, float* ks_dev, float* vs_dev, void* out_dev,
                          const int64_t* pos_dev, const uint8_t* exec_mask_dev, int B, int H, int cap, int nsplit, float max_period,
                          int kv_dtype, void* stream) {

@@ -178,6 +178,10 @@ class LMGen:
         # slots per temporal KV ring; None = the model's context (the reference's RingKVCache).  A pool of sessions younger than
         # `kv_capacity` frames holds the same keys in kv_capacity / context of the memory; stepping past it raises error flag 4
         self.kv_capacity: int | None = None
+        # paged temporal KV rings: the rings of all model rows share a pool of `kv_pool_frames` slots in pages of `kv_page_slots`;
+        # a row takes pages as its fill grows and returns them on reset (None = one full ring per row).  Same numerics, bit for bit
+        self.kv_pool_frames: int | None = None
+        self.kv_page_slots = 64
 
     # ---- plumbing ---------------------------------------------------------------------------------
     def _device(self):
@@ -226,6 +230,7 @@ class LMGen:
                 raise ValueError(f"kv_dtype {self.kv_dtype!r}: expected one of {sorted(kinds)}")
             _lib.check(self._lib.b200_lm_set_kv_dtype(self._h, kinds[self.kv_dtype]))
             _lib.check(self._lib.b200_lm_set_kv_capacity(self._h, int(self.kv_capacity or 0)))
+            _lib.check(self._lib.b200_lm_set_kv_pool(self._h, int(self.kv_pool_frames or 0), int(self.kv_page_slots)))
             until = None
             if self.cfg_coef != 1. and self.cfg_is_masked_until is not None:
                 until = (C.c_int64 * len(self.cfg_is_masked_until))(*[int(v) for v in self.cfg_is_masked_until])
@@ -396,11 +401,19 @@ class LMGen:
 
     def error_flags(self) -> int:
         """Synchronises and returns (and clears) the device error flags (1 = a token id outside its embedding table, 4 = a session
-        stepped past a shortened KV ring, `kv_capacity`)."""
+        stepped past a shortened KV ring, `kv_capacity`; 8 = a session's KV ring did not get a page because the `kv_pool_frames`
+        pool was full: that session's output is garbage until it is reset, the others are unaffected)."""
         v = C.c_int(0)
         with self._device():
             _lib.check(self._lib.b200_lm_error_flags(self._h, C.byref(v)))
         return v.value
+
+    def kv_pool_usage(self) -> tuple[int, int]:
+        """(pages held by the model's rows, pages in the pool) of a `kv_pool_frames` handle; (0, 0) without a pool.  Synchronises."""
+        used, total = C.c_int(0), C.c_int(0)
+        with self._device():
+            _lib.check(self._lib.b200_lm_kv_pool_usage(self._h, C.byref(used), C.byref(total)))
+        return used.value, total.value
 
     # ---- the step ---------------------------------------------------------------------------------
     @torch.no_grad()

@@ -77,7 +77,8 @@ class DialogueService:
     """
 
     def __init__(self, batch_size: int, lm, mimi, use_sampling: bool = True, temp: float = 0.8, temp_text: float = 0.7,
-                 top_k: int = 250, top_k_text: int = 25, kv_dtype: str = "bf16", kv_capacity: int | None = None):
+                 top_k: int = 250, top_k_text: int = 25, kv_dtype: str = "bf16", kv_capacity: int | None = None,
+                 kv_pool_frames: int | None = None):
         import ctypes as C
 
         from . import _lib
@@ -88,6 +89,7 @@ class DialogueService:
                             support_out_of_sync=True)
         self.lm_gen.kv_dtype = kv_dtype
         self.lm_gen.kv_capacity = kv_capacity
+        self.lm_gen.kv_pool_frames = kv_pool_frames
         self.lm_gen.streaming_forever(batch_size)
         self.mimi.streaming_forever(batch_size)
         self._lib = _lib.lib()
@@ -107,6 +109,15 @@ class DialogueService:
         _lib.check(self._lib.b200_frame_read_buffer(self._h, name.encode(), _lib.ptr(out), out.numel() * out.element_size(), C.byref(n)))
         assert n.value == out.numel() * out.element_size(), (name, n.value, shape)
         return out
+
+    def release(self, slots) -> None:
+        """Resets the LM and Mimi rows of closed session slots, so that a paged LM (``kv_pool_frames``) returns their KV pages to
+        the pool now rather than when the slot's next session sends its RESET frame."""
+        mask = torch.zeros(self.batch_size, dtype=torch.bool)
+        mask[list(slots)] = True
+        if mask.any():
+            self.lm_gen.reset_streaming(mask)
+            self.mimi.reset_streaming(mask)
 
     def close(self) -> None:
         if getattr(self, "_h", None):
