@@ -134,6 +134,13 @@ int b200_mimi_state_count(b200_mimi* h);
 int b200_mimi_state_entry(b200_mimi* h, int index, const char** name, int* dtype, int* ndim, int64_t* shape8, int64_t* nbytes);
 int b200_mimi_state_read(b200_mimi* h, const char* name, void* dst_dev, int64_t nbytes);
 int b200_mimi_state_write(b200_mimi* h, const char* name, const void* src_dev, int64_t nbytes);
+/* One session (one row) of a Mimi handle, encoder and decoder state, as a device record of b200_mimi_session_bytes bytes
+ * (fixed per configuration): the row's slice of every entry above.  Export does not change the source; import replaces row
+ * `row` only, after the same checks as b200_lm_session_import (B200_ERR_INVALID: not a record, an LM record, another codec
+ * configuration, row outside [0, B); B200_ERR_SHAPE: nbytes differs).  Both synchronise the handle's stream. */
+int b200_mimi_session_bytes(b200_mimi* h, int64_t* nbytes);
+int b200_mimi_session_export(b200_mimi* h, int row, void* dst_dev, int64_t capacity);
+int b200_mimi_session_import(b200_mimi* h, int row, const void* src_dev, int64_t nbytes);
 /* Synchronises, returns and clears the device error flags: B200_FLAG_CODE_RANGE = MimiModel.decode was given a code outside
  * [0, bins) (it decodes as the zero vector; the reference indexes out of bounds: "dramatic CUDA crash", vq.py:144-145). */
 int b200_mimi_error_flags(b200_mimi* h, int* flags_out);
@@ -289,7 +296,7 @@ int b200_lm_set_kv_dtype(b200_lm* h, int kv_dtype);
  * RingKVCache transformer.py:196-288).  A shorter ring holds the same keys as the reference's for a session's first `slots`
  * frames (nothing is evicted before position `context`), at slots/context of the 1.573 GB per session: a pool of young sessions
  * (SURVEY.md 8f item 3, "rings sized to live fill").  A row that steps past the capacity raises B200_FLAG_KV_CAPACITY; the
- * caller moves such a session to a full-size handle (get / set streaming state) before that. */
+ * caller moves such a session to a full-size handle (b200_lm_session_export / _import) before that. */
 int b200_lm_set_kv_capacity(b200_lm* h, int slots);
 /* Paged temporal KV rings, chosen before b200_lm_streaming_begin (frames = 0: off, the default).  The rings of all model
  * rows share one pool of `frames` slots, rounded up to whole pages of `page_slots` slots (a power of two in [4, 256]) and
@@ -303,6 +310,29 @@ int b200_lm_set_kv_capacity(b200_lm* h, int slots);
 int b200_lm_set_kv_pool(b200_lm* h, int64_t frames, int page_slots);
 /* Pages held by rows and pages in the pool (0 / 0 without a pool).  Synchronises the handle's stream. */
 int b200_lm_kv_pool_usage(b200_lm* h, int* pages_used, int* pages_total);
+/* One session (one row) of an LM handle as a self-describing device record (layout in DESIGN.md §2): moves a session between
+ * rows, handles and GPUs, e.g. from a short ring (B200_FLAG_KV_CAPACITY) or a paged pool close to dry into another handle.
+ * The record holds the session's token ring, offsets, model positions (and under CFG its model exec flags and
+ * cfg_is_masked_until, with condition_sum on its rows) and the temporal K/V of slots [0, min(pos, ring capacity)), so its size
+ * follows the session's fill.  All three synchronise the handle's stream.
+ *   session_bytes: the size b200_lm_session_export would write for `row` now.
+ *   session_export: does not change the source.  It is ordered after every step already enqueued on the handle's stream; the
+ *     row keeps running, and the caller resets or releases it when the move is complete.  B200_ERR_STATE for a short-ring row
+ *     (b200_lm_set_kv_capacity) that has stepped past its capacity: its ring no longer holds the history.  B200_ERR_SHAPE if
+ *     capacity is below the record's size.
+ *   session_import: replaces model rows `row` (and row + B under CFG) with the record and changes no other row, page-table
+ *     entry or output.  On a paged handle the row first gives back its pages, then holds exactly
+ *     ceil(min(pos, context) / page_slots) pages.  Every check runs before the first write; on failure nothing changes:
+ *     B200_ERR_INVALID: not a record of this version, a Mimi record, another model configuration, another KV storage type,
+ *       CFG (or cfg_is_masked_until) or condition_sum on one side only, a row outside [0, B);
+ *     B200_ERR_SHAPE: nbytes differs from the record's size;
+ *     B200_ERR_STATE: the handle cannot hold the history: too few free pages in the pool, or a ring shorter than the
+ *       session's position (this includes a wrapped session, pos > context, sent to a short ring).
+ * Handle-wide values do not travel: the host step counter (offset_cpu) and the noise seed and counter; a moved session
+ * continues with the destination's noise stream.  Its readiness (tokens -2 until offsets > max_delay) travels with offsets. */
+int b200_lm_session_bytes(b200_lm* h, int row, int64_t* nbytes);
+int b200_lm_session_export(b200_lm* h, int row, void* dst_dev, int64_t capacity);
+int b200_lm_session_import(b200_lm* h, int row, const void* src_dev, int64_t nbytes);
 
 /* ------------------------------------------------------------------------------------------ */
 /* One dialogue frame for every session slot: host PCM in, host PCM + tokens out, one host wait  */

@@ -72,6 +72,9 @@ _PROTOTYPES: dict[str, tuple[tp.Any, list]] = {
     "b200_mimi_state_entry": (_I, [_P, _I, C.POINTER(C.c_char_p), C.POINTER(_I), C.POINTER(_I), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "b200_mimi_state_read": (_I, [_P, C.c_char_p, _P, C.c_int64]),
     "b200_mimi_state_write": (_I, [_P, C.c_char_p, _P, C.c_int64]),
+    "b200_mimi_session_bytes": (_I, [_P, C.POINTER(C.c_int64)]),
+    "b200_mimi_session_export": (_I, [_P, _I, _P, C.c_int64]),
+    "b200_mimi_session_import": (_I, [_P, _I, _P, C.c_int64]),
     "b200_mimi_error_flags": (_I, [_P, C.POINTER(_I)]),
     "b200_mimi_read_buffer": (_I, [_P, C.c_char_p, _P, C.c_int64, C.POINTER(C.c_int64)]),
     "b200_mimi_algorithmic_bytes": (C.c_int64, [_P]),
@@ -100,6 +103,9 @@ _PROTOTYPES: dict[str, tuple[tp.Any, list]] = {
     "b200_lm_set_kv_capacity": (_I, [_P, _I]),
     "b200_lm_set_kv_pool": (_I, [_P, C.c_int64, _I]),
     "b200_lm_kv_pool_usage": (_I, [_P, C.POINTER(_I), C.POINTER(_I)]),
+    "b200_lm_session_bytes": (_I, [_P, _I, C.POINTER(C.c_int64)]),
+    "b200_lm_session_export": (_I, [_P, _I, _P, C.c_int64]),
+    "b200_lm_session_import": (_I, [_P, _I, _P, C.c_int64]),
     "b200_lm_set_cfg": (_I, [_P, C.c_float, _I, _P, _I]),
     "b200_lm_set_condition_sum": (_I, [_P, _P, _I]),
     "b200_lm_seed_noise": (_I, [_P, C.c_uint64]),

@@ -1,3 +1,5 @@
+#include <algorithm>
+
 #include "common.cuh"
 
 namespace b200 {
@@ -108,6 +110,31 @@ int state_entry_copy(const Arena& a, const char* name, void* dst_dev, const void
   else if (src_dev) B200_CUDA(cudaMemcpyAsync(e->ptr, src_dev, e->bytes, cudaMemcpyDeviceToDevice, st));
   else B200_FAIL(B200_ERR_INVALID, "state entry copy: null buffer");
   return B200_OK;
+}
+
+// blockIdx.y = slice; 16-byte vectors where both sides and the length allow, bytes otherwise
+static __global__ void row_slice_copy_kernel(const RowSlice* __restrict__ table, char* rec, int row, int gather) {
+  const RowSlice d = table[blockIdx.y];
+  char* p = d.ptr + (long long)(row + d.row_add) * d.row_bytes;
+  char* r = rec + d.rec_off;
+  char* dst = gather ? r : p;
+  const char* src = gather ? p : r;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  const long long i0 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (((uintptr_t)dst | (uintptr_t)src | (uintptr_t)d.row_bytes) & 15) {
+    for (long long i = i0; i < d.row_bytes; i += stride) dst[i] = src[i];
+  } else {
+    for (long long i = i0; i < d.row_bytes / 16; i += stride)
+      reinterpret_cast<uint4*>(dst)[i] = reinterpret_cast<const uint4*>(src)[i];
+  }
+}
+
+int row_slice_copy(const RowSlice* table_dev, int n, long long max_row_bytes, char* rec, int row, bool gather, cudaStream_t st) {
+  if (n <= 0) return B200_OK;
+  if (n > 65535) B200_FAIL(B200_ERR_INVALID, "row_slice_copy: %d slices", n);
+  const unsigned gx = (unsigned)std::min<long long>(std::max<long long>(ceil_div64(max_row_bytes, 16 * 256), 1), 256);
+  B200_LAUNCH(row_slice_copy_kernel, dim3(gx, n), 256, 0, st, table_dev, rec, row, gather ? 1 : 0);
+  return check_launch("row_slice_copy");
 }
 
 }  // namespace b200

@@ -141,6 +141,52 @@ inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
 // ---------------------------------------------------------------------------------------------
+// session records (b200_{lm,mimi}_session_*): one session of a handle as a self-describing device buffer
+// ---------------------------------------------------------------------------------------------
+constexpr uint32_t SESSION_MAGIC = 0x5345534Du;      // "MSES"
+constexpr uint32_t SESSION_VERSION = 1;
+enum { SESSION_LM = 1, SESSION_MIMI = 2 };
+// The first 256 bytes of a record; the host reads them before an import writes anything.  The body's layout is the handle's
+// (lm.cu, mimi.cu).
+struct SessionHeader {
+  uint32_t magic, version, kind, kv_dtype;   // kv_dtype: B200_KV_* of an LM record, 0 for Mimi
+  uint64_t fingerprint;                      // config_fingerprint of the model configuration
+  int32_t rows;                              // model rows per session (LM: 2 under classifier-free guidance, else 1)
+  int32_t flags;                             // LM: SESSION_COND / SESSION_CFG_UNTIL
+  int64_t pos[2];                            // LM: model position of each row
+  int64_t n;                                 // LM: temporal KV slots carried, min(pos, ring capacity)
+  int64_t bytes;                             // size of the whole record
+  uint8_t reserved[256 - 64];
+};
+static_assert(sizeof(SessionHeader) == 256, "session header is 256 bytes");
+enum { SESSION_COND = 1, SESSION_CFG_UNTIL = 2 };
+
+// FNV-1a over a configuration struct: records only go into handles built from the same configuration
+inline uint64_t config_fingerprint(const void* p, size_t n) {
+  uint64_t h = 0xcbf29ce484222325ull;
+  for (size_t i = 0; i < n; ++i) h = (h ^ static_cast<const uint8_t*>(p)[i]) * 0x100000001b3ull;
+  return h;
+}
+
+// One per-session slice of a handle's state: row r's bytes are ptr + (r + row_add) * row_bytes, stored at rec_off in a record.
+struct RowSlice {
+  char* ptr;
+  long long row_bytes, rec_off;
+  int row_add;
+};
+// Copies the slices of row `row` between the handle and `rec` (gather: handle -> record), one launch for the whole table.
+// Offsets into the record are 16-byte aligned; max_row_bytes bounds the grid.
+int row_slice_copy(const RowSlice* table_dev, int n, long long max_row_bytes, char* rec, int row, bool gather, cudaStream_t st);
+// Lays out `slices` (row_bytes / ptr / row_add filled) from record offset `off` on, 16-byte aligned; returns the end offset.
+inline long long layout_row_slices(std::vector<RowSlice>& slices, long long off) {
+  for (auto& s : slices) {
+    s.rec_off = off;
+    off += (s.row_bytes + 15) / 16 * 16;
+  }
+  return off;
+}
+
+// ---------------------------------------------------------------------------------------------
 // device helpers
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {

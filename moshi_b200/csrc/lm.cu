@@ -91,6 +91,12 @@ struct b200_lm {
   int n_pages = 0, tab_ld = 0, page_shift = 0;
   int *page_table = nullptr, *page_held = nullptr;     // [MB][tab_ld] (-1 = unmapped), [MB]
   int *free_stack = nullptr, *free_top = nullptr;      // [n_pages], [1]
+  // session records: the temporal rings (pools) as one device list, bf16 [layer][k|v], 8-bit [layer][k8|v8] then [layer][ks|vs] ...
+  void** kv_arrays = nullptr;
+  // ... and the per-session slices of the small state entries; the condition_sum rows come last and travel while it is on
+  RowSlice* slices_dev = nullptr;
+  int n_slices = 0, n_slices_cond = 0;
+  long long slices_end = 0, slices_end_cond = 0, slices_max = 0;
   float *dep_part0 = nullptr, *dep_part1 = nullptr;
   unsigned* dep_bar = nullptr;
   unsigned long long* dep_trace = nullptr;     // B200_DEP_TRACE=1: barrier timestamps of the fused depformer (diagnostics)
@@ -398,30 +404,51 @@ int pool_map(b200_lm* h, const std::vector<long long>& pos, const char* what) {
   return B200_OK;
 }
 
-// The K / V state entry of a paged layer: its ring view is gathered from / scattered into the pool.  Other entries: nullptr.
-bf16* paged_pool_of(const b200_lm* h, const StateEntry& e) {
-  if (!h->n_pages) return nullptr;
-  for (auto& L : h->layers)
-    if (e.ptr == L.kc || e.ptr == L.vc) return static_cast<bf16*>(e.ptr);
-  return nullptr;
+// The K / V state entry of a paged layer: its index in kv_arrays (its ring view is gathered from / scattered into the pool).
+// Other entries: -1.
+int paged_array_of(const b200_lm* h, const StateEntry& e) {
+  if (!h->n_pages) return -1;
+  for (size_t l = 0; l < h->layers.size(); ++l) {
+    if (e.ptr == h->layers[l].kc) return 2 * (int)l;
+    if (e.ptr == h->layers[l].vc) return 2 * (int)l + 1;
+  }
+  return -1;
+}
+
+// K / V of `n_arrays` rings from kv_arrays[first] on, model rows row0 + k * row_step (k < n_rows), slots [0, n), to or from the
+// flat buffer [array][k][H][n][slot] (kv_copy_kernel), on the handle's stream.  `scales`: the fp32 rings of an 8-bit handle.
+int kv_copy(b200_lm* h, int first, int n_arrays, int row0, int n_rows, int row_step, int n, void* flat, bool gather, bool scales) {
+  if (n <= 0) return B200_OK;
+  KvCopy a;
+  a.arrays = h->kv_arrays + first; a.flat = flat; a.pos = h->pos;
+  a.table = h->n_pages ? h->page_table : nullptr; a.tab_ld = h->tab_ld; a.page_shift = h->page_shift; a.sink = h->n_pages;
+  a.row0 = row0; a.n_rows = n_rows; a.row_step = row_step; a.H = h->cfg.num_heads; a.cap = ring_cap(h); a.n = n;
+  const long long segs = (long long)n_arrays * n_rows * a.H;
+  if (segs > 65535) B200_FAIL(B200_ERR_INVALID, "kv_copy: %lld ring segments in one launch", segs);
+  const int V = scales ? 1 : h->kv_fp8 ? ATT_D / 16 : ATT_D / 8;     // 4-byte scales, 16-byte vectors of bytes or bf16
+  const dim3 grid((unsigned)ceil_div(n * V, 256), (unsigned)segs);
+  if (scales) {
+    if (gather) B200_LAUNCH((kv_copy_kernel<true, uint32_t, 1>), grid, 256, 0, h->stream, a);
+    else B200_LAUNCH((kv_copy_kernel<false, uint32_t, 1>), grid, 256, 0, h->stream, a);
+  } else if (h->kv_fp8) {
+    if (gather) B200_LAUNCH((kv_copy_kernel<true, uint4, ATT_D / 16>), grid, 256, 0, h->stream, a);
+    else B200_LAUNCH((kv_copy_kernel<false, uint4, ATT_D / 16>), grid, 256, 0, h->stream, a);
+  } else {
+    if (gather) B200_LAUNCH((kv_copy_kernel<true, uint4, ATT_D / 8>), grid, 256, 0, h->stream, a);
+    else B200_LAUNCH((kv_copy_kernel<false, uint4, ATT_D / 8>), grid, 256, 0, h->stream, a);
+  }
+  return check_launch("kv_copy");
 }
 
 // One state entry between the handle and a device buffer (exactly one of dst / src is non-null), on the handle's stream.
 int state_copy(b200_lm* h, const StateEntry& e, void* dst, const void* src) {
-  bf16* pool = paged_pool_of(h, e);
-  if (!pool) {
+  const int arr = paged_array_of(h, e);
+  if (arr < 0) {
     if (dst) B200_CUDA(cudaMemcpyAsync(dst, e.ptr, e.bytes, cudaMemcpyDeviceToDevice, h->stream));
     else B200_CUDA(cudaMemcpyAsync(e.ptr, src, e.bytes, cudaMemcpyDeviceToDevice, h->stream));
     return B200_OK;
   }
-  const long long n_vec = (long long)(e.bytes / 16);
-  const unsigned grid = (unsigned)ceil_div64(n_vec, 256);
-  const int H = h->cfg.num_heads, cap = h->cfg.context;
-  if (dst) B200_LAUNCH(kv_page_copy_kernel<true>, grid, 256, 0, h->stream, pool, static_cast<bf16*>(dst), h->page_table, h->pos, H, cap,
-                       h->tab_ld, h->page_shift, h->n_pages, n_vec);
-  else B200_LAUNCH(kv_page_copy_kernel<false>, grid, 256, 0, h->stream, pool, const_cast<bf16*>(static_cast<const bf16*>(src)),
-                   h->page_table, h->pos, H, cap, h->tab_ld, h->page_shift, h->n_pages, n_vec);
-  return check_launch("kv_page_copy");
+  return kv_copy(h, arr, 1, 0, h->MB, 1, h->cfg.context, dst ? dst : const_cast<void*>(src), dst != nullptr, false);
 }
 
 // the model positions a write of `model.offset` from `src_dev` would set, on the host
@@ -429,6 +456,104 @@ int read_positions(b200_lm* h, const void* src_dev, std::vector<long long>* pos)
   pos->assign(h->MB, 0);
   B200_CUDA(cudaStreamSynchronize(h->stream));
   B200_CUDA(cudaMemcpy(pos->data(), src_dev, (size_t)h->MB * 8, cudaMemcpyDeviceToHost));
+  return B200_OK;
+}
+
+// ---- session records (b200_lm_session_*) ----------------------------------------------------------------------------------
+// After the 256-byte SessionHeader: the session's slices of exec_mask, cache, offsets, model.offset (1 or 2 rows), under CFG
+// model.exec_mask (2 rows) and cfg_is_masked_until, and while it is on the condition_sum rows, each 16-byte aligned (the
+// RowSlice table of streaming_begin).  From the next 256-byte boundary, the temporal K/V of slots [0, n), n = min(pos, ring
+// capacity), slot s being position s mod capacity: [layer][k|v][model row][head][n][128] bf16, or for 8-bit rings the bytes in
+// that layout followed by the fp32 scales [layer][k|v][model row][head][n].
+struct SessionPlan {
+  int rows = 1;
+  int64_t pos[2] = {0, 0};
+  int64_t n = 0, kv_off = 0, bytes = 0;
+  bool cond = false;
+};
+
+// K/V bytes of one slot of one model row, all layers
+int64_t kv_slot_bytes(const b200_lm* h) {
+  return (int64_t)h->cfg.num_layers * 2 * h->cfg.num_heads * (h->kv_fp8 ? ATT_D + 4 : ATT_D * 2);
+}
+
+void session_size(const b200_lm* h, SessionPlan* p) {
+  const long long end = p->cond ? h->slices_end_cond : h->slices_end;
+  p->kv_off = (end + 255) / 256 * 256;
+  p->bytes = p->kv_off + kv_slot_bytes(h) * p->rows * p->n;
+}
+
+uint64_t lm_fingerprint(const b200_lm* h) { return config_fingerprint(&h->cfg, sizeof(h->cfg)); }
+
+// The record row `row` would export now (synchronises): B200_ERR_STATE for a short-ring row whose ring has already wrapped.
+int session_plan(b200_lm* h, int row, const char* what, SessionPlan* p) {
+  if (row < 0 || row >= h->batch) B200_FAIL(B200_ERR_INVALID, "%s: row %d outside [0, %d)", what, row, h->batch);
+  p->rows = h->MB / h->batch;
+  B200_CUDA(cudaStreamSynchronize(h->stream));
+  for (int k = 0; k < p->rows; ++k)
+    B200_CUDA(cudaMemcpy(&p->pos[k], h->pos + row + (size_t)k * h->batch, 8, cudaMemcpyDeviceToHost));
+  const int64_t top = std::max(p->pos[0], p->pos[1]);
+  const int cap = ring_cap(h);
+  if (cap < h->cfg.context && top > cap)
+    B200_FAIL(B200_ERR_STATE, "%s: row %d stepped past its %d-slot KV ring (position %lld): its history is lost", what, row, cap,
+              (long long)top);
+  p->n = std::min<int64_t>(top, cap);
+  p->cond = h->cond_on != 0;
+  session_size(h, p);
+  return B200_OK;
+}
+
+// The session's K/V between the rings and the record
+int session_kv(b200_lm* h, int row, const SessionPlan& p, char* rec, bool gather) {
+  const int L2 = 2 * (int)h->layers.size();
+  B200_TRY(kv_copy(h, 0, L2, row, p.rows, h->batch, (int)p.n, rec + p.kv_off, gather, false));
+  if (h->kv_fp8) {
+    const int64_t scales = p.kv_off + (int64_t)L2 * p.rows * h->cfg.num_heads * p.n * ATT_D;
+    B200_TRY(kv_copy(h, L2, L2, row, p.rows, h->batch, (int)p.n, rec + scales, gather, true));
+  }
+  return B200_OK;
+}
+
+// Paged import, synchronous, this session's rows only: each gives back its pages past what pos[k] needs, then takes the
+// missing ones from the free stack.  B200_ERR_STATE, changing nothing, when the pool cannot supply them.
+int session_map(b200_lm* h, int row, const SessionPlan& p) {
+  const int T = h->tab_ld, B = h->batch;
+  std::vector<int> table((size_t)p.rows * T), held(p.rows), stack(h->n_pages);
+  int top = 0;
+  for (int k = 0; k < p.rows; ++k) {
+    B200_CUDA(cudaMemcpy(table.data() + (size_t)k * T, h->page_table + (size_t)(row + k * B) * T, (size_t)T * 4, cudaMemcpyDeviceToHost));
+    B200_CUDA(cudaMemcpy(&held[k], h->page_held + row + k * B, 4, cudaMemcpyDeviceToHost));
+  }
+  B200_CUDA(cudaMemcpy(stack.data(), h->free_stack, stack.size() * 4, cudaMemcpyDeviceToHost));
+  B200_CUDA(cudaMemcpy(&top, h->free_top, 4, cudaMemcpyDeviceToHost));
+  int returned = 0, missing = 0;
+  for (int k = 0; k < p.rows; ++k) {
+    const int want = pages_for(h, p.pos[k]);
+    returned += std::max(held[k] - want, 0);
+    missing += std::max(want - held[k], 0);
+  }
+  if (missing > top + returned)
+    B200_FAIL(B200_ERR_STATE, "lm_session_import: the session needs %d more KV pages, the pool has %d free", missing - returned, top);
+  for (int k = 0; k < p.rows; ++k) {
+    const int want = pages_for(h, p.pos[k]);
+    int* r = table.data() + (size_t)k * T;
+    for (int i = want; i < T; ++i) {
+      if (i < held[k]) stack[top++] = r[i];
+      r[i] = -1;
+    }
+    held[k] = std::min(held[k], want);
+  }
+  for (int k = 0; k < p.rows; ++k) {
+    const int want = pages_for(h, p.pos[k]);
+    for (int i = held[k]; i < want; ++i) table[(size_t)k * T + i] = stack[--top];
+    held[k] = want;
+  }
+  for (int k = 0; k < p.rows; ++k) {
+    B200_CUDA(cudaMemcpy(h->page_table + (size_t)(row + k * B) * T, table.data() + (size_t)k * T, (size_t)T * 4, cudaMemcpyHostToDevice));
+    B200_CUDA(cudaMemcpy(h->page_held + row + k * B, &held[k], 4, cudaMemcpyHostToDevice));
+  }
+  B200_CUDA(cudaMemcpy(h->free_stack, stack.data(), stack.size() * 4, cudaMemcpyHostToDevice));
+  B200_CUDA(cudaMemcpy(h->free_top, &top, 4, cudaMemcpyHostToDevice));
   return B200_OK;
 }
 
@@ -855,6 +980,37 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
       A.mark_state(L.vc, (size_t)MB * H * cap * D * 2, p + ".v", B200_BF16, {MB, H, cap, D});
     }
   }
+  {
+    std::vector<void*> arrays;
+    for (auto& L : h->layers) {
+      if (h->kv_fp8) { arrays.push_back(L.kc8); arrays.push_back(L.vc8); }
+      else { arrays.push_back(L.kc); arrays.push_back(L.vc); }
+    }
+    if (h->kv_fp8)
+      for (auto& L : h->layers) { arrays.push_back(L.ks); arrays.push_back(L.vs); }
+    B200_TRY(A.alloc_t(&h->kv_arrays, arrays.size(), false));
+    B200_CUDA(cudaMemcpy(h->kv_arrays, arrays.data(), arrays.size() * sizeof(void*), cudaMemcpyHostToDevice));
+    const int rows_add[2] = {0, B};
+    std::vector<RowSlice> s;
+    auto add = [&](void* p, long long row_bytes, int model_rows) {
+      for (int k = 0; k < model_rows; ++k) s.push_back({static_cast<char*>(p), row_bytes, 0, rows_add[k]});
+    };
+    add(h->exec_mask, 1, 1);
+    add(h->cache, (long long)h->Kc * h->CT * 8, 1);
+    add(h->offsets, 8, 1);
+    add(h->pos, 8, MB / B);
+    if (cfg) add(h->exec_mask_m, 1, 2);
+    if (h->cfg_until) add(h->cfg_until, 8, 1);
+    h->n_slices = (int)s.size();
+    add(h->cond_sum, (long long)d * 2, MB / B);
+    h->n_slices_cond = (int)s.size();
+    h->slices_end_cond = layout_row_slices(s, sizeof(SessionHeader));
+    h->slices_end = s[h->n_slices].rec_off;
+    h->slices_max = 0;
+    for (auto& e : s) h->slices_max = std::max(h->slices_max, e.row_bytes);
+    B200_TRY(A.alloc_t(&h->slices_dev, s.size(), false));
+    B200_CUDA(cudaMemcpy(h->slices_dev, s.data(), s.size() * sizeof(RowSlice), cudaMemcpyHostToDevice));
+  }
   B200_CUDA(cudaDeviceSynchronize());
   cleanup.armed = false;
   h->batch = B;
@@ -1059,6 +1215,80 @@ int b200_lm_kv_pool_usage(b200_lm* h, int* pages_used, int* pages_total) {
   }
   if (pages_used) *pages_used = h->n_pages - top;
   if (pages_total) *pages_total = h->n_pages;
+  return B200_OK;
+}
+
+int b200_lm_session_bytes(b200_lm* h, int row, int64_t* nbytes) {
+  B200_TRY(ensure_streaming(h, "lm_session_bytes"));
+  DeviceGuard g(h->device);
+  SessionPlan p;
+  B200_TRY(session_plan(h, row, "lm_session_bytes", &p));
+  if (nbytes) *nbytes = p.bytes;
+  return B200_OK;
+}
+
+int b200_lm_session_export(b200_lm* h, int row, void* dst_dev, int64_t capacity) {
+  B200_TRY(ensure_streaming(h, "lm_session_export"));
+  DeviceGuard g(h->device);
+  SessionPlan p;
+  B200_TRY(session_plan(h, row, "lm_session_export", &p));
+  if (!dst_dev) B200_FAIL(B200_ERR_INVALID, "lm_session_export: null destination");
+  if (capacity < p.bytes) B200_FAIL(B200_ERR_SHAPE, "lm_session_export: the record takes %lld bytes, capacity %lld", (long long)p.bytes, (long long)capacity);
+  SessionHeader s;
+  memset(&s, 0, sizeof(s));
+  s.magic = SESSION_MAGIC; s.version = SESSION_VERSION; s.kind = SESSION_LM; s.kv_dtype = (uint32_t)h->kv_fp8;
+  s.fingerprint = lm_fingerprint(h); s.rows = p.rows;
+  s.flags = (p.cond ? SESSION_COND : 0) | (h->cfg_until ? SESSION_CFG_UNTIL : 0);
+  s.pos[0] = p.pos[0]; s.pos[1] = p.pos[1]; s.n = p.n; s.bytes = p.bytes;
+  char* rec = static_cast<char*>(dst_dev);
+  B200_CUDA(cudaMemcpyAsync(rec, &s, sizeof(s), cudaMemcpyHostToDevice, h->stream));
+  B200_TRY(row_slice_copy(h->slices_dev, p.cond ? h->n_slices_cond : h->n_slices, h->slices_max, rec, row, true, h->stream));
+  B200_TRY(session_kv(h, row, p, rec, true));
+  B200_CUDA(cudaStreamSynchronize(h->stream));
+  return B200_OK;
+}
+
+int b200_lm_session_import(b200_lm* h, int row, const void* src_dev, int64_t nbytes) {
+  B200_TRY(ensure_streaming(h, "lm_session_import"));
+  DeviceGuard g(h->device);
+  const auto& c = h->cfg;
+  if (row < 0 || row >= h->batch) B200_FAIL(B200_ERR_INVALID, "lm_session_import: row %d outside [0, %d)", row, h->batch);
+  if (!src_dev) B200_FAIL(B200_ERR_INVALID, "lm_session_import: null record");
+  if (nbytes < (int64_t)sizeof(SessionHeader)) B200_FAIL(B200_ERR_SHAPE, "lm_session_import: %lld bytes hold no record header", (long long)nbytes);
+  SessionHeader s;
+  B200_CUDA(cudaStreamSynchronize(h->stream));
+  B200_CUDA(cudaMemcpy(&s, src_dev, sizeof(s), cudaMemcpyDeviceToHost));
+  if (s.magic != SESSION_MAGIC || s.version != SESSION_VERSION)
+    B200_FAIL(B200_ERR_INVALID, "lm_session_import: not a session record (magic %08x, version %u)", s.magic, s.version);
+  if (s.kind != SESSION_LM) B200_FAIL(B200_ERR_INVALID, "lm_session_import: the record is not an LM session (kind %u)", s.kind);
+  if (s.fingerprint != lm_fingerprint(h)) B200_FAIL(B200_ERR_INVALID, "lm_session_import: the record was taken with another model configuration");
+  if (s.kv_dtype != (uint32_t)h->kv_fp8)
+    B200_FAIL(B200_ERR_INVALID, "lm_session_import: the record's KV storage type %u differs from the handle's %d", s.kv_dtype, h->kv_fp8);
+  SessionPlan p;
+  p.rows = h->MB / h->batch;
+  if (s.rows != p.rows || ((s.flags & SESSION_CFG_UNTIL) != 0) != (h->cfg_until != nullptr))
+    B200_FAIL(B200_ERR_INVALID, "lm_session_import: classifier-free guidance (or cfg_is_masked_until) on one side only");
+  p.cond = (s.flags & SESSION_COND) != 0;
+  if (p.cond != (h->cond_on != 0)) B200_FAIL(B200_ERR_INVALID, "lm_session_import: condition_sum on one side only");
+  p.pos[0] = s.pos[0]; p.pos[1] = p.rows > 1 ? s.pos[1] : 0;
+  const int64_t top = std::max(p.pos[0], p.pos[1]);
+  if (p.pos[0] < 0 || p.pos[1] < 0 || s.n != std::min<int64_t>(top, c.context))
+    B200_FAIL(B200_ERR_INVALID, "lm_session_import: corrupt record (positions %lld / %lld, %lld slots)", (long long)p.pos[0],
+              (long long)p.pos[1], (long long)s.n);
+  p.n = s.n;
+  session_size(h, &p);
+  if (s.bytes != p.bytes || nbytes != p.bytes)
+    B200_FAIL(B200_ERR_SHAPE, "lm_session_import: the record takes %lld bytes, header says %lld, caller passed %lld", (long long)p.bytes,
+              (long long)s.bytes, (long long)nbytes);
+  const int cap = ring_cap(h);
+  if (cap < c.context && top > cap)
+    B200_FAIL(B200_ERR_STATE, "lm_session_import: the session is at position %lld, the %d-slot KV ring cannot hold its history",
+              (long long)top, cap);
+  if (h->n_pages) B200_TRY(session_map(h, row, p));
+  char* rec = const_cast<char*>(static_cast<const char*>(src_dev));
+  B200_TRY(row_slice_copy(h->slices_dev, p.cond ? h->n_slices_cond : h->n_slices, h->slices_max, rec, row, false, h->stream));
+  B200_TRY(session_kv(h, row, p, rec, false));
+  B200_CUDA(cudaStreamSynchronize(h->stream));
   return B200_OK;
 }
 

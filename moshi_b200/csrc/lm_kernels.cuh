@@ -872,27 +872,40 @@ static __global__ void __launch_bounds__(KV_PAGE_THREADS) kv_page_free_kernel(in
   if (r == 0) *top = t0 + total;
 }
 
-// Streaming-state view of a paged layer as the contiguous ring [MB][H][cap][ATT_D]: GATHER reads the pool (slots at or past the
-// row's fill min(pos, cap), and unmapped or sink pages, read as zeros); otherwise the fill's slots are scattered into the pool.
-template <bool GATHER>
-static __global__ void kv_page_copy_kernel(bf16* __restrict__ pool, bf16* __restrict__ ring, const int* __restrict__ table,
-                                           const long long* __restrict__ pos, int H, int cap, int tab_ld, int page_shift, int sink,
-                                           long long n_vec) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;   // one 16-byte vector of 8 elements
-  if (i >= n_vec) return;
-  constexpr int V = ATT_D / 8;
-  const int c = (int)(i % V);
-  const long long rs = i / V;
-  const int s = (int)(rs % cap);
-  const long long bh = rs / cap;
-  const int b = (int)(bh / H), h = (int)(bh % H);
-  const int pg = table[(long long)b * tab_ld + (s >> page_shift)];
-  const bool valid = s < min(pos[b], (long long)cap) && pg >= 0 && pg < sink;
-  uint4* rv = reinterpret_cast<uint4*>(ring) + i;
-  uint4* pv = reinterpret_cast<uint4*>(pool) +
-              ((((long long)pg * H + h) << page_shift) + (s & ((1 << page_shift) - 1))) * V + c;
-  if (GATHER) *rv = valid ? *pv : make_uint4(0, 0, 0, 0);
-  else if (valid) *pv = *rv;
+// Temporal K/V rings <-> a flat buffer [array][k][H][n][slot] for model rows b = row0 + k * row_step, k < n_rows: the streaming
+// state's view of a paged layer (one array, every row, n = cap) and a session record (every layer's K and V, the session's 1 or
+// 2 rows, n = its fill).  `arrays` are the rings [MB][H][cap][slot] or, with a page table, the pools [n_pages + 1][H][page][slot].
+// A slot is valid below the row's fill min(pos, cap) on a mapped, non-sink page: GATHER writes zeros for the others, the scatter
+// leaves them alone.  blockIdx.y = (array, k, head); V units of type U per slot.
+struct KvCopy {
+  void* const* arrays;
+  void* flat;
+  const int* table;            // [MB][tab_ld], or nullptr: contiguous rings
+  const long long* pos;
+  int tab_ld, page_shift, sink;
+  int row0, n_rows, row_step, H, cap, n;
+};
+template <bool GATHER, typename U, int V>
+static __global__ void kv_copy_kernel(KvCopy a) {
+  const int seg = blockIdx.y;
+  const int h = seg % a.H, k = (seg / a.H) % a.n_rows, arr = seg / (a.H * a.n_rows);
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= a.n * V) return;
+  const int s = i / V, c = i - s * V;
+  const int b = a.row0 + k * a.row_step;
+  bool valid = s < min(a.pos[b], (long long)a.cap);
+  long long r;
+  if (a.table != nullptr) {
+    const int pg = a.table[(long long)b * a.tab_ld + (s >> a.page_shift)];
+    valid = valid && pg >= 0 && pg < a.sink;
+    r = ((((long long)pg * a.H + h) << a.page_shift) + (s & ((1 << a.page_shift) - 1))) * V + c;
+  } else {
+    r = (((long long)b * a.H + h) * a.cap + s) * V + c;
+  }
+  U* ring = static_cast<U*>(a.arrays[arr]);
+  U* fv = static_cast<U*>(a.flat) + (long long)seg * a.n * V + i;
+  if (GATHER) *fv = valid ? ring[r] : U{};
+  else if (valid) ring[r] = *fv;
 }
 
 static __global__ void advance_pos_kernel(long long* pos, const uint8_t* exec_mask, int B) {

@@ -114,6 +114,10 @@ struct b200_mimi {
   float* tap_scratch = nullptr; size_t tap_scratch_n = 0;
   std::map<std::string, Tap> taps;
   int64_t weight_bytes = 0;
+  // session records: the [B]-leading slice of every marked state entry, in marking order
+  RowSlice* slices_dev = nullptr;
+  int n_slices = 0;
+  long long session_bytes = 0, slices_max = 0;
 };
 
 namespace {
@@ -953,6 +957,16 @@ int b200_mimi_streaming_begin(b200_mimi* h, int batch, void* stream) {
       A.mark_state(L.vc, (size_t)B * H * c.tr_context * D * 4, p + ".v", B200_F32, {B, H, c.tr_context, D});
     }
   }
+  {
+    std::vector<RowSlice> s;
+    for (auto& e : A.snap) s.push_back({static_cast<char*>(e.ptr), (long long)(e.bytes / B), 0, 0});
+    h->session_bytes = layout_row_slices(s, sizeof(SessionHeader));
+    h->slices_max = 0;
+    for (auto& e : s) h->slices_max = std::max(h->slices_max, e.row_bytes);
+    h->n_slices = (int)s.size();
+    B200_TRY(A.alloc_t(&h->slices_dev, s.size(), false));
+    B200_CUDA(cudaMemcpy(h->slices_dev, s.data(), s.size() * sizeof(RowSlice), cudaMemcpyHostToDevice));
+  }
   B200_TRY(ensure_rvq_workspace(h, B));
   B200_CUDA(cudaDeviceSynchronize());
   cleanup.armed = false;
@@ -1096,6 +1110,55 @@ int b200_mimi_set_state(b200_mimi* h, const void* src_dev, int64_t nbytes) {
     B200_FAIL(B200_ERR_SHAPE, "mimi_set_state: snapshot of %lld bytes does not fit this session layout (%lld)",
               (long long)nbytes, (long long)h->state.state_bytes());
   return h->state.load(src_dev, h->stream);
+}
+
+/* One session as a record: the 256-byte SessionHeader, then row `row` of every marked state entry in marking order, each
+ * 16-byte aligned.  The size depends on the configuration only. */
+int b200_mimi_session_bytes(b200_mimi* h, int64_t* nbytes) {
+  B200_TRY(ensure_streaming(h, "mimi_session_bytes"));
+  if (nbytes) *nbytes = h->session_bytes;
+  return B200_OK;
+}
+
+int b200_mimi_session_export(b200_mimi* h, int row, void* dst_dev, int64_t capacity) {
+  B200_TRY(ensure_streaming(h, "mimi_session_export"));
+  DeviceGuard g(h->device);
+  if (row < 0 || row >= h->batch) B200_FAIL(B200_ERR_INVALID, "mimi_session_export: row %d outside [0, %d)", row, h->batch);
+  if (!dst_dev) B200_FAIL(B200_ERR_INVALID, "mimi_session_export: null destination");
+  if (capacity < h->session_bytes)
+    B200_FAIL(B200_ERR_SHAPE, "mimi_session_export: the record takes %lld bytes, capacity %lld", h->session_bytes, (long long)capacity);
+  SessionHeader s;
+  memset(&s, 0, sizeof(s));
+  s.magic = SESSION_MAGIC; s.version = SESSION_VERSION; s.kind = SESSION_MIMI;
+  s.fingerprint = config_fingerprint(&h->cfg, sizeof(h->cfg)); s.rows = 1; s.bytes = h->session_bytes;
+  char* rec = static_cast<char*>(dst_dev);
+  B200_CUDA(cudaMemcpyAsync(rec, &s, sizeof(s), cudaMemcpyHostToDevice, h->stream));
+  B200_TRY(row_slice_copy(h->slices_dev, h->n_slices, h->slices_max, rec, row, true, h->stream));
+  B200_CUDA(cudaStreamSynchronize(h->stream));
+  return B200_OK;
+}
+
+int b200_mimi_session_import(b200_mimi* h, int row, const void* src_dev, int64_t nbytes) {
+  B200_TRY(ensure_streaming(h, "mimi_session_import"));
+  DeviceGuard g(h->device);
+  if (row < 0 || row >= h->batch) B200_FAIL(B200_ERR_INVALID, "mimi_session_import: row %d outside [0, %d)", row, h->batch);
+  if (!src_dev) B200_FAIL(B200_ERR_INVALID, "mimi_session_import: null record");
+  if (nbytes < (int64_t)sizeof(SessionHeader)) B200_FAIL(B200_ERR_SHAPE, "mimi_session_import: %lld bytes hold no record header", (long long)nbytes);
+  SessionHeader s;
+  B200_CUDA(cudaStreamSynchronize(h->stream));
+  B200_CUDA(cudaMemcpy(&s, src_dev, sizeof(s), cudaMemcpyDeviceToHost));
+  if (s.magic != SESSION_MAGIC || s.version != SESSION_VERSION)
+    B200_FAIL(B200_ERR_INVALID, "mimi_session_import: not a session record (magic %08x, version %u)", s.magic, s.version);
+  if (s.kind != SESSION_MIMI) B200_FAIL(B200_ERR_INVALID, "mimi_session_import: the record is not a Mimi session (kind %u)", s.kind);
+  if (s.fingerprint != config_fingerprint(&h->cfg, sizeof(h->cfg)))
+    B200_FAIL(B200_ERR_INVALID, "mimi_session_import: the record was taken with another codec configuration");
+  if (s.bytes != h->session_bytes || nbytes != h->session_bytes)
+    B200_FAIL(B200_ERR_SHAPE, "mimi_session_import: the record takes %lld bytes, header says %lld, caller passed %lld", h->session_bytes,
+              (long long)s.bytes, (long long)nbytes);
+  B200_TRY(row_slice_copy(h->slices_dev, h->n_slices, h->slices_max, const_cast<char*>(static_cast<const char*>(src_dev)), row, false,
+                          h->stream));
+  B200_CUDA(cudaStreamSynchronize(h->stream));
+  return B200_OK;
 }
 
 int b200_mimi_set_graph(b200_mimi* h, int enable) {

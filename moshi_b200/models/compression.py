@@ -168,6 +168,25 @@ class MimiModel:
         m = self._mask(exec_mask)
         _lib.check(self._lib.b200_mimi_set_exec_mask(self._h, _lib.ptr(m)))
 
+    # ---- one session ----------------------------------------------------------------------------------
+    def export_session(self, row: int) -> torch.Tensor:
+        """Encoder and decoder state of session ``row`` as a uint8 record on the model's device (``b200_mimi_session_export``,
+        fixed size per configuration).  The row is not changed."""
+        assert self._batch is not None, "mimi is not streaming"
+        n = C.c_int64()
+        _lib.check(self._lib.b200_mimi_session_bytes(self._h, C.byref(n)))
+        rec = torch.empty(n.value, dtype=torch.uint8, device=self.device)
+        _lib.check(self._lib.b200_mimi_session_export(self._h, int(row), _lib.ptr(rec), n.value))
+        return rec
+
+    def import_session(self, row: int, record: torch.Tensor) -> None:
+        """Replaces session ``row`` with a record of ``export_session`` from a handle of the same configuration, on any device.
+        Nothing changes if it is refused (ValueError for an incompatible record or row)."""
+        assert self._batch is not None, "mimi is not streaming"
+        rec = record.to(self.device).contiguous()
+        assert rec.dtype == torch.uint8 and rec.dim() == 1, "a session record is a 1-d uint8 tensor"
+        _lib.check(self._lib.b200_mimi_session_import(self._h, int(row), _lib.ptr(rec), rec.numel()))
+
     # ---- streaming state ------------------------------------------------------------------------------
     def _state_entries(self) -> list[tuple[str, torch.dtype, tuple[int, ...], int]]:
         from .lm import _TORCH_DTYPES

@@ -373,6 +373,31 @@ class LMGen:
         if state:
             raise RuntimeError(f"Some states were not consumed: {list(state.keys())}")
 
+    # ---- one session -----------------------------------------------------------------------------
+    def export_session(self, row: int) -> torch.Tensor:
+        """Session ``row`` as a uint8 record on the model's device (``b200_lm_session_export``): its token ring, offsets,
+        positions and the temporal K/V of its live fill, so the size follows the fill.  The row is not changed and keeps
+        running; reset it once the session has moved.  A short-ring row past ``kv_capacity`` raises (its history is lost)."""
+        assert self._batch is not None, "lm_gen is not streaming"
+        n = C.c_int64()
+        with self._device():
+            self._sync_stream()
+            _lib.check(self._lib.b200_lm_session_bytes(self._h, int(row), C.byref(n)))
+            rec = torch.empty(n.value, dtype=torch.uint8, device=self.lm_model.device)
+            _lib.check(self._lib.b200_lm_session_export(self._h, int(row), _lib.ptr(rec), n.value))
+        return rec
+
+    def import_session(self, row: int, record: torch.Tensor) -> None:
+        """Replaces session ``row`` with a record of ``export_session`` from any handle of the same model configuration and
+        KV storage type, on any device (``.to(device)`` copies it across GPUs).  Nothing changes if it is refused: ValueError
+        for an incompatible record or row, ``B200Error`` when the ring or the pool cannot hold the session's history."""
+        assert self._batch is not None, "lm_gen is not streaming"
+        rec = record.to(self.lm_model.device).contiguous()
+        assert rec.dtype == torch.uint8 and rec.dim() == 1, "a session record is a 1-d uint8 tensor"
+        with self._device():
+            self._sync_stream()
+            _lib.check(self._lib.b200_lm_session_import(self._h, int(row), _lib.ptr(rec), rec.numel()))
+
     # ---- sampling noise --------------------------------------------------------------------------
     def draw_noise(self) -> torch.Tensor | None:
         """Exp(1) draws of one step in the reference's order (lm.py:736 then lm.py:836 x dep_q), each

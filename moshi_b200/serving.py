@@ -9,6 +9,7 @@ process per GPU and to reduce timings / counts in the benchmark.
 from __future__ import annotations
 
 import os
+import typing as tp
 
 import torch
 
@@ -67,6 +68,12 @@ def barrier() -> None:
 NODATA, ACTIVE, RESET = 0, -1, -2      # UpdateFlags of rust/moshi-server/batched_asr.py:23-30
 
 
+class SessionRecord(tp.NamedTuple):
+    """One dialogue session of a ``DialogueService``: its LM and Mimi records (uint8 device tensors)."""
+    lm: torch.Tensor
+    mimi: torch.Tensor
+
+
 class DialogueService:
     """Batched full-duplex frame step with the calling convention of ``ASRService.step``
     (``rust/moshi-server/batched_asr.py:100-215``, bound by ``py_basr_module.rs``): numpy host buffers in and
@@ -118,6 +125,19 @@ class DialogueService:
         if mask.any():
             self.lm_gen.reset_streaming(mask)
             self.mimi.reset_streaming(mask)
+
+    def export_session(self, slot: int) -> "SessionRecord":
+        """The LM and Mimi state of session ``slot`` as device records (``LMGen.export_session``, ``MimiModel.export_session``).
+        The slot is not changed; once the session has moved, call ``release([slot])`` so that a paged LM gets its pages back."""
+        return SessionRecord(self.lm_gen.export_session(slot), self.mimi.export_session(slot))
+
+    def import_session(self, slot: int, record: "SessionRecord") -> None:
+        """Continues a session exported from another service (same models, KV storage type; any GPU) in ``slot``.  The next
+        ``step``'s update for the slot must be ``ACTIVE``: ``RESET`` would erase the imported session.  The source calls
+        ``release([slot])`` on its own slot to return its pages.  PCM still buffered in a ``SessionPool`` is the caller's to carry.
+        The LM record is checked and imported first: if it is refused, nothing changes."""
+        self.lm_gen.import_session(slot, record.lm)
+        self.mimi.import_session(slot, record.mimi)
 
     def close(self) -> None:
         if getattr(self, "_h", None):
