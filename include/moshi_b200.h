@@ -434,12 +434,24 @@ int b200_op_attn_step(const void* qkv_dev, void* k_dev, void* v_dev, void* out_d
 int b200_op_attn_step_paged(const void* qkv_dev, void* k_pool_dev, void* v_pool_dev, const int32_t* page_table_dev, void* out_dev,
                             const int64_t* pos_dev, const uint8_t* exec_mask_dev, int B, int H, int cap, int page_slots, int nsplit,
                             float max_period, void* stream);
-/* sample_token (sampling.py:86-106): logits bf16 [B,card], noise f32 [B,min(k,card)] -> i64 [B]. */
 /* The same step over an opt-in 8-bit ring (b200_lm_set_kv_dtype): k8 / v8 u8 [B,H,cap,128] (e4m3 bytes, or
- * round(x * 127 / absmax) + 128), ks / vs f32 [B,H,cap] = absmax / 448 (or / 127) of the row. */
+ * round(x * 127 / absmax) + 128), ks / vs f32 [B,H,cap] = absmax / 448 (or / 127) of the row.  The q.k products are summed
+ * in fp16 four at a time: queries are supported up to |q| = 256 per element (see lm_kernels.cuh). */
 int b200_op_attn_step_q8(const void* qkv_dev, void* k8_dev, void* v8_dev, float* ks_dev, float* vs_dev, void* out_dev,
                          const int64_t* pos_dev, const uint8_t* exec_mask_dev, int B, int H, int cap, int nsplit, float max_period,
                          int kv_dtype, void* stream);
+/* One depformer attention sub-step, as the LM launches it: qkv bf16 [B,3*H*64] (rows q|k|v), the new k / v written to slot
+ * `step` of the per-frame caches [B,H,cap,64], attention over slots 0..step with scale 1/8 and no positional embedding,
+ * out bf16 [B,H*64].  cap <= 16, step < cap. */
+int b200_op_dep_attn_step(const void* qkv_dev, void* k_dev, void* v_dev, void* out_dev, int B, int H, int cap, int step, void* stream);
+/* RMSNorm of the LM (transformer.py:45-58, eps 1e-8): y = bf16(x * alpha * rsqrt(eps + mean(x^2))), x / y bf16 [M,dim],
+ * alpha bf16 [dim], dim even. */
+int b200_op_rmsnorm(const void* x_dev, const void* alpha_dev, void* y_dev, int M, int dim, void* stream);
+/* b200_op_linear_sk on rmsnorm(x, alpha) with the norm folded into the GEMV kernel's activation staging (the LM's path for one
+ * or two sessions).  Only the GEMV path takes a norm: for M above b200_op_set_gemv_max_rows it returns B200_ERR_STATE. */
+int b200_op_linear_sk_norm(const void* x_dev, const void* alpha_dev, const void* w_tiles_dev, void* y_dev, const void* res_dev, int M,
+                           int N, int K, int epi, int gate_rows, void* stream);
+/* sample_token (sampling.py:86-106): logits bf16 [B,card], noise f32 [B,min(k,card)] -> i64 [B]. */
 int b200_op_sample(const void* logits_bf16_dev, const float* noise_dev, int64_t* out_dev, int B,
                    int card, int use_sampling, float temp, int top_k, void* stream);
 

@@ -483,6 +483,9 @@ static void (*const attn_step_paged_kernel)(const AttnStep) = attn_step_kernel<4
 // even.  Attention: a half-warp owns one key (16 lanes x 8 bytes); keys and values are decoded to packed fp16 (exact),
 // the dot product and the per-group weighted value sums run as HFMA2, and everything that accumulates over the ring
 // (softmax statistics, output accumulator) stays fp32; the online softmax is updated once per group of keys.
+// Supported query range: |q| <= 256 per element of the rotated query.  Each fp16 lane partial sums four products
+// (q / sqrt(128)) * key byte value, at most 4 * 22.6 * 448 = 40 544 for e4m3 (int8: 11 494) against the fp16 limit 65 504, so a
+// query lined up with its key overflows to inf (and the row's output to NaN) only past |q| ~ 413 (e4m3) / ~1460 (int8).
 // ---------------------------------------------------------------------------------------------
 constexpr int KV_E4M3 = 1, KV_INT8 = 2;       // = B200_KV_FP8_E4M3, B200_KV_INT8
 

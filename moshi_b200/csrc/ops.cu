@@ -105,7 +105,34 @@ int b200_op_linear_ns(const void* x_dev, const void* w_tiles_dev, void* y_dev, c
                        static_cast<cudaStream_t>(stream), unit_tiles);
 }
 
+// y = epi(rmsnorm(x, alpha) . W^T) with the norm folded into the GEMV's activation staging (norm_linear at one or two
+// sessions); every other path refuses a norm input with B200_ERR_STATE
+int b200_op_linear_sk_norm(const void* x_dev, const void* alpha_dev, const void* w_tiles_dev, void* y_dev, const void* res_dev, int M,
+                           int N, int K, int epi, int gate_rows, void* stream) {
+  if (!x_dev || !alpha_dev || !w_tiles_dev || !y_dev) B200_FAIL(B200_ERR_INVALID, "op_linear_sk_norm: null pointer");
+  if (!tc::sk_supported(M, N, K, epi)) B200_FAIL(B200_ERR_SHAPE, "op_linear_sk_norm: unsupported shape");
+  static tc::GemmPlanCache cache;
+  float* ws = nullptr; int* counters = nullptr;
+  B200_TRY(sk_scratch(&ws, &counters));
+  tc::SkTuning t;
+  t.norm_alpha = static_cast<const __nv_bfloat16*>(alpha_dev);
+  const int out_cols = epi == 2 ? gate_rows : N;
+  return tc::sk_linear(cache, static_cast<const __nv_bfloat16*>(x_dev), K, w_tiles_dev, static_cast<__nv_bfloat16*>(y_dev),
+                       out_cols, static_cast<const __nv_bfloat16*>(res_dev), out_cols, M, N, K, epi, gate_rows, ws, counters, t,
+                       static_cast<cudaStream_t>(stream));
+}
+
 int b200_op_set_gemv_max_rows(int max_rows) { return tc::sk_set_gemv_max_m(max_rows); }
+
+// rmsnorm_kernel as the LM launches it (lm.cu norm_linear and the output norm): one 256-thread CTA per row, eps 1e-8
+int b200_op_rmsnorm(const void* x_dev, const void* alpha_dev, void* y_dev, int M, int dim, void* stream) {
+  using namespace b200::lm;
+  if (!x_dev || !alpha_dev || !y_dev) B200_FAIL(B200_ERR_INVALID, "op_rmsnorm: null pointer");
+  if (M < 1 || dim < 2 || dim % 2) B200_FAIL(B200_ERR_SHAPE, "op_rmsnorm: bad shape M=%d dim=%d", M, dim);
+  B200_LAUNCH(rmsnorm_kernel, M, 256, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(x_dev),
+              static_cast<const bf16*>(alpha_dev), static_cast<bf16*>(y_dev), dim, 1e-8f);
+  return check_launch("op_rmsnorm");
+}
 
 int64_t b200_op_packed_bytes_i8(int N, int K, int epi, int gate_rows) { return (int64_t)tc::sk_packed_bytes_i8(N, K, epi, gate_rows); }
 
@@ -200,6 +227,18 @@ int b200_op_attn_step_q8(const void* qkv_dev, void* k8_dev, void* v8_dev, float*
   if (kv_dtype == B200_KV_INT8) B200_LAUNCH(attn_step_q8_kernel<KV_INT8>, grid, ATT_THREADS, 0, st, a);
   else B200_LAUNCH(attn_step_q8_kernel<KV_E4M3>, grid, ATT_THREADS, 0, st, a);
   return check_launch("op_attn_step_q8");
+}
+
+// dep_attn_step_kernel with the LM's launch shape (lm.cu, depformer layers): one warp per (b, h), 128 threads per CTA
+int b200_op_dep_attn_step(const void* qkv_dev, void* k_dev, void* v_dev, void* out_dev, int B, int H, int cap, int step, void* stream) {
+  using namespace b200::lm;
+  if (!qkv_dev || !k_dev || !v_dev || !out_dev) B200_FAIL(B200_ERR_INVALID, "op_dep_attn_step: null pointer");
+  if (B < 1 || H < 1 || cap < 1 || cap > DEP_MAX_Q || step < 0 || step >= cap)
+    B200_FAIL(B200_ERR_SHAPE, "op_dep_attn_step: B=%d H=%d cap=%d step=%d (cap <= %d, step < cap)", B, H, cap, step, DEP_MAX_Q);
+  B200_LAUNCH(dep_attn_step_kernel, ceil_div(B * H * 32, 128), 128, 0, static_cast<cudaStream_t>(stream),
+              static_cast<const bf16*>(qkv_dev), static_cast<bf16*>(k_dev), static_cast<bf16*>(v_dev), static_cast<bf16*>(out_dev), B, H, cap,
+              step);
+  return check_launch("op_dep_attn_step");
 }
 
 }  // extern "C"

@@ -1,12 +1,12 @@
 """GPU: kernel-level parity through the C ABI (the same kernels the handles launch)."""
 import ctypes as C
-import math
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-from tests.util import cptr, stats
+from tests.util import (ATTN_C, ATTN_REL, attn_err_ratio, attn_ref64, attn_scenario, cptr, dep_scenario, rmsnorm_ref64, rmsnorm_verdict,
+                        stats)
 
 pytestmark = pytest.mark.gpu
 
@@ -88,58 +88,181 @@ def test_streaming_conv1d_exec_mask_freezes_state(lib):
     assert torch.equal(prev[0], x[0, :, -2:])
 
 
-def _rope_ref(x: torch.Tensor, pos: torch.Tensor, max_period: float = 10000.0) -> torch.Tensor:
-    """rope.py:45-82 on [B, H, D] bf16 for one time step at per-row position ``pos``: interleaved pairs, fp32, -> bf16."""
-    B, H, D = x.shape
-    xf = x.float().view(B, H, D // 2, 2)
-    freqs = torch.exp(torch.arange(D // 2, dtype=torch.float32) * (-math.log(max_period) * 2 / D))
-    theta = freqs[None, :] * pos.float()[:, None]
-    c, s_ = torch.cos(theta)[:, None, :], torch.sin(theta)[:, None, :]
-    xr, xi = xf[..., 0], xf[..., 1]
-    return torch.stack([xr * c - xi * s_, xr * s_ + xi * c], dim=-1).view(B, H, D).bfloat16()
-
-
-@pytest.mark.parametrize("B,H,cap,nsplit", [(1, 32, 3000, 0), (5, 4, 3000, 1), (3, 2, 12, 0), (7, 8, 250, 3), (2, 32, 3000, 16)])
-def test_fused_attention_step(lib, B, H, cap, nsplit):
-    """The LM's one-launch attention step == RoPE + ring append + masked SDPA of the reference
-    (transformer.py:557-597, 247-286), including a paused row and wrapped rings."""
+def _attn_launch(lib, sc: dict, k, v, nsplit: int) -> torch.Tensor:
     from moshi_b200 import _lib
-    g = torch.Generator().manual_seed(B * 131 + cap)
-    C = H * 128
-    qkv = torch.randn(B, 3 * C, generator=g).bfloat16()
-    k = torch.randn(B, H, cap, 128, generator=g).bfloat16()
-    v = torch.randn(B, H, cap, 128, generator=g).bfloat16()
-    pos = torch.tensor([0, 1, cap - 1, cap, 3 * cap + 5, 17, cap // 2][:B], dtype=torch.int64)
-    mask = torch.ones(B, dtype=torch.bool)
-    if B > 1:
-        mask[1] = False                      # a paused row: no append, attends over the keys it already has
-    q_in, k_in, v_in = (qkv[:, i * C:(i + 1) * C].reshape(B, H, 128) for i in range(3))
-    q_rot, k_rot = _rope_ref(q_in, pos), _rope_ref(k_in, pos)
-    k_ref, v_ref = k.clone(), v.clone()
-    for b in range(B):
-        if mask[b]:
-            k_ref[b, :, pos[b] % cap] = k_rot[b]
-            v_ref[b, :, pos[b] % cap] = v_in[b]
-    n_valid = (pos + mask.long()).clamp(max=cap)
-    allowed = torch.arange(cap)[None, :] < n_valid[:, None]
-    want = F.scaled_dot_product_attention(q_rot.float()[:, :, None], k_ref.float(), v_ref.float(),
-                                          allowed[:, None, None, :])[:, :, 0].reshape(B, C)
-    kd, vd, out = k.cuda(), v.cuda(), torch.empty(B, C, dtype=torch.bfloat16, device="cuda")
-    qd, pd, md = qkv.cuda(), pos.cuda(), mask.cuda()
-    _lib.check(lib.b200_op_attn_step(cptr(qd), cptr(kd), cptr(vd), cptr(out), cptr(pd), cptr(md), B, H, cap, nsplit,
+    out = torch.full((sc["B"], sc["H"] * 128), float("nan"), dtype=torch.bfloat16, device="cuda")
+    qd, pd, md = sc["qkv"].cuda(), sc["pos"].cuda(), sc["mask"].cuda()
+    _lib.check(lib.b200_op_attn_step(cptr(qd), cptr(k), cptr(v), cptr(out), cptr(pd), cptr(md), sc["B"], sc["H"], sc["cap"], nsplit,
                                      10000.0, _stream()))
     torch.cuda.synchronize()
-    rows = n_valid > 0                       # a paused row with an empty ring has nothing to attend to
-    print(stats(f"attn step B={B} H={H} cap={cap} nsplit={nsplit}", out[rows.cuda()], want[rows]))
-    torch.testing.assert_close(out.float().cpu()[rows], want[rows], rtol=2e-2, atol=2e-2)
-    # ring contents: the appended key is the rotated k (one bf16 ulp of slack for sincos), untouched slots are identical
-    torch.testing.assert_close(kd.cpu().float(), k_ref.float(), rtol=0, atol=4e-2)
+    return out
+
+
+def _check_attn_step(lib, sc: dict, nsplit: int, label: str) -> None:
+    """One step of the kernel on a scenario of tests.util.attn_scenario: outputs against attn_ref64, the ring it leaves behind
+    against the reference ring."""
+    kd, vd = sc["k"].cuda(), sc["v"].cuda()
+    out = _attn_launch(lib, sc, kd, vd, nsplit)
+    k_got, v_got = kd.cpu(), vd.cpu()
+    # the reference attends over the key the kernel appended (checked below against the fp32-RoPE key on its own)
+    want = attn_ref64(sc["q_rot"], k_got, sc["v_ref"], sc["n_valid"])
+    ratio = attn_err_ratio(out, want)
+    print(f"{label}: B={sc['B']} nsplit={sc['nsplit']}: worst |err| / tolerance {ratio:.3f} "
+          f"(tolerance {ATTN_REL:.3g} |want| + {ATTN_C:.3g} rms)")
+    assert torch.isfinite(out.float()).all()
+    assert ratio <= 1.0
+    # ring contents: untouched slots keep their bits (NaN poison included), values are appended bit for bit
+    B, H, cap = sc["B"], sc["H"], sc["cap"]
     same = torch.ones(B, cap, dtype=torch.bool)
     for b in range(B):
-        if mask[b]:
-            same[b, pos[b] % cap] = False
-    assert torch.equal(kd.cpu()[same[:, None].expand(B, H, cap)], k[same[:, None].expand(B, H, cap)])
-    assert torch.equal(vd.cpu(), v_ref)
+        if sc["mask"][b]:
+            same[b, int(sc["pos"][b]) % cap] = False
+    keep = same[:, None].expand(B, H, cap)
+    assert torch.equal(k_got.view(torch.int16)[keep], sc["k"].view(torch.int16)[keep])
+    assert torch.equal(v_got.view(torch.int16), sc["v_ref"].view(torch.int16))
+    # the appended key: the fp32-RoPE reference within one bf16 ulp of the head's largest element (an angle that differs in
+    # the last bits of fp32 moves small elements by more than their own ulp), on >= 99 % of the elements exactly
+    new = ~keep
+    got_k = k_got.permute(0, 2, 1, 3)[new.permute(0, 2, 1)].float()
+    want_k = sc["k_ref"].permute(0, 2, 1, 3)[new.permute(0, 2, 1)].float()
+    top = want_k.abs().amax(-1, keepdim=True)
+    ulp = 2.0 ** (torch.floor(torch.log2(top)) - 7)
+    assert ((got_k - want_k).abs() <= ulp).all(), ((got_k - want_k).abs() / ulp).max()
+    assert (got_k == want_k).float().mean() >= 0.99, (got_k == want_k).float().mean()
+
+
+@pytest.mark.parametrize("nsplit", [1, 2, 3, 5, 16, 0])
+@pytest.mark.parametrize("cap", [3000, 250, 12])
+@pytest.mark.parametrize("H", [32, 20, 2])
+def test_fused_attention_step(lib, H, cap, nsplit):
+    """The LM's one-launch attention step == RoPE + ring append + attention over the valid slots (transformer.py:557-597,
+    247-286) in fp64, on the rows of tests.util.attn_scenario: fills at the group / loop-step / split edges, wrapped rings
+    (one hour at 12.5 Hz), paused rows, needles on every split edge and on the key the step overwrites,
+    NaN poison past the fill.  nsplit 0 is the LM's own choice."""
+    _check_attn_step(lib, attn_scenario(H, cap, nsplit), nsplit, f"attn step H={H} cap={cap}")
+
+
+@pytest.mark.parametrize("H,cap,nsplit,qk_scale,v_scale", [(20, 250, 5, 16.0, 1.0), (2, 12, 3, 16.0, 1.0)] + [
+    (H, cap, ns, qk, v) for H, cap, ns in [(32, 3000, 0), (32, 3000, 16), (20, 250, 5)] for qk, v in [(1e-3, 1.0), (1.0, 1e3)]])
+def test_fused_attention_step_magnitudes(lib, H, cap, nsplit, qk_scale, v_scale):
+    """q and k x16 (the softmax is nearly one-hot), x1e-3 (nearly uniform), v x1e3; no needles, so every key counts.
+    x16 stays at short rings: there one bf16 ulp of a rotated query element, which the kernel's fp32 RoPE and the host's
+    round differently now and then, moves a score by ~0.1, and among 3000 keys two of them are that close."""
+    sc = attn_scenario(H, cap, nsplit, qk_scale=qk_scale, v_scale=v_scale, needles=False, seed=1)
+    _check_attn_step(lib, sc, nsplit, f"attn step H={H} cap={cap} q,k x{qk_scale:g} v x{v_scale:g}")
+
+
+@pytest.mark.parametrize("H", [16, 2])
+@pytest.mark.parametrize("B", [1, 3, 80])
+@pytest.mark.parametrize("dep_q", [8, 16])
+def test_depformer_attention_step(lib, B, H, dep_q):
+    """dep_attn_step_kernel through sub-steps 0..dep_q - 1 of one frame: the new k / v land in row `step` of the cache bit for
+    bit, the query attends over rows 0..step (fp64 reference, needles on key 0 and key `step`), and the NaN poison of the
+    rows after `step` is neither read nor changed."""
+    from moshi_b200 import _lib
+    sc = dep_scenario(B, H, dep_q)
+    D, C = 64, H * 64
+    kc = torch.full((B, H, dep_q, D), float("nan"), dtype=torch.bfloat16, device="cuda")
+    vc = torch.full_like(kc, float("nan"))
+    qkv = sc["qkv"].cuda()
+    worst = 0.0
+    for s in range(dep_q):
+        out = torch.full((B, C), float("nan"), dtype=torch.bfloat16, device="cuda")
+        _lib.check(lib.b200_op_dep_attn_step(cptr(qkv[s]), cptr(kc), cptr(vc), cptr(out), B, H, dep_q, s, _stream()))
+        torch.cuda.synchronize()
+        assert torch.isfinite(out.float()).all(), s
+        r = attn_err_ratio(out, sc["want"][s])
+        worst = max(worst, r)
+        assert r <= 1.0, (s, r)
+        k_got, v_got = kc.cpu(), vc.cpu()
+        assert torch.equal(k_got[:, :, :s + 1].view(torch.int16), sc["k"][:, :, :s + 1].view(torch.int16)), s
+        assert torch.equal(v_got[:, :, :s + 1].view(torch.int16), sc["v"][:, :, :s + 1].view(torch.int16)), s
+        assert torch.isnan(k_got[:, :, s + 1:].float()).all() and torch.isnan(v_got[:, :, s + 1:].float()).all(), s
+    print(f"dep attn B={B} H={H} dep_q={dep_q}: worst |err| / tolerance {worst:.3f}")
+    assert lib.b200_op_dep_attn_step(cptr(qkv[0]), cptr(kc), cptr(vc), cptr(out), B, H, 17, 0, _stream()) == _lib.B200_ERR_SHAPE
+
+
+def _norm_rows(M: int, dim: int, g: torch.Generator) -> torch.Tensor:
+    """randn rows, rows x1e-3 and x1e4, one outlier channel at 2000 in a unit row, an all-zero row (cycled over M)."""
+    x = torch.randn(M, dim, generator=g)
+    for m in range(M):
+        kind = m % 5
+        if kind == 1:
+            x[m] *= 1e-3
+        elif kind == 2:
+            x[m] *= 1e4
+        elif kind == 3:
+            x[m, (m * 37) % dim] = 2000.0
+        elif kind == 4:
+            x[m] = 0.0
+    return x.bfloat16()
+
+
+def _norm_alpha(dim: int, g: torch.Generator) -> torch.Tensor:
+    alpha = torch.randn(dim, generator=g) + 0.5                         # negatives included
+    alpha[::17] = 0.0
+    return alpha.bfloat16()
+
+
+@pytest.mark.parametrize("M", [3, 40, 130])
+@pytest.mark.parametrize("dim", [4096, 2560, 1024, 256])
+def test_rmsnorm_kernel(lib, M, dim):
+    """rmsnorm_kernel (transformer.py:45-58, eps 1e-8): every element within one bf16 ulp of bf16(fp64 RMSNorm), >= 99.9 %
+    exact; an all-zero row gives zeros, not NaN."""
+    from moshi_b200 import _lib
+    g = torch.Generator().manual_seed(M * 3 + dim)
+    x, alpha = _norm_rows(M, dim, g), _norm_alpha(dim, g)
+    xd, ad = x.cuda(), alpha.cuda()
+    y = torch.full((M, dim), float("nan"), dtype=torch.bfloat16, device="cuda")
+    _lib.check(lib.b200_op_rmsnorm(cptr(xd), cptr(ad), cptr(y), M, dim, _stream()))
+    torch.cuda.synchronize()
+    ulps, exact = rmsnorm_verdict(y, x, alpha)
+    print(f"rmsnorm M={M} dim={dim}: worst {ulps:.0f} ulp (tolerance 1), {exact:.5f} exact (tolerance 0.999)")
+    assert ulps <= 1 and exact >= 0.999
+    zero = (x.float() == 0).all(-1)
+    assert torch.equal(y.cpu()[zero].float(), torch.zeros_like(y.cpu()[zero].float()))
+
+
+@pytest.mark.parametrize("M", [1, 2, 3, 4])
+@pytest.mark.parametrize("dim", [4096, 2560, 1024, 256])
+@pytest.mark.parametrize("epi", [0, 1, 2])
+def test_gemv_with_folded_rmsnorm(lib, M, dim, epi):
+    """The RMSNorm folded into the GEMV's activation staging (norm_linear at one or two sessions) against fp64
+    epi(bf16(rmsnorm_ref64(x)) . W^T), with the GEMV test's tolerances; above the GEMV rows the entry point refuses."""
+    from moshi_b200 import _lib
+    from tests.test_gpu_zy_sk_gemm import _pack
+    g = torch.Generator().manual_seed(M * 11 + dim + epi)
+    N = 1024 if epi != 2 else 2048
+    gate_rows = N // 2 if epi == 2 else 0
+    x, alpha = _norm_rows(M, dim, g), _norm_alpha(dim, g)
+    w = (torch.randn(N, dim, generator=g) / dim ** 0.5).bfloat16()
+    res = torch.randn(M, N, generator=g).bfloat16() if epi == 1 else None
+    xn = rmsnorm_ref64(x, alpha).bfloat16()
+    acc = xn.double() @ w.double().t()
+    if epi == 0:
+        want = acc
+    elif epi == 1:
+        want = res.double() + acc.bfloat16().double()
+    else:
+        h = acc.bfloat16()
+        want = (F.silu(h[:, :gate_rows].float()).bfloat16() * h[:, gate_rows:]).double()
+    xd, ad, wd = x.cuda(), alpha.cuda(), w.cuda()
+    rd = res.cuda() if res is not None else None
+    wt = _pack(lib, wd, N, dim, epi, gate_rows)
+    cols = gate_rows if epi == 2 else N
+    y = torch.full((M, cols), float("nan"), dtype=torch.bfloat16, device="cuda")
+    before = lib.b200_op_set_gemv_max_rows(4)
+    try:
+        _lib.check(lib.b200_op_linear_sk_norm(cptr(xd), cptr(ad), cptr(wt), cptr(y), cptr(rd), M, N, dim, epi, gate_rows, _stream()))
+        torch.cuda.synchronize()
+        lib.b200_op_set_gemv_max_rows(M - 1)
+        rc = lib.b200_op_linear_sk_norm(cptr(xd), cptr(ad), cptr(wt), cptr(y), cptr(rd), M, N, dim, epi, gate_rows, _stream())
+    finally:
+        lib.b200_op_set_gemv_max_rows(before)
+    assert rc == _lib.B200_ERR_STATE
+    print(stats(f"gemv + rmsnorm M={M} dim={dim} epi={epi}", y, want.float()))
+    assert torch.isfinite(y.float()).all()
+    torch.testing.assert_close(y.float().cpu(), want.float(), rtol=2e-2, atol=3e-2)
 
 
 def _tie_free_top(B: int, card: int, n_top: int, gen: torch.Generator) -> torch.Tensor:

@@ -15,8 +15,7 @@ import torch
 import torch.nn.functional as F
 
 from oracle.transformer import kv_roundtrip
-from tests.test_gpu_ops import _rope_ref
-from tests.util import cptr
+from tests.util import ATTN_C, ATTN_REL, Q8_FP16_C, Q8_WIDE_C, attn_err_ratio, attn_ref64, attn_scenario, cptr, rope_ref
 
 pytestmark = pytest.mark.gpu
 
@@ -44,59 +43,87 @@ def _decode(u8, scale, fmt):
     return (u8.float() - 128.0) * scale[..., None]
 
 
-@pytest.mark.parametrize("fmt", ["int8", "fp8_e4m3"])
-@pytest.mark.parametrize("B,H,cap,nsplit,steps", [(3, 2, 12, 0, 30), (2, 32, 300, 4, 6), (5, 4, 3000, 0, 3), (1, 32, 3000, 16, 2)])
-def test_q8_attention_step_matches_emulation(B, H, cap, nsplit, steps, fmt):
+def _q8_step(sc: dict, fmt: str, nsplit: int, label: str, c: float = ATTN_C + Q8_FP16_C) -> float:
+    """One 8-bit step on a scenario of tests.util.attn_scenario: the scenario's bf16 rings are stored in the kernel's format
+    (poisoned slots: byte 0x7F, NaN scale) and the outputs are compared with attn_ref64 over the dequantised ring, whose new
+    slot is what the kernel wrote (checked against the emulation separately)."""
     from moshi_b200 import _lib
     lib = _lib.lib()
-    g = torch.Generator().manual_seed(B * 17 + cap)
-    Cd = H * 128
-    # start from a ring that already holds `pos0` keys written by the kernel's own format
-    pos0 = torch.tensor([0, cap - 2, cap + 7, 5, 2 * cap + 1][:B], dtype=torch.int64)
-    hist_k = torch.randn(B, H, cap, 128, generator=g).bfloat16()
-    hist_v = torch.randn(B, H, cap, 128, generator=g).bfloat16() * torch.rand(B, H, cap, 1, generator=g) * 4
+    B, H, cap = sc["B"], sc["H"], sc["cap"]
     kind, qmax = FMT[fmt]
-    ring_k, ring_v = kv_roundtrip(hist_k, fmt), kv_roundtrip(hist_v, fmt)          # dequantised fp32 view of the ring
-    amax_k, amax_v = hist_k.float().abs().amax(-1), hist_v.float().abs().amax(-1)
-    k8, v8 = _encode(hist_k, amax_k, fmt).cuda(), _encode(hist_v, amax_v, fmt).cuda()
-    ks, vs = (amax_k * (1.0 / qmax)).cuda(), (amax_v * (1.0 / qmax)).cuda()
-    assert torch.equal(_decode(k8.cpu(), ks.cpu(), fmt), ring_k)
-    pos = pos0.clone()
-    out = torch.empty(B, Cd, dtype=torch.bfloat16, device="cuda")
-    worst = 0.0
-    for i in range(steps):
-        qkv = torch.randn(B, 3 * Cd, generator=g).bfloat16()
-        mask = torch.ones(B, dtype=torch.bool)
-        if B > 1 and i % 3 == 1:
-            mask[1] = False
-        q_in, k_in, v_in = (qkv[:, j * Cd:(j + 1) * Cd].reshape(B, H, 128) for j in range(3))
-        q_rot, k_rot = _rope_ref(q_in, pos), _rope_ref(k_in, pos)
-        k_new, v_new = kv_roundtrip(k_rot, fmt), kv_roundtrip(v_in, fmt)
-        for b in range(B):
-            if mask[b]:
-                ring_k[b, :, pos[b] % cap] = k_new[b]
-                ring_v[b, :, pos[b] % cap] = v_new[b]
-        n_valid = (pos + mask.long()).clamp(max=cap)
-        allowed = torch.arange(cap)[None, :] < n_valid[:, None]
-        want = F.scaled_dot_product_attention(q_rot.float()[:, :, None], ring_k, ring_v, allowed[:, None, None, :])[:, :, 0].reshape(B, Cd)
-        qd, pd, md = qkv.cuda(), pos.cuda(), mask.cuda()
-        _lib.check(lib.b200_op_attn_step_q8(cptr(qd), cptr(k8), cptr(v8), cptr(ks), cptr(vs), cptr(out), cptr(pd), cptr(md),
-                                            B, H, cap, nsplit, 10000.0, kind, _stream()))
-        torch.cuda.synchronize()
-        rows = n_valid > 0
-        worst = max(worst, (out.float().cpu()[rows] - want[rows]).abs().max().item())
-        # a bf16 ulp of sincos in the rotated key can move it (or its row's absmax) across a rounding boundary of the 8-bit
-        # grid: rare entries differ by one quantisation step of a key the softmax weights heavily; the bulk agrees to
-        # bf16 rounding
-        err = (out.float().cpu()[rows] - want[rows]).abs()
-        assert err.max() < 0.1 and err.mean() < 4e-3, (err.max(), err.mean())
-        pos = pos + mask.long()
-    print(f"{fmt} attn step B={B} H={H} cap={cap}: worst |d| vs emulation {worst:.3e}")
-    # the ring the kernel maintained == the emulation's (keys: one grid step where sincos moved a bf16 ulp of the key)
-    deq_k, deq_v = _decode(k8.cpu(), ks.cpu(), fmt), _decode(v8.cpu(), vs.cpu(), fmt)
-    assert torch.equal(deq_v, ring_v)
-    torch.testing.assert_close(deq_k, ring_k, rtol=0.13, atol=0.05)
-    assert (deq_k != ring_k).float().mean() < 0.02
+    poison = torch.isnan(sc["k"].float()).any(-1)                                   # [B, H, cap]
+    rings = []
+    for t in (sc["k"], sc["v"]):
+        clean = torch.nan_to_num(t.float()).bfloat16()
+        amax = clean.float().abs().amax(-1)
+        u8 = _encode(clean, amax, fmt)
+        u8[poison] = 0x7F
+        scale = torch.where(poison, torch.full_like(amax, float("nan")), amax * (1.0 / qmax))
+        rings += [u8.cuda(), scale.cuda()]
+    k8, ks, v8, vs = rings
+    k8_0, ks_0, v8_0, vs_0 = (r.cpu().clone() for r in rings)
+    out = torch.full((B, H * 128), float("nan"), dtype=torch.bfloat16, device="cuda")
+    qd, pd, md = sc["qkv"].cuda(), sc["pos"].cuda(), sc["mask"].cuda()
+    _lib.check(lib.b200_op_attn_step_q8(cptr(qd), cptr(k8), cptr(v8), cptr(ks), cptr(vs), cptr(out), cptr(pd), cptr(md),
+                                        B, H, cap, nsplit, 10000.0, kind, _stream()))
+    torch.cuda.synchronize()
+    k8, ks, v8, vs = k8.cpu(), ks.cpu(), v8.cpu(), vs.cpu()
+    new = torch.zeros(B, H, cap, dtype=torch.bool)
+    for b in range(B):
+        if sc["mask"][b]:
+            new[b, :, int(sc["pos"][b]) % cap] = True
+    # every other slot keeps its bytes and scales (poison included)
+    assert torch.equal(k8[~new], k8_0[~new]) and torch.equal(v8[~new], v8_0[~new])
+    assert torch.equal(ks.view(torch.int32)[~new], ks_0.view(torch.int32)[~new])
+    assert torch.equal(vs.view(torch.int32)[~new], vs_0.view(torch.int32)[~new])
+    # the appended value is the emulation's exactly; the key within one grid step where sincos moved a bf16 ulp of it
+    deq_k, deq_v = _decode(k8, ks, fmt), _decode(v8, vs, fmt)
+    rows = sc["mask"]
+    v_in = sc["qkv"].view(B, 3, H, 128)[:, 2]
+    em_k, em_v = kv_roundtrip(sc["k_rot"][rows], fmt), kv_roundtrip(v_in[rows], fmt)
+    got_k = deq_k.permute(0, 2, 1, 3)[new.permute(0, 2, 1)].view(-1, H, 128)
+    got_v = deq_v.permute(0, 2, 1, 3)[new.permute(0, 2, 1)].view(-1, H, 128)
+    assert torch.equal(got_v, em_v)
+    torch.testing.assert_close(got_k, em_k, rtol=0.13, atol=0.05)
+    assert (got_k != em_k).float().mean() < 0.02
+    want = attn_ref64(sc["q_rot"], deq_k, deq_v, sc["n_valid"])
+    ratio = attn_err_ratio(out, want, c=c)
+    print(f"{label}: B={B} nsplit={sc['nsplit']}: worst |err| / tolerance {ratio:.3f} "
+          f"(tolerance {ATTN_REL:.3g} |want| + {c:.3g} rms)")
+    assert torch.isfinite(out.float()).all()
+    assert ratio <= 1.0
+    return ratio
+
+
+@pytest.mark.parametrize("fmt", ["int8", "fp8_e4m3"])
+@pytest.mark.parametrize("H,cap,nsplit", [(32, 3000, 16), (32, 3000, 0), (20, 250, 5), (2, 12, 3)])
+def test_q8_attention_step_matches_emulation(H, cap, nsplit, fmt):
+    """The scenarios of the bf16 kernel's test (fills, wraps, paused rows, needles, poison) on the 8-bit rings: the kernel
+    agrees with fp64 attention over the dequantised ring within the bf16 rule plus the fp16 budget Q8_FP16_C."""
+    _q8_step(attn_scenario(H, cap, nsplit), fmt, nsplit, f"{fmt} attn step H={H} cap={cap}")
+
+
+@pytest.mark.parametrize("fmt", ["int8", "fp8_e4m3"])
+def test_q8_attention_step_query_range(fmt):
+    """The supported query range, |q| <= 256 per element of the rotated query: random queries up to that bound over a full
+    ring, and the worst case, a query lined up with a key whose every byte is the format's largest (each fp16 lane partial
+    then sums four products of 22.6 x 448 = 40544 for e4m3, below the fp16 limit 65504)."""
+    sc = attn_scenario(32, 3000, 0, q_scale=85.0, needles=False, seed=2)
+    _q8_step(sc, fmt, 0, f"{fmt} attn step, random |q| <= 256", c=ATTN_C + Q8_WIDE_C)
+    # worst case: rows at position 0 (no rotation), q = +-256, the new key = sign(q) (every byte at +-qmax)
+    B, H, cap = 4, 2, 64
+    g = torch.Generator().manual_seed(9)
+    sign = torch.randint(0, 2, (B, H, 128), generator=g).float() * 2 - 1
+    qkv = torch.cat([sign * 256, sign, torch.randn(B, H, 128, generator=g)], dim=1).reshape(B, 3 * H * 128).bfloat16()
+    pos, mask = torch.zeros(B, dtype=torch.int64), torch.ones(B, dtype=torch.bool)
+    k = torch.full((B, H, cap, 128), float("nan")).bfloat16()
+    q_in, k_in, v_in = (qkv.view(B, 3, H, 128)[:, i] for i in range(3))
+    k_ref, v_ref = k.clone(), k.clone()
+    k_ref[:, :, 0], v_ref[:, :, 0] = k_in, v_in
+    n_valid = torch.ones(B, dtype=torch.int64)
+    worst = dict(H=H, cap=cap, B=B, nsplit=1, qkv=qkv, k=k, v=k.clone(), pos=pos, mask=mask, n_valid=n_valid, q_rot=q_in,
+                 k_rot=k_in, k_ref=k_ref, v_ref=v_ref)
+    _q8_step(worst, fmt, 1, f"{fmt} attn step, q = +-256 lined up with a key at the format's largest bytes")
 
 
 @pytest.mark.parametrize("fmt,use_graph", [("int8", False), ("int8", True), ("fp8_e4m3", True)])
@@ -158,7 +185,7 @@ def test_q8_ring_cost_against_exact_ring(fmt, outlier, bound):
     pos = torch.full((B,), 2 * cap + 11, dtype=torch.int64)
     mask = torch.ones(B, dtype=torch.bool)
     q_in, k_in, v_in = (qkv[:, j * Cd:(j + 1) * Cd].reshape(B, H, 128) for j in range(3))
-    q_rot, k_rot = _rope_ref(q_in, pos), _rope_ref(k_in, pos)
+    q_rot, k_rot = rope_ref(q_in, pos), rope_ref(k_in, pos)
     ek, ev = hist_k.float().clone(), hist_v.float().clone()
     for b in range(B):
         ek[b, :, pos[b] % cap] = k_rot[b].float()

@@ -85,6 +85,50 @@ def test_paged_attention_step_equals_contiguous(H, cap, page_slots, nsplit):
             assert torch.equal(k[b], k0[b]) and (pg < 0 or torch.equal(kp[pg], kp0[pg])), b
 
 
+@pytest.mark.parametrize("H,cap,nsplit,page_slots", [(32, 3000, 16, 64), (32, 3000, 0, 4), (20, 250, 3, 16), (2, 12, 5, 4)])
+def test_paged_attention_step_scenarios_equal_contiguous(H, cap, nsplit, page_slots):
+    """The scenarios of test_fused_attention_step (fills at the group and split edges, wraps, paused rows, needles, NaN
+    poison past the fill) on paged rings: outputs and every mapped slot bit for bit those of the contiguous kernel.  Needles
+    also sit on the last slot of the first page and the first slot of the second, so page boundaries fall on needle keys."""
+    from tests.util import attn_scenario
+    L = _lib()
+    lib = L.lib()
+    sc = attn_scenario(H, cap, nsplit, extra_needles=(page_slots - 1, page_slots))
+    B, D = sc["B"], 128
+    g = torch.Generator().manual_seed(H + cap + page_slots)
+    T = -(-cap // page_slots)
+    n_pages = B * T + 3
+    used = sc["n_valid"]
+    mapped = torch.arange(T)[None, :] * page_slots < used[:, None]
+    table = torch.full((B, T), -1, dtype=torch.int32)
+    table[mapped] = torch.randperm(n_pages, generator=g)[:int(mapped.sum())].int()
+    k, v = sc["k"].cuda(), sc["v"].cuda()
+    kp = torch.randn(n_pages, H, page_slots, D, generator=g).bfloat16().cuda()
+    vp = torch.randn(n_pages, H, page_slots, D, generator=g).bfloat16().cuda()
+    m, tab = mapped.cuda(), table.cuda().long()
+
+    def pages(ring):
+        pad = torch.zeros(B, H, T * page_slots, D, dtype=torch.bfloat16, device="cuda")
+        pad[:, :, :cap] = ring
+        return pad.view(B, H, T, page_slots, D).permute(0, 2, 1, 3, 4)       # [B][T][H][page_slots][D]
+
+    kp[tab[m]] = pages(k)[m]
+    vp[tab[m]] = pages(v)[m]
+    qkv, pos, ex = sc["qkv"].cuda(), sc["pos"].cuda(), sc["mask"].to(torch.uint8).cuda()
+    table_d = table.cuda()
+    out_c = torch.empty(B, H * D, dtype=torch.bfloat16, device="cuda")
+    out_p = torch.empty_like(out_c)
+    st = L.current_stream(torch.device("cuda"))
+    L.check(lib.b200_op_attn_step(L.ptr(qkv), L.ptr(k), L.ptr(v), L.ptr(out_c), L.ptr(pos), L.ptr(ex), B, H, cap, nsplit, 10000.0, st))
+    L.check(lib.b200_op_attn_step_paged(L.ptr(qkv), L.ptr(kp), L.ptr(vp), L.ptr(table_d), L.ptr(out_p), L.ptr(pos), L.ptr(ex), B, H, cap,
+                                        page_slots, nsplit, 10000.0, st))
+    torch.cuda.synchronize()
+    assert torch.isfinite(out_c.float()).all()
+    assert torch.equal(out_p.view(torch.int16), out_c.view(torch.int16))
+    assert torch.equal(kp[tab[m]].view(torch.int16), pages(k)[m].view(torch.int16))
+    assert torch.equal(vp[tab[m]].view(torch.int16), pages(v)[m].view(torch.int16))
+
+
 # ---- LM step --------------------------------------------------------------------------------------------------------------
 def _run(lm, cfg, B, steps, sampling, use_graph, pool=None, page=4, events=None, seed=5):
     """Steps an LMGen (`pool` = kv_pool_frames) and records per step: text logits, audio tokens, output tokens, flags."""

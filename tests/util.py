@@ -2,6 +2,8 @@
 from __future__ import annotations
 
 import ctypes as C
+import functools
+import math
 
 import torch
 
@@ -107,3 +109,220 @@ def to_candle_layout(cfg, sd: dict) -> dict:
             out[dst + "gating.linear_in.weight"] = sd[src + f"gating.{k}.linear_in.weight"]
             out[dst + "gating.linear_out.weight"] = sd[src + f"gating.{k}.linear_out.weight"]
     return out
+
+
+# ---- fp64 references of the LM's attention and RMSNorm kernels -------------------------------------------------------------
+def rope_ref(x: torch.Tensor, pos: torch.Tensor, max_period: float = 10000.0) -> torch.Tensor:
+    """rope.py:45-82 on [B, H, D] bf16 for one time step at per-row position ``pos``: interleaved pairs, fp32, -> bf16.
+
+    The angle is fp32(freq) * fp32(pos) as in the reference, so a position past 2^24 rounds the way the reference's does (a
+    float64 angle would not).  freq, cos and sin are the correctly rounded fp32 values of the fp32 arguments (taken in
+    float64): torch's vectorised CPU exp is one ulp off for one of the 64 frequencies, and at position 2^24 one ulp of a
+    frequency turns the angle by a radian."""
+    B, H, D = x.shape
+    xf = x.float().view(B, H, D // 2, 2)
+    arg = torch.arange(D // 2, dtype=torch.float32) * torch.tensor(-math.log(max_period) * 2 / D, dtype=torch.float32)
+    freqs = torch.exp(arg.double()).float()
+    theta = (freqs[None, :] * pos.float()[:, None]).double()
+    c, s_ = torch.cos(theta).float()[:, None, :], torch.sin(theta).float()[:, None, :]
+    xr, xi = xf[..., 0], xf[..., 1]
+    return torch.stack([xr * c - xi * s_, xr * s_ + xi * c], dim=-1).view(B, H, D).bfloat16()
+
+
+def attn_ref64(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, n_valid, scale: float | None = None) -> torch.Tensor:
+    """softmax(scale * q . k) . v over the slots [0, n_valid[b]) of each row, in float64: q [B, H, D], k / v [B, H, S, D]
+    -> [B, H, D].  The valid slots are selected explicitly (no masked SDPA: a NaN in a masked slot would leak through
+    0 * NaN), and a row without a valid key gives zeros, which is what the kernels write."""
+    B, H, D = q.shape
+    scale = D ** -0.5 if scale is None else scale
+    out = torch.zeros(B, H, D, dtype=torch.float64)
+    for b in range(B):
+        n = int(n_valid[b])
+        if n == 0:
+            continue
+        kk, vv = k[b, :, :n].double(), v[b, :, :n].double()
+        s = torch.einsum("hd,hnd->hn", q[b].double(), kk) * scale
+        out[b] = torch.einsum("hn,hnd->hd", torch.softmax(s, dim=-1), vv)
+    return out
+
+
+def rmsnorm_ref64(x: torch.Tensor, alpha: torch.Tensor, eps: float = 1e-8) -> torch.Tensor:
+    """transformer.py:45-58 in float64: x * alpha / sqrt(eps + mean(x^2)) over the last dimension."""
+    x = x.double()
+    return x * alpha.double() / torch.sqrt(eps + x.pow(2).mean(-1, keepdim=True))
+
+
+# Acceptance rule of the attention outputs: |got - want| <= ATTN_REL * |want| + c * rms(want over the head's D outputs).
+# ATTN_REL is twice the largest bf16 rounding of the output (half an ulp is 2^-8 of the value at the bottom of a binade); c is
+# what fp32 arithmetic adds on top (the bf16 kernels: ATTN_C).  A single lost key out of 3000 moves the largest output of a head
+# by about 0.05 rms, so every c used here stays far below that.
+ATTN_REL = 2.0 ** -7
+ATTN_C = 2.0 ** -8
+
+
+def attn_err_ratio(got: torch.Tensor, want: torch.Tensor, c: float = ATTN_C) -> float:
+    """Largest |got - want| / tolerance over all outputs (<= 1 passes).  Where the tolerance is 0 (a row with no valid key)
+    only an exact zero passes; a NaN never does."""
+    want = want.double().cpu()
+    got = got.detach().double().cpu().reshape(want.shape)
+    err = (got - want).abs()
+    tol = ATTN_REL * want.abs() + c * want.pow(2).mean(-1, keepdim=True).sqrt()
+    ratio = torch.where(tol > 0, err / tol, torch.where(err <= 0, torch.zeros_like(err), torch.full_like(err, math.inf)))
+    return float(torch.nan_to_num(ratio, nan=math.inf, posinf=math.inf).max())
+
+
+def close_to_ref(got: torch.Tensor, want: torch.Tensor, c: float = ATTN_C) -> bool:
+    return attn_err_ratio(got, want, c) <= 1.0
+
+
+# ---- scenarios of one temporal attention step ----------------------------------------------------------------------------
+BF16_NAN = 0x7FC0            # a quiet bf16 NaN, as int16
+
+
+def attn_pick_splits(B: int, H: int, cap: int) -> int:
+    """The LM's split count for a (B, H, cap) step (lm_kernels.cuh attn_pick_splits)."""
+    ns = min(max(-(-592 // (B * H)), 1), 16)
+    return min(ns, -(-cap // 64))
+
+
+def split_ranges(n_valid: int, nsplit: int) -> list[tuple[int, int]]:
+    """The key ranges [s0, s1) of the kernel's splits for a row with n_valid keys (empty ranges included)."""
+    per = -(-n_valid // nsplit)
+    return [(min(j * per, n_valid), min((j + 1) * per, n_valid)) for j in range(nsplit)]
+
+
+def attn_rows(cap: int, nsplit: int) -> list[tuple[int, int]]:
+    """(pos, exec) of the rows of a scenario: fills at the 32-key group and 64-key loop-step edges, fewer keys than splits,
+    around a middle split boundary, cap - 1 and cap; new keys landing on the first slot, the last slot of split 0 and the first
+    slot of split 1 of a wrapped ring, one hour at 12.5 Hz; paused rows young, full, wrapped and empty.
+
+    No position reaches 2^24: there one ulp of a RoPE frequency turns the angle by a radian, and the kernel's fp32 exp / sincos
+    and any host fp32 reference disagree on a few of the 64 frequencies, so no reference can pin the kernel down."""
+    per = -(-cap // nsplit)
+    j = max(nsplit // 2, 1)
+    fills = [1, 31, 32, 33, 63, 64, 65, nsplit - 1, per * j - 1, per * j, per * j + 1, cap - 1, cap]
+    rows = [(n - 1, 1) for n in fills if 1 <= n <= cap]
+    rows += [(p, 1) for p in (cap, cap + per - 1, cap + per, 45000)]
+    rows += [(max(cap // 3, 1), 0), (cap, 0), (2 * cap + 7, 0), (0, 0)]
+    return list(dict.fromkeys(rows))
+
+
+@functools.lru_cache(maxsize=4)
+def _ring_base(H: int, cap: int, D: int, seed: int) -> tuple[torch.Tensor, torch.Tensor]:
+    """Four rings of N(0, 1) keys and values that the rows of a scenario share (saves the host time of generating each)."""
+    g = torch.Generator().manual_seed(seed)
+    return (torch.randn(4, H, cap, D, generator=g).bfloat16(), torch.randn(4, H, cap, D, generator=g).bfloat16())
+
+
+def attn_scenario(H: int, cap: int, nsplit: int, *, D: int = 128, seed: int = 0, qk_scale: float = 1.0, v_scale: float = 1.0,
+                  q_scale: float = 1.0, needles: bool = True, extra_needles: tuple[int, ...] = (), needle_score: float = 12.0) -> dict:
+    """Inputs of one attention step over the rows of ``attn_rows`` and what the step must produce.
+
+    * Rings hold N(0, 1) keys (already rotated) and values on the slots written so far.  Young rings hold bf16 NaN at and after
+      the slot the step writes, and a paused row's unwritten slot is NaN too: the kernel must neither read nor change them.
+    * Needles: keys lined up with the row's rotated query (score ``needle_score``, about +10 over the rest) with values of
+      4 N(0, 1), on the first and last slot of every split, on slot n_valid - 1, on the oldest key of a full ring and on
+      ``extra_needles``.  The new key is a
+      needle (k_in = alpha * q_in).  In a wrapped ring the OLD key at pos % cap is a needle too: an executing row must not
+      attend to it (the step overwrites it), a paused row must.
+    Returns qkv [B, 3 H D] bf16, rings k / v [B, H, cap, D] bf16 (before the step), pos, mask, nsplit (resolved), n_valid,
+    q_rot / k_rot (fp32-RoPE reference), k_ref / v_ref (the rings after the step) and want = attn_ref64 [B, H, D]."""
+    rows = attn_rows(cap, nsplit if nsplit > 0 else attn_pick_splits(24, H, cap))
+    B = len(rows)
+    ns = nsplit if nsplit > 0 else attn_pick_splits(B, H, cap)
+    pos = torch.tensor([p for p, _ in rows], dtype=torch.int64)
+    mask = torch.tensor([e for _, e in rows], dtype=torch.bool)
+    n_valid = (pos + mask.long()).clamp(max=cap)
+    g = torch.Generator().manual_seed(seed * 7919 + H * 131 + cap * 17 + ns)
+    C = H * D
+    qkv = torch.randn(B, 3 * C, generator=g)
+    qkv[:, :2 * C] *= qk_scale
+    qkv[:, :C] = (qkv[:, :C] * q_scale).clamp(-256, 256)       # q_scale: queries alone, at most 256 per element
+    qkv[:, 2 * C:] *= v_scale
+    qkv = qkv.bfloat16()
+    q_in, k_in, v_in = (qkv[:, i * C:(i + 1) * C].reshape(B, H, D) for i in range(3))
+    q_rot = rope_ref(q_in, pos)
+    base_k, base_v = _ring_base(H, cap, D, seed)
+    k = torch.empty(B, H, cap, D, dtype=torch.bfloat16)
+    v = torch.empty_like(k)
+    for b in range(B):
+        written = min(int(pos[b]), cap)                          # slots holding a key before the step
+        k[b].view(torch.int16).fill_(BF16_NAN)
+        v[b].view(torch.int16).fill_(BF16_NAN)
+        k[b, :, :written] = (base_k[b % 4, :, :written].float() * qk_scale).bfloat16()
+        v[b, :, :written] = (base_v[b % 4, :, :written].float() * v_scale).bfloat16()
+    if needles:
+        qn = q_rot.float()
+        # a key lined up with q whose score is needle_score: k = q * needle_score * sqrt(D) / |q|^2
+        k_needle = (qn * (needle_score * D ** 0.5 / qn.pow(2).sum(-1, keepdim=True))).bfloat16()     # [B, H, D]
+        for b in range(B):
+            p, n, ex = int(pos[b]), int(n_valid[b]), bool(mask[b])
+            if n == 0:
+                continue
+            slots = {s for s0, s1 in split_ranges(n, ns) if s1 > s0 for s in (s0, s1 - 1)} | {n - 1}
+            slots |= {s for s in extra_needles if s < n}
+            if p >= cap:
+                slots.add(p % cap)                               # the old key: overwritten by an executing row
+            if n == cap:
+                slots.add((p + ex) % cap)                        # the oldest key the step attends to
+            if ex and p < cap:
+                slots.discard(p)                                 # a young ring's new slot is poison until the step writes it
+            for s in sorted(slots):
+                k[b, :, s] = k_needle[b]
+                v[b, :, s] = (torch.randn(H, D, generator=g) * 4 * v_scale).bfloat16()
+        # the new key: k_in = alpha * q_in, with alpha chosen so that its rotated score is needle_score
+        qf = q_in.float()
+        alpha = needle_score * D ** 0.5 / qf.pow(2).sum(-1, keepdim=True)
+        k_in_new = (qf * alpha).bfloat16()
+        v_in_new = (torch.randn(B, H, D, generator=g) * 4 * v_scale).bfloat16()
+        qkv = qkv.view(B, 3, H, D).clone()
+        qkv[:, 1], qkv[:, 2] = k_in_new, v_in_new
+        qkv = qkv.view(B, 3 * C)
+        k_in, v_in = k_in_new, v_in_new
+    k_rot = rope_ref(k_in, pos)
+    k_ref, v_ref = k.clone(), v.clone()
+    for b in range(B):
+        if mask[b]:
+            k_ref[b, :, int(pos[b]) % cap] = k_rot[b]
+            v_ref[b, :, int(pos[b]) % cap] = v_in[b]
+    want = attn_ref64(q_rot, k_ref, v_ref, n_valid)
+    return dict(H=H, cap=cap, D=D, B=B, nsplit=ns, qkv=qkv, k=k, v=v, pos=pos, mask=mask, n_valid=n_valid, q_rot=q_rot,
+                k_rot=k_rot, k_ref=k_ref, v_ref=v_ref, want=want)
+
+
+# The 8-bit ring kernel forms q.k and the weighted value sums in fp16 (HFMA2, four products per lane partial): its outputs get
+# this much more room per rms on top of ATTN_C.
+Q8_FP16_C = 2.0 ** -8
+# At the end of its supported query range (|q| = 256 per element) the scores are in the hundreds: their fp16 rounding (~2^-11
+# of sum |q_i k_i|) and a RoPE angle that differs in its last fp32 bits move them by tenths, so near-tied keys trade weight.
+# There the outputs are only checked to stay finite and within this much per rms (measured worst: 2.2 x 2^-4 on e4m3).
+Q8_WIDE_C = 2.0 ** -2
+
+
+def dep_scenario(B: int, H: int, dep_q: int, seed: int = 0, needle_score: float = 12.0) -> dict:
+    """Inputs of the depformer attention sub-steps 0..dep_q - 1 on one per-frame cache (D = 64, scale 1/8, no RoPE).  Every
+    query has two needles: key 0 (each query carries a component along k_0) and its own new key (k_s = alpha q_s).  Returns
+    qkv [dep_q, B, 3 H 64] bf16 and want [dep_q, B, H, 64] = attn_ref64 over keys 0..s."""
+    D = 64
+    g = torch.Generator().manual_seed(seed * 31 + B * 7 + H + dep_q)
+    q = torch.randn(dep_q, B, H, D, generator=g)
+    v = torch.randn(dep_q, B, H, D, generator=g).bfloat16()
+    k0 = torch.randn(B, H, D, generator=g)
+    q[1:] += k0 * (needle_score * 8 / k0.pow(2).sum(-1, keepdim=True))
+    q = q.bfloat16()
+    qf = q.float()
+    k = (qf * (needle_score * 8 / qf.pow(2).sum(-1, keepdim=True))).bfloat16()
+    k[0] = k0.bfloat16()
+    qkv = torch.cat([q, k, v], dim=2).reshape(dep_q, B, 3 * H * D)     # rows q (h d) | k (h d) | v (h d)
+    ks, vs = k.permute(1, 2, 0, 3), v.permute(1, 2, 0, 3)            # [B, H, dep_q, D]
+    want = torch.stack([attn_ref64(q[s], ks, vs, [s + 1] * B, scale=0.125) for s in range(dep_q)])
+    return dict(B=B, H=H, D=D, dep_q=dep_q, qkv=qkv, q=q, k=ks, v=vs, want=want)
+
+
+def rmsnorm_verdict(got: torch.Tensor, x: torch.Tensor, alpha: torch.Tensor) -> tuple[float, float]:
+    """(largest distance of ``got`` from bf16(rmsnorm_ref64(x, alpha)) in bf16 ulps of the latter, share of equal elements)."""
+    want = rmsnorm_ref64(x, alpha).bfloat16().float()
+    g = got.detach().cpu().bfloat16().float()
+    ulp = torch.where(want != 0, 2.0 ** (torch.floor(torch.log2(want.abs())) - 7), torch.full_like(want, 2.0 ** -133))
+    d = torch.nan_to_num((g - want).abs() / ulp, nan=math.inf, posinf=math.inf)
+    return float(d.max()), float((g == want).float().mean())
