@@ -243,7 +243,9 @@ int b200_lm_step_host(b200_lm* h, const int64_t* in_codes_host, int n_in, const 
  * on (B, or 2B with CFG):  "text_logits" bf16 [B,text_card] (what LMGen.on_text_logits_hook sees: guided under CFG),
  * "transformer_out" bf16 [MB,dim], "dep_logits" bf16 [dep_q,B,card], "input_tokens" i64 [MB,n_q+1], "text_token" i64 [B],
  * "audio_tokens" i64 [dep_q,B], "extra_heads" bf16 [n_heads,MB,extra_heads_dim] (softmax(extra_head(transformer_out)),
- * lm.py:803-806), "model_text_logits" bf16 [MB,text_card], "model_dep_logits" bf16 [dep_q,MB,card]. */
+ * lm.py:803-806), "model_text_logits" bf16 [MB,text_card], "model_dep_logits" bf16 [dep_q,MB,card], "dep_in" bf16
+ * [MB,dep_q,depformer_dim] (depformer_in[k](transformer_out) for every sub-step k), "depformer.layers.<l>.k" / ".v" bf16
+ * [MB,depformer_heads,dep_q,64] (layer l's per-frame cache: every sub-step's key / value after the frame). */
 int b200_lm_read_buffer(b200_lm* h, const char* name, void* dst_dev, int64_t capacity_bytes, int64_t* nbytes);
 /* LMGen.get_streaming_state / set_streaming_state: token ring, per-row offsets, exec mask, the temporal KV rings
  * (1.573 GB per session at full context) and the host step counter, as one opaque device blob. */

@@ -1445,6 +1445,19 @@ int b200_lm_read_buffer(b200_lm* h, const char* name, void* dst_dev, int64_t cap
   else if (n == "audio_tokens") { src = h->audio_tokens; sz = (int64_t)c.dep_q * B * 8; }
   else if (n == "dep_trace") { src = h->dep_trace; sz = h->dep_trace ? (int64_t)tc::DEP_TRACE_SLOTS * 8 : 0; }
   else if (n == "extra_heads") { src = h->extra_out; sz = (int64_t)h->extra_w.size() * MB * c.extra_heads_dim * 2; }
+  else if (n == "dep_in" && c.dep_q > 0) { src = h->din; sz = (int64_t)MB * c.dep_q * c.depformer_dim * 2; }
+  else if (n.rfind("depformer.layers.", 0) == 0 && c.dep_q > 0) {
+    // the per-frame depformer cache of one layer: after a frame it holds every sub-step's k / v
+    const std::string rest = n.substr(17);
+    const size_t dot = rest.find('.');
+    const std::string idx = rest.substr(0, dot), kind = dot == std::string::npos ? "" : rest.substr(dot + 1);
+    const bool digits = !idx.empty() && idx.size() <= 4 && idx.find_first_not_of("0123456789") == std::string::npos;
+    const int l = digits ? atoi(idx.c_str()) : -1;
+    if (l < 0 || l >= (int)h->dlayers.size() || (kind != "k" && kind != "v"))
+      B200_FAIL(B200_ERR_INVALID, "lm_read_buffer: unknown buffer '%s'", n.c_str());
+    src = kind == "k" ? h->dlayers[l].kc : h->dlayers[l].vc;
+    sz = (int64_t)MB * c.depformer_dim * c.dep_q * 2;
+  }
   else B200_FAIL(B200_ERR_INVALID, "lm_read_buffer: unknown buffer '%s'", n.c_str());
   if (nbytes) *nbytes = sz;
   if (!dst_dev) return B200_OK;
