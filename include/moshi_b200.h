@@ -446,6 +446,16 @@ int b200_op_attn_step_q8(const void* qkv_dev, void* k8_dev, void* v8_dev, float*
  * `step` of the per-frame caches [B,H,cap,64], attention over slots 0..step with scale 1/8 and no positional embedding,
  * out bf16 [B,H*64].  cap <= 16, step < cap. */
 int b200_op_dep_attn_step(const void* qkv_dev, void* k_dev, void* v_dev, void* out_dev, int B, int H, int cap, int step, void* stream);
+/* One attention step of a Mimi bottleneck transformer layer, as the Mimi handle launches it (ring_attn_step_kernel, D = 64):
+ * qkv f32 [B,T,3*H*64] (rows q|k|v, each (h d)), RoPE at position offset[b] + t (fp32 angle), the T new keys / values
+ * appended at slots (offset[b] + t) % cap of the rings k / v f32 [B,H,cap,64] for rows with exec_mask (paused rows write
+ * nothing), attention of the T queries over the ring with the reference's mask (slot positions of RingKVCache.complete,
+ * 0 <= q_pos - k_pos < context), out = out_hi + out_lo f32 [B,T,H*64] (a tf32 hi / lo pair).  offset is not advanced.
+ * B200_ERR_SHAPE for T > 4 (one warp per query, 4 warps) or (T*64 + T*cap)*4 bytes of shared memory above 48 KB.  The qkv
+ * layout is implied by H and T, not checked: the entry receives bare pointers, so a qkv row narrower than 3*H*64 floats cannot be
+ * detected. */
+int b200_op_mimi_ring_attn(const float* qkv_dev, float* k_dev, float* v_dev, float* out_hi_dev, float* out_lo_dev, const int64_t* offset_dev,
+                           const uint8_t* exec_mask_dev, int B, int H, int T, int cap, int context, float max_period, void* stream);
 /* RMSNorm of the LM (transformer.py:45-58, eps 1e-8): y = bf16(x * alpha * rsqrt(eps + mean(x^2))), x / y bf16 [M,dim],
  * alpha bf16 [dim], dim even. */
 int b200_op_rmsnorm(const void* x_dev, const void* alpha_dev, void* y_dev, int M, int dim, void* stream);

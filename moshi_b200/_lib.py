@@ -140,6 +140,7 @@ _PROTOTYPES: dict[str, tuple[tp.Any, list]] = {
     "b200_op_attn_step_paged": (_I, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, C.c_float, _P]),
     "b200_op_attn_step_q8": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, C.c_float, _I, _P]),
     "b200_op_dep_attn_step": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P]),
+    "b200_op_mimi_ring_attn": (_I, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, C.c_float, _P]),
     "b200_op_rmsnorm": (_I, [_P, _P, _P, _I, _I, _P]),
     "b200_op_linear_sk_norm": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "b200_op_sample": (_I, [_P, _P, _P, _I, _I, _I, C.c_float, _I, _P]),

@@ -241,6 +241,24 @@ int b200_op_dep_attn_step(const void* qkv_dev, void* k_dev, void* v_dev, void* o
   return check_launch("op_dep_attn_step");
 }
 
+// ring_attn_step_kernel<64> with the Mimi handle's launch shape (mimi.cu run_transformer): one 128-thread CTA per (b, h)
+int b200_op_mimi_ring_attn(const float* qkv_dev, float* k_dev, float* v_dev, float* out_hi_dev, float* out_lo_dev, const int64_t* offset_dev,
+                           const uint8_t* exec_mask_dev, int B, int H, int T, int cap, int context, float max_period, void* stream) {
+  using namespace b200::mimi;
+  constexpr int D = 64;
+  if (!qkv_dev || !k_dev || !v_dev || !out_hi_dev || !out_lo_dev || !offset_dev || !exec_mask_dev)
+    B200_FAIL(B200_ERR_INVALID, "op_mimi_ring_attn: null pointer");
+  // one warp per query does the softmax and the kernel has 4 warps; the scores of all T queries over the ring sit in shared memory
+  const size_t smem = (size_t)(T * D + T * cap) * sizeof(float);
+  if (B < 1 || H < 1 || T < 1 || T > 4 || cap < 1 || context < 1 || smem > 48 * 1024)
+    B200_FAIL(B200_ERR_SHAPE, "op_mimi_ring_attn: B=%d H=%d T=%d cap=%d context=%d (T <= 4, %zu bytes of shared memory <= 48 KB)", B, H,
+              T, cap, context, smem);
+  const float nl = -logf(max_period) * 2.f / (float)D;
+  B200_LAUNCH((ring_attn_step_kernel<D>), B * H, 128, smem, static_cast<cudaStream_t>(stream), qkv_dev, k_dev, v_dev, out_hi_dev,
+              out_lo_dev, reinterpret_cast<const long long*>(offset_dev), exec_mask_dev, T, H, cap, context, nl);
+  return check_launch("op_mimi_ring_attn");
+}
+
 }  // extern "C"
 
 // ---- Mimi's conv kernels on the reference's [B, C, T] layout (test scaffolding: the handle keeps everything token-major) ----
