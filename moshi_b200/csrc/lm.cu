@@ -25,6 +25,24 @@ struct DLayer {
 
 }  // namespace
 
+void b200::lm::attn_step_launch(const bf16* qkv, const KvRings& r, bf16* out, float* part, int* counters, const long long* pos,
+                                const uint8_t* exec_mask, int B, int H, int cap, int nsplit, float max_period, int storage,
+                                cudaStream_t st) {
+  const dim3 grid(B * H, nsplit);
+  const float nl = -logf(max_period) * 2.f / (float)ATT_D;
+  if (storage) {
+    const AttnStepQ8 a{qkv, static_cast<uint8_t*>(r.k), static_cast<uint8_t*>(r.v), r.ks, r.vs, out, part, counters, pos, exec_mask,
+                       H, cap, nsplit, nl};
+    if (storage == KV_INT8) B200_LAUNCH(attn_step_q8_kernel<KV_INT8>, grid, ATT_THREADS, 0, st, a);
+    else B200_LAUNCH(attn_step_q8_kernel<KV_E4M3>, grid, ATT_THREADS, 0, st, a);
+    return;
+  }
+  const AttnStep a{qkv, static_cast<bf16*>(r.k), static_cast<bf16*>(r.v), out, part, counters, pos, exec_mask, H, cap, nsplit, nl,
+                   r.table, r.tab_ld, r.page_shift};
+  if (r.table) B200_LAUNCH(attn_step_kernel<true>, grid, ATT_THREADS, 0, st, a);
+  else B200_LAUNCH(attn_step_kernel<false>, grid, ATT_THREADS, 0, st, a);
+}
+
 struct b200_lm {
   b200_lm_config cfg;
   TensorStore store;
@@ -120,6 +138,9 @@ namespace {
 
 // slots per temporal KV ring: the reference's context unless b200_lm_set_kv_capacity shortened it
 inline int ring_cap(const b200_lm* h) { return h->kv_cap > 0 && h->kv_cap < h->cfg.context ? h->kv_cap : h->cfg.context; }
+
+// bytes of one head's K (or V) row in one ring slot: ATT_D bf16, or ATT_D 8-bit codes and their fp32 scale
+inline int64_t kv_row_bytes(const b200_lm* h) { return h->kv_fp8 ? ATT_D + 4 : ATT_D * 2; }
 
 int get_bf16(b200_lm* h, const std::string& name, std::vector<int64_t> shape, const bf16** out) {
   const Tensor* t = h->store.find(name);
@@ -254,10 +275,9 @@ TokenRing ring(b200_lm* h) {
 // The whole frame as a fixed launch sequence over static buffers (captured into one CUDA graph).
 int step_body(b200_lm* h) {
   const auto& c = h->cfg;
-  const int B = h->batch, MB = h->MB, d = c.dim, H = c.num_heads, D = d / H, F = c.ffn_hidden;
+  const int B = h->batch, MB = h->MB, d = c.dim, H = c.num_heads, F = c.ffn_hidden;
   const int dd = c.depformer_dim, dH = c.depformer_num_heads, dF = c.depformer_ffn_hidden;
   cudaStream_t st = h->body;
-  const float nl = -logf(c.max_period) * 2.f / (float)D;
 
   B200_LAUNCH(lm_prepare_kernel, ceil_div(B * h->Kc, 128), 128, 0, st, ring(h), h->in_codes, h->n_in_static,
               h->input_tokens, B);
@@ -278,25 +298,11 @@ int step_body(b200_lm* h) {
                 h->exec_mask_m, MB, h->tab_ld, h->page_shift, c.context, h->n_pages, h->err);
   for (auto& L : h->layers) {
     B200_TRY(norm_linear(h, h->x, L.n1, h->xn, L.in_w, h->qkv, 3 * d, MB, 3 * d, d, LIN_STORE, 0, L.in_s));
-    if (h->kv_fp8) {
-      AttnStepQ8 a;
-      a.qkv = h->qkv; a.kc = L.kc8; a.vc = L.vc8; a.ks = L.ks; a.vs = L.vs; a.out = h->ao; a.part = h->attn_part;
-      a.counters = h->attn_counters; a.pos = h->pos; a.exec_mask = h->exec_mask_m; a.H = H; a.cap = ring_cap(h); a.nsplit = h->nsplit;
-      a.neg_log_period_2_over_d = nl;
-      dim3 grid(MB * H, h->nsplit);
-      if (h->kv_fp8 == B200_KV_INT8) B200_LAUNCH(attn_step_q8_kernel<KV_INT8>, grid, ATT_THREADS, 0, st, a);
-      else B200_LAUNCH(attn_step_q8_kernel<KV_E4M3>, grid, ATT_THREADS, 0, st, a);
-    } else {   // RoPE + ring append + split-KV attention + split merge in one launch
-      AttnStep a;
-      a.qkv = h->qkv; a.kc = L.kc; a.vc = L.vc; a.out = h->ao; a.part = h->attn_part; a.counters = h->attn_counters;
-      a.pos = h->pos; a.exec_mask = h->exec_mask_m; a.H = H; a.cap = ring_cap(h); a.nsplit = h->nsplit;
-      a.neg_log_period_2_over_d = nl;
-      a.table = h->page_table; a.tab_ld = h->tab_ld; a.page_shift = h->page_shift;
-      dim3 grid(MB * H, h->nsplit);
-      if (h->n_pages) B200_LAUNCH(attn_step_paged_kernel, grid, ATT_THREADS, 0, st, a);
-      else if (attn_group_keys() == 2) B200_LAUNCH(attn_step_kernel<2>, grid, ATT_THREADS, 0, st, a);
-      else B200_LAUNCH(attn_step_kernel<4>, grid, ATT_THREADS, 0, st, a);
-    }
+    KvRings r{L.kc, L.vc};   // RoPE + ring append + split-KV attention + split merge in one launch
+    if (h->kv_fp8) r = {L.kc8, L.vc8, L.ks, L.vs};
+    if (h->n_pages) r = {L.kc, L.vc, nullptr, nullptr, h->page_table, h->tab_ld, h->page_shift};
+    attn_step_launch(h->qkv, r, h->ao, h->attn_part, h->attn_counters, h->pos, h->exec_mask_m, MB, H, ring_cap(h), h->nsplit,
+                     c.max_period, h->kv_fp8, st);
     B200_TRY(linear(h, h->ao, d, L.out_w, h->x, d, h->x, d, MB, d, d, LIN_RESADD, 0, L.out_s));
     B200_TRY(norm_linear(h, h->x, L.n2, h->xn, L.lin_in, h->hbuf, F, MB, F, d, LIN_GATE, F, L.lin_in_s));
     B200_TRY(linear(h, h->hbuf, F, L.lin_out, h->x, d, h->x, d, MB, d, F, LIN_RESADD, 0, L.lin_out_s));
@@ -368,23 +374,23 @@ int pages_for(const b200_lm* h, long long pos) {
   return (int)((n + h->page_slots - 1) / h->page_slots);
 }
 
-// Paged handle, synchronous: every row holds exactly pages_for(pos[b]) pages.  Excess pages are pushed back first (row and table
-// order), then missing ones are popped (row order).  Fails with B200_ERR_STATE, changing nothing, when they do not all fit.
-int pool_map(b200_lm* h, const std::vector<long long>& pos, const char* what) {
-  const int MB = h->MB, T = h->tab_ld;
-  int64_t want_total = 0;
-  for (int b = 0; b < MB; ++b) want_total += pages_for(h, pos[b]);
-  if (want_total > h->n_pages)
-    B200_FAIL(B200_ERR_STATE, "%s: the rows' fill needs %lld KV pages, the pool has %d", what, (long long)want_total, h->n_pages);
-  std::vector<int> table((size_t)MB * T), held(MB), stack(h->n_pages);
+// Paged handle, synchronous: model rows row0 + k * row_step come to hold exactly pages_for(pos[k]) pages, in ascending row order.
+// Their excess pages are pushed back first (row and table order), then missing ones are popped (row order).  Fails with
+// B200_ERR_STATE, changing nothing, when the free pages do not cover them.
+int pool_map(b200_lm* h, int row0, int row_step, const std::vector<long long>& pos, const char* what) {
+  const int T = h->tab_ld, n_rows = (int)pos.size();
+  std::vector<int> table((size_t)h->MB * T), held(h->MB), stack(h->n_pages);
   int top = 0;
   B200_CUDA(cudaStreamSynchronize(h->stream));
   B200_CUDA(cudaMemcpy(table.data(), h->page_table, table.size() * 4, cudaMemcpyDeviceToHost));
   B200_CUDA(cudaMemcpy(held.data(), h->page_held, held.size() * 4, cudaMemcpyDeviceToHost));
   B200_CUDA(cudaMemcpy(stack.data(), h->free_stack, stack.size() * 4, cudaMemcpyDeviceToHost));
   B200_CUDA(cudaMemcpy(&top, h->free_top, 4, cudaMemcpyDeviceToHost));
-  for (int b = 0; b < MB; ++b) {
-    const int want = pages_for(h, pos[b]);
+  int more = 0;
+  for (int k = 0; k < n_rows; ++k) more += pages_for(h, pos[k]) - held[row0 + k * row_step];
+  if (more > top) B200_FAIL(B200_ERR_STATE, "%s: the rows need %d more KV pages, the pool has %d free", what, more, top);
+  for (int k = 0; k < n_rows; ++k) {
+    const int b = row0 + k * row_step, want = pages_for(h, pos[k]);
     int* row = table.data() + (size_t)b * T;
     for (int i = want; i < T; ++i) {
       if (i < held[b]) stack[top++] = row[i];
@@ -392,8 +398,8 @@ int pool_map(b200_lm* h, const std::vector<long long>& pos, const char* what) {
     }
     held[b] = std::min(held[b], want);
   }
-  for (int b = 0; b < MB; ++b) {
-    const int want = pages_for(h, pos[b]);
+  for (int k = 0; k < n_rows; ++k) {
+    const int b = row0 + k * row_step, want = pages_for(h, pos[k]);
     for (int i = held[b]; i < want; ++i) table[(size_t)b * T + i] = stack[--top];
     held[b] = want;
   }
@@ -472,15 +478,10 @@ struct SessionPlan {
   bool cond = false;
 };
 
-// K/V bytes of one slot of one model row, all layers
-int64_t kv_slot_bytes(const b200_lm* h) {
-  return (int64_t)h->cfg.num_layers * 2 * h->cfg.num_heads * (h->kv_fp8 ? ATT_D + 4 : ATT_D * 2);
-}
-
 void session_size(const b200_lm* h, SessionPlan* p) {
   const long long end = p->cond ? h->slices_end_cond : h->slices_end;
   p->kv_off = (end + 255) / 256 * 256;
-  p->bytes = p->kv_off + kv_slot_bytes(h) * p->rows * p->n;
+  p->bytes = p->kv_off + (int64_t)h->cfg.num_layers * 2 * h->cfg.num_heads * kv_row_bytes(h) * p->rows * p->n;
 }
 
 uint64_t lm_fingerprint(const b200_lm* h) { return config_fingerprint(&h->cfg, sizeof(h->cfg)); }
@@ -511,49 +512,6 @@ int session_kv(b200_lm* h, int row, const SessionPlan& p, char* rec, bool gather
     const int64_t scales = p.kv_off + (int64_t)L2 * p.rows * h->cfg.num_heads * p.n * ATT_D;
     B200_TRY(kv_copy(h, L2, L2, row, p.rows, h->batch, (int)p.n, rec + scales, gather, true));
   }
-  return B200_OK;
-}
-
-// Paged import, synchronous, this session's rows only: each gives back its pages past what pos[k] needs, then takes the
-// missing ones from the free stack.  B200_ERR_STATE, changing nothing, when the pool cannot supply them.
-int session_map(b200_lm* h, int row, const SessionPlan& p) {
-  const int T = h->tab_ld, B = h->batch;
-  std::vector<int> table((size_t)p.rows * T), held(p.rows), stack(h->n_pages);
-  int top = 0;
-  for (int k = 0; k < p.rows; ++k) {
-    B200_CUDA(cudaMemcpy(table.data() + (size_t)k * T, h->page_table + (size_t)(row + k * B) * T, (size_t)T * 4, cudaMemcpyDeviceToHost));
-    B200_CUDA(cudaMemcpy(&held[k], h->page_held + row + k * B, 4, cudaMemcpyDeviceToHost));
-  }
-  B200_CUDA(cudaMemcpy(stack.data(), h->free_stack, stack.size() * 4, cudaMemcpyDeviceToHost));
-  B200_CUDA(cudaMemcpy(&top, h->free_top, 4, cudaMemcpyDeviceToHost));
-  int returned = 0, missing = 0;
-  for (int k = 0; k < p.rows; ++k) {
-    const int want = pages_for(h, p.pos[k]);
-    returned += std::max(held[k] - want, 0);
-    missing += std::max(want - held[k], 0);
-  }
-  if (missing > top + returned)
-    B200_FAIL(B200_ERR_STATE, "lm_session_import: the session needs %d more KV pages, the pool has %d free", missing - returned, top);
-  for (int k = 0; k < p.rows; ++k) {
-    const int want = pages_for(h, p.pos[k]);
-    int* r = table.data() + (size_t)k * T;
-    for (int i = want; i < T; ++i) {
-      if (i < held[k]) stack[top++] = r[i];
-      r[i] = -1;
-    }
-    held[k] = std::min(held[k], want);
-  }
-  for (int k = 0; k < p.rows; ++k) {
-    const int want = pages_for(h, p.pos[k]);
-    for (int i = held[k]; i < want; ++i) table[(size_t)k * T + i] = stack[--top];
-    held[k] = want;
-  }
-  for (int k = 0; k < p.rows; ++k) {
-    B200_CUDA(cudaMemcpy(h->page_table + (size_t)(row + k * B) * T, table.data() + (size_t)k * T, (size_t)T * 4, cudaMemcpyHostToDevice));
-    B200_CUDA(cudaMemcpy(h->page_held + row + k * B, &held[k], 4, cudaMemcpyHostToDevice));
-  }
-  B200_CUDA(cudaMemcpy(h->free_stack, stack.data(), stack.size() * 4, cudaMemcpyHostToDevice));
-  B200_CUDA(cudaMemcpy(h->free_top, &top, 4, cudaMemcpyHostToDevice));
   return B200_OK;
 }
 
@@ -818,7 +776,7 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
     h->n_pages = (int)std::min(ceil_div64(h->pool_frames, h->page_slots), (int64_t)MB * h->tab_ld);
   }
   const size_t ring_slots = h->n_pages ? (size_t)(h->n_pages + 1) * h->page_slots : (size_t)MB * cap;   // per layer and head
-  const size_t kv_bytes = (size_t)c.num_layers * 2 * ring_slots * H * (h->kv_fp8 ? (size_t)D + 4 : (size_t)D * 2);
+  const size_t kv_bytes = (size_t)c.num_layers * 2 * ring_slots * H * kv_row_bytes(h);
   if (kv_bytes + (1ull << 30) > free_b)
     B200_FAIL(B200_ERR_INVALID, "lm_streaming_begin: %d sessions need %.1f GB of KV ring, %.1f GB free", B, kv_bytes / 1e9,
               free_b / 1e9);
@@ -1053,7 +1011,7 @@ int b200_lm_set_state(b200_lm* h, const void* src_dev, int64_t nbytes) {
     }
     std::vector<long long> pos;
     B200_TRY(read_positions(h, static_cast<const char*>(src_dev) + off_pos, &pos));
-    B200_TRY(pool_map(h, pos, "lm_set_state"));
+    B200_TRY(pool_map(h, 0, 1, pos, "lm_set_state"));
     off = 0;
     for (auto& e : h->state.snap) {
       B200_TRY(state_copy(h, e, nullptr, static_cast<const char*>(src_dev) + off));
@@ -1094,7 +1052,7 @@ int b200_lm_state_write(b200_lm* h, const char* name, const void* src_dev, int64
   if (e->name == "model.offset") {     // each row then holds exactly the pages of its new fill
     std::vector<long long> pos;
     B200_TRY(read_positions(h, src_dev, &pos));
-    B200_TRY(pool_map(h, pos, "lm_state_write"));
+    B200_TRY(pool_map(h, 0, 1, pos, "lm_state_write"));
   }
   return state_copy(h, *e, nullptr, src_dev);
 }
@@ -1284,7 +1242,7 @@ int b200_lm_session_import(b200_lm* h, int row, const void* src_dev, int64_t nby
   if (cap < c.context && top > cap)
     B200_FAIL(B200_ERR_STATE, "lm_session_import: the session is at position %lld, the %d-slot KV ring cannot hold its history",
               (long long)top, cap);
-  if (h->n_pages) B200_TRY(session_map(h, row, p));
+  if (h->n_pages) B200_TRY(pool_map(h, row, h->batch, std::vector<long long>(p.pos, p.pos + p.rows), "lm_session_import"));
   char* rec = const_cast<char*>(static_cast<const char*>(src_dev));
   B200_TRY(row_slice_copy(h->slices_dev, p.cond ? h->n_slices_cond : h->n_slices, h->slices_max, rec, row, false, h->stream));
   B200_TRY(session_kv(h, row, p, rec, false));
@@ -1297,7 +1255,7 @@ int b200_lm_assume_fill(b200_lm* h, int fill) {
   DeviceGuard g(h->device);
   if (fill < 0) B200_FAIL(B200_ERR_INVALID, "lm_assume_fill: negative fill");
   std::vector<long long> v(h->MB, fill);
-  if (h->n_pages) B200_TRY(pool_map(h, v, "lm_assume_fill"));
+  if (h->n_pages) B200_TRY(pool_map(h, 0, 1, v, "lm_assume_fill"));
   B200_CUDA(cudaMemcpyAsync(h->offsets, v.data(), (size_t)h->batch * 8, cudaMemcpyHostToDevice, h->stream));
   B200_CUDA(cudaMemcpyAsync(h->pos, v.data(), v.size() * 8, cudaMemcpyHostToDevice, h->stream));
   B200_CUDA(cudaStreamSynchronize(h->stream));
@@ -1481,7 +1439,7 @@ int64_t b200_lm_algorithmic_bytes(b200_lm* h, int kv_fill) {
   w += (int64_t)c.dep_q * c.card * c.depformer_dim * 2;
   if (c.quantize) w /= 2;        // one byte per weight (the fp32 row scales are < 0.1 % of that)
   // per session: KV ring read (valid slots only) + append, embedding rows, logits written + read by the sampler
-  const int64_t kv_row = h->kv_fp8 ? (int64_t)c.dim + 4 * c.num_heads : (int64_t)c.dim * 2;      // bytes of one K (or V) row of a layer
+  const int64_t kv_row = c.num_heads * kv_row_bytes(h);      // bytes of one K (or V) slot of a layer, all heads
   int64_t per = (int64_t)c.num_layers * 2 * kv_fill * kv_row + (int64_t)c.num_layers * 2 * kv_row;
   per += (int64_t)(c.n_q + 1) * c.dim * 2 + (int64_t)c.dep_q * c.depformer_dim * 2;
   per += (int64_t)2 * (c.text_card + (int64_t)c.dep_q * c.card) * 2;

@@ -267,12 +267,7 @@ enum { LIN_STORE = 0, LIN_RESADD = 1, LIN_GATE = 2 };
 
 constexpr int ATT_D = 128;
 constexpr int ATT_THREADS = 128;
-
-// B200_ATT_U=2|4 (diagnostics): register-buffer depth of attn_step_kernel; default 4
-inline int attn_group_keys() {
-  static const int u = [] { const char* e = getenv("B200_ATT_U"); return (e && atoi(e) == 2) ? 2 : 4; }();
-  return u;
-}
+constexpr int ATT_GROUP = 4;                   // keys per half-warp per register buffer of the attention step
 
 // split-KV so that B*H*nsplit CTAs cover the 132 SMs a few times over even at B = 1
 inline int attn_pick_splits(int B, int H, int cap) {
@@ -306,112 +301,62 @@ struct AttnStep {
   const int* table; int tab_ld, page_shift;    // PAGED only: page table [B][tab_ld], log2(page_slots)
 };
 
-template <int ATT_U, bool PAGED = false>       // keys per half-warp per register buffer; paged rings
-static __global__ void __launch_bounds__(ATT_THREADS) attn_step_kernel(const AttnStep a) {
-  pdl_trigger();
-  const int bh = blockIdx.x, split = blockIdx.y;
-  const int b = bh / a.H, h = bh - b * a.H;
-  const int C = a.H * ATT_D;
-  const int tid = threadIdx.x, lane = tid & 31, l16 = lane & 15;
-  const int hw = tid >> 4;                          // half-warp id 0..7
+// Row of slot s of head h on page pg of a paged pool [n_pages + 1][H][1 << page_shift][row]
+__device__ __forceinline__ long long kv_paged_row(int pg, int H, int h, int s, int page_shift) {
+  return (((long long)pg * H + h) << page_shift) + (s & ((1 << page_shift) - 1));
+}
+
+// Split `split` of row b attends to ring slots [s0, s1) of the n_valid = min(pos + exec, cap) valid ones; the new key goes to
+// slot_new = pos % cap, and owns_new (CTA-uniform) says whether this split appends it.
+struct AttnRange {
+  long long p;
+  int s0, s1, slot_new;
+  bool owns_new;
+};
+template <class Args>
+__device__ __forceinline__ AttnRange attn_range(const Args& a, int b, int split) {
+  AttnRange r;
   const bool exec = a.exec_mask[b] != 0;
-  const long long p = a.pos[b];
-  long long n_valid = p + (exec ? 1 : 0);
+  r.p = a.pos[b];
+  long long n_valid = r.p + (exec ? 1 : 0);
   if (n_valid > a.cap) n_valid = a.cap;
   const int per = (int)((n_valid + a.nsplit - 1) / a.nsplit);
-  const int s0 = split * per;
-  const int s1 = (int)min((long long)(s0 + per), n_valid);
-  const int slot_new = (int)(p % a.cap);
-  const bf16* base = a.qkv + (long long)b * 3 * C + h * ATT_D;
-  const float fpos = (float)p;
-  // PAGED: element offset of slot s of this (b, h) in the pool
-  auto paged_off = [&](int s) -> long long {
-    const int pg = __ldg(a.table + (long long)b * a.tab_ld + (s >> a.page_shift));
-    return ((((long long)pg * a.H + h) << a.page_shift) + (s & ((1 << a.page_shift) - 1))) * ATT_D;
-  };
+  r.s0 = split * per;
+  r.s1 = (int)min((long long)(r.s0 + per), n_valid);
+  r.slot_new = (int)(r.p % a.cap);
+  r.owns_new = exec && r.slot_new >= r.s0 && r.slot_new < r.s1;
+  return r;
+}
 
-  if (exec && slot_new >= s0 && slot_new < s1) {    // CTA-uniform: this CTA owns the new key's slot
-    if (tid < ATT_D / 2) {
-      const int pr = tid;
-      float kr = bf2f(base[C + 2 * pr]), ki = bf2f(base[C + 2 * pr + 1]);
-      const float freq = expf((float)pr * a.neg_log_period_2_over_d);
-      float sn, cs;
-      sincosf(freq * fpos, &sn, &cs);
-      const float c2 = kr * cs - ki * sn, d2 = kr * sn + ki * cs;
-      long long o;
-      if constexpr (PAGED) o = paged_off(slot_new) + 2 * pr;
-      else o = ((long long)bh * a.cap + slot_new) * ATT_D + 2 * pr;
-      *reinterpret_cast<__nv_bfloat162*>(a.kc + o) = __floats2bfloat162_rn(c2, d2);
-      *reinterpret_cast<__nv_bfloat162*>(a.vc + o) = *reinterpret_cast<const __nv_bfloat162*>(base + 2 * C + 2 * pr);
-    }
-    __syncthreads();
+// RoPE of the pair (re, im) at position pos (rope.py:45-82)
+__device__ __forceinline__ void rope_pair(float re, float im, int pair, float pos, float neg_log_period_2_over_d, float* o0, float* o1) {
+  const float freq = expf((float)pair * neg_log_period_2_over_d);
+  float sn, cs;
+  sincosf(freq * pos, &sn, &cs);
+  *o0 = re * cs - im * sn;
+  *o1 = re * sn + im * cs;
+}
+
+// Elements [8 * l16, 8 * l16 + 8) of the query q[ATT_D] at position pos, rotated, rounded to bf16 like apply_rope's output and
+// times 1/sqrt(128), as store(j, element 2j, element 2j + 1) for j < 4
+template <class Store>
+__device__ __forceinline__ void attn_query(const bf16* q, int l16, float pos, float neg_log_period_2_over_d, Store store) {
+  float raw[8];
+  unpack8(*reinterpret_cast<const uint4*>(q + l16 * 8), raw);
+  const float scale = 0.08838834764831845f;       // 1/sqrt(128)
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    float o0, o1;
+    rope_pair(raw[2 * j], raw[2 * j + 1], l16 * 4 + j, pos, neg_log_period_2_over_d, &o0, &o1);
+    store(j, rbf(o0) * scale, rbf(o1) * scale);
   }
+}
 
-  float qf[8];
-  {
-    float raw[8];
-    unpack8(*reinterpret_cast<const uint4*>(base + l16 * 8), raw);
-    const float scale = 0.08838834764831845f;       // 1/sqrt(128)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int pr = l16 * 4 + j;
-      const float freq = expf((float)pr * a.neg_log_period_2_over_d);
-      float sn, cs;
-      sincosf(freq * fpos, &sn, &cs);
-      const float qr = raw[2 * j], qi = raw[2 * j + 1];
-      qf[2 * j] = rbf(qr * cs - qi * sn) * scale;
-      qf[2 * j + 1] = rbf(qr * sn + qi * cs) * scale;
-    }
-  }
-
-  const long long row0 = PAGED ? 0 : (long long)bh * a.cap * ATT_D;
-  const bf16* kb = a.kc + row0 + l16 * 8;
-  const bf16* vb = a.vc + row0 + l16 * 8;
-  float m = -INFINITY, l = 0.f, acc[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) acc[i] = 0.f;
-
-  // Groups of U keys per half-warp, double-buffered in registers: the loads of group i + 1 are in flight while group i
-  // is reduced (same structure as attn_step_q8_kernel below).
-  constexpr int U = ATT_U;
-  struct Group { uint4 k[U], v[U]; };
-  auto load_group = [&](int kb0, Group& gp) {
-    const int s = kb0 + hw * U;
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const int ss = s + u < s1 ? s + u : s1 - 1;
-      long long o;
-      if constexpr (PAGED) o = paged_off(ss);
-      else o = (long long)ss * ATT_D;
-      gp.k[u] = *reinterpret_cast<const uint4*>(kb + o);
-      gp.v[u] = *reinterpret_cast<const uint4*>(vb + o);
-    }
-  };
-  auto reduce_group = [&](int kb0, const Group& gp) {
-    const int s = kb0 + hw * U;
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      float kf[8];
-      unpack8(gp.k[u], kf);
-      float d = 0.f;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) d = fmaf(qf[i], kf[i], d);
-      d += __shfl_xor_sync(0xffffffffu, d, 8);
-      d += __shfl_xor_sync(0xffffffffu, d, 4);
-      d += __shfl_xor_sync(0xffffffffu, d, 2);
-      d += __shfl_xor_sync(0xffffffffu, d, 1);
-      if (s + u < s1) {
-        const float mn = fmaxf(m, d);
-        const float corr = __expf(m - mn), pw = __expf(d - mn);
-        float vf[8];
-        unpack8(gp.v[u], vf);
-        l = l * corr + pw;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) acc[i] = fmaf(pw, vf[i], acc[i] * corr);
-        m = mn;
-      }
-    }
-  };
+// Keys [s0, s1) in groups of ATT_GROUP keys per half-warp, double-buffered in registers: the loads of group i + 1 are in flight
+// while group i is reduced.  load_group(first key of the CTA's group, Group&), reduce_group(same, const Group&).
+template <class Group, class Load, class Reduce>
+__device__ __forceinline__ void attn_key_loop(int s0, int s1, Load load_group, Reduce reduce_group) {
+  constexpr int U = ATT_GROUP;
   Group ga, gb;
   if (s0 < s1) load_group(s0, ga);
   for (int kb0 = s0; kb0 < s1; kb0 += 16 * U) {     // CTA-uniform trip count and branches (shuffles inside reduce_group)
@@ -423,7 +368,13 @@ static __global__ void __launch_bounds__(ATT_THREADS) attn_step_kernel(const Att
       reduce_group(k1, gb);
     }
   }
-  // merge the 8 half-warps of the CTA
+}
+
+// Merges the online-softmax states (m, l, acc[8] over this lane's 8 outputs) of the CTA's 8 half-warps and stores out[bh]; with
+// nsplit > 1 each CTA stores its partial and the last to arrive for bh merges the splits in split order.
+template <class Args>
+__device__ __forceinline__ void attn_merge_store(const Args& a, int bh, int split, float m, float l, const float* acc) {
+  const int tid = threadIdx.x, l16 = tid & 15, hw = tid >> 4;
   __shared__ float sm_m[8], sm_l[8], sm_acc[8][ATT_D];
   __shared__ int s_last;
   if (l16 == 0) { sm_m[hw] = m; sm_l[hw] = l; }
@@ -469,8 +420,87 @@ static __global__ void __launch_bounds__(ATT_THREADS) attn_step_kernel(const Att
   }
   a.out[(long long)bh * ATT_D + tid] = f2bf(LL > 0.f ? AA / LL : 0.f);
 }
-// the paged rings run the default register-buffer depth only
-static void (*const attn_step_paged_kernel)(const AttnStep) = attn_step_kernel<4, true>;
+
+template <bool PAGED>
+static __global__ void __launch_bounds__(ATT_THREADS) attn_step_kernel(const AttnStep a) {
+  pdl_trigger();
+  const int bh = blockIdx.x, split = blockIdx.y;
+  const int b = bh / a.H, h = bh - b * a.H;
+  const int C = a.H * ATT_D;
+  const int tid = threadIdx.x, l16 = tid & 15;
+  const int hw = tid >> 4;                          // half-warp id 0..7
+  const AttnRange r = attn_range(a, b, split);
+  const bf16* base = a.qkv + (long long)b * 3 * C + h * ATT_D;
+  const float fpos = (float)r.p;
+  // PAGED: element offset of slot s of this (b, h) in the pool
+  auto paged_off = [&](int s) -> long long {
+    return kv_paged_row(__ldg(a.table + (long long)b * a.tab_ld + (s >> a.page_shift)), a.H, h, s, a.page_shift) * ATT_D;
+  };
+
+  if (r.owns_new) {
+    if (tid < ATT_D / 2) {
+      const int pr = tid;
+      float k0, k1;
+      rope_pair(bf2f(base[C + 2 * pr]), bf2f(base[C + 2 * pr + 1]), pr, fpos, a.neg_log_period_2_over_d, &k0, &k1);
+      long long o;
+      if constexpr (PAGED) o = paged_off(r.slot_new) + 2 * pr;
+      else o = ((long long)bh * a.cap + r.slot_new) * ATT_D + 2 * pr;
+      *reinterpret_cast<__nv_bfloat162*>(a.kc + o) = __floats2bfloat162_rn(k0, k1);
+      *reinterpret_cast<__nv_bfloat162*>(a.vc + o) = *reinterpret_cast<const __nv_bfloat162*>(base + 2 * C + 2 * pr);
+    }
+    __syncthreads();
+  }
+
+  float qf[8];
+  attn_query(base, l16, fpos, a.neg_log_period_2_over_d, [&](int j, float x0, float x1) { qf[2 * j] = x0; qf[2 * j + 1] = x1; });
+
+  const long long row0 = PAGED ? 0 : (long long)bh * a.cap * ATT_D;
+  const bf16* kb = a.kc + row0 + l16 * 8;
+  const bf16* vb = a.vc + row0 + l16 * 8;
+  float m = -INFINITY, l = 0.f, acc[8] = {};
+
+  constexpr int U = ATT_GROUP;
+  struct Group { uint4 k[U], v[U]; };
+  auto load_group = [&](int kb0, Group& gp) {
+    const int s = kb0 + hw * U;
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const int ss = s + u < r.s1 ? s + u : r.s1 - 1;
+      long long o;
+      if constexpr (PAGED) o = paged_off(ss);
+      else o = (long long)ss * ATT_D;
+      gp.k[u] = *reinterpret_cast<const uint4*>(kb + o);
+      gp.v[u] = *reinterpret_cast<const uint4*>(vb + o);
+    }
+  };
+  auto reduce_group = [&](int kb0, const Group& gp) {
+    const int s = kb0 + hw * U;
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      float kf[8];
+      unpack8(gp.k[u], kf);
+      float d = 0.f;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) d = fmaf(qf[i], kf[i], d);
+      d += __shfl_xor_sync(0xffffffffu, d, 8);
+      d += __shfl_xor_sync(0xffffffffu, d, 4);
+      d += __shfl_xor_sync(0xffffffffu, d, 2);
+      d += __shfl_xor_sync(0xffffffffu, d, 1);
+      if (s + u < r.s1) {
+        const float mn = fmaxf(m, d);
+        const float corr = __expf(m - mn), pw = __expf(d - mn);
+        float vf[8];
+        unpack8(gp.v[u], vf);
+        l = l * corr + pw;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) acc[i] = fmaf(pw, vf[i], acc[i] * corr);
+        m = mn;
+      }
+    }
+  };
+  attn_key_loop<Group>(r.s0, r.s1, load_group, reduce_group);
+  attn_merge_store(a, bh, split, m, l, acc);
+}
 
 // ---------------------------------------------------------------------------------------------
 // Opt-in 8-bit KV rings (SURVEY.md 8f item 3; NOT the reference's numerics): the same fused step as attn_step_kernel
@@ -540,28 +570,18 @@ static __global__ void __launch_bounds__(ATT_THREADS) attn_step_q8_kernel(const 
   const int C = a.H * ATT_D;
   const int tid = threadIdx.x, lane = tid & 31, l16 = lane & 15;
   const int hw = tid >> 4;                          // half-warp id 0..7
-  const bool exec = a.exec_mask[b] != 0;
-  const long long p = a.pos[b];
-  long long n_valid = p + (exec ? 1 : 0);
-  if (n_valid > a.cap) n_valid = a.cap;
-  const int per = (int)((n_valid + a.nsplit - 1) / a.nsplit);
-  const int s0 = split * per;
-  const int s1 = (int)min((long long)(s0 + per), n_valid);
-  const int slot_new = (int)(p % a.cap);
+  const AttnRange r = attn_range(a, b, split);
   const bf16* base = a.qkv + (long long)b * 3 * C + h * ATT_D;
-  const float fpos = (float)p;
+  const float fpos = (float)r.p;
 
-  if (exec && slot_new >= s0 && slot_new < s1) {    // CTA-uniform: this CTA owns the new key's slot
+  if (r.owns_new) {
     __shared__ float s_amax[2][2];
     float k0 = 0.f, k1 = 0.f, v0 = 0.f, v1 = 0.f;
     if (tid < ATT_D / 2) {
       const int pr = tid;
-      const float kr = bf2f(base[C + 2 * pr]), ki = bf2f(base[C + 2 * pr + 1]);
-      const float freq = expf((float)pr * a.neg_log_period_2_over_d);
-      float sn, cs;
-      sincosf(freq * fpos, &sn, &cs);
-      k0 = rbf(kr * cs - ki * sn);
-      k1 = rbf(kr * sn + ki * cs);
+      rope_pair(bf2f(base[C + 2 * pr]), bf2f(base[C + 2 * pr + 1]), pr, fpos, a.neg_log_period_2_over_d, &k0, &k1);
+      k0 = rbf(k0);
+      k1 = rbf(k1);
       v0 = bf2f(base[2 * C + 2 * pr]);
       v1 = bf2f(base[2 * C + 2 * pr + 1]);
     }
@@ -572,51 +592,35 @@ static __global__ void __launch_bounds__(ATT_THREADS) attn_step_q8_kernel(const 
       const float amk = fmaxf(s_amax[0][0], s_amax[1][0]), amv = fmaxf(s_amax[0][1], s_amax[1][1]);
       constexpr float QMAX = FMT == KV_INT8 ? 127.f : 448.f;
       const float ik = amk > 0.f ? QMAX / amk : 0.f, iv = amv > 0.f ? QMAX / amv : 0.f;
-      const long long o = ((long long)bh * a.cap + slot_new) * ATT_D + 2 * tid;
+      const long long o = ((long long)bh * a.cap + r.slot_new) * ATT_D + 2 * tid;
       *reinterpret_cast<uint16_t*>(a.kc + o) = quant2_q8<FMT>(k0 * ik, k1 * ik);
       *reinterpret_cast<uint16_t*>(a.vc + o) = quant2_q8<FMT>(v0 * iv, v1 * iv);
       if (tid == 0) {
-        a.ks[(long long)bh * a.cap + slot_new] = amk * (1.f / QMAX);
-        a.vs[(long long)bh * a.cap + slot_new] = amv * (1.f / QMAX);
+        a.ks[(long long)bh * a.cap + r.slot_new] = amk * (1.f / QMAX);
+        a.vs[(long long)bh * a.cap + r.slot_new] = amv * (1.f / QMAX);
       }
     }
     __syncthreads();
   }
 
   __half2 qh[4];
-  {
-    float raw[8];
-    unpack8(*reinterpret_cast<const uint4*>(base + l16 * 8), raw);
-    const float scale = 0.08838834764831845f;       // 1/sqrt(128)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int pr = l16 * 4 + j;
-      const float freq = expf((float)pr * a.neg_log_period_2_over_d);
-      float sn, cs;
-      sincosf(freq * fpos, &sn, &cs);
-      const float qr = raw[2 * j], qi = raw[2 * j + 1];
-      qh[j] = __floats2half2_rn(rbf(qr * cs - qi * sn) * scale, rbf(qr * sn + qi * cs) * scale);
-    }
-  }
+  attn_query(base, l16, fpos, a.neg_log_period_2_over_d, [&](int j, float x0, float x1) { qh[j] = __floats2half2_rn(x0, x1); });
 
   const uint8_t* kb = a.kc + (long long)bh * a.cap * ATT_D + l16 * 8;
   const uint8_t* vb = a.vc + (long long)bh * a.cap * ATT_D + l16 * 8;
   const float* ksb = a.ks + (long long)bh * a.cap;
   const float* vsb = a.vs + (long long)bh * a.cap;
-  float m = -INFINITY, l = 0.f, acc[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) acc[i] = 0.f;
+  float m = -INFINITY, l = 0.f, acc[8] = {};
 
-  // Groups of U keys per half-warp, double-buffered in registers: the loads of group i + 1 are in flight while group i is
-  // reduced, so a warp's time per group is max(memory latency, arithmetic) instead of their sum (the bf16 kernel can
+  // Double buffering makes a warp's time per group max(memory latency, arithmetic) instead of their sum (the bf16 kernel could
   // afford the sum: it moves twice the bytes per key).
-  constexpr int U = 4;
+  constexpr int U = ATT_GROUP;
   struct Group { uint2 k[U], v[U]; float ks[U], vs[U]; };
   auto load_group = [&](int kb0, Group& gp) {
     const int s = kb0 + hw * U;
 #pragma unroll
     for (int u = 0; u < U; ++u) {
-      const int ss = s + u < s1 ? s + u : s1 - 1;
+      const int ss = s + u < r.s1 ? s + u : r.s1 - 1;
       gp.k[u] = *reinterpret_cast<const uint2*>(kb + (long long)ss * ATT_D);
       gp.v[u] = *reinterpret_cast<const uint2*>(vb + (long long)ss * ATT_D);
       gp.ks[u] = ksb[ss];
@@ -641,7 +645,7 @@ static __global__ void __launch_bounds__(ATT_THREADS) attn_step_q8_kernel(const 
       t += __shfl_xor_sync(0xffffffffu, t, 4);
       t += __shfl_xor_sync(0xffffffffu, t, 2);
       t += __shfl_xor_sync(0xffffffffu, t, 1);
-      d[u] = s + u < s1 ? t * gp.ks[u] : -INFINITY;
+      d[u] = s + u < r.s1 ? t * gp.ks[u] : -INFINITY;
       mn = fmaxf(mn, d[u]);
     }
     if (mn > -INFINITY) {                           // uniform over the half-warp; no shuffles inside
@@ -670,63 +674,23 @@ static __global__ void __launch_bounds__(ATT_THREADS) attn_step_q8_kernel(const 
       m = mn;
     }
   };
-  Group ga, gb;
-  if (s0 < s1) load_group(s0, ga);
-  for (int kb0 = s0; kb0 < s1; kb0 += 16 * U) {     // CTA-uniform trip count and branches (shuffles inside reduce_group)
-    const int k1 = kb0 + 8 * U, k2 = kb0 + 16 * U;
-    if (k1 < s1) load_group(k1, gb);
-    reduce_group(kb0, ga);
-    if (k1 < s1) {
-      if (k2 < s1) load_group(k2, ga);
-      reduce_group(k1, gb);
-    }
-  }
-  // merge the 8 half-warps of the CTA, then the splits (same protocol as attn_step_kernel)
-  __shared__ float sm_m[8], sm_l[8], sm_acc[8][ATT_D];
-  __shared__ int s_last;
-  if (l16 == 0) { sm_m[hw] = m; sm_l[hw] = l; }
-#pragma unroll
-  for (int i = 0; i < 8; ++i) sm_acc[hw][l16 * 8 + i] = acc[i];
-  __syncthreads();
-  float M = -INFINITY;
-#pragma unroll
-  for (int w = 0; w < 8; ++w) M = fmaxf(M, sm_m[w]);
-  float L = 0.f, A = 0.f;
-#pragma unroll
-  for (int w = 0; w < 8; ++w) {
-    const float c = sm_m[w] == -INFINITY ? 0.f : __expf(sm_m[w] - M);
-    L += sm_l[w] * c;
-    A += sm_acc[w][tid] * c;
-  }
-  if (a.nsplit == 1) {
-    a.out[(long long)bh * ATT_D + tid] = f2bf(L > 0.f ? A / L : 0.f);
-    return;
-  }
-  float* o = a.part + ((long long)bh * a.nsplit + split) * (ATT_D + 2);
-  __stcg(o + tid, A);
-  if (tid == 0) { __stcg(o + ATT_D, M); __stcg(o + ATT_D + 1, L); }
-  __threadfence();
-  __syncthreads();
-  if (tid == 0) {
-    const int old = atomicAdd(a.counters + bh, 1);
-    s_last = old == a.nsplit - 1;
-    if (s_last) a.counters[bh] = 0;
-  }
-  __syncthreads();
-  if (!s_last) return;
-  __threadfence();
-  const float* pp = a.part + (long long)bh * a.nsplit * (ATT_D + 2);
-  float MM = -INFINITY;
-  for (int s = 0; s < a.nsplit; ++s) MM = fmaxf(MM, __ldcg(pp + s * (ATT_D + 2) + ATT_D));
-  float LL = 0.f, AA = 0.f;
-  for (int s = 0; s < a.nsplit; ++s) {
-    const float ms = __ldcg(pp + s * (ATT_D + 2) + ATT_D);
-    const float c = ms == -INFINITY ? 0.f : __expf(ms - MM);
-    LL += __ldcg(pp + s * (ATT_D + 2) + ATT_D + 1) * c;
-    AA += __ldcg(pp + s * (ATT_D + 2) + tid) * c;
-  }
-  a.out[(long long)bh * ATT_D + tid] = f2bf(LL > 0.f ? AA / LL : 0.f);
+  attn_key_loop<Group>(r.s0, r.s1, load_group, reduce_group);
+  attn_merge_store(a, bh, split, m, l, acc);
 }
+
+// One layer's temporal K/V as the attention step reads them: bf16 rings [B][H][cap][ATT_D], or with a page table [B][tab_ld] the
+// pools [n_pages + 1][H][1 << page_shift][ATT_D]; 8-bit rings: bytes [B][H][cap][ATT_D] and fp32 scales ks / vs [B][H][cap].
+struct KvRings {
+  void *k = nullptr, *v = nullptr;
+  float *ks = nullptr, *vs = nullptr;
+  const int* table = nullptr; int tab_ld = 0, page_shift = 0;
+};
+
+// One temporal attention step of B rows over rings stored as `storage` (0 = bf16, KV_E4M3, KV_INT8); nsplit >= 1 splits per
+// (b, h), whose partials and arrival counters are part [B*H][nsplit][ATT_D + 2] and counters [B*H] (zero between launches).
+// Defined in lm.cu, so the kernels are compiled once for the handle and the b200_op_attn_step* entry points.
+void attn_step_launch(const bf16* qkv, const KvRings& r, bf16* out, float* part, int* counters, const long long* pos,
+                      const uint8_t* exec_mask, int B, int H, int cap, int nsplit, float max_period, int storage, cudaStream_t st);
 
 constexpr int DEP_MAX_Q = 16;              // dep_q of the largest family member (configs/moshi_dev_2b.json)
 
@@ -901,7 +865,7 @@ static __global__ void kv_copy_kernel(KvCopy a) {
   if (a.table != nullptr) {
     const int pg = a.table[(long long)b * a.tab_ld + (s >> a.page_shift)];
     valid = valid && pg >= 0 && pg < a.sink;
-    r = ((((long long)pg * a.H + h) << a.page_shift) + (s & ((1 << a.page_shift) - 1))) * V + c;
+    r = kv_paged_row(pg, a.H, h, s, a.page_shift) * V + c;
   } else {
     r = (((long long)b * a.H + h) * a.cap + s) * V + c;
   }

@@ -172,14 +172,8 @@ int b200_op_attn_step(const void* qkv_dev, void* k_dev, void* v_dev, void* out_d
   float* part = nullptr;
   int* counters = nullptr;
   B200_TRY(attn_scratch(B, H, nsplit, &part, &counters, 0));
-  AttnStep a;
-  a.qkv = static_cast<const bf16*>(qkv_dev); a.kc = static_cast<bf16*>(k_dev); a.vc = static_cast<bf16*>(v_dev);
-  a.out = static_cast<bf16*>(out_dev); a.part = part; a.counters = counters;
-  a.pos = reinterpret_cast<const long long*>(pos_dev); a.exec_mask = exec_mask_dev; a.H = H; a.cap = cap; a.nsplit = nsplit;
-  a.neg_log_period_2_over_d = -logf(max_period) * 2.f / (float)ATT_D;
-  dim3 grid(B * H, nsplit);
-  if (attn_group_keys() == 2) B200_LAUNCH(attn_step_kernel<2>, grid, ATT_THREADS, 0, st, a);
-  else B200_LAUNCH(attn_step_kernel<4>, grid, ATT_THREADS, 0, st, a);
+  attn_step_launch(static_cast<const bf16*>(qkv_dev), KvRings{k_dev, v_dev}, static_cast<bf16*>(out_dev), part, counters,
+                   reinterpret_cast<const long long*>(pos_dev), exec_mask_dev, B, H, cap, nsplit, max_period, 0, st);
   return check_launch("op_attn_step");
 }
 
@@ -196,14 +190,9 @@ int b200_op_attn_step_paged(const void* qkv_dev, void* k_pool_dev, void* v_pool_
   float* part = nullptr;
   int* counters = nullptr;
   B200_TRY(attn_scratch(B, H, nsplit, &part, &counters, 0));
-  AttnStep a;
-  a.qkv = static_cast<const bf16*>(qkv_dev); a.kc = static_cast<bf16*>(k_pool_dev); a.vc = static_cast<bf16*>(v_pool_dev);
-  a.out = static_cast<bf16*>(out_dev); a.part = part; a.counters = counters;
-  a.pos = reinterpret_cast<const long long*>(pos_dev); a.exec_mask = exec_mask_dev; a.H = H; a.cap = cap; a.nsplit = nsplit;
-  a.neg_log_period_2_over_d = -logf(max_period) * 2.f / (float)ATT_D;
-  a.table = page_table_dev; a.tab_ld = (cap + page_slots - 1) / page_slots; a.page_shift = __builtin_ctz(page_slots);
-  dim3 grid(B * H, nsplit);
-  B200_LAUNCH(attn_step_paged_kernel, grid, ATT_THREADS, 0, st, a);
+  const KvRings r{k_pool_dev, v_pool_dev, nullptr, nullptr, page_table_dev, (cap + page_slots - 1) / page_slots, __builtin_ctz(page_slots)};
+  attn_step_launch(static_cast<const bf16*>(qkv_dev), r, static_cast<bf16*>(out_dev), part, counters,
+                   reinterpret_cast<const long long*>(pos_dev), exec_mask_dev, B, H, cap, nsplit, max_period, 0, st);
   return check_launch("op_attn_step_paged");
 }
 
@@ -218,14 +207,8 @@ int b200_op_attn_step_q8(const void* qkv_dev, void* k8_dev, void* v8_dev, float*
   float* part = nullptr;
   int* counters = nullptr;
   B200_TRY(attn_scratch(B, H, nsplit, &part, &counters, 1));
-  AttnStepQ8 a;
-  a.qkv = static_cast<const bf16*>(qkv_dev); a.kc = static_cast<uint8_t*>(k8_dev); a.vc = static_cast<uint8_t*>(v8_dev);
-  a.ks = ks_dev; a.vs = vs_dev; a.out = static_cast<bf16*>(out_dev); a.part = part; a.counters = counters;
-  a.pos = reinterpret_cast<const long long*>(pos_dev); a.exec_mask = exec_mask_dev; a.H = H; a.cap = cap; a.nsplit = nsplit;
-  a.neg_log_period_2_over_d = -logf(max_period) * 2.f / (float)ATT_D;
-  dim3 grid(B * H, nsplit);
-  if (kv_dtype == B200_KV_INT8) B200_LAUNCH(attn_step_q8_kernel<KV_INT8>, grid, ATT_THREADS, 0, st, a);
-  else B200_LAUNCH(attn_step_q8_kernel<KV_E4M3>, grid, ATT_THREADS, 0, st, a);
+  attn_step_launch(static_cast<const bf16*>(qkv_dev), KvRings{k8_dev, v8_dev, ks_dev, vs_dev}, static_cast<bf16*>(out_dev), part, counters,
+                   reinterpret_cast<const long long*>(pos_dev), exec_mask_dev, B, H, cap, nsplit, max_period, kv_dtype, st);
   return check_launch("op_attn_step_q8");
 }
 
