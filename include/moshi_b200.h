@@ -245,8 +245,17 @@ int b200_lm_step_host(b200_lm* h, const int64_t* in_codes_host, int n_in, const 
  * "audio_tokens" i64 [dep_q,B], "extra_heads" bf16 [n_heads,MB,extra_heads_dim] (softmax(extra_head(transformer_out)),
  * lm.py:803-806), "model_text_logits" bf16 [MB,text_card], "model_dep_logits" bf16 [dep_q,MB,card], "dep_in" bf16
  * [MB,dep_q,depformer_dim] (depformer_in[k](transformer_out) for every sub-step k), "depformer.layers.<l>.k" / ".v" bf16
- * [MB,depformer_heads,dep_q,64] (layer l's per-frame cache: every sub-step's key / value after the frame). */
+ * [MB,depformer_heads,dep_q,64] (layer l's per-frame cache: every sub-step's key / value after the frame).  With the taps on
+ * (b200_lm_set_taps), the temporal transformer of the last step: "temporal.embed" bf16 [MB,dim] (the summed input embeddings
+ * entering layer 0) and per layer l "temporal.layers.<l>.attn_out" bf16 [MB,dim] (the attention output, before out_proj),
+ * ".x_attn" [MB,dim] (x after the attention residual), ".gated" [MB,ffn_hidden] (silu(gate) * value) and ".x_out" [MB,dim]
+ * (x after the MLP residual); B200_ERR_STATE if the taps were never turned on while streaming. */
 int b200_lm_read_buffer(b200_lm* h, const char* name, void* dst_dev, int64_t capacity_bytes, int64_t* nbytes);
+/* Test taps of the temporal transformer (read through b200_lm_read_buffer "temporal.*"): when on, every step also copies the
+ * embeddings and each layer's four activations into per-layer buffers, on the step's stream.  Needs streaming; the buffers
+ * are allocated at the first enable and freed at b200_lm_streaming_end.  Turning them on or off drops the captured step graph
+ * (it is captured again at the next step); off, the step launches exactly what it launches without this call. */
+int b200_lm_set_taps(b200_lm* h, int enable);
 /* LMGen.get_streaming_state / set_streaming_state: token ring, per-row offsets, exec mask, the temporal KV rings
  * (1.573 GB per session at full context) and the host step counter, as one opaque device blob. */
 int64_t b200_lm_state_bytes(b200_lm* h);

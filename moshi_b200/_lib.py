@@ -96,6 +96,7 @@ _PROTOTYPES: dict[str, tuple[tp.Any, list]] = {
     "b200_lm_get_state": (_I, [_P, _P, C.c_int64]),
     "b200_lm_set_state": (_I, [_P, _P, C.c_int64]),
     "b200_lm_read_buffer": (_I, [_P, C.c_char_p, _P, C.c_int64, C.POINTER(C.c_int64)]),
+    "b200_lm_set_taps": (_I, [_P, _I]),
     "b200_lm_algorithmic_bytes": (C.c_int64, [_P, _I]),
     "b200_lm_assume_fill": (_I, [_P, _I]),
     "b200_lm_set_graph": (_I, [_P, _I]),

@@ -119,6 +119,9 @@ struct b200_lm {
   unsigned* dep_bar = nullptr;
   unsigned long long* dep_trace = nullptr;     // B200_DEP_TRACE=1: barrier timestamps of the fused depformer (diagnostics)
   int nsplit = 1;
+  // b200_lm_set_taps: the step copies the temporal stack's activations into taps (see tap_slot), allocated on first enable
+  int taps_on = 0;
+  bf16* taps = nullptr;
   int n_in_static = 0;
   int noise_static = 0;                        // 1: the captured step draws its own noise
   int replace_static = 0;                      // 1: this step's audio tokens are given (depformer_replace_tokens, lm.py:751-755)
@@ -272,6 +275,30 @@ TokenRing ring(b200_lm* h) {
   return r;
 }
 
+// Taps of the temporal stack: the summed embeddings, then per layer the attention output [MB][dim], x after the attention
+// residual [MB][dim], the gated hidden [MB][ffn_hidden] and x after the MLP residual [MB][dim].
+enum TapKind { TAP_ATTN_OUT, TAP_X_ATTN, TAP_GATED, TAP_X_OUT };
+int64_t tap_elems(const b200_lm* h) {
+  const int64_t MB = h->MB, d = h->cfg.dim;
+  return MB * d + (int64_t)h->layers.size() * MB * (3 * d + h->cfg.ffn_hidden);
+}
+// first element of a tap (layer -1: the embeddings) and its element count
+int64_t tap_slot(const b200_lm* h, int layer, int kind, int64_t* n) {
+  const int64_t MB = h->MB, d = h->cfg.dim, F = h->cfg.ffn_hidden;
+  *n = kind == TAP_GATED ? MB * F : MB * d;
+  if (layer < 0) return 0;
+  const int64_t at[4] = {0, MB * d, 2 * MB * d, 2 * MB * d + MB * F};
+  return MB * d + (int64_t)layer * MB * (3 * d + F) + at[kind];
+}
+// device-to-device copy on the step's stream (a memcpy node of the captured graph); nothing when taps are off
+int tap(b200_lm* h, const bf16* src, int layer, int kind) {
+  if (!h->taps_on) return B200_OK;
+  int64_t n = 0;
+  const int64_t at = tap_slot(h, layer, kind, &n);
+  B200_CUDA(cudaMemcpyAsync(h->taps + at, src, (size_t)n * 2, cudaMemcpyDeviceToDevice, h->body));
+  return B200_OK;
+}
+
 // The whole frame as a fixed launch sequence over static buffers (captured into one CUDA graph).
 int step_body(b200_lm* h) {
   const auto& c = h->cfg;
@@ -287,6 +314,7 @@ int step_body(b200_lm* h) {
     t.err = h->err;
     B200_LAUNCH(lm_embed_sum_kernel, ceil_div(MB * d / 2, 256), 256, 0, st, t, h->input_tokens, h->x, MB, d);
   }
+  B200_TRY(tap(h, h->x, -1, 0));
   if (h->noise_static) {
     const long long n = (long long)B * noise_per_row(h);
     B200_LAUNCH(lm_noise_kernel, (unsigned)ceil_div64(ceil_div64(n, 4), 256), 256, 0, st, h->noise, n, h->noise_seed, h->noise_ctr);
@@ -296,16 +324,21 @@ int step_body(b200_lm* h) {
   if (h->n_pages)                   // map the page of this step's slot (all layers share the table)
     B200_LAUNCH(kv_page_alloc_kernel, 1, KV_PAGE_THREADS, 0, st, h->page_table, h->page_held, h->free_stack, h->free_top, h->pos,
                 h->exec_mask_m, MB, h->tab_ld, h->page_shift, c.context, h->n_pages, h->err);
-  for (auto& L : h->layers) {
+  for (size_t l = 0; l < h->layers.size(); ++l) {
+    const TLayer& L = h->layers[l];
     B200_TRY(norm_linear(h, h->x, L.n1, h->xn, L.in_w, h->qkv, 3 * d, MB, 3 * d, d, LIN_STORE, 0, L.in_s));
     KvRings r{L.kc, L.vc};   // RoPE + ring append + split-KV attention + split merge in one launch
     if (h->kv_fp8) r = {L.kc8, L.vc8, L.ks, L.vs};
     if (h->n_pages) r = {L.kc, L.vc, nullptr, nullptr, h->page_table, h->tab_ld, h->page_shift};
     attn_step_launch(h->qkv, r, h->ao, h->attn_part, h->attn_counters, h->pos, h->exec_mask_m, MB, H, ring_cap(h), h->nsplit,
                      c.max_period, h->kv_fp8, st);
+    B200_TRY(tap(h, h->ao, (int)l, TAP_ATTN_OUT));
     B200_TRY(linear(h, h->ao, d, L.out_w, h->x, d, h->x, d, MB, d, d, LIN_RESADD, 0, L.out_s));
+    B200_TRY(tap(h, h->x, (int)l, TAP_X_ATTN));
     B200_TRY(norm_linear(h, h->x, L.n2, h->xn, L.lin_in, h->hbuf, F, MB, F, d, LIN_GATE, F, L.lin_in_s));
+    B200_TRY(tap(h, h->hbuf, (int)l, TAP_GATED));
     B200_TRY(linear(h, h->hbuf, F, L.lin_out, h->x, d, h->x, d, MB, d, F, LIN_RESADD, 0, L.lin_out_s));
+    B200_TRY(tap(h, h->x, (int)l, TAP_X_OUT));
   }
   B200_LAUNCH(rmsnorm_kernel, MB, 256, 0, st, h->x, h->out_norm, h->tout, d, 1e-8f);
   B200_TRY(linear(h, h->tout, d, h->text_linear, h->text_logits, c.text_card, nullptr, 0, MB, c.text_card, d, LIN_STORE, 0, h->text_linear_s));
@@ -1082,6 +1115,7 @@ int b200_lm_streaming_end(b200_lm* h) {
   h->cfg_until = nullptr; h->noise_ctr = nullptr; h->err = nullptr; h->cond_sum = nullptr; h->cond_on = 0;
   h->n_pages = 0;
   h->page_table = h->page_held = h->free_stack = h->free_top = nullptr;
+  h->taps = nullptr; h->taps_on = 0;
   if (h->pin_in) cudaFreeHost(h->pin_in);
   if (h->pin_out) cudaFreeHost(h->pin_out);
   if (h->pin_noise) cudaFreeHost(h->pin_noise);
@@ -1128,6 +1162,16 @@ int b200_lm_set_condition_sum(b200_lm* h, const void* sum_bf16_dev, int rows) {
   if (on) B200_CUDA(cudaMemcpyAsync(h->cond_sum, sum_bf16_dev, (size_t)h->MB * h->cfg.dim * 2, cudaMemcpyDeviceToDevice, h->stream));
   if (on != h->cond_on) drop_graph(h);
   h->cond_on = on;
+  return B200_OK;
+}
+
+int b200_lm_set_taps(b200_lm* h, int enable) {
+  B200_TRY(ensure_streaming(h, "lm_set_taps"));
+  DeviceGuard g(h->device);
+  const int on = enable ? 1 : 0;
+  if (on && !h->taps) B200_TRY(h->state.alloc_t(&h->taps, (size_t)tap_elems(h)));     // freed with the state at streaming_end
+  if (on != h->taps_on) drop_graph(h);
+  h->taps_on = on;
   return B200_OK;
 }
 
@@ -1415,6 +1459,24 @@ int b200_lm_read_buffer(b200_lm* h, const char* name, void* dst_dev, int64_t cap
       B200_FAIL(B200_ERR_INVALID, "lm_read_buffer: unknown buffer '%s'", n.c_str());
     src = kind == "k" ? h->dlayers[l].kc : h->dlayers[l].vc;
     sz = (int64_t)MB * c.depformer_dim * c.dep_q * 2;
+  }
+  else if (n.rfind("temporal.", 0) == 0) {
+    // the taps of the last step taken with b200_lm_set_taps on: "temporal.embed", "temporal.layers.<l>.<kind>"
+    if (!h->taps) B200_FAIL(B200_ERR_STATE, "lm_read_buffer: '%s' is a tap; turn the taps on (b200_lm_set_taps) before the step", n.c_str());
+    int layer = -1, kind = 0;
+    if (n != "temporal.embed") {
+      const std::string rest = n.rfind("temporal.layers.", 0) == 0 ? n.substr(16) : "";
+      const size_t dot = rest.find('.');
+      const std::string idx = rest.substr(0, dot), k = dot == std::string::npos ? "" : rest.substr(dot + 1);
+      const bool digits = !idx.empty() && idx.size() <= 4 && idx.find_first_not_of("0123456789") == std::string::npos;
+      layer = digits ? atoi(idx.c_str()) : -1;
+      kind = k == "attn_out" ? TAP_ATTN_OUT : k == "x_attn" ? TAP_X_ATTN : k == "gated" ? TAP_GATED : k == "x_out" ? TAP_X_OUT : -1;
+      if (layer < 0 || layer >= (int)h->layers.size() || kind < 0)
+        B200_FAIL(B200_ERR_INVALID, "lm_read_buffer: unknown buffer '%s'", n.c_str());
+    }
+    int64_t elems = 0;
+    src = h->taps + tap_slot(h, layer, kind, &elems);
+    sz = elems * 2;
   }
   else B200_FAIL(B200_ERR_INVALID, "lm_read_buffer: unknown buffer '%s'", n.c_str());
   if (nbytes) *nbytes = sz;
