@@ -242,7 +242,8 @@ int b200_lm_step_host(b200_lm* h, const int64_t* in_codes_host, int n_in, const 
 /* Hook / debug taps of the last step, copied into dst_dev (capacity in bytes; NULL = query size); MB = rows the model ran
  * on (B, or 2B with CFG):  "text_logits" bf16 [B,text_card] (what LMGen.on_text_logits_hook sees: guided under CFG),
  * "transformer_out" bf16 [MB,dim], "dep_logits" bf16 [dep_q,B,card], "input_tokens" i64 [MB,n_q+1], "text_token" i64 [B],
- * "audio_tokens" i64 [dep_q,B], "extra_heads" bf16 [n_heads,MB,extra_heads_dim] (softmax(extra_head(transformer_out)),
+ * "audio_tokens" i64 [dep_q,B], "noise" f32 [B,b200_lm_noise_per_row] (the Exp(1) draws the samplers read: the step's own
+ * draws, or the caller's copy), "extra_heads" bf16 [n_heads,MB,extra_heads_dim] (softmax(extra_head(transformer_out)),
  * lm.py:803-806), "model_text_logits" bf16 [MB,text_card], "model_dep_logits" bf16 [dep_q,MB,card], "dep_in" bf16
  * [MB,dep_q,depformer_dim] (depformer_in[k](transformer_out) for every sub-step k), "depformer.layers.<l>.k" / ".v" bf16
  * [MB,depformer_heads,dep_q,64] (layer l's per-frame cache: every sub-step's key / value after the frame).  With the taps on
@@ -364,7 +365,8 @@ int b200_frame_create(b200_mimi* mimi, b200_lm* lm, int batch, int n_codebooks, 
 int b200_frame_destroy(b200_frame* f);
 /*   pcm_in_host     f32 [B, frame_size]   one 80 ms frame per slot (idle slots: ignored)
  *   updates_host    i32 [B] or NULL (= no change; every slot active after create)
- *   noise_host / noise_dev  f32 [B, b200_lm_noise_per_row] Exp(1) draws, host or device; both NULL = greedy only
+ *   noise_host / noise_dev  f32 [B, b200_lm_noise_per_row] Exp(1) draws, host or device; both NULL = the LM step draws
+ *                   its own (b200_lm_seed_noise) when sampling is on
  *   pcm_out_host    f32 [B, frame_size]   decoded frame; silence for rows with ready == 0
  *   tokens_out_host i64 [B, dep_q + 1]    LMGen.step output (row 0 text); -2 for rows that are not ready
  *   ready_out_host  u8  [B] or NULL       1 = the row executed and is past its max_delay warm-up (lm.py:774-782)
@@ -475,6 +477,13 @@ int b200_op_linear_sk_norm(const void* x_dev, const void* alpha_dev, const void*
 /* sample_token (sampling.py:86-106): logits bf16 [B,card], noise f32 [B,min(k,card)] -> i64 [B]. */
 int b200_op_sample(const void* logits_bf16_dev, const float* noise_dev, int64_t* out_dev, int B,
                    int card, int use_sampling, float temp, int top_k, void* stream);
+/* The Exp(1) noise the LM step draws itself (b200_lm_seed_noise), as the step launches it: out f32 [n], element i from word
+ * i % 4 of Philox4x32-10 block i / 4 with counter (i / 4 low, high, ctr low, high) and key (seed low, high).  Nothing past n is
+ * written.  The counter is staged in a device word shared by all calls: calls must not overlap. */
+int b200_op_lm_noise(float* out_dev, int64_t n, uint64_t seed, uint64_t ctr, void* stream);
+/* The step's bits -> Exp(1) transform on given 32-bit words: out[i] = -log(((words[i] >> 8) + 1) * 2^-24), and 2^-24 for the top
+ * two 24-bit patterns (u >= 1 - 2^-24, as torch's exponential_ on CUDA); every output is finite and strictly positive. */
+int b200_op_exp1(const uint32_t* words_dev, float* out_dev, int64_t n, void* stream);
 
 #ifdef __cplusplus
 }

@@ -145,6 +145,8 @@ _PROTOTYPES: dict[str, tuple[tp.Any, list]] = {
     "b200_op_rmsnorm": (_I, [_P, _P, _P, _I, _I, _P]),
     "b200_op_linear_sk_norm": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "b200_op_sample": (_I, [_P, _P, _P, _I, _I, _I, C.c_float, _I, _P]),
+    "b200_op_lm_noise": (_I, [_P, C.c_int64, C.c_uint64, C.c_uint64, _P]),
+    "b200_op_exp1": (_I, [_P, _P, C.c_int64, _P]),
 }
 
 EXPORTED_SYMBOLS = tuple(_PROTOTYPES)

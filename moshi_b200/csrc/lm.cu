@@ -1445,6 +1445,7 @@ int b200_lm_read_buffer(b200_lm* h, const char* name, void* dst_dev, int64_t cap
   else if (n == "input_tokens") { src = h->input_tokens; sz = (int64_t)MB * h->Kc * 8; }
   else if (n == "text_token") { src = h->text_token; sz = (int64_t)B * 8; }
   else if (n == "audio_tokens") { src = h->audio_tokens; sz = (int64_t)c.dep_q * B * 8; }
+  else if (n == "noise") { src = h->noise; sz = (int64_t)B * noise_per_row(h) * 4; }
   else if (n == "dep_trace") { src = h->dep_trace; sz = h->dep_trace ? (int64_t)tc::DEP_TRACE_SLOTS * 8 : 0; }
   else if (n == "extra_heads") { src = h->extra_out; sz = (int64_t)h->extra_w.size() * MB * c.extra_heads_dim * 2; }
   else if (n == "dep_in" && c.dep_q > 0) { src = h->din; sz = (int64_t)MB * c.dep_q * c.depformer_dim * 2; }

@@ -202,7 +202,7 @@ static __global__ void extra_heads_kernel(const bf16* __restrict__ tout /*[B][di
 }
 
 // Exp(1) noise for one step's samplers (sampling.py:44: torch.empty_like(probs).exponential_(1)), drawn inside the step's graph:
-// Philox4x32-10 keyed by the session seed, counter = (element / 4, step counter); -log(u), u in (0, 1].
+// Philox4x32-10 keyed by the session seed, counter = (element / 4, step counter); element i is word i % 4 of block i / 4.
 __device__ __forceinline__ void philox4x32_10(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0, uint32_t k1, uint32_t* out) {
 #pragma unroll
   for (int r = 0; r < 10; ++r) {
@@ -213,6 +213,19 @@ __device__ __forceinline__ void philox4x32_10(uint32_t c0, uint32_t c1, uint32_t
     k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
   }
   out[0] = c0; out[1] = c1; out[2] = c2; out[3] = c3;
+}
+// One Exp(1) draw from 32 random bits, as torch's exponential_ makes it on CUDA: u = (m + 1) 2^-24 in (0, 1] from the top
+// 24 bits m, then -log(u) with the accurate logf (__logf's absolute error near 1 is about 2^-22, more than -log(u) itself).
+// u >= 1 - 2^-24 (the top two patterns) gives 2^-24, torch's epsilon / 2: every draw is strictly positive, so no candidate's
+// score p / q becomes -inf.
+__device__ __forceinline__ float exp1_from_bits(uint32_t r) {
+  const float u = ((float)(r >> 8) + 1.0f) * (1.0f / 16777216.0f);
+  return u >= 1.0f - 0x1p-24f ? 0x1p-24f : -logf(u);
+}
+// exp1_from_bits on given words (test entry point b200_op_exp1)
+static __global__ void exp1_kernel(const uint32_t* __restrict__ words, float* __restrict__ out, long long n) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = exp1_from_bits(words[i]);
 }
 static __global__ void lm_noise_kernel(float* __restrict__ noise, long long n, unsigned long long seed,
                                 const unsigned long long* __restrict__ step_ctr) {
@@ -225,7 +238,7 @@ static __global__ void lm_noise_kernel(float* __restrict__ noise, long long n, u
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     const long long i = q * 4 + j;
-    if (i < n) noise[i] = -__logf(((float)(r[j] >> 8) + 1.0f) * (1.0f / 16777216.0f));     // u in (2^-24, 1]
+    if (i < n) noise[i] = exp1_from_bits(r[j]);
   }
 }
 

@@ -405,6 +405,28 @@ int b200_op_tc_conv1d(const float* x_dev, const float* w_dev, const float* bias_
   return check_launch("op_tc_conv1d");
 }
 
+// lm_noise_kernel with the LM's launch shape (lm.cu step_body), the step counter in a device word like the handle's
+int b200_op_lm_noise(float* out_dev, int64_t n, uint64_t seed, uint64_t ctr, void* stream) {
+  using namespace b200::lm;
+  static unsigned long long* g_ctr = nullptr;
+  if (!out_dev || n < 1) B200_FAIL(B200_ERR_INVALID, "op_lm_noise: null output or n < 1");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (!g_ctr) B200_CUDA(cudaMalloc(&g_ctr, sizeof(unsigned long long)));
+  const unsigned long long c = ctr;
+  B200_CUDA(cudaMemcpyAsync(g_ctr, &c, sizeof(c), cudaMemcpyHostToDevice, st));
+  B200_CUDA(cudaStreamSynchronize(st));          // `c` lives on this stack frame
+  B200_LAUNCH(lm_noise_kernel, (unsigned)ceil_div64(ceil_div64(n, 4), 256), 256, 0, st, out_dev, (long long)n,
+              (unsigned long long)seed, g_ctr);
+  return check_launch("op_lm_noise");
+}
+
+int b200_op_exp1(const uint32_t* words_dev, float* out_dev, int64_t n, void* stream) {
+  using namespace b200::lm;
+  if (!words_dev || !out_dev || n < 1) B200_FAIL(B200_ERR_INVALID, "op_exp1: null pointer or n < 1");
+  B200_LAUNCH(exp1_kernel, (unsigned)ceil_div64(n, 256), 256, 0, static_cast<cudaStream_t>(stream), words_dev, out_dev, (long long)n);
+  return check_launch("op_exp1");
+}
+
 int b200_op_sample(const void* logits_bf16_dev, const float* noise_dev, int64_t* out_dev, int B, int card,
                    int use_sampling, float temp, int top_k, void* stream) {
   using namespace b200::lm;

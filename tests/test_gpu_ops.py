@@ -280,10 +280,27 @@ def _tie_free_top(B: int, card: int, n_top: int, gen: torch.Generator) -> torch.
     return out
 
 
+def _edge_rows(card: int, k: int, gen: torch.Generator) -> torch.Tensor:
+    """Three bf16 logit rows [3, card]: six equal logits across the k-th place (ranks k-3 .. k+2; at the top when k is 1);
+    +inf on the sixth-ranked token and -inf on the top one; -inf on the top token alone."""
+    base = _tie_free_top(1, card, min(card, k + 8), gen)[0]
+    srt = torch.sort(base.float(), descending=True, stable=True).indices
+    tie, inf, ninf = base.clone(), base.clone(), base.clone()
+    lo, hi = max(0, k - 3), min(card, k + 3)
+    tie[srt[lo:hi]] = base[srt[lo]]
+    inf[srt[5]] = float("inf")
+    inf[srt[0]] = float("-inf")
+    ninf[srt[0]] = float("-inf")
+    return torch.stack([tie, inf, ninf])
+
+
 @pytest.mark.parametrize("card,k,temp", [(2048, 250, 0.8), (32000, 25, 0.7), (64, 250, 0.8), (500, 25, 0.7),
-                                         (2048, 250, 6.0), (32000, 25, 9.0)])
+                                         (2048, 250, 6.0), (32000, 25, 9.0), (2048, 1, 0.8), (2048, 250, 1e-3),
+                                         (32000, 25, 1e-3)])
 def test_sampler_matches_oracle(lib, card, k, temp):
-    """sample_token with shared Exp(1) noise on logits whose top-(k+8) entries are tie-free."""
+    """sample_token with shared Exp(1) noise on logits whose top-(k+8) entries are tie-free, then on the edge rows of
+    ``_edge_rows`` against the reference sampler with ties ranked by index (the order the kernel defines).  With k = 1 the
+    sample is the greedy token."""
     from moshi_b200 import _lib
     from oracle.lm import sample_token
     g = torch.Generator().manual_seed(3)
@@ -299,6 +316,20 @@ def test_sampler_matches_oracle(lib, card, k, temp):
     agree = (out.cpu() == want).float().mean().item()
     print(f"sampler card={card} k={k} temp={temp}: agreement {agree:.3f}, distinct winners {want.unique().numel()}")
     assert agree == 1.0
+    if k == 1:
+        assert torch.equal(out.cpu(), logits.float().argmax(-1))
+    # edge rows
+    edge = _edge_rows(card, kk, g)
+    en = torch.empty(edge.shape[0], kk).exponential_(1, generator=g)
+    ewant = sample_token(edge.float(), True, temp, k, en, tie_break="index")
+    eout = torch.empty(edge.shape[0], dtype=torch.int64, device="cuda")
+    ed, end = edge.cuda(), en.cuda()
+    _lib.check(lib.b200_op_sample(cptr(ed), cptr(end), cptr(eout), edge.shape[0], card, 1, temp, k, _stream()))
+    torch.cuda.synchronize()
+    print(f"  edge rows (ties at the k-th place, +inf / -inf, -inf): got {eout.tolist()}, want {ewant.tolist()}")
+    assert torch.equal(eout.cpu(), ewant)
+    if k == 1:
+        assert torch.equal(eout.cpu(), edge.float().argmax(-1))
     # greedy
     _lib.check(lib.b200_op_sample(cptr(ld), None, cptr(out), B, card, 0, temp, k, _stream()))
     torch.cuda.synchronize()

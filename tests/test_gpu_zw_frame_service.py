@@ -21,24 +21,30 @@ def _models():
     return cfg, LMModel(cfg, sd, device="cuda"), MimiModel(MimiConfig(), msd, device="cuda")
 
 
-@pytest.mark.parametrize("sampling", [False, True])
+@pytest.mark.parametrize("sampling", [False, True, "internal"])
 def test_frame_service_equals_call_by_call(sampling):
+    """``sampling``: False = greedy; True = sampled with the caller's Exp(1) draws; "internal" = sampled with no noise passed
+    (both pointers NULL), so each LM step draws its own, seeded from torch's generator when streaming starts."""
     from moshi_b200.models import LMGen
     from moshi_b200.serving import ACTIVE, NODATA, RESET, DialogueService
     B, steps = 4, 12
+    internal = sampling == "internal"
+    sampling = bool(sampling)
     cfg, lm_a, mimi_a = _models()
     _, lm_b, mimi_b = _models()
+    torch.manual_seed(1234)
     svc = DialogueService(B, lm_a, mimi_a, use_sampling=sampling)
     gen = LMGen(lm_b, use_sampling=sampling, support_out_of_sync=True)
+    torch.manual_seed(1234)
     gen.streaming_forever(B)
     mimi_b.streaming_forever(B)
     g = torch.Generator().manual_seed(7)
     active = torch.ones(B, dtype=torch.bool)
     npr = svc._lib.b200_lm_noise_per_row(lm_a._h)
-    produced = 0
+    produced = not_greedy = 0
     for i in range(steps):
         pcm = 0.1 * torch.randn(B, 1, 1920, generator=g)
-        noise = torch.empty(B, npr).exponential_(1, generator=g) if sampling else None
+        noise = torch.empty(B, npr).exponential_(1, generator=g) if sampling and not internal else None
         updates = [9] * B                      # a positive marker: slot keeps its state (batched_asr.py:161-170)
         if i == 0:
             updates = [ACTIVE] * B
@@ -74,6 +80,12 @@ def test_frame_service_equals_call_by_call(sampling):
         ready = ready.cpu()
         assert np.array_equal(flags.astype(bool), ready.numpy()), (i, flags, ready)
         want_tok = toks[:, :, 0].cpu()
+        if internal:             # tokens other than the argmax of their own logits: the step did sample
+            tl = gen.read_buffer("text_logits", torch.bfloat16, (B, cfg.text_card)).float()
+            dl = gen.read_buffer("dep_logits", torch.bfloat16, (cfg.dep_q, B, cfg.card)).float()
+            tt = gen.read_buffer("text_token", torch.int64, (B,))
+            at = gen.read_buffer("audio_tokens", torch.int64, (cfg.dep_q, B))
+            not_greedy += int((tt != tl.argmax(-1)).sum()) + int((at != dl.argmax(-1)).sum())
         for b in range(B):
             if ready[b]:
                 assert np.array_equal(tok_out[b], want_tok[b].numpy()), (i, b)
@@ -83,6 +95,8 @@ def test_frame_service_equals_call_by_call(sampling):
                 assert (pcm_out[b] == 0).all()
                 assert (tok_out[b] < 0).any() or not active[b]
     assert produced >= B * (steps - 4)
+    if internal:
+        assert not_greedy > 0, "with no noise passed, every token was the greedy one"
     # warm-up rows: a reset slot is silent for max_delay frames again (lm.py:779-782)
     svc.close()
 

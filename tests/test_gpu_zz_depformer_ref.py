@@ -20,7 +20,8 @@ import torch
 from moshi_b200.config import LMConfig
 from moshi_b200.synth import synth_lm_state_dict
 from oracle.lm import sample_token
-from tests.util import dep_checkpoints, dep_row_ratios, depformer_ref64, greedy_unexcused, sample_is_stable
+from tests.util import (dep_checkpoints, dep_row_ratios, depformer_ref64, greedy_unexcused, sample_is_stable,
+                        sampler_mismatches)
 
 pytestmark = pytest.mark.gpu
 
@@ -86,26 +87,6 @@ def _kind(kind: str, layer) -> str:
     return kind if layer is None else f"{kind}{layer}"
 
 
-def _sampler_mismatches(logits: torch.Tensor, toks: torch.Tensor, sampling: bool, temp: float, top_k: int,
-                        noise: torch.Tensor | None) -> int:
-    """Tokens that differ from the reference sampler run on the device's own logits [B, card] with the same noise.  A
-    difference is excused only where the two best candidates' scores p / q agree to fp32 rounding (relative 1e-5)."""
-    want = sample_token(logits.float(), sampling, temp, top_k, noise, tie_break="index")
-    bad = (want != toks).nonzero().flatten().tolist()
-    n = 0
-    for b in bad:
-        if sampling:
-            lg = logits[b].double()
-            srt = torch.sort(lg, descending=True, stable=True)
-            k = min(top_k, lg.numel())
-            score = torch.softmax(srt.values / temp, -1)[:k] / noise[b, :k].double()
-            top2 = score.topk(2).values
-            if float((top2[0] - top2[1]) / top2[0]) < 1e-5:
-                continue
-        n += 1
-    return n
-
-
 @torch.no_grad()
 def _run(lm, member: str, sd: dict, B: int, sampling: bool, g: torch.Generator) -> dict:
     from moshi_b200.models import LMGen
@@ -137,12 +118,12 @@ def _run(lm, member: str, sd: dict, B: int, sampling: bool, g: torch.Generator) 
                     res["first"] = (f"frame {frame} sub-step {k} layer {layer} checkpoint {kind}: rows {rows[:8]}"
                                     f"{' ...' if len(rows) > 8 else ''} of {B}, worst ratio {float(r.max()):.3g}")
             # the samplers against the reference sampler on the device's own logits and noise
-            res["sampler"] += _sampler_mismatches(tl, text, sampling, smp["temp_text"], smp["top_k_text"],
-                                                  None if noise is None else noise[:, :kt])
+            res["sampler"] += sampler_mismatches(tl, text, sampling, smp["temp_text"], smp["top_k_text"],
+                                                 None if noise is None else noise[:, :kt])
             for k in range(Q):
                 nk = None if noise is None else noise[:, kt + k * ka:kt + (k + 1) * ka]
                 lg = got["logits"][k]
-                res["sampler"] += _sampler_mismatches(lg, toks[k], sampling, smp["temp"], smp["top_k"], nk)
+                res["sampler"] += sampler_mismatches(lg, toks[k], sampling, smp["temp"], smp["top_k"], nk)
                 # and against the reference's own token, margin-aware
                 ref_lg = want["logits"][k].bfloat16().float()
                 ref_tok = sample_token(ref_lg, sampling, smp["temp"], smp["top_k"], nk, tie_break="index")

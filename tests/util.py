@@ -5,6 +5,7 @@ import ctypes as C
 import functools
 import math
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
@@ -54,6 +55,27 @@ def greedy_unexcused(got: torch.Tensor, want: torch.Tensor, logits_oracle: torch
     gap = top2[:, 0] - top2[:, 1]
     bad = got.cpu() != want.cpu()
     return int(bad.sum()), int((bad & (gap > 2 * tol)).sum())
+
+
+def sampler_mismatches(logits: torch.Tensor, toks: torch.Tensor, sampling: bool, temp: float, top_k: int,
+                        noise: torch.Tensor | None) -> int:
+    """Tokens that differ from the reference sampler run on the device's own logits [B, card] with the same noise.  A
+    difference is excused only where the two best candidates' scores p / q agree to fp32 rounding (relative 1e-5)."""
+    from oracle.lm import sample_token
+    want = sample_token(logits.float(), sampling, temp, top_k, noise, tie_break="index")
+    bad = (want != toks).nonzero().flatten().tolist()
+    n = 0
+    for b in bad:
+        if sampling:
+            lg = logits[b].double()
+            srt = torch.sort(lg, descending=True, stable=True)
+            k = min(top_k, lg.numel())
+            score = torch.softmax(srt.values / temp, -1)[:k] / noise[b, :k].double()
+            top2 = score.topk(2).values
+            if float((top2[0] - top2[1]) / top2[0]) < 1e-5:
+                continue
+        n += 1
+    return n
 
 
 def sample_is_stable(logits: torch.Tensor, temp: float, top_k: int, noise: torch.Tensor, tol: float) -> torch.Tensor:
@@ -1044,3 +1066,52 @@ def mimi_checkpoints(want: dict, taps: dict, rings_after: dict, off_before: dict
         else:
             out.append((name, taps[name], w, False))
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------------------------
+# The Exp(1) noise the LM step draws itself (lm_noise_kernel, csrc/lm_kernels.cuh)
+# ---------------------------------------------------------------------------------------------------------------------------
+_PHILOX_M = (0xD2511F53, 0xCD9E8D57)
+_PHILOX_W = (0x9E3779B9, 0xBB67AE85)
+_U32 = np.uint64(0xFFFFFFFF)
+
+
+def philox4x32_10(ctr, key) -> np.ndarray:
+    """Philox4x32-10 (Salmon et al., SC 2011; the Random123 reference): ``ctr`` [..., 4] and ``key`` [..., 2] 32-bit words
+    (broadcast against each other) -> [..., 4] uint32.  Every product is formed exactly in uint64."""
+    c = np.asarray(ctr, dtype=np.uint64) & _U32
+    k = np.asarray(key, dtype=np.uint64) & _U32
+    c0, c1, c2, c3 = c[..., 0], c[..., 1], c[..., 2], c[..., 3]
+    k0, k1 = k[..., 0], k[..., 1]
+    m0, m1 = np.uint64(_PHILOX_M[0]), np.uint64(_PHILOX_M[1])
+    for _ in range(10):
+        p0, p1 = m0 * c0, m1 * c2
+        c0, c1, c2, c3 = ((p1 >> np.uint64(32)) ^ c1 ^ k0, p1 & _U32, (p0 >> np.uint64(32)) ^ c3 ^ k1, p0 & _U32)
+        k0 = (k0 + np.uint64(_PHILOX_W[0])) & _U32
+        k1 = (k1 + np.uint64(_PHILOX_W[1])) & _U32
+    return np.stack([c0, c1, c2, c3], axis=-1).astype(np.uint32)
+
+
+def step_words(seed: int, ctr: int, n: int) -> np.ndarray:
+    """The n raw 32-bit words of one step: element i is word i % 4 of Philox block q = i // 4, with counter
+    (q low, q high, ctr low, ctr high) and key (seed low, seed high)."""
+    q = np.arange((n + 3) // 4, dtype=np.uint64)
+    c = np.stack([q & _U32, q >> np.uint64(32), np.full_like(q, ctr & 0xFFFFFFFF), np.full_like(q, (ctr >> 32) & 0xFFFFFFFF)], -1)
+    return philox4x32_10(c, np.array([seed & 0xFFFFFFFF, (seed >> 32) & 0xFFFFFFFF], dtype=np.uint64)).reshape(-1)[:n]
+
+
+def exp1_ref64(m: np.ndarray) -> np.ndarray:
+    """fp64 -log((m + 1) / 2^24) of 24-bit patterns m."""
+    return -np.log((np.asarray(m, dtype=np.float64) + 1.0) / 2.0 ** 24)
+
+
+def step_noise_ref(seed: int, ctr: int, n: int) -> tuple[np.ndarray, np.ndarray]:
+    """(24-bit patterns r >> 8 as uint32, fp64 Exp(1) draws) of the n noise elements of step ``ctr`` under ``seed``."""
+    m = step_words(seed, ctr, n) >> np.uint32(8)
+    return m, exp1_ref64(m)
+
+
+def f32_ulp(x: np.ndarray) -> np.ndarray:
+    """One fp32 ulp at |x| (the spacing above |x| rounded to fp32)."""
+    a = np.abs(np.asarray(x, dtype=np.float32))
+    return (np.nextafter(a, np.float32(np.inf)) - a).astype(np.float64)
