@@ -380,6 +380,41 @@ int b200_frame_step(b200_frame* f, const float* pcm_in_host, const int32_t* upda
 int b200_frame_read_buffer(b200_frame* f, const char* name, void* dst_dev, int64_t capacity_bytes, int64_t* nbytes);
 
 /* ------------------------------------------------------------------------------------------ */
+/* Batched speech-to-text: ASRService.step for every session slot, one host wait per frame        */
+/* ------------------------------------------------------------------------------------------ */
+/* rust/moshi-server/batched_asr.py:100-213 (ASRService, bound by py_basr_module.rs:224-256) for the STT models: dep_q = 0, every
+ * codebook from the user, extra heads = voice-activity probabilities.  Per-slot client state (active, is_complete, offset,
+ * real_end; ClientState, :85-98) and the end-of-stream countdown live on the device; one frame is slot updates -> resets ->
+ * exec masks -> mimi.encode -> lm_gen.step_with_extra_heads -> flags, one stream-ordered chain with a single host wait.
+ * Flags are MaskFlags (:14-20). */
+typedef struct b200_asr b200_asr;
+#define B200_ASR_ACTIVE 1            /* MaskFlags of batched_asr.py:14-20 */
+#define B200_ASR_MARKER_RECEIVED 2
+#define B200_ASR_IS_EOS 4
+/* Both handles must be streaming with `batch` rows on `stream`.  B200_ERR_INVALID for an LM with dep_q != 0 or with delays (the
+ * reference's warm-up asserts that step() returns a frame), a codec with fewer than n_q - dep_q codebooks, or a batch other than
+ * both handles'.  Runs the reference's warm-up (:119-130: three frames of silence, every row executing) and returns with every
+ * slot inactive, as after ClientState(); a slot used without a RESET continues from that state. */
+int b200_asr_create(b200_mimi* mimi, b200_lm* lm, int batch, int asr_delay_in_tokens, void* stream, b200_asr** out);
+int b200_asr_destroy(b200_asr* a);
+/*   pcm_in_host          f32 [B, frame_size]  one 80 ms frame per slot (read only if some slot executes)
+ *   updates_host         i32 [B]  B200_SLOT_IDLE / _ACTIVE / _RESET, or n > 0: an end-of-stream marker; the slot's activity
+ *                        is unchanged and it ends (IS_EOS, inactive) on the frame its count of executed frames since its
+ *                        reset reaches (the count when the marker arrived) + n + asr_delay_in_tokens + 2.  Other values are
+ *                        ignored, as the reference does.
+ *   flags_inout_host     u8  [B]  written where the reference writes flags_out (NODATA 0, ACTIVE / RESET 1, marker 2, end of
+ *                        stream 4); every other entry keeps the caller's value
+ *   tokens_out_host      i64 [B]  text token of each row (-2 for rows that do not execute)
+ *   extra_heads_out_host f32 [B, extra_heads_num_heads]  element 0 of each softmaxed extra head (NULL without extra heads)
+ *   *ran                 1 if the model ran; 0 if no slot was active (skip_exec, :179-180): tokens and extra heads untouched
+ * B200_ERR_STATE if a row's KV ring did not get a page (B200_FLAG_KV_POOL), as b200_frame_step. */
+int b200_asr_step(b200_asr* a, const float* pcm_in_host, const int32_t* updates_host, uint8_t* flags_inout_host,
+                  int64_t* tokens_out_host, float* extra_heads_out_host, int* ran);
+/* Buffers of the last frame, copied device-to-device (NULL = query size): "codes_in" i64 [B,K] (mimi.encode's output), "tokens"
+ * i64 [B], "extra_heads" f32 [B,n_heads], "exec" / "reset" u8 [B], client state "offset" / "real_end" i64 [B]. */
+int b200_asr_read_buffer(b200_asr* a, const char* name, void* dst_dev, int64_t capacity_bytes, int64_t* nbytes);
+
+/* ------------------------------------------------------------------------------------------ */
 /* Kernel-level entry points (used by the parity tests; same kernels the handles launch)        */
 /* ------------------------------------------------------------------------------------------ */
 

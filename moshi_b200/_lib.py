@@ -123,6 +123,11 @@ _PROTOTYPES: dict[str, tuple[tp.Any, list]] = {
     "b200_frame_destroy": (_I, [_P]),
     "b200_frame_step": (_I, [_P, _P, _P, _P, _P, _P, _P, _P]),
     "b200_frame_read_buffer": (_I, [_P, C.c_char_p, _P, C.c_int64, C.POINTER(C.c_int64)]),
+    # batched speech-to-text service
+    "b200_asr_create": (_I, [_P, _P, _I, _I, _P, C.POINTER(_P)]),
+    "b200_asr_destroy": (_I, [_P]),
+    "b200_asr_step": (_I, [_P, _P, _P, _P, _P, _P, C.POINTER(_I)]),
+    "b200_asr_read_buffer": (_I, [_P, C.c_char_p, _P, C.c_int64, C.POINTER(C.c_int64)]),
     # kernel-level
     "b200_op_linear_bf16": (_I, [_P, _P, _P, _I, _I, _I, _P]),
     "b200_op_packed_bytes": (C.c_int64, [_I, _I, _I, _I]),

@@ -137,6 +137,18 @@ struct DeviceGuard {
 int state_entry_info(const Arena& a, int index, const char** name, int* dtype, int* ndim, int64_t* shape8, int64_t* nbytes);
 int state_entry_copy(const Arena& a, const char* name, void* dst_dev, const void* src_dev, int64_t nbytes, cudaStream_t st);
 
+// What the frame services (frame.cu) check their handles against and read from them; B200_ERR_STATE unless streaming.  The
+// pointer stays valid until the handle's streaming ends.
+struct LmFrameView {
+  int batch, model_rows, n_q, dep_q, max_delay, extra_heads, extra_dim;
+  const __nv_bfloat16* extra_out;          // [extra_heads][model_rows][extra_dim] softmaxed heads of the last step
+};
+struct MimiFrameView {
+  int batch, num_codebooks, frame_size;
+};
+int lm_frame_view(b200_lm* h, LmFrameView* out);         // lm.cu
+int mimi_frame_view(b200_mimi* h, MimiFrameView* out);   // mimi.cu
+
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 

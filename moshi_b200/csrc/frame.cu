@@ -7,6 +7,10 @@
 //   * rust/moshi-server/batched_asr.py:138-215 (ASRService.step: per-slot update flags -> reset / exec masks ->
 //     encode -> step -> host copies), the batched form the Rust server binds through py_basr_module.rs.
 // Everything is enqueued on the stream both handles stream on; the only wait is the one before the host reads.
+//
+// b200_frame_* is the dialogue frame (encode -> step -> decode).  b200_asr_* is ASRService itself (batched_asr.py:100-213) for
+// the speech-to-text models (dep_q = 0, extra heads): per-slot client state and end-of-stream countdown on the device, encode ->
+// step_with_extra_heads, no decoder.
 #include <algorithm>
 #include <string>
 
@@ -15,6 +19,61 @@
 namespace b200 {
 int lm_check_kv_pool(b200_lm* h);      // lm.cu: B200_ERR_STATE (and clears the flag) if B200_FLAG_KV_POOL was raised; no-op without a pool
 namespace {
+
+// ClientState of every slot (batched_asr.py:85-98), one array per field.
+struct AsrSlots {
+  uint8_t* active;
+  uint8_t* complete;
+  int64_t* offset;
+  int64_t* real_end;
+};
+
+// Slot updates -> client state, flags and the reset / exec masks (batched_asr.py:142-177).  flags[b] is the MaskFlags value the
+// reference assigns to flags_out[b], flags[B + b] = 1 where it assigns one at all: a slot it leaves alone keeps the caller's value.
+__global__ void asr_updates_kernel(const int32_t* __restrict__ updates, AsrSlots s, uint8_t* __restrict__ flags,
+                                   uint8_t* __restrict__ reset, uint8_t* __restrict__ exec, int B, int asr_delay) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const int u = updates[b];
+  uint8_t f = 0, written = 1, r = 0;
+  if (u == B200_SLOT_IDLE) {
+    s.active[b] = 0;
+  } else if (u == B200_SLOT_ACTIVE) {
+    s.active[b] = 1;
+    f = B200_ASR_ACTIVE;
+  } else if (u == B200_SLOT_RESET) {           // ClientState.reset(), then active
+    s.complete[b] = 0; s.offset[b] = 0; s.real_end[b] = 0; s.active[b] = 1;
+    f = B200_ASR_ACTIVE;
+    r = 1;
+  } else if (u > 0) {                          // end-of-stream marker: `u` more steps, the ASR delay and 2 frames of padding
+    s.complete[b] = 1;
+    s.real_end[b] = s.offset[b] + u + asr_delay + 2;
+    f = B200_ASR_MARKER_RECEIVED;
+  } else {
+    written = 0;
+  }
+  flags[b] = f;
+  flags[B + b] = written;
+  reset[b] = r;
+  exec[b] = s.active[b];
+}
+
+// After the step (batched_asr.py:196-213): extra[b][i] = heads[i][b][0] as f32 (extra_heads_stacked[:, :, 0, 0].T), then every
+// active slot advances; a slot whose marker has run out becomes inactive with IS_EOS.
+__global__ void asr_finish_kernel(const __nv_bfloat16* __restrict__ heads, int n_heads, int model_rows, int head_dim,
+                                  float* __restrict__ extra, AsrSlots s, uint8_t* __restrict__ flags, int B) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  for (int i = 0; i < n_heads; ++i) extra[(size_t)b * n_heads + i] = bf2f(heads[((size_t)i * model_rows + b) * head_dim]);
+  if (!s.active[b]) return;
+  const int64_t off = s.offset[b] + 1;
+  s.offset[b] = off;
+  if (s.complete[b] && off >= s.real_end[b]) {
+    s.active[b] = 0;
+    flags[b] = B200_ASR_IS_EOS;
+    flags[B + b] = 1;
+  }
+}
 
 // Slot updates -> reset / exec masks (batched_asr.py:146-177 builds them on the host and copies three tensors).
 __global__ void frame_masks_kernel(const int32_t* __restrict__ updates, uint8_t* __restrict__ active, uint8_t* __restrict__ reset,
@@ -75,6 +134,84 @@ struct b200_frame {
   cudaEvent_t done = nullptr;
   std::vector<uint8_t> h_active;     // host mirror of `active` (only to skip a frame in which no slot executes)
 };
+
+struct b200_asr {
+  b200_mimi* mimi = nullptr;
+  b200_lm* lm = nullptr;
+  int B = 0, n_codes = 0, n_user = 0, frame = 0, asr_delay = 0, n_heads = 0;   // n_codes: the codec's, n_user: the LM's n_q - dep_q
+  cudaStream_t stream = nullptr;
+  // device
+  float* pcm_in = nullptr; float* extra = nullptr;
+  int64_t* codes_in = nullptr; int64_t* codes_lm = nullptr; int64_t* tokens = nullptr;
+  int32_t* updates = nullptr;
+  uint8_t* flags = nullptr; uint8_t* reset = nullptr; uint8_t* exec = nullptr; uint8_t* all_rows = nullptr;
+  AsrSlots slots{};
+  // pinned host staging
+  float* h_pcm_in = nullptr; float* h_extra = nullptr; int64_t* h_tokens = nullptr; int32_t* h_updates = nullptr; uint8_t* h_flags = nullptr;
+  cudaEvent_t done = nullptr;
+  std::vector<uint8_t> h_active;     // host mirror of ClientState.active (only to skip a frame in which no slot executes)
+};
+
+namespace {
+
+// Exec masks -> mimi.encode -> lm_gen.step_with_extra_heads (batched_asr.py:182-197), enqueued on the handles' stream.
+int asr_run(b200_asr* a, const uint8_t* exec) {
+  B200_TRY(b200_lm_set_exec_mask(a->lm, exec));
+  B200_TRY(b200_mimi_set_exec_mask(a->mimi, exec));
+  B200_TRY(b200_mimi_encode(a->mimi, a->pcm_in, 1, a->codes_in));
+  const int64_t* codes = a->codes_in;
+  if (a->n_codes > a->n_user) {      // the step reads the first n_q - dep_q codebooks (lm.py:688-689)
+    B200_CUDA(cudaMemcpy2DAsync(a->codes_lm, (size_t)a->n_user * 8, a->codes_in, (size_t)a->n_codes * 8, (size_t)a->n_user * 8,
+                                (size_t)a->B, cudaMemcpyDeviceToDevice, a->stream));
+    codes = a->codes_lm;
+  }
+  int ready = 0;                     // always 1: b200_asr_create refuses models with delays
+  return b200_lm_step(a->lm, codes, a->n_user, nullptr, a->tokens, /*support_out_of_sync=*/0, &ready);
+}
+
+int asr_init(b200_asr* a) {
+  const size_t B = (size_t)a->B;
+  B200_CUDA(cudaMalloc(&a->pcm_in, B * a->frame * 4));
+  B200_CUDA(cudaMalloc(&a->extra, B * std::max(a->n_heads, 1) * 4));
+  B200_CUDA(cudaMalloc(&a->codes_in, B * a->n_codes * 8));
+  B200_CUDA(cudaMalloc(&a->codes_lm, B * a->n_user * 8));
+  B200_CUDA(cudaMalloc(&a->tokens, B * 8));
+  B200_CUDA(cudaMalloc(&a->updates, B * 4));
+  B200_CUDA(cudaMalloc(&a->flags, 2 * B));
+  B200_CUDA(cudaMalloc(&a->reset, B));
+  B200_CUDA(cudaMalloc(&a->exec, B));
+  B200_CUDA(cudaMalloc(&a->all_rows, B));
+  B200_CUDA(cudaMalloc(&a->slots.active, B));
+  B200_CUDA(cudaMalloc(&a->slots.complete, B));
+  B200_CUDA(cudaMalloc(&a->slots.offset, B * 8));
+  B200_CUDA(cudaMalloc(&a->slots.real_end, B * 8));
+  B200_CUDA(cudaMallocHost(&a->h_pcm_in, B * a->frame * 4));
+  B200_CUDA(cudaMallocHost(&a->h_extra, B * std::max(a->n_heads, 1) * 4));
+  B200_CUDA(cudaMallocHost(&a->h_tokens, B * 8));
+  B200_CUDA(cudaMallocHost(&a->h_updates, B * 4));
+  B200_CUDA(cudaMallocHost(&a->h_flags, 2 * B));
+  B200_CUDA(cudaEventCreateWithFlags(&a->done, cudaEventDisableTiming));
+  cudaStream_t st = a->stream;
+  B200_CUDA(cudaMemsetAsync(a->all_rows, 1, B, st));
+  B200_CUDA(cudaMemsetAsync(a->exec, 0, B, st));
+  B200_CUDA(cudaMemsetAsync(a->reset, 0, B, st));
+  B200_CUDA(cudaMemsetAsync(a->flags, 0, 2 * B, st));
+  B200_CUDA(cudaMemsetAsync(a->extra, 0, B * std::max(a->n_heads, 1) * 4, st));
+  B200_CUDA(cudaMemsetAsync(a->tokens, 0, B * 8, st));
+  // ClientState() for every slot: inactive, no marker
+  B200_CUDA(cudaMemsetAsync(a->slots.active, 0, B, st));
+  B200_CUDA(cudaMemsetAsync(a->slots.complete, 0, B, st));
+  B200_CUDA(cudaMemsetAsync(a->slots.offset, 0, B * 8, st));
+  B200_CUDA(cudaMemsetAsync(a->slots.real_end, 0, B * 8, st));
+  // warm-up (batched_asr.py:119-130): three frames of silence with every row executing
+  B200_CUDA(cudaMemsetAsync(a->pcm_in, 0, B * a->frame * 4, st));
+  for (int i = 0; i < 3; ++i) B200_TRY(asr_run(a, a->all_rows));
+  a->h_active.assign(B, 0);
+  B200_CUDA(cudaStreamSynchronize(st));
+  return lm_check_kv_pool(a->lm);
+}
+
+}  // namespace
 
 extern "C" {
 
@@ -203,6 +340,121 @@ int b200_frame_step(b200_frame* f, const float* pcm_in_host, const int32_t* upda
   memcpy(pcm_out_host, f->h_pcm_out, B * f->frame * 4);
   if (ready_out_host) memcpy(ready_out_host, f->h_ready, B);
   return lm_check_kv_pool(f->lm);
+}
+
+int b200_asr_create(b200_mimi* mimi, b200_lm* lm, int batch, int asr_delay_in_tokens, void* stream, b200_asr** out) {
+  if (!mimi || !lm || !out || batch <= 0) B200_FAIL(B200_ERR_INVALID, "asr_create: bad arguments");
+  MimiFrameView mv{};
+  LmFrameView lv{};
+  B200_TRY(mimi_frame_view(mimi, &mv));
+  B200_TRY(lm_frame_view(lm, &lv));
+  if (lv.dep_q != 0)
+    B200_FAIL(B200_ERR_INVALID, "asr_create: the speech-to-text service runs models without depformer (dep_q = 0), got dep_q = %d", lv.dep_q);
+  if (mv.num_codebooks < lv.n_q - lv.dep_q)
+    B200_FAIL(B200_ERR_INVALID, "asr_create: the LM reads %d codebooks, the codec produces %d", lv.n_q - lv.dep_q, mv.num_codebooks);
+  if (mv.batch != batch || lv.batch != batch)
+    B200_FAIL(B200_ERR_INVALID, "asr_create: batch %d, but the codec streams %d rows and the LM %d", batch, mv.batch, lv.batch);
+  if (lv.max_delay != 0)     // step() would return None for the first frames: the reference's warm-up asserts it does not
+    B200_FAIL(B200_ERR_INVALID, "asr_create: the speech-to-text service runs models without delays, got max delay %d", lv.max_delay);
+  auto* a = new b200_asr();
+  a->mimi = mimi; a->lm = lm; a->B = batch; a->n_codes = mv.num_codebooks; a->n_user = lv.n_q - lv.dep_q; a->frame = mv.frame_size;
+  a->asr_delay = asr_delay_in_tokens; a->n_heads = lv.extra_heads;
+  a->stream = static_cast<cudaStream_t>(stream);
+  const int rc = asr_init(a);
+  if (rc != B200_OK) {
+    const std::string msg = b200_last_error();
+    b200_asr_destroy(a);
+    B200_FAIL(rc, "%s", msg.c_str());
+  }
+  *out = a;
+  return B200_OK;
+}
+
+int b200_asr_destroy(b200_asr* a) {
+  if (!a) return B200_OK;
+  cudaStreamSynchronize(a->stream);
+  cudaFree(a->pcm_in); cudaFree(a->extra); cudaFree(a->codes_in); cudaFree(a->codes_lm); cudaFree(a->tokens); cudaFree(a->updates);
+  cudaFree(a->flags); cudaFree(a->reset); cudaFree(a->exec); cudaFree(a->all_rows);
+  cudaFree(a->slots.active); cudaFree(a->slots.complete); cudaFree(a->slots.offset); cudaFree(a->slots.real_end);
+  cudaFreeHost(a->h_pcm_in); cudaFreeHost(a->h_extra); cudaFreeHost(a->h_tokens); cudaFreeHost(a->h_updates); cudaFreeHost(a->h_flags);
+  if (a->done) cudaEventDestroy(a->done);
+  delete a;
+  return B200_OK;
+}
+
+int b200_asr_read_buffer(b200_asr* a, const char* name, void* dst_dev, int64_t capacity_bytes, int64_t* nbytes) {
+  if (!a || !name) B200_FAIL(B200_ERR_INVALID, "asr_read_buffer: null argument");
+  const std::string n = name;
+  const size_t B = (size_t)a->B;
+  const void* src = nullptr; int64_t sz = 0;
+  if (n == "codes_in") { src = a->codes_in; sz = (int64_t)(B * a->n_codes * 8); }
+  else if (n == "tokens") { src = a->tokens; sz = (int64_t)(B * 8); }
+  else if (n == "extra_heads") { src = a->extra; sz = (int64_t)(B * a->n_heads * 4); }
+  else if (n == "exec") { src = a->exec; sz = (int64_t)B; }
+  else if (n == "reset") { src = a->reset; sz = (int64_t)B; }
+  else if (n == "offset") { src = a->slots.offset; sz = (int64_t)(B * 8); }
+  else if (n == "real_end") { src = a->slots.real_end; sz = (int64_t)(B * 8); }
+  else B200_FAIL(B200_ERR_INVALID, "asr_read_buffer: unknown buffer '%s'", name);
+  if (nbytes) *nbytes = sz;
+  if (!dst_dev || !sz) return B200_OK;
+  if (capacity_bytes < sz) B200_FAIL(B200_ERR_SHAPE, "asr_read_buffer: destination too small");
+  B200_CUDA(cudaMemcpyAsync(dst_dev, src, (size_t)sz, cudaMemcpyDeviceToDevice, a->stream));
+  return B200_OK;
+}
+
+int b200_asr_step(b200_asr* a, const float* pcm_in_host, const int32_t* updates_host, uint8_t* flags_inout_host,
+                  int64_t* tokens_out_host, float* extra_heads_out_host, int* ran) {
+  if (ran) *ran = 0;
+  if (!a || !pcm_in_host || !updates_host || !flags_inout_host || !tokens_out_host || (a->n_heads && !extra_heads_out_host))
+    B200_FAIL(B200_ERR_INVALID, "asr_step: null buffers");
+  MimiFrameView mv{};
+  LmFrameView lv{};
+  B200_TRY(mimi_frame_view(a->mimi, &mv));
+  B200_TRY(lm_frame_view(a->lm, &lv));
+  if (mv.batch != a->B || mv.num_codebooks != a->n_codes || lv.batch != a->B)
+    B200_FAIL(B200_ERR_STATE, "asr_step: the handles' streaming batch or the codec's codebooks changed since asr_create");
+  const size_t B = (size_t)a->B;
+  cudaStream_t st = a->stream;
+  bool any_reset = false, any_active = false;
+  for (size_t b = 0; b < B; ++b) {             // the host mirror of `active`; EOS is merged in below
+    const int32_t u = updates_host[b];
+    if (u == B200_SLOT_IDLE) a->h_active[b] = 0;
+    else if (u == B200_SLOT_ACTIVE || u == B200_SLOT_RESET) a->h_active[b] = 1;
+    any_reset |= u == B200_SLOT_RESET;
+    any_active |= a->h_active[b] != 0;
+  }
+  memcpy(a->h_updates, updates_host, B * 4);
+  B200_CUDA(cudaMemcpyAsync(a->updates, a->h_updates, B * 4, cudaMemcpyHostToDevice, st));
+  B200_LAUNCH(asr_updates_kernel, (unsigned)((B + 127) / 128), 128, 0, st, a->updates, a->slots, a->flags, a->reset, a->exec, (int)B,
+              a->asr_delay);
+  B200_TRY(check_launch("asr_updates"));
+  if (any_reset) {                             // batched_asr.py:175-177
+    B200_TRY(b200_lm_reset(a->lm, a->reset));
+    B200_TRY(b200_mimi_reset(a->mimi, a->reset));
+  }
+  if (any_active) {                            // else skip_exec (batched_asr.py:179-180): no step, tokens and extra heads untouched
+    memcpy(a->h_pcm_in, pcm_in_host, B * a->frame * 4);
+    B200_CUDA(cudaMemcpyAsync(a->pcm_in, a->h_pcm_in, B * a->frame * 4, cudaMemcpyHostToDevice, st));
+    B200_TRY(asr_run(a, a->exec));
+    B200_LAUNCH(asr_finish_kernel, (unsigned)((B + 127) / 128), 128, 0, st, lv.extra_out, a->n_heads, lv.model_rows, lv.extra_dim,
+                a->extra, a->slots, a->flags, (int)B);
+    B200_TRY(check_launch("asr_finish"));
+    B200_CUDA(cudaMemcpyAsync(a->h_tokens, a->tokens, B * 8, cudaMemcpyDeviceToHost, st));
+    if (a->n_heads) B200_CUDA(cudaMemcpyAsync(a->h_extra, a->extra, B * a->n_heads * 4, cudaMemcpyDeviceToHost, st));
+  }
+  B200_CUDA(cudaMemcpyAsync(a->h_flags, a->flags, 2 * B, cudaMemcpyDeviceToHost, st));
+  B200_CUDA(cudaEventRecord(a->done, st));
+  B200_CUDA(cudaEventSynchronize(a->done));    // the frame's only host wait
+  for (size_t b = 0; b < B; ++b) {
+    if (!a->h_flags[B + b]) continue;
+    flags_inout_host[b] = a->h_flags[b];
+    if (a->h_flags[b] == B200_ASR_IS_EOS) a->h_active[b] = 0;
+  }
+  if (!any_active) return B200_OK;
+  memcpy(tokens_out_host, a->h_tokens, B * 8);
+  if (a->n_heads) memcpy(extra_heads_out_host, a->h_extra, B * a->n_heads * 4);
+  if (ran) *ran = 1;
+  return lm_check_kv_pool(a->lm);
 }
 
 }  // extern "C"

@@ -565,6 +565,13 @@ int lm_check_kv_pool(b200_lm* h) {
   B200_CUDA(cudaStreamSynchronize(h->stream));
   B200_FAIL(B200_ERR_STATE, "frame_step: a session's KV ring did not get a page: the KV pool of %d pages is full (flags %d)", h->n_pages, v);
 }
+
+int lm_frame_view(b200_lm* h, LmFrameView* v) {
+  B200_TRY(ensure_streaming(h, "lm_frame_view"));
+  const auto& c = h->cfg;
+  *v = LmFrameView{h->batch, h->MB, c.n_q, c.dep_q, h->max_delay, (int)h->extra_w.size(), c.extra_heads_dim, h->extra_out};
+  return B200_OK;
+}
 }  // namespace b200
 
 extern "C" {

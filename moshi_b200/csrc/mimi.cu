@@ -661,6 +661,12 @@ int plan_layer(b200_mimi* h, mtc::TcLayer& L, const float* in_hi, const float* i
 
 }  // namespace
 
+int b200::mimi_frame_view(b200_mimi* h, MimiFrameView* v) {
+  B200_TRY(ensure_streaming(h, "mimi_frame_view"));
+  *v = MimiFrameView{h->batch, h->num_codebooks, h->frame_size};
+  return B200_OK;
+}
+
 // =============================================================================================
 // C ABI
 // =============================================================================================

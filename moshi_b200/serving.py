@@ -195,6 +195,127 @@ class DialogueService:
             self._np_ptr(flags_out, np.uint8, B, "flags_out")))
 
 
+MASK_ACTIVE, MASK_MARKER_RECEIVED, MASK_IS_EOS = 1, 2, 4     # MaskFlags of rust/moshi-server/batched_asr.py:14-20
+
+
+class ASRService:
+    """``ASRService`` of ``rust/moshi-server/batched_asr.py:100-213`` for the speech-to-text models (``dep_q = 0``, extra heads),
+    with its calling convention: ``step(batch_pcm, flags_out, tokens_out, extra_heads, updates)`` every 80 ms for all slots,
+    numpy buffers in and out, as ``py_basr_module.rs`` calls it.  The per-slot client state (``ClientState``, :85-98) and the
+    end-of-stream countdown live on the device; a frame (updates -> resets -> ``mimi.encode`` -> ``step_with_extra_heads`` ->
+    flags) is one stream-ordered chain with a single host wait (``b200_asr_step``).  Construction runs the reference's warm-up
+    (:119-130); afterwards every slot is inactive until its first ``ACTIVE`` or ``RESET``."""
+
+    def __init__(self, batch_size: int, lm, mimi, asr_delay_in_tokens: int = 32, temp: float = 0.0, kv_dtype: str = "bf16",
+                 kv_capacity: int | None = None, kv_pool_frames: int | None = None):
+        import ctypes as C
+
+        import numpy as np
+
+        from . import _lib
+        from .models import LMGen
+        self.batch_size = batch_size
+        self.lm, self.mimi = lm, mimi
+        self.asr_delay_in_tokens = asr_delay_in_tokens
+        self.lm_gen = LMGen(lm, temp_text=temp)                     # batched_asr.py:114
+        self.lm_gen.kv_dtype = kv_dtype
+        self.lm_gen.kv_capacity = kv_capacity
+        self.lm_gen.kv_pool_frames = kv_pool_frames
+        self._lib = _lib.lib()
+        self._h = C.c_void_p()
+        self.lm_gen.streaming_forever(batch_size)
+        try:
+            self.mimi.streaming_forever(batch_size)
+        except BaseException:
+            self.lm_gen._stop()
+            raise
+        try:
+            with torch.cuda.device(lm.device):
+                _lib.check(self._lib.b200_asr_create(mimi._h, lm._h, batch_size, int(asr_delay_in_tokens),
+                                                     _lib.current_stream(lm.device), C.byref(self._h)))
+        except BaseException:
+            self._h = None
+            self.lm_gen._stop()
+            self.mimi._stop()
+            raise
+        self.frame_size = mimi.frame_size
+        self.extra_heads_num_heads = lm.cfg.extra_heads_num_heads
+        self._tokens = np.zeros(batch_size, dtype=np.int64)
+
+    def read_buffer(self, name: str, dtype: torch.dtype, shape: tuple) -> torch.Tensor:
+        """Buffers of the last frame (``b200_asr_read_buffer``): "codes_in", "tokens", "extra_heads", "exec", "reset", "offset",
+        "real_end"."""
+        import ctypes as C
+
+        from . import _lib
+        out = torch.empty(shape, dtype=dtype, device=self.lm.device)
+        n = C.c_int64()
+        _lib.check(self._lib.b200_asr_read_buffer(self._h, name.encode(), _lib.ptr(out), out.numel() * out.element_size(), C.byref(n)))
+        assert n.value == out.numel() * out.element_size(), (name, n.value, shape)
+        return out
+
+    def release(self, slots) -> None:
+        """Resets the LM and Mimi rows of closed session slots, so that a paged LM (``kv_pool_frames``) returns their KV pages to
+        the pool now.  The slot's client state is left as it is: its next session still starts with ``RESET``."""
+        mask = torch.zeros(self.batch_size, dtype=torch.bool)
+        mask[list(slots)] = True
+        if mask.any():
+            self.lm_gen.reset_streaming(mask)
+            self.mimi.reset_streaming(mask)
+
+    def export_session(self, slot: int) -> SessionRecord:
+        """The LM and Mimi state of session ``slot`` as device records (see ``DialogueService.export_session``).  The client
+        state (offset, end-of-stream countdown) does not travel: move a session before it sends its end-of-stream marker."""
+        return SessionRecord(self.lm_gen.export_session(slot), self.mimi.export_session(slot))
+
+    def import_session(self, slot: int, record: SessionRecord) -> None:
+        """Continues a session exported from another service in ``slot``; its next update must be ``ACTIVE`` (``RESET`` would
+        erase it).  The LM record is checked and imported first: if it is refused, nothing changes."""
+        self.lm_gen.import_session(slot, record.lm)
+        self.mimi.import_session(slot, record.mimi)
+
+    def close(self) -> None:
+        if getattr(self, "_h", None):
+            self._lib.b200_asr_destroy(self._h)
+            self._h = None
+            self.lm_gen._stop()
+            self.mimi._stop()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def step(self, batch_pcm, flags_out, tokens_out, extra_heads, updates) -> bool:
+        """``ASRService.step`` (batched_asr.py:132-213).  ``batch_pcm`` f32 [B * frame_size]; ``flags_out`` u8 [B], read and
+        written (entries the reference does not assign keep their value); ``tokens_out`` any integer dtype [B], assigned like the
+        reference (``tokens_out[:] = ...``: -2 wraps in an unsigned array); ``extra_heads`` f32 [B, extra_heads_num_heads];
+        ``updates`` B ints (NODATA / ACTIVE / RESET, or a positive end-of-stream marker).  Returns whether the model ran: when
+        no slot is active, tokens and extra heads are not written."""
+        import ctypes as C
+
+        import numpy as np
+
+        from . import _lib
+        B, n = self.batch_size, self.extra_heads_num_heads
+        upd = np.ascontiguousarray(np.asarray(updates, dtype=np.int32))
+        assert upd.shape == (B,), f"expected {B} slot updates"
+        assert isinstance(tokens_out, np.ndarray) and tokens_out.shape == (B,) and np.issubdtype(tokens_out.dtype, np.integer), \
+            f"tokens_out: expected an integer array of shape ({B},)"
+        assert isinstance(extra_heads, np.ndarray) and extra_heads.shape == (B, n), f"extra_heads: expected shape ({B}, {n})"
+        ran = C.c_int(0)
+        _np = DialogueService._np_ptr
+        with torch.cuda.device(self.lm.device):
+            _lib.check(self._lib.b200_asr_step(
+                self._h, _np(batch_pcm, np.float32, B * self.frame_size, "batch_pcm"), _np(upd, np.int32, B, "updates"),
+                _np(flags_out, np.uint8, B, "flags_out"), _np(self._tokens, np.int64, B, "tokens"),
+                _np(extra_heads, np.float32, B * n, "extra_heads") if n else C.c_void_p(0), C.byref(ran)))
+        if ran.value:
+            tokens_out[:] = self._tokens
+        return bool(ran.value)
+
+
 class SessionPool:
     """Slot allocator and PCM framing in front of ``DialogueService.step`` (host logic only; no device work).
 
