@@ -208,6 +208,20 @@ int b200_lm_set_cfg(b200_lm* h, float cfg_coef, int cfg_is_no_text, const int64_
  * [rows = batch (2 * batch with CFG)][dim], added to the summed input embeddings of every step.  NULL switches it off.
  * While streaming; the tensor is copied.  (Evaluating the conditioners themselves is per-session work outside the step.) */
 int b200_lm_set_condition_sum(b200_lm* h, const void* sum_bf16_dev, int rows);
+/* Cross-attention conditioning (LMModel(cross_attention=True), transformer.py:727-732, 779-798): every temporal layer runs
+ * x = x + cross_attention(norm_cross(x), condition) between its self-attention and its MLP, the query from x, keys and values
+ * from a per-row condition memory.  Before finalize; the layers then need "transformer.layers.<i>.cross_attention.in_projs.0
+ * .weight" [3*dim,dim], ".cross_attention.out_projs.0.weight" [dim,dim] and ".norm_cross.weight" / ".norm_cross.bias" [dim].
+ * Not with quantize (B200_ERR_INVALID). */
+int b200_lm_set_cross_attention(b200_lm* h, int enable);
+/* Keys T of every row's condition memory (k_cross / v_cross bf16 [MB,H,T,128] per layer, allocated at streaming_begin).
+ * Before streaming_begin; a cross-attention handle cannot stream without it. */
+int b200_lm_set_cross_len(b200_lm* h, int keys);
+/* _MHAState.k_cross / v_cross of model rows rows_host[0..n_rows) (b, and batch + b under CFG): K and V = condition @
+ * in_projs.0.weight[dim:]^T of every layer (transformer.py:495-505) for condition bf16 [n_rows,T,dim] (fuser.get_cross of
+ * lm.py:616-627, one row per model row).  rows_host NULL: all MB rows, n_rows = MB.  While streaming, on the handle's stream,
+ * outside the step; the other rows' memory and every row's position are unchanged (a reset keeps the memory). */
+int b200_lm_set_condition_cross(b200_lm* h, const void* src_bf16_dev, const int32_t* rows_host, int n_rows);
 /* Seed of the Exp(1) noise the step draws itself when the caller passes noise = NULL with sampling on (sampling.py:44 draws
  * it from torch's generator; here a Philox4x32-10 stream keyed by (seed, step counter) inside the step's CUDA graph). */
 int b200_lm_seed_noise(b200_lm* h, uint64_t seed);
@@ -250,7 +264,9 @@ int b200_lm_step_host(b200_lm* h, const int64_t* in_codes_host, int n_in, const 
  * (b200_lm_set_taps), the temporal transformer of the last step: "temporal.embed" bf16 [MB,dim] (the summed input embeddings
  * entering layer 0) and per layer l "temporal.layers.<l>.attn_out" bf16 [MB,dim] (the attention output, before out_proj),
  * ".x_attn" [MB,dim] (x after the attention residual), ".gated" [MB,ffn_hidden] (silu(gate) * value) and ".x_out" [MB,dim]
- * (x after the MLP residual); B200_ERR_STATE if the taps were never turned on while streaming. */
+ * (x after the MLP residual); on a cross-attention handle also ".cross_out" [MB,dim] (the cross-attention output, before its
+ * out_proj) and ".x_cross" [MB,dim] (x after the cross-attention residual); B200_ERR_STATE if the taps were never turned on
+ * while streaming. */
 int b200_lm_read_buffer(b200_lm* h, const char* name, void* dst_dev, int64_t capacity_bytes, int64_t* nbytes);
 /* Test taps of the temporal transformer (read through b200_lm_read_buffer "temporal.*"): when on, every step also copies the
  * embeddings and each layer's four activations into per-layer buffers, on the step's stream.  Needs streaming; the buffers
@@ -505,6 +521,13 @@ int b200_op_mimi_ring_attn(const float* qkv_dev, float* k_dev, float* v_dev, flo
 /* RMSNorm of the LM (transformer.py:45-58, eps 1e-8): y = bf16(x * alpha * rsqrt(eps + mean(x^2))), x / y bf16 [M,dim],
  * alpha bf16 [dim], dim even. */
 int b200_op_rmsnorm(const void* x_dev, const void* alpha_dev, void* y_dev, int M, int dim, void* stream);
+/* LayerNorm of the cross-attention layers (norm_cross, nn.LayerNorm eps 1e-5): y = bf16((x - mean) * rstd * w + b) with fp32
+ * statistics, x / y bf16 [M,dim], w / b bf16 [dim], dim even. */
+int b200_op_layernorm(const void* x_dev, const void* w_dev, const void* b_dev, void* y_dev, int M, int dim, void* stream);
+/* One cross-attention step, as the LM launches it: q bf16 [B,H*128], attention over all T keys of k / v bf16 [B,H,T,128]
+ * (no RoPE, no mask), out bf16 [B,H*128].  nsplit <= 0: the LM's choice of splits. */
+int b200_op_cross_attn_step(const void* q_dev, const void* k_dev, const void* v_dev, void* out_dev, int B, int H, int T, int nsplit,
+                            void* stream);
 /* b200_op_linear_sk on rmsnorm(x, alpha) with the norm folded into the GEMV kernel's activation staging (the LM's path for one
  * or two sessions).  Only the GEMV path takes a norm: for M above b200_op_set_gemv_max_rows it returns B200_ERR_STATE. */
 int b200_op_linear_sk_norm(const void* x_dev, const void* alpha_dev, const void* w_tiles_dev, void* y_dev, const void* res_dev, int M,

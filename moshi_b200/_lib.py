@@ -109,6 +109,9 @@ _PROTOTYPES: dict[str, tuple[tp.Any, list]] = {
     "b200_lm_session_import": (_I, [_P, _I, _P, C.c_int64]),
     "b200_lm_set_cfg": (_I, [_P, C.c_float, _I, _P, _I]),
     "b200_lm_set_condition_sum": (_I, [_P, _P, _I]),
+    "b200_lm_set_cross_attention": (_I, [_P, _I]),
+    "b200_lm_set_cross_len": (_I, [_P, _I]),
+    "b200_lm_set_condition_cross": (_I, [_P, _P, _P, _I]),
     "b200_lm_seed_noise": (_I, [_P, C.c_uint64]),
     "b200_lm_set_stream": (_I, [_P, _P]),
     "b200_lm_state_count": (_I, [_P]),
@@ -148,6 +151,8 @@ _PROTOTYPES: dict[str, tuple[tp.Any, list]] = {
     "b200_op_dep_attn_step": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "b200_op_mimi_ring_attn": (_I, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, C.c_float, _P]),
     "b200_op_rmsnorm": (_I, [_P, _P, _P, _I, _I, _P]),
+    "b200_op_layernorm": (_I, [_P, _P, _P, _P, _I, _I, _P]),
+    "b200_op_cross_attn_step": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "b200_op_linear_sk_norm": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "b200_op_sample": (_I, [_P, _P, _P, _I, _I, _I, C.c_float, _I, _P]),
     "b200_op_lm_noise": (_I, [_P, C.c_int64, C.c_uint64, C.c_uint64, _P]),

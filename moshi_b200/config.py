@@ -166,7 +166,8 @@ class LMConfig:
     extra_heads_num_heads: int = 0   # lm.py:108-109, 224-226: nn.Linear(dim, extra_heads_dim) heads on the temporal output (STT)
     extra_heads_dim: int = 6
     # lm.py:110-118 via loaders.get_conditioner_provider / get_condition_fuser (loaders.py:449-487): the JSON's "conditioners"
-    # and "fuser" sections (configs/moshi_dev_2b.json).  Only LUT conditioners fused by "sum" are on the step path.
+    # and "fuser" sections (configs/moshi_dev_2b.json).  LUT conditioners fused by "sum", and tensor conditioners fused by
+    # "cross" into the temporal layers' cross-attention (cross_attention=True, the TTS models) are on the step path.
     conditioners: tp.Optional[dict] = None
     fuser: tp.Optional[dict] = None
     cross_attention: bool = False
@@ -233,11 +234,19 @@ class LMConfig:
             bad.append("causal=False")
         if self.dep_q and self.depformer_context < self.dep_q:
             bad.append("depformer_context < dep_q (the depformer attends over all of a frame's codebooks)")
-        if self.cross_attention or (self.fuser or {}).get("cross") or (self.fuser or {}).get("prepend"):
-            bad.append("cross-attention / prepend conditioning (only fuser.sum is on the step path)")
+        fuser = self.fuser or {}
+        if fuser.get("prepend"):
+            bad.append("prepend conditioning (only fuser.sum and fuser.cross are on the step path)")
+        if fuser.get("cross") and not self.cross_attention:     # the reference fails at the first step (transformer.py:786)
+            bad.append("fuser.cross on a model without cross_attention")
+        if self.cross_attention and self.quantize:              # _compute_cross_attention asserts an nn.Linear in_proj
+            bad.append("cross_attention with quantize=True")
         for name, c in (self.conditioners or {}).items():
-            if c.get("type") != "lut":
-                bad.append(f"conditioner {name!r} of type {c.get('type')!r} (only 'lut')")
+            if c.get("type") == "tensor":
+                if name not in (fuser.get("cross") or []):
+                    bad.append(f"tensor conditioner {name!r} that no fuser.cross consumes")
+            elif c.get("type") != "lut":
+                bad.append(f"conditioner {name!r} of type {c.get('type')!r} (only 'lut' and 'tensor')")
         if not 0 <= self.dep_q <= 16 or not 1 <= self.n_q <= 32 or self.dep_q > self.n_q:
             bad.append("n_q / dep_q (n_q <= 32, 0 <= dep_q <= 16)")
         if self.dim % self.num_heads or (self.dep_q and self.depformer_dim % self.depformer_num_heads):

@@ -15,6 +15,10 @@ struct TLayer {
   bf16 *kc = nullptr, *vc = nullptr;
   uint8_t *kc8 = nullptr, *vc8 = nullptr;      // opt-in fp8 ring: e4m3 bytes [B][H][cap][D] ...
   float *ks = nullptr, *vs = nullptr;          // ... and one scale per (session, head, slot)
+  // cross-attention layers (b200_lm_set_cross_attention): norm_cross, the query / K|V / output linears, and the condition memory
+  // k_cross / v_cross [MB][H][cross_len][ATT_D] bf16
+  const bf16 *ncw = nullptr, *ncb = nullptr, *cq_w = nullptr, *ckv_w = nullptr, *co_w = nullptr;
+  bf16 *kx = nullptr, *vx = nullptr;
 };
 struct DLayer {
   std::vector<const bf16*> in_w, out_w, lin_in, lin_out;   // one per depformer step
@@ -41,6 +45,12 @@ void b200::lm::attn_step_launch(const bf16* qkv, const KvRings& r, bf16* out, fl
                    r.table, r.tab_ld, r.page_shift};
   if (r.table) B200_LAUNCH(attn_step_kernel<true>, grid, ATT_THREADS, 0, st, a);
   else B200_LAUNCH(attn_step_kernel<false>, grid, ATT_THREADS, 0, st, a);
+}
+
+void b200::lm::cross_attn_launch(const bf16* q, long long ldq, const bf16* kc, const bf16* vc, bf16* out, float* part, int* counters,
+                                 int B, int H, int T, int nsplit, cudaStream_t st) {
+  const CrossAttnStep a{q, ldq, kc, vc, out, part, counters, H, T, nsplit};
+  B200_LAUNCH(cross_attn_step_kernel, dim3(B * H, nsplit), ATT_THREADS, 0, st, a);
 }
 
 struct b200_lm {
@@ -122,6 +132,12 @@ struct b200_lm {
   // b200_lm_set_taps: the step copies the temporal stack's activations into taps (see tap_slot), allocated on first enable
   int taps_on = 0;
   bf16* taps = nullptr;
+  // cross-attention conditioning (transformer.py:727-732, 779-798): every temporal layer attends to its row's condition memory
+  int cross_on = 0;                            // b200_lm_set_cross_attention, before finalize
+  int cross_len = 0;                           // b200_lm_set_cross_len: keys per condition memory, before streaming_begin
+  int cross_nsplit = 1;
+  bf16 *cross_src = nullptr, *cross_kv = nullptr;      // fill staging: [CROSS_CHUNK][dim] rows of the condition, their K|V
+  int* cross_rows = nullptr;                   // [MB] model rows of the condition rows being filled
   int n_in_static = 0;
   int noise_static = 0;                        // 1: the captured step draws its own noise
   int replace_static = 0;                      // 1: this step's audio tokens are given (depformer_replace_tokens, lm.py:751-755)
@@ -251,6 +267,18 @@ int get_linear(b200_lm* h, const std::string& name, int N, int K, int epi, int g
   return B200_OK;
 }
 
+// A bf16 weight [N][K] already on the device (a slice of a loaded tensor) -> packed tiles; the caller releases the tensor
+int pack_bf16(b200_lm* h, const bf16* w, int N, int K, int epi, const bf16** out) {
+  void* packed = nullptr;
+  B200_TRY(h->weights.alloc(&packed, tc::sk_packed_bytes(N, K, epi, 0), false));
+  B200_TRY(tc::sk_pack_weights(w, packed, N, K, epi, 0, nullptr));
+  *out = static_cast<const bf16*>(packed);
+  return B200_OK;
+}
+
+// condition rows (x T keys) per K/V projection GEMM of b200_lm_set_condition_cross: the LM GEMMs take at most 256 rows
+constexpr int CROSS_CHUNK = 256;
+
 // logits [MB][card] of the model -> the [batch][card] rows the sampler reads: the conditioned rows themselves, or (CFG) the
 // guided combination written to `guided`
 const bf16* guide(b200_lm* h, const bf16* logits, bf16* guided, int card, bool combine) {
@@ -277,18 +305,19 @@ TokenRing ring(b200_lm* h) {
 
 // Taps of the temporal stack: the summed embeddings, then per layer the attention output [MB][dim], x after the attention
 // residual [MB][dim], the gated hidden [MB][ffn_hidden] and x after the MLP residual [MB][dim].
-enum TapKind { TAP_ATTN_OUT, TAP_X_ATTN, TAP_GATED, TAP_X_OUT };
+// Cross-attention handles add, after those four, the cross-attention output [MB][dim] and x after the cross residual [MB][dim].
+enum TapKind { TAP_ATTN_OUT, TAP_X_ATTN, TAP_GATED, TAP_X_OUT, TAP_CROSS_OUT, TAP_X_CROSS };
 int64_t tap_elems(const b200_lm* h) {
   const int64_t MB = h->MB, d = h->cfg.dim;
-  return MB * d + (int64_t)h->layers.size() * MB * (3 * d + h->cfg.ffn_hidden);
+  return MB * d + (int64_t)h->layers.size() * MB * ((h->cross_on ? 5 : 3) * d + h->cfg.ffn_hidden);
 }
 // first element of a tap (layer -1: the embeddings) and its element count
 int64_t tap_slot(const b200_lm* h, int layer, int kind, int64_t* n) {
   const int64_t MB = h->MB, d = h->cfg.dim, F = h->cfg.ffn_hidden;
   *n = kind == TAP_GATED ? MB * F : MB * d;
   if (layer < 0) return 0;
-  const int64_t at[4] = {0, MB * d, 2 * MB * d, 2 * MB * d + MB * F};
-  return MB * d + (int64_t)layer * MB * (3 * d + F) + at[kind];
+  const int64_t at[6] = {0, MB * d, 2 * MB * d, 2 * MB * d + MB * F, 3 * MB * d + MB * F, 4 * MB * d + MB * F};
+  return MB * d + (int64_t)layer * MB * ((h->cross_on ? 5 : 3) * d + F) + at[kind];
 }
 // device-to-device copy on the step's stream (a memcpy node of the captured graph); nothing when taps are off
 int tap(b200_lm* h, const bf16* src, int layer, int kind) {
@@ -335,6 +364,14 @@ int step_body(b200_lm* h) {
     B200_TRY(tap(h, h->ao, (int)l, TAP_ATTN_OUT));
     B200_TRY(linear(h, h->ao, d, L.out_w, h->x, d, h->x, d, MB, d, d, LIN_RESADD, 0, L.out_s));
     B200_TRY(tap(h, h->x, (int)l, TAP_X_ATTN));
+    if (h->cross_on) {     // x = x + cross_attention(norm_cross(x), condition memory) (transformer.py:779-798)
+      B200_LAUNCH(layernorm_kernel, MB, 256, 0, st, h->x, L.ncw, L.ncb, h->xn, d, 1e-5f);
+      B200_TRY(linear(h, h->xn, d, L.cq_w, h->qkv, d, nullptr, 0, MB, d, d, LIN_STORE, 0));
+      cross_attn_launch(h->qkv, d, L.kx, L.vx, h->ao, h->attn_part, h->attn_counters, MB, H, h->cross_len, h->cross_nsplit, st);
+      B200_TRY(tap(h, h->ao, (int)l, TAP_CROSS_OUT));
+      B200_TRY(linear(h, h->ao, d, L.co_w, h->x, d, h->x, d, MB, d, d, LIN_RESADD, 0));
+      B200_TRY(tap(h, h->x, (int)l, TAP_X_CROSS));
+    }
     B200_TRY(norm_linear(h, h->x, L.n2, h->xn, L.lin_in, h->hbuf, F, MB, F, d, LIN_GATE, F, L.lin_in_s));
     B200_TRY(tap(h, h->hbuf, (int)l, TAP_GATED));
     B200_TRY(linear(h, h->hbuf, F, L.lin_out, h->x, d, h->x, d, MB, d, F, LIN_RESADD, 0, L.lin_out_s));
@@ -503,18 +540,27 @@ int read_positions(b200_lm* h, const void* src_dev, std::vector<long long>* pos)
 // model.exec_mask (2 rows) and cfg_is_masked_until, and while it is on the condition_sum rows, each 16-byte aligned (the
 // RowSlice table of streaming_begin).  From the next 256-byte boundary, the temporal K/V of slots [0, n), n = min(pos, ring
 // capacity), slot s being position s mod capacity: [layer][k|v][model row][head][n][128] bf16, or for 8-bit rings the bytes in
-// that layout followed by the fp32 scales [layer][k|v][model row][head][n].
+// that layout followed by the fp32 scales [layer][k|v][model row][head][n].  A cross-attention handle's record (SESSION_CROSS, the
+// memory's key count T in the header's first reserved bytes) ends, from the next 256-byte boundary, with the session's condition
+// memory [layer][k|v][model row][head][T][128] bf16.
 struct SessionPlan {
   int rows = 1;
   int64_t pos[2] = {0, 0};
-  int64_t n = 0, kv_off = 0, bytes = 0;
+  int64_t n = 0, kv_off = 0, cross_off = 0, bytes = 0;
   bool cond = false;
 };
+
+// bytes of one model row's condition memory in one layer (K or V)
+int64_t cross_row_bytes(const b200_lm* h) { return (int64_t)h->cfg.num_heads * h->cross_len * ATT_D * 2; }
 
 void session_size(const b200_lm* h, SessionPlan* p) {
   const long long end = p->cond ? h->slices_end_cond : h->slices_end;
   p->kv_off = (end + 255) / 256 * 256;
   p->bytes = p->kv_off + (int64_t)h->cfg.num_layers * 2 * h->cfg.num_heads * kv_row_bytes(h) * p->rows * p->n;
+  if (h->cross_on) {
+    p->cross_off = (p->bytes + 255) / 256 * 256;
+    p->bytes = p->cross_off + (int64_t)h->cfg.num_layers * 2 * p->rows * cross_row_bytes(h);
+  }
 }
 
 uint64_t lm_fingerprint(const b200_lm* h) { return config_fingerprint(&h->cfg, sizeof(h->cfg)); }
@@ -544,6 +590,16 @@ int session_kv(b200_lm* h, int row, const SessionPlan& p, char* rec, bool gather
   if (h->kv_fp8) {
     const int64_t scales = p.kv_off + (int64_t)L2 * p.rows * h->cfg.num_heads * p.n * ATT_D;
     B200_TRY(kv_copy(h, L2, L2, row, p.rows, h->batch, (int)p.n, rec + scales, gather, true));
+  }
+  if (h->cross_on) {         // the condition memory of the session's model rows, each contiguous [H][T][128]
+    const int64_t rb = cross_row_bytes(h);
+    char* at = rec + p.cross_off;
+    for (auto& L : h->layers)
+      for (bf16* m : {L.kx, L.vx})
+        for (int k = 0; k < p.rows; ++k, at += rb) {
+          char* mem = reinterpret_cast<char*>(m) + (int64_t)(row + k * h->batch) * rb;
+          B200_CUDA(cudaMemcpyAsync(gather ? at : mem, gather ? mem : at, (size_t)rb, cudaMemcpyDeviceToDevice, h->stream));
+        }
   }
   return B200_OK;
 }
@@ -621,6 +677,8 @@ int b200_lm_finalize(b200_lm* h) {
   if (h->finalized) return B200_OK;
   const auto& c = h->cfg;
   const int d = c.dim, dd = c.depformer_dim, F = c.ffn_hidden, dF = c.depformer_ffn_hidden;
+  if (h->cross_on && c.quantize)      // the reference's _compute_cross_attention asserts an nn.Linear in_proj
+    B200_FAIL(B200_ERR_INVALID, "lm_finalize: cross-attention layers with quantize=True (int8 linears) are not supported");
   h->emb.n_q = c.n_q; h->emb.card = c.card; h->emb.text_card = c.text_card; h->emb.condition_sum = nullptr; h->emb.err = nullptr;
   DeviceGuard guard_dev(h->device);
   for (int k = 0; k < c.n_q; ++k)
@@ -638,6 +696,19 @@ int b200_lm_finalize(b200_lm* h) {
     B200_TRY(get_bf16(h, p + ".norm2.alpha", {1, 1, d}, &L.n2));
     B200_TRY(get_linear(h, p + ".gating.linear_in.weight", 2 * F, d, LIN_GATE, F, &L.lin_in, &L.lin_in_s));
     B200_TRY(get_linear(h, p + ".gating.linear_out.weight", d, F, LIN_RESADD, 0, &L.lin_out, &L.lin_out_s));
+    if (h->cross_on) {      // transformer.py:495-505, 727-732: in_projs.0 rows [0, d) the query, [d, 3d) K|V of the condition
+      const std::string x = p + ".cross_attention.in_projs.0.weight";
+      const bf16* w = nullptr;
+      const float* no_scales = nullptr;
+      B200_TRY(get_bf16(h, x, {3 * d, d}, &w));
+      B200_TRY(pack_bf16(h, w, d, d, LIN_STORE, &L.cq_w));
+      B200_TRY(pack_bf16(h, w + (size_t)d * d, 2 * d, d, LIN_STORE, &L.ckv_w));
+      B200_CUDA(cudaStreamSynchronize(nullptr));
+      h->store.release(x);
+      B200_TRY(get_linear(h, p + ".cross_attention.out_projs.0.weight", d, d, LIN_RESADD, 0, &L.co_w, &no_scales));
+      B200_TRY(get_bf16(h, p + ".norm_cross.weight", {d}, &L.ncw));
+      B200_TRY(get_bf16(h, p + ".norm_cross.bias", {d}, &L.ncb));
+    }
   }
   for (int i = 0; i < c.extra_heads_num_heads; ++i) {      // lm.py:224-226
     const bf16* w = nullptr;
@@ -816,7 +887,11 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
     h->n_pages = (int)std::min(ceil_div64(h->pool_frames, h->page_slots), (int64_t)MB * h->tab_ld);
   }
   const size_t ring_slots = h->n_pages ? (size_t)(h->n_pages + 1) * h->page_slots : (size_t)MB * cap;   // per layer and head
-  const size_t kv_bytes = (size_t)c.num_layers * 2 * ring_slots * H * kv_row_bytes(h);
+  if (h->cross_on && h->cross_len < 1)
+    B200_FAIL(B200_ERR_STATE, "lm_streaming_begin: set the condition memory's length (b200_lm_set_cross_len) first");
+  // the cross-attention handle's condition memory: K and V [MB][H][T][128] bf16 per layer
+  const size_t cross_bytes = h->cross_on ? (size_t)c.num_layers * 2 * MB * h->cross_len * d * 2 : 0;
+  const size_t kv_bytes = (size_t)c.num_layers * 2 * ring_slots * H * kv_row_bytes(h) + cross_bytes;
   if (kv_bytes + (1ull << 30) > free_b)
     B200_FAIL(B200_ERR_INVALID, "lm_streaming_begin: %d sessions need %.1f GB of KV ring, %.1f GB free", B, kv_bytes / 1e9,
               free_b / 1e9);
@@ -853,6 +928,15 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
       B200_TRY(A.alloc_t(&L.kc, ring_slots * H * D));
       B200_TRY(A.alloc_t(&L.vc, ring_slots * H * D));
     }
+    if (h->cross_on) {
+      B200_TRY(A.alloc_t(&L.kx, (size_t)MB * H * h->cross_len * D));
+      B200_TRY(A.alloc_t(&L.vx, (size_t)MB * H * h->cross_len * D));
+    }
+  }
+  if (h->cross_on) {
+    B200_TRY(A.alloc_t(&h->cross_src, (size_t)CROSS_CHUNK * d, false));
+    B200_TRY(A.alloc_t(&h->cross_kv, (size_t)CROSS_CHUNK * 2 * d, false));
+    B200_TRY(A.alloc_t(&h->cross_rows, MB, false));
   }
   if (h->n_pages) {
     B200_TRY(A.alloc_t(&h->page_table, (size_t)MB * h->tab_ld, false));
@@ -903,11 +987,13 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
   B200_TRY(A.alloc_t(&h->dao, (size_t)MB * dd));
   B200_TRY(A.alloc_t(&h->dh, (size_t)MB * c.depformer_ffn_hidden));
   B200_TRY(A.alloc_t(&h->dep_logits, (size_t)MB * dq1 * c.card));
-  B200_TRY(A.alloc(reinterpret_cast<void**>(&h->sk_ws), tc::sk_workspace_bytes(MB), false));
+  // (the condition memory's K/V projection runs CROSS_CHUNK rows at a time)
+  B200_TRY(A.alloc(reinterpret_cast<void**>(&h->sk_ws), tc::sk_workspace_bytes(h->cross_on ? std::max(MB, CROSS_CHUNK) : MB), false));
   B200_TRY(A.alloc_t(&h->sk_counters, tc::SK_MAX_TILES));
   const int ns = attn_pick_splits(MB, H, cap);
   h->nsplit = ns;
-  B200_TRY(A.alloc_t(&h->attn_part, (size_t)MB * H * ns * (ATT_D + 2)));
+  h->cross_nsplit = h->cross_on ? attn_pick_splits(MB, H, h->cross_len) : 1;      // the cross step shares the partials
+  B200_TRY(A.alloc_t(&h->attn_part, (size_t)MB * H * (h->cross_on ? std::max(ns, h->cross_nsplit) : ns) * (ATT_D + 2)));
   B200_TRY(A.alloc_t(&h->attn_counters, (size_t)MB * H));
   B200_CUDA(cudaStreamCreateWithFlags(&h->gstream, cudaStreamNonBlocking));
   B200_CUDA(cudaEventCreateWithFlags(&h->ev_in, cudaEventDisableTiming));
@@ -977,6 +1063,13 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
       A.mark_state(L.kc, (size_t)MB * H * cap * D * 2, p + ".k", B200_BF16, {MB, H, cap, D});
       A.mark_state(L.vc, (size_t)MB * H * cap * D * 2, p + ".v", B200_BF16, {MB, H, cap, D});
     }
+  }
+  for (size_t l = 0; h->cross_on && l < h->layers.size(); ++l) {     // _MHAState.k_cross / v_cross (transformer.py:321-327)
+    auto& L = h->layers[l];
+    const std::string p = "layers." + std::to_string(l);
+    const int T = h->cross_len;
+    A.mark_state(L.kx, (size_t)MB * H * T * D * 2, p + ".k_cross", B200_BF16, {MB, H, T, D});
+    A.mark_state(L.vx, (size_t)MB * H * T * D * 2, p + ".v_cross", B200_BF16, {MB, H, T, D});
   }
   {
     std::vector<void*> arrays;
@@ -1172,6 +1265,56 @@ int b200_lm_set_condition_sum(b200_lm* h, const void* sum_bf16_dev, int rows) {
   return B200_OK;
 }
 
+int b200_lm_set_cross_attention(b200_lm* h, int enable) {
+  if (!h) B200_FAIL(B200_ERR_INVALID, "lm_set_cross_attention: null handle");
+  if (h->finalized) B200_FAIL(B200_ERR_STATE, "lm_set_cross_attention: the layers' weights are packed at finalize; set it before");
+  if (enable && h->cfg.quantize)
+    B200_FAIL(B200_ERR_INVALID, "lm_set_cross_attention: cross-attention layers with quantize=True (int8 linears) are not supported");
+  h->cross_on = enable ? 1 : 0;
+  return B200_OK;
+}
+
+int b200_lm_set_cross_len(b200_lm* h, int keys) {
+  if (!h) B200_FAIL(B200_ERR_INVALID, "lm_set_cross_len: null handle");
+  if (!h->cross_on) B200_FAIL(B200_ERR_INVALID, "lm_set_cross_len: the model has no cross-attention layers");
+  if (h->batch > 0) B200_FAIL(B200_ERR_STATE, "lm_set_cross_len: the condition memory is allocated at streaming_begin; set it before");
+  if (keys < 1 || keys > (1 << 20)) B200_FAIL(B200_ERR_INVALID, "lm_set_cross_len: %d keys", keys);
+  h->cross_len = keys;
+  return B200_OK;
+}
+
+int b200_lm_set_condition_cross(b200_lm* h, const void* src_bf16_dev, const int32_t* rows_host, int n_rows) {
+  B200_TRY(ensure_streaming(h, "lm_set_condition_cross"));
+  DeviceGuard g(h->device);
+  if (!h->cross_on) B200_FAIL(B200_ERR_INVALID, "lm_set_condition_cross: the model has no cross-attention layers");
+  if (!src_bf16_dev || n_rows < 1 || n_rows > h->MB) B200_FAIL(B200_ERR_INVALID, "lm_set_condition_cross: %d condition rows", n_rows);
+  if (!rows_host && n_rows != h->MB)       // lm.py:650-651: "cfg requires 2x more conditions"
+    B200_FAIL(B200_ERR_SHAPE, "lm_set_condition_cross: %d rows given, the model runs on %d", n_rows, h->MB);
+  std::vector<int> rows(n_rows);
+  for (int k = 0; k < n_rows; ++k) {
+    rows[k] = rows_host ? rows_host[k] : k;
+    if (rows[k] < 0 || rows[k] >= h->MB) B200_FAIL(B200_ERR_INVALID, "lm_set_condition_cross: model row %d outside [0, %d)", rows[k], h->MB);
+  }
+  const int d = h->cfg.dim, H = h->cfg.num_heads, T = h->cross_len;
+  B200_CUDA(cudaMemcpyAsync(h->cross_rows, rows.data(), rows.size() * 4, cudaMemcpyHostToDevice, h->stream));
+  B200_TRY(tc::prepare_plans(h->plans));
+  // transformer.py:495-505 per layer, outside the step: kv = src @ W[d:]^T in chunks of rows, then "b t (p h d) -> p b h t d"
+  // into the rows' memory.  The chunk is staged in a fixed buffer so that the GEMM's activation plan is the same every call.
+  h->body = h->stream;
+  const long long total = (long long)n_rows * T;
+  for (long long i0 = 0; i0 < total; i0 += CROSS_CHUNK) {
+    const int n = (int)std::min<long long>(CROSS_CHUNK, total - i0);
+    B200_CUDA(cudaMemcpyAsync(h->cross_src, static_cast<const bf16*>(src_bf16_dev) + i0 * d, (size_t)n * d * 2, cudaMemcpyDeviceToDevice,
+                              h->stream));
+    for (auto& L : h->layers) {
+      B200_TRY(linear(h, h->cross_src, d, L.ckv_w, h->cross_kv, 2 * d, nullptr, 0, n, 2 * d, d, LIN_STORE, 0));
+      B200_LAUNCH(cross_kv_scatter_kernel, (unsigned)ceil_div64((long long)n * 2 * H * (ATT_D / 8), 256), 256, 0, h->stream, h->cross_kv,
+                  i0, n, h->cross_rows, L.kx, L.vx, H, T);
+    }
+  }
+  return check_launch("lm_set_condition_cross");
+}
+
 int b200_lm_set_taps(b200_lm* h, int enable) {
   B200_TRY(ensure_streaming(h, "lm_set_taps"));
   DeviceGuard g(h->device);
@@ -1247,7 +1390,8 @@ int b200_lm_session_export(b200_lm* h, int row, void* dst_dev, int64_t capacity)
   memset(&s, 0, sizeof(s));
   s.magic = SESSION_MAGIC; s.version = SESSION_VERSION; s.kind = SESSION_LM; s.kv_dtype = (uint32_t)h->kv_fp8;
   s.fingerprint = lm_fingerprint(h); s.rows = p.rows;
-  s.flags = (p.cond ? SESSION_COND : 0) | (h->cfg_until ? SESSION_CFG_UNTIL : 0);
+  s.flags = (p.cond ? SESSION_COND : 0) | (h->cfg_until ? SESSION_CFG_UNTIL : 0) | (h->cross_on ? SESSION_CROSS : 0);
+  if (h->cross_on) memcpy(s.reserved, &h->cross_len, sizeof(int32_t));
   s.pos[0] = p.pos[0]; s.pos[1] = p.pos[1]; s.n = p.n; s.bytes = p.bytes;
   char* rec = static_cast<char*>(dst_dev);
   B200_CUDA(cudaMemcpyAsync(rec, &s, sizeof(s), cudaMemcpyHostToDevice, h->stream));
@@ -1279,6 +1423,14 @@ int b200_lm_session_import(b200_lm* h, int row, const void* src_dev, int64_t nby
     B200_FAIL(B200_ERR_INVALID, "lm_session_import: classifier-free guidance (or cfg_is_masked_until) on one side only");
   p.cond = (s.flags & SESSION_COND) != 0;
   if (p.cond != (h->cond_on != 0)) B200_FAIL(B200_ERR_INVALID, "lm_session_import: condition_sum on one side only");
+  if (((s.flags & SESSION_CROSS) != 0) != (h->cross_on != 0))
+    B200_FAIL(B200_ERR_INVALID, "lm_session_import: cross-attention conditioning on one side only");
+  if (h->cross_on) {
+    int32_t T = 0;
+    memcpy(&T, s.reserved, sizeof(T));
+    if (T != h->cross_len)
+      B200_FAIL(B200_ERR_INVALID, "lm_session_import: the record's condition memory has %d keys, the handle's %d", T, h->cross_len);
+  }
   p.pos[0] = s.pos[0]; p.pos[1] = p.rows > 1 ? s.pos[1] : 0;
   const int64_t top = std::max(p.pos[0], p.pos[1]);
   if (p.pos[0] < 0 || p.pos[1] < 0 || s.n != std::min<int64_t>(top, c.context))
@@ -1479,6 +1631,7 @@ int b200_lm_read_buffer(b200_lm* h, const char* name, void* dst_dev, int64_t cap
       const bool digits = !idx.empty() && idx.size() <= 4 && idx.find_first_not_of("0123456789") == std::string::npos;
       layer = digits ? atoi(idx.c_str()) : -1;
       kind = k == "attn_out" ? TAP_ATTN_OUT : k == "x_attn" ? TAP_X_ATTN : k == "gated" ? TAP_GATED : k == "x_out" ? TAP_X_OUT : -1;
+      if (h->cross_on && kind < 0) kind = k == "cross_out" ? TAP_CROSS_OUT : k == "x_cross" ? TAP_X_CROSS : -1;
       if (layer < 0 || layer >= (int)h->layers.size() || kind < 0)
         B200_FAIL(B200_ERR_INVALID, "lm_read_buffer: unknown buffer '%s'", n.c_str());
     }
@@ -1513,6 +1666,10 @@ int64_t b200_lm_algorithmic_bytes(b200_lm* h, int kv_fill) {
   int64_t per = (int64_t)c.num_layers * 2 * kv_fill * kv_row + (int64_t)c.num_layers * 2 * kv_row;
   per += (int64_t)(c.n_q + 1) * c.dim * 2 + (int64_t)c.dep_q * c.depformer_dim * 2;
   per += (int64_t)2 * (c.text_card + (int64_t)c.dep_q * c.card) * 2;
+  if (h->cross_on) {          // the query, K|V and output linears of every layer; each row reads its condition memory
+    w += (int64_t)c.num_layers * 4 * c.dim * c.dim * 2;
+    per += (int64_t)c.num_layers * 2 * h->cross_len * c.dim * 2;
+  }
   return w + per * B;
 }
 

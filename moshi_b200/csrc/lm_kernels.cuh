@@ -705,6 +705,143 @@ struct KvRings {
 void attn_step_launch(const bf16* qkv, const KvRings& r, bf16* out, float* part, int* counters, const long long* pos,
                       const uint8_t* exec_mask, int B, int H, int cap, int nsplit, float max_period, int storage, cudaStream_t st);
 
+// ---------------------------------------------------------------------------------------------
+// LayerNorm with weight and bias (the cross-attention layers' norm_cross, nn.LayerNorm(dim, eps=1e-5), transformer.py:727-732):
+// bf16 in and out, fp32 statistics (the mean, then the mean of the squared deviations), y = bf16((x - mean) * rstd * w + b).
+// One 256-thread CTA per row.
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ float block_sum_256(float v, float* red) {
+  v = warp_sum(v);
+  __syncthreads();                                 // red is reused by consecutive calls
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float t = 0.f;
+#pragma unroll
+  for (int w = 0; w < 8; ++w) t += red[w];
+  return t;
+}
+
+static __global__ void __launch_bounds__(256) layernorm_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w,
+                                                        const bf16* __restrict__ bias, bf16* __restrict__ y, int dim, float eps) {
+  pdl_trigger();
+  __shared__ float red[8];
+  const bf16* xr = x + (long long)blockIdx.x * dim;
+  float s = 0.f;
+  for (int c = threadIdx.x * 2; c < dim; c += 512) {
+    const float2 v = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(xr + c));
+    s += v.x + v.y;
+  }
+  const float mean = block_sum_256(s, red) / (float)dim;
+  float ss = 0.f;
+  for (int c = threadIdx.x * 2; c < dim; c += 512) {
+    const float2 v = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(xr + c));
+    ss += (v.x - mean) * (v.x - mean) + (v.y - mean) * (v.y - mean);
+  }
+  const float rstd = rsqrtf(block_sum_256(ss, red) / (float)dim + eps);
+  for (int c = threadIdx.x * 2; c < dim; c += 512) {
+    const float2 v = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(xr + c));
+    const float2 g = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(w + c));
+    const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(bias + c));
+    *reinterpret_cast<__nv_bfloat162*>(y + (long long)blockIdx.x * dim + c) =
+        __floats2bfloat162_rn((v.x - mean) * rstd * g.x + b.x, (v.y - mean) * rstd * g.y + b.y);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Cross-attention step of a temporal layer (transformer.py:544-597 with cross_attention=True): one query per (row, head)
+// against all T keys of that row's condition memory k_cross / v_cross [B][H][T][ATT_D].  No RoPE, no mask, no append and no
+// exec mask: every row computes, as in the reference.  The CTA layout, the key loop and the split merge are attn_step_kernel's
+// (grid = (B*H, nsplit), 128 threads, a half-warp per key, partials merged in split order); only the query load (no rotation)
+// and the key range [0, T) differ.  q [B][ldq] bf16, head h at columns [h * ATT_D, (h + 1) * ATT_D).
+// ---------------------------------------------------------------------------------------------
+struct CrossAttnStep {
+  const bf16* q; long long ldq;
+  const bf16* kc; const bf16* vc;              // [B][H][T][ATT_D]
+  bf16* out;                                   // [B][H * ATT_D]
+  float* part; int* counters;                  // [B*H][nsplit][ATT_D + 2], [B*H] (zero between launches)
+  int H, T, nsplit;
+};
+
+static __global__ void __launch_bounds__(ATT_THREADS) cross_attn_step_kernel(const CrossAttnStep a) {
+  pdl_trigger();
+  const int bh = blockIdx.x, split = blockIdx.y;
+  const int b = bh / a.H, h = bh - b * a.H;
+  const int tid = threadIdx.x, l16 = tid & 15;
+  const int hw = tid >> 4;                          // half-warp id 0..7
+  const int per = (a.T + a.nsplit - 1) / a.nsplit;
+  const int s0 = split * per, s1 = min(s0 + per, a.T);
+
+  float qf[8];
+  unpack8(*reinterpret_cast<const uint4*>(a.q + (long long)b * a.ldq + h * ATT_D + l16 * 8), qf);
+  const float scale = 0.08838834764831845f;       // 1/sqrt(128)
+#pragma unroll
+  for (int i = 0; i < 8; ++i) qf[i] *= scale;
+
+  const long long row0 = (long long)bh * a.T * ATT_D;
+  const bf16* kb = a.kc + row0 + l16 * 8;
+  const bf16* vb = a.vc + row0 + l16 * 8;
+  float m = -INFINITY, l = 0.f, acc[8] = {};
+
+  constexpr int U = ATT_GROUP;
+  struct Group { uint4 k[U], v[U]; };
+  auto load_group = [&](int kb0, Group& gp) {
+    const int s = kb0 + hw * U;
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const long long o = (long long)(s + u < s1 ? s + u : s1 - 1) * ATT_D;
+      gp.k[u] = *reinterpret_cast<const uint4*>(kb + o);
+      gp.v[u] = *reinterpret_cast<const uint4*>(vb + o);
+    }
+  };
+  auto reduce_group = [&](int kb0, const Group& gp) {
+    const int s = kb0 + hw * U;
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      float kf[8];
+      unpack8(gp.k[u], kf);
+      float d = 0.f;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) d = fmaf(qf[i], kf[i], d);
+      d += __shfl_xor_sync(0xffffffffu, d, 8);
+      d += __shfl_xor_sync(0xffffffffu, d, 4);
+      d += __shfl_xor_sync(0xffffffffu, d, 2);
+      d += __shfl_xor_sync(0xffffffffu, d, 1);
+      if (s + u < s1) {
+        const float mn = fmaxf(m, d);
+        const float corr = __expf(m - mn), pw = __expf(d - mn);
+        float vf[8];
+        unpack8(gp.v[u], vf);
+        l = l * corr + pw;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) acc[i] = fmaf(pw, vf[i], acc[i] * corr);
+        m = mn;
+      }
+    }
+  };
+  attn_key_loop<Group>(s0, s1, load_group, reduce_group);
+  attn_merge_store(a, bh, split, m, l, acc);
+}
+
+// The cross-attention K/V of condition rows (transformer.py:495-505: kv = src @ W[d:]^T, "b t (p h d) -> p b h t d") from a
+// chunk of the projection, kv [n][2 * H * ATT_D] = flat rows [i0, i0 + n) of (condition row r, t), into the condition memory
+// k_cross / v_cross [B][H][T][ATT_D] of model row rows[r].  One thread per 16 bytes.
+static __global__ void cross_kv_scatter_kernel(const bf16* __restrict__ kv, long long i0, int n, const int* __restrict__ rows,
+                                               bf16* __restrict__ kc, bf16* __restrict__ vc, int H, int T) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const int per_row = 2 * H * (ATT_D / 8);
+  if (i >= (long long)n * per_row) return;
+  const int j = (int)(i / per_row), e = (int)(i - (long long)j * per_row);
+  const int p = e / (H * (ATT_D / 8)), hh = (e / (ATT_D / 8)) % H, c = e % (ATT_D / 8);
+  const long long g = i0 + j;
+  const int r = (int)(g / T), t = (int)(g - (long long)r * T);
+  bf16* dst = (p ? vc : kc) + (((long long)rows[r] * H + hh) * T + t) * ATT_D + c * 8;
+  *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(kv + (long long)j * 2 * H * ATT_D + (long long)p * H * ATT_D + hh * ATT_D + c * 8);
+}
+
+// One cross-attention step of B rows over condition memories of T keys (defined in lm.cu next to attn_step_launch)
+void cross_attn_launch(const bf16* q, long long ldq, const bf16* kc, const bf16* vc, bf16* out, float* part, int* counters, int B,
+                       int H, int T, int nsplit, cudaStream_t st);
+
 constexpr int DEP_MAX_Q = 16;              // dep_q of the largest family member (configs/moshi_dev_2b.json)
 
 // Depformer attention step: the new key/value of sub-step `step` is appended to the per-frame cache and the query

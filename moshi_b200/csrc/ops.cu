@@ -134,6 +134,29 @@ int b200_op_rmsnorm(const void* x_dev, const void* alpha_dev, void* y_dev, int M
   return check_launch("op_rmsnorm");
 }
 
+int b200_op_layernorm(const void* x_dev, const void* w_dev, const void* b_dev, void* y_dev, int M, int dim, void* stream) {
+  using namespace b200::lm;
+  if (!x_dev || !w_dev || !b_dev || !y_dev) B200_FAIL(B200_ERR_INVALID, "op_layernorm: null pointer");
+  if (M < 1 || dim < 2 || dim % 2) B200_FAIL(B200_ERR_SHAPE, "op_layernorm: bad shape M=%d dim=%d", M, dim);
+  B200_LAUNCH(layernorm_kernel, M, 256, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(x_dev),
+              static_cast<const bf16*>(w_dev), static_cast<const bf16*>(b_dev), static_cast<bf16*>(y_dev), dim, 1e-5f);
+  return check_launch("op_layernorm");
+}
+
+int b200_op_cross_attn_step(const void* q_dev, const void* k_dev, const void* v_dev, void* out_dev, int B, int H, int T, int nsplit,
+                            void* stream) {
+  using namespace b200::lm;
+  if (!q_dev || !k_dev || !v_dev || !out_dev) B200_FAIL(B200_ERR_INVALID, "op_cross_attn_step: null pointer");
+  if (B < 1 || H < 1 || T < 1) B200_FAIL(B200_ERR_SHAPE, "op_cross_attn_step: bad shape");
+  if (nsplit <= 0) nsplit = attn_pick_splits(B, H, T);
+  float* part = nullptr;
+  int* counters = nullptr;
+  B200_TRY(attn_scratch(B, H, nsplit, &part, &counters, 0));
+  cross_attn_launch(static_cast<const bf16*>(q_dev), (long long)H * ATT_D, static_cast<const bf16*>(k_dev), static_cast<const bf16*>(v_dev),
+                    static_cast<bf16*>(out_dev), part, counters, B, H, T, nsplit, static_cast<cudaStream_t>(stream));
+  return check_launch("op_cross_attn_step");
+}
+
 int64_t b200_op_packed_bytes_i8(int N, int K, int epi, int gate_rows) { return (int64_t)tc::sk_packed_bytes_i8(N, K, epi, gate_rows); }
 
 int b200_op_quant_pack_tiles(const void* w_dev, void* tiles_dev, float* scales_dev, int N, int K, int epi, int gate_rows,

@@ -4,7 +4,8 @@ Mirrors ``moshi/moshi/models/lm.py``: ``LMModel`` exposes the attributes callers
 (``dep_q, n_q, card, text_card, delays, device, dtype, num_codebooks, condition_provider, fuser, ...``,
 lm.py:248-295) and owns the weights on the device; ``LMGen`` (lm.py:555-850) owns the streaming state and runs one
 ``step`` per 80 ms frame, including classifier-free guidance (lm.py:596-604, 646-662, 714-732, 820-833), conditioning by
-sum (lm.py:616-626), forced audio tokens (lm.py:751-755) and the STT models' extra heads (lm.py:793-807).
+sum (lm.py:616-626), cross-attention conditioning of the temporal layers (lm.py:616-651, transformer.py:727-732, 779-798),
+forced audio tokens (lm.py:751-755) and the STT models' extra heads (lm.py:793-807).
 
 Sampling noise: the reference draws ``Exp(1)`` from torch's generator inside ``sample_token`` (sampling.py:44).  Here
 the step draws it itself (a Philox stream inside the step's CUDA graph, seeded once per session from torch's CPU
@@ -23,7 +24,7 @@ import torch
 from .. import _lib
 from ..conditioners import ConditionFuser, ConditionProvider, ConditionTensors, build_conditioning
 from ..config import LMConfig
-from .state_dict import normalize_lm_state_dict
+from .state_dict import _CANDLE, normalize_lm_state_dict
 
 _TORCH_DTYPES = {_lib.B200_F32: torch.float32, _lib.B200_BF16: torch.bfloat16, _lib.B200_F16: torch.float16,
                  _lib.B200_I64: torch.int64, _lib.B200_U8: torch.uint8}
@@ -75,10 +76,14 @@ class LMModel:
         host_side: dict[str, torch.Tensor] = {}       # conditioner weights stay with the Python-side provider
         with torch.cuda.device(self.device):
             _lib.check(self._lib.b200_lm_create(C.byref(_config_struct(cfg)), C.byref(self._h)))
+            if cfg.cross_attention:
+                _lib.check(self._lib.b200_lm_set_cross_attention(self._h, 1))
             for name, t in items:
                 if name.startswith("condition_provider."):
                     host_side[name] = t.detach()
                     continue
+                if cfg.cross_attention and _CANDLE.match(name):
+                    raise ValueError("candle-layout checkpoints of a cross-attention LM are not supported; load its safetensors checkpoint")
                 for n2, t2 in normalize_lm_state_dict({name: t}).items():
                     # a q8 checkpoint stores a QLinear as `weight` int8 + `weight_scb` float32, and the scale must stay float32
                     # (utils/quantize.py:13-35; the reference's loader casts it with the rest, loaders.py:415-421, and then fails)
@@ -95,7 +100,8 @@ class LMModel:
                     del t2
             _lib.check(self._lib.b200_lm_finalize(self._h))
         if cfg.conditioners:
-            self.condition_provider, self.fuser = build_conditioning(cfg.conditioners, cfg.fuser, cfg.dim, host_side, self.device)
+            self.condition_provider, self.fuser = build_conditioning(cfg.conditioners, cfg.fuser, cfg.dim, host_side, self.device,
+                                                                     cfg.cross_attention)
 
     def __del__(self):
         h = getattr(self, "_h", None)
@@ -209,8 +215,8 @@ class LMGen:
     def _start(self, batch_size: int) -> None:
         assert self._batch is None, "lm_gen is already streaming!"
         lm, dev = self.lm_model, self.lm_model.device
-        # lm.py:613-626: the sum-fused condition, cast to the model dtype
-        condition_sum = None
+        # lm.py:613-627: the sum- and cross-fused conditions, cast to the model dtype
+        condition_sum = condition_cross = None
         if lm.fuser is None:
             assert not self.condition_tensors
         else:
@@ -218,9 +224,16 @@ class LMGen:
             condition_sum = lm.fuser.get_sum(self.condition_tensors)
             if condition_sum is not None:
                 condition_sum = condition_sum.to(device=dev, dtype=lm.dtype)
+            condition_cross = lm.fuser.get_cross(self.condition_tensors)
+            if condition_cross is not None:
+                condition_cross = condition_cross.to(device=dev, dtype=lm.dtype)
         model_batch = batch_size * 2 if self.cfg_coef != 1. else batch_size
         if condition_sum is not None:
             assert condition_sum.shape[0] == model_batch, "cfg requires 2x more conditions."     # lm.py:648-649
+        if condition_cross is not None:
+            assert condition_cross.shape[0] == model_batch, "cfg requires 2x more conditions."   # lm.py:650-651
+        # transformer.py:786: every cross-attention layer needs its source
+        assert condition_cross is not None or not lm.cfg.cross_attention, "a cross-attention LM needs cross condition tensors"
         with self._device():
             self._pushed_sampling = None
             self._push_sampling()
@@ -236,6 +249,8 @@ class LMGen:
                 until = (C.c_int64 * len(self.cfg_is_masked_until))(*[int(v) for v in self.cfg_is_masked_until])
             _lib.check(self._lib.b200_lm_set_cfg(self._h, float(self.cfg_coef), int(bool(self.cfg_is_no_text)), until,
                                                  0 if until is None else len(self.cfg_is_masked_until)))
+            if lm.cfg.cross_attention:       # the condition memory holds T keys per row for the whole session
+                _lib.check(self._lib.b200_lm_set_cross_len(self._h, int(condition_cross.shape[1])))
             self._stream = torch.cuda.current_stream(dev).cuda_stream
             _lib.check(self._lib.b200_lm_streaming_begin(self._h, int(batch_size), C.c_void_p(self._stream)))
             # one draw from torch's CPU generator seeds the session's in-step noise stream
@@ -246,6 +261,8 @@ class LMGen:
                 _lib.check(self._lib.b200_lm_set_condition_sum(self._h, _lib.ptr(cs), model_batch))
         self._batch = int(batch_size)
         self._model_batch = model_batch
+        if condition_cross is not None:
+            self.set_condition_cross(condition_cross)
         self._noise_per_row = int(self._lib.b200_lm_noise_per_row(self._h))
         self._kt = min(self.top_k_text, lm.text_card)
         self._ka = min(self.top_k, lm.card)
@@ -278,6 +295,33 @@ class LMGen:
         with self._device():
             self._sync_stream()
             _lib.check(self._lib.b200_lm_reset(self._h, _lib.ptr(m)))
+
+    def set_condition_cross(self, cross: torch.Tensor, rows: tp.Sequence[int] | torch.Tensor | None = None) -> None:
+        """Replaces the condition memory (``_MHAState.k_cross / v_cross`` of every cross-attention layer) of model rows ``rows``
+        (None: all of them) with the keys and values of ``cross`` [len(rows), T, dim], e.g. ``fuser.get_cross`` of new condition
+        tensors: what the TTS service does when a slot takes a new voice (tts.py:422-440).  Model rows are the sessions ``b``
+        and, under classifier-free guidance, ``batch + b`` for their null half.  T is the one the session started with.  The
+        rows' positions and every other row are unchanged; ``reset_streaming`` keeps the memory, as in the reference."""
+        assert self._batch is not None, "lm_gen is not streaming"
+        assert self.lm_model.cfg.cross_attention, "the model has no cross-attention layers"
+        if rows is not None:
+            rows = [int(r) for r in (rows.tolist() if isinstance(rows, torch.Tensor) else rows)]
+        n = self._model_batch if rows is None else len(rows)
+        src = cross.to(device=self.lm_model.device, dtype=self.lm_model.dtype).contiguous()
+        assert src.dim() == 3 and src.shape[0] == n and src.shape[2] == self.lm_model.dim, \
+            f"expected a condition [{n}, T, {self.lm_model.dim}], got {tuple(src.shape)}"
+        keys = self._entry_shape("layers.0.k_cross")[2]
+        assert src.shape[1] == keys, f"the condition memory holds {keys} keys per row for this session, got {src.shape[1]}"
+        rows_c = None if rows is None else (C.c_int32 * n)(*rows)
+        with self._device():
+            self._sync_stream()
+            _lib.check(self._lib.b200_lm_set_condition_cross(self._h, _lib.ptr(src), rows_c, n))
+
+    def _entry_shape(self, name: str) -> tuple[int, ...]:
+        for n, _, shape, _ in self._state_entries():
+            if n == name:
+                return shape
+        raise KeyError(name)
 
     def set_exec_mask(self, exec_mask: torch.Tensor) -> None:
         assert self._batch is not None
@@ -333,6 +377,10 @@ class LMGen:
                                      end_offset=raw["model.offset"].clone())
             state[f"lm_model.transformer.layers.{i}.self_attn"] = SimpleNamespace(
                 batch_size=self._model_batch, exec_mask=mexec, kv_cache=kv, offset=raw["model.offset"].clone(), offset_cpu=offset_cpu)
+            if p + ".k_cross" in raw:     # _MHAState of the cross-attention module (transformer.py:321-327): only its memory
+                state[f"lm_model.transformer.layers.{i}.cross_attention"] = SimpleNamespace(
+                    batch_size=self._model_batch, exec_mask=mexec, kv_cache=None, k_cross=raw[p + ".k_cross"],
+                    v_cross=raw[p + ".v_cross"])
         return state
 
     def set_streaming_state(self, state: dict[str, tp.Any]) -> None:
@@ -341,6 +389,8 @@ class LMGen:
         state = dict(state)
         L = self.lm_model.cfg.num_layers
         expected = ["", "lm_model", "lm_model.transformer"] + [f"lm_model.transformer.layers.{i}.self_attn" for i in range(L)]
+        if self.lm_model.cfg.cross_attention:
+            expected += [f"lm_model.transformer.layers.{i}.cross_attention" for i in range(L)]
         for name in expected:
             if name not in state:
                 raise RuntimeError(f"Expected to find a streaming state for {name}.")
@@ -370,13 +420,18 @@ class LMGen:
                     self._write_state(f"layers.{i}.v8", kv.cache_q8[1])
                     self._write_state(f"layers.{i}.k_scale", kv.scales[0])
                     self._write_state(f"layers.{i}.v_scale", kv.scales[1])
+                if self.lm_model.cfg.cross_attention:
+                    cx = state.pop(f"lm_model.transformer.layers.{i}.cross_attention")
+                    self._write_state(f"layers.{i}.k_cross", cx.k_cross)
+                    self._write_state(f"layers.{i}.v_cross", cx.v_cross)
         if state:
             raise RuntimeError(f"Some states were not consumed: {list(state.keys())}")
 
     # ---- one session -----------------------------------------------------------------------------
     def export_session(self, row: int) -> torch.Tensor:
         """Session ``row`` as a uint8 record on the model's device (``b200_lm_session_export``): its token ring, offsets,
-        positions and the temporal K/V of its live fill, so the size follows the fill.  The row is not changed and keeps
+        positions and the temporal K/V of its live fill, so the size follows the fill, and on a cross-attention model its
+        condition memory.  The row is not changed and keeps
         running; reset it once the session has moved.  A short-ring row past ``kv_capacity`` raises (its history is lost)."""
         assert self._batch is not None, "lm_gen is not streaming"
         n = C.c_int64()

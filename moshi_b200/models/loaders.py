@@ -79,6 +79,8 @@ def get_moshi_lm(filename: str | Path | None, lm_kwargs: dict | None = None,
         tensors = _stream()
     elif Path(filename).suffix == ".gguf":
         # the Rust stack's quantised checkpoints (rust/moshi-core/src/nn.rs:9-116): candle tensor names, Q8_0 blocks dequantised
+        if cfg.cross_attention:
+            raise ValueError("GGUF checkpoints of a cross-attention LM are not supported; load its safetensors checkpoint")
         from .gguf import read_gguf
         _, tensors = read_gguf(filename)
     else:

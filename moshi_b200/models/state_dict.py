@@ -1,7 +1,7 @@
 """Checkpoint key normalisation: the on-disk names the reference accepts map to the module names.
 
-* packed attention weights ``self_attn.in_proj_weight`` / ``in_proj.weight`` / ``out_proj.weight``
-  of shape ``[mult * rows, in]`` become ``in_projs.{i}.weight`` / ``out_projs.{i}.weight``
+* packed attention weights ``self_attn.in_proj_weight`` / ``in_proj.weight`` / ``out_proj.weight`` (and the same names
+  under ``cross_attention.``) of shape ``[mult * rows, in]`` become ``in_projs.{i}.weight`` / ``out_projs.{i}.weight``
   (load hook ``moshi/moshi/modules/transformer.py:422-446``);
 * legacy codebook buffers ``inited`` / ``cluster_size`` / ``embed_avg`` / ``embed_sum``
   become ``_initialized`` / ``cluster_usage`` / ``embedding_sum`` (``core_vq.py:162-176``);
@@ -21,12 +21,13 @@ _CODEBOOK_RENAMES = {"inited": "_initialized", "cluster_size": "cluster_usage",
 def _split_attention(sd: tp.Mapping[str, torch.Tensor]) -> dict[str, torch.Tensor]:
     out: dict[str, torch.Tensor] = {}
     for key, w in sd.items():
-        if key.endswith("self_attn.in_proj_weight") or key.endswith("self_attn.in_proj.weight"):
+        if key.endswith(("self_attn.in_proj_weight", "self_attn.in_proj.weight", "cross_attention.in_proj_weight",
+                         "cross_attention.in_proj.weight")):
             base = key[: key.rindex("in_proj")]
             mult = max(1, w.shape[0] // (3 * w.shape[1]))
             for i, part in enumerate(w.view(mult, -1, w.shape[1])):
                 out[f"{base}in_projs.{i}.weight"] = part
-        elif key.endswith("self_attn.out_proj.weight"):
+        elif key.endswith(("self_attn.out_proj.weight", "cross_attention.out_proj.weight")):
             base = key[: key.rindex("out_proj")]
             mult = max(1, w.shape[0] // w.shape[1])
             for i, part in enumerate(w.view(mult, -1, w.shape[1])):

@@ -177,11 +177,20 @@ def lm_tensor_specs(cfg: LMConfig) -> list[tuple[str, tuple[int, ...], float]]:
         specs.append((p + ".norm2.alpha", (1, 1, d), 0))
         specs.append((p + ".gating.linear_in.weight", (2 * h, d), d))
         specs.append((p + ".gating.linear_out.weight", (d, h), h))
+        if cfg.cross_attention:                                      # transformer.py:727-732, 495-505
+            specs.append((p + ".cross_attention.in_projs.0.weight", (3 * d, d), d))
+            specs.append((p + ".cross_attention.out_projs.0.weight", (d, d), d))
+            specs.append((p + ".norm_cross.weight", (d,), 0))
+            specs.append((p + ".norm_cross.bias", (d,), -1))
     for i in range(cfg.extra_heads_num_heads):                       # lm.py:224-226
         specs.append((f"extra_heads.{i}.weight", (cfg.extra_heads_dim, d), d))
     for name, c in (cfg.conditioners or {}).items():                 # conditioners/text.py:106-134, base.py:105-129
-        lut = c["lut"]
         p = f"condition_provider.conditioners.{name}"
+        if c["type"] == "tensor":                                    # conditioners/tensors.py: output_proj + learnt padding only
+            specs.append((p + ".output_proj.weight", (d, c["tensor"]["dim"]), c["tensor"]["dim"]))
+            specs.append((p + ".learnt_padding", (1, 1, d), 75.0))
+            continue
+        lut = c["lut"]
         specs.append((p + ".embed.weight", (lut["n_bins"] + 1, lut["dim"]), 3.0))
         specs.append((p + ".output_proj.weight", (d, lut["dim"]), lut["dim"]))
         specs.append((p + ".learnt_padding", (1, 1, d), 75.0))
@@ -212,8 +221,10 @@ def iter_synth_lm_tensors(cfg: LMConfig, seed: int = 4242, device: str | torch.d
     """Yields (key, tensor) one at a time so that a 7B model never needs two copies in memory."""
     g = _gen(seed, device)
     for key, shape, fan_in in lm_tensor_specs(cfg):
-        if fan_in == 0:  # RMSNorm alpha
+        if fan_in == 0:  # RMSNorm alpha / LayerNorm weight
             t = (1.0 + _uniform(g, shape, 0.1, device)).to(dtype)
+        elif fan_in < 0:  # LayerNorm bias
+            t = _uniform(g, shape, 0.05, device).to(dtype)
         else:
             # same variance as the reference's trunc-normal(std = 1/sqrt(fan_in)) init, lm_utils.py:44-56
             bound = math.sqrt(3.0 / fan_in)
@@ -246,6 +257,9 @@ def tiled_lm_state_dict(cfg: LMConfig, seed: int = 7, block_elems: int = 1 << 25
             n *= s_
         if fan_in == 0:
             sd[key] = (1.0 + 0.1 * unit[:n]).to(torch.bfloat16).view(shape)
+            continue
+        if fan_in < 0:
+            sd[key] = (0.05 * unit[:n]).to(torch.bfloat16).view(shape)
             continue
         bound = math.sqrt(3.0 / fan_in)
         if ".out_projs." in key or "linear_out" in key:
