@@ -837,7 +837,12 @@ def _tm_tensor(sd: dict, name: str, layer: int | None) -> torch.Tensor:
     key = {"in": p + "self_attn.in_projs.0.weight", "out": p + "self_attn.out_projs.0.weight",
            "lin_in": p + "gating.linear_in.weight", "lin_out": p + "gating.linear_out.weight", "n1": p + "norm1.alpha",
            "n2": p + "norm2.alpha", "out_norm": "out_norm.alpha", "head": "text_linear.weight",
-           "din": f"depformer_in.{layer}.weight"}[name]
+           "din": f"depformer_in.{layer}.weight", "cq": p + "cross_attention.in_projs.0.weight",
+           "ckv": p + "cross_attention.in_projs.0.weight", "co": p + "cross_attention.out_projs.0.weight",
+           "ncw": p + "norm_cross.weight", "ncb": p + "norm_cross.bias"}[name]
+    if name in ("cq", "ckv"):       # transformer.py:495-505: rows [0, d) of in_projs.0 the query, [d, 3d) K|V of the condition
+        d = sd[key].shape[1]
+        return sd[key][:d] if name == "cq" else sd[key][d:]
     return sd[key]
 
 
@@ -865,10 +870,82 @@ def _tm_rmsnorm(x: torch.Tensor, alpha: torch.Tensor) -> torch.Tensor:
     return x * alpha.double().reshape(-1) / torch.sqrt(1e-8 + x.pow(2).mean(-1, keepdim=True))
 
 
+def _res_add(cfg, layer: int, x: torch.Tensor, upd: torch.Tensor, which: str, mutant: dict) -> torch.Tensor:
+    """x + upd of one residual (the fp32 add of the int8 epilogue under cfg.quantize); mutant["residual"] may drop it."""
+    if not mutant.get("residual", lambda *a: True)(layer, which):
+        return upd
+    return (x.float() + upd.float()).double() if cfg.quantize else x.double() + upd
+
+
+def _layernorm64(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor, eps: float = 1e-5) -> torch.Tensor:
+    """nn.LayerNorm over the last dimension in float64, not rounded."""
+    x = x.double()
+    mu = x.mean(-1, keepdim=True)
+    var = (x - mu).pow(2).mean(-1, keepdim=True)
+    return (x - mu) / torch.sqrt(var + eps) * w.double().reshape(-1) + b.double().reshape(-1)
+
+
+def _softmax_attention64(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, chunk: int = 16) -> torch.Tensor:
+    """softmax(q . k_t / sqrt(D)) . v_t over every t, q [R, H, D], k / v [R, H, T, D] (any dtype) -> float64 [R, H, D], in
+    chunks of rows on k's device (a memory of 625 keys at 512 rows is 5 GB in float64)."""
+    R, H, D = q.shape
+    out = []
+    for i in range(0, R, chunk):
+        kk, vv = k[i:i + chunk].double(), v[i:i + chunk].double()
+        s = torch.einsum("rhd,rhtd->rht", q[i:i + chunk].to(kk.device, torch.float64), kk) * D ** -0.5
+        out.append(torch.einsum("rht,rhtd->rhd", torch.softmax(s, dim=-1), vv))
+        del kk, vv
+    return torch.cat(out)
+
+
+@torch.no_grad()
+def cross_block_ref64(sd: dict, cfg, layer: int, x_attn: torch.Tensor, cross_out: torch.Tensor,
+                      memory: tuple[torch.Tensor, torch.Tensor], mutant: dict | None = None) -> dict:
+    """The cross-attention block of one temporal layer (transformer.py:779-798, tests/cross_oracle.py cross_block) in float64
+    for R model rows, teacher-forced on the implementation's taps like temporal_layer_ref64:
+
+      xn = bf16(layernorm(x_attn, norm_cross.weight, norm_cross.bias, eps 1e-5));  q = bf16(xn . in_projs.0[:d]^T);
+      cross_out = softmax(q . k_t / sqrt(128)) . v_t over all T keys of the row's ``memory`` (the implementation's k_cross /
+                  v_cross [R, H, T, 128]; no RoPE, no mask);
+      x_cross = bf16(x_attn + bf16(out_projs.0(cross_out))).
+
+    ``x_attn`` / ``cross_out`` are the implementation's x after the self-attention residual and its cross-attention output
+    ([R, dim] bf16).  Returns, before their final bf16 rounding, as float64: "cross_out" [R, H, D], "x_cross" and the out
+    linear's own output "x_cross.upd".  ``mutant`` as in temporal_layer_ref64 (weight / linear names cq, co, ncw, ncb;
+    "residual" with "cross")."""
+    mutant = mutant or {}
+    dev = x_attn.device
+    R, d = x_attn.shape
+    H = cfg.num_heads
+    W = _tm_weights(sd, layer, mutant, dev)
+    xn = _bf(_layernorm64(x_attn, W("ncw"), W("ncb")))
+    q = _bf(_tm_linear(xn, W("cq"), "cq", layer, False, mutant)).view(R, H, d // H)
+    kx, vx = memory
+    o = _softmax_attention64(q, kx, vx).to(dev)
+    upd = _bf(_tm_linear(cross_out.double(), W("co"), "co", layer, False, mutant))
+    return {"cross_out": o, "x_cross": _res_add(cfg, layer, x_attn, upd, "cross", mutant), "x_cross.upd": upd}
+
+
+@torch.no_grad()
+def cross_memory_ref64(sd: dict, cfg, layer: int, src: torch.Tensor, rows: int = 16):
+    """The condition memory of one layer (transformer.py:495-505) in float64: k_cross | v_cross = src . in_projs.0[d:3d]^T
+    split as "b t (p h d) -> p b h t d", for src [R, T, dim] bf16 (the fused condition, fuser.get_cross).  Yields (r0, k, v)
+    per chunk of ``rows`` rows, k / v [n, H, T, 128] float64 before their bf16 rounding, on src's device: at R = 256 and
+    T = 625 the whole product is 5 GB."""
+    R, T, d = src.shape
+    H = cfg.num_heads
+    w = _tm_tensor(sd, "ckv", layer).to(src.device, torch.float64)
+    for r0 in range(0, R, rows):
+        kv = src[r0:r0 + rows].double() @ w.T
+        kv = kv.view(-1, T, 2, H, d // H).permute(2, 0, 3, 1, 4)
+        yield r0, kv[0], kv[1]
+        del kv
+
+
 @torch.no_grad()
 def temporal_layer_ref64(sd: dict, cfg, layer: int, x_in: torch.Tensor, ao: torch.Tensor, x_attn: torch.Tensor, h: torch.Tensor,
                          kv_ring: tuple[torch.Tensor, torch.Tensor], pos: torch.Tensor, executing: torch.Tensor,
-                         mutant: dict | None = None, rope_freqs: torch.Tensor | None = None) -> dict:
+                         mutant: dict | None = None, rope_freqs: torch.Tensor | None = None, cross: dict | None = None) -> dict:
     """One temporal-transformer layer (transformer.py:752-802 with the gated SiLU of gating.py:13-22, as oracle/transformer.py
     states it) in float64 for R model rows, teacher-forced on the implementation's own taps so that each linear is judged on
     its own input and the error bound stays one cast point wide at every depth:
@@ -887,10 +964,15 @@ def temporal_layer_ref64(sd: dict, cfg, layer: int, x_in: torch.Tensor, ao: torc
     is a QLinear and the residual adds are the fp32 adds of the int8 epilogue, so "x_attn" / "x_out" round to the exact bf16
     result given the taps.
 
+    ``cross`` (a cross-attention layer): the implementation's "cross_out" and "x_cross" taps and its condition memory "kx" /
+    "vx" [R, H, T, D].  The layer then also returns cross_block_ref64's "cross_out", "x_cross" and "x_cross.upd", and the MLP
+    runs on the "x_cross" tap instead of x_attn: gated from rmsnorm(x_cross, norm2), x_out = x_cross + linear_out(h).
+
     ``mutant`` (for the tests of the acceptance rule) changes one thing:
-      "weight": f(name, layer, fetch) -> the raw tensor (names in, out, lin_in, lin_out, n1, n2; fetch(name, layer) is right);
+      "weight": f(name, layer, fetch) -> the raw tensor (names in, out, lin_in, lin_out, n1, n2, and cq, co, ncw, ncb of the
+                cross block; fetch(name, layer) is right);
       "linear": f(name, layer, x, w, y) -> the linear's float64 output y (x its input, w its weight);
-      "residual": f(layer, "attn" | "ffn") -> False to drop that residual;   "rope_shift": added to k's RoPE position."""
+      "residual": f(layer, "attn" | "cross" | "ffn") -> False to drop that residual;   "rope_shift": added to k's RoPE position."""
     mutant = mutant or {}
     dev = x_in.device
     R, d = x_in.shape
@@ -902,9 +984,7 @@ def temporal_layer_ref64(sd: dict, cfg, layer: int, x_in: torch.Tensor, ao: torc
         return _tm_linear(x, W(name), name, layer, cfg.quantize, mutant)
 
     def res_add(x, upd, which):
-        if not mutant.get("residual", lambda *a: True)(layer, which):
-            return upd
-        return (x.float() + upd.float()).double() if cfg.quantize else x.double() + upd
+        return _res_add(cfg, layer, x, upd, which, mutant)
 
     qkv = lin(_bf(_tm_rmsnorm(x_in, W("n1"))), "in").view(R, 3, H, D)
     p = pos.cpu()
@@ -916,12 +996,17 @@ def temporal_layer_ref64(sd: dict, cfg, layer: int, x_in: torch.Tensor, ao: torc
                    for i in range(0, R, 16)])[:, 0]
     upd1 = _bf(lin(ao.double(), "out"))
     xa = res_add(x_in, upd1, "attn")
-    gu = lin(_bf(_tm_rmsnorm(x_attn, W("n2"))), "lin_in")
+    out = {}
+    x_mlp = x_attn
+    if cross is not None:
+        out = cross_block_ref64(sd, cfg, layer, x_attn, cross["cross_out"], (cross["kx"], cross["vx"]), mutant)
+        x_mlp = cross["x_cross"]
+    gu = lin(_bf(_tm_rmsnorm(x_mlp, W("n2"))), "lin_in")
     F_ = gu.shape[1] // 2
     g, u = _bf(gu[:, :F_]), _bf(gu[:, F_:])
     upd2 = _bf(lin(h.double(), "lin_out"))
-    xo = res_add(x_attn, upd2, "ffn")
-    return {"k": k.to(dev), "v": qkv[:, 2], "attn_out": o, "x_attn": xa, "x_attn.upd": upd1,
+    xo = res_add(x_mlp, upd2, "ffn")
+    return {"k": k.to(dev), "v": qkv[:, 2], "attn_out": o, "x_attn": xa, "x_attn.upd": upd1, **out,
             "gated": _bf(g * torch.sigmoid(g)) * u, "x_out": xo, "x_out.upd": upd2}
 
 
@@ -978,9 +1063,17 @@ def temporal_heads_ref64(sd: dict, cfg, x_last: torch.Tensor, tout: torch.Tensor
 #   gated 0.076 (the 32-layer model) gets 0.15;   v 0.0015 (int8: one int8 step of an activation that sits on a rounding
 #     boundary of the quantiser moves the whole row's product) gets 0.003.
 # The mutants of tests/test_temporal_ref_cpu.py need at least 0.41 at x_attn / x_out and 3.3 at gated: still far outside.
+# Cross-attention layers add four kinds, calibrated by tests/test_cross_ref_cpu.py on the bf16 cross oracle (dim 2048, 16
+# heads, T = 125 condition keys, B = 4 / 256):
+#   kx / vx, the condition memory with the rms per (row, head, key), need 4.7e-7 (one bf16 rounding of an fp32 product,
+#     inside the relative term) and get the floor 2^-10;   cross_out (rms per row and head) needs 0.0031 and gets 0.008;
+#   x_cross needs 0.0022 from the oracle but about 0.017 on the handle (tests/test_gpu_zz_cross_ref.py over all its cases, one
+#     H100 80GB HBM3, power limit 700 W: the update's own rounding one ulp away, as at x_attn) and gets x_attn's 0.035.
+# The cross mutants need at least 0.13 at cross_out, 0.86 at x_cross and 1.5 at kx.
 TM_REL = 2.0 ** -7
 TM_C = {"embed": 0.09, "k": 0.015, "v": 0.003, "attn_out": 0.027, "x_attn": 0.035, "gated": 0.15, "x_out": 0.03,
-        "transformer_out": 2.0 ** -10, "text_logits": 2.0 ** -10, "dep_in": 2.0 ** -10}
+        "transformer_out": 2.0 ** -10, "text_logits": 2.0 ** -10, "dep_in": 2.0 ** -10,
+        "kx": 2.0 ** -10, "vx": 2.0 ** -10, "cross_out": 0.008, "x_cross": 0.035}
 TM_KINDS = tuple(TM_C)
 
 
@@ -1008,13 +1101,16 @@ def tm_c_needed(got: torch.Tensor, want: torch.Tensor, scale: torch.Tensor | Non
 
 def tm_layer_checkpoints(want: dict, got: dict, rows: torch.Tensor) -> list[tuple[str, torch.Tensor, torch.Tensor, torch.Tensor | None]]:
     """(kind, got, want, rms source) of one layer in the order the layer computes them, the rms dimension last.  ``got`` holds
-    the implementation's "k" / "v" [R, H, D] (its ring entries at the step's slot), "attn_out", "x_attn", "gated", "x_out";
-    ``rows`` selects the executing rows for k and v (only they append)."""
+    the implementation's "k" / "v" [R, H, D] (its ring entries at the step's slot), "attn_out", "x_attn", "gated", "x_out",
+    and on a cross-attention layer (``want`` from temporal_layer_ref64 with ``cross``) "cross_out" and "x_cross" between
+    x_attn and gated; ``rows`` selects the executing rows for k and v (only they append)."""
     R = want["attn_out"].shape[0]
     H, D = want["attn_out"].shape[1:]
+    cross = [("cross_out", got["cross_out"].reshape(R, H, D), want["cross_out"], None),
+             ("x_cross", got["x_cross"], want["x_cross"], want["x_cross.upd"])] if "cross_out" in want else []
     return [("k", got["k"][rows], want["k"][rows], None), ("v", got["v"][rows], want["v"][rows], None),
             ("attn_out", got["attn_out"].reshape(R, H, D), want["attn_out"], None),
-            ("x_attn", got["x_attn"], want["x_attn"], want["x_attn.upd"]),
+            ("x_attn", got["x_attn"], want["x_attn"], want["x_attn.upd"]), *cross,
             ("gated", got["gated"], want["gated"], None),
             ("x_out", got["x_out"], want["x_out"], want["x_out.upd"])]
 
