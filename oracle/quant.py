@@ -55,14 +55,20 @@ def cached_quantize_weight(w: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]
     return val
 
 
+def qproduct_f32(qx: torch.Tensor, sa: torch.Tensor, qw: torch.Tensor, sw: torch.Tensor) -> torch.Tensor:
+    """The int8 x int8 product of quantised rows qx [M, K] (scales sa [M]) and qw [N, K] (scales sw [N]), dequantised in
+    fp32: [M, N]."""
+    acc = qx.double() @ qw.double().t()                       # exact integers (|acc| < 2^31)
+    scale = (sa[:, None] * sw[None, :]) * torch.tensor(float(INV_127_SQ), dtype=torch.float32)
+    return acc.float() * scale
+
+
 def qlinear_f32(x: torch.Tensor, w: torch.Tensor) -> torch.Tensor:
     """Dequantised product in fp32 (before the caller's bf16 rounding): [..., K] x [N, K] -> [..., N]."""
     qw, sw = cached_quantize_weight(w)
     lead = x.shape[:-1]
     qx, sa = quantize_rows(x.reshape(-1, x.shape[-1]))
-    acc = qx.double() @ qw.double().t()                       # exact integers (|acc| < 2^31)
-    scale = (sa[:, None] * sw[None, :]) * torch.tensor(float(INV_127_SQ), dtype=torch.float32)
-    return (acc.float() * scale).reshape(*lead, w.shape[0])
+    return qproduct_f32(qx, sa, qw, sw).reshape(*lead, w.shape[0])
 
 
 def qlinear(x: torch.Tensor, w: torch.Tensor) -> torch.Tensor:

@@ -19,6 +19,21 @@ previous-but-one token 0.13 / 0.004 at layer 0; norm2's alpha in norm1 0.25 / 0.
 not added 3.5 / 0.05.  A k-block missing from the LAST layer's linear_out only reaches the logits, where it moves them by 0.05
 to 0.1 rms, about the logits constant: it is not rejected in every row, so the mutant sits at layer 2, where the next layer's k
 rejects it.
+
+int8 (quantize=True): the int8 oracle (oracle/quant.py's QLinear in every linear) passes depformer_ref64(quantize=True) at every
+checkpoint, din bit for bit, under the DEP_C_*_I8 constants, on weights whose rows carry unequal int8 scales (dep_row_scaled:
+synthetic uniform weights give every row, linear and sub-step the same scale, which would hide a scale read from the wrong
+one).  Its mutants sit in layer 0, whose k / v the int8 oracle matches within the relative term: an activation row paired with
+its neighbour row's scale, another sub-step's weight scales, a truncating quantiser and a lost 128-wide int8 k-block of in_proj
+are rejected at layer 0's k (smallest admitting c 0.09 to 2.6, against 2^-7); a lost k-block of gate/value in or of linear_out
+at layer 1's k (0.79 and 0.27, against 0.25) and of the head at the logits (1.6 against 0.5).  Not claimed: the gate and value
+scales swapped, which needs only 0.245 at layer 1's k, below the 0.25 set there (twice the 0.126 the int8 oracle needs).
+
+Classifier-free guidance: the bf16 oracle's depformer_step with cfg_coef = 3 over 2B rows passes at every checkpoint of both
+halves with the bf16 constants, and its guided logits equal cfg_guide_bf16 of its model logits bit for bit.  Rejected in every
+row: the null rows fed the conditioned rows' transformer_out (at din), the null rows given another row's previous token (at
+layer 0's k), and, at the bit-exact guided logits, the combination with the halves swapped or with the previous sub-step's null
+logits.
 """
 import dataclasses
 
@@ -29,7 +44,9 @@ from moshi_b200.config import LMConfig
 from moshi_b200.synth import iter_synth_lm_tensors
 from oracle import transformer as tr
 from oracle.lm import LMOracle, LMSpec, scaled_embedding
-from tests.util import (DEP_C_DIN, DEP_C_LOGITS, c_needed, dep_c_kv, dep_checkpoints, dep_row_ratios, depformer_ref64)
+from tests.util import (DEP_C_DIN, DEP_C_LOGITS, DEP_C_LOGITS_I8, c_needed, cfg_guide64, cfg_guide_bf16, dep_c, dep_c_kv,
+                        dep_checkpoints,
+                        dep_row_ratios, dep_row_scaled, depformer_ref64, exact_row_ratios, greedy_unexcused)
 
 # the 7B depformer (dd 1024, 16 heads, ffn 2816, 6 layers, dep_q 8, card 2048) behind a 4096-wide temporal output
 CFG = LMConfig(num_layers=1, context=16)
@@ -43,8 +60,8 @@ def sd():
 
 
 def _oracle_frame(orc: LMOracle, sd: dict, tout: torch.Tensor, text_token: torch.Tensor) -> tuple[dict, torch.Tensor]:
-    """One frame of the bf16 oracle, greedy, with its per-frame cache kept: (checkpoints in depformer_ref64's layout, the
-    audio tokens [dep_q, B] it sampled)."""
+    """One frame of the oracle (bf16, or int8 with orc.quantize), greedy, with its per-frame cache kept: (checkpoints in
+    depformer_ref64's layout, the audio tokens [dep_q, B] it sampled)."""
     st = tr.init_state(orc.dep_spec, tout.shape[0], torch.bfloat16)
     prev, toks, logits = text_token, [], []
     for k in range(CFG.dep_q):
@@ -52,7 +69,7 @@ def _oracle_frame(orc: LMOracle, sd: dict, tout: torch.Tensor, text_token: torch
         logits.append(lg)
         prev = lg.float().argmax(-1)
         toks.append(prev)
-    din = torch.stack([tr.linear(tout, sd[f"depformer_in.{k}.weight"]) for k in range(CFG.dep_q)], dim=1)
+    din = torch.stack([tr.linear(tout, sd[f"depformer_in.{k}.weight"], orc.quantize) for k in range(CFG.dep_q)], dim=1)
     got = dict(din=din, k=[ls.k for ls in st.layers], v=[ls.v for ls in st.layers], logits=torch.stack(logits))
     return got, torch.stack(toks)
 
@@ -158,4 +175,243 @@ def test_mutant_rejected_at_its_checkpoint_in_every_row(sd, frames, name):
     cps = {(kd, kk, ll): (g, w) for kd, kk, ll, g, w in dep_checkpoints(got, want)}
     r = dep_row_ratios(*cps[(kind, k, layer)], kind, layer)
     print(f"{name}: rejected at {kind} sub-step {k} layer {layer}, row ratios {[round(float(x), 2) for x in r]}")
+    assert (r > 1).all(), (name, r)
+
+
+# ---- int8: LMModel(quantize=True), every depformer linear a QLinear --------------------------------------------------------
+def _kinds_needed(frames_: list, need: dict) -> None:
+    for _, _, _, got, want in frames_:
+        for kind, k, layer, g, w in dep_checkpoints(got, want):
+            key = kind if kind in ("din", "logits") else f"kv{layer}"
+            need[key] = max(need.get(key, 0.0), c_needed(g, w))
+
+
+@pytest.fixture(scope="module")
+def qsd(sd):
+    return dep_row_scaled(sd, seed=3)
+
+
+@pytest.fixture(scope="module")
+def qframes(qsd):
+    """As ``frames``, for the int8 oracle (oracle/quant.py's QLinear in every linear) against depformer_ref64(quantize=True), on
+    weights whose rows have unequal int8 scales (dep_row_scaled)."""
+    sd = qsd
+    orc = LMOracle({**sd, "text_emb.weight": torch.zeros(1, dtype=torch.bfloat16)}, LMSpec.from_config(CFG), use_sampling=False,
+                   quantize=True)
+    g = torch.Generator().manual_seed(6)
+    out = []
+    for _ in range(FRAMES):
+        tout = torch.randn(B, CFG.dim, generator=g).bfloat16()
+        text = torch.randint(0, CFG.text_card, (B,), generator=g)
+        got, toks = _oracle_frame(orc, sd, tout, text)
+        out.append((tout, text, toks, got, depformer_ref64(sd, CFG, tout, text, toks, quantize=True)))
+    return out
+
+
+def test_int8_oracle_passes_every_checkpoint(qframes):
+    """din is exact given transformer_out (one QLinear of a bf16 input), so it must match bit for bit; every other checkpoint
+    is held to the bf16 rule."""
+    need = {}
+    for _, _, _, got, want in qframes:
+        for kind, k, layer, g, w in dep_checkpoints(got, want):
+            r = exact_row_ratios(g, w) if kind == "din" else dep_row_ratios(g, w, kind, layer, int8=True)
+            assert not (r > 1).any(), (kind, k, layer, r)
+    _kinds_needed(qframes, need)
+    print("c the int8 oracle needs: " + ", ".join(f"{k} {v:.4f}" for k, v in need.items()))
+    print(f"c used: din exact, kv {[dep_c_kv(l, True) for l in range(CFG.depformer_num_layers)]}, logits {DEP_C_LOGITS_I8}")
+
+
+def test_int8_oracle_passes_layer0_at_serving_batch(qsd):
+    """Layer 0's k / v of the int8 oracle at B = 256, as test_bf16_oracle_passes_layer0_at_serving_batch does for bf16."""
+    from oracle.quant import qlinear
+    sd = qsd
+    Bs = 256
+    g = torch.Generator().manual_seed(8)
+    need = 0.0
+    for _ in range(FRAMES):
+        tout = torch.randn(Bs, CFG.dim, generator=g).bfloat16()
+        text = torch.randint(0, CFG.text_card, (Bs,), generator=g)
+        toks = torch.randint(0, CFG.card, (CFG.dep_q, Bs), generator=g)
+        want = depformer_ref64(sd, dataclasses.replace(CFG, depformer_num_layers=1), tout, text, toks, quantize=True)
+        prev = [text] + list(toks[:-1])
+        for k in range(CFG.dep_q):
+            emb = scaled_embedding(sd, "depformer_text_emb" if k == 0 else f"depformer_emb.{k - 1}", prev[k])
+            din = qlinear(tout, sd[f"depformer_in.{k}.weight"])
+            assert torch.equal(din, want["din"][:, k].bfloat16()), k
+            x = din + emb
+            xn = tr.apply_norm("rms_norm_f32", x[:, None], sd, "depformer.layers.0.norm1")[:, 0]
+            qkv = qlinear(xn, sd[f"depformer.layers.0.self_attn.in_projs.{k}.weight"]).view(Bs, 3, CFG.depformer_num_heads, 64)
+            for i, kind in ((1, "k"), (2, "v")):
+                w = want[kind][0][:, :, k]
+                need = max(need, c_needed(qkv[:, i], w))
+                assert not (dep_row_ratios(qkv[:, i], w, kind, 0, int8=True) > 1).any(), (kind, k)
+    print(f"int8 layer 0 at B = {Bs}: c the int8 oracle needs {need:.4f}, c used {dep_c_kv(0, True)}")
+
+
+def _qat(name: str, k: int, layer, f):
+    """A "qlinear" mutant that changes the quantised operands of one linear: f(x, q) -> q."""
+    def g(n, kk, ll, x, q):
+        return f(x, q) if (n, kk, ll) == (name, k, layer) else q
+    return {"qlinear": g}
+
+
+def _neighbour_scale(x, q):
+    return {**q, "sa": q["sa"].roll(-1)}                     # row b's integers dequantised with row b + 1's scale
+
+
+def _qkblock(x, q, kb: int = 5):
+    qx = q["qx"].clone()
+    qx[:, kb * 128:(kb + 1) * 128] = 0                          # one 128-byte int8 k-block of every row lost
+    return {**q, "qx": qx}
+
+
+def _gate_value_swapped(x, q):
+    F_ = q["sw"].numel() // 2
+    return {**q, "sw": torch.cat([q["sw"][F_:], q["sw"][:F_]])}
+
+
+def _truncating(x, q):
+    t = x.float()
+    absmax = t.abs().amax(dim=-1)
+    inv = torch.where(absmax > 0, torch.tensor(127.0, dtype=torch.float32) / absmax, torch.zeros_like(absmax))
+    return {**q, "qx": torch.trunc(t * inv[:, None]).clamp_(-127, 127).to(torch.int8)}
+
+
+def _other_step_scales(sd, name: str, layer):
+    from oracle.quant import cached_quantize_weight
+    from tests.util import _dep_tensor
+    return lambda x, q: {**q, "sw": cached_quantize_weight(_dep_tensor(sd, name, K - 1, layer))[1]}
+
+
+QMUTANTS = {
+    # name: (mutant of sd, (checkpoint kind, sub-step, layer) that must reject it in every row).  The int8 mutants sit in layer
+    # 0, whose k / v the int8 oracle matches to the relative term (c 2^-8), or act on its output at layer 1.
+    "activation row with its neighbour row's scale: in_proj": (lambda sd: _qat("in", K, 0, _neighbour_scale), ("k", K, 0)),
+    "weight scales of sub-step k-1: in_proj": (lambda sd: _qat("in", K, 0, _other_step_scales(sd, "in", 0)), ("k", K, 0)),
+    "int8 k-block missing: in_proj": (lambda sd: _qat("in", K, 0, _qkblock), ("k", K, 0)),
+    "int8 k-block missing: gate/value in": (lambda sd: _qat("lin_in", K, 0, _qkblock), ("k", K, 1)),
+    "int8 k-block missing: linear_out": (lambda sd: _qat("lin_out", K, 0, _qkblock), ("k", K, 1)),
+    "int8 k-block missing: head": (lambda sd: _qat("head", K, None, _qkblock), ("logits", K, None)),
+    "quantiser truncating: in_proj": (lambda sd: _qat("in", K, 0, _truncating), ("k", K, 0)),
+}
+
+
+# Not claimed: measured where they would be caught, but admitted by the constant set there.
+QMUTANTS_NOT_CLAIMED = {
+    "gate and value scales swapped": (lambda sd: _qat("lin_in", K, 0, _gate_value_swapped), ("k", K, 1)),
+}
+
+
+@pytest.mark.parametrize("name", list(QMUTANTS) + list(QMUTANTS_NOT_CLAIMED))
+def test_int8_mutant_rejected_at_its_checkpoint_in_every_row(qsd, qframes, name):
+    sd = qsd
+    make, (kind, k, layer) = {**QMUTANTS, **QMUTANTS_NOT_CLAIMED}[name]
+    tout, text, toks, _, want = qframes[0]
+    bad = depformer_ref64(sd, CFG, tout, text, toks, make(sd), quantize=True)
+    got = {n: [t.bfloat16() for t in v] if isinstance(v, list) else v.bfloat16() for n, v in bad.items()}
+    cps = {(kd, kk, ll): (g, w) for kd, kk, ll, g, w in dep_checkpoints(got, want)}
+    g, w = cps[(kind, k, layer)]
+    r = dep_row_ratios(g, w, kind, layer, int8=True)
+    need = min(c_needed(g[b:b + 1], w[b:b + 1]) for b in range(B))
+    print(f"{name}: rejected at {kind} sub-step {k} layer {layer}, row ratios {[round(float(x), 2) for x in r]}, "
+          f"smallest c admitting it {need:.3f} / {dep_c(kind, layer, True)}"
+          f"{' (not claimed)' if name in QMUTANTS_NOT_CLAIMED else ''}")
+    if name not in QMUTANTS_NOT_CLAIMED:
+        assert (r > 1).all(), (name, r)
+
+
+# ---- classifier-free guidance: 2B model rows, the samplers read the guided B rows ------------------------------------------
+COEF = 3.0
+
+
+@pytest.fixture(scope="module")
+def cfg_frames(sd):
+    """Per frame of the bf16 oracle's depformer_step with cfg_coef = 3 over 2B rows: (transformer_out [2B, dim], text token
+    [B], tokens [dep_q, B], checkpoints over 2B rows with the model's own logits, guided logits [dep_q, B, card] of the step,
+    depformer_ref64 of the 2B rows teacher-forced on the tokens repeated for the null half, as lm.py:826-832 feeds them)."""
+    orc = LMOracle({**sd, "text_emb.weight": torch.zeros(1, dtype=torch.bfloat16)}, LMSpec.from_config(CFG), use_sampling=False,
+                   cfg_coef=COEF, cfg_is_no_text=True)
+    g = torch.Generator().manual_seed(9)
+    out = []
+    for _ in range(FRAMES):
+        tout = torch.randn(2 * B, CFG.dim, generator=g).bfloat16()
+        text = torch.randint(0, CFG.text_card, (B,), generator=g)
+        rec, guided = {"model": []}, []
+        forward = orc.forward_depformer
+
+        def recording(k, prev, transformer_out, st):
+            lg = forward(k, prev, transformer_out, st)
+            rec["model"].append(lg[:, 0, 0])
+            rec["st"] = st
+            return lg
+        orc.forward_depformer = recording
+        try:
+            toks = orc.depformer_step(text, tout[:, None], logits_out=guided).T
+        finally:
+            del orc.forward_depformer
+        st = rec["st"]
+        din = torch.stack([tr.linear(tout, sd[f"depformer_in.{k}.weight"]) for k in range(CFG.dep_q)], dim=1)
+        got = dict(din=din, k=[ls.k for ls in st.layers], v=[ls.v for ls in st.layers], logits=torch.stack(rec["model"]))
+        want = depformer_ref64(sd, CFG, tout, text.repeat(2), toks.repeat(1, 2))
+        out.append((tout, text, toks, got, torch.stack([x[:, 0, 0] for x in guided]), want))
+    return out
+
+
+def test_cfg_oracle_passes_every_checkpoint_of_both_halves(cfg_frames):
+    need = {}
+    for _, _, toks, got, guided, want in cfg_frames:
+        for kind, k, layer, g, w in dep_checkpoints(got, want):
+            r = dep_row_ratios(g, w, kind, layer)
+            assert not (r > 1).any(), (kind, k, layer, r)
+        for k in range(CFG.dep_q):
+            # the step's guided logits are the reference's three bf16 operations on its own model logits
+            assert torch.equal(guided[k], cfg_guide_bf16(got["logits"][k], B, COEF)), k
+            # its tokens are the reference's guided tokens, unless the decision is within the guided logits' difference
+            ref = cfg_guide64(want["logits"][k], B, COEF)
+            need["guided"] = max(need.get("guided", 0.0), c_needed(guided[k], ref))
+            for b in range(B):
+                tol = float((guided[k][b].double() - ref[b]).abs().max()) + 1e-6
+                _, unexcused = greedy_unexcused(toks[k][b:b + 1], ref[b:b + 1].argmax(-1), ref[b:b + 1].float(), tol)
+                assert not unexcused, (k, b)
+    _kinds_needed([(None, None, None, got, want) for _, _, _, got, _, want in cfg_frames], need)
+    print(f"CFG {COEF}, 2B = {2 * B} rows: c the bf16 oracle needs " + ", ".join(f"{k} {v:.4f}" for k, v in need.items()))
+    print(f"c used: din {DEP_C_DIN}, kv {[dep_c_kv(l) for l in range(CFG.depformer_num_layers)]}, logits {DEP_C_LOGITS}, "
+          "guided logits exact against cfg_guide_bf16 of the model logits")
+
+
+def _cfg_swapped(model, k):
+    return cfg_guide_bf16(torch.cat([model[k][B:], model[k][:B]]), B, COEF)
+
+
+def _cfg_null_of_previous_step(model, k):
+    return cfg_guide_bf16(torch.cat([model[k][:B], model[k - 1][B:]]), B, COEF)
+
+
+CFG_MUTANTS = {
+    # name: (what the mutant changes, (checkpoint kind, sub-step, layer), rows that must reject it)
+    "null rows fed the conditioned rows' transformer_out": ("tout", ("din", 0, None), "null"),
+    "null rows given another row's previous token": ("prev", ("k", 0, 0), "null"),
+    "combination with the halves swapped": (_cfg_swapped, ("guided", K, None), "guided"),
+    "null logits of the previous sub-step": (_cfg_null_of_previous_step, ("guided", K, None), "guided"),
+}
+
+
+@pytest.mark.parametrize("name", list(CFG_MUTANTS))
+def test_cfg_mutant_rejected_at_its_checkpoint_in_every_row(sd, cfg_frames, name):
+    what, (kind, k, layer), rows = CFG_MUTANTS[name]
+    tout, text, toks, got, guided, want = cfg_frames[0]
+    if kind == "guided":            # the guided logits are held bit for bit to cfg_guide_bf16 of the model logits
+        r = exact_row_ratios(what(got["logits"], k), guided[k])
+    else:
+        if what == "tout":
+            bad = depformer_ref64(sd, CFG, torch.cat([tout[:B], tout[:B]]), text.repeat(2), toks.repeat(1, 2))
+        else:
+            assert (text != text.roll(-1)).all()           # else the mutant computes the right frame for that row
+            mut = {"prev": lambda kk, t: torch.cat([t[kk][:B], t[kk][:B].roll(-1)])}
+            bad = depformer_ref64(sd, CFG, tout, text.repeat(2), toks.repeat(1, 2), mut)
+        g = {n: [t.bfloat16() for t in v] if isinstance(v, list) else v.bfloat16() for n, v in bad.items()}
+        cps = {(kd, kk, ll): (gg, w) for kd, kk, ll, gg, w in dep_checkpoints(g, want)}
+        r = dep_row_ratios(*cps[(kind, k, layer)], kind, layer)[B:]
+    print(f"{name}: rejected at {kind} sub-step {k}{'' if layer is None else f' layer {layer}'} in the {rows} rows, "
+          f"row ratios {[round(float(x), 2) for x in r]}")
     assert (r > 1).all(), (name, r)

@@ -375,7 +375,7 @@ def _dep_tensor(sd: dict, name: str, k: int, layer: int | None) -> torch.Tensor:
 
 @torch.no_grad()
 def depformer_ref64(sd: dict, cfg, transformer_out: torch.Tensor, text_token: torch.Tensor, audio_tokens: torch.Tensor,
-                    mutant: dict | None = None) -> dict:
+                    mutant: dict | None = None, quantize: bool = False) -> dict:
     """One depformer frame (lm.py:450-493 and 809-850 with transformer.py's weights-per-step layers, as oracle/lm.py
     forward_depformer / depformer_step state it) in float64, teacher-forced: sub-step k's previous token is ``text_token`` [B]
     for k = 0 and ``audio_tokens[k - 1]`` ([dep_q, B], the tokens the model under test sampled) after.  Values are rounded to
@@ -384,6 +384,12 @@ def depformer_ref64(sd: dict, cfg, transformer_out: torch.Tensor, text_token: to
       out = bf16(softmax(q . k_j / 8) . v_j over the keys j = 0..k);  x = bf16(x + bf16(out_proj(out)));
       h = bf16(bf16(silu(bf16 g)) * bf16 u);  x = bf16(x + bf16(linear_out(h)));  logits = linears[k](x).
     Runs on transformer_out's device.  Weights are converted to float64 one (sub-step, layer) at a time, never all at once.
+
+    ``quantize`` (LMModel(quantize=True), every linear a QLinear): each linear of the frame (din, in, out, lin_in, lin_out and
+    head) is oracle/quant.py's restatement on the bf16 value at its cast point: the activation rows quantised in fp32 with
+    ties to even, the weight rows quantised through fp16 once (quant.cached_quantize_weight; the gate and value rows of lin_in
+    keep their own scales), the exact integer product, dequantised in qlinear_f32's fp32 order.  The RMSNorm, the attention
+    and the SiLU stay float64.
 
     Returns the checkpoints before their final bf16 rounding, as float64: "din" [B, dep_q, dd] (depformer_in[k] of
     transformer_out), "k" / "v" per layer [B, H, dep_q, 64] (what the layer's per-frame cache holds after the frame) and
@@ -394,7 +400,9 @@ def depformer_ref64(sd: dict, cfg, transformer_out: torch.Tensor, text_token: to
                 din, emb, in, out, lin_in, lin_out, n1, n2, head);
       "keys":   f(k, layer) -> (lo, hi): the keys the sub-step attends over (default (0, k + 1));
       "prev":   f(k, tokens) -> the previous tokens of sub-step k, tokens = [text_token, audio_tokens[0], ...];
-      "residual": f(k, layer, "attn" | "ffn") -> False to drop that residual."""
+      "residual": f(k, layer, "attn" | "ffn") -> False to drop that residual;
+      "qlinear": f(name, k, layer, x, q) -> q (quantize only): q = dict(qx, sa, qw, sw) holds the quantised activation rows,
+                 their scales, the quantised weight and its row scales of that linear, x its bf16 input."""
     mutant = mutant or {}
     dev, f64 = transformer_out.device, torch.float64
     B = transformer_out.shape[0]
@@ -404,19 +412,35 @@ def depformer_ref64(sd: dict, cfg, transformer_out: torch.Tensor, text_token: to
     def fetch(name, k, layer=None):
         return _dep_tensor(sd, name, k, layer)
 
+    def raw(name, k, layer=None):
+        return mutant["weight"](name, k, layer, fetch) if "weight" in mutant else fetch(name, k, layer)
+
     def W(name, k, layer=None):
-        t = mutant["weight"](name, k, layer, fetch) if "weight" in mutant else fetch(name, k, layer)
+        t = raw(name, k, layer)
         if name == "emb":
             return t                                    # only the rows of the previous tokens are gathered and converted
         t = t.to(dev, f64)
         return t.reshape(-1) if name in ("n1", "n2") else t
+
+    def lin(x, name, k, layer=None):
+        """x . w^T of one linear for bf16-valued x, before the output's rounding."""
+        if not quantize:
+            return x @ W(name, k, layer).T
+        from oracle.quant import cached_quantize_weight, qproduct_f32, quantize_rows
+        xb = x.to(torch.bfloat16)
+        qx, sa = quantize_rows(xb)
+        qw, sw = cached_quantize_weight(raw(name, k, layer).to(dev))
+        q = dict(qx=qx, sa=sa, qw=qw, sw=sw)
+        if "qlinear" in mutant:
+            q = mutant["qlinear"](name, k, layer, xb, q)
+        return qproduct_f32(q["qx"], q["sa"], q["qw"], q["sw"]).to(f64)
 
     def rmsnorm(x, alpha):
         return _bf(x * alpha / torch.sqrt(1e-8 + x.pow(2).mean(-1, keepdim=True)))
 
     tout = transformer_out.to(f64)
     tokens = [text_token.to(dev)] + [audio_tokens[k].to(dev) for k in range(Q - 1)]
-    din = torch.stack([tout @ W("din", k).T for k in range(Q)], dim=1)
+    din = torch.stack([lin(tout, "din", k) for k in range(Q)], dim=1)
     kc = [torch.zeros(B, H, Q, D, dtype=f64, device=dev) for _ in range(L)]
     vc = [torch.zeros(B, H, Q, D, dtype=f64, device=dev) for _ in range(L)]
     logits = []
@@ -427,21 +451,21 @@ def depformer_ref64(sd: dict, cfg, transformer_out: torch.Tensor, text_token: to
         x = _bf(_bf(din[:, k]) + e)
         for layer in range(L):
             xn = rmsnorm(x, W("n1", k, layer))
-            qkv = (xn @ W("in", k, layer).T).view(B, 3, H, D)
+            qkv = lin(xn, "in", k, layer).view(B, 3, H, D)
             kc[layer][:, :, k], vc[layer][:, :, k] = qkv[:, 1], qkv[:, 2]
             lo, hi = mutant["keys"](k, layer) if "keys" in mutant else (0, k + 1)
             s = torch.einsum("bhd,bhnd->bhn", _bf(qkv[:, 0]), _bf(kc[layer][:, :, lo:hi])) * 0.125
             o = _bf(torch.einsum("bhn,bhnd->bhd", torch.softmax(s, dim=-1), _bf(vc[layer][:, :, lo:hi]))).reshape(B, dd)
-            upd = _bf(o @ W("out", k, layer).T)
+            upd = _bf(lin(o, "out", k, layer))
             x = _bf(x + upd) if mutant.get("residual", lambda *a: True)(k, layer, "attn") else upd
             xn = rmsnorm(x, W("n2", k, layer))
-            gu = xn @ W("lin_in", k, layer).T
+            gu = lin(xn, "lin_in", k, layer)
             F_ = gu.shape[1] // 2
             g, u = _bf(gu[:, :F_]), _bf(gu[:, F_:])
             h = _bf(_bf(g * torch.sigmoid(g)) * u)
-            upd = _bf(h @ W("lin_out", k, layer).T)
+            upd = _bf(lin(h, "lin_out", k, layer))
             x = _bf(x + upd) if mutant.get("residual", lambda *a: True)(k, layer, "ffn") else upd
-        logits.append(x @ W("head", k).T)                                             # depformer_norms is Identity (lm.py:197-198)
+        logits.append(lin(x, "head", k))                                             # depformer_norms is Identity (lm.py:197-198)
     return dict(din=din, k=kc, v=vc, logits=torch.stack(logits))
 
 
@@ -461,10 +485,18 @@ def depformer_ref64(sd: dict, cfg, transformer_out: torch.Tensor, text_token: to
 DEP_C_DIN = 2.0 ** -10
 DEP_C_KV = (2.0 ** -8, 0.025, 0.04, 0.05, 0.0625, 0.094)
 DEP_C_LOGITS = 0.08
+# int8 (quantize=True, depformer_ref64(quantize=True)): din is exact given transformer_out and is checked bit for bit.  An
+# activation one bf16 ulp away from the reference's that sits on a rounding boundary of the row quantiser moves by a whole int8
+# step (about absmax / 127, several bf16 ulps of the rms), so the random walk through the layers is wider than in bf16.  The
+# int8 oracle on dep_row_scaled weights (the same shapes, B = 4, two frames, three draws) needs: k / v of layers 0..5 0,
+# 0.126, 0.237, 0.240, 0.251, 0.313, logits 0.257; layer 0 at B = 256 needs 0.0033.  Each constant is about twice that.
+DEP_C_KV_I8 = (2.0 ** -7, 0.25, 0.5, 0.5, 0.5, 0.625)
+DEP_C_LOGITS_I8 = 0.5
 
 
-def dep_c_kv(layer: int) -> float:
-    return DEP_C_KV[min(layer, len(DEP_C_KV) - 1)]
+def dep_c_kv(layer: int, int8: bool = False) -> float:
+    c = DEP_C_KV_I8 if int8 else DEP_C_KV
+    return c[min(layer, len(c) - 1)]
 
 
 def c_needed(got: torch.Tensor, want: torch.Tensor) -> float:
@@ -492,14 +524,56 @@ def dep_checkpoints(got: dict, want: dict) -> list[tuple[str, int, int | None, t
     return out
 
 
-def dep_c(kind: str, layer: int | None) -> float:
-    return DEP_C_DIN if kind == "din" else DEP_C_LOGITS if kind == "logits" else dep_c_kv(layer)
+def dep_c(kind: str, layer: int | None, int8: bool = False) -> float:
+    if kind == "din":
+        return DEP_C_DIN
+    if kind == "logits":
+        return DEP_C_LOGITS_I8 if int8 else DEP_C_LOGITS
+    return dep_c_kv(layer, int8)
 
 
-def dep_row_ratios(got: torch.Tensor, want: torch.Tensor, kind: str, layer: int | None) -> torch.Tensor:
-    """Worst err_ratios of each batch row of one checkpoint under its constant: [B] (<= 1 passes)."""
-    r = err_ratios(got, want, dep_c(kind, layer))
+def dep_row_ratios(got: torch.Tensor, want: torch.Tensor, kind: str, layer: int | None, int8: bool = False) -> torch.Tensor:
+    """Worst err_ratios of each batch row of one checkpoint under its constant (``int8``: the DEP_C_*_I8 constants): [B]
+    (<= 1 passes)."""
+    r = err_ratios(got, want, dep_c(kind, layer, int8))
     return r.reshape(r.shape[0], -1).amax(dim=1)
+
+
+def dep_row_scaled(sd: dict, seed: int = 0) -> dict:
+    """``sd`` with every row of each depformer linear (depformer_in, the in / out projections, gate / value, linear_out and the
+    heads) multiplied by its own factor 2^u, u uniform in [-1, 1].  Synthetic uniform weights give every row the same absmax,
+    hence the same int8 row scale in every linear and sub-step; trained weights do not.  On these weights a scale taken from
+    the wrong row, half, linear or sub-step changes the int8 product."""
+    g = torch.Generator().manual_seed(seed)
+    out = dict(sd)
+    for n, t in sd.items():
+        if n.startswith(("depformer_in.", "linears.")) or (n.startswith("depformer.layers.") and ".norm" not in n):
+            f = torch.exp2(torch.empty(t.shape[0]).uniform_(-1, 1, generator=g)).to(t.device)
+            out[n] = (t.float() * f[:, None]).to(t.dtype)
+    return out
+
+
+def exact_row_ratios(got: torch.Tensor, want: torch.Tensor) -> torch.Tensor:
+    """The verdict of a bit-exact checkpoint per batch row, on dep_row_ratios' scale: [B], 0 where the row equals bf16(want),
+    1e9 where any element differs."""
+    want = want.to(got.device).bfloat16()
+    bad = got.reshape(got.shape[0], -1) != want.reshape(want.shape[0], -1)
+    return bad.any(1).double().cpu() * 1e9
+
+
+# Classifier-free guidance (lm.py:728-732, 828-833): the model runs 2B rows, rows [0, B) conditioned and [B, 2B) null, and the
+# samplers read null + (cond - null) * coef.
+def cfg_guide_bf16(model_logits: torch.Tensor, B: int, coef: float) -> torch.Tensor:
+    """The guided logits as the reference computes them: three bf16 tensor operations on the model's bf16 logits [2B, card]
+    (bf16(n + bf16(bf16(l - n) * coef))): [B, card] bf16, for bit-exact checks."""
+    lg, null = model_logits[:B].bfloat16(), model_logits[B:2 * B].bfloat16()
+    return null + (lg - null) * coef
+
+
+def cfg_guide64(ref_logits: torch.Tensor, B: int, coef: float) -> torch.Tensor:
+    """The same combination in float64, of a reference's float64 logits [2B, card]: [B, card]."""
+    lg, null = ref_logits[:B].double(), ref_logits[B:2 * B].double()
+    return null + (lg - null) * coef
 
 
 # ---- fp64 reference of one Mimi streaming frame ----------------------------------------------------------------------------
