@@ -1,4 +1,5 @@
-"""CPU: the fp64 depformer reference and the acceptance rule of tests/test_gpu_zz_depformer_ref.py, at the 7B depformer shapes.
+"""CPU: the fp64 depformer reference and the acceptance rule of tests/test_gpu_zz_depformer_ref.py, at the 7B depformer shapes
+and at the 2B model's depformer (the same layer shapes over dep_q 16 sub-steps, depformer_in with K 2560).
 
 ``depformer_ref64`` restates one frame of the depformer in float64 with the bf16 model's cast points.  Two things are shown here:
 
@@ -7,6 +8,10 @@
 * The rule rejects depformers with a bug that leaves the greedy tokens mostly intact: each mutant below computes a subtly wrong
   frame, and the checkpoint named beside it must reject it in every batch row.  The mutants sit at sub-step 3 and layer 2 of 6
   unless said otherwise, so that keys before and after the newest one exist and the error has layers to cross.
+
+At the 2B depformer the oracle passes every layer at all 16 sub-steps (and layer 0 at B = 256), and a newest or first key
+dropped from sub-step 14's attention (15 keys), the last k-block of depformer_in, sub-step 13's weights or embedding table
+in sub-step 14 and a lost k-block of sub-step 15's head are each rejected in every row.
 
 Not claimed: ulp-level cast-point mutants (a missing bf16 round of the gate, of q, or of the attention output).  Such a bug moves
 a value by at most half a bf16 ulp, which is what the rule's 2^-7 relative term admits by design.
@@ -36,6 +41,8 @@ layer 0's k), and, at the bit-exact guided logits, the combination with the halv
 logits.
 """
 import dataclasses
+import json
+import pathlib
 
 import pytest
 import torch
@@ -50,13 +57,28 @@ from tests.util import (DEP_C_DIN, DEP_C_LOGITS, DEP_C_LOGITS_I8, c_needed, cfg_
 
 # the 7B depformer (dd 1024, 16 heads, ffn 2816, 6 layers, dep_q 8, card 2048) behind a 4096-wide temporal output
 CFG = LMConfig(num_layers=1, context=16)
+# the 2B model's depformer (tests/golden/moshi_dev_2b.json: the same layer shapes, but dep_q 16 sub-steps with
+# depformer_context 16, so the last sub-steps attend over up to 16 keys, and depformer_in reads a 2560-wide transformer_out)
+_2B = json.loads((pathlib.Path(__file__).parent / "golden" / "moshi_dev_2b.json").read_text())
+CFG_2B = LMConfig.from_dict({**{k: v for k, v in _2B.items() if k not in ("conditioners", "fuser")}, "num_layers": 1,
+                             "context": 16})
 B, FRAMES = 4, 2
 K, LAYER = 3, 2          # where the mutants act
+K_2B = 14                # where the 2B mutants act: 15 keys in the sub-step's attention
+
+
+def _dep_sd(cfg: LMConfig, seed: int) -> dict:
+    return {k: v for k, v in iter_synth_lm_tensors(cfg, seed=seed) if k.startswith(("depformer", "linears."))}
 
 
 @pytest.fixture(scope="module")
 def sd():
-    return {k: v for k, v in iter_synth_lm_tensors(CFG, seed=21) if k.startswith(("depformer", "linears."))}
+    return _dep_sd(CFG, 21)
+
+
+@pytest.fixture(scope="module")
+def sd_2b():
+    return _dep_sd(CFG_2B, 22)
 
 
 def _oracle_frame(orc: LMOracle, sd: dict, tout: torch.Tensor, text_token: torch.Tensor) -> tuple[dict, torch.Tensor]:
@@ -64,33 +86,42 @@ def _oracle_frame(orc: LMOracle, sd: dict, tout: torch.Tensor, text_token: torch
     depformer_ref64's layout, the audio tokens [dep_q, B] it sampled)."""
     st = tr.init_state(orc.dep_spec, tout.shape[0], torch.bfloat16)
     prev, toks, logits = text_token, [], []
-    for k in range(CFG.dep_q):
+    for k in range(orc.spec.dep_q):
         lg = orc.forward_depformer(k, prev[:, None], tout[:, None], st)[:, 0, 0]
         logits.append(lg)
         prev = lg.float().argmax(-1)
         toks.append(prev)
-    din = torch.stack([tr.linear(tout, sd[f"depformer_in.{k}.weight"], orc.quantize) for k in range(CFG.dep_q)], dim=1)
+    din = torch.stack([tr.linear(tout, sd[f"depformer_in.{k}.weight"], orc.quantize) for k in range(orc.spec.dep_q)], dim=1)
     got = dict(din=din, k=[ls.k for ls in st.layers], v=[ls.v for ls in st.layers], logits=torch.stack(logits))
     return got, torch.stack(toks)
+
+
+def _frames(sd: dict, cfg: LMConfig, seed: int) -> list:
+    orc = LMOracle({**sd, "text_emb.weight": torch.zeros(1, dtype=torch.bfloat16)}, LMSpec.from_config(cfg), use_sampling=False)
+    g = torch.Generator().manual_seed(seed)
+    out = []
+    for _ in range(FRAMES):
+        tout = torch.randn(B, cfg.dim, generator=g).bfloat16()
+        text = torch.randint(0, cfg.text_card, (B,), generator=g)
+        got, toks = _oracle_frame(orc, sd, tout, text)
+        out.append((tout, text, toks, got, depformer_ref64(sd, cfg, tout, text, toks)))
+    return out
 
 
 @pytest.fixture(scope="module")
 def frames(sd):
     """Per frame: (transformer_out, text token, the oracle's tokens, the oracle's checkpoints, depformer_ref64 of the frame)."""
-    orc = LMOracle({**sd, "text_emb.weight": torch.zeros(1, dtype=torch.bfloat16)}, LMSpec.from_config(CFG), use_sampling=False)
-    g = torch.Generator().manual_seed(5)
-    out = []
-    for _ in range(FRAMES):
-        tout = torch.randn(B, CFG.dim, generator=g).bfloat16()
-        text = torch.randint(0, CFG.text_card, (B,), generator=g)
-        got, toks = _oracle_frame(orc, sd, tout, text)
-        out.append((tout, text, toks, got, depformer_ref64(sd, CFG, tout, text, toks)))
-    return out
+    return _frames(sd, CFG, 5)
 
 
-def test_bf16_oracle_passes_every_checkpoint(frames):
+@pytest.fixture(scope="module")
+def frames_2b(sd_2b):
+    return _frames(sd_2b, CFG_2B, 4)
+
+
+def _oracle_passes(frames_: list) -> None:
     need = {}
-    for _, _, _, got, want in frames:
+    for _, _, _, got, want in frames_:
         for kind, k, layer, g, w in dep_checkpoints(got, want):
             key = kind if kind in ("din", "logits") else f"kv{layer}"
             need[key] = max(need.get(key, 0.0), c_needed(g, w))
@@ -100,29 +131,47 @@ def test_bf16_oracle_passes_every_checkpoint(frames):
     print(f"c used: din {DEP_C_DIN}, kv {[dep_c_kv(l) for l in range(CFG.depformer_num_layers)]}, logits {DEP_C_LOGITS}")
 
 
-def test_bf16_oracle_passes_layer0_at_serving_batch(sd):
-    """Layer 0's k / v at B = 256: only din, the embedding, RMSNorm and in_proj precede them, so their rare rounding flips are
-    sampled here over as many rows as the fused kernel serves (the oracle's own ops, against depformer_ref64 restricted to
-    layer 0, random tokens)."""
+def test_bf16_oracle_passes_every_checkpoint(frames):
+    _oracle_passes(frames)
+
+
+def test_bf16_oracle_passes_every_checkpoint_at_2b(frames_2b):
+    """All six layers at all 16 sub-steps of the 2B depformer."""
+    _oracle_passes(frames_2b)
+
+
+def _layer0_at_serving_batch(sd: dict, cfg: LMConfig, seed: int) -> None:
     Bs = 256
-    g = torch.Generator().manual_seed(7)
+    g = torch.Generator().manual_seed(seed)
     need = 0.0
     for _ in range(FRAMES):
-        tout = torch.randn(Bs, CFG.dim, generator=g).bfloat16()
-        text = torch.randint(0, CFG.text_card, (Bs,), generator=g)
-        toks = torch.randint(0, CFG.card, (CFG.dep_q, Bs), generator=g)
-        want = depformer_ref64(sd, dataclasses.replace(CFG, depformer_num_layers=1), tout, text, toks)
+        tout = torch.randn(Bs, cfg.dim, generator=g).bfloat16()
+        text = torch.randint(0, cfg.text_card, (Bs,), generator=g)
+        toks = torch.randint(0, cfg.card, (cfg.dep_q, Bs), generator=g)
+        want = depformer_ref64(sd, dataclasses.replace(cfg, depformer_num_layers=1), tout, text, toks)
         prev = [text] + list(toks[:-1])
-        for k in range(CFG.dep_q):
+        for k in range(cfg.dep_q):
             emb = scaled_embedding(sd, "depformer_text_emb" if k == 0 else f"depformer_emb.{k - 1}", prev[k])
             x = tr.linear(tout, sd[f"depformer_in.{k}.weight"]) + emb
             xn = tr.apply_norm("rms_norm_f32", x[:, None], sd, "depformer.layers.0.norm1")[:, 0]
-            qkv = tr.linear(xn, sd[f"depformer.layers.0.self_attn.in_projs.{k}.weight"]).view(Bs, 3, CFG.depformer_num_heads, 64)
+            qkv = tr.linear(xn, sd[f"depformer.layers.0.self_attn.in_projs.{k}.weight"]).view(Bs, 3, cfg.depformer_num_heads, 64)
             for i, kind in ((1, "k"), (2, "v")):
                 w = want[kind][0][:, :, k]
                 need = max(need, c_needed(qkv[:, i], w))
                 assert not (dep_row_ratios(qkv[:, i], w, kind, 0) > 1).any(), (kind, k)
     print(f"layer 0 at B = {Bs}: c the bf16 oracle needs {need:.4f}, c used {dep_c_kv(0)}")
+
+
+def test_bf16_oracle_passes_layer0_at_serving_batch(sd):
+    """Layer 0's k / v at B = 256: only din, the embedding, RMSNorm and in_proj precede them, so their rare rounding flips are
+    sampled here over as many rows as the fused kernel serves (the oracle's own ops, against depformer_ref64 restricted to
+    layer 0, random tokens)."""
+    _layer0_at_serving_batch(sd, CFG, 7)
+
+
+def test_bf16_oracle_passes_layer0_at_serving_batch_at_2b(sd_2b):
+    """As above for the 2B depformer: 16 sub-steps, depformer_in with K 2560."""
+    _layer0_at_serving_batch(sd_2b, CFG_2B, 8)
 
 
 def _kblock(name: str, k: int, layer, kb: int = 5):
@@ -178,6 +227,30 @@ def test_mutant_rejected_at_its_checkpoint_in_every_row(sd, frames, name):
     assert (r > 1).all(), (name, r)
 
 
+MUTANTS_2B = {
+    # at sub-step 14 of 16, where 15 keys are in the attention
+    "newest key dropped": ({"keys": lambda k, l: (0, k) if (k, l) == (K_2B, LAYER) else (0, k + 1)}, ("k", K_2B, LAYER + 1)),
+    "key 0 dropped": ({"keys": lambda k, l: (1, k + 1) if (k, l) == (K_2B, LAYER) else (0, k + 1)}, ("k", K_2B, LAYER + 1)),
+    "last k-block missing: depformer_in (K 2560)": (_kblock("din", 15, None, 2560 // 64 - 1), ("din", 15, None)),
+    "sub-step k-1 weights in one layer": (_swap({(n, K_2B, LAYER): (n, K_2B - 1, LAYER)
+                                                 for n in ("in", "out", "lin_in", "lin_out")}), ("k", K_2B, LAYER)),
+    "embedding table of sub-step k-1": (_swap({("emb", K_2B, None): ("emb", K_2B - 1, None)}), ("k", K_2B, 0)),
+    "k-block missing: head of sub-step 15": (_kblock("head", 15, None), ("logits", 15, None)),
+}
+
+
+@pytest.mark.parametrize("name", list(MUTANTS_2B))
+def test_mutant_rejected_at_2b_shapes(sd_2b, frames_2b, name):
+    mutant, (kind, k, layer) = MUTANTS_2B[name]
+    tout, text, toks, _, want = frames_2b[0]
+    bad = depformer_ref64(sd_2b, CFG_2B, tout, text, toks, mutant)
+    got = {n: [t.bfloat16() for t in v] if isinstance(v, list) else v.bfloat16() for n, v in bad.items()}
+    cps = {(kd, kk, ll): (g, w) for kd, kk, ll, g, w in dep_checkpoints(got, want)}
+    r = dep_row_ratios(*cps[(kind, k, layer)], kind, layer)
+    print(f"2B {name}: rejected at {kind} sub-step {k} layer {layer}, row ratios {[round(float(x), 2) for x in r]}")
+    assert (r > 1).all(), (name, r)
+
+
 # ---- int8: LMModel(quantize=True), every depformer linear a QLinear --------------------------------------------------------
 def _kinds_needed(frames_: list, need: dict) -> None:
     for _, _, _, got, want in frames_:
@@ -221,31 +294,39 @@ def test_int8_oracle_passes_every_checkpoint(qframes):
     print(f"c used: din exact, kv {[dep_c_kv(l, True) for l in range(CFG.depformer_num_layers)]}, logits {DEP_C_LOGITS_I8}")
 
 
-def test_int8_oracle_passes_layer0_at_serving_batch(qsd):
-    """Layer 0's k / v of the int8 oracle at B = 256, as test_bf16_oracle_passes_layer0_at_serving_batch does for bf16."""
+def _int8_layer0_at_serving_batch(sd: dict, cfg: LMConfig, seed: int) -> None:
     from oracle.quant import qlinear
-    sd = qsd
     Bs = 256
-    g = torch.Generator().manual_seed(8)
+    g = torch.Generator().manual_seed(seed)
     need = 0.0
     for _ in range(FRAMES):
-        tout = torch.randn(Bs, CFG.dim, generator=g).bfloat16()
-        text = torch.randint(0, CFG.text_card, (Bs,), generator=g)
-        toks = torch.randint(0, CFG.card, (CFG.dep_q, Bs), generator=g)
-        want = depformer_ref64(sd, dataclasses.replace(CFG, depformer_num_layers=1), tout, text, toks, quantize=True)
+        tout = torch.randn(Bs, cfg.dim, generator=g).bfloat16()
+        text = torch.randint(0, cfg.text_card, (Bs,), generator=g)
+        toks = torch.randint(0, cfg.card, (cfg.dep_q, Bs), generator=g)
+        want = depformer_ref64(sd, dataclasses.replace(cfg, depformer_num_layers=1), tout, text, toks, quantize=True)
         prev = [text] + list(toks[:-1])
-        for k in range(CFG.dep_q):
+        for k in range(cfg.dep_q):
             emb = scaled_embedding(sd, "depformer_text_emb" if k == 0 else f"depformer_emb.{k - 1}", prev[k])
             din = qlinear(tout, sd[f"depformer_in.{k}.weight"])
             assert torch.equal(din, want["din"][:, k].bfloat16()), k
             x = din + emb
             xn = tr.apply_norm("rms_norm_f32", x[:, None], sd, "depformer.layers.0.norm1")[:, 0]
-            qkv = qlinear(xn, sd[f"depformer.layers.0.self_attn.in_projs.{k}.weight"]).view(Bs, 3, CFG.depformer_num_heads, 64)
+            qkv = qlinear(xn, sd[f"depformer.layers.0.self_attn.in_projs.{k}.weight"]).view(Bs, 3, cfg.depformer_num_heads, 64)
             for i, kind in ((1, "k"), (2, "v")):
                 w = want[kind][0][:, :, k]
                 need = max(need, c_needed(qkv[:, i], w))
                 assert not (dep_row_ratios(qkv[:, i], w, kind, 0, int8=True) > 1).any(), (kind, k)
     print(f"int8 layer 0 at B = {Bs}: c the int8 oracle needs {need:.4f}, c used {dep_c_kv(0, True)}")
+
+
+def test_int8_oracle_passes_layer0_at_serving_batch(qsd):
+    """Layer 0's k / v of the int8 oracle at B = 256, as test_bf16_oracle_passes_layer0_at_serving_batch does for bf16."""
+    _int8_layer0_at_serving_batch(qsd, CFG, 8)
+
+
+def test_int8_oracle_passes_layer0_at_serving_batch_at_2b(sd_2b):
+    """The same at the 2B depformer: 16 sub-steps, depformer_in with K 2560."""
+    _int8_layer0_at_serving_batch(dep_row_scaled(sd_2b, seed=3), CFG_2B, 9)
 
 
 def _qat(name: str, k: int, layer, f):

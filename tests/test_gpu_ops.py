@@ -265,17 +265,19 @@ def test_gemv_with_folded_rmsnorm(lib, M, dim, epi):
     torch.testing.assert_close(y.float().cpu(), want.float(), rtol=2e-2, atol=3e-2)
 
 
-def _tie_free_top(B: int, card: int, n_top: int, gen: torch.Generator) -> torch.Tensor:
+def _tie_free_top(B: int, card: int, n_top: int, gen: torch.Generator, lo_index: int = 0) -> torch.Tensor:
     """bf16 logits whose n_top largest entries are pairwise distinct (bf16 cannot hold 32000 distinct
-    values in a sane range, so the bulk may tie; ties below the top-k never influence the sample)."""
-    bulk = (torch.randn(B, card, generator=gen) * 1.5).clamp(-6, 3.5).bfloat16()
-    # the 384 bf16 values in [4, 32): three binades x 128 mantissas
-    top_vals = torch.cat([torch.arange(128, dtype=torch.float32) * s + lo for lo, s in ((4, 2 ** -5), (8, 2 ** -4), (16, 2 ** -3))])
-    assert top_vals.bfloat16().float().unique().numel() == 384 and n_top <= 384
+    values in a sane range, so the bulk may tie; ties below the top-k never influence the sample), placed at indices
+    >= ``lo_index``."""
+    # the 384 bf16 values in [4, 32): three binades x 128 mantissas; for more, the 1152 in [1/16, 32) above a lower bulk
+    nb, bulk_hi = (3, 3.5) if n_top <= 384 else (9, 0.06)
+    bulk = (torch.randn(B, card, generator=gen) * 1.5).clamp(-6, bulk_hi).bfloat16()
+    top_vals = torch.cat([torch.arange(128, dtype=torch.float32) * 2.0 ** (e - 7) + 2.0 ** e for e in range(5 - nb, 5)])
+    assert top_vals.bfloat16().float().unique().numel() == 128 * nb and n_top <= 128 * nb
     out = bulk.clone()
     for b in range(B):
-        pos = torch.randperm(card, generator=gen)[:n_top]
-        vals = top_vals[torch.randperm(384, generator=gen)[:n_top]]
+        pos = lo_index + torch.randperm(card - lo_index, generator=gen)[:n_top]
+        vals = top_vals[torch.randperm(top_vals.numel(), generator=gen)[:n_top]]
         out[b, pos] = vals.bfloat16()
     return out
 
@@ -294,13 +296,27 @@ def _edge_rows(card: int, k: int, gen: torch.Generator) -> torch.Tensor:
     return torch.stack([tie, inf, ninf])
 
 
+def _high_index_rows(card: int, k: int, gen: torch.Generator) -> torch.Tensor:
+    """Four bf16 logit rows [4, card] for vocabularies past 32768, where the kernel's sort key holds the index as 0xFFFF - i
+    and indices >= 32768 clear bit 15 of that field: the top-(k+8) entirely at indices >= 32768; a tie at the top across
+    32767 / 32768 (the lower index wins); the same tie at the k-th place; the top-(k+8) at >= 32768 with a tie at the top
+    between 32768 and the last index."""
+    rows = _tie_free_top(4, card, min(card - 32768, k + 8), gen, lo_index=32768)
+    top = float(rows.float().max()) * 2
+    rows[1, [32767, 32768]] = top
+    kth = torch.sort(rows[2].float(), descending=True, stable=True).values[k - 1]
+    rows[2, [32767, 32768]] = kth.bfloat16()
+    rows[3, [32768, card - 1]] = top
+    return rows
+
+
 @pytest.mark.parametrize("card,k,temp", [(2048, 250, 0.8), (32000, 25, 0.7), (64, 250, 0.8), (500, 25, 0.7),
                                          (2048, 250, 6.0), (32000, 25, 9.0), (2048, 1, 0.8), (2048, 250, 1e-3),
-                                         (32000, 25, 1e-3)])
+                                         (32000, 25, 1e-3), (48000, 25, 0.7), (48000, 1024, 0.8), (48000, 1, 0.7)])
 def test_sampler_matches_oracle(lib, card, k, temp):
     """sample_token with shared Exp(1) noise on logits whose top-(k+8) entries are tie-free, then on the edge rows of
-    ``_edge_rows`` against the reference sampler with ties ranked by index (the order the kernel defines).  With k = 1 the
-    sample is the greedy token."""
+    ``_edge_rows`` (and past 32768 tokens those of ``_high_index_rows``) against the reference sampler with ties ranked by
+    index (the order the kernel defines), sampled and greedy.  With k = 1 the sample is the greedy token."""
     from moshi_b200 import _lib
     from oracle.lm import sample_token
     g = torch.Generator().manual_seed(3)
@@ -334,6 +350,20 @@ def test_sampler_matches_oracle(lib, card, k, temp):
     _lib.check(lib.b200_op_sample(cptr(ld), None, cptr(out), B, card, 0, temp, k, _stream()))
     torch.cuda.synchronize()
     assert torch.equal(out.cpu(), logits.float().argmax(-1))
+    if card <= 32768:
+        return
+    high = _high_index_rows(card, kk, g)
+    hn = torch.empty(high.shape[0], kk).exponential_(1, generator=g)
+    hd, hnd = high.cuda(), hn.cuda()
+    for sampling in (1, 0):
+        hwant = sample_token(high.float(), bool(sampling), temp, k, hn, tie_break="index")
+        hout = torch.empty(high.shape[0], dtype=torch.int64, device="cuda")
+        _lib.check(lib.b200_op_sample(cptr(hd), cptr(hnd) if sampling else None, cptr(hout), high.shape[0], card, sampling,
+                                      temp, k, _stream()))
+        torch.cuda.synchronize()
+        print(f"  rows past index 32767 ({'sampled' if sampling else 'greedy'}): got {hout.tolist()}, want {hwant.tolist()}")
+        assert torch.equal(hout.cpu(), hwant)
+    assert high.float()[[1, 3]].argmax(-1).tolist() == [32767, 32768]          # the rows hold the ties they are built for
 
 
 def test_sampler_ties_pick_lowest_index(lib):

@@ -18,11 +18,26 @@ the tokens repeated for the null half), int8 din bit for bit and the rest under 
 ``dep_logits`` and ``text_logits`` the samplers read must equal cfg_guide_bf16 of the model's own logits bit for bit (under
 cfg_is_no_text the text logits are the conditioned rows), and the reference's own token comes from cfg_guide64 of its logits.
 
-On one H100 80GB HBM3 (power limit 700 W) the whole file takes about 35 s.  The worst ratios of the guided and int8 cases
-(din, k / v, logits) were 0.48, 0.80, 0.58 under guidance and 0 (exact), 0.77, 0.52 with int8.
+The "2b" member is the 2B model's geometry (tests/golden/moshi_dev_2b.json) with one temporal layer: the full 6-layer
+depformer over dep_q 16 sub-steps, depformer_in with K 2560 and, in its sampled rows, the in-step text sampler over 48000
+logits, whose indices past 32767 clear bit 15 of the sampler key's index field.
+
+On one H100 80GB HBM3 (power limit 700 W) the whole file takes about 45 s.  The worst ratios of the guided and int8 cases
+(din, k / v, logits) were 0.48, 0.80, 0.58 under guidance and 0 (exact), 0.77, 0.52 with int8; the 2B member's fused,
+chain, GEMV and guided cases stayed below 0.47, 0.78 and 0.59, its int8 case (3, 33 and 129 sessions) at 0 (exact),
+0.53 and 0.58.
+
+A value the reference rounds to bf16 near a midpoint must be rounded correctly: torch casts float64 to bf16 through float32,
+which turns a value within half a float32 ulp of a midpoint into a tie.  At 129 sessions of the 2B int8 chain one row's
+layer-0 RMSNorm output had its largest element at -4.828125177 (fp64), past the midpoint of -4.8125 and -4.84375 by 1.8e-7:
+the handle rounded it to -4.84375, correctly, while the cast gave -4.8125.  That element is the row's int8 scale, so every
+element of the row re-quantised and layer-0 k / v moved by 5.5 / 4.6 times the rule; the handle's k is bit for bit the
+QLinear of the correctly rounded RMSNorm output.  tests/util.py's _bf now rounds float64 correctly.
 """
 import dataclasses
+import json
 import os
+import pathlib
 
 import pytest
 import torch
@@ -36,6 +51,7 @@ from tests.util import (cfg_guide64, cfg_guide_bf16, dep_checkpoints, dep_row_ra
 
 pytestmark = pytest.mark.gpu
 
+_2B = json.loads((pathlib.Path(__file__).parent / "golden" / "moshi_dev_2b.json").read_text())
 MEMBERS = {
     # one temporal layer of the 7B shape in front of the full 7B depformer (dd 1024, 16 heads, ffn 2816, 6 layers, dep_q 8)
     "7b": LMConfig(num_layers=1, context=16),
@@ -45,10 +61,15 @@ MEMBERS = {
     # ragged: ffn hidden 1000 (a K tail of 40 in linear_out, a partial 128-row tile in gate/value), card 1000, dd 512
     "ragged": LMConfig(dim=1024, num_heads=8, num_layers=1, context=16, text_card=1000, card=1000, depformer_dim=512,
                        depformer_num_heads=8, depformer_dim_feedforward=1500, depformer_num_layers=2),
+    # the 2B model (tests/golden/moshi_dev_2b.json) with one temporal layer: the full 6-layer depformer over 16 sub-steps,
+    # depformer_in with K 2560 and the in-step text sampler over 48000 logits (indices past 32767)
+    "2b": LMConfig.from_dict({**{k: v for k, v in _2B.items() if k not in ("conditioners", "fuser")}, "num_layers": 1,
+                              "context": 16}),
 }
 SAMPLING = {
     "7b": dict(temp=0.8, top_k=250, temp_text=0.7, top_k_text=25),
     "q16": dict(temp=0.8, top_k=250, temp_text=0.7, top_k_text=25),
+    "2b": dict(temp=0.8, top_k=250, temp_text=0.7, top_k_text=25),
     # top-k at or above the vocabulary (1024 is the sampler's largest): the text top-k moves where the audio noise starts, the
     # clamp to card sets its width
     "ragged": dict(temp=0.8, top_k=1024, temp_text=0.7, top_k_text=1000),
@@ -65,6 +86,9 @@ CASES = [
     ("q16", "chain", "0", (3, 65, 129), (65,)),
     ("ragged", "fused", None, (3, 65, 129), (3, 129)),
     ("ragged", "chain", "0", (3, 65, 129), (65,)),
+    ("2b", "fused", None, (3, 17, 64, 65, 129, 256), (3, 129, 256)),
+    ("2b", "chain", "0", (3, 65, 129), (65,)),
+    ("2b", "gemv", None, (1, 2), (2,)),
 ]
 # Classifier-free guidance and int8 linears: the handle builds no persistent kernel for either, so every frame runs the launch
 # chain over MB model rows (2B under guidance).  Batches sit on the schedule edges of MB: GEMV up to 2 rows (4 with gemv_rows),
@@ -79,6 +103,8 @@ CASES_CHAIN = [
     ("7b", "int8", (1, 2, 3, 32, 33, 64, 65, 128, 129, 256), (3, 129), dict(int8=True)),
     ("q16", "int8", (3, 65, 129), (65,), dict(int8=True)),
     ("7b", "int8-cfg3", (3, 65), (65,), dict(int8=True, cfg=3.0, no_text=True)),
+    ("2b", "cfg3-notext", (3, 65), (65,), dict(cfg=3.0, no_text=True)),
+    ("2b", "int8", (3, 33, 129), (129,), dict(int8=True)),
 ]
 FRAMES = 2                  # the second frame starts from the first frame's cache: it checks the per-frame restart
 

@@ -358,8 +358,16 @@ def rmsnorm_verdict(got: torch.Tensor, x: torch.Tensor, alpha: torch.Tensor) -> 
 
 # ---- fp64 reference of one depformer frame ---------------------------------------------------------------------------------
 def _bf(x: torch.Tensor) -> torch.Tensor:
-    """Round to bf16 and back (a cast point of the bf16 model)."""
-    return x.to(torch.bfloat16).to(x.dtype)
+    """Round to bf16 and back (a cast point of the bf16 model), to nearest with ties to even.  torch casts float64 to bf16
+    through float32, which turns a value within half a float32 ulp of a bf16 midpoint into a tie and can round it the wrong
+    way; float64 input therefore goes to float32 rounded to odd (toward zero, then the last bit set where inexact), after
+    which float32 -> bf16 rounds correctly."""
+    if x.dtype != torch.float64:
+        return x.to(torch.bfloat16).to(x.dtype)
+    f = x.float()
+    f = torch.where(f.double().abs() > x.abs(), torch.nextafter(f, torch.zeros_like(f)), f)
+    f = torch.where(f.double() != x, (f.view(torch.int32) | 1).view(torch.float32), f)
+    return f.to(torch.bfloat16).to(x.dtype)
 
 
 def _dep_tensor(sd: dict, name: str, k: int, layer: int | None) -> torch.Tensor:
@@ -482,8 +490,12 @@ def depformer_ref64(sd: dict, cfg, transformer_out: torch.Tensor, text_token: to
 # tail poorly: at B = 256 (two frames, the same test file) the oracle needs 0.0015 there (0.0019 with other draws), and
 # layer 0 gets 2^-8, twice the larger.  din gets
 # a floor of 2^-10 of the rms for fp32 accumulation in another order.
+# The 2B depformer (the same layer shapes, dep_q 16 sub-steps, depformer_in with K 2560) needs din 0, k / v 0.0002, 0.0126,
+# 0.0252, 0.0261, 0.0394, 0.0401, logits 0.0387, and 0.0019 at layer 0 at B = 256: layers 2 and 4 (0.04 and 0.0625 from the
+# 7B shapes, 1.6 times what they need there) get 0.05 and 0.08.  (Measured with _bf rounding float64 correctly; the 7B
+# numbers above were taken with torch's cast, which rounds through float32, and move by at most 0.005 with it.)
 DEP_C_DIN = 2.0 ** -10
-DEP_C_KV = (2.0 ** -8, 0.025, 0.04, 0.05, 0.0625, 0.094)
+DEP_C_KV = (2.0 ** -8, 0.025, 0.05, 0.05, 0.08, 0.094)
 DEP_C_LOGITS = 0.08
 # int8 (quantize=True, depformer_ref64(quantize=True)): din is exact given transformer_out and is checked bit for bit.  An
 # activation one bf16 ulp away from the reference's that sits on a rounding boundary of the row quantiser moves by a whole int8
@@ -1101,12 +1113,30 @@ def temporal_embed_ref64(sd: dict, cfg, input_tokens: torch.Tensor, condition_su
 
 
 @torch.no_grad()
+def temporal_embed_bf16(sd: dict, input_tokens: torch.Tensor, condition_sum: torch.Tensor | None = None) -> torch.Tensor:
+    """The summed input embeddings as the bf16 model computes them (lm.py:390-399, oracle/lm.py forward_text): the audio tables
+    emb.0 .. emb.<n_q - 1> in order, then text_emb, then ``condition_sum``, each add one bf16 tensor add (an fp32 sum rounded to
+    bf16).  Every bf16 implementation that adds in this order gets these bits: [MB, dim] bf16."""
+    tok = input_tokens
+    x = None
+    for k in list(range(1, tok.shape[1])) + [0]:
+        table = sd["text_emb.weight" if k == 0 else f"emb.{k - 1}.weight"]
+        t = tok[:, k].to(table.device)
+        e = torch.where((t >= 0)[:, None], table[t.clamp(min=0)], torch.zeros((), dtype=table.dtype, device=table.device))
+        x = e if x is None else x + e
+    if condition_sum is not None:
+        x = x + condition_sum.to(x.device, torch.bfloat16)
+    return x
+
+
+@torch.no_grad()
 def temporal_heads_ref64(sd: dict, cfg, x_last: torch.Tensor, tout: torch.Tensor, mutant: dict | None = None) -> dict:
     """The heads of the temporal transformer in float64, teacher-forced: "transformer_out" = rmsnorm(``x_last``, out_norm) (the
     implementation's x after the last layer), "text_logits" [MB, text_card] and "dep_in" [MB, dep_q, depformer_dim]
     (depformer_in[k] for every k, which the implementation writes as one [MB, dep_q * dd] product) of its ``tout``, all before
-    their final rounding.  ``mutant``: "weight" / "linear" as in temporal_layer_ref64 (names out_norm, head, din; din's layer is
-    the sub-step k)."""
+    their final rounding; with extra heads (the STT models) also "extra_heads" (extra_heads_ref64).  ``mutant``: "weight" /
+    "linear" as in temporal_layer_ref64 (names out_norm, head, din; din's layer is the sub-step k); it does not reach the
+    extra heads, whose mutants extra_heads_ref64 takes in its own form."""
     mutant = mutant or {}
     dev = tout.device
     W = _tm_weights(sd, None, mutant, dev)
@@ -1115,7 +1145,52 @@ def temporal_heads_ref64(sd: dict, cfg, x_last: torch.Tensor, tout: torch.Tensor
     if cfg.dep_q > 0:
         out["dep_in"] = torch.stack([_tm_linear(tout.double(), W("din", k), "din", k, cfg.quantize, mutant)
                                      for k in range(cfg.dep_q)], dim=1)
+    if cfg.extra_heads_num_heads > 0:
+        out["extra_heads"] = extra_heads_ref64(sd, cfg, tout)
     return out
+
+
+# ---- the extra heads of the STT models ---------------------------------------------------------------------------------------
+@torch.no_grad()
+def extra_heads_ref64(sd: dict, cfg, tout: torch.Tensor, mutant: dict | None = None) -> dict:
+    """softmax(extra_heads.<i>(transformer_out)) of every head (lm.py:224-226, 803-806) in float64, teacher-forced on the
+    implementation's ``tout`` [MB, dim] bf16: the logits tout . w_i^T in float64 rounded to bf16 (nn.Linear's output is a bf16
+    tensor), then a float64 softmax over the E = extra_heads_dim logits of the head.  Returns "logits" [n, MB, E] (bf16-valued)
+    and "p" [n, MB, E], the probabilities before their bf16 rounding.
+
+    ``mutant`` (for the tests of the rule): "weight": f(i, fetch) -> head i's [E, dim] weight (fetch(i) is right);
+    "logits": f(logits [n, MB, E] float64 before rounding) -> the logits the softmax of each head runs over (may add entries)."""
+    mutant = mutant or {}
+    n = cfg.extra_heads_num_heads
+
+    def fetch(i):
+        return sd[f"extra_heads.{i}.weight"]
+    x = tout.double()
+    w = [(mutant["weight"](i, fetch) if "weight" in mutant else fetch(i)).to(x.device, torch.float64) for i in range(n)]
+    lg = torch.stack([x @ wi.T for wi in w])
+    if "logits" in mutant:
+        lg = mutant["logits"](lg)
+    lg = _bf(lg)
+    return {"logits": lg[..., :cfg.extra_heads_dim], "p": torch.softmax(lg, dim=-1)[..., :cfg.extra_heads_dim]}
+
+
+def _bf16_ulp(x: torch.Tensor) -> torch.Tensor:
+    """The spacing of bf16 numbers just above |x| (float64; the smallest normal's spacing at 0)."""
+    e = torch.floor(torch.log2(x.abs().clamp(min=2.0 ** -126)))
+    return torch.exp2(e - 7)
+
+
+def extra_heads_ratios(got: torch.Tensor, ref: dict) -> torch.Tensor:
+    """Worst |got - p| / tol of each (head, row) of the extra heads' probabilities ``got`` [n, MB, E] (bf16): [n, MB], <= 1
+    passes.  The implementation's bf16 logit may land one bf16 ulp u_j away from the reference's (an fp32 sum in another order
+    near a rounding boundary), which moves p_i by at most p_i (u_i + sum_j p_j u_j) to first order; its fp32 softmax adds a
+    relative 2^-16 and the bf16 rounding of the probability half an ulp of p:
+        tol_i = 1.25 p_i (u_i + sum_j p_j u_j) + 2^-16 p_i + ulp(p_i) / 2."""
+    p, u = ref["p"], _bf16_ulp(ref["logits"])
+    got = got.to(p.device, torch.float64).reshape(p.shape)
+    tol = 1.25 * p * (u + (p * u).sum(-1, keepdim=True)) + 2.0 ** -16 * p + 0.5 * _bf16_ulp(p)
+    r = torch.nan_to_num((got - p).abs() / tol, nan=math.inf, posinf=math.inf)
+    return r.amax(-1)
 
 
 # Acceptance rule of the temporal checkpoints: |got - want| <= TM_REL |want| + c rms, one c per checkpoint kind for every layer.
@@ -1130,6 +1205,14 @@ def temporal_heads_ref64(sd: dict, cfg, x_last: torch.Tensor, tout: torch.Tensor
 # B = 256 samples the rare rounding flips (a gate input one ulp off moves silu(g) u by far more than its rms share) that four
 # rows miss, so it sets the constants.  transformer_out and the heads need nothing beyond the relative term: they get a floor
 # of 2^-10 for fp32 accumulation in another order.
+# At the 2B shapes (tests/golden/moshi_dev_2b.json: dim 2560, 20 heads, ffn 7040, RoPE period 1e5, 33 embedding tables and a
+# condition sum, text_card 48000, depformer_in 16 x 1024; two layers, B = 4 / 256, the same test file) the oracle needs:
+#   embed 0.010 / 0.013, k 1.6e-6 / 0.0124, v 0 / 5.9e-4, attn_out 0.0081 / 0.012, x_attn 0 / 0.0042, gated 1.6e-4 / 0.014,
+#   x_out 0 / 0.012, transformer_out 0 / 0, text_logits 8.3e-9 / 3.7e-7, dep_in 7.9e-9 / 2.8e-7.
+# k (0.015 from the 7B shapes, 1.2 times that) gets 0.025; the k mutants need at least 0.48 at either geometry.  How much of
+# embed's constant a correct sum needs depends on the tables' values: on tiled_lm_state_dict weights with a condition sum the
+# handle's sum, bit-exact to the reference's order of bf16 adds, reached 0.83 of it.  tests/test_gpu_zz_temporal_ref.py
+# therefore holds the embeddings bit for bit to temporal_embed_bf16, which every bf16 implementation in that order computes.
 # Three kinds are set from what the handle needs instead (tests/test_gpu_zz_temporal_ref.py over all its cases, one H100 80GB
 # HBM3, power limit 700 W), because the handle samples the same rare flips over far more rows and layers than the oracle:
 #   x_attn 0.017 and x_out 0.013: the update's own bf16 rounding may land one ulp away from the reference's (fp32 sums in
@@ -1145,7 +1228,7 @@ def temporal_heads_ref64(sd: dict, cfg, x_last: torch.Tensor, tout: torch.Tensor
 #     H100 80GB HBM3, power limit 700 W: the update's own rounding one ulp away, as at x_attn) and gets x_attn's 0.035.
 # The cross mutants need at least 0.13 at cross_out, 0.86 at x_cross and 1.5 at kx.
 TM_REL = 2.0 ** -7
-TM_C = {"embed": 0.09, "k": 0.015, "v": 0.003, "attn_out": 0.027, "x_attn": 0.035, "gated": 0.15, "x_out": 0.03,
+TM_C = {"embed": 0.09, "k": 0.025, "v": 0.003, "attn_out": 0.027, "x_attn": 0.035, "gated": 0.15, "x_out": 0.03,
         "transformer_out": 2.0 ** -10, "text_logits": 2.0 ** -10, "dep_in": 2.0 ** -10,
         "kx": 2.0 ** -10, "vx": 2.0 ** -10, "cross_out": 0.008, "x_cross": 0.035}
 TM_KINDS = tuple(TM_C)
