@@ -455,8 +455,18 @@ int b200_op_linear_sk(const void* x_dev, const void* w_tiles_dev, void* y_dev, c
 int b200_op_linear_ns(const void* x_dev, const void* w_tiles_dev, void* y_dev, const void* res_dev, int M, int N, int K,
                       int epi, int gate_rows, int cluster, void* stream);
 /* Up to how many activation rows the linears take the GEMV path (plain 16-byte loads on the CUDA cores instead of the
- * tensor-core GEMM; csrc/gemm_sk.cu): 0..4, default 2 (or B200_GEMV_MAX_M).  Returns the previous value. */
+ * tensor-core GEMM; csrc/gemm_sk.cu): 0..4, default 2.  Returns the previous value. */
 int b200_op_set_gemv_max_rows(int max_rows);
+/* The launches the LM makes for one linear (b200_op_linear_sk / b200_op_linear_i8 with the LM's own choice, rows contiguous), for a
+ * device of `sms` multiprocessors and GEMV path up to `gemv_max_rows` rows; needs no GPU.  norm: an RMSNorm in front, folded
+ * where the plan takes the GEMV.  out[0] = launches, out[1] = 1 if the norm is folded, then 19 values per launch: kernel
+ * (1 GEMV, 2 non-swapped, 3 cluster split-K, 4 swap-AB stream-K), first row, rows, grid, cluster size, dynamic shared memory,
+ * stages, stage bytes, activation box rows, padded rows, k-blocks per split, GEMV splits, GEMV k-blocks per split,
+ * weight tiles per unit, receive row floats, cluster columns per rank, whole rounds, first stream-K tile, stream-K items
+ * (0 where a kernel has no such parameter).  `capacity` int64 slots at out; 2 + 4 * 19 always suffice.  Returns the errors
+ * the linear would return for the shape. */
+int b200_op_linear_plan(int M, int N, int K, int epi, int gate_rows, int int8, int norm, int sms, int gemv_max_rows, int64_t* out,
+                        int capacity);
 /* int8 x int8 linear (QLinear, utils/quantize.py:13-40: bitsandbytes row-wise absmax quantisation of weights and
  * activations, int32 accumulation, dequantisation by both row scales / 127^2), on wgmma s8 x s8 -> s32.
  *   b200_op_quant_pack_tiles: w bf16 [N,K] -> int8 SWIZZLE_128B tiles (b200_op_packed_bytes_i8 bytes) + scales f32 [N]
@@ -529,7 +539,8 @@ int b200_op_layernorm(const void* x_dev, const void* w_dev, const void* b_dev, v
 int b200_op_cross_attn_step(const void* q_dev, const void* k_dev, const void* v_dev, void* out_dev, int B, int H, int T, int nsplit,
                             void* stream);
 /* b200_op_linear_sk on rmsnorm(x, alpha) with the norm folded into the GEMV kernel's activation staging (the LM's path for one
- * or two sessions).  Only the GEMV path takes a norm: for M above b200_op_set_gemv_max_rows it returns B200_ERR_STATE. */
+ * or two sessions).  Only the GEMV path takes a norm: where the plan takes another kernel (for M above
+ * b200_op_set_gemv_max_rows) it returns B200_ERR_STATE. */
 int b200_op_linear_sk_norm(const void* x_dev, const void* alpha_dev, const void* w_tiles_dev, void* y_dev, const void* res_dev, int M,
                            int N, int K, int epi, int gate_rows, void* stream);
 /* sample_token (sampling.py:86-106): logits bf16 [B,card], noise f32 [B,min(k,card)] -> i64 [B]. */

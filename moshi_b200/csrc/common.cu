@@ -1,6 +1,6 @@
 #include <algorithm>
 
-#include "common.cuh"
+#include "tc_host.cuh"
 
 namespace b200 {
 
@@ -135,6 +135,41 @@ int row_slice_copy(const RowSlice* table_dev, int n, long long max_row_bytes, ch
   const unsigned gx = (unsigned)std::min<long long>(std::max<long long>(ceil_div64(max_row_bytes, 16 * 256), 1), 256);
   B200_LAUNCH(row_slice_copy_kernel, dim3(gx, n), 256, 0, st, table_dev, rec, row, gather ? 1 : 0);
   return check_launch("row_slice_copy");
+}
+
+int encode_tiled(CUtensorMap* m, CUtensorMapDataType type, cuuint32_t rank, const void* base, const cuuint64_t* dims,
+                 const cuuint64_t* strides, const cuuint32_t* box, const cuuint32_t* estr, const char* what) {
+  typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+  static EncodeTiledFn encode = nullptr;
+  if (!encode) {
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    B200_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
+    if (!fn || qres != cudaDriverEntryPointSuccess) B200_FAIL(B200_ERR_CUDA, "cuTensorMapEncodeTiled not available");
+    encode = reinterpret_cast<EncodeTiledFn>(fn);
+  }
+  const CUresult r = encode(m, type, rank, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) B200_FAIL(B200_ERR_CUDA, "%s: cuTensorMapEncodeTiled failed (%d)", what, (int)r);
+  return B200_OK;
+}
+
+int act_map(CUtensorMap* m, const void* base, long long ld, int rows, int cols, int box_rows, int elem_bytes) {
+  const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  const cuuint64_t strides[1] = {(cuuint64_t)ld * elem_bytes};
+  const cuuint32_t box[2] = {(cuuint32_t)(128 / elem_bytes), (cuuint32_t)box_rows};
+  const cuuint32_t estr[2] = {1, 1};
+  return encode_tiled(m, elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, base, dims, strides, box,
+                      estr, "activation map");
+}
+
+int num_sms() {
+  static int sms = 0;
+  int dev = 0;
+  if (!sms && cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  return sms;
 }
 
 }  // namespace b200

@@ -431,22 +431,6 @@ dep_fused_kernel(const __grid_constant__ CUtensorMap map_xn, const __grid_consta
   }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-int make_map(EncodeTiledFn enc, CUtensorMap* m, const void* ptr, int rows, int cols, int box_rows) {
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)cols * 2};
-  cuuint32_t box[2] = {(cuuint32_t)BLOCK_K, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) B200_FAIL(B200_ERR_CUDA, "depformer: cuTensorMapEncodeTiled failed (%d)", (int)r);
-  return B200_OK;
-}
-
 Gemm plan(int N, int K, int A, int M, int grid) {
   Gemm g;
   g.wt = nullptr; g.A = A; g.N = N;
@@ -476,7 +460,7 @@ struct DepFused {
 };
 
 size_t dep_fused_partial_floats(const DepFusedConfig& c) {
-  const int grid = sk_num_sms();
+  const int grid = num_sms();
   size_t mx = 0;
   const Gemm gs[5] = {plan(3 * c.dd, c.dd, 1, c.B, grid), plan(c.dd, c.dd, 1, c.B, grid), plan(c.F, c.dd, 2, c.B, grid),
                       plan(c.dd, c.F, 1, c.B, grid), plan(c.card, c.dd, 1, c.B, grid)};
@@ -490,15 +474,10 @@ size_t dep_fused_partial_floats(const DepFusedConfig& c) {
 int dep_fused_create(const DepFusedConfig& c, DepFused** out) {
   if (c.dd % 64 || c.dd > 4 * THREADS || c.dd / c.H != DD || c.dep_q > lm::DEP_MAX_Q || c.dep_q < 1 || c.F % 8 || c.B < 1 || c.B > 256)
     B200_FAIL(B200_ERR_INVALID, "fused depformer: unsupported configuration");
-  void* fn = nullptr;
-  cudaDriverEntryPointQueryResult qres;
-  B200_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
-  if (!fn || qres != cudaDriverEntryPointSuccess) B200_FAIL(B200_ERR_CUDA, "cuTensorMapEncodeTiled not available");
-  EncodeTiledFn enc = reinterpret_cast<EncodeTiledFn>(fn);
   DepFused* d = new DepFused();
   DepParams& p = d->p;
   memset(&p, 0, sizeof(p));
-  d->grid = sk_num_sms();
+  d->grid = num_sms();
   p.B = c.B; p.Mpad = ((c.B + 15) / 16) * 16; p.dd = c.dd; p.H = c.H; p.F = c.F; p.card = c.card; p.text_card = c.text_card; p.err = c.err; p.dep_q = c.dep_q; p.L = c.L;
   p.stage_bytes = (uint32_t)(2 * TILE_BYTES + MC * BLOCK_K * 2);
   int stages = (200 * 1024) / (int)p.stage_bytes;
@@ -544,10 +523,10 @@ int dep_fused_create(const DepFusedConfig& c, DepFused** out) {
   p.noise = c.noise; p.noise_ld = c.noise_ld; p.noise_off = c.noise_off; p.ka = c.ka;
   p.use_sampling = c.use_sampling; p.top_k = c.top_k; p.temp = c.temp;
   p.bar = c.bar; p.trace = c.trace;
-  B200_TRY(make_map(enc, &d->map_xn, c.xn, c.B, c.dd, MC));
-  B200_TRY(make_map(enc, &d->map_ao, c.ao, c.B, c.dd, MC));
-  B200_TRY(make_map(enc, &d->map_h, c.hbuf, c.B, c.F, MC));
-  B200_TRY(make_map(enc, &d->map_x, c.x, c.B, c.dd, MC));
+  B200_TRY(act_map(&d->map_xn, c.xn, c.dd, c.B, c.dd, MC, 2));
+  B200_TRY(act_map(&d->map_ao, c.ao, c.dd, c.B, c.dd, MC, 2));
+  B200_TRY(act_map(&d->map_h, c.hbuf, c.F, c.B, c.F, MC, 2));
+  B200_TRY(act_map(&d->map_x, c.x, c.dd, c.B, c.dd, MC, 2));
   d->smem = (size_t)stages * p.stage_bytes + 1024 + 16 * MAX_STAGES + 64;
   B200_CUDA(cudaFuncSetAttribute(dep_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
   int per_sm = 0, coop = 0, dev = 0;
@@ -577,17 +556,10 @@ void dep_fused_destroy(DepFused* d) {
 // barrier cannot deadlock against another handle's persistent kernel, an MPS neighbour or a second replica on the same GPU.
 int dep_fused_launch(DepFused* d, cudaStream_t stream) {
   B200_CUDA(cudaMemsetAsync(d->p.bar, 0, sizeof(unsigned), stream));
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3((unsigned)d->grid); cfg.blockDim = dim3(THREADS); cfg.dynamicSmemBytes = d->smem; cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeCooperative;
-  attr[0].val.cooperative = 1;
-  cfg.attrs = attr; cfg.numAttrs = 1;
-  const cudaError_t le = cudaLaunchKernelEx(&cfg, dep_fused_kernel, d->map_xn, d->map_ao, d->map_h, d->map_x, d->p);
-  if (le != cudaSuccess) B200_FAIL(B200_ERR_CUDA, "fused depformer: cooperative launch failed: %s", cudaGetErrorString(le));
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  return check_launch("dep_fused");
+  LaunchOpts o;
+  o.cooperative = true;
+  return launch("dep_fused", dep_fused_kernel, dim3((unsigned)d->grid), dim3(THREADS), d->smem, stream, o, d->map_xn, d->map_ao, d->map_h,
+                d->map_x, d->p);
 }
 
 }  // namespace tc

@@ -5,7 +5,7 @@
 //
 //   * A = the activations, one [128 sessions x 64 k] SWIZZLE_128B box per k-block (2-D TMA, rows beyond M zero-filled);
 //     consumer warpgroup w multiplies sessions 64w..64w+63 (a warpgroup without sessions skips its MMAs).  Above 128
-//     sessions ns_linear runs two launches, one per block of 128 sessions;
+//     sessions the plan runs two launches, one per block of 128 sessions;
 //   * B = TWO pre-tiled 128-row weight tiles side by side (N = 256 per instruction: twice the weight bytes per MMA);
 //     for the gated MLP the pair is (gate rows, value rows) of the same outputs, already stored back to back, so the
 //     accumulator holds gate in columns 0..127 and value in 128..255 of the SAME thread and silu(g) * u needs no exchange;
@@ -15,7 +15,7 @@
 //     32 single tiles x 4, N = 128 per instruction there so that 128 SMs pull on the weights); the partial accumulators are
 //     reduce-scattered over distributed shared memory by output columns (the stage ring is dead by then and serves as the
 //     receive buffer), summed in rank order (deterministic) and stored by the owning rank: no workspace, no atomics.
-//     ns_default_plan() holds the choice per shape.
+//     ns_default_plan() (gemm_sk.cu) holds the choice per shape.
 //
 // Same packed weights, same epilogues and cast points as gemm_sk.cu (residual add bf16(res + bf16(acc)), gated SiLU
 // bf16(bf16(silu(g)) * u), gating.py:18-20); same PDL protocol (weights requested before griddepcontrol.wait).
@@ -35,9 +35,8 @@ constexpr int NUM_THREADS = 288;             // warps 0-7: two consumer warpgrou
 constexpr int PRODUCER_WARP = 8;
 constexpr int CONSUMERS = 256;
 constexpr int TILE_BYTES = BLOCK_ROWS * BLOCK_K * 2;
-constexpr int A_BYTES = 128 * BLOCK_K * 2;   // one activation box: 128 session rows x 64 k
-constexpr int MAX_STAGES = 8;
-constexpr int MAX_CS = 8;
+constexpr int A_BYTES = NS_A_BYTES;         // one activation box: 128 session rows x 64 k
+constexpr int MAX_STAGES = NS_MAX_STAGES;
 
 struct NsParams {
   int M, N, K, out_rows, gate_rows, CS, num_kb, kb_per, stages, n_tiles, ldw;
@@ -45,20 +44,6 @@ struct NsParams {
   __nv_bfloat16* y; long long ldy;
   const __nv_bfloat16* res; long long ldr;
 };
-
-__device__ __forceinline__ uint32_t ns_map_to_rank(uint32_t local_smem_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_smem_addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void ns_st_cluster_v2(uint32_t addr, uint32_t a, uint32_t b) {
-  asm volatile("st.shared::cluster.v2.b32 [%0], {%1, %2};" ::"r"(addr), "r"(a), "r"(b) : "memory");
-}
-__device__ __forceinline__ void ns_cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ float ns_bf16_round(float v) { return __bfloat162float(__float2bfloat16_rn(v)); }
 
 // first accumulator column of rank q's share of `width` columns (multiples of 16; the last rank takes the remainder)
 __device__ __forceinline__ int col_begin(int width, int cs, int q) { return q >= cs ? width : ((width * q / cs) >> 4) << 4; }
@@ -212,8 +197,8 @@ gemm_ns_kernel(const __grid_constant__ CUtensorMap tmap_x, const NsParams p) {
           float v[2];
 #pragma unroll
           for (int j = 0; j < 2; ++j) {
-            const float gt = ns_bf16_round(__uint_as_float(d[i + j])), ut = ns_bf16_round(__uint_as_float(d[64 + i + j]));
-            v[j] = ns_bf16_round(gt / (1.f + expf(-gt))) * ut;
+            const float gt = bf16_round(__uint_as_float(d[i + j])), ut = bf16_round(__uint_as_float(d[64 + i + j]));
+            v[j] = bf16_round(gt / (1.f + expf(-gt))) * ut;
           }
           store2(p.y + (long long)m * p.ldy + n, v, p.out_rows - n);
         }
@@ -228,7 +213,7 @@ gemm_ns_kernel(const __grid_constant__ CUtensorMap tmap_x, const NsParams p) {
           if (EPI == EPI_RESADD) {
             float rv[2];
             load2(p.res + (long long)m * p.ldr + n, rv, p.out_rows - n);
-            v[0] = rv[0] + ns_bf16_round(v[0]); v[1] = rv[1] + ns_bf16_round(v[1]);
+            v[0] = rv[0] + bf16_round(v[0]); v[1] = rv[1] + bf16_round(v[1]);
           }
           store2(p.y + (long long)m * p.ldy + n, v, p.out_rows - n);
         }
@@ -237,7 +222,7 @@ gemm_ns_kernel(const __grid_constant__ CUtensorMap tmap_x, const NsParams p) {
     return;
   }
   // K split over the cluster: column c of every rank's accumulator goes to the rank that owns c, slot = sender rank
-  ns_cluster_sync();                            // every rank's MMAs have retired: the rings are free to receive
+  cluster_sync_all();                            // every rank's MMAs have retired: the rings are free to receive
   if (warp != PRODUCER_WARP) {
 #pragma unroll
     for (int i = 0; i < NW / 2; i += 2) {
@@ -245,12 +230,12 @@ gemm_ns_kernel(const __grid_constant__ CUtensorMap tmap_x, const NsParams p) {
       if (c < width && m < p.M) {
         int q = 0;
         while (c >= col_begin(width, p.CS, q + 1)) ++q;
-        const uint32_t dst = ns_map_to_rank(base + (uint32_t)((me * 128 + m) * p.ldw + (c - col_begin(width, p.CS, q))) * 4u, (uint32_t)q);
-        ns_st_cluster_v2(dst, d[i], d[i + 1]);
+        const uint32_t dst = map_to_rank(base + (uint32_t)((me * 128 + m) * p.ldw + (c - col_begin(width, p.CS, q))) * 4u, (uint32_t)q);
+        st_cluster_v2(dst, d[i], d[i + 1]);
       }
     }
   }
-  ns_cluster_sync();                            // every partial has landed in its owner's receive buffer
+  cluster_sync_all();                            // every partial has landed in its owner's receive buffer
   if (warp != PRODUCER_WARP) {
     const int my_c0 = col_begin(width, p.CS, me), my_c1 = col_begin(width, p.CS, me + 1);
     const int et = threadIdx.x, m = et & 127;
@@ -274,165 +259,49 @@ gemm_ns_kernel(const __grid_constant__ CUtensorMap tmap_x, const NsParams p) {
         }
         if (EPI == EPI_RESADD) {
 #pragma unroll
-          for (int j = 0; j < 16; ++j) acc[j] = rv[j] + ns_bf16_round(acc[j]);
+          for (int j = 0; j < 16; ++j) acc[j] = rv[j] + bf16_round(acc[j]);
         }
         store16(p.y + (long long)m * p.ldy + nb + c, acc, valid);
       }
     }
   }
-  ns_cluster_sync();                            // no CTA exits while a peer could still address its shared memory
+  cluster_sync_all();                            // no CTA exits while a peer could still address its shared memory
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn g_ns_encode = nullptr;
-bool g_ns_attr = false;
-int g_ns_sms = 0;
-
-int ns_init() {
-  if (!g_ns_encode) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    B200_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
-    if (!fn || qres != cudaDriverEntryPointSuccess) B200_FAIL(B200_ERR_CUDA, "cuTensorMapEncodeTiled not available");
-    g_ns_encode = reinterpret_cast<EncodeTiledFn>(fn);
-  }
-  if (!g_ns_attr) {
-    const int max_smem = 220 * 1024;
-    B200_CUDA(cudaFuncSetAttribute(gemm_ns_kernel<EPI_STORE, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-    B200_CUDA(cudaFuncSetAttribute(gemm_ns_kernel<EPI_RESADD, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-    B200_CUDA(cudaFuncSetAttribute(gemm_ns_kernel<EPI_STORE, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-    B200_CUDA(cudaFuncSetAttribute(gemm_ns_kernel<EPI_RESADD, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-    B200_CUDA(cudaFuncSetAttribute(gemm_ns_kernel<EPI_GATE, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-    int dev = 0;
-    B200_CUDA(cudaGetDevice(&dev));
-    B200_CUDA(cudaDeviceGetAttribute(&g_ns_sms, cudaDevAttrMultiProcessorCount, dev));
-    g_ns_attr = true;
-  }
-  return B200_OK;
-}
+using NsKernel = void (*)(CUtensorMap, NsParams);
 
 }  // namespace
 
-bool ns_supported(int M, int N, int K, int epi) {
-  (void)N; (void)epi;
-  return M >= 1 && M <= 256 && K >= 8 && K % 8 == 0;
+int ns_init() {
+  static bool done = false;
+  if (done) return B200_OK;
+  const int max_smem = 220 * 1024;
+  B200_CUDA(cudaFuncSetAttribute(gemm_ns_kernel<EPI_STORE, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+  B200_CUDA(cudaFuncSetAttribute(gemm_ns_kernel<EPI_RESADD, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+  B200_CUDA(cudaFuncSetAttribute(gemm_ns_kernel<EPI_STORE, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+  B200_CUDA(cudaFuncSetAttribute(gemm_ns_kernel<EPI_RESADD, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+  B200_CUDA(cudaFuncSetAttribute(gemm_ns_kernel<EPI_GATE, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+  done = true;
+  return B200_OK;
 }
 
-int ns_prepare() { return ns_init(); }
-
-// The LM's choice of unit and K-split for a shape:
-//   * >= 40 pairs of tiles (in_proj 48, the gated MLP's input 88, the text head 125): N = 256 units, two K-splits while both CTAs
-//     of every unit are resident at once (in_proj: 96 CTAs), else one;
-//   * fewer (out_proj / linear_out: 32 tiles, depformer_in: 64): single-tile units (N = 128) so that more SMs pull on the
-//     weights, K cut over the largest power of two <= 4 that keeps the grid resident (32 x 4, 64 x 2 = 128 CTAs).
-static void ns_default_plan(int n_tiles, int num_kb, int epi, int* unit_tiles, int* cs) {
-  if (epi == EPI_GATE) { *unit_tiles = 2; *cs = 1; return; }
-  const int pairs = (n_tiles + 1) / 2;
-  if (pairs >= 40) {
-    *unit_tiles = 2;
-    *cs = (2 * pairs <= g_ns_sms && num_kb >= 8) ? 2 : 1;
-    return;
-  }
-  *unit_tiles = 1;
-  int c = 1;
-  while (c < 4 && n_tiles * c * 2 <= g_ns_sms && num_kb / (c * 2) >= 4) c *= 2;
-  *cs = c;
-}
-
-int ns_linear(GemmPlanCache& cache, const __nv_bfloat16* x, long long ldx, const void* w_tiles, __nv_bfloat16* y, long long ldy,
-              const __nv_bfloat16* res, long long ldr, int M, int N, int K, int epi, int gate_rows, int cluster, int pdl,
-              cudaStream_t stream, int unit_tiles) {
-  if (!ns_supported(M, N, K, epi) || ldx % 8) B200_FAIL(B200_ERR_SHAPE, "ns GEMM: unsupported shape M=%d N=%d K=%d", M, N, K);
-  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(w_tiles) | reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(res)) & 15)
-    B200_FAIL(B200_ERR_SHAPE, "ns GEMM: operands must be 16-byte aligned");
-  if ((ldy % 8) || (res && ldr % 8)) B200_FAIL(B200_ERR_SHAPE, "ns GEMM: row strides must be multiples of 8");
+// one block of an NS plan (plan_linear, gemm_sk.cu); the operands of `a` start at the block's first row
+int ns_launch(const CUtensorMap& mx, const LinearPlan& plan, const LinearBlock& b, const LinearArgs& a, cudaStream_t stream) {
   B200_TRY(ns_init());
-  // the accumulator [128 sessions x 256 weight rows] lives in the registers of the two consumer warpgroups: above 128
-  // sessions the batch runs as two launches (each streams the weights again)
-  if (M > 128) {
-    B200_TRY(ns_linear(cache, x, ldx, w_tiles, y, ldy, res, ldr, 128, N, K, epi, gate_rows, cluster, pdl, stream, unit_tiles));
-    return ns_linear(cache, x + 128 * ldx, ldx, w_tiles, y + 128 * ldy, ldy, res ? res + 128 * ldr : nullptr, ldr, M - 128, N, K, epi,
-                     gate_rows, cluster, pdl, stream, unit_tiles);
-  }
+  const int epi = plan.epi;
   NsParams p;
-  p.M = M; p.N = N; p.K = K; p.gate_rows = gate_rows;
-  p.out_rows = epi == EPI_GATE ? gate_rows : N;
+  p.M = b.rows; p.N = plan.N; p.K = plan.K; p.gate_rows = plan.gate_rows;
+  p.out_rows = epi == EPI_GATE ? plan.gate_rows : plan.N;
   p.n_tiles = (p.out_rows + BLOCK_ROWS - 1) / BLOCK_ROWS;
-  p.num_kb = (K + BLOCK_K - 1) / BLOCK_K;
-  int def_ut = 2, def_cs = 1;
-  ns_default_plan(p.n_tiles, p.num_kb, epi, &def_ut, &def_cs);
-  if (unit_tiles == 0) unit_tiles = cluster > 0 ? 2 : def_ut;
-  const int ut = (unit_tiles == 1 && epi != EPI_GATE) ? 1 : 2;
-  const uint32_t stage_bytes = (uint32_t)ut * TILE_BYTES + (uint32_t)A_BYTES;
-  const int n_units = (epi == EPI_GATE || ut == 1) ? p.n_tiles : (p.n_tiles + 1) / 2;
-  int cs = cluster > 0 ? cluster : def_cs;
-  if (epi == EPI_GATE) cs = 1;
-  if (cs > MAX_CS) cs = MAX_CS;
-  if (cs > p.num_kb) cs = p.num_kb;
-  p.CS = cs;
-  p.kb_per = (p.num_kb + cs - 1) / cs;
-  // receive buffer rows: the widest column share + 4, an odd number of 16-byte units (conflict-free float4 rows)
-  int wmax = 0;
-  for (int q = 0; q < cs; ++q) {
-    const int a = q >= cs ? 256 : ((256 * q / cs) >> 4) << 4, b = q + 1 >= cs ? 256 : ((256 * (q + 1) / cs) >> 4) << 4;
-    if (b - a > wmax) wmax = b - a;
-  }
-  p.ldw = wmax + 4;
-  if (((p.ldw / 4) & 1) == 0) p.ldw += 4;
-  int stages = (200 * 1024) / (int)stage_bytes;
-  if (stages > MAX_STAGES) stages = MAX_STAGES;
-  if (stages > p.kb_per && p.kb_per >= 2) stages = p.kb_per;
-  if (stages < 2) stages = 2;
-  const size_t recv_bytes = cs > 1 ? (size_t)cs * 128 * p.ldw * 4 : 0;
-  while ((size_t)stages * stage_bytes < recv_bytes) ++stages;          // the ring doubles as the receive buffer
-  if (stages > MAX_STAGES || (size_t)stages * stage_bytes > 204 * 1024)
-    B200_FAIL(B200_ERR_SHAPE, "ns GEMM: the receive buffer of a %d-way split does not fit", cs);
-  p.stages = stages;
-  p.wt = static_cast<const uint8_t*>(w_tiles);
-  p.y = y; p.ldy = ldy; p.res = res; p.ldr = ldr;
-  // activations x [M][K]: boxes of [128 rows x 64 k]; rows >= M are zero-filled by the TMA unit
-  PlanKey key{x, ldx, M, K, 128};
-  auto it = cache.maps.find(key);
-  if (it == cache.maps.end()) {
-    CUtensorMap mp;
-    cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)M};
-    cuuint64_t strides[1] = {(cuuint64_t)ldx * 2};
-    cuuint32_t box[2] = {(cuuint32_t)BLOCK_K, 128u};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = g_ns_encode(&mp, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<__nv_bfloat16*>(x), dims, strides, box, estr,
-                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) B200_FAIL(B200_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d) M=%d K=%d ld=%lld", (int)r, M, K, ldx);
-    it = cache.maps.emplace(key, mp).first;
-  }
-  const size_t smem = (size_t)stages * stage_bytes + 1024 + 16 * MAX_STAGES + 64;
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3((unsigned)(n_units * cs)); cfg.blockDim = dim3(NUM_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  int na = 0;
-  if (cs > 1) {
-    attr[na].id = cudaLaunchAttributeClusterDimension;
-    attr[na].val.clusterDim.x = cs; attr[na].val.clusterDim.y = 1; attr[na].val.clusterDim.z = 1;
-    ++na;
-  }
-  if (pdl) {
-    attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[na].val.programmaticStreamSerializationAllowed = 1;
-    ++na;
-  }
-  cfg.attrs = attr; cfg.numAttrs = na;
-  cudaError_t le;
-  if (epi == EPI_GATE) le = cudaLaunchKernelEx(&cfg, gemm_ns_kernel<EPI_GATE, 2>, it->second, p);
-  else if (ut == 1) le = epi == EPI_STORE ? cudaLaunchKernelEx(&cfg, gemm_ns_kernel<EPI_STORE, 1>, it->second, p)
-                                         : cudaLaunchKernelEx(&cfg, gemm_ns_kernel<EPI_RESADD, 1>, it->second, p);
-  else le = epi == EPI_STORE ? cudaLaunchKernelEx(&cfg, gemm_ns_kernel<EPI_STORE, 2>, it->second, p)
-                             : cudaLaunchKernelEx(&cfg, gemm_ns_kernel<EPI_RESADD, 2>, it->second, p);
-  if (le != cudaSuccess) B200_FAIL(B200_ERR_CUDA, "gemm_ns launch failed: %s", cudaGetErrorString(le));
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  return check_launch("gemm_ns");
+  p.num_kb = (plan.K + BLOCK_K - 1) / BLOCK_K;
+  p.CS = b.cluster; p.kb_per = b.kb_per; p.ldw = b.ldw; p.stages = b.stages;
+  p.wt = static_cast<const uint8_t*>(a.w);
+  p.y = a.y; p.ldy = a.ldy; p.res = a.res; p.ldr = a.ldr;
+  const NsKernel k = epi == EPI_GATE ? gemm_ns_kernel<EPI_GATE, 2>
+                     : b.unit_tiles == 1 ? (epi == EPI_STORE ? gemm_ns_kernel<EPI_STORE, 1> : gemm_ns_kernel<EPI_RESADD, 1>)
+                                         : (epi == EPI_STORE ? gemm_ns_kernel<EPI_STORE, 2> : gemm_ns_kernel<EPI_RESADD, 2>);
+  return launch("gemm_ns", k, dim3((unsigned)b.grid), dim3(NUM_THREADS), b.smem, stream, LaunchOpts{a.pdl, b.cluster > 1 ? b.cluster : 0},
+                mx, p);
 }
 
 }  // namespace tc

@@ -9,14 +9,14 @@
 
 #include <cuda.h>
 
-#include "common.cuh"
+#include "tc_host.cuh"
 
 namespace b200 {
 namespace tc {
 
-struct PlanKey {
+struct MapKey {
   const void* ptr; long long ld; int rows, cols, box_rows;
-  bool operator<(const PlanKey& o) const {
+  bool operator<(const MapKey& o) const {
     if (ptr != o.ptr) return ptr < o.ptr;
     if (ld != o.ld) return ld < o.ld;
     if (rows != o.rows) return rows < o.rows;
@@ -25,31 +25,76 @@ struct PlanKey {
   }
 };
 
-struct GemmPlanCache {
-  std::map<PlanKey, CUtensorMap> maps;
+// activation tensor maps of the linears, encoded once per (buffer, shape, box)
+struct TensorMapCache {
+  std::map<MapKey, CUtensorMap> maps;
   void clear() { maps.clear(); }
 };
 
-// resolves cuTensorMapEncodeTiled and sets the kernels' shared-memory attributes (call before capturing a graph)
-int prepare_plans(GemmPlanCache& cache);
+// shared-memory attributes of the swap-AB / cluster kernels (linear_init) and of those and the non-swapped kernels
+// (linear_prepare; call before capturing a graph).  Setting an attribute loads the kernel's code into device memory, which
+// moves the buffers allocated after it: the LM calls linear_init when a batch starts streaming, before its depformer buffers.
+int linear_init();
+int linear_prepare();
 
-// ---- stream-K kernel over pre-tiled weights (gemm_sk.cu) --------------------------------------
-struct SkTuning {
-  int grid = 0;          // CTAs (0 = one per SM)
-  int smem_budget = 0;   // bytes of pipeline stages per CTA (0 = 200 KB)
-  int stream_only = 0;   // diagnostics: run the copy pipeline without MMAs / stores
-  int no_split = 0;      // never cut a tile across CTAs (whole tiles only)
-  int force_split = 0;   // tests: cut tiles even where the default policy keeps them whole
-  int no_cluster = 0;    // never use the cluster split-K kernel
-  int cluster = 0;       // force a cluster size (tests)
-  // int8 path (QLinear): row-wise absmax int8 activations [M][K] + their scales, and the weight-row scales [N]
-  const void* xq = nullptr; const float* sa = nullptr; const float* sw = nullptr;
-  int pdl = 0;           // launch with programmatic stream serialization (the kernel waits on its own)
-  int ns = 0;            // 33..256 sessions: 0 = the non-swapped kernel (gemm_ns.cu) unless B200_GEMM_NS=0, -1 = never, 1 = always (tests)
-  // GEMV path only (M <= sk_gemv_max_m()): x is the residual stream and the linear's input is rmsnorm(x, norm_alpha)
-  const __nv_bfloat16* norm_alpha = nullptr;
+// ---- the plan of one linear:  y[M][N] = epi(x[M][K] . w[N][K]^T) over packed weight tiles ---------------------------
+//   GEMV (gemm_sk.cu): one to gemv_max_m rows, plain loads on the CUDA cores;
+//   NS   (gemm_ns.cu): 33..256 rows, activations as the wgmma A operand, two weight tiles as B;
+//   CK   (gemm_sk.cu): more than 32 rows over few row tiles, K cut over a cluster and reduced over DSMEM;
+//   SK   (gemm_sk.cu): swap-AB stream-K, up to 128 rows per launch (64 gated).
+enum LinearKernel { LK_GEMV = 1, LK_NS = 2, LK_CK = 3, LK_SK = 4 };
+
+// Forces for tests and tools (the b200_op_* entry points); all zero = the LM's own choice
+struct LinearForce {
+  int kernel = 0;         // LK_NS: the non-swapped kernel at any M; LK_SK: never the non-swapped kernel
+  int sk_grid = 0;        // stream-K with this many CTAs, tiles cut at every M
+  int ck_cluster = 0;     // cluster split-K with this many CTAs per tile
+  int ns_splits = 0;      // NS: K-splits over a cluster
+  int ns_unit_tiles = 0;  // NS: weight tiles per CTA (1 = N 128, 2 = N 256)
+  int stage_budget = 0;   // SK: bytes of pipeline stages per CTA (0 = 200 KB)
+  int stream_only = 0;    // diagnostics: SK runs the copy pipeline without MMAs / stores
 };
-int sk_num_sms();
+
+// One launch over rows [m0, m0 + rows); fields a kernel does not use are 0
+struct LinearBlock {
+  int kernel, m0, rows;
+  int grid, cluster, smem, stages, stage_bytes;   // cluster: CK / NS K-splits
+  int np, Mpad, kb_per;                           // np: activation box rows (SK / CK: the wgmma width, NS: 128)
+  int S, kbps;                                    // GEMV splits and k-blocks per split
+  int unit_tiles, ldw;                            // NS
+  int Wc;                                         // CK
+  int whole_rounds, sk_tile0, sk_items;           // SK schedule
+};
+constexpr int LINEAR_MAX_BLOCKS = 4;
+struct LinearPlan {
+  int M, N, K, epi, gate_rows, i8;
+  int norm_folded;        // the RMSNorm asked for is folded into the GEMV's activation staging
+  int stream_only;        // LinearForce::stream_only
+  int n_blocks;
+  LinearBlock blocks[LINEAR_MAX_BLOCKS];
+};
+// Pure host function (no CUDA call).  ld_aligned: the output and residual row strides are multiples of 8.
+int plan_linear(int M, int N, int K, int epi, int gate_rows, bool i8, bool norm, bool ld_aligned, int sms, int gemv_max_m,
+                const LinearForce& force, LinearPlan* plan);
+
+struct LinearArgs {
+  const __nv_bfloat16* x; long long ldx;     // bf16 activations (the residual stream when the norm is folded)
+  const void* w;                             // packed tiles
+  __nv_bfloat16* y; long long ldy;
+  const __nv_bfloat16* res; long long ldr;
+  float* ws; int* counters;                  // sk_workspace_bytes(M) and SK_MAX_TILES ints, zeroed once
+  // int8 path (QLinear): row-wise absmax int8 activations [M][K] + their scales, and the weight-row scales [N]
+  const void* xq; const float* sa; const float* sw;
+  const __nv_bfloat16* norm_alpha;           // a folded RMSNorm's alpha (plan.norm_folded)
+  int pdl;
+};
+int run_linear(TensorMapCache& maps, const LinearPlan& plan, const LinearArgs& a, cudaStream_t stream);
+// the non-swapped kernel (gemm_ns.cu): shared-memory attributes, and the launch of one block of an NS plan
+constexpr int NS_MAX_STAGES = 8, NS_MAX_CS = 8;
+constexpr int NS_A_BYTES = 128 * 64 * 2;   // one activation box: 128 session rows x 64 k
+int ns_init();
+int ns_launch(const CUtensorMap& mx, const LinearPlan& plan, const LinearBlock& b, const LinearArgs& a, cudaStream_t stream);
+
 int sk_gemv_max_m();
 int sk_set_gemv_max_m(int max_m);      // rows up to which the GEMV path is taken (0..4); returns the previous value
 bool sk_supported(int M, int N, int K, int epi);
@@ -65,18 +110,6 @@ int sk_pack_weights_i8(const int8_t* q, void* out_tiles, int N, int K, int epi, 
 int sk_quantize_rows(const __nv_bfloat16* x, long long ldx, void* xq, float* sa, int M, int K, cudaStream_t stream, int pdl = 0);
 constexpr int SK_MAX_GRID = 304;     // 2 CTAs per SM at most
 constexpr int SK_MAX_TILES = 1024;   // ints in the arrival-counter array
-int sk_linear(GemmPlanCache& cache, const __nv_bfloat16* x, long long ldx, const void* w_tiles, __nv_bfloat16* y,
-              long long ldy, const __nv_bfloat16* res, long long ldr, int M, int N, int K, int epi, int gate_rows,
-              float* ws, int* counters, const SkTuning& tune, cudaStream_t stream);
-
-// ---- non-swapped kernel for 33..256 sessions (gemm_ns.cu): A = activations, B = two weight tiles (N = 256) ------------
-bool ns_supported(int M, int N, int K, int epi);
-int ns_prepare();
-// cluster: K-splits (0 = the default plan for the shape); same packed weights and epilogues as sk_linear
-// unit_tiles: weight tiles per CTA as the B operand (2 = N 256; 1 = N 128: twice the units for few-tile shapes; 0 = the LM's choice)
-int ns_linear(GemmPlanCache& cache, const __nv_bfloat16* x, long long ldx, const void* w_tiles, __nv_bfloat16* y, long long ldy,
-              const __nv_bfloat16* res, long long ldr, int M, int N, int K, int epi, int gate_rows, int cluster, int pdl,
-              cudaStream_t stream, int unit_tiles = 0);
 
 // ---- the depformer of one frame as one persistent kernel (dep_fused.cu) ---------------------------
 struct DepFusedConfig {

@@ -70,7 +70,6 @@ struct b200_lm {
   int use_sampling = 1, top_k = 250, top_k_text = 25;
   float temp = 0.8f, temp_text = 0.7f;
   int pdl = 1;                                 // programmatic dependent launch of the GEMMs (B200_PDL=0 disables)
-  int sk_smem = 0;                             // bytes of pipeline stages per GEMM CTA (B200_SK_SMEM_KB; 0 = 200 KB, one CTA per SM)
   float* sk_ws = nullptr;                      // stream-K partial-accumulator slots (L2-resident)
   int* sk_counters = nullptr;                  // per-tile arrival counters (zero between launches)
   // weights
@@ -110,7 +109,6 @@ struct b200_lm {
   int* attn_counters = nullptr;                // split arrival counters [B*H]
   tc::DepFused* depf = nullptr;                // the depformer of a frame as one persistent kernel (B200_DEP_FUSED=0: off)
   int dep_fused = 1;
-  int fuse_norm = 1;                           // B200_FUSE_NORM=0: keep rmsnorm_kernel in front of the GEMV path too (diagnostics)
   int kv_cap = 0;                              // b200_lm_set_kv_capacity: slots per ring (0 = cfg.context, the reference's ring)
   int kv_fp8 = 0;                              // b200_lm_set_kv_dtype / B200_KV_DTYPE: opt-in 8-bit KV ring (B200_KV_FP8_E4M3 or B200_KV_INT8; 0 = bf16)
   // b200_lm_set_kv_pool: the temporal rings live in pages of page_slots slots (TLayer kc / vc are then the pools
@@ -150,7 +148,7 @@ struct b200_lm {
   long long *pin_in = nullptr, *pin_out = nullptr;
   float* pin_noise = nullptr;
   int64_t weight_bytes = 0;
-  tc::GemmPlanCache plans;
+  tc::TensorMapCache maps;
 };
 
 namespace {
@@ -183,30 +181,41 @@ int noise_per_row(const b200_lm* h) {
   return kt + h->cfg.dep_q * ka;
 }
 
-// y[M][N] = epi(x[M][K] . w[N][K]^T); `w` is the packed-tile form of gemm_sk.cu.
-int linear(b200_lm* h, const bf16* x, long long ldx, const bf16* w, bf16* y, long long ldy, const bf16* res,
-           long long ldr, int M, int N, int K, int epi, int gate_rows, const float* w_scales = nullptr,
-           const bf16* norm_alpha = nullptr) {
-  tc::SkTuning t;
-  t.pdl = h->pdl;
-  t.smem_budget = h->sk_smem;
-  t.norm_alpha = norm_alpha;
-  if (h->cfg.quantize) {       // QLinear.forward (utils/quantize.py:22-40): row-wise int8 activations, int8 x int8 -> int32
-    if (!w_scales) B200_FAIL(B200_ERR_STATE, "quantised LM: linear without weight scales");
-    B200_TRY(tc::sk_quantize_rows(x, ldx, h->xq, h->xq_scale, M, K, h->body, h->pdl));
-    t.xq = h->xq; t.sa = h->xq_scale; t.sw = w_scales;
-  }
-  return tc::sk_linear(h->plans, x, ldx, w, y, ldy, res, ldr, M, N, K, epi, gate_rows, h->sk_ws, h->sk_counters, t, h->body);
+// The plan of y[M][N] = epi(x[M][K] . w[N][K]^T) on this device; norm: an RMSNorm in front that may fold into the GEMV.
+int plan(const b200_lm* h, int M, int N, int K, int epi, int gate_rows, long long ldy, long long ldr, bool norm, tc::LinearPlan* out) {
+  return tc::plan_linear(M, N, K, epi, gate_rows, h->cfg.quantize != 0, norm, ldy % 8 == 0 && ldr % 8 == 0, num_sms(), tc::sk_gemv_max_m(),
+                         tc::LinearForce(), out);
 }
 
-// y = epi(rmsnorm(x, alpha) . w^T).  One or two sessions: the norm is folded into the GEMV's activation staging (one kernel
-// and one dependency less per linear); otherwise rmsnorm_kernel writes xn and the GEMM reads it.
+// Runs a plan; `w` is the packed-tile form of gemm_sk.cu.
+int run(b200_lm* h, const tc::LinearPlan& p, const bf16* x, long long ldx, const bf16* w, bf16* y, long long ldy, const bf16* res,
+        long long ldr, const float* w_scales, const bf16* norm_alpha = nullptr) {
+  tc::LinearArgs a{x, ldx, w, y, ldy, res, ldr, h->sk_ws, h->sk_counters, nullptr, nullptr, nullptr, norm_alpha, h->pdl};
+  if (h->cfg.quantize) {       // QLinear.forward (utils/quantize.py:22-40): row-wise int8 activations, int8 x int8 -> int32
+    if (!w_scales) B200_FAIL(B200_ERR_STATE, "quantised LM: linear without weight scales");
+    B200_TRY(tc::sk_quantize_rows(x, ldx, h->xq, h->xq_scale, p.M, p.K, h->body, h->pdl));
+    a.xq = h->xq; a.sa = h->xq_scale; a.sw = w_scales;
+  }
+  return tc::run_linear(h->maps, p, a, h->body);
+}
+
+// y[M][N] = epi(x[M][K] . w[N][K]^T)
+int linear(b200_lm* h, const bf16* x, long long ldx, const bf16* w, bf16* y, long long ldy, const bf16* res,
+           long long ldr, int M, int N, int K, int epi, int gate_rows, const float* w_scales = nullptr) {
+  tc::LinearPlan p;
+  B200_TRY(plan(h, M, N, K, epi, gate_rows, ldy, res ? ldr : 0, false, &p));
+  return run(h, p, x, ldx, w, y, ldy, res, ldr, w_scales);
+}
+
+// y = epi(rmsnorm(x, alpha) . w^T).  Where the plan takes the GEMV (one or two sessions), the norm is folded into its
+// activation staging (one kernel and one dependency less per linear); otherwise rmsnorm_kernel writes xn and the GEMM reads it.
 int norm_linear(b200_lm* h, const bf16* x, const bf16* alpha, bf16* xn, const bf16* w, bf16* y, long long ldy, int M, int N, int K,
                 int epi, int gate_rows, const float* w_scales) {
-  if (!h->cfg.quantize && h->fuse_norm && M <= tc::sk_gemv_max_m())
-    return linear(h, x, K, w, y, ldy, nullptr, 0, M, N, K, epi, gate_rows, w_scales, alpha);
+  tc::LinearPlan p;
+  B200_TRY(plan(h, M, N, K, epi, gate_rows, ldy, 0, true, &p));
+  if (p.norm_folded) return run(h, p, x, K, w, y, ldy, nullptr, 0, w_scales, alpha);
   B200_LAUNCH(rmsnorm_kernel, M, 256, 0, h->body, x, alpha, xn, K, 1e-8f);
-  return linear(h, xn, K, w, y, ldy, nullptr, 0, M, N, K, epi, gate_rows, w_scales);
+  return run(h, p, xn, K, w, y, ldy, nullptr, 0, w_scales);
 }
 
 // A QLinear as model.q8.safetensors stores it (utils/quantize.py:16-21): "<name>" int8 [rows][K] + "<name>_scb" fp32 [rows]
@@ -654,9 +663,7 @@ int b200_lm_create(const b200_lm_config* cfg, b200_lm** out) {
   for (int k = 0; k < h->Kc; ++k) h->max_delay = cfg->delays[k] > h->max_delay ? cfg->delays[k] : h->max_delay;
   h->CT = h->max_delay + 2;     // lm.py:606-611
   if (const char* e = getenv("B200_PDL")) h->pdl = atoi(e) != 0;
-  if (const char* e = getenv("B200_SK_SMEM_KB")) h->sk_smem = atoi(e) * 1024;
   if (const char* e = getenv("B200_DEP_FUSED")) h->dep_fused = atoi(e);
-  if (const char* e = getenv("B200_FUSE_NORM")) h->fuse_norm = atoi(e) != 0;
   if (const char* e = getenv("B200_KV_DTYPE")) {
     const std::string v = e;
     h->kv_fp8 = (v == "fp8" || v == "fp8_e4m3") ? B200_KV_FP8_E4M3 : v == "int8" ? B200_KV_INT8 : 0;
@@ -1006,6 +1013,7 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
     B200_TRY(A.alloc_t(&h->xq, (size_t)MB * kmax, false));
     B200_TRY(A.alloc_t(&h->xq_scale, (size_t)MB, false));
   }
+  B200_TRY(tc::linear_init());
   // One or two sessions: the depformer's linears take the GEMV path and the PDL-chained launches beat the persistent kernel
   // (a grid barrier per phase costs more than the launch it saves).  B200_DEP_FUSED=2 forces the kernel at any batch.
   // Under classifier-free guidance the two halves of the batch meet before every sampler (lm.py:828-833): launch chain.
@@ -1208,7 +1216,7 @@ int b200_lm_streaming_end(b200_lm* h) {
   if (h->ev_in) cudaEventDestroy(h->ev_in);
   if (h->ev_out) cudaEventDestroy(h->ev_out);
   h->gstream = nullptr; h->ev_in = h->ev_out = nullptr;
-  h->plans.clear();
+  h->maps.clear();
   tc::dep_fused_destroy(h->depf);
   h->depf = nullptr;
   h->state.free_all();
@@ -1297,7 +1305,7 @@ int b200_lm_set_condition_cross(b200_lm* h, const void* src_bf16_dev, const int3
   }
   const int d = h->cfg.dim, H = h->cfg.num_heads, T = h->cross_len;
   B200_CUDA(cudaMemcpyAsync(h->cross_rows, rows.data(), rows.size() * 4, cudaMemcpyHostToDevice, h->stream));
-  B200_TRY(tc::prepare_plans(h->plans));
+  B200_TRY(tc::linear_prepare());
   // transformer.py:495-505 per layer, outside the step: kv = src @ W[d:]^T in chunks of rows, then "b t (p h d) -> p b h t d"
   // into the rows' memory.  The chunk is staged in a fixed buffer so that the GEMM's activation plan is the same every call.
   h->body = h->stream;
@@ -1486,7 +1494,7 @@ static int run_step(b200_lm* h, int n_in, int replace, int internal_noise) {
     h->noise_static = internal_noise;
     drop_graph(h);
   }
-  B200_TRY(tc::prepare_plans(h->plans));
+  B200_TRY(tc::linear_prepare());
   if (!h->graph_enabled) {
     h->body = h->stream;
     return step_body(h);

@@ -3,6 +3,7 @@
 #include <cstring>
 
 #include "mimi_tc.cuh"
+#include "tc_host.cuh"
 #include "tc_prims.cuh"
 
 namespace b200 {
@@ -258,22 +259,11 @@ __global__ void tc_pack_kernel(const float* __restrict__ w, float4* __restrict__
   out[o + per_tile] = make_float4(lo[0], lo[1], lo[2], lo[3]);
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn g_encode = nullptr;
 bool g_attr = false;
 
 }  // namespace
 
 int tc_init() {
-  if (!g_encode) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    B200_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
-    if (!fn || qres != cudaDriverEntryPointSuccess) B200_FAIL(B200_ERR_CUDA, "cuTensorMapEncodeTiled not available");
-    g_encode = reinterpret_cast<EncodeTiledFn>(fn);
-  }
   if (!g_attr) {
     B200_CUDA(cudaFuncSetAttribute(mimi_tc_kernel<TC_MAX_NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
     B200_CUDA(cudaFuncSetAttribute(mimi_tc_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
@@ -317,13 +307,7 @@ int tc_make_map(CUtensorMap* m, const float* base, int Cin, long long rows_per_s
   cuuint32_t box[3] = {(cuuint32_t)TC_KB, (cuuint32_t)(tt * stride), (cuuint32_t)bb};
   cuuint32_t estr[3] = {1, (cuuint32_t)stride, 1};
   if (box[1] > 256 || box[2] > 256) B200_FAIL(B200_ERR_SHAPE, "tc_make_map: box %u x %u exceeds the TMA limit of 256", box[1], box[2]);
-  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS)
-    B200_FAIL(B200_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d): Cin %d rows %lld sessions %d box %u/%u/%u stride %d", (int)r, Cin,
-              rows_per_session, n_sessions, box[0], box[1], box[2], stride);
-  return B200_OK;
+  return encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, base, dims, strides, box, estr, "tc_make_map");
 }
 
 // Fills the launch plan of a layer for `n_sessions` sessions of T output steps each (linear: n_sessions = 1, T = tokens).
@@ -362,17 +346,8 @@ int tc_launch(const TcLayer& L, cudaStream_t st) {
   // programmatic dependent launch (B200_MIMI_PDL=0: off): the kernel may start while its predecessor drains; it requests its
   // first weight tiles, then waits (griddepcontrol.wait) before it reads an activation or writes anything
   static const int pdl = [] { const char* e = getenv("B200_MIMI_PDL"); return e ? atoi(e) : 1; }();
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3((unsigned)L.grid); cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = L.smem; cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
-  const cudaError_t le = L.p.NT == TC_MAX_NT ? cudaLaunchKernelEx(&cfg, mimi_tc_kernel<TC_MAX_NT>, L.map_hi, L.map_lo, L.p)
-                                             : cudaLaunchKernelEx(&cfg, mimi_tc_kernel<16>, L.map_hi, L.map_lo, L.p);
-  if (le != cudaSuccess) B200_FAIL(B200_ERR_CUDA, "mimi_tc launch failed: %s", cudaGetErrorString(le));
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  B200_TRY(launch("mimi_tc", L.p.NT == TC_MAX_NT ? mimi_tc_kernel<TC_MAX_NT> : mimi_tc_kernel<16>, dim3((unsigned)L.grid), dim3(TC_THREADS),
+                  L.smem, st, LaunchOpts{pdl}, L.map_hi, L.map_lo, L.p));
   if (L.p.ksplit > 1) {
     const long long n = (long long)L.p.m_tiles * TC_ROWS * (L.p.N / 4);
     mimi_tc_reduce_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(L.p);

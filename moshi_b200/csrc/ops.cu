@@ -44,20 +44,32 @@ static int attn_scratch(int B, int H, int nsplit, float** part, int** counters, 
   return B200_OK;
 }
 
+// The LM's linear as the kernel-level entry points run it: rows of x, y and res are contiguous (ldx = K, ldy = ldr = output
+// columns); `which` picks the bf16 or the int8 scratch and tensor-map cache
+static int op_linear(const void* x, const void* w, void* y, const void* res, int M, int N, int K, int epi, int gate_rows,
+                     const tc::LinearForce& force, const void* xq, const float* sa, const float* sw, const void* norm_alpha, int which,
+                     cudaStream_t st) {
+  static tc::TensorMapCache caches[2];
+  float* ws = nullptr; int* counters = nullptr;
+  B200_TRY(sk_scratch(&ws, &counters, which));
+  const int out_cols = epi == 2 ? gate_rows : N;
+  tc::LinearPlan plan;
+  B200_TRY(tc::plan_linear(M, N, K, epi, gate_rows, xq != nullptr, norm_alpha != nullptr, out_cols % 8 == 0, num_sms(), tc::sk_gemv_max_m(),
+                           force, &plan));
+  const tc::LinearArgs a{static_cast<const __nv_bfloat16*>(x), K, w, static_cast<__nv_bfloat16*>(y), out_cols,
+                         static_cast<const __nv_bfloat16*>(res), out_cols, ws, counters, xq, sa, sw,
+                         static_cast<const __nv_bfloat16*>(norm_alpha), 0};
+  return tc::run_linear(caches[which], plan, a, st);
+}
+
 int b200_op_linear_bf16(const void* x_dev, const void* w_dev, void* y_dev, int M, int N, int K, void* stream) {
   if (!x_dev || !w_dev || !y_dev || M < 1 || N < 1 || K < 8 || K % 8) B200_FAIL(B200_ERR_SHAPE, "op_linear_bf16: bad shape");
   if (!tc::sk_supported(M, N, K, 0)) B200_FAIL(B200_ERR_SHAPE, "op_linear_bf16: unsupported shape");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  static tc::GemmPlanCache cache;
-  float* ws = nullptr; int* counters = nullptr;
-  B200_TRY(sk_scratch(&ws, &counters));
   void* tiles = nullptr;
   B200_CUDA(cudaMalloc(&tiles, tc::sk_packed_bytes(N, K, 0, 0)));
   int rc = tc::sk_pack_weights(static_cast<const __nv_bfloat16*>(w_dev), tiles, N, K, 0, 0, st);
-  tc::SkTuning t;
-  if (rc == B200_OK)
-    rc = tc::sk_linear(cache, static_cast<const __nv_bfloat16*>(x_dev), K, tiles, static_cast<__nv_bfloat16*>(y_dev), N, nullptr, 0,
-                       M, N, K, 0, 0, ws, counters, t, st);
+  if (rc == B200_OK) rc = op_linear(x_dev, tiles, y_dev, nullptr, M, N, K, 0, 0, tc::LinearForce(), nullptr, nullptr, nullptr, nullptr, 0, st);
   cudaStreamSynchronize(st);
   cudaFree(tiles);
   return rc;
@@ -75,34 +87,28 @@ int b200_op_linear_sk(const void* x_dev, const void* w_tiles_dev, void* y_dev, c
                       int epi, int gate_rows, int grid, int smem_budget, int stream_only, void* stream) {
   if (!x_dev || !w_tiles_dev || !y_dev) B200_FAIL(B200_ERR_INVALID, "op_linear_sk: null pointer");
   if (!tc::sk_supported(M, N, K, epi)) B200_FAIL(B200_ERR_SHAPE, "op_linear_sk: unsupported shape");
-  static tc::GemmPlanCache cache;
-  float* ws = nullptr; int* counters = nullptr;
-  B200_TRY(sk_scratch(&ws, &counters));
-  tc::SkTuning t;
-  // grid > 0: stream-K with that many CTAs; grid < 0: cluster split-K with |grid| CTAs per tile; 0: the LM's own choice
-  t.grid = grid > 0 ? grid : 0; t.cluster = grid < 0 ? -grid : 0; t.smem_budget = smem_budget; t.stream_only = stream_only;
-  t.force_split = grid > 0;     // an explicit grid (parity tests) exercises the tile-cutting path at every M
-  t.ns = smem_budget == -1 ? -1 : 0;   // smem_budget -1: the swap-AB kernels at any M (comparison row of tools/kbench.py)
-  if (smem_budget < 0) t.smem_budget = 0;
-  const int out_cols = epi == 2 ? gate_rows : N;
-  return tc::sk_linear(cache, static_cast<const __nv_bfloat16*>(x_dev), K, w_tiles_dev, static_cast<__nv_bfloat16*>(y_dev),
-                       out_cols, static_cast<const __nv_bfloat16*>(res_dev), out_cols, M, N, K, epi, gate_rows, ws, counters, t,
-                       static_cast<cudaStream_t>(stream));
+  tc::LinearForce f;
+  // grid > 0: stream-K with that many CTAs (tiles cut at every M); grid < 0: cluster split-K with |grid| CTAs per tile; 0: the LM's own choice
+  f.sk_grid = grid > 0 ? grid : 0; f.ck_cluster = grid < 0 ? -grid : 0; f.stream_only = stream_only;
+  // smem_budget > 0: the stage ring's bytes; -1: never the non-swapped kernel (the swap-AB comparison row of tools/kbench.py)
+  f.stage_budget = smem_budget > 0 ? smem_budget : 0;
+  f.kernel = smem_budget == -1 ? tc::LK_SK : 0;
+  return op_linear(x_dev, w_tiles_dev, y_dev, res_dev, M, N, K, epi, gate_rows, f, nullptr, nullptr, nullptr, nullptr, 0,
+                   static_cast<cudaStream_t>(stream));
 }
 
 // the non-swapped kernel (33..256 sessions in the LM) at any M <= 256; cluster = K-splits (0 = the LM's own choice)
 int b200_op_linear_ns(const void* x_dev, const void* w_tiles_dev, void* y_dev, const void* res_dev, int M, int N, int K, int epi,
                       int gate_rows, int cluster, void* stream) {
   if (!x_dev || !w_tiles_dev || !y_dev) B200_FAIL(B200_ERR_INVALID, "op_linear_ns: null pointer");
-  if (!tc::ns_supported(M, N, K, epi)) B200_FAIL(B200_ERR_SHAPE, "op_linear_ns: unsupported shape");
-  static tc::GemmPlanCache cache;
-  const int out_cols = epi == 2 ? gate_rows : N;
+  if (!tc::sk_supported(M, N, K, epi)) B200_FAIL(B200_ERR_SHAPE, "op_linear_ns: unsupported shape");
+  tc::LinearForce f;
+  f.kernel = tc::LK_NS;
   // cluster >= 100: single-tile units (N = 128 per instruction) with cluster - 100 K-splits
-  const int unit_tiles = cluster >= 100 ? 1 : (cluster > 0 ? 2 : 0);
-  if (cluster >= 100) cluster -= 100;
-  return tc::ns_linear(cache, static_cast<const __nv_bfloat16*>(x_dev), K, w_tiles_dev, static_cast<__nv_bfloat16*>(y_dev), out_cols,
-                       static_cast<const __nv_bfloat16*>(res_dev), out_cols, M, N, K, epi, gate_rows, cluster, 0,
-                       static_cast<cudaStream_t>(stream), unit_tiles);
+  f.ns_unit_tiles = cluster >= 100 ? 1 : (cluster > 0 ? 2 : 0);
+  f.ns_splits = cluster >= 100 ? cluster - 100 : cluster;
+  return op_linear(x_dev, w_tiles_dev, y_dev, res_dev, M, N, K, epi, gate_rows, f, nullptr, nullptr, nullptr, nullptr, 0,
+                   static_cast<cudaStream_t>(stream));
 }
 
 // y = epi(rmsnorm(x, alpha) . W^T) with the norm folded into the GEMV's activation staging (norm_linear at one or two
@@ -111,18 +117,29 @@ int b200_op_linear_sk_norm(const void* x_dev, const void* alpha_dev, const void*
                            int N, int K, int epi, int gate_rows, void* stream) {
   if (!x_dev || !alpha_dev || !w_tiles_dev || !y_dev) B200_FAIL(B200_ERR_INVALID, "op_linear_sk_norm: null pointer");
   if (!tc::sk_supported(M, N, K, epi)) B200_FAIL(B200_ERR_SHAPE, "op_linear_sk_norm: unsupported shape");
-  static tc::GemmPlanCache cache;
-  float* ws = nullptr; int* counters = nullptr;
-  B200_TRY(sk_scratch(&ws, &counters));
-  tc::SkTuning t;
-  t.norm_alpha = static_cast<const __nv_bfloat16*>(alpha_dev);
-  const int out_cols = epi == 2 ? gate_rows : N;
-  return tc::sk_linear(cache, static_cast<const __nv_bfloat16*>(x_dev), K, w_tiles_dev, static_cast<__nv_bfloat16*>(y_dev),
-                       out_cols, static_cast<const __nv_bfloat16*>(res_dev), out_cols, M, N, K, epi, gate_rows, ws, counters, t,
-                       static_cast<cudaStream_t>(stream));
+  return op_linear(x_dev, w_tiles_dev, y_dev, res_dev, M, N, K, epi, gate_rows, tc::LinearForce(), nullptr, nullptr, nullptr, alpha_dev,
+                   0, static_cast<cudaStream_t>(stream));
 }
 
 int b200_op_set_gemv_max_rows(int max_rows) { return tc::sk_set_gemv_max_m(max_rows); }
+
+int b200_op_linear_plan(int M, int N, int K, int epi, int gate_rows, int int8, int norm, int sms, int gemv_max_rows, int64_t* out,
+                        int capacity) {
+  if (!out || capacity < 2) B200_FAIL(B200_ERR_INVALID, "op_linear_plan: no room for the plan");
+  tc::LinearPlan plan;
+  B200_TRY(tc::plan_linear(M, N, K, epi, gate_rows, int8 != 0, norm != 0, (epi == 2 ? gate_rows : N) % 8 == 0, sms, gemv_max_rows,
+                           tc::LinearForce(), &plan));
+  constexpr int F = 19;
+  if (capacity < 2 + F * plan.n_blocks) B200_FAIL(B200_ERR_INVALID, "op_linear_plan: %d launches need %d slots", plan.n_blocks, 2 + F * plan.n_blocks);
+  out[0] = plan.n_blocks; out[1] = plan.norm_folded;
+  for (int i = 0; i < plan.n_blocks; ++i) {
+    const tc::LinearBlock& b = plan.blocks[i];
+    const int v[F] = {b.kernel, b.m0, b.rows, b.grid, b.cluster, b.smem, b.stages, b.stage_bytes, b.np, b.Mpad, b.kb_per, b.S, b.kbps,
+                      b.unit_tiles, b.ldw, b.Wc, b.whole_rounds, b.sk_tile0, b.sk_items};
+    for (int j = 0; j < F; ++j) out[2 + F * i + j] = v[j];
+  }
+  return B200_OK;
+}
 
 // rmsnorm_kernel as the LM launches it (lm.cu norm_linear and the output norm): one 256-thread CTA per row, eps 1e-8
 int b200_op_rmsnorm(const void* x_dev, const void* alpha_dev, void* y_dev, int M, int dim, void* stream) {
@@ -175,15 +192,9 @@ int b200_op_linear_i8(const void* xq_dev, const float* sa_dev, const void* w_til
                       const void* res_dev, int M, int N, int K, int epi, int gate_rows, void* stream) {
   if (!xq_dev || !sa_dev || !w_tiles_dev || !sw_dev || !y_dev) B200_FAIL(B200_ERR_INVALID, "op_linear_i8: null pointer");
   if (!tc::sk_supported(M, N, K, epi)) B200_FAIL(B200_ERR_SHAPE, "op_linear_i8: unsupported shape");
-  static tc::GemmPlanCache cache;
-  float* ws = nullptr; int* counters = nullptr;
-  B200_TRY(sk_scratch(&ws, &counters, 1));   // int32 partials of cut tiles
-  tc::SkTuning t;
-  t.xq = xq_dev; t.sa = sa_dev; t.sw = sw_dev;
-  const int out_cols = epi == 2 ? gate_rows : N;
-  return tc::sk_linear(cache, nullptr, K, w_tiles_dev, static_cast<__nv_bfloat16*>(y_dev), out_cols,
-                       static_cast<const __nv_bfloat16*>(res_dev), out_cols, M, N, K, epi, gate_rows, ws, counters, t,
-                       static_cast<cudaStream_t>(stream));
+  // int32 partials of cut tiles in their own scratch
+  return op_linear(nullptr, w_tiles_dev, y_dev, res_dev, M, N, K, epi, gate_rows, tc::LinearForce(), xq_dev, sa_dev, sw_dev, nullptr, 1,
+                   static_cast<cudaStream_t>(stream));
 }
 
 int b200_op_attn_step(const void* qkv_dev, void* k_dev, void* v_dev, void* out_dev, const int64_t* pos_dev,

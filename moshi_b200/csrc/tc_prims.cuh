@@ -93,5 +93,21 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
   return d;
 }
 
+// distributed shared memory of a thread block cluster: the address of `local_smem_addr` in rank `rank`'s shared memory, a
+// two-word store there, and a barrier over every thread of the cluster (release / acquire)
+__device__ __forceinline__ uint32_t map_to_rank(uint32_t local_smem_addr, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_smem_addr), "r"(rank));
+  return r;
+}
+__device__ __forceinline__ void st_cluster_v2(uint32_t addr, uint32_t a, uint32_t b) {
+  asm volatile("st.shared::cluster.v2.b32 [%0], {%1, %2};" ::"r"(addr), "r"(a), "r"(b) : "memory");
+}
+__device__ __forceinline__ void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
+  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+__device__ __forceinline__ float bf16_round(float v) { return __bfloat162float(__float2bfloat16_rn(v)); }
+
 }  // namespace tcp
 }  // namespace b200
