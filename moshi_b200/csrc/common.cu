@@ -61,7 +61,9 @@ int Arena::alloc(void** out, size_t bytes, bool zero) {
 
 void Arena::free_all() {
   for (void* p : ptrs) cudaFree(p);
+  for (void* p : host) cudaFreeHost(p);
   ptrs.clear();
+  host.clear();
   snap.clear();
 }
 
@@ -73,27 +75,115 @@ size_t Arena::state_bytes() const {
   return n;
 }
 
-int Arena::save(void* dst, cudaStream_t st) const {
-  size_t off = 0;
-  for (auto& s : snap) {
-    B200_CUDA(cudaMemcpyAsync(static_cast<char*>(dst) + off, s.ptr, s.bytes, cudaMemcpyDeviceToDevice, st));
-    off += pad256(s.bytes);
-  }
+int copy_out(const void* src, int64_t size, int64_t bytes, void* dst, int64_t capacity, int64_t* size_out, cudaStream_t st,
+             const char* what) {
+  if (size_out) *size_out = size;
+  if (!dst || !size) return B200_OK;
+  if (capacity < size) B200_FAIL(B200_ERR_SHAPE, "%s: destination too small", what);
+  if (bytes) B200_CUDA(cudaMemcpyAsync(dst, src, (size_t)bytes, cudaMemcpyDeviceToDevice, st));
   return B200_OK;
 }
 
-int Arena::load(const void* src, cudaStream_t st) const {
-  size_t off = 0;
-  for (auto& s : snap) {
-    B200_CUDA(cudaMemcpyAsync(s.ptr, static_cast<const char*>(src) + off, s.bytes, cudaMemcpyDeviceToDevice, st));
-    off += pad256(s.bytes);
-  }
+// ---- the streaming core -------------------------------------------------------------------------------------------------------
+int check_streaming(const StreamCore* h, const char* what) {
+  if (!h) B200_FAIL(B200_ERR_INVALID, "%s: null handle", what);
+  if (!h->finalized) B200_FAIL(B200_ERR_STATE, "%s: handle not finalized", what);
+  if (h->batch <= 0) B200_FAIL(B200_ERR_STATE, "%s: not streaming (call streaming_begin first)", what);
   return B200_OK;
 }
 
-int state_entry_info(const Arena& a, int index, const char** name, int* dtype, int* ndim, int64_t* shape8, int64_t* nbytes) {
-  if (index < 0 || index >= (int)a.snap.size()) B200_FAIL(B200_ERR_INVALID, "state_entry: index %d out of range", index);
-  const StateEntry& e = a.snap[index];
+int check_begin(const StreamCore* h, int batch, const char* what) {
+  if (!h || !h->finalized) B200_FAIL(B200_ERR_STATE, "%s: handle not finalized", what);
+  if (h->batch > 0) B200_FAIL(B200_ERR_STATE, "%s: already streaming", what);     // streaming.py:112
+  if (batch < 1) B200_FAIL(B200_ERR_INVALID, "%s: batch %d", what, batch);
+  return B200_OK;
+}
+
+int StreamCore::open_streams() {
+  B200_CUDA(cudaStreamCreateWithFlags(&gstream, cudaStreamNonBlocking));
+  B200_CUDA(cudaEventCreateWithFlags(&ev_in, cudaEventDisableTiming));
+  B200_CUDA(cudaEventCreateWithFlags(&ev_out, cudaEventDisableTiming));
+  return B200_OK;
+}
+
+void StreamCore::end_streaming() {
+  if (batch > 0) {
+    cudaStreamSynchronize(stream);
+    if (gstream) cudaStreamSynchronize(gstream);
+  }
+  drop_graphs();
+  if (gstream) cudaStreamDestroy(gstream);
+  if (ev_in) cudaEventDestroy(ev_in);
+  if (ev_out) cudaEventDestroy(ev_out);
+  gstream = nullptr;
+  ev_in = ev_out = nullptr;
+  state.free_all();
+  err = nullptr;
+  batch = 0;
+}
+
+int StreamCore::run(Graph& g, const char* what, const std::function<int()>& fn) {
+  if (!graph_enabled) {
+    body = stream;
+    return fn();
+  }
+  B200_CUDA(cudaEventRecord(ev_in, stream));
+  B200_CUDA(cudaStreamWaitEvent(gstream, ev_in, 0));
+  if (!g.exec) {
+    cudaGraph_t graph = nullptr;
+    const int64_t before = g_launches.load();
+    body = gstream;
+    B200_CUDA(cudaStreamBeginCapture(gstream, cudaStreamCaptureModeRelaxed));
+    const int rc = fn();
+    cudaError_t e = cudaStreamEndCapture(gstream, &graph);
+    g.kernels = g_launches.load() - before;
+    g_launches.fetch_sub(g.kernels);      // recorded, not executed
+    body = stream;
+    if (rc != B200_OK) {
+      if (graph) cudaGraphDestroy(graph);
+      return rc;
+    }
+    if (e != cudaSuccess) B200_FAIL(B200_ERR_CUDA, "graph capture of %s failed: %s", what, cudaGetErrorString(e));
+    e = cudaGraphInstantiate(&g.exec, graph, 0);
+    cudaGraphDestroy(graph);
+    if (e != cudaSuccess) {
+      g.exec = nullptr;
+      B200_FAIL(B200_ERR_CUDA, "graph instantiate failed: %s", cudaGetErrorString(e));
+    }
+  }
+  B200_CUDA(cudaGraphLaunch(g.exec, gstream));
+  g_launches.fetch_add(g.kernels);
+  B200_CUDA(cudaEventRecord(ev_out, gstream));
+  B200_CUDA(cudaStreamWaitEvent(stream, ev_out, 0));
+  return B200_OK;
+}
+
+int StreamCore::error_flags(int* flags_out) {
+  int v = 0;
+  B200_CUDA(cudaMemcpyAsync(&v, err, 4, cudaMemcpyDeviceToHost, stream));
+  B200_CUDA(cudaStreamSynchronize(stream));
+  if (v) B200_CUDA(cudaMemsetAsync(err, 0, 4, stream));
+  if (flags_out) *flags_out = v;
+  return B200_OK;
+}
+
+int StreamCore::copy_entry(const StateEntry& e, void* dst, const void* src) {
+  if (dst) B200_CUDA(cudaMemcpyAsync(dst, e.ptr, e.bytes, cudaMemcpyDeviceToDevice, stream));
+  else B200_CUDA(cudaMemcpyAsync(e.ptr, src, e.bytes, cudaMemcpyDeviceToDevice, stream));
+  return B200_OK;
+}
+
+int StreamCore::find_entry(const char* name, int64_t nbytes, const StateEntry** out) const {
+  const StateEntry* e = state.find_state(name ? name : "");
+  if (!e) B200_FAIL(B200_ERR_INVALID, "state entry '%s' does not exist", name ? name : "(null)");
+  if (nbytes != (int64_t)e->bytes) B200_FAIL(B200_ERR_SHAPE, "state entry '%s' holds %zu bytes, caller passed %lld", e->name.c_str(), e->bytes, (long long)nbytes);
+  *out = e;
+  return B200_OK;
+}
+
+int StreamCore::state_entry_info(int index, const char** name, int* dtype, int* ndim, int64_t* shape8, int64_t* nbytes) const {
+  if (index < 0 || index >= (int)state.snap.size()) B200_FAIL(B200_ERR_INVALID, "state_entry: index %d out of range", index);
+  const StateEntry& e = state.snap[index];
   if (name) *name = e.name.c_str();
   if (dtype) *dtype = e.dtype;
   if (ndim) *ndim = (int)e.shape.size();
@@ -102,13 +192,62 @@ int state_entry_info(const Arena& a, int index, const char** name, int* dtype, i
   return B200_OK;
 }
 
-int state_entry_copy(const Arena& a, const char* name, void* dst_dev, const void* src_dev, int64_t nbytes, cudaStream_t st) {
-  const StateEntry* e = a.find_state(name ? name : "");
-  if (!e) B200_FAIL(B200_ERR_INVALID, "state entry '%s' does not exist", name ? name : "(null)");
-  if (nbytes != (int64_t)e->bytes) B200_FAIL(B200_ERR_SHAPE, "state entry '%s' holds %zu bytes, caller passed %lld", e->name.c_str(), e->bytes, (long long)nbytes);
-  if (dst_dev) B200_CUDA(cudaMemcpyAsync(dst_dev, e->ptr, e->bytes, cudaMemcpyDeviceToDevice, st));
-  else if (src_dev) B200_CUDA(cudaMemcpyAsync(e->ptr, src_dev, e->bytes, cudaMemcpyDeviceToDevice, st));
-  else B200_FAIL(B200_ERR_INVALID, "state entry copy: null buffer");
+int StreamCore::state_entry(const char* name, void* dst, const void* src, int64_t nbytes, const char* what) {
+  if (!dst && !src) B200_FAIL(B200_ERR_INVALID, "%s: null buffer", what);
+  const StateEntry* e = nullptr;
+  B200_TRY(find_entry(name, nbytes, &e));
+  return copy_entry(*e, dst, src);
+}
+
+int StreamCore::save_state(void* dst, int64_t capacity, size_t trailer, const char* what) {
+  if (!dst || capacity < (int64_t)(state.state_bytes() + trailer)) B200_FAIL(B200_ERR_SHAPE, "%s: destination too small", what);
+  size_t off = 0;
+  for (auto& e : state.snap) {
+    B200_TRY(copy_entry(e, static_cast<char*>(dst) + off, nullptr));
+    off += pad256(e.bytes);
+  }
+  return B200_OK;
+}
+
+int StreamCore::check_blob(const void* src, int64_t nbytes, size_t trailer, const char* what) const {
+  const int64_t n = (int64_t)(state.state_bytes() + trailer);
+  if (!src || nbytes != n)
+    B200_FAIL(B200_ERR_SHAPE, "%s: snapshot of %lld bytes does not fit this session layout (%lld)", what, (long long)nbytes, (long long)n);
+  return B200_OK;
+}
+
+int StreamCore::load_state(const void* src) {
+  size_t off = 0;
+  for (auto& e : state.snap) {
+    B200_TRY(copy_entry(e, nullptr, static_cast<const char*>(src) + off));
+    off += pad256(e.bytes);
+  }
+  return B200_OK;
+}
+
+int StreamCore::check_row(int row, const char* what) const {
+  if (row < 0 || row >= batch) B200_FAIL(B200_ERR_INVALID, "%s: row %d outside [0, %d)", what, row, batch);
+  return B200_OK;
+}
+
+SessionHeader StreamCore::session_header(int64_t bytes) const {
+  SessionHeader s;
+  memset(&s, 0, sizeof(s));
+  s.magic = SESSION_MAGIC; s.version = SESSION_VERSION; s.kind = session_kind;
+  s.fingerprint = fingerprint; s.rows = 1; s.bytes = bytes;
+  return s;
+}
+
+int StreamCore::read_session_header(const void* src, int64_t nbytes, const char* what, SessionHeader* s) {
+  if (!src) B200_FAIL(B200_ERR_INVALID, "%s: null record", what);
+  if (nbytes < (int64_t)sizeof(SessionHeader)) B200_FAIL(B200_ERR_SHAPE, "%s: %lld bytes hold no record header", what, (long long)nbytes);
+  B200_CUDA(cudaStreamSynchronize(stream));
+  B200_CUDA(cudaMemcpy(s, src, sizeof(*s), cudaMemcpyDeviceToHost));
+  if (s->magic != SESSION_MAGIC || s->version != SESSION_VERSION)
+    B200_FAIL(B200_ERR_INVALID, "%s: not a session record (magic %08x, version %u)", what, s->magic, s->version);
+  if (s->kind != session_kind)
+    B200_FAIL(B200_ERR_INVALID, "%s: the record is not %s session (kind %u)", what, session_kind == SESSION_LM ? "an LM" : "a Mimi", s->kind);
+  if (s->fingerprint != fingerprint) B200_FAIL(B200_ERR_INVALID, "%s: the record was taken with another configuration", what);
   return B200_OK;
 }
 

@@ -9,6 +9,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <string>
 #include <vector>
@@ -94,13 +95,13 @@ struct TensorStore {
   void release_all();
 };
 
-// Device allocation bookkeeping for a handle: everything freed in one place.
+// Device and pinned host allocation bookkeeping for a handle: everything freed in one place, at the latest when the arena goes.
 struct StateEntry {
   std::string name;        // handle-local name; the Python shims map these onto the reference's per-module State fields
   void* ptr; size_t bytes; int dtype; std::vector<int64_t> shape;
 };
 struct Arena {
-  std::vector<void*> ptrs;
+  std::vector<void*> ptrs, host;
   // buffers that make up the streaming state (get/set_streaming_state, streaming.py:158-181), in registration order
   std::vector<StateEntry> snap;
   void mark_state(void* p, size_t bytes, const std::string& name = "", int dtype = B200_U8, std::vector<int64_t> shape = {}) {
@@ -113,14 +114,23 @@ struct Arena {
     return nullptr;
   }
   size_t state_bytes() const;                 // each segment padded to 256 B
-  int save(void* dst, cudaStream_t st) const;
-  int load(const void* src, cudaStream_t st) const;
   int alloc(void** out, size_t bytes, bool zero = true);
   template <typename T>
   int alloc_t(T** out, size_t count, bool zero = true) {
     return alloc(reinterpret_cast<void**>(out), count * sizeof(T), zero);
   }
+  template <typename T>
+  int alloc_host(T** out, size_t count) {     // pinned host memory
+    *out = nullptr;
+    B200_CUDA(cudaMallocHost(reinterpret_cast<void**>(out), count * sizeof(T)));
+    host.push_back(*out);
+    return B200_OK;
+  }
   void free_all();
+  Arena() = default;
+  Arena(const Arena&) = delete;
+  Arena& operator=(const Arena&) = delete;
+  ~Arena() { free_all(); }
 };
 
 // Makes the handle's device current for the duration of an entry point (the reference's modules carry their device; a caller
@@ -133,9 +143,10 @@ struct DeviceGuard {
   ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
 };
 
-// shared body of b200_{lm,mimi}_state_{count,entry,read,write}
-int state_entry_info(const Arena& a, int index, const char** name, int* dtype, int* ndim, int64_t* shape8, int64_t* nbytes);
-int state_entry_copy(const Arena& a, const char* name, void* dst_dev, const void* src_dev, int64_t nbytes, cudaStream_t st);
+// The tail of every *_read_buffer entry point: reports the buffer's size, then (dst non-null) checks the capacity and copies
+// `bytes` from src on `st`.  size and capacity are in the entry point's unit.
+int copy_out(const void* src, int64_t size, int64_t bytes, void* dst, int64_t capacity, int64_t* size_out, cudaStream_t st,
+             const char* what);
 
 // What the frame services (frame.cu) check their handles against and read from them; B200_ERR_STATE unless streaming.  The
 // pointer stays valid until the handle's streaming ends.
@@ -148,6 +159,7 @@ struct MimiFrameView {
 };
 int lm_frame_view(b200_lm* h, LmFrameView* out);         // lm.cu
 int mimi_frame_view(b200_mimi* h, MimiFrameView* out);   // mimi.cu
+int lm_device(const b200_lm* h);                         // lm.cu: the device the frame services allocate and run on
 
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
@@ -197,6 +209,81 @@ inline long long layout_row_slices(std::vector<RowSlice>& slices, long long off)
   }
   return off;
 }
+
+// ---------------------------------------------------------------------------------------------
+// the streaming core of the LM and Mimi handles
+// ---------------------------------------------------------------------------------------------
+// A CUDA graph captured from a fixed launch sequence over static buffers.
+struct Graph {
+  cudaGraphExec_t exec = nullptr;
+  int64_t kernels = 0;                 // kernel launches recorded in it: b200_launch_count advances by these per replay
+  void drop() {
+    if (exec) cudaGraphExecDestroy(exec);
+    exec = nullptr;
+  }
+};
+
+// What b200_lm and b200_mimi share: the device, the streams a batch of sessions runs on, its state arena and error flags, the
+// captured graphs, the state blob and entries, and session-record framing.
+struct StreamCore {
+  int device = -1;                     // CUDA device the handle lives on (made current by every entry point)
+  bool finalized = false;
+  int batch = 0;                       // sessions streaming; 0: not streaming
+  cudaStream_t stream = nullptr;       // caller's stream (inputs and outputs are ordered on it)
+  cudaStream_t gstream = nullptr;      // private stream: graphs cannot be captured on the legacy default stream
+  cudaStream_t body = nullptr;         // stream the kernels are being enqueued on (caller's, or gstream while capturing)
+  cudaEvent_t ev_in = nullptr, ev_out = nullptr;
+  int graph_enabled = 1;
+  Graph graphs[2];                     // the handle's captured bodies (LM: the step; Mimi: encode, decode)
+  Arena state;                         // everything a streaming batch allocates, freed by end_streaming
+  int* err = nullptr;                  // device error flags (B200_FLAG_*)
+  uint32_t session_kind = 0;           // SESSION_LM / SESSION_MIMI
+  uint64_t fingerprint = 0;            // config_fingerprint of the handle's configuration
+
+  virtual ~StreamCore() = default;
+  // streaming_begin: the private stream and the fence events; end_streaming: waits for both streams, then drops the graphs,
+  // destroys the streams and events and frees the state (also on a failed streaming_begin)
+  int open_streams();
+  void end_streaming();
+  void drop_graphs() {
+    for (auto& g : graphs) g.drop();
+  }
+  void set_graph(int enable) {
+    graph_enabled = enable;
+    if (!enable) drop_graphs();
+  }
+  // Runs `fn` (a fixed launch sequence over static buffers, enqueued on `body`) as graph g on the private stream, fenced against
+  // the caller's stream on both sides; the first call captures it, and a failed capture leaves no graph.  With graphs off `fn`
+  // runs eagerly on the caller's stream.
+  int run(Graph& g, const char* what, const std::function<int()>& fn);
+  // Synchronises the caller's stream, returns the device error flags and clears them.
+  int error_flags(int* flags_out);
+
+  // One state entry between the handle and a device buffer (exactly one of dst / src non-null), on the caller's stream.
+  virtual int copy_entry(const StateEntry& e, void* dst, const void* src);
+  int find_entry(const char* name, int64_t nbytes, const StateEntry** out) const;   // the entry, if it holds nbytes bytes
+  int state_entry_info(int index, const char** name, int* dtype, int* ndim, int64_t* shape8, int64_t* nbytes) const;
+  int state_entry(const char* name, void* dst, const void* src, int64_t nbytes, const char* what);
+  // The state blob: every entry in marking order, each 256-byte aligned, then `trailer` bytes the handle owns.  save_state checks
+  // the capacity, check_blob the size of a blob to load.
+  int save_state(void* dst, int64_t capacity, size_t trailer, const char* what);
+  int check_blob(const void* src, int64_t nbytes, size_t trailer, const char* what) const;
+  int load_state(const void* src);
+  // Session records: the header of this handle's kind and configuration for a record of `bytes` (one row, the rest zero), and the
+  // header read back from a device record (synchronises) after checking the size, magic, version, kind and fingerprint.
+  int check_row(int row, const char* what) const;
+  SessionHeader session_header(int64_t bytes) const;
+  int read_session_header(const void* src, int64_t nbytes, const char* what, SessionHeader* s);
+};
+
+// The prologue of every entry point that needs a streaming handle: B200_ERR_INVALID for a null handle, B200_ERR_STATE unless it
+// is finalized and streaming; then the handle's device stays current until the entry point returns.
+int check_streaming(const StreamCore* h, const char* what);
+#define B200_STREAMING_ENTRY(h, what)          \
+  B200_TRY(b200::check_streaming((h), (what))); \
+  b200::DeviceGuard b200_entry_device_((h)->device)
+// The checks of streaming_begin: a finalized handle that is not streaming yet, at least one session.
+int check_begin(const StreamCore* h, int batch, const char* what);
 
 // ---------------------------------------------------------------------------------------------
 // device helpers

@@ -121,8 +121,10 @@ using namespace b200;
 struct b200_frame {
   b200_mimi* mimi = nullptr;
   b200_lm* lm = nullptr;
+  int device = -1;                   // the LM handle's: every entry point makes it current
   int B = 0, dep_q = 0, n_in = 0, frame = 0, noise_row = 0;
   cudaStream_t stream = nullptr;
+  Arena mem;                         // the buffers below
   // device
   float* pcm_in = nullptr; float* pcm_out = nullptr; float* noise = nullptr;
   int64_t* codes_in = nullptr; int64_t* tokens = nullptr; int64_t* codes_out = nullptr;
@@ -138,6 +140,8 @@ struct b200_frame {
 struct b200_asr {
   b200_mimi* mimi = nullptr;
   b200_lm* lm = nullptr;
+  int device = -1;                   // the LM handle's: every entry point makes it current
+  Arena mem;                         // the buffers below
   int B = 0, n_codes = 0, n_user = 0, frame = 0, asr_delay = 0, n_heads = 0;   // n_codes: the codec's, n_user: the LM's n_q - dep_q
   cudaStream_t stream = nullptr;
   // device
@@ -171,25 +175,26 @@ int asr_run(b200_asr* a, const uint8_t* exec) {
 
 int asr_init(b200_asr* a) {
   const size_t B = (size_t)a->B;
-  B200_CUDA(cudaMalloc(&a->pcm_in, B * a->frame * 4));
-  B200_CUDA(cudaMalloc(&a->extra, B * std::max(a->n_heads, 1) * 4));
-  B200_CUDA(cudaMalloc(&a->codes_in, B * a->n_codes * 8));
-  B200_CUDA(cudaMalloc(&a->codes_lm, B * a->n_user * 8));
-  B200_CUDA(cudaMalloc(&a->tokens, B * 8));
-  B200_CUDA(cudaMalloc(&a->updates, B * 4));
-  B200_CUDA(cudaMalloc(&a->flags, 2 * B));
-  B200_CUDA(cudaMalloc(&a->reset, B));
-  B200_CUDA(cudaMalloc(&a->exec, B));
-  B200_CUDA(cudaMalloc(&a->all_rows, B));
-  B200_CUDA(cudaMalloc(&a->slots.active, B));
-  B200_CUDA(cudaMalloc(&a->slots.complete, B));
-  B200_CUDA(cudaMalloc(&a->slots.offset, B * 8));
-  B200_CUDA(cudaMalloc(&a->slots.real_end, B * 8));
-  B200_CUDA(cudaMallocHost(&a->h_pcm_in, B * a->frame * 4));
-  B200_CUDA(cudaMallocHost(&a->h_extra, B * std::max(a->n_heads, 1) * 4));
-  B200_CUDA(cudaMallocHost(&a->h_tokens, B * 8));
-  B200_CUDA(cudaMallocHost(&a->h_updates, B * 4));
-  B200_CUDA(cudaMallocHost(&a->h_flags, 2 * B));
+  Arena& m = a->mem;
+  B200_TRY(m.alloc_t(&a->pcm_in, B * a->frame, false));
+  B200_TRY(m.alloc_t(&a->extra, B * std::max(a->n_heads, 1), false));
+  B200_TRY(m.alloc_t(&a->codes_in, B * a->n_codes, false));
+  B200_TRY(m.alloc_t(&a->codes_lm, B * a->n_user, false));
+  B200_TRY(m.alloc_t(&a->tokens, B, false));
+  B200_TRY(m.alloc_t(&a->updates, B, false));
+  B200_TRY(m.alloc_t(&a->flags, 2 * B, false));
+  B200_TRY(m.alloc_t(&a->reset, B, false));
+  B200_TRY(m.alloc_t(&a->exec, B, false));
+  B200_TRY(m.alloc_t(&a->all_rows, B, false));
+  B200_TRY(m.alloc_t(&a->slots.active, B, false));
+  B200_TRY(m.alloc_t(&a->slots.complete, B, false));
+  B200_TRY(m.alloc_t(&a->slots.offset, B, false));
+  B200_TRY(m.alloc_t(&a->slots.real_end, B, false));
+  B200_TRY(m.alloc_host(&a->h_pcm_in, B * a->frame));
+  B200_TRY(m.alloc_host(&a->h_extra, B * std::max(a->n_heads, 1)));
+  B200_TRY(m.alloc_host(&a->h_tokens, B));
+  B200_TRY(m.alloc_host(&a->h_updates, B));
+  B200_TRY(m.alloc_host(&a->h_flags, 2 * B));
   B200_CUDA(cudaEventCreateWithFlags(&a->done, cudaEventDisableTiming));
   cudaStream_t st = a->stream;
   B200_CUDA(cudaMemsetAsync(a->all_rows, 1, B, st));
@@ -211,6 +216,34 @@ int asr_init(b200_asr* a) {
   return lm_check_kv_pool(a->lm);
 }
 
+int frame_init(b200_frame* f) {
+  const size_t B = (size_t)f->B;
+  Arena& m = f->mem;
+  B200_TRY(m.alloc_t(&f->pcm_in, B * f->frame, false));
+  B200_TRY(m.alloc_t(&f->pcm_out, B * f->frame, false));
+  B200_TRY(m.alloc_t(&f->noise, B * std::max(f->noise_row, 1), false));
+  B200_TRY(m.alloc_t(&f->codes_in, B * f->n_in, false));
+  B200_TRY(m.alloc_t(&f->tokens, B * (f->dep_q + 1), false));
+  B200_TRY(m.alloc_t(&f->codes_out, B * f->dep_q, false));
+  B200_TRY(m.alloc_t(&f->updates, B, false));
+  B200_TRY(m.alloc_t(&f->active, B, false));
+  B200_TRY(m.alloc_t(&f->reset, B, false));
+  B200_TRY(m.alloc_t(&f->exec, B, false));
+  B200_TRY(m.alloc_t(&f->dec_exec, B, false));
+  B200_TRY(m.alloc_t(&f->ready, B, false));
+  B200_CUDA(cudaMemsetAsync(f->active, 1, B, f->stream));          // streaming() starts with every row executing (streaming.py:31-33)
+  B200_CUDA(cudaMemsetAsync(f->exec, 1, B, f->stream));
+  B200_CUDA(cudaMemsetAsync(f->reset, 0, B, f->stream));
+  B200_TRY(m.alloc_host(&f->h_pcm_in, B * f->frame));
+  B200_TRY(m.alloc_host(&f->h_pcm_out, B * f->frame));
+  B200_TRY(m.alloc_host(&f->h_noise, B * std::max(f->noise_row, 1)));
+  B200_TRY(m.alloc_host(&f->h_tokens, B * (f->dep_q + 1)));
+  B200_TRY(m.alloc_host(&f->h_updates, B));
+  B200_TRY(m.alloc_host(&f->h_ready, B));
+  B200_CUDA(cudaEventCreateWithFlags(&f->done, cudaEventDisableTiming));
+  return B200_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -222,43 +255,25 @@ int b200_frame_create(b200_mimi* mimi, b200_lm* lm, int batch, int n_codebooks, 
   if (n_codebooks != dep_q)
     B200_FAIL(B200_ERR_SHAPE, "frame_create: the decoder takes the dep_q generated codebooks (%d), the codec has %d", dep_q, n_codebooks);
   auto* f = new b200_frame();
-  f->mimi = mimi; f->lm = lm; f->B = batch; f->dep_q = dep_q; f->n_in = n_codebooks; f->frame = frame_size;
+  f->mimi = mimi; f->lm = lm; f->device = lm_device(lm);
+  f->B = batch; f->dep_q = dep_q; f->n_in = n_codebooks; f->frame = frame_size;
   f->stream = static_cast<cudaStream_t>(stream);
   f->noise_row = b200_lm_noise_per_row(lm);
   f->h_active.assign((size_t)batch, 1);
-  const size_t B = (size_t)batch;
-  B200_CUDA(cudaMalloc(&f->pcm_in, B * frame_size * 4));
-  B200_CUDA(cudaMalloc(&f->pcm_out, B * frame_size * 4));
-  B200_CUDA(cudaMalloc(&f->noise, B * (size_t)std::max(f->noise_row, 1) * 4));
-  B200_CUDA(cudaMalloc(&f->codes_in, B * n_codebooks * 8));
-  B200_CUDA(cudaMalloc(&f->tokens, B * (dep_q + 1) * 8));
-  B200_CUDA(cudaMalloc(&f->codes_out, B * dep_q * 8));
-  B200_CUDA(cudaMalloc(&f->updates, B * 4));
-  B200_CUDA(cudaMalloc(&f->active, B));
-  B200_CUDA(cudaMalloc(&f->reset, B));
-  B200_CUDA(cudaMalloc(&f->exec, B));
-  B200_CUDA(cudaMalloc(&f->dec_exec, B));
-  B200_CUDA(cudaMalloc(&f->ready, B));
-  B200_CUDA(cudaMemsetAsync(f->active, 1, B, f->stream));          // streaming() starts with every row executing (streaming.py:31-33)
-  B200_CUDA(cudaMemsetAsync(f->exec, 1, B, f->stream));
-  B200_CUDA(cudaMemsetAsync(f->reset, 0, B, f->stream));
-  B200_CUDA(cudaMallocHost(&f->h_pcm_in, B * frame_size * 4));
-  B200_CUDA(cudaMallocHost(&f->h_pcm_out, B * frame_size * 4));
-  B200_CUDA(cudaMallocHost(&f->h_noise, B * (size_t)std::max(f->noise_row, 1) * 4));
-  B200_CUDA(cudaMallocHost(&f->h_tokens, B * (dep_q + 1) * 8));
-  B200_CUDA(cudaMallocHost(&f->h_updates, B * 4));
-  B200_CUDA(cudaMallocHost(&f->h_ready, B));
-  B200_CUDA(cudaEventCreateWithFlags(&f->done, cudaEventDisableTiming));
+  DeviceGuard g(f->device);
+  const int rc = frame_init(f);
+  if (rc != B200_OK) {
+    const std::string msg = b200_last_error();
+    b200_frame_destroy(f);
+    B200_FAIL(rc, "%s", msg.c_str());
+  }
   *out = f;
   return B200_OK;
 }
 
 int b200_frame_destroy(b200_frame* f) {
   if (!f) return B200_OK;
-  cudaFree(f->pcm_in); cudaFree(f->pcm_out); cudaFree(f->noise); cudaFree(f->codes_in); cudaFree(f->tokens); cudaFree(f->codes_out);
-  cudaFree(f->updates); cudaFree(f->active); cudaFree(f->reset); cudaFree(f->exec); cudaFree(f->dec_exec); cudaFree(f->ready);
-  cudaFreeHost(f->h_pcm_in); cudaFreeHost(f->h_pcm_out); cudaFreeHost(f->h_noise); cudaFreeHost(f->h_tokens);
-  cudaFreeHost(f->h_updates); cudaFreeHost(f->h_ready);
+  DeviceGuard g(f->device);
   if (f->done) cudaEventDestroy(f->done);
   delete f;
   return B200_OK;
@@ -266,6 +281,7 @@ int b200_frame_destroy(b200_frame* f) {
 
 int b200_frame_read_buffer(b200_frame* f, const char* name, void* dst_dev, int64_t capacity_bytes, int64_t* nbytes) {
   if (!f || !name) B200_FAIL(B200_ERR_INVALID, "frame_read_buffer: null argument");
+  DeviceGuard g(f->device);
   const std::string n = name;
   const size_t B = (size_t)f->B;
   const void* src = nullptr; int64_t sz = 0;
@@ -275,16 +291,13 @@ int b200_frame_read_buffer(b200_frame* f, const char* name, void* dst_dev, int64
   else if (n == "exec") { src = f->exec; sz = (int64_t)B; }
   else if (n == "decoder_exec") { src = f->dec_exec; sz = (int64_t)B; }
   else B200_FAIL(B200_ERR_INVALID, "frame_read_buffer: unknown buffer '%s'", name);
-  if (nbytes) *nbytes = sz;
-  if (!dst_dev) return B200_OK;
-  if (capacity_bytes < sz) B200_FAIL(B200_ERR_SHAPE, "frame_read_buffer: destination too small");
-  B200_CUDA(cudaMemcpyAsync(dst_dev, src, (size_t)sz, cudaMemcpyDeviceToDevice, f->stream));
-  return B200_OK;
+  return copy_out(src, sz, sz, dst_dev, capacity_bytes, nbytes, f->stream, "frame_read_buffer");
 }
 
 int b200_frame_step(b200_frame* f, const float* pcm_in_host, const int32_t* updates_host, const float* noise_host,
                     const float* noise_dev, float* pcm_out_host, int64_t* tokens_out_host, uint8_t* ready_out_host) {
   if (!f || !pcm_in_host || !pcm_out_host || !tokens_out_host) B200_FAIL(B200_ERR_INVALID, "frame_step: null buffers");
+  DeviceGuard g(f->device);
   const size_t B = (size_t)f->B;
   cudaStream_t st = f->stream;
   memcpy(f->h_pcm_in, pcm_in_host, B * f->frame * 4);
@@ -357,9 +370,10 @@ int b200_asr_create(b200_mimi* mimi, b200_lm* lm, int batch, int asr_delay_in_to
   if (lv.max_delay != 0)     // step() would return None for the first frames: the reference's warm-up asserts it does not
     B200_FAIL(B200_ERR_INVALID, "asr_create: the speech-to-text service runs models without delays, got max delay %d", lv.max_delay);
   auto* a = new b200_asr();
-  a->mimi = mimi; a->lm = lm; a->B = batch; a->n_codes = mv.num_codebooks; a->n_user = lv.n_q - lv.dep_q; a->frame = mv.frame_size;
+  a->mimi = mimi; a->lm = lm; a->device = lm_device(lm); a->B = batch; a->n_codes = mv.num_codebooks; a->n_user = lv.n_q - lv.dep_q; a->frame = mv.frame_size;
   a->asr_delay = asr_delay_in_tokens; a->n_heads = lv.extra_heads;
   a->stream = static_cast<cudaStream_t>(stream);
+  DeviceGuard g(a->device);
   const int rc = asr_init(a);
   if (rc != B200_OK) {
     const std::string msg = b200_last_error();
@@ -372,11 +386,8 @@ int b200_asr_create(b200_mimi* mimi, b200_lm* lm, int batch, int asr_delay_in_to
 
 int b200_asr_destroy(b200_asr* a) {
   if (!a) return B200_OK;
+  DeviceGuard g(a->device);
   cudaStreamSynchronize(a->stream);
-  cudaFree(a->pcm_in); cudaFree(a->extra); cudaFree(a->codes_in); cudaFree(a->codes_lm); cudaFree(a->tokens); cudaFree(a->updates);
-  cudaFree(a->flags); cudaFree(a->reset); cudaFree(a->exec); cudaFree(a->all_rows);
-  cudaFree(a->slots.active); cudaFree(a->slots.complete); cudaFree(a->slots.offset); cudaFree(a->slots.real_end);
-  cudaFreeHost(a->h_pcm_in); cudaFreeHost(a->h_extra); cudaFreeHost(a->h_tokens); cudaFreeHost(a->h_updates); cudaFreeHost(a->h_flags);
   if (a->done) cudaEventDestroy(a->done);
   delete a;
   return B200_OK;
@@ -384,6 +395,7 @@ int b200_asr_destroy(b200_asr* a) {
 
 int b200_asr_read_buffer(b200_asr* a, const char* name, void* dst_dev, int64_t capacity_bytes, int64_t* nbytes) {
   if (!a || !name) B200_FAIL(B200_ERR_INVALID, "asr_read_buffer: null argument");
+  DeviceGuard g(a->device);
   const std::string n = name;
   const size_t B = (size_t)a->B;
   const void* src = nullptr; int64_t sz = 0;
@@ -395,11 +407,7 @@ int b200_asr_read_buffer(b200_asr* a, const char* name, void* dst_dev, int64_t c
   else if (n == "offset") { src = a->slots.offset; sz = (int64_t)(B * 8); }
   else if (n == "real_end") { src = a->slots.real_end; sz = (int64_t)(B * 8); }
   else B200_FAIL(B200_ERR_INVALID, "asr_read_buffer: unknown buffer '%s'", name);
-  if (nbytes) *nbytes = sz;
-  if (!dst_dev || !sz) return B200_OK;
-  if (capacity_bytes < sz) B200_FAIL(B200_ERR_SHAPE, "asr_read_buffer: destination too small");
-  B200_CUDA(cudaMemcpyAsync(dst_dev, src, (size_t)sz, cudaMemcpyDeviceToDevice, a->stream));
-  return B200_OK;
+  return copy_out(src, sz, sz, dst_dev, capacity_bytes, nbytes, a->stream, "asr_read_buffer");
 }
 
 int b200_asr_step(b200_asr* a, const float* pcm_in_host, const int32_t* updates_host, uint8_t* flags_inout_host,
@@ -407,6 +415,7 @@ int b200_asr_step(b200_asr* a, const float* pcm_in_host, const int32_t* updates_
   if (ran) *ran = 0;
   if (!a || !pcm_in_host || !updates_host || !flags_inout_host || !tokens_out_host || (a->n_heads && !extra_heads_out_host))
     B200_FAIL(B200_ERR_INVALID, "asr_step: null buffers");
+  DeviceGuard g(a->device);
   MimiFrameView mv{};
   LmFrameView lv{};
   B200_TRY(mimi_frame_view(a->mimi, &mv));

@@ -53,18 +53,11 @@ void b200::lm::cross_attn_launch(const bf16* q, long long ldq, const bf16* kc, c
   B200_LAUNCH(cross_attn_step_kernel, dim3(B * H, nsplit), ATT_THREADS, 0, st, a);
 }
 
-struct b200_lm {
+struct b200_lm : StreamCore {       // batch: sessions (LMGen batch); graphs[0]: the step
   b200_lm_config cfg;
   TensorStore store;
-  Arena weights, state;
-  bool finalized = false;
-  int device = -1;                     // CUDA device the handle lives on (made current by every entry point)
-  int batch = 0;                       // sessions (LMGen batch)
+  Arena weights;
   int MB = 0;                          // rows the model runs on: batch, or 2 * batch under classifier-free guidance (lm.py:646-647)
-  cudaStream_t stream = nullptr;       // caller's stream (inputs/outputs are ordered on it)
-  cudaStream_t gstream = nullptr;      // private stream: graphs cannot be captured on the legacy default stream
-  cudaStream_t body = nullptr;         // stream the step body is currently being enqueued on
-  cudaEvent_t ev_in = nullptr, ev_out = nullptr;
   int Kc = 0, max_delay = 0, CT = 0;
   // sampling (LMGen defaults, lm.py:556-571)
   int use_sampling = 1, top_k = 250, top_k_text = 25;
@@ -98,7 +91,6 @@ struct b200_lm {
   std::vector<const bf16*> extra_w; const bf16** extra_w_dev = nullptr; bf16* extra_out = nullptr;
   // Exp(1) noise drawn inside the step (when the caller passes none): Philox keyed by (seed, step counter)
   unsigned long long noise_seed = 0x9E3779B97F4A7C15ull; unsigned long long* noise_ctr = nullptr; int noise_internal = 0;
-  int* err = nullptr;                          // device error flags (lm::ERR_*)
   // activations
   long long *in_codes = nullptr, *input_tokens = nullptr, *text_token = nullptr, *audio_tokens = nullptr, *out_tokens = nullptr;
   float* noise = nullptr;
@@ -140,15 +132,13 @@ struct b200_lm {
   int noise_static = 0;                        // 1: the captured step draws its own noise
   int replace_static = 0;                      // 1: this step's audio tokens are given (depformer_replace_tokens, lm.py:751-755)
   long long* replace_tokens = nullptr;         // [B][dep_q] staging of those tokens
-  // graph
-  int graph_enabled = 1;
-  cudaGraphExec_t graph_exec = nullptr;
-  int64_t graph_kernels = 0;                   // kernel nodes in the captured step (for b200_launch_count)
-  // host staging
+  // pinned host staging
   long long *pin_in = nullptr, *pin_out = nullptr;
   float* pin_noise = nullptr;
   int64_t weight_bytes = 0;
   tc::TensorMapCache maps;
+  // a paged handle gathers its K / V entries into ring layout and scatters them back (kv_copy)
+  int copy_entry(const StateEntry& e, void* dst, const void* src) override;
 };
 
 namespace {
@@ -433,20 +423,6 @@ int step_body(b200_lm* h) {
   return check_launch("lm step");
 }
 
-int ensure_streaming(b200_lm* h, const char* what) {
-  if (!h) B200_FAIL(B200_ERR_INVALID, "%s: null handle", what);
-  if (!h->finalized) B200_FAIL(B200_ERR_STATE, "%s: handle not finalized", what);
-  if (h->batch <= 0) B200_FAIL(B200_ERR_STATE, "%s: not streaming (wrap calls in streaming())", what);   // lm.py:673-676
-  return B200_OK;
-}
-
-void drop_graph(b200_lm* h) {
-  if (h->graph_exec) {
-    cudaGraphExecDestroy(h->graph_exec);
-    h->graph_exec = nullptr;
-  }
-}
-
 // pages a row holds at model position `pos`: those of slots [0, min(pos, context))
 int pages_for(const b200_lm* h, long long pos) {
   const long long n = std::min(std::max(pos, 0LL), (long long)h->cfg.context);
@@ -525,17 +501,6 @@ int kv_copy(b200_lm* h, int first, int n_arrays, int row0, int n_rows, int row_s
   return check_launch("kv_copy");
 }
 
-// One state entry between the handle and a device buffer (exactly one of dst / src is non-null), on the handle's stream.
-int state_copy(b200_lm* h, const StateEntry& e, void* dst, const void* src) {
-  const int arr = paged_array_of(h, e);
-  if (arr < 0) {
-    if (dst) B200_CUDA(cudaMemcpyAsync(dst, e.ptr, e.bytes, cudaMemcpyDeviceToDevice, h->stream));
-    else B200_CUDA(cudaMemcpyAsync(e.ptr, src, e.bytes, cudaMemcpyDeviceToDevice, h->stream));
-    return B200_OK;
-  }
-  return kv_copy(h, arr, 1, 0, h->MB, 1, h->cfg.context, dst ? dst : const_cast<void*>(src), dst != nullptr, false);
-}
-
 // the model positions a write of `model.offset` from `src_dev` would set, on the host
 int read_positions(b200_lm* h, const void* src_dev, std::vector<long long>* pos) {
   pos->assign(h->MB, 0);
@@ -572,11 +537,9 @@ void session_size(const b200_lm* h, SessionPlan* p) {
   }
 }
 
-uint64_t lm_fingerprint(const b200_lm* h) { return config_fingerprint(&h->cfg, sizeof(h->cfg)); }
-
 // The record row `row` would export now (synchronises): B200_ERR_STATE for a short-ring row whose ring has already wrapped.
 int session_plan(b200_lm* h, int row, const char* what, SessionPlan* p) {
-  if (row < 0 || row >= h->batch) B200_FAIL(B200_ERR_INVALID, "%s: row %d outside [0, %d)", what, row, h->batch);
+  B200_TRY(h->check_row(row, what));
   p->rows = h->MB / h->batch;
   B200_CUDA(cudaStreamSynchronize(h->stream));
   for (int k = 0; k < p->rows; ++k)
@@ -615,6 +578,12 @@ int session_kv(b200_lm* h, int row, const SessionPlan& p, char* rec, bool gather
 
 }  // namespace
 
+int b200_lm::copy_entry(const StateEntry& e, void* dst, const void* src) {
+  const int arr = paged_array_of(this, e);
+  if (arr < 0) return StreamCore::copy_entry(e, dst, src);
+  return kv_copy(this, arr, 1, 0, MB, 1, cfg.context, dst ? dst : const_cast<void*>(src), dst != nullptr, false);
+}
+
 namespace b200 {
 // b200_frame_step: a row the KV pool could not serve fails the frame (B200_ERR_STATE), as b200_lm_step_host does.  Synchronises;
 // clears that flag only, the others stay for b200_lm_error_flags.
@@ -632,11 +601,13 @@ int lm_check_kv_pool(b200_lm* h) {
 }
 
 int lm_frame_view(b200_lm* h, LmFrameView* v) {
-  B200_TRY(ensure_streaming(h, "lm_frame_view"));
+  B200_TRY(check_streaming(h, "lm_frame_view"));
   const auto& c = h->cfg;
   *v = LmFrameView{h->batch, h->MB, c.n_q, c.dep_q, h->max_delay, (int)h->extra_w.size(), c.extra_heads_dim, h->extra_out};
   return B200_OK;
 }
+
+int lm_device(const b200_lm* h) { return h->device; }
 }  // namespace b200
 
 extern "C" {
@@ -658,6 +629,8 @@ int b200_lm_create(const b200_lm_config* cfg, b200_lm** out) {
   b200_lm* h = new b200_lm();
   h->cfg = *cfg;
   cudaGetDevice(&h->device);
+  h->session_kind = SESSION_LM;
+  h->fingerprint = config_fingerprint(&h->cfg, sizeof(h->cfg));
   h->Kc = cfg->n_q + 1;
   h->max_delay = 0;
   for (int k = 0; k < h->Kc; ++k) h->max_delay = cfg->delays[k] > h->max_delay ? cfg->delays[k] : h->max_delay;
@@ -829,7 +802,7 @@ int b200_lm_set_sampling(b200_lm* h, int use_sampling, float temp, float temp_te
     return B200_OK;
   h->use_sampling = use_sampling; h->temp = temp; h->temp_text = temp_text; h->top_k = top_k; h->top_k_text = top_k_text;
   tc::dep_fused_set_sampling(h->depf, use_sampling, temp, top_k);
-  drop_graph(h);         // the sampling parameters are kernel arguments of the captured step
+  h->graphs[0].drop();         // the sampling parameters are kernel arguments of the captured step
   return B200_OK;
 }
 
@@ -837,8 +810,7 @@ int b200_lm_noise_per_row(b200_lm* h) { return h ? noise_per_row(h) : 0; }
 
 int b200_lm_set_graph(b200_lm* h, int enable) {
   if (!h) B200_FAIL(B200_ERR_INVALID, "lm_set_graph: null handle");
-  h->graph_enabled = enable;
-  if (!enable) drop_graph(h);
+  h->set_graph(enable);
   return B200_OK;
 }
 
@@ -858,20 +830,18 @@ int b200_lm_seed_noise(b200_lm* h, uint64_t seed) {
   h->noise_seed = seed;
   DeviceGuard g(h->device);
   if (h->noise_ctr) B200_CUDA(cudaMemsetAsync(h->noise_ctr, 0, 8, h->stream));
-  drop_graph(h);         // the seed is a kernel argument of the captured step
+  h->graphs[0].drop();         // the seed is a kernel argument of the captured step
   return B200_OK;
 }
 
 int b200_lm_set_stream(b200_lm* h, void* stream) {
-  B200_TRY(ensure_streaming(h, "lm_set_stream"));
+  B200_STREAMING_ENTRY(h, "lm_set_stream");
   h->stream = static_cast<cudaStream_t>(stream);
   return B200_OK;
 }
 
 int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
-  if (!h || !h->finalized) B200_FAIL(B200_ERR_STATE, "lm_streaming_begin: handle not finalized");
-  if (h->batch > 0) B200_FAIL(B200_ERR_STATE, "lm_streaming_begin: already streaming");
-  if (batch < 1) B200_FAIL(B200_ERR_INVALID, "lm_streaming_begin: batch %d", batch);
+  B200_TRY(check_begin(h, batch, "lm_streaming_begin"));
   DeviceGuard guard_dev(h->device);
   const auto& c = h->cfg;
   const bool cfg = cfg_on(h);
@@ -881,7 +851,7 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
     B200_FAIL(B200_ERR_SHAPE, "lm_streaming_begin: cfg_is_masked_until has %zu entries for %d sessions", h->cfg_until_host.size(), B);
   h->stream = static_cast<cudaStream_t>(stream);
   Arena& A = h->state;
-  struct Cleanup { b200_lm* h; bool armed = true; ~Cleanup() { if (armed) { h->state.free_all(); h->cfg_until = nullptr; h->noise_ctr = nullptr; h->n_pages = 0; } } } cleanup{h};
+  struct Cleanup { b200_lm* h; bool armed = true; ~Cleanup() { if (armed) b200_lm_streaming_end(h); } } cleanup{h};
   size_t free_b = 0, total_b = 0;
   cudaMemGetInfo(&free_b, &total_b);
   const int cap = ring_cap(h);
@@ -1002,12 +972,10 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
   h->cross_nsplit = h->cross_on ? attn_pick_splits(MB, H, h->cross_len) : 1;      // the cross step shares the partials
   B200_TRY(A.alloc_t(&h->attn_part, (size_t)MB * H * (h->cross_on ? std::max(ns, h->cross_nsplit) : ns) * (ATT_D + 2)));
   B200_TRY(A.alloc_t(&h->attn_counters, (size_t)MB * H));
-  B200_CUDA(cudaStreamCreateWithFlags(&h->gstream, cudaStreamNonBlocking));
-  B200_CUDA(cudaEventCreateWithFlags(&h->ev_in, cudaEventDisableTiming));
-  B200_CUDA(cudaEventCreateWithFlags(&h->ev_out, cudaEventDisableTiming));
-  B200_CUDA(cudaMallocHost(&h->pin_in, (size_t)B * n_in_max * 8));
-  B200_CUDA(cudaMallocHost(&h->pin_out, (size_t)B * (c.dep_q + 1) * 8));
-  B200_CUDA(cudaMallocHost(&h->pin_noise, (size_t)B * noise_per_row(h) * 4));
+  B200_TRY(h->open_streams());
+  B200_TRY(A.alloc_host(&h->pin_in, (size_t)B * n_in_max));
+  B200_TRY(A.alloc_host(&h->pin_out, (size_t)B * (c.dep_q + 1)));
+  B200_TRY(A.alloc_host(&h->pin_noise, (size_t)B * noise_per_row(h)));
   if (c.quantize) {     // activations are re-quantised row-wise before every linear (QLinear.forward, utils/quantize.py:28-36)
     const int kmax = std::max(std::max(d, c.ffn_hidden), std::max(dd, c.depformer_ffn_hidden));
     B200_TRY(A.alloc_t(&h->xq, (size_t)MB * kmax, false));
@@ -1121,46 +1089,29 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
 int64_t b200_lm_state_bytes(b200_lm* h) { return (h && h->batch > 0) ? (int64_t)h->state.state_bytes() + 256 : 0; }
 
 int b200_lm_get_state(b200_lm* h, void* dst_dev, int64_t capacity) {
-  B200_TRY(ensure_streaming(h, "lm_get_state"));
-  DeviceGuard g(h->device);
+  B200_STREAMING_ENTRY(h, "lm_get_state");
+  B200_TRY(h->save_state(dst_dev, capacity, 256, "lm_get_state"));    // a paged handle's blob is a contiguous one's
   const size_t n = h->state.state_bytes();
-  if (!dst_dev || capacity < (int64_t)n + 256) B200_FAIL(B200_ERR_SHAPE, "lm_get_state: destination too small");
-  if (h->n_pages) {          // the same blob as a contiguous handle's: the K / V entries are gathered into ring layout
-    size_t off = 0;
-    for (auto& e : h->state.snap) {
-      B200_TRY(state_copy(h, e, static_cast<char*>(dst_dev) + off, nullptr));
-      off += (e.bytes + 255) / 256 * 256;
-    }
-  } else {
-    B200_TRY(h->state.save(dst_dev, h->stream));
-  }
   B200_CUDA(cudaMemcpyAsync(static_cast<char*>(dst_dev) + n, &h->offset_cpu, 8, cudaMemcpyHostToDevice, h->stream));
   B200_CUDA(cudaStreamSynchronize(h->stream));
   return B200_OK;
 }
 
 int b200_lm_set_state(b200_lm* h, const void* src_dev, int64_t nbytes) {
-  B200_TRY(ensure_streaming(h, "lm_set_state"));
-  DeviceGuard g(h->device);
+  B200_STREAMING_ENTRY(h, "lm_set_state");
+  B200_TRY(h->check_blob(src_dev, nbytes, 256, "lm_set_state"));
   const size_t n = h->state.state_bytes();
-  if (!src_dev || nbytes != (int64_t)n + 256) B200_FAIL(B200_ERR_SHAPE, "lm_set_state: snapshot does not fit this session layout");
   if (h->n_pages) {          // map the snapshot's fill first (nothing changes if it does not fit), then scatter its K / V
-    size_t off = 0, off_pos = 0;
+    size_t off_pos = 0;
     for (auto& e : h->state.snap) {
-      if (e.name == "model.offset") off_pos = off;
-      off += (e.bytes + 255) / 256 * 256;
+      if (e.name == "model.offset") break;
+      off_pos += (e.bytes + 255) / 256 * 256;
     }
     std::vector<long long> pos;
     B200_TRY(read_positions(h, static_cast<const char*>(src_dev) + off_pos, &pos));
     B200_TRY(pool_map(h, 0, 1, pos, "lm_set_state"));
-    off = 0;
-    for (auto& e : h->state.snap) {
-      B200_TRY(state_copy(h, e, nullptr, static_cast<const char*>(src_dev) + off));
-      off += (e.bytes + 255) / 256 * 256;
-    }
-  } else {
-    B200_TRY(h->state.load(src_dev, h->stream));
   }
+  B200_TRY(h->load_state(src_dev));
   B200_CUDA(cudaMemcpyAsync(&h->offset_cpu, static_cast<const char*>(src_dev) + n, 8, cudaMemcpyDeviceToHost, h->stream));
   B200_CUDA(cudaStreamSynchronize(h->stream));
   return B200_OK;
@@ -1169,37 +1120,27 @@ int b200_lm_set_state(b200_lm* h, const void* src_dev, int64_t nbytes) {
 /* the same state, entry by entry (the Python shim groups them into the reference's per-module State objects) */
 int b200_lm_state_count(b200_lm* h) { return (h && h->batch > 0) ? (int)h->state.snap.size() : 0; }
 int b200_lm_state_entry(b200_lm* h, int index, const char** name, int* dtype, int* ndim, int64_t* shape8, int64_t* nbytes) {
-  B200_TRY(ensure_streaming(h, "lm_state_entry"));
-  return state_entry_info(h->state, index, name, dtype, ndim, shape8, nbytes);
+  B200_TRY(check_streaming(h, "lm_state_entry"));
+  return h->state_entry_info(index, name, dtype, ndim, shape8, nbytes);
 }
 int b200_lm_state_read(b200_lm* h, const char* name, void* dst_dev, int64_t nbytes) {
-  B200_TRY(ensure_streaming(h, "lm_state_read"));
-  DeviceGuard g(h->device);
-  if (!dst_dev) B200_FAIL(B200_ERR_INVALID, "lm_state_read: null destination");
-  if (!h->n_pages) return state_entry_copy(h->state, name, dst_dev, nullptr, nbytes, h->stream);
-  const StateEntry* e = h->state.find_state(name ? name : "");
-  if (!e) B200_FAIL(B200_ERR_INVALID, "state entry '%s' does not exist", name ? name : "(null)");
-  if (nbytes != (int64_t)e->bytes) B200_FAIL(B200_ERR_SHAPE, "state entry '%s' holds %zu bytes, caller passed %lld", name, e->bytes, (long long)nbytes);
-  return state_copy(h, *e, dst_dev, nullptr);
+  B200_STREAMING_ENTRY(h, "lm_state_read");
+  return h->state_entry(name, dst_dev, nullptr, nbytes, "lm_state_read");
 }
 int b200_lm_state_write(b200_lm* h, const char* name, const void* src_dev, int64_t nbytes) {
-  B200_TRY(ensure_streaming(h, "lm_state_write"));
-  DeviceGuard g(h->device);
-  if (!src_dev) B200_FAIL(B200_ERR_INVALID, "lm_state_write: null source");
-  if (!h->n_pages) return state_entry_copy(h->state, name, nullptr, src_dev, nbytes, h->stream);
-  const StateEntry* e = h->state.find_state(name ? name : "");
-  if (!e) B200_FAIL(B200_ERR_INVALID, "state entry '%s' does not exist", name ? name : "(null)");
-  if (nbytes != (int64_t)e->bytes) B200_FAIL(B200_ERR_SHAPE, "state entry '%s' holds %zu bytes, caller passed %lld", name, e->bytes, (long long)nbytes);
-  if (e->name == "model.offset") {     // each row then holds exactly the pages of its new fill
+  B200_STREAMING_ENTRY(h, "lm_state_write");
+  if (h->n_pages && src_dev && name && !strcmp(name, "model.offset")) {     // each row then holds exactly the pages of its new fill
+    const StateEntry* e = nullptr;
+    B200_TRY(h->find_entry(name, nbytes, &e));
     std::vector<long long> pos;
     B200_TRY(read_positions(h, src_dev, &pos));
     B200_TRY(pool_map(h, 0, 1, pos, "lm_state_write"));
   }
-  return state_copy(h, *e, nullptr, src_dev);
+  return h->state_entry(name, nullptr, src_dev, nbytes, "lm_state_write");
 }
 int64_t b200_lm_get_offset_cpu(b200_lm* h) { return h ? h->offset_cpu : 0; }
 int b200_lm_set_offset_cpu(b200_lm* h, int64_t v) {
-  B200_TRY(ensure_streaming(h, "lm_set_offset_cpu"));
+  B200_TRY(check_streaming(h, "lm_set_offset_cpu"));
   h->offset_cpu = v;
   return B200_OK;
 }
@@ -1207,36 +1148,22 @@ int b200_lm_set_offset_cpu(b200_lm* h, int64_t v) {
 int b200_lm_streaming_end(b200_lm* h) {
   if (!h) return B200_OK;
   DeviceGuard g(h->device);
-  if (h->batch > 0) {
-    cudaStreamSynchronize(h->stream);
-    if (h->gstream) cudaStreamSynchronize(h->gstream);
-  }
-  drop_graph(h);
-  if (h->gstream) cudaStreamDestroy(h->gstream);
-  if (h->ev_in) cudaEventDestroy(h->ev_in);
-  if (h->ev_out) cudaEventDestroy(h->ev_out);
-  h->gstream = nullptr; h->ev_in = h->ev_out = nullptr;
+  h->end_streaming();
   h->maps.clear();
   tc::dep_fused_destroy(h->depf);
   h->depf = nullptr;
-  h->state.free_all();
-  h->cfg_until = nullptr; h->noise_ctr = nullptr; h->err = nullptr; h->cond_sum = nullptr; h->cond_on = 0;
+  h->cfg_until = nullptr; h->noise_ctr = nullptr; h->cond_sum = nullptr; h->cond_on = 0;
   h->n_pages = 0;
   h->page_table = h->page_held = h->free_stack = h->free_top = nullptr;
   h->taps = nullptr; h->taps_on = 0;
-  if (h->pin_in) cudaFreeHost(h->pin_in);
-  if (h->pin_out) cudaFreeHost(h->pin_out);
-  if (h->pin_noise) cudaFreeHost(h->pin_noise);
   h->pin_in = h->pin_out = nullptr;
   h->pin_noise = nullptr;
-  h->batch = 0;
   h->MB = 0;
   return B200_OK;
 }
 
 int b200_lm_reset(b200_lm* h, const uint8_t* reset_mask_dev) {
-  B200_TRY(ensure_streaming(h, "lm_reset"));
-  DeviceGuard g(h->device);
+  B200_STREAMING_ENTRY(h, "lm_reset");
   const int B = h->batch;
   if (h->n_pages)         // a reset row's pages return to the pool
     B200_LAUNCH(kv_page_free_kernel, 1, KV_PAGE_THREADS, 0, h->stream, h->page_table, h->page_held, h->free_stack, h->free_top,
@@ -1250,8 +1177,7 @@ int b200_lm_reset(b200_lm* h, const uint8_t* reset_mask_dev) {
 }
 
 int b200_lm_set_exec_mask(b200_lm* h, const uint8_t* exec_mask_dev) {
-  B200_TRY(ensure_streaming(h, "lm_set_exec_mask"));
-  DeviceGuard g(h->device);
+  B200_STREAMING_ENTRY(h, "lm_set_exec_mask");
   if (!exec_mask_dev) B200_FAIL(B200_ERR_INVALID, "lm_set_exec_mask: null mask");
   B200_CUDA(cudaMemcpyAsync(h->exec_mask, exec_mask_dev, h->batch, cudaMemcpyDeviceToDevice, h->stream));
   if (cfg_on(h)) {      // exec_mask.repeat(2) (lm.py:658-661)
@@ -1262,13 +1188,12 @@ int b200_lm_set_exec_mask(b200_lm* h, const uint8_t* exec_mask_dev) {
 }
 
 int b200_lm_set_condition_sum(b200_lm* h, const void* sum_bf16_dev, int rows) {
-  B200_TRY(ensure_streaming(h, "lm_set_condition_sum"));
-  DeviceGuard g(h->device);
+  B200_STREAMING_ENTRY(h, "lm_set_condition_sum");
   const int on = sum_bf16_dev ? 1 : 0;
   if (on && rows != h->MB)      // lm.py:648-651: "cfg requires 2x more conditions"
     B200_FAIL(B200_ERR_SHAPE, "lm_set_condition_sum: %d rows given, the model runs on %d", rows, h->MB);
   if (on) B200_CUDA(cudaMemcpyAsync(h->cond_sum, sum_bf16_dev, (size_t)h->MB * h->cfg.dim * 2, cudaMemcpyDeviceToDevice, h->stream));
-  if (on != h->cond_on) drop_graph(h);
+  if (on != h->cond_on) h->graphs[0].drop();
   h->cond_on = on;
   return B200_OK;
 }
@@ -1292,8 +1217,7 @@ int b200_lm_set_cross_len(b200_lm* h, int keys) {
 }
 
 int b200_lm_set_condition_cross(b200_lm* h, const void* src_bf16_dev, const int32_t* rows_host, int n_rows) {
-  B200_TRY(ensure_streaming(h, "lm_set_condition_cross"));
-  DeviceGuard g(h->device);
+  B200_STREAMING_ENTRY(h, "lm_set_condition_cross");
   if (!h->cross_on) B200_FAIL(B200_ERR_INVALID, "lm_set_condition_cross: the model has no cross-attention layers");
   if (!src_bf16_dev || n_rows < 1 || n_rows > h->MB) B200_FAIL(B200_ERR_INVALID, "lm_set_condition_cross: %d condition rows", n_rows);
   if (!rows_host && n_rows != h->MB)       // lm.py:650-651: "cfg requires 2x more conditions"
@@ -1324,11 +1248,10 @@ int b200_lm_set_condition_cross(b200_lm* h, const void* src_bf16_dev, const int3
 }
 
 int b200_lm_set_taps(b200_lm* h, int enable) {
-  B200_TRY(ensure_streaming(h, "lm_set_taps"));
-  DeviceGuard g(h->device);
+  B200_STREAMING_ENTRY(h, "lm_set_taps");
   const int on = enable ? 1 : 0;
   if (on && !h->taps) B200_TRY(h->state.alloc_t(&h->taps, (size_t)tap_elems(h)));     // freed with the state at streaming_end
-  if (on != h->taps_on) drop_graph(h);
+  if (on != h->taps_on) h->graphs[0].drop();
   h->taps_on = on;
   return B200_OK;
 }
@@ -1366,8 +1289,7 @@ int b200_lm_set_kv_pool(b200_lm* h, int64_t frames, int page_slots) {
 }
 
 int b200_lm_kv_pool_usage(b200_lm* h, int* pages_used, int* pages_total) {
-  B200_TRY(ensure_streaming(h, "lm_kv_pool_usage"));
-  DeviceGuard g(h->device);
+  B200_STREAMING_ENTRY(h, "lm_kv_pool_usage");
   int top = 0;
   if (h->n_pages) {
     B200_CUDA(cudaMemcpyAsync(&top, h->free_top, 4, cudaMemcpyDeviceToHost, h->stream));
@@ -1379,8 +1301,7 @@ int b200_lm_kv_pool_usage(b200_lm* h, int* pages_used, int* pages_total) {
 }
 
 int b200_lm_session_bytes(b200_lm* h, int row, int64_t* nbytes) {
-  B200_TRY(ensure_streaming(h, "lm_session_bytes"));
-  DeviceGuard g(h->device);
+  B200_STREAMING_ENTRY(h, "lm_session_bytes");
   SessionPlan p;
   B200_TRY(session_plan(h, row, "lm_session_bytes", &p));
   if (nbytes) *nbytes = p.bytes;
@@ -1388,19 +1309,16 @@ int b200_lm_session_bytes(b200_lm* h, int row, int64_t* nbytes) {
 }
 
 int b200_lm_session_export(b200_lm* h, int row, void* dst_dev, int64_t capacity) {
-  B200_TRY(ensure_streaming(h, "lm_session_export"));
-  DeviceGuard g(h->device);
+  B200_STREAMING_ENTRY(h, "lm_session_export");
   SessionPlan p;
   B200_TRY(session_plan(h, row, "lm_session_export", &p));
   if (!dst_dev) B200_FAIL(B200_ERR_INVALID, "lm_session_export: null destination");
   if (capacity < p.bytes) B200_FAIL(B200_ERR_SHAPE, "lm_session_export: the record takes %lld bytes, capacity %lld", (long long)p.bytes, (long long)capacity);
-  SessionHeader s;
-  memset(&s, 0, sizeof(s));
-  s.magic = SESSION_MAGIC; s.version = SESSION_VERSION; s.kind = SESSION_LM; s.kv_dtype = (uint32_t)h->kv_fp8;
-  s.fingerprint = lm_fingerprint(h); s.rows = p.rows;
+  SessionHeader s = h->session_header(p.bytes);
+  s.kv_dtype = (uint32_t)h->kv_fp8; s.rows = p.rows;
   s.flags = (p.cond ? SESSION_COND : 0) | (h->cfg_until ? SESSION_CFG_UNTIL : 0) | (h->cross_on ? SESSION_CROSS : 0);
   if (h->cross_on) memcpy(s.reserved, &h->cross_len, sizeof(int32_t));
-  s.pos[0] = p.pos[0]; s.pos[1] = p.pos[1]; s.n = p.n; s.bytes = p.bytes;
+  s.pos[0] = p.pos[0]; s.pos[1] = p.pos[1]; s.n = p.n;
   char* rec = static_cast<char*>(dst_dev);
   B200_CUDA(cudaMemcpyAsync(rec, &s, sizeof(s), cudaMemcpyHostToDevice, h->stream));
   B200_TRY(row_slice_copy(h->slices_dev, p.cond ? h->n_slices_cond : h->n_slices, h->slices_max, rec, row, true, h->stream));
@@ -1410,19 +1328,11 @@ int b200_lm_session_export(b200_lm* h, int row, void* dst_dev, int64_t capacity)
 }
 
 int b200_lm_session_import(b200_lm* h, int row, const void* src_dev, int64_t nbytes) {
-  B200_TRY(ensure_streaming(h, "lm_session_import"));
-  DeviceGuard g(h->device);
+  B200_STREAMING_ENTRY(h, "lm_session_import");
   const auto& c = h->cfg;
-  if (row < 0 || row >= h->batch) B200_FAIL(B200_ERR_INVALID, "lm_session_import: row %d outside [0, %d)", row, h->batch);
-  if (!src_dev) B200_FAIL(B200_ERR_INVALID, "lm_session_import: null record");
-  if (nbytes < (int64_t)sizeof(SessionHeader)) B200_FAIL(B200_ERR_SHAPE, "lm_session_import: %lld bytes hold no record header", (long long)nbytes);
+  B200_TRY(h->check_row(row, "lm_session_import"));
   SessionHeader s;
-  B200_CUDA(cudaStreamSynchronize(h->stream));
-  B200_CUDA(cudaMemcpy(&s, src_dev, sizeof(s), cudaMemcpyDeviceToHost));
-  if (s.magic != SESSION_MAGIC || s.version != SESSION_VERSION)
-    B200_FAIL(B200_ERR_INVALID, "lm_session_import: not a session record (magic %08x, version %u)", s.magic, s.version);
-  if (s.kind != SESSION_LM) B200_FAIL(B200_ERR_INVALID, "lm_session_import: the record is not an LM session (kind %u)", s.kind);
-  if (s.fingerprint != lm_fingerprint(h)) B200_FAIL(B200_ERR_INVALID, "lm_session_import: the record was taken with another model configuration");
+  B200_TRY(h->read_session_header(src_dev, nbytes, "lm_session_import", &s));
   if (s.kv_dtype != (uint32_t)h->kv_fp8)
     B200_FAIL(B200_ERR_INVALID, "lm_session_import: the record's KV storage type %u differs from the handle's %d", s.kv_dtype, h->kv_fp8);
   SessionPlan p;
@@ -1462,8 +1372,7 @@ int b200_lm_session_import(b200_lm* h, int row, const void* src_dev, int64_t nby
 }
 
 int b200_lm_assume_fill(b200_lm* h, int fill) {
-  B200_TRY(ensure_streaming(h, "lm_assume_fill"));
-  DeviceGuard g(h->device);
+  B200_STREAMING_ENTRY(h, "lm_assume_fill");
   if (fill < 0) B200_FAIL(B200_ERR_INVALID, "lm_assume_fill: negative fill");
   std::vector<long long> v(h->MB, fill);
   if (h->n_pages) B200_TRY(pool_map(h, 0, 1, v, "lm_assume_fill"));
@@ -1477,14 +1386,8 @@ int b200_lm_assume_fill(b200_lm* h, int fill) {
 /* Synchronises the handle's stream and returns (and clears) the device error flags: B200_FLAG_TOKEN_RANGE = a token id outside
  * its embedding table reached the model (the reference would hit a device assert in F.embedding). */
 int b200_lm_error_flags(b200_lm* h, int* flags_out) {
-  B200_TRY(ensure_streaming(h, "lm_error_flags"));
-  DeviceGuard g(h->device);
-  int v = 0;
-  B200_CUDA(cudaMemcpyAsync(&v, h->err, 4, cudaMemcpyDeviceToHost, h->stream));
-  B200_CUDA(cudaStreamSynchronize(h->stream));
-  if (v) B200_CUDA(cudaMemsetAsync(h->err, 0, 4, h->stream));
-  if (flags_out) *flags_out = v;
-  return B200_OK;
+  B200_STREAMING_ENTRY(h, "lm_error_flags");
+  return h->error_flags(flags_out);
 }
 
 static int run_step(b200_lm* h, int n_in, int replace, int internal_noise) {
@@ -1492,39 +1395,10 @@ static int run_step(b200_lm* h, int n_in, int replace, int internal_noise) {
     h->n_in_static = n_in;
     h->replace_static = replace;
     h->noise_static = internal_noise;
-    drop_graph(h);
+    h->graphs[0].drop();
   }
   B200_TRY(tc::linear_prepare());
-  if (!h->graph_enabled) {
-    h->body = h->stream;
-    return step_body(h);
-  }
-  // the step runs on the private stream, fenced against the caller's stream on both sides
-  B200_CUDA(cudaEventRecord(h->ev_in, h->stream));
-  B200_CUDA(cudaStreamWaitEvent(h->gstream, h->ev_in, 0));
-  if (!h->graph_exec) {
-    cudaGraph_t graph = nullptr;
-    const int64_t before = g_launches.load();
-    h->body = h->gstream;
-    B200_CUDA(cudaStreamBeginCapture(h->gstream, cudaStreamCaptureModeRelaxed));
-    const int rc = step_body(h);
-    cudaError_t e = cudaStreamEndCapture(h->gstream, &graph);
-    h->graph_kernels = g_launches.load() - before;
-    g_launches.fetch_sub(h->graph_kernels);      // recorded, not executed
-    if (rc != B200_OK) {
-      if (graph) cudaGraphDestroy(graph);
-      return rc;
-    }
-    if (e != cudaSuccess) B200_FAIL(B200_ERR_CUDA, "graph capture of the LM step failed: %s", cudaGetErrorString(e));
-    e = cudaGraphInstantiate(&h->graph_exec, graph, 0);
-    cudaGraphDestroy(graph);
-    if (e != cudaSuccess) B200_FAIL(B200_ERR_CUDA, "graph instantiate failed: %s", cudaGetErrorString(e));
-  }
-  B200_CUDA(cudaGraphLaunch(h->graph_exec, h->gstream));
-  g_launches.fetch_add(h->graph_kernels);
-  B200_CUDA(cudaEventRecord(h->ev_out, h->gstream));
-  B200_CUDA(cudaStreamWaitEvent(h->stream, h->ev_out, 0));
-  return B200_OK;
+  return h->run(h->graphs[0], "the LM step", [h] { return step_body(h); });
 }
 
 static bool sampling_on(const b200_lm* h) { return h->use_sampling && (h->temp > 0.f || h->temp_text > 0.f); }
@@ -1536,8 +1410,7 @@ int b200_lm_step(b200_lm* h, const int64_t* in_codes_dev, int n_in, const float*
 
 int b200_lm_step_ex(b200_lm* h, const int64_t* in_codes_dev, int n_in, const float* noise_dev, const int64_t* replace_audio_dev,
                     int64_t* out_tokens_dev, int support_out_of_sync, int* ready_host) {
-  B200_TRY(ensure_streaming(h, "lm_step"));
-  DeviceGuard g(h->device);
+  B200_STREAMING_ENTRY(h, "lm_step");
   const auto& c = h->cfg;
   const int B = h->batch, needed = c.n_q - c.dep_q;
   if (!in_codes_dev || !out_tokens_dev) B200_FAIL(B200_ERR_SHAPE, "lm_step: null buffers");
@@ -1559,8 +1432,7 @@ int b200_lm_step_ex(b200_lm* h, const int64_t* in_codes_dev, int n_in, const flo
 
 int b200_lm_step_host(b200_lm* h, const int64_t* in_codes_host, int n_in, const float* noise_host,
                       int64_t* out_tokens_host, int support_out_of_sync, int* ready_host) {
-  B200_TRY(ensure_streaming(h, "lm_step_host"));
-  DeviceGuard g(h->device);
+  B200_STREAMING_ENTRY(h, "lm_step_host");
   const auto& c = h->cfg;
   const int B = h->batch, needed = c.n_q - c.dep_q;
   if (!in_codes_host || !out_tokens_host) B200_FAIL(B200_ERR_SHAPE, "lm_step_host: null buffers");
@@ -1591,8 +1463,7 @@ int b200_lm_step_host(b200_lm* h, const int64_t* in_codes_host, int n_in, const 
 }
 
 int b200_lm_read_buffer(b200_lm* h, const char* name, void* dst_dev, int64_t capacity_bytes, int64_t* nbytes) {
-  B200_TRY(ensure_streaming(h, "lm_read_buffer"));
-  DeviceGuard g(h->device);
+  B200_STREAMING_ENTRY(h, "lm_read_buffer");
   const auto& c = h->cfg;
   const std::string n = name ? name : "";
   const int B = h->batch, MB = h->MB;
@@ -1648,11 +1519,7 @@ int b200_lm_read_buffer(b200_lm* h, const char* name, void* dst_dev, int64_t cap
     sz = elems * 2;
   }
   else B200_FAIL(B200_ERR_INVALID, "lm_read_buffer: unknown buffer '%s'", n.c_str());
-  if (nbytes) *nbytes = sz;
-  if (!dst_dev) return B200_OK;
-  if (capacity_bytes < sz) B200_FAIL(B200_ERR_SHAPE, "lm_read_buffer: destination too small");
-  if (sz > 0) B200_CUDA(cudaMemcpyAsync(dst_dev, src, (size_t)sz, cudaMemcpyDeviceToDevice, h->stream));
-  return B200_OK;
+  return copy_out(src, sz, sz, dst_dev, capacity_bytes, nbytes, h->stream, "lm_read_buffer");
 }
 
 int64_t b200_lm_algorithmic_bytes(b200_lm* h, int kv_fill) {

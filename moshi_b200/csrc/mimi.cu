@@ -64,15 +64,11 @@ struct DownLayer {             // ConvDownsample1d (resample.py:14-65): k = 2 * 
 
 }  // namespace
 
-struct b200_mimi {
+struct b200_mimi : StreamCore {     // graphs[ENC_GRAPH] / graphs[DEC_GRAPH]: one frame's encode / decode
   b200_mimi_config cfg;
   TensorStore store;
-  Arena weights, state;
-  bool finalized = false;
-  int device = -1;
-  int batch = 0;
+  Arena weights;
   int num_codebooks = 8;
-  cudaStream_t stream = nullptr;
   int frame_size = 0, hop = 0, rs = 0;       // rs = resample stride (2)
   int sms = 148;
 
@@ -92,26 +88,18 @@ struct b200_mimi {
         *tr_ao_lo = nullptr, *tr_h_hi = nullptr, *tr_h_lo = nullptr;
   uint8_t* exec_mask = nullptr;
   TmCommit *enc_tm = nullptr, *dec_tm = nullptr; int n_enc_tm = 0, n_dec_tm = 0; long long max_enc_tm = 0, max_dec_tm = 0;
-  long long* scratch_codes = nullptr;          // [B][K][1] for the host variants
-  float* rvq_res[2] = {nullptr, nullptr};      // RVQ workspace: residuals, per-chunk partial argmin
+  float* rvq_res[2] = {nullptr, nullptr};      // RVQ workspace for B queries: residuals, per-chunk partial argmin
   float* rvq_best[2] = {nullptr, nullptr};
   int* rvq_idx[2] = {nullptr, nullptr};
-  int rvq_cap = 0;
   float* splitk_ws = nullptr;                            // split-K partial sums of the deep / skinny layers
-  int* err = nullptr;                                     // device error flags (B200_FLAG_CODE_RANGE)
   // one-frame encode / decode as CUDA graphs over static buffers (frame in enc[0].ext -> enc_codes, dec_codes -> out_frame)
-  cudaStream_t body = nullptr;                 // stream the kernels are being enqueued on (caller's, or gstream in capture)
-  cudaStream_t gstream = nullptr;
-  cudaEvent_t ev_in = nullptr, ev_out = nullptr;
-  cudaGraphExec_t enc_graph = nullptr, dec_graph = nullptr;
-  int64_t enc_graph_kernels = 0, dec_graph_kernels = 0;
   int dec_graph_ncb = 0;
-  int graph_enabled = 1;
   long long *enc_codes = nullptr, *dec_codes = nullptr;   // [B][K], [B][q_n_q]
   float* out_frame = nullptr;                              // [B][frame_size]
+  // staging of the host variants: pinned and device buffers of pin_pcm_n samples and pin_codes_n codes, grown on demand
+  Arena staging;
   float *pin_pcm = nullptr; long long* pin_codes = nullptr; size_t pin_pcm_n = 0, pin_codes_n = 0;
-  float* dev_pcm = nullptr; long long* dev_codes = nullptr; size_t dev_pcm_n = 0, dev_codes_n = 0;
-  float* tap_scratch = nullptr; size_t tap_scratch_n = 0;
+  float* dev_pcm = nullptr; long long* dev_codes = nullptr;
   std::map<std::string, Tap> taps;
   int64_t weight_bytes = 0;
   // session records: the [B]-leading slice of every marked state entry, in marking order
@@ -121,6 +109,8 @@ struct b200_mimi {
 };
 
 namespace {
+
+enum { ENC_GRAPH, DEC_GRAPH };
 
 // ---------------------------------------------------------------------------------------------
 // structure (seanet.py:170-236, 323-388; resample.py; loaders.py:38-88)
@@ -236,8 +226,6 @@ int get_f32(b200_mimi* h, const std::string& name, std::vector<int64_t> shape, c
   return B200_OK;
 }
 
-struct ScratchFree { void* p = nullptr; ~ScratchFree() { if (p) cudaFree(p); } };
-
 // nn.Linear-shaped weight [N][n_taps * Cin] (fp32, device) -> packed hi / lo tiles owned by the handle
 int pack_tc(b200_mimi* h, mtc::TcLayer& L, const float* w_ntc, int N, int Cin, int n_taps) {
   if (Cin % mtc::TC_KB || N % 16 || (N > mtc::TC_MAX_NT && N % mtc::TC_MAX_NT))
@@ -271,9 +259,9 @@ int pack_sea(b200_mimi* h, SeaLayer& l) {
     B200_LAUNCH(tm_weight_conv_kernel, (unsigned)ceil_div64(n, 256), 256, 0, 0, w, l.w_simt, 1, l.cin, l.k);
     h->weight_bytes += n * 4;
   } else {
-    ScratchFree tmp;
-    B200_CUDA(cudaMalloc(&tmp.p, (size_t)n * 4));
-    float* wk = static_cast<float*>(tmp.p);
+    Arena tmp;
+    float* wk = nullptr;
+    B200_TRY(tmp.alloc_t(&wk, (size_t)n, false));
     if (l.kind == 0) B200_LAUNCH(tm_weight_conv_kernel, (unsigned)ceil_div64(n, 256), 256, 0, 0, w, wk, l.cout, l.cin, l.k);
     else B200_LAUNCH(tm_weight_convtr_kernel, (unsigned)ceil_div64(n, 256), 256, 0, 0, w, wk, l.cin, l.cout, l.stride);
     B200_TRY(pack_tc(h, l.tc, wk, l.N, l.cin, l.kind == 0 ? l.k : 2));
@@ -510,36 +498,17 @@ int load_frame(b200_mimi* h, const float* pcm, int n_frames, int f) {
   return B200_OK;
 }
 
-// RVQ workspace (residuals + per-chunk partial argmin); sized at streaming_begin for Q = batch and
-// grown only by the multi-frame `quantize` entry point.
-int ensure_rvq_workspace(b200_mimi* h, int Q) {
-  if (Q <= h->rvq_cap) return B200_OK;
-  const int Dq = h->cfg.q_dimension, n_chunks = ceil_div(h->cfg.q_bins, RVQ_CHUNK);
-  if (h->stream) B200_CUDA(cudaStreamSynchronize(h->stream));
-  for (int w = 0; w < 2; ++w) {
-    if (h->rvq_res[w]) cudaFree(h->rvq_res[w]);
-    if (h->rvq_best[w]) cudaFree(h->rvq_best[w]);
-    if (h->rvq_idx[w]) cudaFree(h->rvq_idx[w]);
-    B200_CUDA(cudaMalloc(&h->rvq_res[w], (size_t)Q * Dq * 4));
-    B200_CUDA(cudaMalloc(&h->rvq_best[w], (size_t)Q * n_chunks * 4));
-    B200_CUDA(cudaMalloc(&h->rvq_idx[w], (size_t)Q * n_chunks * 4));
-  }
-  h->rvq_cap = Q;
-  return B200_OK;
-}
-
-int quantize_cols(b200_mimi* h, const float* lat, long long lb, long long lc, long long lt, int n_cols,
-                  long long* codes, long long cs_b, long long cs_k, long long cs_f) {
+// One frame's latent [B][C] (row b at lat + b * lb, channel c at + c * lc) -> codes[b * cs_b + k * cs_k], B queries.
+int quantize_frame(b200_mimi* h, const float* lat, long long lb, long long lc, long long* codes, long long cs_b, long long cs_k) {
   const auto& c = h->cfg;
-  const int Q = h->batch * n_cols, Dq = c.q_dimension, bins = c.q_bins;
+  const int Q = h->batch, Dq = c.q_dimension, bins = c.q_bins;
   const int n_chunks = ceil_div(bins, RVQ_CHUNK);
-  B200_TRY(ensure_rvq_workspace(h, Q));
   int levels[2];
   levels[0] = c.q_n_semantic < h->num_codebooks ? c.q_n_semantic : h->num_codebooks;
   levels[1] = h->num_codebooks - levels[0];
   {
     dim3 grid(ceil_div(Q, RVQ_PQ), 2, ceil_div(Dq, 64));
-    B200_LAUNCH(rvq_project_kernel, grid, 256, (size_t)(RVQ_PQ * c.dimension + 4 * RVQ_PQ * 64) * 4, h->body, lat, lb, lc, lt, n_cols, Q,
+    B200_LAUNCH(rvq_project_kernel, grid, 256, (size_t)(RVQ_PQ * c.dimension + 4 * RVQ_PQ * 64) * 4, h->body, lat, lb, lc, 1LL, 1, Q,
                 h->wT[0], h->wT[1], h->rvq_res[0], h->rvq_res[1], c.dimension, Dq);
   }
   const int max_levels = levels[0] > levels[1] ? levels[0] : levels[1];
@@ -553,8 +522,8 @@ int quantize_cols(b200_mimi* h, const float* lat, long long lb, long long lc, lo
       a.active[w] = level < levels[w];
       a.code_index[w] = (w == 0 ? 0 : levels[0]) + level;
     }
-    a.codes = codes; a.cs_b = cs_b; a.cs_k = cs_k; a.cs_f = cs_f;
-    a.n_query = Q; a.n_frames = n_cols; a.Dq = Dq; a.bins = bins; a.n_chunks = n_chunks;
+    a.codes = codes; a.cs_b = cs_b; a.cs_k = cs_k; a.cs_f = 1;
+    a.n_query = Q; a.n_frames = 1; a.Dq = Dq; a.bins = bins; a.n_chunks = n_chunks;
     dim3 g1(n_chunks, ceil_div(Q, RVQ_QT), 2);
     B200_LAUNCH(rvq_search_kernel, g1, RVQ_CHUNK, (size_t)RVQ_QT * Dq * 4, h->body, a);
     dim3 g2(Q, 2);
@@ -595,55 +564,6 @@ int decode_latent_body(b200_mimi* h) {
   return B200_OK;
 }
 
-void drop_graphs(b200_mimi* h) {
-  if (h->enc_graph) cudaGraphExecDestroy(h->enc_graph);
-  if (h->dec_graph) cudaGraphExecDestroy(h->dec_graph);
-  h->enc_graph = h->dec_graph = nullptr;
-}
-
-// Runs `body` (a fixed launch sequence over static buffers) as one CUDA graph on the private stream, fenced against
-// the caller's stream on both sides; the first call captures it.  With graphs disabled the body runs eagerly.
-template <class F>
-int run_captured(b200_mimi* h, cudaGraphExec_t* exec, int64_t* n_kernels, F body) {
-  if (!h->graph_enabled) {
-    h->body = h->stream;
-    return body();
-  }
-  B200_CUDA(cudaEventRecord(h->ev_in, h->stream));
-  B200_CUDA(cudaStreamWaitEvent(h->gstream, h->ev_in, 0));
-  if (!*exec) {
-    cudaGraph_t graph = nullptr;
-    const int64_t before = g_launches.load();
-    h->body = h->gstream;
-    B200_CUDA(cudaStreamBeginCapture(h->gstream, cudaStreamCaptureModeRelaxed));
-    const int rc = body();
-    cudaError_t e = cudaStreamEndCapture(h->gstream, &graph);
-    *n_kernels = g_launches.load() - before;
-    g_launches.fetch_sub(*n_kernels);      // recorded, not executed
-    h->body = h->stream;
-    if (rc != B200_OK) {
-      if (graph) cudaGraphDestroy(graph);
-      return rc;
-    }
-    if (e != cudaSuccess) B200_FAIL(B200_ERR_CUDA, "graph capture of a Mimi frame failed: %s", cudaGetErrorString(e));
-    e = cudaGraphInstantiate(exec, graph, 0);
-    cudaGraphDestroy(graph);
-    if (e != cudaSuccess) B200_FAIL(B200_ERR_CUDA, "graph instantiate failed: %s", cudaGetErrorString(e));
-  }
-  B200_CUDA(cudaGraphLaunch(*exec, h->gstream));
-  g_launches.fetch_add(*n_kernels);
-  B200_CUDA(cudaEventRecord(h->ev_out, h->gstream));
-  B200_CUDA(cudaStreamWaitEvent(h->stream, h->ev_out, 0));
-  return B200_OK;
-}
-
-int ensure_streaming(b200_mimi* h, const char* what) {
-  if (!h) B200_FAIL(B200_ERR_INVALID, "%s: null handle", what);
-  if (!h->finalized) B200_FAIL(B200_ERR_STATE, "%s: handle not finalized", what);
-  if (h->batch <= 0) B200_FAIL(B200_ERR_STATE, "%s: not streaming (call streaming_begin first)", what);
-  return B200_OK;
-}
-
 void register_tap(b200_mimi* h, const std::string& name, const float* p, int C, int T, bool transpose) { h->taps[name] = Tap{p, C, T, transpose}; }
 
 // Plans one tensor-core layer for B sessions of T GEMM rows: A maps over `in_hi / in_lo` ([B][rows][Cin]), epilogue pointers set
@@ -662,7 +582,7 @@ int plan_layer(b200_mimi* h, mtc::TcLayer& L, const float* in_hi, const float* i
 }  // namespace
 
 int b200::mimi_frame_view(b200_mimi* h, MimiFrameView* v) {
-  B200_TRY(ensure_streaming(h, "mimi_frame_view"));
+  B200_TRY(check_streaming(h, "mimi_frame_view"));
   *v = MimiFrameView{h->batch, h->num_codebooks, h->frame_size};
   return B200_OK;
 }
@@ -684,6 +604,8 @@ int b200_mimi_create(const b200_mimi_config* cfg, b200_mimi** out) {
   b200_mimi* h = new b200_mimi();
   h->cfg = *cfg;
   cudaGetDevice(&h->device);
+  h->session_kind = SESSION_MIMI;
+  h->fingerprint = config_fingerprint(&h->cfg, sizeof(h->cfg));
   h->num_codebooks = cfg->num_codebooks;
   h->hop = 1;
   for (int i = 0; i < cfg->n_ratios; ++i) h->hop *= cfg->ratios[i];
@@ -736,16 +658,6 @@ int b200_mimi_destroy(b200_mimi* h) {
   b200_mimi_streaming_end(h);
   h->store.release_all();
   h->weights.free_all();
-  if (h->pin_pcm) cudaFreeHost(h->pin_pcm);
-  if (h->pin_codes) cudaFreeHost(h->pin_codes);
-  if (h->dev_pcm) cudaFree(h->dev_pcm);
-  if (h->dev_codes) cudaFree(h->dev_codes);
-  if (h->tap_scratch) cudaFree(h->tap_scratch);
-  for (int w = 0; w < 2; ++w) {
-    if (h->rvq_res[w]) cudaFree(h->rvq_res[w]);
-    if (h->rvq_best[w]) cudaFree(h->rvq_best[w]);
-    if (h->rvq_idx[w]) cudaFree(h->rvq_idx[w]);
-  }
   delete h;
   return B200_OK;
 }
@@ -755,23 +667,20 @@ int b200_mimi_set_num_codebooks(b200_mimi* h, int n) {
   if (n < h->cfg.q_n_semantic || n > h->cfg.q_n_q)   // vq.py:315-317 assertion
     B200_FAIL(B200_ERR_SHAPE, "set_num_codebooks(%d): must be in [%d, %d]", n, h->cfg.q_n_semantic, h->cfg.q_n_q);
   h->num_codebooks = n;
-  if (h->enc_graph) { cudaGraphExecDestroy(h->enc_graph); h->enc_graph = nullptr; }
+  h->graphs[ENC_GRAPH].drop();
   return B200_OK;
 }
 
 int b200_mimi_streaming_begin(b200_mimi* h, int batch, void* stream) {
-  if (!h || !h->finalized) B200_FAIL(B200_ERR_STATE, "streaming_begin: handle not finalized");
-  if (h->batch > 0) B200_FAIL(B200_ERR_STATE, "streaming_begin: already streaming");   // streaming.py:112
-  if (batch < 1) B200_FAIL(B200_ERR_INVALID, "streaming_begin: batch %d", batch);
+  B200_TRY(check_begin(h, batch, "streaming_begin"));
   DeviceGuard guard_dev(h->device);
   const auto& c = h->cfg;
   const int B = batch, d = c.dimension;
   h->stream = static_cast<cudaStream_t>(stream);
   h->taps.clear();
   Arena& A = h->state;
-  struct Cleanup { b200_mimi* h; bool armed = true; ~Cleanup() { if (armed) h->state.free_all(); } } cleanup{h};
-  h->batch = B;                              // plan_layer reads it (reset below on failure paths by the caller's streaming_end)
-  struct BatchReset { b200_mimi* h; bool armed = true; ~BatchReset() { if (armed) h->batch = 0; } } batch_reset{h};
+  struct Cleanup { b200_mimi* h; bool armed = true; ~Cleanup() { if (armed) b200_mimi_streaming_end(h); } } cleanup{h};
+  h->batch = B;                              // plan_layer reads it
   B200_TRY(A.alloc_t(&h->exec_mask, B, false));
   B200_CUDA(cudaMemset(h->exec_mask, 1, B));
   B200_TRY(A.alloc_t(&h->err, 1));
@@ -931,12 +840,9 @@ int b200_mimi_streaming_begin(b200_mimi* h, int batch, void* stream) {
       B200_TRY(plan_layer(h, L.l2, h->tr_h_hi, h->tr_h_lo, T, 0, T));
     }
   }
-  B200_TRY(A.alloc_t(&h->scratch_codes, (size_t)B * c.q_n_q));
   B200_TRY(A.alloc_t(&h->enc_codes, (size_t)B * c.q_n_q));
   B200_TRY(A.alloc_t(&h->dec_codes, (size_t)B * c.q_n_q));
-  B200_CUDA(cudaStreamCreateWithFlags(&h->gstream, cudaStreamNonBlocking));
-  B200_CUDA(cudaEventCreateWithFlags(&h->ev_in, cudaEventDisableTiming));
-  B200_CUDA(cudaEventCreateWithFlags(&h->ev_out, cudaEventDisableTiming));
+  B200_TRY(h->open_streams());
   h->body = h->stream;
   // what a streaming-state snapshot holds (streaming.py:158-181): masks, carried conv rows (the transposed convs' carry is
   // their previous input step), both transformers' KV rings and offsets
@@ -973,35 +879,29 @@ int b200_mimi_streaming_begin(b200_mimi* h, int batch, void* stream) {
     B200_TRY(A.alloc_t(&h->slices_dev, s.size(), false));
     B200_CUDA(cudaMemcpy(h->slices_dev, s.data(), s.size() * sizeof(RowSlice), cudaMemcpyHostToDevice));
   }
-  B200_TRY(ensure_rvq_workspace(h, B));
+  {
+    const int n_chunks = ceil_div(c.q_bins, RVQ_CHUNK);
+    for (int w = 0; w < 2; ++w) {
+      B200_TRY(A.alloc_t(&h->rvq_res[w], (size_t)B * c.q_dimension, false));
+      B200_TRY(A.alloc_t(&h->rvq_best[w], (size_t)B * n_chunks, false));
+      B200_TRY(A.alloc_t(&h->rvq_idx[w], (size_t)B * n_chunks, false));
+    }
+  }
   B200_CUDA(cudaDeviceSynchronize());
   cleanup.armed = false;
-  batch_reset.armed = false;
   return B200_OK;
 }
 
 int b200_mimi_streaming_end(b200_mimi* h) {
   if (!h) return B200_OK;
   DeviceGuard g(h->device);
-  if (h->batch > 0) {
-    cudaStreamSynchronize(h->stream);
-    if (h->gstream) cudaStreamSynchronize(h->gstream);
-  }
-  drop_graphs(h);
-  if (h->gstream) cudaStreamDestroy(h->gstream);
-  if (h->ev_in) cudaEventDestroy(h->ev_in);
-  if (h->ev_out) cudaEventDestroy(h->ev_out);
-  h->gstream = nullptr; h->ev_in = h->ev_out = nullptr;
-  h->state.free_all();
-  h->err = nullptr;
-  h->batch = 0;
+  h->end_streaming();
   h->taps.clear();
   return B200_OK;
 }
 
 int b200_mimi_reset(b200_mimi* h, const uint8_t* reset_mask_dev) {
-  B200_TRY(ensure_streaming(h, "mimi_reset"));
-  DeviceGuard g(h->device);
+  B200_STREAMING_ENTRY(h, "mimi_reset");
   const int B = h->batch;
   auto zero = [&](float* buf, long long per_row) {
     if (!buf || per_row <= 0) return;
@@ -1021,15 +921,14 @@ int b200_mimi_reset(b200_mimi* h, const uint8_t* reset_mask_dev) {
 }
 
 int b200_mimi_set_exec_mask(b200_mimi* h, const uint8_t* exec_mask_dev) {
-  B200_TRY(ensure_streaming(h, "mimi_set_exec_mask"));
-  DeviceGuard g(h->device);
+  B200_STREAMING_ENTRY(h, "mimi_set_exec_mask");
   if (!exec_mask_dev) B200_FAIL(B200_ERR_INVALID, "mimi_set_exec_mask: null mask");
   B200_CUDA(cudaMemcpyAsync(h->exec_mask, exec_mask_dev, h->batch, cudaMemcpyDeviceToDevice, h->stream));
   return B200_OK;
 }
 
 int b200_mimi_encode_to_latent(b200_mimi* h, const float* pcm_dev, int n_frames, float* latent_dev) {
-  B200_TRY(ensure_streaming(h, "mimi_encode_to_latent"));
+  B200_STREAMING_ENTRY(h, "mimi_encode_to_latent");
   if (!pcm_dev || !latent_dev || n_frames < 1) B200_FAIL(B200_ERR_SHAPE, "mimi_encode_to_latent: bad arguments");
   const int d = h->cfg.dimension;
   for (int f = 0; f < n_frames; ++f) {
@@ -1043,23 +942,25 @@ int b200_mimi_encode_to_latent(b200_mimi* h, const float* pcm_dev, int n_frames,
 }
 
 int b200_mimi_quantize(b200_mimi* h, const float* latent_dev, int n_frames, int64_t* codes_dev) {
-  B200_TRY(ensure_streaming(h, "mimi_quantize"));
+  B200_STREAMING_ENTRY(h, "mimi_quantize");
   if (!latent_dev || !codes_dev || n_frames < 1) B200_FAIL(B200_ERR_SHAPE, "mimi_quantize: bad arguments");
   const int d = h->cfg.dimension, K = h->num_codebooks;
   h->body = h->stream;
-  return quantize_cols(h, latent_dev, (long long)d * n_frames, n_frames, 1, n_frames,
-                       reinterpret_cast<long long*>(codes_dev), (long long)K * n_frames, n_frames, 1);
+  for (int f = 0; f < n_frames; ++f)       // latent [B][C][n_frames] -> codes [B][K][n_frames], the pass encode runs per frame
+    B200_TRY(quantize_frame(h, latent_dev + f, (long long)d * n_frames, n_frames, reinterpret_cast<long long*>(codes_dev) + f,
+                            (long long)K * n_frames, n_frames));
+  return B200_OK;
 }
 
 int b200_mimi_encode(b200_mimi* h, const float* pcm_dev, int n_frames, int64_t* codes_dev) {
-  B200_TRY(ensure_streaming(h, "mimi_encode"));
+  B200_STREAMING_ENTRY(h, "mimi_encode");
   if (!pcm_dev || !codes_dev || n_frames < 1) B200_FAIL(B200_ERR_SHAPE, "mimi_encode: bad arguments");
   const int d = h->cfg.dimension, K = h->num_codebooks;
   for (int f = 0; f < n_frames; ++f) {
     B200_TRY(load_frame(h, pcm_dev, n_frames, f));
-    B200_TRY(run_captured(h, &h->enc_graph, &h->enc_graph_kernels, [&]() -> int {
+    B200_TRY(h->run(h->graphs[ENC_GRAPH], "a Mimi frame", [&]() -> int {
       B200_TRY(encode_body(h));
-      return quantize_cols(h, h->latent, d, 1, 1, 1, h->enc_codes, K, 1, 1);
+      return quantize_frame(h, h->latent, d, 1, h->enc_codes, K, 1);
     }));
     // enc_codes [B][K] -> codes[b][k][f]
     B200_CUDA(cudaMemcpy2DAsync(reinterpret_cast<long long*>(codes_dev) + f, (size_t)n_frames * 8, h->enc_codes, 8, 8,
@@ -1069,7 +970,7 @@ int b200_mimi_encode(b200_mimi* h, const float* pcm_dev, int n_frames, int64_t* 
 }
 
 int b200_mimi_decode_latent(b200_mimi* h, const int64_t* codes_dev, int n_codebooks, int n_frames, float* latent_dev) {
-  B200_TRY(ensure_streaming(h, "mimi_decode_latent"));
+  B200_STREAMING_ENTRY(h, "mimi_decode_latent");
   if (!codes_dev || !latent_dev || n_frames < 1) B200_FAIL(B200_ERR_SHAPE, "mimi_decode_latent: bad arguments");
   const int d = h->cfg.dimension;
   h->body = h->stream;
@@ -1078,20 +979,17 @@ int b200_mimi_decode_latent(b200_mimi* h, const int64_t* codes_dev, int n_codebo
 }
 
 int b200_mimi_decode(b200_mimi* h, const int64_t* codes_dev, int n_codebooks, int n_frames, float* pcm_dev) {
-  B200_TRY(ensure_streaming(h, "mimi_decode"));
+  B200_STREAMING_ENTRY(h, "mimi_decode");
   if (!codes_dev || !pcm_dev || n_frames < 1) B200_FAIL(B200_ERR_SHAPE, "mimi_decode: bad arguments");
   if (n_codebooks < 1 || n_codebooks > h->cfg.q_n_q) B200_FAIL(B200_ERR_SHAPE, "decode: %d codebooks", n_codebooks);
   const int d = h->cfg.dimension, fs = h->frame_size;
-  if (h->dec_graph && h->dec_graph_ncb != n_codebooks) {
-    cudaGraphExecDestroy(h->dec_graph);
-    h->dec_graph = nullptr;
-  }
+  if (h->dec_graph_ncb != n_codebooks) h->graphs[DEC_GRAPH].drop();
   h->dec_graph_ncb = n_codebooks;
   for (int f = 0; f < n_frames; ++f) {
     // codes[b][k][f] -> dec_codes [B][n_codebooks]
     B200_CUDA(cudaMemcpy2DAsync(h->dec_codes, 8, reinterpret_cast<const long long*>(codes_dev) + f, (size_t)n_frames * 8, 8,
                                 (size_t)h->batch * n_codebooks, cudaMemcpyDeviceToDevice, h->stream));
-    B200_TRY(run_captured(h, &h->dec_graph, &h->dec_graph_kernels, [&]() -> int {
+    B200_TRY(h->run(h->graphs[DEC_GRAPH], "a Mimi frame", [&]() -> int {
       B200_TRY(dequantize_cols(h, h->dec_codes, n_codebooks, 1, 1, n_codebooks, 1, h->latent_q, d, 1, 1));
       return decode_latent_body(h);
     }));
@@ -1105,38 +1003,31 @@ int b200_mimi_decode(b200_mimi* h, const int64_t* codes_dev, int n_codebooks, in
 int64_t b200_mimi_state_bytes(b200_mimi* h) { return (h && h->batch > 0) ? (int64_t)h->state.state_bytes() : 0; }
 
 int b200_mimi_get_state(b200_mimi* h, void* dst_dev, int64_t capacity) {
-  B200_TRY(ensure_streaming(h, "mimi_get_state"));
-  if (!dst_dev || capacity < (int64_t)h->state.state_bytes()) B200_FAIL(B200_ERR_SHAPE, "mimi_get_state: destination too small");
-  return h->state.save(dst_dev, h->stream);
+  B200_STREAMING_ENTRY(h, "mimi_get_state");
+  return h->save_state(dst_dev, capacity, 0, "mimi_get_state");
 }
 
 int b200_mimi_set_state(b200_mimi* h, const void* src_dev, int64_t nbytes) {
-  B200_TRY(ensure_streaming(h, "mimi_set_state"));
-  if (!src_dev || nbytes != (int64_t)h->state.state_bytes())
-    B200_FAIL(B200_ERR_SHAPE, "mimi_set_state: snapshot of %lld bytes does not fit this session layout (%lld)",
-              (long long)nbytes, (long long)h->state.state_bytes());
-  return h->state.load(src_dev, h->stream);
+  B200_STREAMING_ENTRY(h, "mimi_set_state");
+  B200_TRY(h->check_blob(src_dev, nbytes, 0, "mimi_set_state"));
+  return h->load_state(src_dev);
 }
 
 /* One session as a record: the 256-byte SessionHeader, then row `row` of every marked state entry in marking order, each
  * 16-byte aligned.  The size depends on the configuration only. */
 int b200_mimi_session_bytes(b200_mimi* h, int64_t* nbytes) {
-  B200_TRY(ensure_streaming(h, "mimi_session_bytes"));
+  B200_TRY(check_streaming(h, "mimi_session_bytes"));
   if (nbytes) *nbytes = h->session_bytes;
   return B200_OK;
 }
 
 int b200_mimi_session_export(b200_mimi* h, int row, void* dst_dev, int64_t capacity) {
-  B200_TRY(ensure_streaming(h, "mimi_session_export"));
-  DeviceGuard g(h->device);
-  if (row < 0 || row >= h->batch) B200_FAIL(B200_ERR_INVALID, "mimi_session_export: row %d outside [0, %d)", row, h->batch);
+  B200_STREAMING_ENTRY(h, "mimi_session_export");
+  B200_TRY(h->check_row(row, "mimi_session_export"));
   if (!dst_dev) B200_FAIL(B200_ERR_INVALID, "mimi_session_export: null destination");
   if (capacity < h->session_bytes)
     B200_FAIL(B200_ERR_SHAPE, "mimi_session_export: the record takes %lld bytes, capacity %lld", h->session_bytes, (long long)capacity);
-  SessionHeader s;
-  memset(&s, 0, sizeof(s));
-  s.magic = SESSION_MAGIC; s.version = SESSION_VERSION; s.kind = SESSION_MIMI;
-  s.fingerprint = config_fingerprint(&h->cfg, sizeof(h->cfg)); s.rows = 1; s.bytes = h->session_bytes;
+  const SessionHeader s = h->session_header(h->session_bytes);
   char* rec = static_cast<char*>(dst_dev);
   B200_CUDA(cudaMemcpyAsync(rec, &s, sizeof(s), cudaMemcpyHostToDevice, h->stream));
   B200_TRY(row_slice_copy(h->slices_dev, h->n_slices, h->slices_max, rec, row, true, h->stream));
@@ -1145,19 +1036,10 @@ int b200_mimi_session_export(b200_mimi* h, int row, void* dst_dev, int64_t capac
 }
 
 int b200_mimi_session_import(b200_mimi* h, int row, const void* src_dev, int64_t nbytes) {
-  B200_TRY(ensure_streaming(h, "mimi_session_import"));
-  DeviceGuard g(h->device);
-  if (row < 0 || row >= h->batch) B200_FAIL(B200_ERR_INVALID, "mimi_session_import: row %d outside [0, %d)", row, h->batch);
-  if (!src_dev) B200_FAIL(B200_ERR_INVALID, "mimi_session_import: null record");
-  if (nbytes < (int64_t)sizeof(SessionHeader)) B200_FAIL(B200_ERR_SHAPE, "mimi_session_import: %lld bytes hold no record header", (long long)nbytes);
+  B200_STREAMING_ENTRY(h, "mimi_session_import");
+  B200_TRY(h->check_row(row, "mimi_session_import"));
   SessionHeader s;
-  B200_CUDA(cudaStreamSynchronize(h->stream));
-  B200_CUDA(cudaMemcpy(&s, src_dev, sizeof(s), cudaMemcpyDeviceToHost));
-  if (s.magic != SESSION_MAGIC || s.version != SESSION_VERSION)
-    B200_FAIL(B200_ERR_INVALID, "mimi_session_import: not a session record (magic %08x, version %u)", s.magic, s.version);
-  if (s.kind != SESSION_MIMI) B200_FAIL(B200_ERR_INVALID, "mimi_session_import: the record is not a Mimi session (kind %u)", s.kind);
-  if (s.fingerprint != config_fingerprint(&h->cfg, sizeof(h->cfg)))
-    B200_FAIL(B200_ERR_INVALID, "mimi_session_import: the record was taken with another codec configuration");
+  B200_TRY(h->read_session_header(src_dev, nbytes, "mimi_session_import", &s));
   if (s.bytes != h->session_bytes || nbytes != h->session_bytes)
     B200_FAIL(B200_ERR_SHAPE, "mimi_session_import: the record takes %lld bytes, header says %lld, caller passed %lld", h->session_bytes,
               (long long)s.bytes, (long long)nbytes);
@@ -1169,31 +1051,26 @@ int b200_mimi_session_import(b200_mimi* h, int row, const void* src_dev, int64_t
 
 int b200_mimi_set_graph(b200_mimi* h, int enable) {
   if (!h) B200_FAIL(B200_ERR_INVALID, "mimi_set_graph: null handle");
-  h->graph_enabled = enable;
-  if (!enable) drop_graphs(h);
+  h->set_graph(enable);
   return B200_OK;
 }
 
 static int ensure_host_staging(b200_mimi* h, size_t pcm_n, size_t codes_n) {
-  if (pcm_n > h->pin_pcm_n) {
-    if (h->pin_pcm) cudaFreeHost(h->pin_pcm);
-    if (h->dev_pcm) cudaFree(h->dev_pcm);
-    B200_CUDA(cudaMallocHost(&h->pin_pcm, pcm_n * 4));
-    B200_CUDA(cudaMalloc(&h->dev_pcm, pcm_n * 4));
-    h->pin_pcm_n = h->dev_pcm_n = pcm_n;
-  }
-  if (codes_n > h->pin_codes_n) {
-    if (h->pin_codes) cudaFreeHost(h->pin_codes);
-    if (h->dev_codes) cudaFree(h->dev_codes);
-    B200_CUDA(cudaMallocHost(&h->pin_codes, codes_n * 8));
-    B200_CUDA(cudaMalloc(&h->dev_codes, codes_n * 8));
-    h->pin_codes_n = h->dev_codes_n = codes_n;
-  }
+  if (pcm_n <= h->pin_pcm_n && codes_n <= h->pin_codes_n) return B200_OK;
+  const size_t pn = std::max(pcm_n, h->pin_pcm_n), cn = std::max(codes_n, h->pin_codes_n);
+  h->staging.free_all();
+  h->pin_pcm_n = h->pin_codes_n = 0;
+  B200_TRY(h->staging.alloc_host(&h->pin_pcm, pn));
+  B200_TRY(h->staging.alloc_t(&h->dev_pcm, pn, false));
+  B200_TRY(h->staging.alloc_host(&h->pin_codes, cn));
+  B200_TRY(h->staging.alloc_t(&h->dev_codes, cn, false));
+  h->pin_pcm_n = pn;
+  h->pin_codes_n = cn;
   return B200_OK;
 }
 
 int b200_mimi_encode_host(b200_mimi* h, const float* pcm_host, int n_frames, int64_t* codes_host) {
-  B200_TRY(ensure_streaming(h, "mimi_encode_host"));
+  B200_STREAMING_ENTRY(h, "mimi_encode_host");
   if (!pcm_host || !codes_host || n_frames < 1) B200_FAIL(B200_ERR_SHAPE, "mimi_encode_host: bad arguments");
   const size_t pn = (size_t)h->batch * h->frame_size * n_frames, cn = (size_t)h->batch * h->num_codebooks * n_frames;
   B200_TRY(ensure_host_staging(h, pn, cn));
@@ -1207,7 +1084,7 @@ int b200_mimi_encode_host(b200_mimi* h, const float* pcm_host, int n_frames, int
 }
 
 int b200_mimi_decode_host(b200_mimi* h, const int64_t* codes_host, int n_codebooks, int n_frames, float* pcm_host) {
-  B200_TRY(ensure_streaming(h, "mimi_decode_host"));
+  B200_STREAMING_ENTRY(h, "mimi_decode_host");
   if (!pcm_host || !codes_host || n_frames < 1) B200_FAIL(B200_ERR_SHAPE, "mimi_decode_host: bad arguments");
   const size_t pn = (size_t)h->batch * h->frame_size * n_frames, cn = (size_t)h->batch * n_codebooks * n_frames;
   B200_TRY(ensure_host_staging(h, pn, cn));
@@ -1223,49 +1100,34 @@ int b200_mimi_decode_host(b200_mimi* h, const int64_t* codes_host, int n_codeboo
 /* the same state entry by entry (names in include/moshi_b200.h) */
 int b200_mimi_state_count(b200_mimi* h) { return (h && h->batch > 0) ? (int)h->state.snap.size() : 0; }
 int b200_mimi_state_entry(b200_mimi* h, int index, const char** name, int* dtype, int* ndim, int64_t* shape8, int64_t* nbytes) {
-  B200_TRY(ensure_streaming(h, "mimi_state_entry"));
-  return state_entry_info(h->state, index, name, dtype, ndim, shape8, nbytes);
+  B200_TRY(check_streaming(h, "mimi_state_entry"));
+  return h->state_entry_info(index, name, dtype, ndim, shape8, nbytes);
 }
 int b200_mimi_state_read(b200_mimi* h, const char* name, void* dst_dev, int64_t nbytes) {
-  B200_TRY(ensure_streaming(h, "mimi_state_read"));
-  DeviceGuard g(h->device);
-  if (!dst_dev) B200_FAIL(B200_ERR_INVALID, "mimi_state_read: null destination");
-  return state_entry_copy(h->state, name, dst_dev, nullptr, nbytes, h->stream);
+  B200_STREAMING_ENTRY(h, "mimi_state_read");
+  return h->state_entry(name, dst_dev, nullptr, nbytes, "mimi_state_read");
 }
 int b200_mimi_state_write(b200_mimi* h, const char* name, const void* src_dev, int64_t nbytes) {
-  B200_TRY(ensure_streaming(h, "mimi_state_write"));
-  DeviceGuard g(h->device);
-  if (!src_dev) B200_FAIL(B200_ERR_INVALID, "mimi_state_write: null source");
-  return state_entry_copy(h->state, name, nullptr, src_dev, nbytes, h->stream);
+  B200_STREAMING_ENTRY(h, "mimi_state_write");
+  return h->state_entry(name, nullptr, src_dev, nbytes, "mimi_state_write");
 }
 
 int b200_mimi_error_flags(b200_mimi* h, int* flags_out) {
-  B200_TRY(ensure_streaming(h, "mimi_error_flags"));
-  DeviceGuard g(h->device);
-  int v = 0;
-  B200_CUDA(cudaMemcpyAsync(&v, h->err, 4, cudaMemcpyDeviceToHost, h->stream));
-  B200_CUDA(cudaStreamSynchronize(h->stream));
-  if (v) B200_CUDA(cudaMemsetAsync(h->err, 0, 4, h->stream));
-  if (flags_out) *flags_out = v;
-  return B200_OK;
+  B200_STREAMING_ENTRY(h, "mimi_error_flags");
+  return h->error_flags(flags_out);
 }
 
 int b200_mimi_read_buffer(b200_mimi* h, const char* name, float* dst_dev, int64_t capacity, int64_t* numel) {
-  B200_TRY(ensure_streaming(h, "mimi_read_buffer"));
-  DeviceGuard g(h->device);
+  B200_STREAMING_ENTRY(h, "mimi_read_buffer");
   auto it = h->taps.find(name ? name : "");
   if (it == h->taps.end()) B200_FAIL(B200_ERR_INVALID, "mimi_read_buffer: unknown buffer '%s'", name ? name : "(null)");
   const Tap& t = it->second;
   const int64_t n = (int64_t)h->batch * t.C * t.T;
-  if (numel) *numel = n;
-  if (!dst_dev) return B200_OK;
-  if (capacity < n) B200_FAIL(B200_ERR_SHAPE, "mimi_read_buffer: destination too small");
-  if (t.transpose && t.T > 1) {        // stored token-major [B][T][C], reported in the reference's [B][C][T]
-    B200_LAUNCH(tm_to_bct_kernel, (unsigned)ceil_div64(n, 256), 256, 0, h->stream, t.p, dst_dev, h->batch, t.C, t.T);
-    return check_launch("mimi_read_buffer");
-  }
-  B200_CUDA(cudaMemcpyAsync(dst_dev, t.p, (size_t)n * 4, cudaMemcpyDeviceToDevice, h->stream));
-  return B200_OK;
+  const bool transpose = t.transpose && t.T > 1;     // stored token-major [B][T][C], reported in the reference's [B][C][T]
+  B200_TRY(copy_out(t.p, n, transpose ? 0 : n * 4, dst_dev, capacity, numel, h->stream, "mimi_read_buffer"));
+  if (!transpose || !dst_dev) return B200_OK;
+  B200_LAUNCH(tm_to_bct_kernel, (unsigned)ceil_div64(n, 256), 256, 0, h->stream, t.p, dst_dev, h->batch, t.C, t.T);
+  return check_launch("mimi_read_buffer");
 }
 
 int64_t b200_mimi_algorithmic_bytes(b200_mimi* h) {

@@ -260,6 +260,27 @@ def test_graph_replay_equals_eager_launches(gpu):
 
 
 @torch.no_grad()
+def test_graph_replay_after_multiframe_quantize(gpu):
+    """A multi-frame quantize between encodes (encode_to_latent(quantize=True)) leaves the captured encode graph valid:
+    encode, quantize four frames at once, encode again, with graphs on == with graphs off, bit for bit at every call."""
+    B = 3
+    pcm = scenarios.mimi_noise(B, 7, seed=31).cuda()
+
+    def run(use_graph):
+        gpu.use_graph = use_graph
+        with gpu.streaming(B):
+            first = gpu.encode(pcm[..., :1920]).cpu()
+            latent = gpu.encode_to_latent(pcm[..., 1920:5 * 1920], quantize=True).cpu()
+            again = gpu.encode(pcm[..., 5 * 1920:]).cpu()
+        gpu.use_graph = True
+        return first, latent, again
+
+    eager, graph = run(False), run(True)
+    for want, got in zip(eager, graph):
+        assert torch.equal(want, got)
+
+
+@torch.no_grad()
 def test_streaming_state_snapshot_roundtrip(gpu):
     """get_streaming_state / set_streaming_state (streaming.py:158-181): replaying from a snapshot reproduces the
     continuation bit for bit (conv carries, overlap-add partials, KV rings, offsets, masks all restored)."""
