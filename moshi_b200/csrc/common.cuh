@@ -160,6 +160,9 @@ struct MimiFrameView {
 int lm_frame_view(b200_lm* h, LmFrameView* out);         // lm.cu
 int mimi_frame_view(b200_mimi* h, MimiFrameView* out);   // mimi.cu
 int lm_device(const b200_lm* h);                         // lm.cu: the device the frame services allocate and run on
+// lm.cu: a row the KV pool could not serve (B200_FLAG_KV_POOL) fails the frame with B200_ERR_STATE, as b200_lm_step_host does.
+// Synchronises; clears that flag only, the others stay for b200_lm_error_flags.  Nothing without a pool.
+int lm_check_kv_pool(b200_lm* h);
 
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }

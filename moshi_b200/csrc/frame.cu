@@ -17,7 +17,6 @@
 #include "common.cuh"
 
 namespace b200 {
-int lm_check_kv_pool(b200_lm* h);      // lm.cu: B200_ERR_STATE (and clears the flag) if B200_FLAG_KV_POOL was raised; no-op without a pool
 namespace {
 
 // ClientState of every slot (batched_asr.py:85-98), one array per field.

@@ -12,9 +12,6 @@ namespace {
 struct TLayer {
   const bf16 *in_w, *out_w, *n1, *n2, *lin_in, *lin_out;
   const float *in_s = nullptr, *out_s = nullptr, *lin_in_s = nullptr, *lin_out_s = nullptr;   // int8 path: weight-row scales
-  bf16 *kc = nullptr, *vc = nullptr;
-  uint8_t *kc8 = nullptr, *vc8 = nullptr;      // opt-in fp8 ring: e4m3 bytes [B][H][cap][D] ...
-  float *ks = nullptr, *vs = nullptr;          // ... and one scale per (session, head, slot)
   // cross-attention layers (b200_lm_set_cross_attention): norm_cross, the query / K|V / output linears, and the condition memory
   // k_cross / v_cross [MB][H][cross_len][ATT_D] bf16
   const bf16 *ncw = nullptr, *ncb = nullptr, *cq_w = nullptr, *ckv_w = nullptr, *co_w = nullptr;
@@ -52,6 +49,288 @@ void b200::lm::cross_attn_launch(const bf16* q, long long ldq, const bf16* kc, c
   const CrossAttnStep a{q, ldq, kc, vc, out, part, counters, H, T, nsplit};
   B200_LAUNCH(cross_attn_step_kernel, dim3(B * H, nsplit), ATT_THREADS, 0, st, a);
 }
+
+// ---- temporal K/V storage -----------------------------------------------------------------------------------------------------
+// The temporal K/V of one LM handle, in one of four forms: bf16 rings of the model's context (the reference's RingKVCache), rings
+// shortened to kv_capacity slots, 8-bit rings (kv_dtype), or one pool of pages shared by all rows (kv_pool_frames).  Only this
+// unit knows which: the handle asks it for the step's prologue and each layer's rings, position writes, the state entries, the K/V
+// section of a session record and the meaning of error flags 4 and 8.
+namespace {
+
+struct TemporalKv {
+  // configuration, before streaming_begin
+  int kind = B200_KV_BF16;                     // B200_KV_BF16, or 8-bit rings B200_KV_FP8_E4M3 / B200_KV_INT8 (= KV_E4M3 / KV_INT8)
+  int capacity = 0;                            // slots per ring when shorter than the context, else 0
+  int64_t pool_frames = 0;                     // > 0: the bf16 rings live in pages of page_slots slots
+  int page_slots = 64;
+  int context = 0, H = 0;                      // the model's
+  // geometry, from streaming_begin
+  int MB = 0, cap = 0;                         // model rows, slots per ring
+  int n_pages = 0, tab_ld = 0, page_shift = 0;   // n_pages = 0: no pool
+  // per layer K and V: bf16 rings [MB][H][cap][ATT_D] or pools [n_pages + 1][H][page_slots][ATT_D] (the last page a sink), or
+  // 8-bit rings [MB][H][cap][ATT_D] and their fp32 scales ks / vs [MB][H][cap]
+  struct Layer { void *k = nullptr, *v = nullptr; float *ks = nullptr, *vs = nullptr; };
+  std::vector<Layer> layers;
+  int *table = nullptr, *held = nullptr;             // [MB][tab_ld] (-1 = unmapped), pages held per row [MB]
+  int *free_stack = nullptr, *free_top = nullptr;    // [n_pages], [1]
+  void** arrays = nullptr;                     // what kv_copy_kernel reads: [layer][k|v], then for 8-bit rings [layer][ks|vs]
+  const long long* pos = nullptr;              // the handle's model.offset [MB]
+
+  // bytes of one head's K (or V) in one slot: ATT_D bf16, or ATT_D 8-bit codes and their fp32 scale
+  int64_t slot_bytes() const { return kind ? ATT_D + 4 : ATT_D * 2; }
+  size_t ring_slots() const { return n_pages ? (size_t)(n_pages + 1) * page_slots : (size_t)MB * cap; }   // per layer and head
+  size_t bytes() const { return layers.size() * 2 * ring_slots() * H * slot_bytes(); }
+
+  int pool_conflict(int64_t frames, const char* what) const {
+    if (frames > 0 && (kind || capacity > 0))
+      B200_FAIL(B200_ERR_INVALID, "%s: the KV pool holds bf16 rings of the model's context (no kv_dtype or kv_capacity)", what);
+    return B200_OK;
+  }
+  int set_dtype(int dtype) {
+    if (dtype != B200_KV_BF16 && dtype != B200_KV_FP8_E4M3 && dtype != B200_KV_INT8)
+      B200_FAIL(B200_ERR_INVALID, "lm_set_kv_dtype: unknown dtype %d", dtype);
+    kind = dtype;
+    return B200_OK;
+  }
+  int set_capacity(int slots) {
+    if (slots < 0) B200_FAIL(B200_ERR_INVALID, "lm_set_kv_capacity: negative capacity");
+    capacity = slots >= context ? 0 : slots;
+    return B200_OK;
+  }
+  int set_pool(int64_t frames, int slots) {
+    if (frames < 0) B200_FAIL(B200_ERR_INVALID, "lm_set_kv_pool: negative size");
+    if (frames > 0) {
+      if (slots < 4 || slots > 256 || (slots & (slots - 1)))
+        B200_FAIL(B200_ERR_INVALID, "lm_set_kv_pool: page_slots %d (a power of two in [4, 256])", slots);
+      B200_TRY(pool_conflict(frames, "lm_set_kv_pool"));
+      page_slots = slots;
+    }
+    pool_frames = frames;
+    return B200_OK;
+  }
+
+  // streaming_begin, before it allocates: the geometry of `rows` model rows and `n_layers` layers
+  int plan(int rows, int n_layers) {
+    B200_TRY(pool_conflict(pool_frames, "lm_streaming_begin"));
+    MB = rows;
+    cap = capacity > 0 ? capacity : context;
+    n_pages = tab_ld = page_shift = 0;
+    if (pool_frames > 0) {
+      tab_ld = ceil_div(context, page_slots);
+      page_shift = __builtin_ctz(page_slots);
+      n_pages = (int)std::min(ceil_div64(pool_frames, page_slots), (int64_t)MB * tab_ld);
+    }
+    layers.assign(n_layers, Layer{});
+    return B200_OK;
+  }
+  // layer l's K and V, where streaming_begin allocates that layer's state
+  int alloc_layer(Arena& A, int l) {
+    Layer& L = layers[l];
+    const size_t n = ring_slots() * H;         // (head, slot) pairs
+    B200_TRY(A.alloc(&L.k, n * (kind ? ATT_D : ATT_D * 2)));
+    B200_TRY(A.alloc(&L.v, n * (kind ? ATT_D : ATT_D * 2)));
+    if (kind) {
+      B200_TRY(A.alloc_t(&L.ks, n));
+      B200_TRY(A.alloc_t(&L.vs, n));
+    }
+    return B200_OK;
+  }
+  // the page table, page counts and free stack (nothing without a pool)
+  int alloc_pages(Arena& A) {
+    if (!n_pages) return B200_OK;
+    B200_TRY(A.alloc_t(&table, (size_t)MB * tab_ld, false));
+    B200_CUDA(cudaMemset(table, 0xFF, (size_t)MB * tab_ld * 4));      // -1: unmapped
+    B200_TRY(A.alloc_t(&held, MB));
+    B200_TRY(A.alloc_t(&free_stack, n_pages, false));
+    B200_TRY(A.alloc_t(&free_top, 1, false));
+    std::vector<int> stack(n_pages);
+    for (int i = 0; i < n_pages; ++i) stack[i] = n_pages - 1 - i;        // page 0 is popped first
+    B200_CUDA(cudaMemcpy(free_stack, stack.data(), stack.size() * 4, cudaMemcpyHostToDevice));
+    B200_CUDA(cudaMemcpy(free_top, &n_pages, 4, cudaMemcpyHostToDevice));
+    return B200_OK;
+  }
+  // The state entries layers.<l>.k / .v [MB][H][cap][ATT_D] bf16 (a paged layer's in that ring layout too, see copy_entry), or
+  // .k8 / .v8 and .k_scale / .v_scale; then the device list of the arrays.
+  int mark_state(Arena& A) {
+    const int D = ATT_D;
+    const size_t n = (size_t)MB * H * cap;
+    std::vector<void*> list;
+    for (size_t l = 0; l < layers.size(); ++l) {
+      const Layer& L = layers[l];
+      const std::string p = "layers." + std::to_string(l);
+      if (kind) {
+        A.mark_state(L.k, n * D, p + ".k8", B200_U8, {MB, H, cap, D});
+        A.mark_state(L.v, n * D, p + ".v8", B200_U8, {MB, H, cap, D});
+        A.mark_state(L.ks, n * 4, p + ".k_scale", B200_F32, {MB, H, cap});
+        A.mark_state(L.vs, n * 4, p + ".v_scale", B200_F32, {MB, H, cap});
+      } else {
+        A.mark_state(L.k, n * D * 2, p + ".k", B200_BF16, {MB, H, cap, D});
+        A.mark_state(L.v, n * D * 2, p + ".v", B200_BF16, {MB, H, cap, D});
+      }
+      list.insert(list.end(), {L.k, L.v});
+    }
+    for (auto& L : layers)
+      if (kind) list.insert(list.end(), {L.ks, L.vs});
+    B200_TRY(A.alloc_t(&arrays, list.size(), false));
+    B200_CUDA(cudaMemcpy(arrays, list.data(), list.size() * sizeof(void*), cudaMemcpyHostToDevice));
+    return B200_OK;
+  }
+  void end() {
+    MB = cap = n_pages = tab_ld = page_shift = 0;
+    layers.clear();
+    table = held = free_stack = free_top = nullptr;
+    arrays = nullptr; pos = nullptr;
+  }
+
+  // Before the step's first layer: a shortened ring serves a session only until it is full, so a row about to overwrite a live key
+  // raises flag 4 instead of silently forgetting; a pool maps the page of this step's slot (all layers share the table).
+  void prologue(const uint8_t* exec_mask, int* err, cudaStream_t st) const {
+    if (cap < context) B200_LAUNCH(kv_capacity_check_kernel, ceil_div(MB, 128), 128, 0, st, pos, exec_mask, MB, cap, err);
+    if (n_pages)
+      B200_LAUNCH(kv_page_alloc_kernel, 1, KV_PAGE_THREADS, 0, st, table, held, free_stack, free_top, pos, exec_mask, MB, tab_ld,
+                  page_shift, context, n_pages, err);
+  }
+  KvRings rings(int l) const { return {layers[l].k, layers[l].v, layers[l].ks, layers[l].vs, table, tab_ld, page_shift}; }
+  // b200_lm_reset: the masked sessions' rows (b and b + B under CFG; null mask = all) return their pages to the pool
+  void release(const uint8_t* mask, int B, cudaStream_t st) const {
+    if (n_pages)
+      B200_LAUNCH(kv_page_free_kernel, 1, KV_PAGE_THREADS, 0, st, table, held, free_stack, free_top, mask, B, MB, tab_ld);
+  }
+
+  // Model rows row0 + k * row_step are about to hold positions at[k], in ascending row order.  A pool gives each exactly the pages of
+  // slots [0, min(at[k], context)) (synchronises): excess pages are pushed back first (row and table order), then missing ones
+  // are popped (row order); B200_ERR_STATE, changing nothing, when the free pages do not cover them.  Rings need nothing.
+  int hold(int row0, int row_step, const std::vector<long long>& at, const char* what, cudaStream_t st) {
+    if (!n_pages) return B200_OK;
+    auto pages_for = [&](long long p) { return (int)((std::min(std::max(p, 0LL), (long long)context) + page_slots - 1) / page_slots); };
+    const int T = tab_ld, n_rows = (int)at.size();
+    std::vector<int> tab((size_t)MB * T), got(MB), stack(n_pages);
+    int top = 0;
+    const struct { int* dev; int* host; size_t n; } io[4] = {{table, tab.data(), tab.size()}, {held, got.data(), got.size()},
+                                                            {free_stack, stack.data(), stack.size()}, {free_top, &top, 1}};
+    B200_CUDA(cudaStreamSynchronize(st));
+    for (auto& x : io) B200_CUDA(cudaMemcpy(x.host, x.dev, x.n * 4, cudaMemcpyDeviceToHost));
+    int more = 0;
+    for (int k = 0; k < n_rows; ++k) more += pages_for(at[k]) - got[row0 + k * row_step];
+    if (more > top) B200_FAIL(B200_ERR_STATE, "%s: the rows need %d more KV pages, the pool has %d free", what, more, top);
+    for (int k = 0; k < n_rows; ++k) {
+      const int b = row0 + k * row_step, want = pages_for(at[k]);
+      int* row = tab.data() + (size_t)b * T;
+      for (int i = want; i < T; ++i) {
+        if (i < got[b]) stack[top++] = row[i];
+        row[i] = -1;
+      }
+      got[b] = std::min(got[b], want);
+    }
+    for (int k = 0; k < n_rows; ++k) {
+      const int b = row0 + k * row_step, want = pages_for(at[k]);
+      for (int i = got[b]; i < want; ++i) tab[(size_t)b * T + i] = stack[--top];
+      got[b] = want;
+    }
+    for (auto& x : io) B200_CUDA(cudaMemcpy(x.dev, x.host, x.n * 4, cudaMemcpyHostToDevice));
+    return B200_OK;
+  }
+  // the same for every model row, the positions being a model.offset [MB] on the device about to be written
+  int hold_dev(const void* at_dev, const char* what, cudaStream_t st) {
+    if (!n_pages) return B200_OK;
+    std::vector<long long> at(MB);
+    B200_CUDA(cudaStreamSynchronize(st));
+    B200_CUDA(cudaMemcpy(at.data(), at_dev, (size_t)MB * 8, cudaMemcpyDeviceToHost));
+    return hold(0, 1, at, what, st);
+  }
+  // a shortened ring holds a session's history until position cap: B200_ERR_STATE past it
+  int check_history(int64_t top, const char* what) const {
+    if (cap < context && top > cap)
+      B200_FAIL(B200_ERR_STATE, "%s: the session is at position %lld, past its %d-slot KV ring: the ring no longer holds its history", what,
+                (long long)top, cap);
+    return B200_OK;
+  }
+
+  // K / V of n_arrays arrays from arrays[first] on, model rows row0 + k * row_step (k < n_rows), slots [0, n), to or from the flat
+  // buffer [array][k][H][n][slot] (kv_copy_kernel).  scales: the arrays are 8-bit rings' fp32 scales.
+  template <typename U, int V>
+  static void launch_copy(bool gather, dim3 grid, const KvCopy& a, cudaStream_t st) {
+    if (gather) B200_LAUNCH((kv_copy_kernel<true, U, V>), grid, 256, 0, st, a);
+    else B200_LAUNCH((kv_copy_kernel<false, U, V>), grid, 256, 0, st, a);
+  }
+  int copy(int first, int n_arrays, int row0, int n_rows, int row_step, int n, void* flat, bool gather, bool scales,
+           cudaStream_t st) const {
+    if (n <= 0) return B200_OK;
+    KvCopy a;
+    a.arrays = arrays + first; a.flat = flat; a.pos = pos;
+    a.table = table; a.tab_ld = tab_ld; a.page_shift = page_shift; a.sink = n_pages;
+    a.row0 = row0; a.n_rows = n_rows; a.row_step = row_step; a.H = H; a.cap = cap; a.n = n;
+    const long long segs = (long long)n_arrays * n_rows * H;
+    if (segs > 65535) B200_FAIL(B200_ERR_INVALID, "kv_copy: %lld ring segments in one launch", segs);
+    const int V = scales ? 1 : kind ? ATT_D / 16 : ATT_D / 8;     // 4-byte scales, 16-byte vectors of bytes or bf16
+    const dim3 grid((unsigned)ceil_div(n * V, 256), (unsigned)segs);
+    if (scales) launch_copy<uint32_t, 1>(gather, grid, a, st);
+    else if (kind) launch_copy<uint4, ATT_D / 16>(gather, grid, a, st);
+    else launch_copy<uint4, ATT_D / 8>(gather, grid, a, st);
+    return check_launch("kv_copy");
+  }
+  // A paged layer's K / V state entry keeps the ring layout: its index in `arrays`, or -1 (another entry, or no pool) ...
+  int paged_array(const void* p) const {
+    for (size_t l = 0; n_pages && l < layers.size(); ++l) {
+      if (p == layers[l].k) return 2 * (int)l;
+      if (p == layers[l].v) return 2 * (int)l + 1;
+    }
+    return -1;
+  }
+  // ... gathered from the pool into dst, or scattered from src into it
+  int copy_entry(int arr, void* dst, const void* src, cudaStream_t st) const {
+    return copy(arr, 1, 0, MB, 1, cap, dst ? dst : const_cast<void*>(src), dst != nullptr, false, st);
+  }
+
+  // The K/V section of a session record: slots [0, n) of `rows` model rows (row, row + row_step) as
+  // [layer][k|v][model row][head][n][ATT_D], 8-bit rings' bytes followed by their fp32 scales [layer][k|v][model row][head][n]
+  int64_t record_bytes(int rows, int64_t n) const { return (int64_t)layers.size() * 2 * H * slot_bytes() * rows * n; }
+  int check_record(uint32_t record_kind, const char* what) const {
+    if (record_kind != (uint32_t)kind)
+      B200_FAIL(B200_ERR_INVALID, "%s: the record's KV storage type %u differs from the handle's %d", what, record_kind, kind);
+    return B200_OK;
+  }
+  int record(int row, int rows, int row_step, int n, char* rec, bool gather, cudaStream_t st) const {
+    const int L2 = 2 * (int)layers.size();
+    B200_TRY(copy(0, L2, row, rows, row_step, n, rec, gather, false, st));
+    if (kind) B200_TRY(copy(L2, L2, row, rows, row_step, n, rec + (int64_t)L2 * rows * H * n * ATT_D, gather, true, st));
+    return B200_OK;
+  }
+
+  // error flags 4 (a row stepped past its shortened ring) and 8 (a row's ring did not get a page) as B200_ERR_STATE
+  int flag_error(int flags, const char* what) const {
+    if (flags & ERR_KV_CAPACITY)
+      B200_FAIL(B200_ERR_STATE, "%s: a session stepped past its %d-slot KV ring (b200_lm_set_kv_capacity; flags %d)", what, cap, flags);
+    if (flags & ERR_KV_POOL)
+      B200_FAIL(B200_ERR_STATE, "%s: a session's KV ring did not get a page: the KV pool of %d pages is full (flags %d)", what, n_pages,
+                flags);
+    return B200_OK;
+  }
+  // flag 8 alone, read and cleared on the device (synchronises); the other flags stay
+  int check_pool_flag(int* err, const char* what, cudaStream_t st) const {
+    if (!n_pages) return B200_OK;
+    int v = 0;
+    B200_CUDA(cudaMemcpyAsync(&v, err, 4, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaStreamSynchronize(st));
+    if (!(v & ERR_KV_POOL)) return B200_OK;
+    const int rest = v & ~ERR_KV_POOL;
+    B200_CUDA(cudaMemcpyAsync(err, &rest, 4, cudaMemcpyHostToDevice, st));
+    B200_CUDA(cudaStreamSynchronize(st));
+    return flag_error(v, what);
+  }
+  int usage(int* used, int* total, cudaStream_t st) const {
+    int top = 0;
+    if (n_pages) {
+      B200_CUDA(cudaMemcpyAsync(&top, free_top, 4, cudaMemcpyDeviceToHost, st));
+      B200_CUDA(cudaStreamSynchronize(st));
+    }
+    if (used) *used = n_pages - top;
+    if (total) *total = n_pages;
+    return B200_OK;
+  }
+};
+
+}  // namespace
 
 struct b200_lm : StreamCore {       // batch: sessions (LMGen batch); graphs[0]: the step
   b200_lm_config cfg;
@@ -101,17 +380,8 @@ struct b200_lm : StreamCore {       // batch: sessions (LMGen batch); graphs[0]:
   int* attn_counters = nullptr;                // split arrival counters [B*H]
   tc::DepFused* depf = nullptr;                // the depformer of a frame as one persistent kernel (B200_DEP_FUSED=0: off)
   int dep_fused = 1;
-  int kv_cap = 0;                              // b200_lm_set_kv_capacity: slots per ring (0 = cfg.context, the reference's ring)
-  int kv_fp8 = 0;                              // b200_lm_set_kv_dtype / B200_KV_DTYPE: opt-in 8-bit KV ring (B200_KV_FP8_E4M3 or B200_KV_INT8; 0 = bf16)
-  // b200_lm_set_kv_pool: the temporal rings live in pages of page_slots slots (TLayer kc / vc are then the pools
-  // [n_pages + 1][H][page_slots][D], the last page a sink); n_pages = 0: contiguous rings
-  int64_t pool_frames = 0; int page_slots = 64;
-  int n_pages = 0, tab_ld = 0, page_shift = 0;
-  int *page_table = nullptr, *page_held = nullptr;     // [MB][tab_ld] (-1 = unmapped), [MB]
-  int *free_stack = nullptr, *free_top = nullptr;      // [n_pages], [1]
-  // session records: the temporal rings (pools) as one device list, bf16 [layer][k|v], 8-bit [layer][k8|v8] then [layer][ks|vs] ...
-  void** kv_arrays = nullptr;
-  // ... and the per-session slices of the small state entries; the condition_sum rows come last and travel while it is on
+  TemporalKv kv;                               // the temporal K/V: rings or pool, their state entries and record section
+  // session records: the per-session slices of the small state entries; the condition_sum rows come last and travel while it is on
   RowSlice* slices_dev = nullptr;
   int n_slices = 0, n_slices_cond = 0;
   long long slices_end = 0, slices_end_cond = 0, slices_max = 0;
@@ -137,17 +407,11 @@ struct b200_lm : StreamCore {       // batch: sessions (LMGen batch); graphs[0]:
   float* pin_noise = nullptr;
   int64_t weight_bytes = 0;
   tc::TensorMapCache maps;
-  // a paged handle gathers its K / V entries into ring layout and scatters them back (kv_copy)
+  // a paged handle gathers its K / V entries into ring layout and scatters them back (TemporalKv::copy_entry)
   int copy_entry(const StateEntry& e, void* dst, const void* src) override;
 };
 
 namespace {
-
-// slots per temporal KV ring: the reference's context unless b200_lm_set_kv_capacity shortened it
-inline int ring_cap(const b200_lm* h) { return h->kv_cap > 0 && h->kv_cap < h->cfg.context ? h->kv_cap : h->cfg.context; }
-
-// bytes of one head's K (or V) row in one ring slot: ATT_D bf16, or ATT_D 8-bit codes and their fp32 scale
-inline int64_t kv_row_bytes(const b200_lm* h) { return h->kv_fp8 ? ATT_D + 4 : ATT_D * 2; }
 
 int get_bf16(b200_lm* h, const std::string& name, std::vector<int64_t> shape, const bf16** out) {
   const Tensor* t = h->store.find(name);
@@ -347,19 +611,13 @@ int step_body(b200_lm* h) {
     const long long n = (long long)B * noise_per_row(h);
     B200_LAUNCH(lm_noise_kernel, (unsigned)ceil_div64(ceil_div64(n, 4), 256), 256, 0, st, h->noise, n, h->noise_seed, h->noise_ctr);
   }
-  if (ring_cap(h) < c.context)      // a shortened ring serves a session only until it is full: flag instead of silently forgetting
-    B200_LAUNCH(kv_capacity_check_kernel, ceil_div(MB, 128), 128, 0, st, h->pos, h->exec_mask_m, MB, ring_cap(h), h->err);
-  if (h->n_pages)                   // map the page of this step's slot (all layers share the table)
-    B200_LAUNCH(kv_page_alloc_kernel, 1, KV_PAGE_THREADS, 0, st, h->page_table, h->page_held, h->free_stack, h->free_top, h->pos,
-                h->exec_mask_m, MB, h->tab_ld, h->page_shift, c.context, h->n_pages, h->err);
+  h->kv.prologue(h->exec_mask_m, h->err, st);
   for (size_t l = 0; l < h->layers.size(); ++l) {
     const TLayer& L = h->layers[l];
     B200_TRY(norm_linear(h, h->x, L.n1, h->xn, L.in_w, h->qkv, 3 * d, MB, 3 * d, d, LIN_STORE, 0, L.in_s));
-    KvRings r{L.kc, L.vc};   // RoPE + ring append + split-KV attention + split merge in one launch
-    if (h->kv_fp8) r = {L.kc8, L.vc8, L.ks, L.vs};
-    if (h->n_pages) r = {L.kc, L.vc, nullptr, nullptr, h->page_table, h->tab_ld, h->page_shift};
-    attn_step_launch(h->qkv, r, h->ao, h->attn_part, h->attn_counters, h->pos, h->exec_mask_m, MB, H, ring_cap(h), h->nsplit,
-                     c.max_period, h->kv_fp8, st);
+    // RoPE + ring append + split-KV attention + split merge in one launch
+    attn_step_launch(h->qkv, h->kv.rings((int)l), h->ao, h->attn_part, h->attn_counters, h->pos, h->exec_mask_m, MB, H, h->kv.cap,
+                     h->nsplit, c.max_period, h->kv.kind, st);
     B200_TRY(tap(h, h->ao, (int)l, TAP_ATTN_OUT));
     B200_TRY(linear(h, h->ao, d, L.out_w, h->x, d, h->x, d, MB, d, d, LIN_RESADD, 0, L.out_s));
     B200_TRY(tap(h, h->x, (int)l, TAP_X_ATTN));
@@ -423,98 +681,11 @@ int step_body(b200_lm* h) {
   return check_launch("lm step");
 }
 
-// pages a row holds at model position `pos`: those of slots [0, min(pos, context))
-int pages_for(const b200_lm* h, long long pos) {
-  const long long n = std::min(std::max(pos, 0LL), (long long)h->cfg.context);
-  return (int)((n + h->page_slots - 1) / h->page_slots);
-}
-
-// Paged handle, synchronous: model rows row0 + k * row_step come to hold exactly pages_for(pos[k]) pages, in ascending row order.
-// Their excess pages are pushed back first (row and table order), then missing ones are popped (row order).  Fails with
-// B200_ERR_STATE, changing nothing, when the free pages do not cover them.
-int pool_map(b200_lm* h, int row0, int row_step, const std::vector<long long>& pos, const char* what) {
-  const int T = h->tab_ld, n_rows = (int)pos.size();
-  std::vector<int> table((size_t)h->MB * T), held(h->MB), stack(h->n_pages);
-  int top = 0;
-  B200_CUDA(cudaStreamSynchronize(h->stream));
-  B200_CUDA(cudaMemcpy(table.data(), h->page_table, table.size() * 4, cudaMemcpyDeviceToHost));
-  B200_CUDA(cudaMemcpy(held.data(), h->page_held, held.size() * 4, cudaMemcpyDeviceToHost));
-  B200_CUDA(cudaMemcpy(stack.data(), h->free_stack, stack.size() * 4, cudaMemcpyDeviceToHost));
-  B200_CUDA(cudaMemcpy(&top, h->free_top, 4, cudaMemcpyDeviceToHost));
-  int more = 0;
-  for (int k = 0; k < n_rows; ++k) more += pages_for(h, pos[k]) - held[row0 + k * row_step];
-  if (more > top) B200_FAIL(B200_ERR_STATE, "%s: the rows need %d more KV pages, the pool has %d free", what, more, top);
-  for (int k = 0; k < n_rows; ++k) {
-    const int b = row0 + k * row_step, want = pages_for(h, pos[k]);
-    int* row = table.data() + (size_t)b * T;
-    for (int i = want; i < T; ++i) {
-      if (i < held[b]) stack[top++] = row[i];
-      row[i] = -1;
-    }
-    held[b] = std::min(held[b], want);
-  }
-  for (int k = 0; k < n_rows; ++k) {
-    const int b = row0 + k * row_step, want = pages_for(h, pos[k]);
-    for (int i = held[b]; i < want; ++i) table[(size_t)b * T + i] = stack[--top];
-    held[b] = want;
-  }
-  B200_CUDA(cudaMemcpy(h->page_table, table.data(), table.size() * 4, cudaMemcpyHostToDevice));
-  B200_CUDA(cudaMemcpy(h->page_held, held.data(), held.size() * 4, cudaMemcpyHostToDevice));
-  B200_CUDA(cudaMemcpy(h->free_stack, stack.data(), stack.size() * 4, cudaMemcpyHostToDevice));
-  B200_CUDA(cudaMemcpy(h->free_top, &top, 4, cudaMemcpyHostToDevice));
-  return B200_OK;
-}
-
-// The K / V state entry of a paged layer: its index in kv_arrays (its ring view is gathered from / scattered into the pool).
-// Other entries: -1.
-int paged_array_of(const b200_lm* h, const StateEntry& e) {
-  if (!h->n_pages) return -1;
-  for (size_t l = 0; l < h->layers.size(); ++l) {
-    if (e.ptr == h->layers[l].kc) return 2 * (int)l;
-    if (e.ptr == h->layers[l].vc) return 2 * (int)l + 1;
-  }
-  return -1;
-}
-
-// K / V of `n_arrays` rings from kv_arrays[first] on, model rows row0 + k * row_step (k < n_rows), slots [0, n), to or from the
-// flat buffer [array][k][H][n][slot] (kv_copy_kernel), on the handle's stream.  `scales`: the fp32 rings of an 8-bit handle.
-int kv_copy(b200_lm* h, int first, int n_arrays, int row0, int n_rows, int row_step, int n, void* flat, bool gather, bool scales) {
-  if (n <= 0) return B200_OK;
-  KvCopy a;
-  a.arrays = h->kv_arrays + first; a.flat = flat; a.pos = h->pos;
-  a.table = h->n_pages ? h->page_table : nullptr; a.tab_ld = h->tab_ld; a.page_shift = h->page_shift; a.sink = h->n_pages;
-  a.row0 = row0; a.n_rows = n_rows; a.row_step = row_step; a.H = h->cfg.num_heads; a.cap = ring_cap(h); a.n = n;
-  const long long segs = (long long)n_arrays * n_rows * a.H;
-  if (segs > 65535) B200_FAIL(B200_ERR_INVALID, "kv_copy: %lld ring segments in one launch", segs);
-  const int V = scales ? 1 : h->kv_fp8 ? ATT_D / 16 : ATT_D / 8;     // 4-byte scales, 16-byte vectors of bytes or bf16
-  const dim3 grid((unsigned)ceil_div(n * V, 256), (unsigned)segs);
-  if (scales) {
-    if (gather) B200_LAUNCH((kv_copy_kernel<true, uint32_t, 1>), grid, 256, 0, h->stream, a);
-    else B200_LAUNCH((kv_copy_kernel<false, uint32_t, 1>), grid, 256, 0, h->stream, a);
-  } else if (h->kv_fp8) {
-    if (gather) B200_LAUNCH((kv_copy_kernel<true, uint4, ATT_D / 16>), grid, 256, 0, h->stream, a);
-    else B200_LAUNCH((kv_copy_kernel<false, uint4, ATT_D / 16>), grid, 256, 0, h->stream, a);
-  } else {
-    if (gather) B200_LAUNCH((kv_copy_kernel<true, uint4, ATT_D / 8>), grid, 256, 0, h->stream, a);
-    else B200_LAUNCH((kv_copy_kernel<false, uint4, ATT_D / 8>), grid, 256, 0, h->stream, a);
-  }
-  return check_launch("kv_copy");
-}
-
-// the model positions a write of `model.offset` from `src_dev` would set, on the host
-int read_positions(b200_lm* h, const void* src_dev, std::vector<long long>* pos) {
-  pos->assign(h->MB, 0);
-  B200_CUDA(cudaStreamSynchronize(h->stream));
-  B200_CUDA(cudaMemcpy(pos->data(), src_dev, (size_t)h->MB * 8, cudaMemcpyDeviceToHost));
-  return B200_OK;
-}
-
 // ---- session records (b200_lm_session_*) ----------------------------------------------------------------------------------
 // After the 256-byte SessionHeader: the session's slices of exec_mask, cache, offsets, model.offset (1 or 2 rows), under CFG
 // model.exec_mask (2 rows) and cfg_is_masked_until, and while it is on the condition_sum rows, each 16-byte aligned (the
 // RowSlice table of streaming_begin).  From the next 256-byte boundary, the temporal K/V of slots [0, n), n = min(pos, ring
-// capacity), slot s being position s mod capacity: [layer][k|v][model row][head][n][128] bf16, or for 8-bit rings the bytes in
-// that layout followed by the fp32 scales [layer][k|v][model row][head][n].  A cross-attention handle's record (SESSION_CROSS, the
+// capacity), slot s being position s mod capacity (TemporalKv::record).  A cross-attention handle's record (SESSION_CROSS, the
 // memory's key count T in the header's first reserved bytes) ends, from the next 256-byte boundary, with the session's condition
 // memory [layer][k|v][model row][head][T][128] bf16.
 struct SessionPlan {
@@ -530,7 +701,7 @@ int64_t cross_row_bytes(const b200_lm* h) { return (int64_t)h->cfg.num_heads * h
 void session_size(const b200_lm* h, SessionPlan* p) {
   const long long end = p->cond ? h->slices_end_cond : h->slices_end;
   p->kv_off = (end + 255) / 256 * 256;
-  p->bytes = p->kv_off + (int64_t)h->cfg.num_layers * 2 * h->cfg.num_heads * kv_row_bytes(h) * p->rows * p->n;
+  p->bytes = p->kv_off + h->kv.record_bytes(p->rows, p->n);
   if (h->cross_on) {
     p->cross_off = (p->bytes + 255) / 256 * 256;
     p->bytes = p->cross_off + (int64_t)h->cfg.num_layers * 2 * p->rows * cross_row_bytes(h);
@@ -545,11 +716,8 @@ int session_plan(b200_lm* h, int row, const char* what, SessionPlan* p) {
   for (int k = 0; k < p->rows; ++k)
     B200_CUDA(cudaMemcpy(&p->pos[k], h->pos + row + (size_t)k * h->batch, 8, cudaMemcpyDeviceToHost));
   const int64_t top = std::max(p->pos[0], p->pos[1]);
-  const int cap = ring_cap(h);
-  if (cap < h->cfg.context && top > cap)
-    B200_FAIL(B200_ERR_STATE, "%s: row %d stepped past its %d-slot KV ring (position %lld): its history is lost", what, row, cap,
-              (long long)top);
-  p->n = std::min<int64_t>(top, cap);
+  B200_TRY(h->kv.check_history(top, what));
+  p->n = std::min<int64_t>(top, h->kv.cap);
   p->cond = h->cond_on != 0;
   session_size(h, p);
   return B200_OK;
@@ -557,12 +725,7 @@ int session_plan(b200_lm* h, int row, const char* what, SessionPlan* p) {
 
 // The session's K/V between the rings and the record
 int session_kv(b200_lm* h, int row, const SessionPlan& p, char* rec, bool gather) {
-  const int L2 = 2 * (int)h->layers.size();
-  B200_TRY(kv_copy(h, 0, L2, row, p.rows, h->batch, (int)p.n, rec + p.kv_off, gather, false));
-  if (h->kv_fp8) {
-    const int64_t scales = p.kv_off + (int64_t)L2 * p.rows * h->cfg.num_heads * p.n * ATT_D;
-    B200_TRY(kv_copy(h, L2, L2, row, p.rows, h->batch, (int)p.n, rec + scales, gather, true));
-  }
+  B200_TRY(h->kv.record(row, p.rows, h->batch, (int)p.n, rec + p.kv_off, gather, h->stream));
   if (h->cross_on) {         // the condition memory of the session's model rows, each contiguous [H][T][128]
     const int64_t rb = cross_row_bytes(h);
     char* at = rec + p.cross_off;
@@ -579,25 +742,15 @@ int session_kv(b200_lm* h, int row, const SessionPlan& p, char* rec, bool gather
 }  // namespace
 
 int b200_lm::copy_entry(const StateEntry& e, void* dst, const void* src) {
-  const int arr = paged_array_of(this, e);
-  if (arr < 0) return StreamCore::copy_entry(e, dst, src);
-  return kv_copy(this, arr, 1, 0, MB, 1, cfg.context, dst ? dst : const_cast<void*>(src), dst != nullptr, false);
+  const int arr = kv.paged_array(e.ptr);
+  return arr < 0 ? StreamCore::copy_entry(e, dst, src) : kv.copy_entry(arr, dst, src, stream);
 }
 
 namespace b200 {
-// b200_frame_step: a row the KV pool could not serve fails the frame (B200_ERR_STATE), as b200_lm_step_host does.  Synchronises;
-// clears that flag only, the others stay for b200_lm_error_flags.
 int lm_check_kv_pool(b200_lm* h) {
-  if (!h || !h->n_pages || h->batch <= 0) return B200_OK;
+  if (!h || h->batch <= 0) return B200_OK;
   DeviceGuard g(h->device);
-  int v = 0;
-  B200_CUDA(cudaMemcpyAsync(&v, h->err, 4, cudaMemcpyDeviceToHost, h->stream));
-  B200_CUDA(cudaStreamSynchronize(h->stream));
-  if (!(v & ERR_KV_POOL)) return B200_OK;
-  const int rest = v & ~ERR_KV_POOL;
-  B200_CUDA(cudaMemcpyAsync(h->err, &rest, 4, cudaMemcpyHostToDevice, h->stream));
-  B200_CUDA(cudaStreamSynchronize(h->stream));
-  B200_FAIL(B200_ERR_STATE, "frame_step: a session's KV ring did not get a page: the KV pool of %d pages is full (flags %d)", h->n_pages, v);
+  return h->kv.check_pool_flag(h->err, "frame_step", h->stream);
 }
 
 int lm_frame_view(b200_lm* h, LmFrameView* v) {
@@ -637,9 +790,11 @@ int b200_lm_create(const b200_lm_config* cfg, b200_lm** out) {
   h->CT = h->max_delay + 2;     // lm.py:606-611
   if (const char* e = getenv("B200_PDL")) h->pdl = atoi(e) != 0;
   if (const char* e = getenv("B200_DEP_FUSED")) h->dep_fused = atoi(e);
+  h->kv.context = cfg->context;
+  h->kv.H = cfg->num_heads;
   if (const char* e = getenv("B200_KV_DTYPE")) {
     const std::string v = e;
-    h->kv_fp8 = (v == "fp8" || v == "fp8_e4m3") ? B200_KV_FP8_E4M3 : v == "int8" ? B200_KV_INT8 : 0;
+    h->kv.kind = (v == "fp8" || v == "fp8_e4m3") ? B200_KV_FP8_E4M3 : v == "int8" ? B200_KV_INT8 : B200_KV_BF16;
   }
   *out = h;
   return B200_OK;
@@ -854,21 +1009,12 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
   struct Cleanup { b200_lm* h; bool armed = true; ~Cleanup() { if (armed) b200_lm_streaming_end(h); } } cleanup{h};
   size_t free_b = 0, total_b = 0;
   cudaMemGetInfo(&free_b, &total_b);
-  const int cap = ring_cap(h);
-  if (h->pool_frames > 0 && (h->kv_fp8 || cap < c.context))
-    B200_FAIL(B200_ERR_INVALID, "lm_streaming_begin: the KV pool holds bf16 rings of the model's context (no kv_dtype or kv_capacity)");
-  h->n_pages = 0;
-  if (h->pool_frames > 0) {
-    h->tab_ld = ceil_div(c.context, h->page_slots);
-    h->page_shift = __builtin_ctz(h->page_slots);
-    h->n_pages = (int)std::min(ceil_div64(h->pool_frames, h->page_slots), (int64_t)MB * h->tab_ld);
-  }
-  const size_t ring_slots = h->n_pages ? (size_t)(h->n_pages + 1) * h->page_slots : (size_t)MB * cap;   // per layer and head
+  B200_TRY(h->kv.plan(MB, c.num_layers));
   if (h->cross_on && h->cross_len < 1)
     B200_FAIL(B200_ERR_STATE, "lm_streaming_begin: set the condition memory's length (b200_lm_set_cross_len) first");
   // the cross-attention handle's condition memory: K and V [MB][H][T][128] bf16 per layer
   const size_t cross_bytes = h->cross_on ? (size_t)c.num_layers * 2 * MB * h->cross_len * d * 2 : 0;
-  const size_t kv_bytes = (size_t)c.num_layers * 2 * ring_slots * H * kv_row_bytes(h) + cross_bytes;
+  const size_t kv_bytes = h->kv.bytes() + cross_bytes;
   if (kv_bytes + (1ull << 30) > free_b)
     B200_FAIL(B200_ERR_INVALID, "lm_streaming_begin: %d sessions need %.1f GB of KV ring, %.1f GB free", B, kv_bytes / 1e9,
               free_b / 1e9);
@@ -894,17 +1040,11 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
   }
   B200_TRY(A.alloc_t(&h->offsets, B));
   B200_TRY(A.alloc_t(&h->pos, MB));
+  h->kv.pos = h->pos;
   h->offset_cpu = 0;
-  for (auto& L : h->layers) {
-    if (h->kv_fp8) {
-      B200_TRY(A.alloc_t(&L.kc8, (size_t)MB * H * cap * D));
-      B200_TRY(A.alloc_t(&L.vc8, (size_t)MB * H * cap * D));
-      B200_TRY(A.alloc_t(&L.ks, (size_t)MB * H * cap));
-      B200_TRY(A.alloc_t(&L.vs, (size_t)MB * H * cap));
-    } else {
-      B200_TRY(A.alloc_t(&L.kc, ring_slots * H * D));
-      B200_TRY(A.alloc_t(&L.vc, ring_slots * H * D));
-    }
+  for (size_t l = 0; l < h->layers.size(); ++l) {
+    TLayer& L = h->layers[l];
+    B200_TRY(h->kv.alloc_layer(A, (int)l));
     if (h->cross_on) {
       B200_TRY(A.alloc_t(&L.kx, (size_t)MB * H * h->cross_len * D));
       B200_TRY(A.alloc_t(&L.vx, (size_t)MB * H * h->cross_len * D));
@@ -915,17 +1055,7 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
     B200_TRY(A.alloc_t(&h->cross_kv, (size_t)CROSS_CHUNK * 2 * d, false));
     B200_TRY(A.alloc_t(&h->cross_rows, MB, false));
   }
-  if (h->n_pages) {
-    B200_TRY(A.alloc_t(&h->page_table, (size_t)MB * h->tab_ld, false));
-    B200_CUDA(cudaMemset(h->page_table, 0xFF, (size_t)MB * h->tab_ld * 4));      // -1: unmapped
-    B200_TRY(A.alloc_t(&h->page_held, MB));
-    B200_TRY(A.alloc_t(&h->free_stack, h->n_pages, false));
-    B200_TRY(A.alloc_t(&h->free_top, 1, false));
-    std::vector<int> stack(h->n_pages);
-    for (int i = 0; i < h->n_pages; ++i) stack[i] = h->n_pages - 1 - i;        // page 0 is popped first
-    B200_CUDA(cudaMemcpy(h->free_stack, stack.data(), stack.size() * 4, cudaMemcpyHostToDevice));
-    B200_CUDA(cudaMemcpy(h->free_top, &h->n_pages, 4, cudaMemcpyHostToDevice));
-  }
+  B200_TRY(h->kv.alloc_pages(A));
   for (auto& L : h->dlayers) {
     B200_TRY(A.alloc_t(&L.kc, (size_t)MB * dd * c.dep_q));
     B200_TRY(A.alloc_t(&L.vc, (size_t)MB * dd * c.dep_q));
@@ -967,7 +1097,7 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
   // (the condition memory's K/V projection runs CROSS_CHUNK rows at a time)
   B200_TRY(A.alloc(reinterpret_cast<void**>(&h->sk_ws), tc::sk_workspace_bytes(h->cross_on ? std::max(MB, CROSS_CHUNK) : MB), false));
   B200_TRY(A.alloc_t(&h->sk_counters, tc::SK_MAX_TILES));
-  const int ns = attn_pick_splits(MB, H, cap);
+  const int ns = attn_pick_splits(MB, H, h->kv.cap);
   h->nsplit = ns;
   h->cross_nsplit = h->cross_on ? attn_pick_splits(MB, H, h->cross_len) : 1;      // the cross step shares the partials
   B200_TRY(A.alloc_t(&h->attn_part, (size_t)MB * H * (h->cross_on ? std::max(ns, h->cross_nsplit) : ns) * (ATT_D + 2)));
@@ -1027,19 +1157,7 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
   A.mark_state(h->offsets, (size_t)B * 8, "offsets", B200_I64, {B});
   A.mark_state(h->pos, (size_t)MB * 8, "model.offset", B200_I64, {MB});
   A.mark_state(h->noise_ctr, 8, "noise_counter", B200_I64, {1});
-  for (size_t l = 0; l < h->layers.size(); ++l) {
-    auto& L = h->layers[l];
-    const std::string p = "layers." + std::to_string(l);
-    if (h->kv_fp8) {
-      A.mark_state(L.kc8, (size_t)MB * H * cap * D, p + ".k8", B200_U8, {MB, H, cap, D});
-      A.mark_state(L.vc8, (size_t)MB * H * cap * D, p + ".v8", B200_U8, {MB, H, cap, D});
-      A.mark_state(L.ks, (size_t)MB * H * cap * 4, p + ".k_scale", B200_F32, {MB, H, cap});
-      A.mark_state(L.vs, (size_t)MB * H * cap * 4, p + ".v_scale", B200_F32, {MB, H, cap});
-    } else {
-      A.mark_state(L.kc, (size_t)MB * H * cap * D * 2, p + ".k", B200_BF16, {MB, H, cap, D});
-      A.mark_state(L.vc, (size_t)MB * H * cap * D * 2, p + ".v", B200_BF16, {MB, H, cap, D});
-    }
-  }
+  B200_TRY(h->kv.mark_state(A));
   for (size_t l = 0; h->cross_on && l < h->layers.size(); ++l) {     // _MHAState.k_cross / v_cross (transformer.py:321-327)
     auto& L = h->layers[l];
     const std::string p = "layers." + std::to_string(l);
@@ -1048,15 +1166,6 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
     A.mark_state(L.vx, (size_t)MB * H * T * D * 2, p + ".v_cross", B200_BF16, {MB, H, T, D});
   }
   {
-    std::vector<void*> arrays;
-    for (auto& L : h->layers) {
-      if (h->kv_fp8) { arrays.push_back(L.kc8); arrays.push_back(L.vc8); }
-      else { arrays.push_back(L.kc); arrays.push_back(L.vc); }
-    }
-    if (h->kv_fp8)
-      for (auto& L : h->layers) { arrays.push_back(L.ks); arrays.push_back(L.vs); }
-    B200_TRY(A.alloc_t(&h->kv_arrays, arrays.size(), false));
-    B200_CUDA(cudaMemcpy(h->kv_arrays, arrays.data(), arrays.size() * sizeof(void*), cudaMemcpyHostToDevice));
     const int rows_add[2] = {0, B};
     std::vector<RowSlice> s;
     auto add = [&](void* p, long long row_bytes, int model_rows) {
@@ -1101,16 +1210,12 @@ int b200_lm_set_state(b200_lm* h, const void* src_dev, int64_t nbytes) {
   B200_STREAMING_ENTRY(h, "lm_set_state");
   B200_TRY(h->check_blob(src_dev, nbytes, 256, "lm_set_state"));
   const size_t n = h->state.state_bytes();
-  if (h->n_pages) {          // map the snapshot's fill first (nothing changes if it does not fit), then scatter its K / V
-    size_t off_pos = 0;
-    for (auto& e : h->state.snap) {
-      if (e.name == "model.offset") break;
-      off_pos += (e.bytes + 255) / 256 * 256;
-    }
-    std::vector<long long> pos;
-    B200_TRY(read_positions(h, static_cast<const char*>(src_dev) + off_pos, &pos));
-    B200_TRY(pool_map(h, 0, 1, pos, "lm_set_state"));
+  size_t off_pos = 0;        // the rows take the snapshot's positions first (nothing changes if they cannot), then its K / V
+  for (auto& e : h->state.snap) {
+    if (e.name == "model.offset") break;
+    off_pos += (e.bytes + 255) / 256 * 256;
   }
+  B200_TRY(h->kv.hold_dev(static_cast<const char*>(src_dev) + off_pos, "lm_set_state", h->stream));
   B200_TRY(h->load_state(src_dev));
   B200_CUDA(cudaMemcpyAsync(&h->offset_cpu, static_cast<const char*>(src_dev) + n, 8, cudaMemcpyDeviceToHost, h->stream));
   B200_CUDA(cudaStreamSynchronize(h->stream));
@@ -1129,12 +1234,10 @@ int b200_lm_state_read(b200_lm* h, const char* name, void* dst_dev, int64_t nbyt
 }
 int b200_lm_state_write(b200_lm* h, const char* name, const void* src_dev, int64_t nbytes) {
   B200_STREAMING_ENTRY(h, "lm_state_write");
-  if (h->n_pages && src_dev && name && !strcmp(name, "model.offset")) {     // each row then holds exactly the pages of its new fill
+  if (src_dev && name && !strcmp(name, "model.offset")) {     // the rows take their new positions before they are written
     const StateEntry* e = nullptr;
     B200_TRY(h->find_entry(name, nbytes, &e));
-    std::vector<long long> pos;
-    B200_TRY(read_positions(h, src_dev, &pos));
-    B200_TRY(pool_map(h, 0, 1, pos, "lm_state_write"));
+    B200_TRY(h->kv.hold_dev(src_dev, "lm_state_write", h->stream));
   }
   return h->state_entry(name, nullptr, src_dev, nbytes, "lm_state_write");
 }
@@ -1153,8 +1256,7 @@ int b200_lm_streaming_end(b200_lm* h) {
   tc::dep_fused_destroy(h->depf);
   h->depf = nullptr;
   h->cfg_until = nullptr; h->noise_ctr = nullptr; h->cond_sum = nullptr; h->cond_on = 0;
-  h->n_pages = 0;
-  h->page_table = h->page_held = h->free_stack = h->free_top = nullptr;
+  h->kv.end();
   h->taps = nullptr; h->taps_on = 0;
   h->pin_in = h->pin_out = nullptr;
   h->pin_noise = nullptr;
@@ -1165,9 +1267,7 @@ int b200_lm_streaming_end(b200_lm* h) {
 int b200_lm_reset(b200_lm* h, const uint8_t* reset_mask_dev) {
   B200_STREAMING_ENTRY(h, "lm_reset");
   const int B = h->batch;
-  if (h->n_pages)         // a reset row's pages return to the pool
-    B200_LAUNCH(kv_page_free_kernel, 1, KV_PAGE_THREADS, 0, h->stream, h->page_table, h->page_held, h->free_stack, h->free_top,
-                reset_mask_dev, B, h->MB, h->tab_ld);
+  h->kv.release(reset_mask_dev, B, h->stream);
   // per-row device offsets (lm.py:539, transformer.py:229-234, 331-333) ...
   B200_LAUNCH(lm_reset_kernel, ceil_div(B, 128), 128, 0, h->stream, h->offsets, h->pos, h->exec_mask, h->exec_mask_m,
               reset_mask_dev, B, cfg_on(h) ? 1 : 0);
@@ -1259,45 +1359,24 @@ int b200_lm_set_taps(b200_lm* h, int enable) {
 int b200_lm_set_kv_dtype(b200_lm* h, int kv_dtype) {
   if (!h) B200_FAIL(B200_ERR_INVALID, "lm_set_kv_dtype: null handle");
   if (h->batch > 0) B200_FAIL(B200_ERR_STATE, "lm_set_kv_dtype: the rings are allocated at streaming_begin; set the dtype before it");
-  if (kv_dtype != B200_KV_BF16 && kv_dtype != B200_KV_FP8_E4M3 && kv_dtype != B200_KV_INT8)
-    B200_FAIL(B200_ERR_INVALID, "lm_set_kv_dtype: unknown dtype %d", kv_dtype);
-  h->kv_fp8 = kv_dtype;
-  return B200_OK;
+  return h->kv.set_dtype(kv_dtype);
 }
 
 int b200_lm_set_kv_capacity(b200_lm* h, int slots) {
   if (!h) B200_FAIL(B200_ERR_INVALID, "lm_set_kv_capacity: null handle");
   if (h->batch > 0) B200_FAIL(B200_ERR_STATE, "lm_set_kv_capacity: the rings are allocated at streaming_begin; set the capacity before it");
-  if (slots < 0) B200_FAIL(B200_ERR_INVALID, "lm_set_kv_capacity: negative capacity");
-  h->kv_cap = slots >= h->cfg.context ? 0 : slots;
-  return B200_OK;
+  return h->kv.set_capacity(slots);
 }
 
 int b200_lm_set_kv_pool(b200_lm* h, int64_t frames, int page_slots) {
   if (!h) B200_FAIL(B200_ERR_INVALID, "lm_set_kv_pool: null handle");
   if (h->batch > 0) B200_FAIL(B200_ERR_STATE, "lm_set_kv_pool: the pool is allocated at streaming_begin; set it before it");
-  if (frames < 0) B200_FAIL(B200_ERR_INVALID, "lm_set_kv_pool: negative size");
-  if (frames > 0) {
-    if (page_slots < 4 || page_slots > 256 || (page_slots & (page_slots - 1)))
-      B200_FAIL(B200_ERR_INVALID, "lm_set_kv_pool: page_slots %d (a power of two in [4, 256])", page_slots);
-    if (h->kv_fp8 || h->kv_cap > 0)
-      B200_FAIL(B200_ERR_INVALID, "lm_set_kv_pool: the pool holds bf16 rings of the model's context (no kv_dtype or kv_capacity)");
-    h->page_slots = page_slots;
-  }
-  h->pool_frames = frames;
-  return B200_OK;
+  return h->kv.set_pool(frames, page_slots);
 }
 
 int b200_lm_kv_pool_usage(b200_lm* h, int* pages_used, int* pages_total) {
   B200_STREAMING_ENTRY(h, "lm_kv_pool_usage");
-  int top = 0;
-  if (h->n_pages) {
-    B200_CUDA(cudaMemcpyAsync(&top, h->free_top, 4, cudaMemcpyDeviceToHost, h->stream));
-    B200_CUDA(cudaStreamSynchronize(h->stream));
-  }
-  if (pages_used) *pages_used = h->n_pages - top;
-  if (pages_total) *pages_total = h->n_pages;
-  return B200_OK;
+  return h->kv.usage(pages_used, pages_total, h->stream);
 }
 
 int b200_lm_session_bytes(b200_lm* h, int row, int64_t* nbytes) {
@@ -1315,7 +1394,7 @@ int b200_lm_session_export(b200_lm* h, int row, void* dst_dev, int64_t capacity)
   if (!dst_dev) B200_FAIL(B200_ERR_INVALID, "lm_session_export: null destination");
   if (capacity < p.bytes) B200_FAIL(B200_ERR_SHAPE, "lm_session_export: the record takes %lld bytes, capacity %lld", (long long)p.bytes, (long long)capacity);
   SessionHeader s = h->session_header(p.bytes);
-  s.kv_dtype = (uint32_t)h->kv_fp8; s.rows = p.rows;
+  s.kv_dtype = (uint32_t)h->kv.kind; s.rows = p.rows;
   s.flags = (p.cond ? SESSION_COND : 0) | (h->cfg_until ? SESSION_CFG_UNTIL : 0) | (h->cross_on ? SESSION_CROSS : 0);
   if (h->cross_on) memcpy(s.reserved, &h->cross_len, sizeof(int32_t));
   s.pos[0] = p.pos[0]; s.pos[1] = p.pos[1]; s.n = p.n;
@@ -1333,8 +1412,7 @@ int b200_lm_session_import(b200_lm* h, int row, const void* src_dev, int64_t nby
   B200_TRY(h->check_row(row, "lm_session_import"));
   SessionHeader s;
   B200_TRY(h->read_session_header(src_dev, nbytes, "lm_session_import", &s));
-  if (s.kv_dtype != (uint32_t)h->kv_fp8)
-    B200_FAIL(B200_ERR_INVALID, "lm_session_import: the record's KV storage type %u differs from the handle's %d", s.kv_dtype, h->kv_fp8);
+  B200_TRY(h->kv.check_record(s.kv_dtype, "lm_session_import"));
   SessionPlan p;
   p.rows = h->MB / h->batch;
   if (s.rows != p.rows || ((s.flags & SESSION_CFG_UNTIL) != 0) != (h->cfg_until != nullptr))
@@ -1359,11 +1437,8 @@ int b200_lm_session_import(b200_lm* h, int row, const void* src_dev, int64_t nby
   if (s.bytes != p.bytes || nbytes != p.bytes)
     B200_FAIL(B200_ERR_SHAPE, "lm_session_import: the record takes %lld bytes, header says %lld, caller passed %lld", (long long)p.bytes,
               (long long)s.bytes, (long long)nbytes);
-  const int cap = ring_cap(h);
-  if (cap < c.context && top > cap)
-    B200_FAIL(B200_ERR_STATE, "lm_session_import: the session is at position %lld, the %d-slot KV ring cannot hold its history",
-              (long long)top, cap);
-  if (h->n_pages) B200_TRY(pool_map(h, row, h->batch, std::vector<long long>(p.pos, p.pos + p.rows), "lm_session_import"));
+  B200_TRY(h->kv.check_history(top, "lm_session_import"));
+  B200_TRY(h->kv.hold(row, h->batch, std::vector<long long>(p.pos, p.pos + p.rows), "lm_session_import", h->stream));
   char* rec = const_cast<char*>(static_cast<const char*>(src_dev));
   B200_TRY(row_slice_copy(h->slices_dev, p.cond ? h->n_slices_cond : h->n_slices, h->slices_max, rec, row, false, h->stream));
   B200_TRY(session_kv(h, row, p, rec, false));
@@ -1375,7 +1450,7 @@ int b200_lm_assume_fill(b200_lm* h, int fill) {
   B200_STREAMING_ENTRY(h, "lm_assume_fill");
   if (fill < 0) B200_FAIL(B200_ERR_INVALID, "lm_assume_fill: negative fill");
   std::vector<long long> v(h->MB, fill);
-  if (h->n_pages) B200_TRY(pool_map(h, 0, 1, v, "lm_assume_fill"));
+  B200_TRY(h->kv.hold(0, 1, v, "lm_assume_fill", h->stream));
   B200_CUDA(cudaMemcpyAsync(h->offsets, v.data(), (size_t)h->batch * 8, cudaMemcpyHostToDevice, h->stream));
   B200_CUDA(cudaMemcpyAsync(h->pos, v.data(), v.size() * 8, cudaMemcpyHostToDevice, h->stream));
   B200_CUDA(cudaStreamSynchronize(h->stream));
@@ -1453,10 +1528,7 @@ int b200_lm_step_host(b200_lm* h, const int64_t* in_codes_host, int n_in, const 
   if (ready_host) *ready_host = (support_out_of_sync || h->offset_cpu > h->max_delay) ? 1 : 0;
   if (flags) {
     cudaMemsetAsync(h->err, 0, 4, h->stream);
-    if (flags & lm::ERR_KV_CAPACITY)
-      B200_FAIL(B200_ERR_STATE, "lm_step_host: a session stepped past its %d-slot KV ring (b200_lm_set_kv_capacity; flags %d)", ring_cap(h), flags);
-    if (flags & lm::ERR_KV_POOL)
-      B200_FAIL(B200_ERR_STATE, "lm_step_host: a session's KV ring did not get a page: the KV pool of %d pages is full (flags %d)", h->n_pages, flags);
+    B200_TRY(h->kv.flag_error(flags, "lm_step_host"));
     B200_FAIL(B200_ERR_INVALID, "lm_step_host: a token id outside its embedding table reached the model (flags %d)", flags);
   }
   return B200_OK;
@@ -1537,7 +1609,7 @@ int64_t b200_lm_algorithmic_bytes(b200_lm* h, int kv_fill) {
   w += (int64_t)c.dep_q * c.card * c.depformer_dim * 2;
   if (c.quantize) w /= 2;        // one byte per weight (the fp32 row scales are < 0.1 % of that)
   // per session: KV ring read (valid slots only) + append, embedding rows, logits written + read by the sampler
-  const int64_t kv_row = c.num_heads * kv_row_bytes(h);      // bytes of one K (or V) slot of a layer, all heads
+  const int64_t kv_row = c.num_heads * h->kv.slot_bytes();      // bytes of one K (or V) slot of a layer, all heads
   int64_t per = (int64_t)c.num_layers * 2 * kv_fill * kv_row + (int64_t)c.num_layers * 2 * kv_row;
   per += (int64_t)(c.n_q + 1) * c.dim * 2 + (int64_t)c.dep_q * c.depformer_dim * 2;
   per += (int64_t)2 * (c.text_card + (int64_t)c.dep_q * c.card) * 2;
