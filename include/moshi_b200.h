@@ -312,6 +312,14 @@ int b200_lm_assume_fill(b200_lm* h, int fill);
 /* 0 = one launch per kernel, 1 = replay the whole step as one CUDA graph (default 1): the reference graphs forward_text and
  * depformer_step separately (lm.py:628-634, utils/compile.py:190-280). */
 int b200_lm_set_graph(b200_lm* h, int enable);
+/* How the depformer runs, chosen before b200_lm_streaming_begin (B200_ERR_STATE while streaming).  B200_DEPFORMER_AUTO (default):
+ * one persistent cooperative kernel per frame from three sessions on, a launch chain of GEMVs at one or two, and a launch chain
+ * of tensor-core GEMMs under classifier-free guidance or int8 linears.  B200_DEPFORMER_CHAIN: always the launch chain.
+ * B200_DEPFORMER_FUSED: the persistent kernel wherever it can run, at any batch.  Every mode computes what the reference does. */
+#define B200_DEPFORMER_AUTO 0
+#define B200_DEPFORMER_CHAIN 1
+#define B200_DEPFORMER_FUSED 2
+int b200_lm_set_depformer(b200_lm* h, int mode);
 /* Storage type of the temporal KV rings, chosen before b200_lm_streaming_begin.  B200_KV_BF16 (default) is the
  * reference's ring (RingKVCache, transformer.py:196-288: 1.573 GB per session at context 3000).  B200_KV_FP8_E4M3 is
  * an opt-in extension outside the reference's numerics (SURVEY.md 8f item 3): e4m3 bytes plus one fp32 scale per
@@ -467,6 +475,14 @@ int b200_op_set_gemv_max_rows(int max_rows);
  * the linear would return for the shape. */
 int b200_op_linear_plan(int M, int N, int K, int epi, int gate_rows, int int8, int norm, int sms, int gemv_max_rows, int64_t* out,
                         int capacity);
+/* The depformer path the LM plans at streaming_begin (needs no GPU): `batch` sessions, cfg = classifier-free guidance on, int8 =
+ * quantize=True, mode as b200_lm_set_depformer, for a device of `sms` multiprocessors and GEMV path up to `gemv_max_rows` rows.
+ * out[0] = path (0 none: dep_q = 0, 1 launch chain, 2 persistent kernel); for the kernel out[1..5] = partial-buffer floats,
+ * stages, stage bytes, dynamic shared memory, grid, then 6 values per GEMM phase (in_proj, out_proj, linear_in, linear_out,
+ * head): weight tiles, k-blocks, k-blocks per split, splits, accumulators, output columns; 0 elsewhere.  `capacity` int64 slots
+ * at out, at least 36.  B200_ERR_INVALID for out-of-range input and for a configuration the kernel refuses. */
+int b200_op_depformer_plan(int dep_q, int depformer_dim, int depformer_num_heads, int depformer_ffn_hidden, int card, int batch,
+                           int cfg, int int8, int mode, int sms, int gemv_max_rows, int64_t* out, int capacity);
 /* int8 x int8 linear (QLinear, utils/quantize.py:13-40: bitsandbytes row-wise absmax quantisation of weights and
  * activations, int32 accumulation, dequantisation by both row scales / 127^2), on wgmma s8 x s8 -> s32.
  *   b200_op_quant_pack_tiles: w bf16 [N,K] -> int8 SWIZZLE_128B tiles (b200_op_packed_bytes_i8 bytes) + scales f32 [N]

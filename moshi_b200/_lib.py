@@ -14,6 +14,7 @@ LIB_PATH = Path(__file__).resolve().parent / "_C" / "libmoshi_b200.so"
 
 B200_OK, B200_ERR_INVALID, B200_ERR_SHAPE, B200_ERR_STATE, B200_ERR_CUDA, B200_ERR_MISSING = range(6)
 B200_F32, B200_BF16, B200_F16, B200_I64, B200_U8, B200_I8 = range(6)
+B200_DEPFORMER_AUTO, B200_DEPFORMER_CHAIN, B200_DEPFORMER_FUSED = range(3)     # b200_lm_set_depformer
 ABI_VERSION = 2
 
 
@@ -100,6 +101,7 @@ _PROTOTYPES: dict[str, tuple[tp.Any, list]] = {
     "b200_lm_algorithmic_bytes": (C.c_int64, [_P, _I]),
     "b200_lm_assume_fill": (_I, [_P, _I]),
     "b200_lm_set_graph": (_I, [_P, _I]),
+    "b200_lm_set_depformer": (_I, [_P, _I]),
     "b200_lm_set_kv_dtype": (_I, [_P, _I]),
     "b200_lm_set_kv_capacity": (_I, [_P, _I]),
     "b200_lm_set_kv_pool": (_I, [_P, C.c_int64, _I]),
@@ -139,6 +141,7 @@ _PROTOTYPES: dict[str, tuple[tp.Any, list]] = {
     "b200_op_linear_ns": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
     "b200_op_set_gemv_max_rows": (_I, [_I]),
     "b200_op_linear_plan": (_I, [_I, _I, _I, _I, _I, _I, _I, _I, _I, C.POINTER(C.c_int64), _I]),
+    "b200_op_depformer_plan": (_I, [_I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, C.POINTER(C.c_int64), _I]),
     "b200_op_packed_bytes_i8": (C.c_int64, [_I, _I, _I, _I]),
     "b200_op_quant_pack_tiles": (_I, [_P, _P, _P, _I, _I, _I, _I, _P]),
     "b200_op_quantize_rows": (_I, [_P, _P, _P, _I, _I, _P]),

@@ -43,44 +43,12 @@ constexpr int MAX_STAGES = 8;
 constexpr int DD = 64;                       // depformer head dim
 static_assert(THREADS == lm::SAMPLE_THREADS, "sample_row needs a SAMPLE_THREADS-wide CTA");
 
-struct Gemm {                                // one GEMM phase
-  const uint8_t* wt;                         // packed tiles [n_tile][kb][A][16 KB]
-  int n_tiles, num_kb, kbps, S, A, N;        // S splits of kbps k-blocks; N = output columns per accumulator
-};
-
 using namespace tcp;
 __device__ __forceinline__ unsigned ld_acquire(const unsigned* p) {
   unsigned v;
   asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
   return v;
 }
-
-}  // namespace
-
-struct DepLayerW { const uint8_t *in_w, *out_w, *lin_in, *lin_out; };
-struct DepParams {
-  int B, Mpad, dd, H, F, card, text_card, dep_q, L, n_tables;
-  int* err;                                                  // device error flags (lm::ERR_*)
-  int stages; uint32_t stage_bytes;
-  Gemm g_in, g_out, g_lin_in, g_lin_out, g_head;              // shapes (wt filled per (k, l) from the tables below)
-  const DepLayerW* w;                                        // [dep_q][L] packed weight pointers (device)
-  const uint8_t* const* heads;                               // [dep_q]
-  const bf16* const* tables;                                 // [dep_q] embedding tables ([0] = text)
-  const bf16* const* n1; const bf16* const* n2;              // [L] RMSNorm alphas
-  const bf16* din; long long din_ld;                         // depformer_in_all output [B][dep_q*dd]
-  const long long* text_token;                               // [B]
-  bf16 *x, *xn, *ao, *hbuf;                                  // [B][dd] x3, [B][F]
-  bf16* const* kc; bf16* const* vc;                          // [L] per-frame KV [B][H][dep_q][64]
-  float *part0, *part1;                                      // split partials [S][B][Nmax]
-  bf16* logits;                                              // [dep_q][B][card]
-  long long* audio_tokens;                                   // [dep_q][B]
-  const float* noise; long long noise_ld; int noise_off, ka; // Exp(1) noise, row stride, offset of sub-step 0, per-step width
-  int use_sampling, top_k; float temp;
-  unsigned* bar;                                             // grid barrier counter (zero at launch)
-  unsigned long long* trace;                                 // optional [DEP_TRACE_SLOTS]: %globaltimer of CTA 0 after every grid barrier
-};
-
-namespace {
 
 struct Pipe { int s; uint32_t ph; int pre; };   // per-role pipeline cursor, carried across phases
 // (pre: producer only — stages of the upcoming GEMM phase whose weight copy is already in flight)
@@ -451,6 +419,39 @@ Gemm plan(int N, int K, int A, int M, int grid) {
 
 }  // namespace
 
+int plan_depformer(int dep_q, int dd, int H, int F, int card, int B, bool cfg, bool i8, int sms, int gemv_max_m, int mode,
+                   DepformerPlan* out) {
+  if (!out || dep_q < 0 || dep_q > lm::DEP_MAX_Q || (dep_q > 0 && (dd < 1 || H < 1 || F < 1 || card < 1)) || B < 1 ||
+      (cfg ? 2 * B : B) > 256 || sms < 1 || gemv_max_m < 0 || gemv_max_m > 4 || mode < B200_DEPFORMER_AUTO || mode > B200_DEPFORMER_FUSED)
+    B200_FAIL(B200_ERR_INVALID, "depformer plan: dep_q %d, dd %d, %d sessions, %d SMs, GEMV rows %d, mode %d out of range", dep_q, dd, B,
+              sms, gemv_max_m, mode);
+  DepformerPlan& P = *out;
+  memset(&P, 0, sizeof(P));
+  P.path = dep_q == 0 ? DEP_NONE : DEP_CHAIN;
+  // One or two sessions: the depformer's linears take the GEMV path and the PDL-chained launches beat the persistent kernel
+  // (a grid barrier per phase costs more than the launch it saves); B200_DEPFORMER_FUSED takes the kernel at any batch.  Under
+  // classifier-free guidance the two halves of the batch meet before every sampler (lm.py:828-833), and the kernel has no int8
+  // GEMM phases: launch chain.  Its row phases hold dd <= 4 * THREADS in registers.
+  if (dep_q == 0 || mode == B200_DEPFORMER_CHAIN || cfg || i8 || (B <= gemv_max_m && mode != B200_DEPFORMER_FUSED) || dd > 4 * THREADS ||
+      dd % 64)
+    return B200_OK;
+  if (dd / H != DD || F % 8) B200_FAIL(B200_ERR_INVALID, "fused depformer: unsupported configuration");
+  P.stage_bytes = 2 * TILE_BYTES + MC * BLOCK_K * 2;
+  P.stages = std::min((200 * 1024) / P.stage_bytes, MAX_STAGES);
+  if (P.stages < 2) B200_FAIL(B200_ERR_INVALID, "fused depformer: batch too large for the stage ring");
+  P.path = DEP_FUSED;
+  P.grid = sms;
+  P.g_in = plan(3 * dd, dd, 1, B, sms);
+  P.g_out = plan(dd, dd, 1, B, sms);
+  P.g_lin_in = plan(F, dd, 2, B, sms);
+  P.g_lin_out = plan(dd, F, 1, B, sms);
+  P.g_head = plan(card, dd, 1, B, sms);
+  for (const Gemm* g : {&P.g_in, &P.g_out, &P.g_lin_in, &P.g_lin_out, &P.g_head})
+    P.part_floats = std::max(P.part_floats, (long long)g->S * B * g->N);
+  P.smem = P.stages * P.stage_bytes + 1024 + 16 * MAX_STAGES + 64;
+  return B200_OK;
+}
+
 // ---- host side -------------------------------------------------------------------------------------------------------
 struct DepFused {
   DepParams p;
@@ -459,75 +460,38 @@ struct DepFused {
   void* dev_tables = nullptr;     // one allocation holding the pointer tables
 };
 
-size_t dep_fused_partial_floats(const DepFusedConfig& c) {
-  const int grid = num_sms();
-  size_t mx = 0;
-  const Gemm gs[5] = {plan(3 * c.dd, c.dd, 1, c.B, grid), plan(c.dd, c.dd, 1, c.B, grid), plan(c.F, c.dd, 2, c.B, grid),
-                      plan(c.dd, c.F, 1, c.B, grid), plan(c.card, c.dd, 1, c.B, grid)};
-  for (const Gemm& g : gs) {
-    const size_t n = (size_t)g.S * c.B * g.N;
-    if (n > mx) mx = n;
-  }
-  return mx;
-}
-
-int dep_fused_create(const DepFusedConfig& c, DepFused** out) {
-  if (c.dd % 64 || c.dd > 4 * THREADS || c.dd / c.H != DD || c.dep_q > lm::DEP_MAX_Q || c.dep_q < 1 || c.F % 8 || c.B < 1 || c.B > 256)
-    B200_FAIL(B200_ERR_INVALID, "fused depformer: unsupported configuration");
+int dep_fused_create(const DepformerPlan& P, const DepParams& host, DepFused** out) {
+  if (P.path != DEP_FUSED) B200_FAIL(B200_ERR_INVALID, "fused depformer: the plan takes another path");
   DepFused* d = new DepFused();
   DepParams& p = d->p;
-  memset(&p, 0, sizeof(p));
-  d->grid = num_sms();
-  p.B = c.B; p.Mpad = ((c.B + 15) / 16) * 16; p.dd = c.dd; p.H = c.H; p.F = c.F; p.card = c.card; p.text_card = c.text_card; p.err = c.err; p.dep_q = c.dep_q; p.L = c.L;
-  p.stage_bytes = (uint32_t)(2 * TILE_BYTES + MC * BLOCK_K * 2);
-  int stages = (200 * 1024) / (int)p.stage_bytes;
-  if (stages > MAX_STAGES) stages = MAX_STAGES;
-  if (stages < 2) { delete d; B200_FAIL(B200_ERR_INVALID, "fused depformer: batch too large for the stage ring"); }
-  p.stages = stages;
-  p.g_in = plan(3 * c.dd, c.dd, 1, c.B, d->grid);
-  p.g_out = plan(c.dd, c.dd, 1, c.B, d->grid);
-  p.g_lin_in = plan(c.F, c.dd, 2, c.B, d->grid);
-  p.g_lin_out = plan(c.dd, c.F, 1, c.B, d->grid);
-  p.g_head = plan(c.card, c.dd, 1, c.B, d->grid);
+  p = host;
+  d->grid = P.grid;
+  p.Mpad = ((p.B + 15) / 16) * 16;
+  p.stages = P.stages; p.stage_bytes = (uint32_t)P.stage_bytes;
+  p.g_in = P.g_in; p.g_out = P.g_out; p.g_lin_in = P.g_lin_in; p.g_lin_out = P.g_lin_out; p.g_head = P.g_head;
   // pointer tables -> one device allocation
-  const size_t n_w = (size_t)c.dep_q * c.L;
-  const size_t bytes = n_w * sizeof(DepLayerW) + (size_t)c.dep_q * 8 * 2 + (size_t)c.L * 8 * 4;
-  std::vector<uint8_t> host(bytes);
-  uint8_t* hp = host.data();
-  size_t off = 0;
-  auto put = [&](const void* src, size_t n) { memcpy(hp + off, src, n); const size_t o = off; off += n; return o; };
-  std::vector<DepLayerW> w(n_w);
-  for (size_t i = 0; i < n_w; ++i) w[i] = DepLayerW{(const uint8_t*)c.in_w[i], (const uint8_t*)c.out_w[i], (const uint8_t*)c.lin_in[i], (const uint8_t*)c.lin_out[i]};
-  const size_t o_w = put(w.data(), n_w * sizeof(DepLayerW));
-  const size_t o_heads = put(c.heads, (size_t)c.dep_q * 8);
-  const size_t o_tables = put(c.tables, (size_t)c.dep_q * 8);
-  const size_t o_n1 = put(c.n1, (size_t)c.L * 8);
-  const size_t o_n2 = put(c.n2, (size_t)c.L * 8);
-  const size_t o_kc = put(c.kc, (size_t)c.L * 8);
-  const size_t o_vc = put(c.vc, (size_t)c.L * 8);
-  if (cudaMalloc(&d->dev_tables, bytes) != cudaSuccess) { delete d; B200_FAIL(B200_ERR_CUDA, "fused depformer: cudaMalloc failed"); }
-  B200_CUDA(cudaMemcpy(d->dev_tables, hp, bytes, cudaMemcpyHostToDevice));
+  const size_t nq = (size_t)p.dep_q * 8, nl = (size_t)p.L * 8;
+  const void* src[7] = {host.w, host.heads, host.tables, host.n1, host.n2, host.kc, host.vc};
+  const size_t n[7] = {p.dep_q * p.L * sizeof(DepLayerW), nq, nq, nl, nl, nl, nl};
+  size_t off[8] = {0};
+  for (int i = 0; i < 7; ++i) off[i + 1] = off[i] + n[i];
+  std::vector<uint8_t> hp(off[7]);
+  for (int i = 0; i < 7; ++i) memcpy(hp.data() + off[i], src[i], n[i]);
+  if (cudaMalloc(&d->dev_tables, off[7]) != cudaSuccess) { delete d; B200_FAIL(B200_ERR_CUDA, "fused depformer: cudaMalloc failed"); }
+  B200_CUDA(cudaMemcpy(d->dev_tables, hp.data(), off[7], cudaMemcpyHostToDevice));
   uint8_t* dv = static_cast<uint8_t*>(d->dev_tables);
-  p.w = reinterpret_cast<const DepLayerW*>(dv + o_w);
-  p.heads = reinterpret_cast<const uint8_t* const*>(dv + o_heads);
-  p.tables = reinterpret_cast<const bf16* const*>(dv + o_tables);
-  p.n1 = reinterpret_cast<const bf16* const*>(dv + o_n1);
-  p.n2 = reinterpret_cast<const bf16* const*>(dv + o_n2);
-  p.kc = reinterpret_cast<bf16* const*>(dv + o_kc);
-  p.vc = reinterpret_cast<bf16* const*>(dv + o_vc);
-  p.din = static_cast<const bf16*>(c.din); p.din_ld = c.din_ld;
-  p.text_token = c.text_token;
-  p.x = static_cast<bf16*>(c.x); p.xn = static_cast<bf16*>(c.xn); p.ao = static_cast<bf16*>(c.ao); p.hbuf = static_cast<bf16*>(c.hbuf);
-  p.part0 = c.part0; p.part1 = c.part1;
-  p.logits = static_cast<bf16*>(c.logits); p.audio_tokens = c.audio_tokens;
-  p.noise = c.noise; p.noise_ld = c.noise_ld; p.noise_off = c.noise_off; p.ka = c.ka;
-  p.use_sampling = c.use_sampling; p.top_k = c.top_k; p.temp = c.temp;
-  p.bar = c.bar; p.trace = c.trace;
-  B200_TRY(act_map(&d->map_xn, c.xn, c.dd, c.B, c.dd, MC, 2));
-  B200_TRY(act_map(&d->map_ao, c.ao, c.dd, c.B, c.dd, MC, 2));
-  B200_TRY(act_map(&d->map_h, c.hbuf, c.F, c.B, c.F, MC, 2));
-  B200_TRY(act_map(&d->map_x, c.x, c.dd, c.B, c.dd, MC, 2));
-  d->smem = (size_t)stages * p.stage_bytes + 1024 + 16 * MAX_STAGES + 64;
+  p.w = reinterpret_cast<const DepLayerW*>(dv + off[0]);
+  p.heads = reinterpret_cast<const uint8_t* const*>(dv + off[1]);
+  p.tables = reinterpret_cast<const bf16* const*>(dv + off[2]);
+  p.n1 = reinterpret_cast<const bf16* const*>(dv + off[3]);
+  p.n2 = reinterpret_cast<const bf16* const*>(dv + off[4]);
+  p.kc = reinterpret_cast<bf16* const*>(dv + off[5]);
+  p.vc = reinterpret_cast<bf16* const*>(dv + off[6]);
+  B200_TRY(act_map(&d->map_xn, p.xn, p.dd, p.B, p.dd, MC, 2));
+  B200_TRY(act_map(&d->map_ao, p.ao, p.dd, p.B, p.dd, MC, 2));
+  B200_TRY(act_map(&d->map_h, p.hbuf, p.F, p.B, p.F, MC, 2));
+  B200_TRY(act_map(&d->map_x, p.x, p.dd, p.B, p.dd, MC, 2));
+  d->smem = (size_t)P.smem;
   B200_CUDA(cudaFuncSetAttribute(dep_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
   int per_sm = 0, coop = 0, dev = 0;
   B200_CUDA(cudaGetDevice(&dev));

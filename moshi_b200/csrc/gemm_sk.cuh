@@ -111,29 +111,48 @@ int sk_quantize_rows(const __nv_bfloat16* x, long long ldx, void* xq, float* sa,
 constexpr int SK_MAX_GRID = 304;     // 2 CTAs per SM at most
 constexpr int SK_MAX_TILES = 1024;   // ints in the arrival-counter array
 
-// ---- the depformer of one frame as one persistent kernel (dep_fused.cu) ---------------------------
-struct DepFusedConfig {
-  int B, dd, H, F, card, text_card, dep_q, L;
-  int* err;                                        // device error flags (lm::ERR_*), may be null
-  const void* const* in_w; const void* const* out_w; const void* const* lin_in; const void* const* lin_out;   // [dep_q*L] packed tiles
-  const void* const* heads;        // [dep_q] packed tiles
-  const void* const* tables;       // [dep_q] embedding tables (bf16 [V][dd]); [0] = text
-  const void* const* n1; const void* const* n2;   // [L] RMSNorm alphas (bf16 [dd])
-  void* const* kc; void* const* vc;               // [L] KV [B][H][dep_q][64] bf16
-  const void* din; long long din_ld;              // depformer_in_all output, bf16 [B][dep_q*dd]
-  const long long* text_token;
-  void *x, *xn, *ao, *hbuf;                       // bf16 [B][dd] x3, [B][F]
-  float *part0, *part1;                           // dep_fused_partial_floats() floats each
-  void* logits; long long* audio_tokens;          // bf16 [dep_q][B][card], i64 [dep_q][B]
-  const float* noise; long long noise_ld; int noise_off, ka;
+// ---- the depformer of one frame: its plan and the persistent kernel (dep_fused.cu) ---------------------------
+struct Gemm {                                      // one GEMM phase of the persistent kernel
+  const uint8_t* wt;                               // packed tiles [n_tile][kb][A][16 KB] (filled per sub-step and layer)
+  int n_tiles, num_kb, kbps, S, A, N;              // S splits of kbps k-blocks; N = output columns per accumulator
+};
+enum DepPath { DEP_NONE = 0, DEP_CHAIN = 1, DEP_FUSED = 2 };
+struct DepformerPlan {
+  int path;                                        // DEP_NONE: dep_q = 0; DEP_CHAIN: one launch per kernel; DEP_FUSED
+  Gemm g_in, g_out, g_lin_in, g_lin_out, g_head;   // DEP_FUSED: the five GEMM phases
+  long long part_floats;                           // floats of each of the two split-partial buffers
+  int stages, stage_bytes, smem, grid;
+};
+// Pure host function (no CUDA call).  mode: B200_DEPFORMER_AUTO / _CHAIN / _FUSED; B sessions (2B model rows under cfg).
+int plan_depformer(int dep_q, int dd, int H, int F, int card, int B, bool cfg, bool i8, int sms, int gemv_max_m, int mode,
+                   DepformerPlan* plan);
+
+struct DepLayerW { const uint8_t *in_w, *out_w, *lin_in, *lin_out; };
+struct DepParams {
+  int B, Mpad, dd, H, F, card, text_card, dep_q, L, n_tables;
+  int* err;                                                  // device error flags (lm::ERR_*)
+  int stages; uint32_t stage_bytes;
+  Gemm g_in, g_out, g_lin_in, g_lin_out, g_head;              // shapes (wt filled per (k, l) from the tables below)
+  const DepLayerW* w;                                        // [dep_q][L] packed weight pointers (device)
+  const uint8_t* const* heads;                               // [dep_q]
+  const __nv_bfloat16* const* tables;                        // [dep_q] embedding tables ([0] = text)
+  const __nv_bfloat16* const* n1; const __nv_bfloat16* const* n2;   // [L] RMSNorm alphas
+  const __nv_bfloat16* din; long long din_ld;                // depformer_in_all output [B][dep_q*dd]
+  const long long* text_token;                               // [B]
+  __nv_bfloat16 *x, *xn, *ao, *hbuf;                         // [B][dd] x3, [B][F]
+  __nv_bfloat16* const* kc; __nv_bfloat16* const* vc;        // [L] per-frame KV [B][H][dep_q][64]
+  float *part0, *part1;                                      // split partials [S][B][Nmax]
+  __nv_bfloat16* logits;                                     // [dep_q][B][card]
+  long long* audio_tokens;                                   // [dep_q][B]
+  const float* noise; long long noise_ld; int noise_off, ka; // Exp(1) noise, row stride, offset of sub-step 0, per-step width
   int use_sampling, top_k; float temp;
-  unsigned* bar;
-  unsigned long long* trace;                       // optional [DEP_TRACE_SLOTS] barrier timestamps of CTA 0 (diagnostics), may be null
+  unsigned* bar;                                             // grid barrier counter (zero at launch)
+  unsigned long long* trace;                                 // optional [DEP_TRACE_SLOTS]: %globaltimer of CTA 0 after every grid barrier
 };
 constexpr int DEP_TRACE_SLOTS = 512;
 struct DepFused;
-size_t dep_fused_partial_floats(const DepFusedConfig& c);
-int dep_fused_create(const DepFusedConfig& c, DepFused** out);
+// p: every field but the plan's, its pointer tables (w .. n2, kc, vc) on the host; they are copied to the device
+int dep_fused_create(const DepformerPlan& plan, const DepParams& p, DepFused** out);
 void dep_fused_set_sampling(DepFused* d, int use_sampling, float temp, int top_k);
 void dep_fused_destroy(DepFused* d);
 int dep_fused_launch(DepFused* d, cudaStream_t stream);

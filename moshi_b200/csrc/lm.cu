@@ -17,12 +17,6 @@ struct TLayer {
   const bf16 *ncw = nullptr, *ncb = nullptr, *cq_w = nullptr, *ckv_w = nullptr, *co_w = nullptr;
   bf16 *kx = nullptr, *vx = nullptr;
 };
-struct DLayer {
-  std::vector<const bf16*> in_w, out_w, lin_in, lin_out;   // one per depformer step
-  std::vector<const float*> in_s, out_s, lin_in_s, lin_out_s;   // int8 path: weight-row scales
-  const bf16 *n1, *n2;
-  bf16 *kc = nullptr, *vc = nullptr;
-};
 
 }  // namespace
 
@@ -332,6 +326,106 @@ struct TemporalKv {
 
 }  // namespace
 
+// ---- depformer ----------------------------------------------------------------------------------------------------------------
+// The depformer (lm.py:450-493, 809-850): weights, per-batch buffers, the path a batch takes (tc::plan_depformer: none, the launch
+// chain or the persistent kernel of dep_fused.cu) and where each sub-step's Exp(1) draws start in a noise row.  Its allocations
+// keep their place in streaming_begin's order (begin, alloc_guided, alloc_activations, and alloc_fused after linear_init).
+namespace {
+
+struct Depformer {
+  // sub-step k of layer l: packed tiles, and under int8 their weight-row scales
+  struct Step { const bf16 *in_w, *out_w, *lin_in, *lin_out; const float *in_s, *out_s, *lin_in_s, *lin_out_s; };
+  // configuration
+  int dep_q = 0, dd = 0, H = 0, F = 0, L = 0, card = 0, text_card = 0;
+  int mode = B200_DEPFORMER_AUTO;              // b200_lm_set_depformer, before streaming_begin
+  int kt = 0, ka = 0;                          // Exp(1) draws per noise row of the text sampler, and of each sub-step's
+  // weights
+  const bf16* in_all = nullptr;                // depformer_in.{k} stacked: all dep_q projections of transformer_out are one GEMM
+  const float* in_s = nullptr;
+  std::vector<Step> w;                         // [dep_q][L]
+  std::vector<const bf16*> n1, n2;             // [L]
+  std::vector<const bf16*> tables;             // [0] = depformer_text_emb, [k] = depformer_emb[k-1]
+  std::vector<const bf16*> heads; std::vector<const float*> heads_s;    // linears[k]
+  // per batch
+  tc::DepformerPlan plan{};
+  int B = 0, MB = 0;
+  bf16 *din = nullptr, *dx = nullptr, *dxn = nullptr, *dqkv = nullptr, *dao = nullptr, *dh = nullptr;
+  bf16 *logits = nullptr, *logits_cfg = nullptr;       // [dep_q][MB][card], under CFG the guided [dep_q][B][card]
+  std::vector<bf16*> kc, vc;                   // [L] the frame's K / V [MB][H][dep_q][64]
+  float *part0 = nullptr, *part1 = nullptr;    // the persistent kernel's split partials, its grid barrier ...
+  unsigned* bar = nullptr;
+  unsigned long long* trace = nullptr;         // ... and (B200_DEP_TRACE=1, diagnostics) its barrier timestamps
+  tc::DepFused* fused = nullptr;
+
+  void configure(const b200_lm_config& c) {
+    dep_q = c.dep_q; dd = c.depformer_dim; H = c.depformer_num_heads; F = c.depformer_ffn_hidden;
+    L = c.dep_q > 0 ? c.depformer_num_layers : 0; card = c.card; text_card = c.text_card;
+  }
+  // where sub-step k's draws start in a noise row (k = dep_q: the row's length)
+  long long noise_at(int k) const { return kt + (long long)k * ka; }
+  void set_sampling(int use_sampling, float temp, int top_k, int top_k_text) {
+    kt = std::min(top_k_text, text_card);
+    ka = std::min(top_k, card);
+    tc::dep_fused_set_sampling(fused, use_sampling, temp, top_k);
+  }
+  // streaming_begin: the plan of `batch` sessions, and the frame's K / V
+  int begin(Arena& A, int batch, bool cfg, bool i8) {
+    B = batch;
+    MB = cfg ? 2 * batch : batch;
+    B200_TRY(tc::plan_depformer(dep_q, dd, H, F, card, B, cfg, i8, num_sms(), tc::sk_gemv_max_m(), mode, &plan));
+    kc = vc = std::vector<bf16*>(L);
+    for (int l = 0; l < L; ++l) {
+      B200_TRY(A.alloc_t(&kc[l], (size_t)MB * dd * dep_q));
+      B200_TRY(A.alloc_t(&vc[l], (size_t)MB * dd * dep_q));
+    }
+    return B200_OK;
+  }
+  int alloc_guided(Arena& A) { return A.alloc_t(&logits_cfg, (size_t)B * std::max(dep_q, 1) * card); }
+  int alloc_activations(Arena& A) {
+    const size_t q1 = std::max(dep_q, 1);
+    B200_TRY(A.alloc_t(&din, (size_t)MB * q1 * dd));
+    B200_TRY(A.alloc_t(&dx, (size_t)MB * dd));
+    B200_TRY(A.alloc_t(&dxn, (size_t)MB * dd));
+    B200_TRY(A.alloc_t(&dqkv, (size_t)MB * 3 * dd));
+    B200_TRY(A.alloc_t(&dao, (size_t)MB * dd));
+    B200_TRY(A.alloc_t(&dh, (size_t)MB * F));
+    return A.alloc_t(&logits, (size_t)MB * q1 * card);
+  }
+  int alloc_fused(b200_lm* h);
+  int load(b200_lm* h);
+  int run(b200_lm* h, bool replace);
+  void end() {
+    tc::dep_fused_destroy(fused);
+    fused = nullptr; plan = tc::DepformerPlan{}; B = MB = 0; kc.clear(); vc.clear();
+    din = dx = dxn = dqkv = dao = dh = logits = logits_cfg = nullptr; part0 = part1 = nullptr; bar = nullptr; trace = nullptr;
+  }
+
+  // b200_lm_read_buffer's depformer entries; false for any other name
+  bool buffer(const std::string& n, bool cfg, const void** src, int64_t* sz) const {
+    // with CFG "dep_logits" are what the samplers read (the guided rows, lm.py:828-833), "model_dep_logits" the model's 2B rows
+    if (n == "dep_logits") { *src = cfg ? logits_cfg : logits; *sz = (int64_t)dep_q * B * card * 2; }
+    else if (n == "model_dep_logits") { *src = logits; *sz = (int64_t)dep_q * MB * card * 2; }
+    else if (n == "dep_trace") { *src = trace; *sz = trace ? (int64_t)tc::DEP_TRACE_SLOTS * 8 : 0; }
+    else if (n == "dep_in" && dep_q > 0) { *src = din; *sz = (int64_t)MB * dep_q * dd * 2; }
+    else if (n.rfind("depformer.layers.", 0) == 0 && dep_q > 0) {
+      // the per-frame cache of one layer: after a frame it holds every sub-step's k / v
+      const std::string rest = n.substr(17);
+      const size_t dot = rest.find('.');
+      const std::string idx = rest.substr(0, dot), kind = dot == std::string::npos ? "" : rest.substr(dot + 1);
+      const bool digits = !idx.empty() && idx.size() <= 4 && idx.find_first_not_of("0123456789") == std::string::npos;
+      const int l = digits ? atoi(idx.c_str()) : -1;
+      if (l < 0 || l >= L || (kind != "k" && kind != "v")) return false;
+      *src = kind == "k" ? kc[l] : vc[l];
+      *sz = (int64_t)MB * dd * dep_q * 2;
+    } else {
+      return false;
+    }
+    return true;
+  }
+};
+
+}  // namespace
+
 struct b200_lm : StreamCore {       // batch: sessions (LMGen batch); graphs[0]: the step
   b200_lm_config cfg;
   TensorStore store;
@@ -347,14 +441,9 @@ struct b200_lm : StreamCore {       // batch: sessions (LMGen batch); graphs[0]:
   // weights
   EmbedTables emb;
   std::vector<TLayer> layers;
-  std::vector<DLayer> dlayers;
   const bf16 *out_norm = nullptr, *text_linear = nullptr;
-  const float *text_linear_s = nullptr, *dep_in_s = nullptr;
-  std::vector<const float*> dep_heads_s;
+  const float* text_linear_s = nullptr;
   int8_t* xq = nullptr; float* xq_scale = nullptr;     // int8 path: the current GEMM's quantised activations [B][max K] and row scales
-  bf16* dep_in_all = nullptr;                  // [dep_q * dd][dim]
-  std::vector<const bf16*> dep_tables;         // [0] = depformer_text_emb, [k] = depformer_emb[k-1]
-  std::vector<const bf16*> dep_heads;          // linears[k]
   int* delays_dev = nullptr;
   // state
   long long *cache = nullptr, *offsets = nullptr, *pos = nullptr;
@@ -364,7 +453,7 @@ struct b200_lm : StreamCore {       // batch: sessions (LMGen batch); graphs[0]:
   // classifier-free guidance (lm.py:596-604, 714-732, 820-833) and conditioning by sum (lm.py:398-399, 616-626)
   float cfg_coef = 1.f; int cfg_is_no_text = 0;
   std::vector<long long> cfg_until_host; long long* cfg_until = nullptr;
-  bf16 *text_logits_cfg = nullptr, *dep_logits_cfg = nullptr;       // guided logits [batch][card] / [dep_q][batch][card]
+  bf16* text_logits_cfg = nullptr;             // guided logits [batch][text_card]
   bf16* cond_sum = nullptr; int cond_on = 0;                          // [MB][dim]
   // extra heads of the STT models (lm.py:224-226, 793-807)
   std::vector<const bf16*> extra_w; const bf16** extra_w_dev = nullptr; bf16* extra_out = nullptr;
@@ -374,20 +463,15 @@ struct b200_lm : StreamCore {       // batch: sessions (LMGen batch); graphs[0]:
   long long *in_codes = nullptr, *input_tokens = nullptr, *text_token = nullptr, *audio_tokens = nullptr, *out_tokens = nullptr;
   float* noise = nullptr;
   bf16 *x = nullptr, *xn = nullptr, *qkv = nullptr, *ao = nullptr, *hbuf = nullptr, *tout = nullptr;
-  bf16 *text_logits = nullptr, *din = nullptr, *dx = nullptr, *dxn = nullptr, *dqkv = nullptr, *dao = nullptr,
-       *dh = nullptr, *dep_logits = nullptr;
+  bf16* text_logits = nullptr;
   float* attn_part = nullptr;
   int* attn_counters = nullptr;                // split arrival counters [B*H]
-  tc::DepFused* depf = nullptr;                // the depformer of a frame as one persistent kernel (B200_DEP_FUSED=0: off)
-  int dep_fused = 1;
+  Depformer dep;                               // the depformer: weights, buffers and the path it runs on
   TemporalKv kv;                               // the temporal K/V: rings or pool, their state entries and record section
   // session records: the per-session slices of the small state entries; the condition_sum rows come last and travel while it is on
   RowSlice* slices_dev = nullptr;
   int n_slices = 0, n_slices_cond = 0;
   long long slices_end = 0, slices_end_cond = 0, slices_max = 0;
-  float *dep_part0 = nullptr, *dep_part1 = nullptr;
-  unsigned* dep_bar = nullptr;
-  unsigned long long* dep_trace = nullptr;     // B200_DEP_TRACE=1: barrier timestamps of the fused depformer (diagnostics)
   int nsplit = 1;
   // b200_lm_set_taps: the step copies the temporal stack's activations into taps (see tap_slot), allocated on first enable
   int taps_on = 0;
@@ -429,11 +513,7 @@ int get_bf16(b200_lm* h, const std::string& name, std::vector<int64_t> shape, co
 
 bool cfg_on(const b200_lm* h) { return h->cfg_coef != 1.f; }
 
-int noise_per_row(const b200_lm* h) {
-  const int kt = h->top_k_text < h->cfg.text_card ? h->top_k_text : h->cfg.text_card;
-  const int ka = h->top_k < h->cfg.card ? h->top_k : h->cfg.card;
-  return kt + h->cfg.dep_q * ka;
-}
+int noise_per_row(const b200_lm* h) { return (int)h->dep.noise_at(h->cfg.dep_q); }
 
 // The plan of y[M][N] = epi(x[M][K] . w[N][K]^T) on this device; norm: an RMSNorm in front that may fold into the GEMV.
 int plan(const b200_lm* h, int M, int N, int K, int epi, int gate_rows, long long ldy, long long ldr, bool norm, tc::LinearPlan* out) {
@@ -486,47 +566,58 @@ int get_prequantised(b200_lm* h, const std::string& name, int rows, int K, const
   return B200_OK;
 }
 
-// Linear weight from the store -> packed tiles (gemm_sk.cu), which replace the row-major
-// tensor (which is released), so the 15.4 GB checkpoint is resident once.
-int get_linear(b200_lm* h, const std::string& name, int N, int K, int epi, int gate_rows, const bf16** out,
+// Linear weight from the store -> packed tiles (gemm_sk.cu), which replace the row-major tensors (which are released), so the
+// 15.4 GB checkpoint is resident once.  Several names: tensors of equal row counts stacked along N into one linear.
+int get_linear(b200_lm* h, const std::vector<std::string>& names, int N, int K, int epi, int gate_rows, const bf16** out,
                const float** scales_out) {
-  const int w_rows = epi == LIN_GATE ? 2 * gate_rows : N;
+  const int n = (int)names.size(), w_rows = epi == LIN_GATE ? 2 * gate_rows : N, rows = w_rows / n;
+  const Tensor* t = h->store.find(names[0]);
+  const bool pre = t && t->dtype == B200_I8;      // pre-quantised checkpoint: tile CB as it is, keep SCB
+  const size_t el = pre ? 1 : 2;
   *scales_out = nullptr;
-  void* packed = nullptr;
-  const Tensor* t = h->store.find(name);
-  if (t && t->dtype == B200_I8) {      // pre-quantised checkpoint: tile CB as it is, keep SCB
-    const int8_t* q = nullptr; const float* scb = nullptr;
-    B200_TRY(get_prequantised(h, name, w_rows, K, &q, &scb));
-    float* scales = nullptr;
-    B200_TRY(h->weights.alloc(&packed, tc::sk_packed_bytes_i8(N, K, epi, gate_rows), false));
-    B200_TRY(h->weights.alloc_t(&scales, (size_t)w_rows, false));
-    B200_TRY(tc::sk_pack_weights_i8(q, packed, N, K, epi, gate_rows, nullptr));
-    B200_CUDA(cudaMemcpy(scales, scb, (size_t)w_rows * 4, cudaMemcpyDeviceToDevice));
-    *scales_out = scales;
-    h->weight_bytes += (int64_t)w_rows * K + (int64_t)w_rows * 4;
-    B200_CUDA(cudaStreamSynchronize(nullptr));
-    h->store.release(name);
-    h->store.release(name + "_scb");
-    *out = static_cast<const bf16*>(packed);
-    return B200_OK;
+  struct Guard { void* p = nullptr; ~Guard() { cudaFree(p); } } stacked;      // several tensors: stacked here first
+  if (n > 1) B200_CUDA(cudaMalloc(&stacked.p, (size_t)w_rows * K * el));
+  float* scales = nullptr;
+  if (pre) B200_TRY(h->weights.alloc_t(&scales, (size_t)w_rows, false));
+  const void* w = nullptr;
+  for (int i = 0; i < n; ++i) {
+    if (pre) {
+      const int8_t* q = nullptr; const float* scb = nullptr;
+      if (!h->store.find(names[i])) B200_FAIL(B200_ERR_MISSING, "lm finalize: tensor '%s' was not loaded", names[i].c_str());
+      B200_TRY(get_prequantised(h, names[i], rows, K, &q, &scb));
+      B200_CUDA(cudaMemcpy(scales + (size_t)i * rows, scb, (size_t)rows * 4, cudaMemcpyDeviceToDevice));
+      w = q;
+    } else {
+      const bf16* b = nullptr;
+      B200_TRY(get_bf16(h, names[i], {rows, K}, &b));
+      w = b;
+    }
+    if (n > 1)
+      B200_CUDA(cudaMemcpy(static_cast<char*>(stacked.p) + (size_t)i * rows * K * el, w, (size_t)rows * K * el, cudaMemcpyDeviceToDevice));
   }
-  const bf16* w = nullptr;
-  B200_TRY(get_bf16(h, name, {w_rows, K}, &w));
-  if (h->cfg.quantize) {        // QLinear.__init__ (utils/quantize.py:16-21): row-wise absmax int8 of weight.to(float16)
-    float* scales = nullptr;
+  if (n > 1) w = stacked.p;
+  void* packed = nullptr;
+  if (pre) {
+    B200_TRY(h->weights.alloc(&packed, tc::sk_packed_bytes_i8(N, K, epi, gate_rows), false));
+    B200_TRY(tc::sk_pack_weights_i8(static_cast<const int8_t*>(w), packed, N, K, epi, gate_rows, nullptr));
+    h->weight_bytes += (int64_t)w_rows * K + (int64_t)w_rows * 4;
+  } else if (h->cfg.quantize) {        // QLinear.__init__ (utils/quantize.py:16-21): row-wise absmax int8 of weight.to(float16)
     B200_TRY(h->weights.alloc(&packed, tc::sk_packed_bytes_i8(N, K, epi, gate_rows), false));
     B200_TRY(h->weights.alloc_t(&scales, (size_t)w_rows, false));
-    B200_TRY(tc::sk_quant_pack_weights(w, packed, scales, N, K, epi, gate_rows, nullptr));
-    *scales_out = scales;
+    B200_TRY(tc::sk_quant_pack_weights(static_cast<const bf16*>(w), packed, scales, N, K, epi, gate_rows, nullptr));
     h->weight_bytes -= (int64_t)w_rows * K;        // one byte per weight instead of two (get_bf16 counted two) ...
     h->weight_bytes += (int64_t)w_rows * 4;        // ... plus the row scales
   } else {
     B200_TRY(h->weights.alloc(&packed, tc::sk_packed_bytes(N, K, epi, gate_rows), false));
-    B200_TRY(tc::sk_pack_weights(w, packed, N, K, epi, gate_rows, nullptr));
+    B200_TRY(tc::sk_pack_weights(static_cast<const bf16*>(w), packed, N, K, epi, gate_rows, nullptr));
   }
   B200_CUDA(cudaStreamSynchronize(nullptr));
-  h->store.release(name);
+  for (const std::string& name : names) {
+    h->store.release(name);
+    if (pre) h->store.release(name + "_scb");
+  }
   *out = static_cast<const bf16*>(packed);
+  *scales_out = scales;
   return B200_OK;
 }
 
@@ -591,11 +682,97 @@ int tap(b200_lm* h, const bf16* src, int layer, int kind) {
   return B200_OK;
 }
 
+// ---- depformer: loading and running ------------------------------------------------------------------------------------------
+int Depformer::load(b200_lm* h) {
+  if (dep_q == 0) return B200_OK;
+  std::vector<std::string> in_names;
+  for (int k = 0; k < dep_q; ++k) in_names.push_back("depformer_in." + std::to_string(k) + ".weight");
+  B200_TRY(get_linear(h, in_names, dep_q * dd, h->cfg.dim, LIN_STORE, 0, &in_all, &in_s));
+  tables.resize(dep_q); heads.resize(dep_q); heads_s.resize(dep_q); w.resize((size_t)dep_q * L); n1.resize(L); n2.resize(L);
+  B200_TRY(get_bf16(h, "depformer_text_emb.weight", {text_card + 1, dd}, &tables[0]));
+  for (int k = 1; k < dep_q; ++k)
+    B200_TRY(get_bf16(h, "depformer_emb." + std::to_string(k - 1) + ".weight", {card + 1, dd}, &tables[k]));
+  for (int k = 0; k < dep_q; ++k)
+    B200_TRY(get_linear(h, {"linears." + std::to_string(k) + ".weight"}, card, dd, LIN_STORE, 0, &heads[k], &heads_s[k]));
+  for (int l = 0; l < L; ++l) {
+    const std::string p = "depformer.layers." + std::to_string(l);
+    for (int k = 0; k < dep_q; ++k) {
+      const std::string ks = std::to_string(k);
+      Step& S = w[(size_t)k * L + l];
+      B200_TRY(get_linear(h, {p + ".self_attn.in_projs." + ks + ".weight"}, 3 * dd, dd, LIN_STORE, 0, &S.in_w, &S.in_s));
+      B200_TRY(get_linear(h, {p + ".self_attn.out_projs." + ks + ".weight"}, dd, dd, LIN_RESADD, 0, &S.out_w, &S.out_s));
+      B200_TRY(get_linear(h, {p + ".gating." + ks + ".linear_in.weight"}, 2 * F, dd, LIN_GATE, F, &S.lin_in, &S.lin_in_s));
+      B200_TRY(get_linear(h, {p + ".gating." + ks + ".linear_out.weight"}, dd, F, LIN_RESADD, 0, &S.lin_out, &S.lin_out_s));
+    }
+    B200_TRY(get_bf16(h, p + ".norm1.alpha", {1, 1, dd}, &n1[l]));
+    B200_TRY(get_bf16(h, p + ".norm2.alpha", {1, 1, dd}, &n2[l]));
+  }
+  return B200_OK;
+}
+
+// streaming_begin, after linear_init: the persistent kernel's buffers and the kernel itself, where the plan takes it
+int Depformer::alloc_fused(b200_lm* h) {
+  if (plan.path != tc::DEP_FUSED) return B200_OK;
+  Arena& A = h->state;
+  B200_TRY(A.alloc_t(&part0, (size_t)plan.part_floats, false));
+  B200_TRY(A.alloc_t(&part1, (size_t)plan.part_floats, false));
+  B200_TRY(A.alloc_t(&bar, 1));
+  if (const char* e = getenv("B200_DEP_TRACE")) {
+    if (atoi(e)) B200_TRY(A.alloc_t(&trace, (size_t)tc::DEP_TRACE_SLOTS));
+  }
+  std::vector<tc::DepLayerW> lw;
+  for (const Step& S : w)
+    lw.push_back({reinterpret_cast<const uint8_t*>(S.in_w), reinterpret_cast<const uint8_t*>(S.out_w),
+                  reinterpret_cast<const uint8_t*>(S.lin_in), reinterpret_cast<const uint8_t*>(S.lin_out)});
+  tc::DepParams p{};
+  p.B = B; p.dd = dd; p.H = H; p.F = F; p.card = card; p.text_card = text_card; p.dep_q = dep_q; p.L = L; p.err = h->err;
+  p.w = lw.data(); p.heads = reinterpret_cast<const uint8_t* const*>(heads.data()); p.tables = tables.data();
+  p.n1 = n1.data(); p.n2 = n2.data(); p.kc = kc.data(); p.vc = vc.data();
+  p.din = din; p.din_ld = (long long)dep_q * dd; p.text_token = h->text_token;
+  p.x = dx; p.xn = dxn; p.ao = dao; p.hbuf = dh; p.part0 = part0; p.part1 = part1;
+  p.logits = logits; p.audio_tokens = h->audio_tokens;
+  p.noise = h->noise; p.noise_ld = noise_at(dep_q); p.noise_off = (int)noise_at(0); p.ka = ka;
+  p.use_sampling = h->use_sampling; p.top_k = h->top_k; p.temp = h->temp;
+  p.bar = bar; p.trace = trace;
+  return tc::dep_fused_create(plan, p, &fused);
+}
+
+// The step from the depformer's input projection to the last sub-step's sampler (lm.py:809-850): fresh K / V every frame, all
+// rows advance together.  replace: depformer_replace_tokens (lm.py:751-755), the caller supplies this frame's audio tokens and the
+// depformer does not run; without a depformer (dep_q = 0, lm.py:219-222, "No-Depformer --- e.g., an ASR model") nothing runs.
+int Depformer::run(b200_lm* h, bool replace) {
+  cudaStream_t st = h->body;
+  if (replace || plan.path == tc::DEP_NONE) {
+    if (dep_q > 0) B200_LAUNCH(replace_audio_kernel, ceil_div(B * dep_q, 128), 128, 0, st, h->replace_tokens, h->audio_tokens, B, dep_q);
+    return B200_OK;
+  }
+  const int d = h->cfg.dim;
+  B200_TRY(linear(h, h->tout, d, in_all, din, (long long)dep_q * dd, nullptr, 0, MB, dep_q * dd, d, LIN_STORE, 0, in_s));
+  if (plan.path == tc::DEP_FUSED) return tc::dep_fused_launch(fused, st);
+  for (int k = 0; k < dep_q; ++k) {
+    const long long* prev = k == 0 ? h->text_token : h->audio_tokens + (long long)(k - 1) * B;
+    B200_LAUNCH(dep_input_kernel, ceil_div(MB * dd, 256), 256, 0, st, din, (long long)dep_q * dd, k * dd, tables[k], prev, dx, MB, dd, B,
+                k == 0 ? text_card : card, h->err);
+    for (int l = 0; l < L; ++l) {
+      const Step& S = w[(size_t)k * L + l];
+      B200_TRY(norm_linear(h, dx, n1[l], dxn, S.in_w, dqkv, 3 * dd, MB, 3 * dd, dd, LIN_STORE, 0, S.in_s));
+      B200_LAUNCH(dep_attn_step_kernel, ceil_div(MB * H * 32, 128), 128, 0, st, dqkv, kc[l], vc[l], dao, MB, H, dep_q, k);
+      B200_TRY(linear(h, dao, dd, S.out_w, dx, dd, dx, dd, MB, dd, dd, LIN_RESADD, 0, S.out_s));
+      B200_TRY(norm_linear(h, dx, n2[l], dxn, S.lin_in, dh, F, MB, F, dd, LIN_GATE, F, S.lin_in_s));
+      B200_TRY(linear(h, dh, F, S.lin_out, dx, dd, dx, dd, MB, dd, F, LIN_RESADD, 0, S.lin_out_s));
+    }
+    bf16* lg = logits + (long long)k * MB * card;
+    B200_TRY(linear(h, dx, dd, heads[k], lg, card, nullptr, 0, MB, card, dd, LIN_STORE, 0, heads_s[k]));
+    const bf16* gl = guide(h, lg, cfg_on(h) ? logits_cfg + (long long)k * B * card : nullptr, card, true);   // lm.py:828-833
+    B200_TRY(sample(h, gl, card, h->noise + noise_at(k), h->audio_tokens + (long long)k * B, h->temp, h->top_k));
+  }
+  return B200_OK;
+}
+
 // The whole frame as a fixed launch sequence over static buffers (captured into one CUDA graph).
 int step_body(b200_lm* h) {
   const auto& c = h->cfg;
   const int B = h->batch, MB = h->MB, d = c.dim, H = c.num_heads, F = c.ffn_hidden;
-  const int dd = c.depformer_dim, dH = c.depformer_num_heads, dF = c.depformer_ffn_hidden;
   cudaStream_t st = h->body;
 
   B200_LAUNCH(lm_prepare_kernel, ceil_div(B * h->Kc, 128), 128, 0, st, ring(h), h->in_codes, h->n_in_static,
@@ -643,39 +820,7 @@ int step_body(b200_lm* h) {
     B200_LAUNCH(extra_heads_kernel, ceil_div((int)h->extra_w.size() * MB * 32, 128), 128, 0, st, h->tout, h->extra_w_dev, h->extra_out, MB, d,
                 c.extra_heads_dim, (int)h->extra_w.size());
 
-  // Depformer (lm.py:809-850): fresh KV state every frame, all rows advance together.
-  const int kt = h->top_k_text < c.text_card ? h->top_k_text : c.text_card;
-  const int ka = h->top_k < c.card ? h->top_k : c.card;
-  if (h->replace_static || c.dep_q == 0) {
-    // depformer_replace_tokens (lm.py:751-755): the caller supplies this frame's audio tokens, the depformer does not run;
-    // dep_q == 0 (lm.py:219-222, "No-Depformer --- e.g., an ASR model"): there is none
-    if (c.dep_q > 0)
-      B200_LAUNCH(replace_audio_kernel, ceil_div(B * c.dep_q, 128), 128, 0, st, h->replace_tokens, h->audio_tokens, B, c.dep_q);
-    B200_LAUNCH(advance_pos_kernel, ceil_div(MB, 128), 128, 0, st, h->pos, h->exec_mask_m, MB);
-    B200_LAUNCH(lm_finish_kernel, ceil_div(B, 128), 128, 0, st, ring(h), h->text_token, h->audio_tokens, h->out_tokens, B, h->noise_ctr);
-    return check_launch("lm step (no depformer)");
-  }
-  B200_TRY(linear(h, h->tout, d, h->dep_in_all, h->din, (long long)c.dep_q * dd, nullptr, 0, MB, c.dep_q * dd, d, LIN_STORE, 0, h->dep_in_s));
-  if (h->depf) {
-    B200_TRY(tc::dep_fused_launch(h->depf, st));
-  } else {
-    for (int k = 0; k < c.dep_q; ++k) {
-      const long long* prev = k == 0 ? h->text_token : h->audio_tokens + (long long)(k - 1) * B;
-      B200_LAUNCH(dep_input_kernel, ceil_div(MB * dd, 256), 256, 0, st, h->din, (long long)c.dep_q * dd, k * dd,
-                  h->dep_tables[k], prev, h->dx, MB, dd, B, k == 0 ? c.text_card : c.card, h->err);
-      for (auto& L : h->dlayers) {
-        B200_TRY(norm_linear(h, h->dx, L.n1, h->dxn, L.in_w[k], h->dqkv, 3 * dd, MB, 3 * dd, dd, LIN_STORE, 0, L.in_s[k]));
-        B200_LAUNCH(dep_attn_step_kernel, ceil_div(MB * dH * 32, 128), 128, 0, st, h->dqkv, L.kc, L.vc, h->dao, MB, dH, c.dep_q, k);
-        B200_TRY(linear(h, h->dao, dd, L.out_w[k], h->dx, dd, h->dx, dd, MB, dd, dd, LIN_RESADD, 0, L.out_s[k]));
-        B200_TRY(norm_linear(h, h->dx, L.n2, h->dxn, L.lin_in[k], h->dh, dF, MB, dF, dd, LIN_GATE, dF, L.lin_in_s[k]));
-        B200_TRY(linear(h, h->dh, dF, L.lin_out[k], h->dx, dd, h->dx, dd, MB, dd, dF, LIN_RESADD, 0, L.lin_out_s[k]));
-      }
-      bf16* logits = h->dep_logits + (long long)k * MB * c.card;
-      B200_TRY(linear(h, h->dx, dd, h->dep_heads[k], logits, c.card, nullptr, 0, MB, c.card, dd, LIN_STORE, 0, h->dep_heads_s[k]));
-      const bf16* gl = guide(h, logits, cfg_on(h) ? h->dep_logits_cfg + (long long)k * B * c.card : nullptr, c.card, true);   // lm.py:828-833
-      B200_TRY(sample(h, gl, c.card, h->noise + kt + (long long)k * ka, h->audio_tokens + (long long)k * B, h->temp, h->top_k));
-    }
-  }
+  B200_TRY(h->dep.run(h, h->replace_static != 0));
   B200_LAUNCH(advance_pos_kernel, ceil_div(MB, 128), 128, 0, st, h->pos, h->exec_mask_m, MB);
   B200_LAUNCH(lm_finish_kernel, ceil_div(B, 128), 128, 0, st, ring(h), h->text_token, h->audio_tokens, h->out_tokens, B, h->noise_ctr);
   return check_launch("lm step");
@@ -789,9 +934,10 @@ int b200_lm_create(const b200_lm_config* cfg, b200_lm** out) {
   for (int k = 0; k < h->Kc; ++k) h->max_delay = cfg->delays[k] > h->max_delay ? cfg->delays[k] : h->max_delay;
   h->CT = h->max_delay + 2;     // lm.py:606-611
   if (const char* e = getenv("B200_PDL")) h->pdl = atoi(e) != 0;
-  if (const char* e = getenv("B200_DEP_FUSED")) h->dep_fused = atoi(e);
   h->kv.context = cfg->context;
   h->kv.H = cfg->num_heads;
+  h->dep.configure(*cfg);
+  h->dep.set_sampling(h->use_sampling, h->temp, h->top_k, h->top_k_text);
   if (const char* e = getenv("B200_KV_DTYPE")) {
     const std::string v = e;
     h->kv.kind = (v == "fp8" || v == "fp8_e4m3") ? B200_KV_FP8_E4M3 : v == "int8" ? B200_KV_INT8 : B200_KV_BF16;
@@ -811,7 +957,7 @@ int b200_lm_finalize(b200_lm* h) {
   if (!h) B200_FAIL(B200_ERR_INVALID, "lm_finalize: null handle");
   if (h->finalized) return B200_OK;
   const auto& c = h->cfg;
-  const int d = c.dim, dd = c.depformer_dim, F = c.ffn_hidden, dF = c.depformer_ffn_hidden;
+  const int d = c.dim, F = c.ffn_hidden;
   if (h->cross_on && c.quantize)      // the reference's _compute_cross_attention asserts an nn.Linear in_proj
     B200_FAIL(B200_ERR_INVALID, "lm_finalize: cross-attention layers with quantize=True (int8 linears) are not supported");
   h->emb.n_q = c.n_q; h->emb.card = c.card; h->emb.text_card = c.text_card; h->emb.condition_sum = nullptr; h->emb.err = nullptr;
@@ -819,18 +965,18 @@ int b200_lm_finalize(b200_lm* h) {
   for (int k = 0; k < c.n_q; ++k)
     B200_TRY(get_bf16(h, "emb." + std::to_string(k) + ".weight", {c.card + 1, d}, &h->emb.audio[k]));
   B200_TRY(get_bf16(h, "text_emb.weight", {c.text_card + 1, d}, &h->emb.text));
-  B200_TRY(get_linear(h, "text_linear.weight", c.text_card, d, LIN_STORE, 0, &h->text_linear, &h->text_linear_s));
+  B200_TRY(get_linear(h, {"text_linear.weight"}, c.text_card, d, LIN_STORE, 0, &h->text_linear, &h->text_linear_s));
   B200_TRY(get_bf16(h, "out_norm.alpha", {1, 1, d}, &h->out_norm));
   h->layers.resize(c.num_layers);
   for (int l = 0; l < c.num_layers; ++l) {
     const std::string p = "transformer.layers." + std::to_string(l);
     TLayer& L = h->layers[l];
-    B200_TRY(get_linear(h, p + ".self_attn.in_projs.0.weight", 3 * d, d, LIN_STORE, 0, &L.in_w, &L.in_s));
-    B200_TRY(get_linear(h, p + ".self_attn.out_projs.0.weight", d, d, LIN_RESADD, 0, &L.out_w, &L.out_s));
+    B200_TRY(get_linear(h, {p + ".self_attn.in_projs.0.weight"}, 3 * d, d, LIN_STORE, 0, &L.in_w, &L.in_s));
+    B200_TRY(get_linear(h, {p + ".self_attn.out_projs.0.weight"}, d, d, LIN_RESADD, 0, &L.out_w, &L.out_s));
     B200_TRY(get_bf16(h, p + ".norm1.alpha", {1, 1, d}, &L.n1));
     B200_TRY(get_bf16(h, p + ".norm2.alpha", {1, 1, d}, &L.n2));
-    B200_TRY(get_linear(h, p + ".gating.linear_in.weight", 2 * F, d, LIN_GATE, F, &L.lin_in, &L.lin_in_s));
-    B200_TRY(get_linear(h, p + ".gating.linear_out.weight", d, F, LIN_RESADD, 0, &L.lin_out, &L.lin_out_s));
+    B200_TRY(get_linear(h, {p + ".gating.linear_in.weight"}, 2 * F, d, LIN_GATE, F, &L.lin_in, &L.lin_in_s));
+    B200_TRY(get_linear(h, {p + ".gating.linear_out.weight"}, d, F, LIN_RESADD, 0, &L.lin_out, &L.lin_out_s));
     if (h->cross_on) {      // transformer.py:495-505, 727-732: in_projs.0 rows [0, d) the query, [d, 3d) K|V of the condition
       const std::string x = p + ".cross_attention.in_projs.0.weight";
       const bf16* w = nullptr;
@@ -840,7 +986,7 @@ int b200_lm_finalize(b200_lm* h) {
       B200_TRY(pack_bf16(h, w + (size_t)d * d, 2 * d, d, LIN_STORE, &L.ckv_w));
       B200_CUDA(cudaStreamSynchronize(nullptr));
       h->store.release(x);
-      B200_TRY(get_linear(h, p + ".cross_attention.out_projs.0.weight", d, d, LIN_RESADD, 0, &L.co_w, &no_scales));
+      B200_TRY(get_linear(h, {p + ".cross_attention.out_projs.0.weight"}, d, d, LIN_RESADD, 0, &L.co_w, &no_scales));
       B200_TRY(get_bf16(h, p + ".norm_cross.weight", {d}, &L.ncw));
       B200_TRY(get_bf16(h, p + ".norm_cross.bias", {d}, &L.ncb));
     }
@@ -854,82 +1000,7 @@ int b200_lm_finalize(b200_lm* h) {
     B200_TRY(h->weights.alloc_t(&h->extra_w_dev, h->extra_w.size(), false));
     B200_CUDA(cudaMemcpy(h->extra_w_dev, h->extra_w.data(), h->extra_w.size() * sizeof(void*), cudaMemcpyHostToDevice));
   }
-  // depformer_in.{k} stacked so that all dep_q projections of transformer_out are one GEMM
-  const Tensor* din0 = c.dep_q > 0 ? h->store.find("depformer_in.0.weight") : nullptr;
-  if (din0 && din0->dtype == B200_I8) {          // pre-quantised: stack CB and SCB
-    int8_t* stacked = nullptr; float* scales = nullptr; void* packed = nullptr;
-    B200_CUDA(cudaMalloc(&stacked, (size_t)c.dep_q * dd * d));
-    struct Guard { void* p; ~Guard() { cudaFree(p); } } guard{stacked};
-    B200_TRY(h->weights.alloc_t(&scales, (size_t)c.dep_q * dd, false));
-    for (int k = 0; k < c.dep_q; ++k) {
-      const std::string name = "depformer_in." + std::to_string(k) + ".weight";
-      const int8_t* q = nullptr; const float* scb = nullptr;
-      if (!h->store.find(name)) B200_FAIL(B200_ERR_MISSING, "lm finalize: tensor '%s' was not loaded", name.c_str());
-      B200_TRY(get_prequantised(h, name, dd, d, &q, &scb));
-      B200_CUDA(cudaMemcpy(stacked + (size_t)k * dd * d, q, (size_t)dd * d, cudaMemcpyDeviceToDevice));
-      B200_CUDA(cudaMemcpy(scales + (size_t)k * dd, scb, (size_t)dd * 4, cudaMemcpyDeviceToDevice));
-      h->store.release(name);
-      h->store.release(name + "_scb");
-    }
-    B200_TRY(h->weights.alloc(&packed, tc::sk_packed_bytes_i8(c.dep_q * dd, d, LIN_STORE, 0), false));
-    B200_TRY(tc::sk_pack_weights_i8(stacked, packed, c.dep_q * dd, d, LIN_STORE, 0, nullptr));
-    B200_CUDA(cudaStreamSynchronize(nullptr));
-    h->dep_in_s = scales;
-    h->dep_in_all = static_cast<bf16*>(packed);
-    h->weight_bytes += (int64_t)c.dep_q * dd * d + (int64_t)c.dep_q * dd * 4;
-  } else if (c.dep_q > 0) {
-    bf16* stacked = nullptr;
-    B200_CUDA(cudaMalloc(&stacked, (size_t)c.dep_q * dd * d * 2));
-    struct Guard { void* p; ~Guard() { cudaFree(p); } } guard{stacked};      // released on every path out of this block
-    for (int k = 0; k < c.dep_q; ++k) {
-      const bf16* w = nullptr;
-      const std::string name = "depformer_in." + std::to_string(k) + ".weight";
-      B200_TRY(get_bf16(h, name, {dd, d}, &w));
-      B200_CUDA(cudaMemcpy(stacked + (size_t)k * dd * d, w, (size_t)dd * d * 2, cudaMemcpyDeviceToDevice));
-      h->store.release(name);
-    }
-    void* packed = nullptr;
-    int rc = B200_OK;
-    if (c.quantize) {
-      float* scales = nullptr;
-      rc = h->weights.alloc(&packed, tc::sk_packed_bytes_i8(c.dep_q * dd, d, LIN_STORE, 0), false);
-      if (rc == B200_OK) rc = h->weights.alloc_t(&scales, (size_t)c.dep_q * dd, false);
-      if (rc == B200_OK) rc = tc::sk_quant_pack_weights(stacked, packed, scales, c.dep_q * dd, d, LIN_STORE, 0, nullptr);
-      h->dep_in_s = scales;
-      h->weight_bytes -= (int64_t)c.dep_q * dd * d;
-      h->weight_bytes += (int64_t)c.dep_q * dd * 4;
-    } else {
-      rc = h->weights.alloc(&packed, tc::sk_packed_bytes(c.dep_q * dd, d, LIN_STORE, 0), false);
-      if (rc == B200_OK) rc = tc::sk_pack_weights(stacked, packed, c.dep_q * dd, d, LIN_STORE, 0, nullptr);
-    }
-    B200_TRY(rc);
-    B200_CUDA(cudaStreamSynchronize(nullptr));
-    h->dep_in_all = static_cast<bf16*>(packed);
-  }
-  h->dep_tables.resize(c.dep_q);
-  if (c.dep_q > 0) B200_TRY(get_bf16(h, "depformer_text_emb.weight", {c.text_card + 1, dd}, &h->dep_tables[0]));
-  for (int k = 1; k < c.dep_q; ++k)
-    B200_TRY(get_bf16(h, "depformer_emb." + std::to_string(k - 1) + ".weight", {c.card + 1, dd}, &h->dep_tables[k]));
-  h->dep_heads.resize(c.dep_q);
-  h->dep_heads_s.resize(c.dep_q);
-  for (int k = 0; k < c.dep_q; ++k)
-    B200_TRY(get_linear(h, "linears." + std::to_string(k) + ".weight", c.card, dd, LIN_STORE, 0, &h->dep_heads[k], &h->dep_heads_s[k]));
-  h->dlayers.resize(c.dep_q > 0 ? c.depformer_num_layers : 0);
-  for (int l = 0; l < (int)h->dlayers.size(); ++l) {
-    const std::string p = "depformer.layers." + std::to_string(l);
-    DLayer& L = h->dlayers[l];
-    L.in_w.resize(c.dep_q); L.out_w.resize(c.dep_q); L.lin_in.resize(c.dep_q); L.lin_out.resize(c.dep_q);
-    L.in_s.resize(c.dep_q); L.out_s.resize(c.dep_q); L.lin_in_s.resize(c.dep_q); L.lin_out_s.resize(c.dep_q);
-    for (int k = 0; k < c.dep_q; ++k) {
-      const std::string ks = std::to_string(k);
-      B200_TRY(get_linear(h, p + ".self_attn.in_projs." + ks + ".weight", 3 * dd, dd, LIN_STORE, 0, &L.in_w[k], &L.in_s[k]));
-      B200_TRY(get_linear(h, p + ".self_attn.out_projs." + ks + ".weight", dd, dd, LIN_RESADD, 0, &L.out_w[k], &L.out_s[k]));
-      B200_TRY(get_linear(h, p + ".gating." + ks + ".linear_in.weight", 2 * dF, dd, LIN_GATE, dF, &L.lin_in[k], &L.lin_in_s[k]));
-      B200_TRY(get_linear(h, p + ".gating." + ks + ".linear_out.weight", dd, dF, LIN_RESADD, 0, &L.lin_out[k], &L.lin_out_s[k]));
-    }
-    B200_TRY(get_bf16(h, p + ".norm1.alpha", {1, 1, dd}, &L.n1));
-    B200_TRY(get_bf16(h, p + ".norm2.alpha", {1, 1, dd}, &L.n2));
-  }
+  B200_TRY(h->dep.load(h));
   B200_TRY(h->weights.alloc_t(&h->delays_dev, h->Kc, false));
   B200_CUDA(cudaMemcpy(h->delays_dev, c.delays, h->Kc * sizeof(int), cudaMemcpyHostToDevice));
   B200_CUDA(cudaDeviceSynchronize());
@@ -956,7 +1027,7 @@ int b200_lm_set_sampling(b200_lm* h, int use_sampling, float temp, float temp_te
   if (use_sampling == h->use_sampling && temp == h->temp && temp_text == h->temp_text && top_k == h->top_k && top_k_text == h->top_k_text)
     return B200_OK;
   h->use_sampling = use_sampling; h->temp = temp; h->temp_text = temp_text; h->top_k = top_k; h->top_k_text = top_k_text;
-  tc::dep_fused_set_sampling(h->depf, use_sampling, temp, top_k);
+  h->dep.set_sampling(use_sampling, temp, top_k, top_k_text);
   h->graphs[0].drop();         // the sampling parameters are kernel arguments of the captured step
   return B200_OK;
 }
@@ -966,6 +1037,14 @@ int b200_lm_noise_per_row(b200_lm* h) { return h ? noise_per_row(h) : 0; }
 int b200_lm_set_graph(b200_lm* h, int enable) {
   if (!h) B200_FAIL(B200_ERR_INVALID, "lm_set_graph: null handle");
   h->set_graph(enable);
+  return B200_OK;
+}
+
+int b200_lm_set_depformer(b200_lm* h, int mode) {
+  if (!h) B200_FAIL(B200_ERR_INVALID, "lm_set_depformer: null handle");
+  if (h->batch > 0) B200_FAIL(B200_ERR_STATE, "lm_set_depformer: the depformer's path is planned at streaming_begin; set it before");
+  if (mode < B200_DEPFORMER_AUTO || mode > B200_DEPFORMER_FUSED) B200_FAIL(B200_ERR_INVALID, "lm_set_depformer: unknown mode %d", mode);
+  h->dep.mode = mode;
   return B200_OK;
 }
 
@@ -1000,7 +1079,7 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
   DeviceGuard guard_dev(h->device);
   const auto& c = h->cfg;
   const bool cfg = cfg_on(h);
-  const int B = batch, MB = cfg ? 2 * batch : batch, d = c.dim, H = c.num_heads, D = d / H, dd = c.depformer_dim;
+  const int B = batch, MB = cfg ? 2 * batch : batch, d = c.dim, H = c.num_heads, D = d / H;
   if (MB > 256) B200_FAIL(B200_ERR_INVALID, "lm_streaming_begin: %d model rows (the linears take at most 256)", MB);
   if (cfg && !h->cfg_until_host.empty() && (int)h->cfg_until_host.size() != B)      // lm.py:717 view(-1, 1, 1) broadcast
     B200_FAIL(B200_ERR_SHAPE, "lm_streaming_begin: cfg_is_masked_until has %zu entries for %d sessions", h->cfg_until_host.size(), B);
@@ -1056,10 +1135,7 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
     B200_TRY(A.alloc_t(&h->cross_rows, MB, false));
   }
   B200_TRY(h->kv.alloc_pages(A));
-  for (auto& L : h->dlayers) {
-    B200_TRY(A.alloc_t(&L.kc, (size_t)MB * dd * c.dep_q));
-    B200_TRY(A.alloc_t(&L.vc, (size_t)MB * dd * c.dep_q));
-  }
+  B200_TRY(h->dep.begin(A, B, cfg, c.quantize != 0));
   const int n_in_max = c.n_q;   // callers may pass more columns than needed (lm.py:688-689)
   const int dq1 = c.dep_q > 0 ? c.dep_q : 1;
   B200_TRY(A.alloc_t(&h->in_codes, (size_t)B * n_in_max));
@@ -1084,16 +1160,10 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
   B200_TRY(A.alloc_t(&h->text_logits, (size_t)MB * c.text_card));
   if (cfg) {
     B200_TRY(A.alloc_t(&h->text_logits_cfg, (size_t)B * c.text_card));
-    B200_TRY(A.alloc_t(&h->dep_logits_cfg, (size_t)B * dq1 * c.card));
+    B200_TRY(h->dep.alloc_guided(A));
   }
   if (!h->extra_w.empty()) B200_TRY(A.alloc_t(&h->extra_out, h->extra_w.size() * (size_t)MB * c.extra_heads_dim));
-  B200_TRY(A.alloc_t(&h->din, (size_t)MB * dq1 * dd));
-  B200_TRY(A.alloc_t(&h->dx, (size_t)MB * dd));
-  B200_TRY(A.alloc_t(&h->dxn, (size_t)MB * dd));
-  B200_TRY(A.alloc_t(&h->dqkv, (size_t)MB * 3 * dd));
-  B200_TRY(A.alloc_t(&h->dao, (size_t)MB * dd));
-  B200_TRY(A.alloc_t(&h->dh, (size_t)MB * c.depformer_ffn_hidden));
-  B200_TRY(A.alloc_t(&h->dep_logits, (size_t)MB * dq1 * c.card));
+  B200_TRY(h->dep.alloc_activations(A));
   // (the condition memory's K/V projection runs CROSS_CHUNK rows at a time)
   B200_TRY(A.alloc(reinterpret_cast<void**>(&h->sk_ws), tc::sk_workspace_bytes(h->cross_on ? std::max(MB, CROSS_CHUNK) : MB), false));
   B200_TRY(A.alloc_t(&h->sk_counters, tc::SK_MAX_TILES));
@@ -1107,49 +1177,12 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
   B200_TRY(A.alloc_host(&h->pin_out, (size_t)B * (c.dep_q + 1)));
   B200_TRY(A.alloc_host(&h->pin_noise, (size_t)B * noise_per_row(h)));
   if (c.quantize) {     // activations are re-quantised row-wise before every linear (QLinear.forward, utils/quantize.py:28-36)
-    const int kmax = std::max(std::max(d, c.ffn_hidden), std::max(dd, c.depformer_ffn_hidden));
+    const int kmax = std::max(std::max(d, c.ffn_hidden), std::max(c.depformer_dim, c.depformer_ffn_hidden));
     B200_TRY(A.alloc_t(&h->xq, (size_t)MB * kmax, false));
     B200_TRY(A.alloc_t(&h->xq_scale, (size_t)MB, false));
   }
   B200_TRY(tc::linear_init());
-  // One or two sessions: the depformer's linears take the GEMV path and the PDL-chained launches beat the persistent kernel
-  // (a grid barrier per phase costs more than the launch it saves).  B200_DEP_FUSED=2 forces the kernel at any batch.
-  // Under classifier-free guidance the two halves of the batch meet before every sampler (lm.py:828-833): launch chain.
-  const bool dep_small = B <= tc::sk_gemv_max_m() && h->dep_fused != 2;
-  h->depf = nullptr;
-  if (c.dep_q > 0 && !cfg && !c.quantize && h->dep_fused && !dep_small && B <= 256 && dd <= 1024 && dd % 64 == 0) {
-    tc::DepFusedConfig fc;
-    memset(&fc, 0, sizeof(fc));
-    fc.B = B; fc.dd = dd; fc.H = c.depformer_num_heads; fc.F = c.depformer_ffn_hidden; fc.card = c.card; fc.text_card = c.text_card;
-    fc.dep_q = c.dep_q; fc.L = c.depformer_num_layers; fc.err = h->err;
-    std::vector<const void*> in_w, out_w, lin_in, lin_out, heads, tables, n1, n2;
-    std::vector<void*> kc, vc;
-    for (int k = 0; k < c.dep_q; ++k)
-      for (auto& L : h->dlayers) {
-        in_w.push_back(L.in_w[k]); out_w.push_back(L.out_w[k]); lin_in.push_back(L.lin_in[k]); lin_out.push_back(L.lin_out[k]);
-      }
-    for (int k = 0; k < c.dep_q; ++k) { heads.push_back(h->dep_heads[k]); tables.push_back(h->dep_tables[k]); }
-    for (auto& L : h->dlayers) { n1.push_back(L.n1); n2.push_back(L.n2); kc.push_back(L.kc); vc.push_back(L.vc); }
-    fc.in_w = in_w.data(); fc.out_w = out_w.data(); fc.lin_in = lin_in.data(); fc.lin_out = lin_out.data();
-    fc.heads = heads.data(); fc.tables = tables.data(); fc.n1 = n1.data(); fc.n2 = n2.data(); fc.kc = kc.data(); fc.vc = vc.data();
-    fc.din = h->din; fc.din_ld = (long long)c.dep_q * dd; fc.text_token = h->text_token;
-    fc.x = h->dx; fc.xn = h->dxn; fc.ao = h->dao; fc.hbuf = h->dh;
-    const size_t pf = tc::dep_fused_partial_floats(fc);
-    B200_TRY(A.alloc_t(&h->dep_part0, pf, false));
-    B200_TRY(A.alloc_t(&h->dep_part1, pf, false));
-    B200_TRY(A.alloc_t(&h->dep_bar, 1));
-    fc.part0 = h->dep_part0; fc.part1 = h->dep_part1; fc.bar = h->dep_bar;
-    if (const char* e = getenv("B200_DEP_TRACE")) {
-      if (atoi(e)) B200_TRY(A.alloc_t(&h->dep_trace, (size_t)tc::DEP_TRACE_SLOTS));
-    }
-    fc.trace = h->dep_trace;
-    fc.logits = h->dep_logits; fc.audio_tokens = h->audio_tokens;
-    fc.noise = h->noise; fc.noise_ld = noise_per_row(h);
-    fc.noise_off = h->top_k_text < c.text_card ? h->top_k_text : c.text_card;
-    fc.ka = h->top_k < c.card ? h->top_k : c.card;
-    fc.use_sampling = h->use_sampling; fc.top_k = h->top_k; fc.temp = h->temp;
-    B200_TRY(tc::dep_fused_create(fc, &h->depf));
-  }
+  B200_TRY(h->dep.alloc_fused(h));
   // streaming-state snapshot (lm.py:527-542 _LMGenState + the temporal transformer's ring caches, transformer.py:196-288)
   A.mark_state(h->exec_mask, B, "exec_mask", B200_U8, {B});
   if (cfg) A.mark_state(h->exec_mask_m, MB, "model.exec_mask", B200_U8, {MB});
@@ -1253,8 +1286,7 @@ int b200_lm_streaming_end(b200_lm* h) {
   DeviceGuard g(h->device);
   h->end_streaming();
   h->maps.clear();
-  tc::dep_fused_destroy(h->depf);
-  h->depf = nullptr;
+  h->dep.end();
   h->cfg_until = nullptr; h->noise_ctr = nullptr; h->cond_sum = nullptr; h->cond_on = 0;
   h->kv.end();
   h->taps = nullptr; h->taps_on = 0;
@@ -1542,35 +1574,17 @@ int b200_lm_read_buffer(b200_lm* h, const char* name, void* dst_dev, int64_t cap
   const bool cfg = cfg_on(h);
   const void* src = nullptr;
   int64_t sz = 0;
-  // with CFG "text_logits" / "dep_logits" are what the samplers read (the guided rows, lm.py:728-732, 828-833); the model's
-  // own 2B rows are "model_text_logits" / "model_dep_logits"
-  if (n == "text_logits") { src = (cfg && !h->cfg_is_no_text) ? h->text_logits_cfg : h->text_logits; sz = (int64_t)B * c.text_card * 2; }
+  // with CFG "text_logits" is what the sampler reads (the guided rows, lm.py:728-732); the model's own 2B rows are
+  // "model_text_logits"
+  if (h->dep.buffer(n, cfg, &src, &sz)) {}
+  else if (n == "text_logits") { src = (cfg && !h->cfg_is_no_text) ? h->text_logits_cfg : h->text_logits; sz = (int64_t)B * c.text_card * 2; }
   else if (n == "model_text_logits") { src = h->text_logits; sz = (int64_t)MB * c.text_card * 2; }
   else if (n == "transformer_out") { src = h->tout; sz = (int64_t)MB * c.dim * 2; }
-  else if (n == "dep_logits") {
-    if (cfg) { src = h->dep_logits_cfg; sz = (int64_t)c.dep_q * B * c.card * 2; }
-    else { src = h->dep_logits; sz = (int64_t)c.dep_q * B * c.card * 2; }
-  }
-  else if (n == "model_dep_logits") { src = h->dep_logits; sz = (int64_t)c.dep_q * MB * c.card * 2; }
   else if (n == "input_tokens") { src = h->input_tokens; sz = (int64_t)MB * h->Kc * 8; }
   else if (n == "text_token") { src = h->text_token; sz = (int64_t)B * 8; }
   else if (n == "audio_tokens") { src = h->audio_tokens; sz = (int64_t)c.dep_q * B * 8; }
   else if (n == "noise") { src = h->noise; sz = (int64_t)B * noise_per_row(h) * 4; }
-  else if (n == "dep_trace") { src = h->dep_trace; sz = h->dep_trace ? (int64_t)tc::DEP_TRACE_SLOTS * 8 : 0; }
   else if (n == "extra_heads") { src = h->extra_out; sz = (int64_t)h->extra_w.size() * MB * c.extra_heads_dim * 2; }
-  else if (n == "dep_in" && c.dep_q > 0) { src = h->din; sz = (int64_t)MB * c.dep_q * c.depformer_dim * 2; }
-  else if (n.rfind("depformer.layers.", 0) == 0 && c.dep_q > 0) {
-    // the per-frame depformer cache of one layer: after a frame it holds every sub-step's k / v
-    const std::string rest = n.substr(17);
-    const size_t dot = rest.find('.');
-    const std::string idx = rest.substr(0, dot), kind = dot == std::string::npos ? "" : rest.substr(dot + 1);
-    const bool digits = !idx.empty() && idx.size() <= 4 && idx.find_first_not_of("0123456789") == std::string::npos;
-    const int l = digits ? atoi(idx.c_str()) : -1;
-    if (l < 0 || l >= (int)h->dlayers.size() || (kind != "k" && kind != "v"))
-      B200_FAIL(B200_ERR_INVALID, "lm_read_buffer: unknown buffer '%s'", n.c_str());
-    src = kind == "k" ? h->dlayers[l].kc : h->dlayers[l].vc;
-    sz = (int64_t)MB * c.depformer_dim * c.dep_q * 2;
-  }
   else if (n.rfind("temporal.", 0) == 0) {
     // the taps of the last step taken with b200_lm_set_taps on: "temporal.embed", "temporal.layers.<l>.<kind>"
     if (!h->taps) B200_FAIL(B200_ERR_STATE, "lm_read_buffer: '%s' is a tap; turn the taps on (b200_lm_set_taps) before the step", n.c_str());

@@ -141,6 +141,21 @@ int b200_op_linear_plan(int M, int N, int K, int epi, int gate_rows, int int8, i
   return B200_OK;
 }
 
+int b200_op_depformer_plan(int dep_q, int depformer_dim, int depformer_num_heads, int depformer_ffn_hidden, int card, int batch,
+                           int cfg, int int8, int mode, int sms, int gemv_max_rows, int64_t* out, int capacity) {
+  constexpr int F = 6 + 5 * 6;
+  if (!out || capacity < F) B200_FAIL(B200_ERR_INVALID, "op_depformer_plan: %d slots, the plan needs %d", capacity, F);
+  tc::DepformerPlan P;
+  B200_TRY(tc::plan_depformer(dep_q, depformer_dim, depformer_num_heads, depformer_ffn_hidden, card, batch, cfg != 0, int8 != 0, sms,
+                              gemv_max_rows, mode, &P));
+  const long long v[6] = {P.path, P.part_floats, P.stages, P.stage_bytes, P.smem, P.grid};
+  int i = 0;
+  for (long long x : v) out[i++] = x;
+  for (const tc::Gemm& g : {P.g_in, P.g_out, P.g_lin_in, P.g_lin_out, P.g_head})
+    for (int x : {g.n_tiles, g.num_kb, g.kbps, g.S, g.A, g.N}) out[i++] = x;
+  return B200_OK;
+}
+
 // rmsnorm_kernel as the LM launches it (lm.cu norm_linear and the output norm): one 256-thread CTA per row, eps 1e-8
 int b200_op_rmsnorm(const void* x_dev, const void* alpha_dev, void* y_dev, int M, int dim, void* stream) {
   using namespace b200::lm;

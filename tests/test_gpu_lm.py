@@ -413,10 +413,11 @@ def test_streaming_state_snapshot_roundtrip(lm, tiny):
 
 @torch.no_grad()
 @pytest.mark.parametrize("B", [17, 130])
-def test_fused_depformer_equals_launch_chain(B, monkeypatch):
+def test_fused_depformer_equals_launch_chain(B):
     """The persistent depformer kernel against the per-kernel launch chain on a mid-size member of the 7B family, at batch
     sizes that exercise odd paddings (Mpad 32 / 144, two launches above 128 sessions) and the cluster
     split-K GEMMs: same text logits, same depformer logits within bf16 accumulation-order noise, near-identical greedy ids."""
+    from moshi_b200 import _lib
     from moshi_b200.models import LMGen, LMModel
     cfg = LMConfig(dim=1024, num_heads=8, num_layers=2, context=64, text_card=4000, card=2048,
                    depformer_dim=1024, depformer_num_heads=16, depformer_dim_feedforward=4224, depformer_num_layers=3)
@@ -424,9 +425,9 @@ def test_fused_depformer_equals_launch_chain(B, monkeypatch):
     g = torch.Generator().manual_seed(B)
     codes = torch.randint(0, cfg.card, (4, B, 8, 1), generator=g).cuda()
 
-    def run(fused: str):
-        monkeypatch.setenv("B200_DEP_FUSED", fused)
+    def run(mode: int):
         lm = LMModel(cfg, sd, device="cuda")
+        _lib.check(_lib.lib().b200_lm_set_depformer(lm._h, mode))
         gen = LMGen(lm, use_sampling=False)
         outs = []
         with gen.streaming(B):
@@ -438,7 +439,7 @@ def test_fused_depformer_equals_launch_chain(B, monkeypatch):
         del gen, lm
         return outs
 
-    chain, fused = run("0"), run("1")
+    chain, fused = run(_lib.B200_DEPFORMER_CHAIN), run(_lib.B200_DEPFORMER_AUTO)
     same = total = 0
     on_track = torch.ones(B, dtype=torch.bool)             # rows whose sampled history is still identical in both runs
     for (tl_c, dl_c, at_c), (tl_f, dl_f, at_f) in zip(chain, fused):

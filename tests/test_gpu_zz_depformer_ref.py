@@ -1,7 +1,7 @@
 """GPU: every depformer path against the fp64 reference, at every layer and sub-step of a frame.
 
 The depformer runs as one persistent kernel (csrc/dep_fused.cu, 3..256 sessions), as a launch chain of tensor-core GEMMs
-(B200_DEP_FUSED=0) or as a chain of GEMVs (one and two sessions).  After each frame the test reads
+(B200_DEPFORMER_CHAIN) or as a chain of GEMVs (one and two sessions).  After each frame the test reads
 what the device computed inside the frame: ``dep_in`` (depformer_in[k] of transformer_out), every layer's per-frame cache
 (``depformer.layers.<l>.k`` / ``.v``: bf16(in_proj(rmsnorm(x))) for every sub-step) and the logits, and holds each of them to
 ``depformer_ref64`` (tests/util.py), teacher-forced on the device's own transformer_out and tokens, under the rule whose
@@ -36,7 +36,6 @@ QLinear of the correctly rounded RMSNorm output.  tests/util.py's _bf now rounds
 """
 import dataclasses
 import json
-import os
 import pathlib
 
 import pytest
@@ -50,6 +49,8 @@ from tests.util import (cfg_guide64, cfg_guide_bf16, dep_checkpoints, dep_row_ra
                         exact_row_ratios, greedy_unexcused, sample_is_stable, sampler_mismatches)
 
 pytestmark = pytest.mark.gpu
+
+AUTO, CHAIN, FUSED = _lib.B200_DEPFORMER_AUTO, _lib.B200_DEPFORMER_CHAIN, _lib.B200_DEPFORMER_FUSED
 
 _2B = json.loads((pathlib.Path(__file__).parent / "golden" / "moshi_dev_2b.json").read_text())
 MEMBERS = {
@@ -74,21 +75,21 @@ SAMPLING = {
     # clamp to card sets its width
     "ragged": dict(temp=0.8, top_k=1024, temp_text=0.7, top_k_text=1000),
 }
-# (member, path, B200_DEP_FUSED, batch sizes, of which also run with sampling).  The fused kernel's batches sit on the edges
+# (member, path, depformer mode, batch sizes, of which also run with sampling).  The fused kernel's batches sit on the edges
 # of its 64-session GEMM units, of the padded batch and of its 256-session limit.  No batch past 256 runs: streaming_begin
 # refuses more than 256 model rows (the LM's linears take at most 256), so no handle reaches the fused kernel's limit.
 CASES = [
-    ("7b", "fused", None, (3, 17, 63, 64, 65, 128, 129, 200, 256), (3, 129, 256)),
-    ("7b", "chain", "0", (3, 65, 129, 256), (65, 256)),
-    ("7b", "gemv", None, (1, 2), (2,)),
-    ("7b", "fused-forced", "2", (1, 2), (1,)),
-    ("q16", "fused", None, (3, 65, 129), (65,)),
-    ("q16", "chain", "0", (3, 65, 129), (65,)),
-    ("ragged", "fused", None, (3, 65, 129), (3, 129)),
-    ("ragged", "chain", "0", (3, 65, 129), (65,)),
-    ("2b", "fused", None, (3, 17, 64, 65, 129, 256), (3, 129, 256)),
-    ("2b", "chain", "0", (3, 65, 129), (65,)),
-    ("2b", "gemv", None, (1, 2), (2,)),
+    ("7b", "fused", AUTO, (3, 17, 63, 64, 65, 128, 129, 200, 256), (3, 129, 256)),
+    ("7b", "chain", CHAIN, (3, 65, 129, 256), (65, 256)),
+    ("7b", "gemv", AUTO, (1, 2), (2,)),
+    ("7b", "fused-forced", FUSED, (1, 2), (1,)),
+    ("q16", "fused", AUTO, (3, 65, 129), (65,)),
+    ("q16", "chain", CHAIN, (3, 65, 129), (65,)),
+    ("ragged", "fused", AUTO, (3, 65, 129), (3, 129)),
+    ("ragged", "chain", CHAIN, (3, 65, 129), (65,)),
+    ("2b", "fused", AUTO, (3, 17, 64, 65, 129, 256), (3, 129, 256)),
+    ("2b", "chain", CHAIN, (3, 65, 129), (65,)),
+    ("2b", "gemv", AUTO, (1, 2), (2,)),
 ]
 # Classifier-free guidance and int8 linears: the handle builds no persistent kernel for either, so every frame runs the launch
 # chain over MB model rows (2B under guidance).  Batches sit on the schedule edges of MB: GEMV up to 2 rows (4 with gemv_rows),
@@ -121,18 +122,12 @@ def _state_dict(member: str, int8: bool = False) -> dict:
     return _sd_cache[(member, int8)]
 
 
-def _model(cfg: LMConfig, sd: dict, fused: str | None):
-    """LMModel built with B200_DEP_FUSED = ``fused`` (None: the default), which the handle reads when it is created."""
+def _model(cfg: LMConfig, sd: dict, mode: int):
+    """LMModel whose depformer runs in ``mode`` (b200_lm_set_depformer)."""
     from moshi_b200.models import LMModel
-    old = os.environ.pop("B200_DEP_FUSED", None)
-    try:
-        if fused is not None:
-            os.environ["B200_DEP_FUSED"] = fused
-        return LMModel(cfg, sd, device="cuda")
-    finally:
-        os.environ.pop("B200_DEP_FUSED", None)
-        if old is not None:
-            os.environ["B200_DEP_FUSED"] = old
+    lm = LMModel(cfg, sd, device="cuda")
+    _lib.check(_lib.lib().b200_lm_set_depformer(lm._h, mode))
+    return lm
 
 
 def _kind(kind: str, layer) -> str:
@@ -221,11 +216,11 @@ def _run(lm, member: str, sd: dict, B: int, sampling: bool, g: torch.Generator, 
     return res
 
 
-@pytest.mark.parametrize("member,path,fused,batches,sampled", CASES, ids=[f"{c[0]}-{c[1]}" for c in CASES])
-def test_depformer_matches_fp64_reference(member, path, fused, batches, sampled):
+@pytest.mark.parametrize("member,path,mode,batches,sampled", CASES, ids=[f"{c[0]}-{c[1]}" for c in CASES])
+def test_depformer_matches_fp64_reference(member, path, mode, batches, sampled):
     cfg = MEMBERS[member]
     sd = _state_dict(member)
-    lm = _model(cfg, sd, fused)
+    lm = _model(cfg, sd, mode)
     g = torch.Generator().manual_seed(len(path) * 101 + len(member))
     failures = []
     try:
@@ -258,7 +253,7 @@ def test_guided_and_int8_depformer_matches_fp64_reference(member, path, batches,
     if int8:
         cfg = dataclasses.replace(cfg, quantize=True)
     sd = _state_dict(member, int8)
-    lm = _model(cfg, sd, None)
+    lm = _model(cfg, sd, AUTO)
     g = torch.Generator().manual_seed(len(path) * 103 + len(member))
     min_launches = cfg.dep_q * cfg.depformer_num_layers * 5      # one launch per depformer linear or attention at least
     failures = []

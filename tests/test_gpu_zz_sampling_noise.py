@@ -21,12 +21,15 @@ import numpy as np
 import pytest
 import torch
 
+from moshi_b200 import _lib
 from moshi_b200.config import LMConfig, tiny_lm_config
 from moshi_b200.synth import synth_lm_state_dict
 from oracle import scenarios
 from tests.util import cptr, exp1_ref64, f32_ulp, sampler_mismatches, step_noise_ref, step_words
 
 pytestmark = pytest.mark.gpu
+
+AUTO, CHAIN, FUSED = _lib.B200_DEPFORMER_AUTO, _lib.B200_DEPFORMER_CHAIN, _lib.B200_DEPFORMER_FUSED
 
 SMP = dict(temp=0.8, top_k=250, temp_text=0.7, top_k_text=25)     # LMGen's defaults: 25 + 8 x 250 = 2025 draws per row
 
@@ -132,30 +135,24 @@ def _member(name: str):
     return _sd_cache[name]
 
 
-def _model(cfg: LMConfig, sd: dict, fused: str | None):
-    """LMModel built with B200_DEP_FUSED = ``fused`` (None: the default), which the handle reads when it is created."""
+def _model(cfg: LMConfig, sd: dict, mode: int):
+    """LMModel whose depformer runs in ``mode`` (b200_lm_set_depformer)."""
     from moshi_b200.models import LMModel
-    old = os.environ.pop("B200_DEP_FUSED", None)
-    try:
-        if fused is not None:
-            os.environ["B200_DEP_FUSED"] = fused
-        return LMModel(cfg, sd, device="cuda")
-    finally:
-        os.environ.pop("B200_DEP_FUSED", None)
-        if old is not None:
-            os.environ["B200_DEP_FUSED"] = old
+    lm = LMModel(cfg, sd, device="cuda")
+    _lib.check(_lib.lib().b200_lm_set_depformer(lm._h, mode))
+    return lm
 
 
-# (member, depformer path, B200_DEP_FUSED, batch sizes, CFG coefficient).  At 1 and 2 sessions the default depformer is the
+# (member, depformer path, depformer mode, batch sizes, CFG coefficient).  At 1 and 2 sessions the default depformer is the
 # GEMV chain; "fused-forced" runs the persistent kernel there.  CFG doubles the model rows, so its batches stay at <= 128.
 STEP_CASES = [
-    ("tiny", "fused", None, (3, 40, 129), 1.0),
-    ("tiny", "chain", "0", (3, 40, 129), 1.0),
-    ("tiny", "gemv", None, (1,), 1.0),
-    ("tiny", "fused-forced", "2", (1,), 1.0),
-    ("tiny", "fused-cfg", None, (3, 40), 3.0),
-    ("tiny", "chain-cfg", "0", (3,), 3.0),
-    ("stt", "none", None, (1, 3, 40), 1.0),
+    ("tiny", "fused", AUTO, (3, 40, 129), 1.0),
+    ("tiny", "chain", CHAIN, (3, 40, 129), 1.0),
+    ("tiny", "gemv", AUTO, (1,), 1.0),
+    ("tiny", "fused-forced", FUSED, (1,), 1.0),
+    ("tiny", "fused-cfg", AUTO, (3, 40), 3.0),
+    ("tiny", "chain-cfg", CHAIN, (3,), 3.0),
+    ("stt", "none", AUTO, (1, 3, 40), 1.0),
 ]
 STEPS = 5
 SEED = 0x5EED_0000_0000_0001 + 2 ** 40
@@ -202,10 +199,10 @@ def _check_steps(lib, lm, cfg, B: int, graph: bool, cfg_coef: float, g: torch.Ge
     return res
 
 
-@pytest.mark.parametrize("member,path,fused,batches,cfg_coef", STEP_CASES, ids=[f"{c[0]}-{c[1]}" for c in STEP_CASES])
-def test_step_draws_its_noise_and_samples_with_it(lib, member, path, fused, batches, cfg_coef):
+@pytest.mark.parametrize("member,path,mode,batches,cfg_coef", STEP_CASES, ids=[f"{c[0]}-{c[1]}" for c in STEP_CASES])
+def test_step_draws_its_noise_and_samples_with_it(lib, member, path, mode, batches, cfg_coef):
     cfg, sd = _member(member)
-    lm = _model(cfg, sd, fused)
+    lm = _model(cfg, sd, mode)
     g = torch.Generator().manual_seed(17)
     failures = []
     try:
@@ -248,7 +245,7 @@ def test_step_noise_is_reproducible_and_restorable(lib, graph):
     from moshi_b200 import _lib
     from moshi_b200.models import LMGen
     cfg, sd = _member("tiny")
-    lm = _model(cfg, sd, None)
+    lm = _model(cfg, sd, AUTO)
     B, n = 5, 8
     g = torch.Generator().manual_seed(23)
     codes = [torch.randint(0, cfg.card, (B, cfg.n_q - cfg.dep_q, 1), generator=g) for _ in range(n)]
