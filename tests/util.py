@@ -383,7 +383,7 @@ def _dep_tensor(sd: dict, name: str, k: int, layer: int | None) -> torch.Tensor:
 
 @torch.no_grad()
 def depformer_ref64(sd: dict, cfg, transformer_out: torch.Tensor, text_token: torch.Tensor, audio_tokens: torch.Tensor,
-                    mutant: dict | None = None, quantize: bool = False) -> dict:
+                    mutant: dict | None = None, quantize: bool = False, din: torch.Tensor | None = None) -> dict:
     """One depformer frame (lm.py:450-493 and 809-850 with transformer.py's weights-per-step layers, as oracle/lm.py
     forward_depformer / depformer_step state it) in float64, teacher-forced: sub-step k's previous token is ``text_token`` [B]
     for k = 0 and ``audio_tokens[k - 1]`` ([dep_q, B], the tokens the model under test sampled) after.  Values are rounded to
@@ -398,6 +398,9 @@ def depformer_ref64(sd: dict, cfg, transformer_out: torch.Tensor, text_token: to
     ties to even, the weight rows quantised through fp16 once (quant.cached_quantize_weight; the gate and value rows of lin_in
     keep their own scales), the exact integer product, dequantised in qlinear_f32's fp32 order.  The RMSNorm, the attention
     and the SiLU stay float64.
+
+    ``din`` (bf16 [B, dep_q, dd], the device's own din) teacher-forces every sub-step's input on it: the returned "din" is still
+    depformer_in[k] of transformer_out, to judge the device's din by.
 
     Returns the checkpoints before their final bf16 rounding, as float64: "din" [B, dep_q, dd] (depformer_in[k] of
     transformer_out), "k" / "v" per layer [B, H, dep_q, 64] (what the layer's per-frame cache holds after the frame) and
@@ -448,7 +451,9 @@ def depformer_ref64(sd: dict, cfg, transformer_out: torch.Tensor, text_token: to
 
     tout = transformer_out.to(f64)
     tokens = [text_token.to(dev)] + [audio_tokens[k].to(dev) for k in range(Q - 1)]
+    din_in = din
     din = torch.stack([lin(tout, "din", k) for k in range(Q)], dim=1)
+    x_din = din if din_in is None else din_in.to(dev, f64)
     kc = [torch.zeros(B, H, Q, D, dtype=f64, device=dev) for _ in range(L)]
     vc = [torch.zeros(B, H, Q, D, dtype=f64, device=dev) for _ in range(L)]
     logits = []
@@ -456,7 +461,7 @@ def depformer_ref64(sd: dict, cfg, transformer_out: torch.Tensor, text_token: to
         prev = mutant["prev"](k, tokens) if "prev" in mutant else tokens[k]
         table = W("emb", k)
         e = table.to(dev)[prev.clamp(min=0)].to(f64) * (prev >= 0)[:, None]          # token -1 -> zero row (lm_utils.py:103-121)
-        x = _bf(_bf(din[:, k]) + e)
+        x = _bf(_bf(x_din[:, k]) + e)
         for layer in range(L):
             xn = rmsnorm(x, W("n1", k, layer))
             qkv = lin(xn, "in", k, layer).view(B, 3, H, D)
@@ -1368,3 +1373,194 @@ def f32_ulp(x: np.ndarray) -> np.ndarray:
     """One fp32 ulp at |x| (the spacing above |x| rounded to fp32)."""
     a = np.abs(np.asarray(x, dtype=np.float32))
     return (np.nextafter(a, np.float32(np.inf)) - a).astype(np.float64)
+
+
+# ---- the plans of the LM's linears and of the fused depformer, as runs of batch sizes ------------------------------------------
+LINEAR_PLAN_FIELDS = ["kernel", "m0", "rows", "grid", "cluster", "smem", "stages", "stage_bytes", "np", "Mpad", "kb_per", "S", "kbps",
+                      "unit_tiles", "ldw", "Wc", "whole_rounds", "sk_tile0", "sk_items"]
+LINEAR_KERNELS = {1: "gemv", 2: "ns", 3: "cluster-sk", 4: "stream-k"}
+DEPFORMER_PHASES = ["in_proj", "out_proj", "linear_in", "linear_out", "head"]
+DEPFORMER_PLAN_FIELDS = ["path", "part_floats", "stages", "stage_bytes", "smem", "grid"] + [
+    f"{p}.{f}" for p in DEPFORMER_PHASES for f in ("n_tiles", "num_kb", "kbps", "S", "A", "N")]
+
+
+def linear_plan(lib, M: int, N: int, K: int, epi: int, gate_rows: int, norm: int, int8: int, sms: int,
+                gemv_max_rows: int) -> tuple[int, list[list[int]]]:
+    """(norm folded, launches) of b200_op_linear_plan: LINEAR_PLAN_FIELDS per launch."""
+    from moshi_b200 import _lib
+    n = len(LINEAR_PLAN_FIELDS)
+    cap = 2 + 4 * n
+    buf = (C.c_int64 * cap)()
+    rc = lib.b200_op_linear_plan(M, N, K, epi, gate_rows, int8, norm, sms, gemv_max_rows, buf, cap)
+    assert rc == _lib.B200_OK, (M, N, K, epi, gate_rows, norm, int8, sms, gemv_max_rows, rc)
+    return int(buf[1]), [list(buf[2 + n * i:2 + n * (i + 1)]) for i in range(int(buf[0]))]
+
+
+def linear_plan_runs(lib, N: int, K: int, epi: int, gate_rows: int, norm: int, int8: int, sms: int, gemv_max_rows: int,
+                     max_m: int = 256) -> list[tuple[int, int, list[list[int]]]]:
+    """The batch sizes 1..max_m of one linear grouped into runs (first M, last M, launches of the first M) of equal plans, as
+    tools/gen_linear_plans.py compresses them: within a run the launches are the same except for the row count of the last."""
+    rows = LINEAR_PLAN_FIELDS.index("rows")
+    runs: list[list] = []
+    for M in range(1, max_m + 1):
+        folded, blocks = linear_plan(lib, M, N, K, epi, gate_rows, norm, int8, sms, gemv_max_rows)
+        if runs:
+            first, _, f0, b0 = runs[-1]
+            grown = [list(b) for b in b0]
+            grown[-1][rows] += M - first
+            if f0 == folded and grown == blocks:
+                runs[-1][1] = M
+                continue
+        runs.append([M, M, folded, blocks])
+    return [(first, last, blocks) for first, last, _, blocks in runs]
+
+
+def depformer_plan(lib, geom, B: int, cfg: int, int8: int, mode: int, sms: int, gemv_max_rows: int) -> list[int]:
+    """b200_op_depformer_plan for `geom` = (dep_q, depformer_dim, heads, ffn, card): DEPFORMER_PLAN_FIELDS."""
+    from moshi_b200 import _lib
+    n = len(DEPFORMER_PLAN_FIELDS)
+    buf = (C.c_int64 * n)()
+    rc = lib.b200_op_depformer_plan(*geom, B, cfg, int8, mode, sms, gemv_max_rows, buf, n)
+    assert rc == _lib.B200_OK, (geom, B, cfg, int8, mode, sms, gemv_max_rows, rc)
+    return list(buf)
+
+
+def depformer_plan_runs(lib, geom, cfg: int, int8: int, mode: int, sms: int, gemv_max_rows: int,
+                        max_b: int = 256) -> list[tuple[int, int, list[int]]]:
+    """The sessions 1..max_b (1..max_b / 2 under guidance) grouped into runs (first B, last B, plan of the first B) of equal
+    depformer plans, as tools/gen_depformer_plans.py compresses them: within a run only the partial-buffer floats change, in
+    proportion to B."""
+    runs: list[list] = []
+    for B in range(1, (max_b // 2 if cfg else max_b) + 1):
+        p = depformer_plan(lib, geom, B, cfg, int8, mode, sms, gemv_max_rows)
+        if runs:
+            first, _, p0 = runs[-1]
+            grown = list(p0)
+            grown[1] = p0[1] // first * B
+            if grown == p:
+                runs[-1][1] = B
+                continue
+        runs.append([B, B, p])
+    return [tuple(r) for r in runs]
+
+
+# ---- one linear against fp64 -----------------------------------------------------------------------------------------------
+# Acceptance rule of one LM linear y = epi(x . W^T) (bf16 operands, fp32 accumulation): y must be a faithful bf16 rounding of
+# the fp64 reference, where the product may be off by LINEAR_C * 2^-24 * sum_k |x_k w_k| (an fp32 sum in another order; it only
+# decides near-zero outputs and rounding boundaries), every intermediate the epilogue rounds to bf16 (the residual add's
+# update, the gated MLP's gate and value, the RMSNorm output folded into the GEMV) may be either faithful rounding of its
+# reference, and silu one bf16 ulp off (or -0 where fp32's exp(-g) overflows).  A lost or doubled k-block, a lost K tail of 8 columns, a partial added twice, a wrong
+# row or a wrong weight tile moves outputs by many ulps: tests/test_plan_runs_cpu.py shows that the rule rejects each of them.
+# On one H100 every linear plan of tests/test_gpu_zz_plan_runs.py needed LINEAR_C of at most 4.
+STORE, RESADD, GATE = 0, 1, 2
+LINEAR_C = 32.0
+# the RMSNorm the GEMV folds in is fp32: where fp64 puts an element within NORM_BAND (relative) of a bf16 midpoint, the kernel
+# may round it the other way
+NORM_BAND = 2.0 ** -16
+_SILU_ARGMIN = -1.2784645427610738
+
+
+def _bf_grid(v: torch.Tensor) -> torch.Tensor:
+    """Spacing of bf16 numbers in the binade of each |v| (float64; 2^-133 below the smallest normal)."""
+    _, e = torch.frexp(v)
+    return torch.ldexp(torch.ones_like(v), (e - 8).clamp(min=-133))
+
+
+def bf_floor(v: torch.Tensor) -> torch.Tensor:
+    """The largest bf16 number <= v (float64 in, float64 out)."""
+    sp = _bf_grid(v)
+    return torch.floor(v / sp) * sp
+
+
+def bf_ceil(v: torch.Tensor) -> torch.Tensor:
+    """The smallest bf16 number >= v (float64 in, float64 out)."""
+    sp = _bf_grid(v)
+    return torch.ceil(v / sp) * sp
+
+
+def bf_next_up(v: torch.Tensor) -> torch.Tensor:
+    """The bf16 number after the bf16 number v (float64)."""
+    m, e = torch.frexp(v)
+    sp = torch.ldexp(torch.ones_like(v), (e - 8).clamp(min=-133))
+    sp = torch.where(m == -0.5, sp / 2, sp)              # from -2^k up: the spacing of the binade below 2^k
+    return torch.where(v == 0, torch.full_like(v, 2.0 ** -133), v + sp)
+
+
+def bf_next_down(v: torch.Tensor) -> torch.Tensor:
+    return -bf_next_up(-v)
+
+
+def _silu64(v: torch.Tensor) -> torch.Tensor:
+    return v / (1.0 + torch.exp(-v))
+
+
+def linear_ref64(x: torch.Tensor, w: torch.Tensor, epi: int = STORE, gate_rows: int = 0, res: torch.Tensor | None = None,
+                 alpha: torch.Tensor | None = None) -> dict:
+    """fp64 reference of y = epi(x . w^T) (w [N, K], gated: rows gate | value) on the operands' device: the product ``acc``,
+    ``mag`` = sum_k |x_k w_k|, and, with ``alpha``, the product of bf16(rmsnorm_ref64(x, alpha)) plus in ``norm_slack`` what
+    rounding its elements within NORM_BAND of a midpoint the other way can move it."""
+    xd = x.double()
+    wd, wa = w.double(), w.double().abs()
+    norm_slack = None
+    if alpha is not None:
+        xn = rmsnorm_ref64(x, alpha)
+        xd = _bf(xn)
+        norm_slack = (_bf(xn * (1 + NORM_BAND)) - _bf(xn * (1 - NORM_BAND))).abs() @ wa.t()
+    return dict(acc=xd @ wd.t(), mag=xd.abs() @ wa.t(), norm_slack=norm_slack, epi=epi, gate_rows=gate_rows,
+                res=None if res is None else res.to(xd.device, torch.float64))
+
+
+def linear_bounds(ref: dict, c: float = LINEAR_C) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """(lowest, highest, nominal) output the rule of LINEAR_C accepts, per element (float64)."""
+    acc = ref["acc"]
+    s = c * 2.0 ** -24 * ref["mag"]
+    if ref["norm_slack"] is not None:
+        s = s + ref["norm_slack"]
+    t_lo, t_hi = bf_floor(acc - s), bf_ceil(acc + s)
+    if ref["epi"] == STORE:
+        return t_lo, t_hi, acc
+    if ref["epi"] == RESADD:
+        r = ref["res"]
+        return bf_floor(r + t_lo), bf_ceil(r + t_hi), r + _bf(acc)
+    H = ref["gate_rows"]
+    g_lo, g_hi, u_lo, u_hi = t_lo[:, :H], t_hi[:, :H], t_lo[:, H:], t_hi[:, H:]
+    a, b = _silu64(g_lo), _silu64(g_hi)
+    s_lo = torch.minimum(a, b)
+    s_lo = torch.where((g_lo <= _SILU_ARGMIN) & (g_hi >= _SILU_ARGMIN), _silu64(torch.full_like(s_lo, _SILU_ARGMIN)), s_lo)
+    s_hi = torch.maximum(a, b)
+    # an fp32 silu g / (1 + exp(-g)) is -0 once exp(-g) overflows (g < -88.7, where silu > -2^-121)
+    s_hi = torch.where(s_lo > -2.0 ** -100, s_hi.clamp(min=0.0), s_hi)
+    s_lo, s_hi = bf_next_down(bf_floor(s_lo)), bf_next_up(bf_ceil(s_hi))        # silu one bf16 ulp off
+    corners = torch.stack([s_lo * u_lo, s_lo * u_hi, s_hi * u_lo, s_hi * u_hi])
+    nominal = _bf(_silu64(_bf(acc[:, :H]))) * _bf(acc[:, H:])
+    return bf_floor(corners.amin(0)), bf_ceil(corners.amax(0)), nominal
+
+
+def linear_ratios(y: torch.Tensor, ref: dict, c: float = LINEAR_C) -> torch.Tensor:
+    """Per output element, how far y sits from the nominal reference toward the bound the rule accepts on its side (<= 1
+    passes; a NaN never does).  A faithful rounding on the far side of the reference sits on that bound and scores exactly 1,
+    so past pass / fail the ratio says little; linear_c_needed grades a passing output."""
+    lo, hi, nom = linear_bounds(ref, c)
+    y = y.detach().to(nom.device, torch.float64).reshape(nom.shape)
+    r = torch.where(y > nom, (y - nom) / (hi - nom), torch.where(y < nom, (nom - y) / (nom - lo), torch.zeros_like(y)))
+    return torch.nan_to_num(r, nan=math.inf, posinf=math.inf)
+
+
+def linear_c_needed(y: torch.Tensor, ref: dict) -> float:
+    """The smallest of 0, 2^-6 LINEAR_C, ..., LINEAR_C under which y passes (inf if none does)."""
+    for c in [0.0] + [LINEAR_C * 2.0 ** -i for i in range(6, -1, -1)]:
+        if float(linear_ratios(y, ref, c).max()) <= 1:
+            return c
+    return math.inf
+
+
+def linear_rows(M: int, K: int, gen: torch.Generator, device: str = "cpu") -> torch.Tensor:
+    """bf16 [M, K] activations of the linear tests: randn rows, row 0 scaled by 1e-3, row M - 1 by 1e3 and row M // 2 zero (where
+    those rows are distinct)."""
+    x = torch.randn(M, K, generator=gen, device=device)
+    used = set()
+    for m, scale in ((0, 1e-3), (M - 1, 1e3), (M // 2, 0.0)):
+        if m not in used:
+            x[m] *= scale
+            used.add(m)
+    return x.bfloat16()
