@@ -483,6 +483,16 @@ int b200_op_linear_plan(int M, int N, int K, int epi, int gate_rows, int int8, i
  * at out, at least 36.  B200_ERR_INVALID for out-of-range input and for a configuration the kernel refuses. */
 int b200_op_depformer_plan(int dep_q, int depformer_dim, int depformer_num_heads, int depformer_ffn_hidden, int card, int batch,
                            int cfg, int int8, int mode, int sms, int gemv_max_rows, int64_t* out, int capacity);
+/* What one Mimi frame launches at `batch` sessions (b200_mimi_streaming_begin's plan; needs no GPU), for a device of `sms`
+ * multiprocessors and `num_codebooks` active codebooks.  out[0..5] = tensor-core layers of the encoder SEANet and of the
+ * decoder SEANet, K slices of the down-sampling conv, split-K workspace bytes, kernels of one encode frame (RVQ included) and
+ * of one decode frame (a split layer counts its reduction); then 21 values per tensor-core layer (encoder SEANet, decoder
+ * SEANet, then the transformers' in_proj, out_proj, linear1, linear2, each serving every layer of both): SEANet layer index
+ * (0..3 for the linears), kind (0 conv, 1 transposed conv, 2 linear), Cin, N, taps, dilation, stride, features per tile,
+ * feature tiles, k-blocks, tile steps tt, tile sessions bb, steps per session T, sessions, row tiles, K splits, k-blocks per
+ * split, stages, stage bytes, grid, dynamic shared memory.  `capacity` int64 slots at out (6 + 21 * layers; 1024 suffice for
+ * the default configuration).  B200_ERR_INVALID for out-of-range input and for a configuration b200_mimi_create refuses. */
+int b200_op_mimi_plan(const b200_mimi_config* cfg, int batch, int sms, int num_codebooks, int64_t* out, int capacity);
 /* int8 x int8 linear (QLinear, utils/quantize.py:13-40: bitsandbytes row-wise absmax quantisation of weights and
  * activations, int32 accumulation, dequantisation by both row scales / 127^2), on wgmma s8 x s8 -> s32.
  *   b200_op_quant_pack_tiles: w bf16 [N,K] -> int8 SWIZZLE_128B tiles (b200_op_packed_bytes_i8 bytes) + scales f32 [N]

@@ -142,6 +142,7 @@ _PROTOTYPES: dict[str, tuple[tp.Any, list]] = {
     "b200_op_set_gemv_max_rows": (_I, [_I]),
     "b200_op_linear_plan": (_I, [_I, _I, _I, _I, _I, _I, _I, _I, _I, C.POINTER(C.c_int64), _I]),
     "b200_op_depformer_plan": (_I, [_I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, C.POINTER(C.c_int64), _I]),
+    "b200_op_mimi_plan": (_I, [C.POINTER(MimiConfigC), _I, _I, _I, C.POINTER(C.c_int64), _I]),
     "b200_op_packed_bytes_i8": (C.c_int64, [_I, _I, _I, _I]),
     "b200_op_quant_pack_tiles": (_I, [_P, _P, _P, _I, _I, _I, _I, _P]),
     "b200_op_quantize_rows": (_I, [_P, _P, _P, _I, _I, _P]),

@@ -11,13 +11,12 @@
 #include "mimi_kernels.cuh"
 #include "mimi_tc.cuh"
 #include "mimi_tm_kernels.cuh"
+#include "tc_host.cuh"
 
 using namespace b200;
 using namespace b200::mimi;
 
 namespace {
-
-constexpr size_t kTcSplitBytes = (size_t)64 << 20;   // split-K partials budget of a tensor-core layer (tc_plan)
 
 struct SeaLayer {
   int kind = 0;              // 0 = StreamingConv1d, 1 = StreamingConvTranspose1d
@@ -62,18 +61,31 @@ struct DownLayer {             // ConvDownsample1d (resample.py:14-65): k = 2 * 
   uint8_t* first = nullptr;    // replicate flags [B]
 };
 
+// what the configuration fixes (plan_seanet): frame geometry, layer lists, the tensor-core layers' shapes
+struct MimiShape {
+  b200_mimi_config cfg;
+  int frame_size = 0, hop = 0, rs = 0;       // rs = resample stride (2)
+  std::vector<SeaLayer> enc, dec;
+  DownLayer down;                            // learnt down-sampling conv (replicate padding): split-K fp32 SIMT kernels
+  mtc::TcShape in_proj, out_proj, linear1, linear2;   // every layer of both transformers
+};
+
+// what one frame of B sessions launches (plan_mimi)
+struct MimiPlan {
+  std::vector<mtc::TcSchedule> enc, dec;     // per SEANet layer (the SIMT layers' entries stay empty)
+  mtc::TcSchedule in_proj, out_proj, linear1, linear2;   // both transformers run rs tokens per session
+  int down_ksplit = 0;                       // K slices of the down-sampling conv
+  size_t ws_bytes = 0;                       // split-K workspace
+  int enc_launches = 0, dec_launches = 0;    // kernels of one encode frame (RVQ included) and of one decode frame
+};
+
 }  // namespace
 
-struct b200_mimi : StreamCore {     // graphs[ENC_GRAPH] / graphs[DEC_GRAPH]: one frame's encode / decode
-  b200_mimi_config cfg;
+struct b200_mimi : StreamCore, MimiShape {     // graphs[ENC_GRAPH] / graphs[DEC_GRAPH]: one frame's encode / decode
   TensorStore store;
   Arena weights;
   int num_codebooks = 8;
-  int frame_size = 0, hop = 0, rs = 0;       // rs = resample stride (2)
-  int sms = 148;
 
-  std::vector<SeaLayer> enc, dec;
-  DownLayer down;                            // learnt down-sampling conv (replicate padding): split-K fp32 SIMT kernels
   // up-sampling (depth-wise convtr)
   float *up_w = nullptr, *up_partial = nullptr, *up_scratch = nullptr;
   Transformer enc_tr, dec_tr;
@@ -115,10 +127,25 @@ enum { ENC_GRAPH, DEC_GRAPH };
 // ---------------------------------------------------------------------------------------------
 // structure (seanet.py:170-236, 323-388; resample.py; loaders.py:38-88)
 // ---------------------------------------------------------------------------------------------
-void plan_seanet(b200_mimi* h) {
-  const auto& c = h->cfg;
-  h->enc.clear();
-  h->dec.clear();
+// Everything the configuration fixes, or why mimi_create refuses it: frame geometry, both SEANets' layers with their steps
+// per frame in and out, carried rows P and GEMM widths N, the down-sampling conv and the tensor-core layers' shapes.
+int plan_seanet(const b200_mimi_config& c, MimiShape* g) {
+  if (c.n_ratios < 1 || c.n_ratios > 8) B200_FAIL(B200_ERR_INVALID, "mimi_create: n_ratios out of range");
+  if (c.channels != 1) B200_FAIL(B200_ERR_INVALID, "mimi_create: only mono audio is on the hot path");
+  if (c.q_dimension % 8) B200_FAIL(B200_ERR_INVALID, "mimi_create: codebook dimension must be a multiple of 8");
+  if (c.tr_d_model / c.tr_num_heads != 64) B200_FAIL(B200_ERR_INVALID, "mimi_create: head dim must be 64");
+  if (c.tr_d_model != c.dimension) B200_FAIL(B200_ERR_INVALID, "mimi_create: projected transformer unsupported");
+  if (c.n_filters % 32 || c.compress != 2 || c.n_filters / c.compress % 32)
+    B200_FAIL(B200_ERR_INVALID, "mimi_create: SEANet channel counts must be multiples of 32 (tensor-core k-blocks)");
+  g->cfg = c;
+  g->hop = 1;
+  for (int i = 0; i < c.n_ratios; ++i) g->hop *= c.ratios[i];
+  g->frame_size = (int)(c.sample_rate / c.frame_rate);
+  const double enc_rate = (double)c.sample_rate / g->hop;
+  g->rs = (int)(enc_rate / c.frame_rate);
+  if (g->rs < 1 || g->frame_size != g->hop * g->rs) B200_FAIL(B200_ERR_INVALID, "mimi_create: frame size %d is not hop*stride", g->frame_size);
+  g->enc.clear();
+  g->dec.clear();
   auto conv = [](const std::string& key, int cin, int cout, int k, int stride, int dil, bool elu) {
     SeaLayer l;
     l.kind = 0; l.key = key; l.cin = cin; l.cout = cout; l.k = k; l.stride = stride; l.dil = dil; l.elu_in = elu;
@@ -128,7 +155,7 @@ void plan_seanet(b200_mimi* h) {
   {
     auto l = conv("encoder.model.0.conv.conv", c.channels, mult * c.n_filters, c.kernel_size, 1, 1, false);
     l.tap = "enc.0";
-    h->enc.push_back(l);
+    g->enc.push_back(l);
   }
   idx = 1;
   for (int ri = c.n_ratios - 1; ri >= 0; --ri) {
@@ -140,16 +167,16 @@ void plan_seanet(b200_mimi* h) {
       const std::string base = "encoder.model." + std::to_string(idx);
       auto a = conv(base + ".block.1.conv.conv", ch, ch / c.compress, c.residual_kernel_size, 1, dil, true);
       auto b = conv(base + ".block.3.conv.conv", ch / c.compress, ch, 1, 1, 1, true);
-      b.res_from = (int)h->enc.size() - 1;      // skip connection: the input of the block = the previous module's raw output
+      b.res_from = (int)g->enc.size() - 1;      // skip connection: the input of the block = the previous module's raw output
       b.tap = "enc." + std::to_string(idx);
-      h->enc.push_back(a);
-      h->enc.push_back(b);
+      g->enc.push_back(a);
+      g->enc.push_back(b);
       ++idx;
     }
     ++idx;  // ELU
     auto l = conv("encoder.model." + std::to_string(idx) + ".conv.conv", ch, ch * 2, 2 * ratio, ratio, 1, true);
     l.tap = "enc." + std::to_string(idx);
-    h->enc.push_back(l);
+    g->enc.push_back(l);
     ++idx;
     mult *= 2;
   }
@@ -158,7 +185,7 @@ void plan_seanet(b200_mimi* h) {
     auto l = conv("encoder.model." + std::to_string(idx) + ".conv.conv", mult * c.n_filters, c.dimension,
                   c.last_kernel_size, 1, 1, true);
     l.tap = "enc." + std::to_string(idx);
-    h->enc.push_back(l);
+    g->enc.push_back(l);
   }
 
   idx = 0;
@@ -166,7 +193,7 @@ void plan_seanet(b200_mimi* h) {
   {
     auto l = conv("decoder.model.0.conv.conv", c.dimension, mult * c.n_filters, c.kernel_size, 1, 1, false);
     l.tap = "dec.0";
-    h->dec.push_back(l);
+    g->dec.push_back(l);
   }
   idx = 1;
   for (int ri = 0; ri < c.n_ratios; ++ri) {
@@ -177,7 +204,7 @@ void plan_seanet(b200_mimi* h) {
     t.kind = 1; t.key = "decoder.model." + std::to_string(idx) + ".convtr.convtr";
     t.cin = ch; t.cout = ch / 2; t.k = 2 * ratio; t.stride = ratio; t.elu_in = true;
     t.tap = "dec." + std::to_string(idx);
-    h->dec.push_back(t);
+    g->dec.push_back(t);
     ++idx;
     for (int j = 0; j < c.n_residual_layers; ++j) {
       int dil = 1;
@@ -185,10 +212,10 @@ void plan_seanet(b200_mimi* h) {
       const std::string base = "decoder.model." + std::to_string(idx);
       auto a = conv(base + ".block.1.conv.conv", ch / 2, ch / 2 / c.compress, c.residual_kernel_size, 1, dil, true);
       auto b = conv(base + ".block.3.conv.conv", ch / 2 / c.compress, ch / 2, 1, 1, 1, true);
-      b.res_from = (int)h->dec.size() - 1;
+      b.res_from = (int)g->dec.size() - 1;
       b.tap = "dec." + std::to_string(idx);
-      h->dec.push_back(a);
-      h->dec.push_back(b);
+      g->dec.push_back(a);
+      g->dec.push_back(b);
       ++idx;
     }
     mult /= 2;
@@ -198,19 +225,78 @@ void plan_seanet(b200_mimi* h) {
     auto l = conv("decoder.model." + std::to_string(idx) + ".conv.conv", c.n_filters, c.channels,
                   c.last_kernel_size, 1, 1, true);
     l.tap = "dec." + std::to_string(idx);
-    h->dec.push_back(l);
+    g->dec.push_back(l);
   }
-  for (auto* layers : {&h->enc, &h->dec})
+  for (auto* layers : {&g->enc, &g->dec}) {
+    int t = layers == &g->enc ? g->frame_size : g->rs;
     for (auto& l : *layers) {
       l.simt_first = l.kind == 0 && l.cin == 1;
       l.simt_last = l.kind == 0 && l.cout == 1;
       l.N = l.kind == 1 ? l.stride * l.cout : l.cout;
       l.P = l.kind == 1 ? 1 : (l.k - 1) * l.dil + 1 - l.stride;
+      l.t_in = t;
+      if (l.kind == 0) {
+        if (t % l.stride) B200_FAIL(B200_ERR_INVALID, "%s: %d samples not divisible by stride %d", l.key.c_str(), t, l.stride);
+        l.t_out = t / l.stride;
+      } else {
+        l.t_out = t;                            // GEMM rows per session; each row holds `stride` output steps
+      }
+      t = l.kind == 1 ? l.t_out * l.stride : l.t_out;
+      if (!l.simt_first && !l.simt_last)
+        l.tc.s = l.kind == 0 ? mtc::tc_shape(mtc::TC_CONV, l.N, l.cin, l.k, l.dil, l.stride, l.cout)
+                             : mtc::tc_shape(mtc::TC_CONVTR, l.N, l.cin, 2, 1, 1, l.cout);
     }
-  h->down = DownLayer();
-  h->down.key = "downsample.conv.conv.conv"; h->down.cin = c.dimension; h->down.cout = c.dimension;
-  h->down.k = 2 * h->rs; h->down.stride = h->rs;
-  h->down.t_in = h->rs; h->down.t_out = 1; h->down.P = h->down.k - h->down.stride;   // the encoder transformer's rs tokens -> one frame
+    if (layers == &g->enc && t != g->rs) B200_FAIL(B200_ERR_INVALID, "encoder yields %d tokens/frame, expected %d", t, g->rs);
+  }
+  if (g->dec.back().t_out != g->frame_size) B200_FAIL(B200_ERR_INVALID, "decoder yields %d samples/frame", g->dec.back().t_out);
+  g->down = DownLayer();
+  g->down.key = "downsample.conv.conv.conv"; g->down.cin = c.dimension; g->down.cout = c.dimension;
+  g->down.k = 2 * g->rs; g->down.stride = g->rs;
+  g->down.t_in = g->rs; g->down.t_out = 1; g->down.P = g->down.k - g->down.stride;   // the encoder transformer's rs tokens -> one frame
+  const int d = c.tr_d_model, ff = c.tr_dim_feedforward;
+  g->in_proj = mtc::tc_shape(mtc::TC_LINEAR, 3 * d, d, 1);
+  g->out_proj = mtc::tc_shape(mtc::TC_LINEAR, d, d, 1);
+  g->linear1 = mtc::tc_shape(mtc::TC_LINEAR, ff, d, 1);
+  g->linear2 = mtc::tc_shape(mtc::TC_LINEAR, d, ff, 1);
+  return B200_OK;
+}
+
+// The schedule of every tensor-core layer at B sessions, the split-K workspace and the kernels one frame launches
+// (encode_body + quantize_frame, dequantize_cols + decode_latent_body; a split layer adds its reduction); no CUDA call.
+int plan_mimi(const MimiShape& g, int B, int sms, int num_codebooks, MimiPlan* out) {
+  const auto& c = g.cfg;
+  MimiPlan q;
+  int sea[2] = {0, 0}, commit[2] = {0, 0};
+  for (int w = 0; w < 2; ++w) {
+    const std::vector<SeaLayer>& layers = w == 0 ? g.enc : g.dec;
+    std::vector<mtc::TcSchedule>& s = w == 0 ? q.enc : q.dec;
+    s.resize(layers.size());
+    for (size_t i = 0; i < layers.size(); ++i) {
+      const SeaLayer& l = layers[i];
+      if (!l.simt_first && !l.simt_last) B200_TRY(mtc::plan_tc(l.tc.s, B, l.t_out, sms, mtc::TC_SPLIT_BYTES, &s[i]));
+      sea[w] += 1 + (s[i].ksplit > 1);
+      if (l.P > 0) commit[w] = 1;             // tm_commit_kernel
+    }
+  }
+  B200_TRY(mtc::plan_tc(g.in_proj, B, g.rs, sms, mtc::TC_SPLIT_BYTES, &q.in_proj));
+  B200_TRY(mtc::plan_tc(g.out_proj, B, g.rs, sms, mtc::TC_SPLIT_BYTES, &q.out_proj));
+  B200_TRY(mtc::plan_tc(g.linear1, B, g.rs, sms, mtc::TC_SPLIT_BYTES, &q.linear1));
+  B200_TRY(mtc::plan_tc(g.linear2, B, g.rs, sms, mtc::TC_SPLIT_BYTES, &q.linear2));
+  // per layer: two LayerNorms, the attention step and four linears; then advance_offsets
+  int tr = 7;
+  for (const auto* s : {&q.in_proj, &q.out_proj, &q.linear1, &q.linear2}) tr += s->ksplit > 1;
+  tr = c.tr_num_layers * tr + 1;
+  // the down-sampling conv's partials outgrow the tensor-core layers' budget above 1024 sessions
+  q.down_ksplit = ds_splits(g.down.cin * g.down.k);
+  const size_t down_bytes = (size_t)q.down_ksplit * B * g.down.t_out * g.down.cout * 4;
+  q.ws_bytes = down_bytes > mtc::TC_SPLIT_BYTES ? down_bytes : mtc::TC_SPLIT_BYTES;
+  const int semantic = std::min(c.q_n_semantic, num_codebooks), levels = std::max(semantic, num_codebooks - semantic);
+  // encode: SEANet, transformer, down conv + reduction, conv_commit (+ tm_commit), RVQ projection + search / pick per level
+  q.enc_launches = sea[0] + tr + 2 + 1 + commit[0] + 1 + 2 * levels;
+  // decode: RVQ decode, up-sampling, transformer, SEANet, (tm_commit +) convtr_commit
+  q.dec_launches = 2 + tr + sea[1] + commit[1] + 1;
+  *out = q;
+  return B200_OK;
 }
 
 int get_f32(b200_mimi* h, const std::string& name, std::vector<int64_t> shape, const float** out) {
@@ -226,15 +312,15 @@ int get_f32(b200_mimi* h, const std::string& name, std::vector<int64_t> shape, c
   return B200_OK;
 }
 
-// nn.Linear-shaped weight [N][n_taps * Cin] (fp32, device) -> packed hi / lo tiles owned by the handle
-int pack_tc(b200_mimi* h, mtc::TcLayer& L, const float* w_ntc, int N, int Cin, int n_taps) {
-  if (Cin % mtc::TC_KB || N % 16 || (N > mtc::TC_MAX_NT && N % mtc::TC_MAX_NT))
-    B200_FAIL(B200_ERR_INVALID, "mimi: a %d x %d (x %d taps) contraction does not tile on the tensor-core kernel", N, Cin, n_taps);
-  mtc::tc_set_shape(L, N, Cin, n_taps);
-  const size_t bytes = mtc::tc_packed_bytes(L);
+// nn.Linear-shaped weight [N][n_taps * Cin] (fp32, device) -> packed hi / lo tiles of L's shape owned by the handle
+int pack_tc(b200_mimi* h, mtc::TcLayer& L, const float* w_ntc) {
+  const mtc::TcShape& s = L.s;
+  if (s.Cin % mtc::TC_KB || s.N % 16 || (s.N > mtc::TC_MAX_NT && s.N % mtc::TC_MAX_NT))
+    B200_FAIL(B200_ERR_INVALID, "mimi: a %d x %d (x %d taps) contraction does not tile on the tensor-core kernel", s.N, s.Cin, s.n_taps);
+  const size_t bytes = mtc::tc_packed_bytes(s);
   void* out = nullptr;
   B200_TRY(h->weights.alloc(&out, bytes, false));
-  B200_TRY(mtc::tc_pack_weights(w_ntc, out, L, nullptr));
+  B200_TRY(mtc::tc_pack_weights(w_ntc, out, s, nullptr));
   L.wt = static_cast<uint8_t*>(out);
   h->weight_bytes += (int64_t)bytes;
   return B200_OK;
@@ -264,10 +350,8 @@ int pack_sea(b200_mimi* h, SeaLayer& l) {
     B200_TRY(tmp.alloc_t(&wk, (size_t)n, false));
     if (l.kind == 0) B200_LAUNCH(tm_weight_conv_kernel, (unsigned)ceil_div64(n, 256), 256, 0, 0, w, wk, l.cout, l.cin, l.k);
     else B200_LAUNCH(tm_weight_convtr_kernel, (unsigned)ceil_div64(n, 256), 256, 0, 0, w, wk, l.cin, l.cout, l.stride);
-    B200_TRY(pack_tc(h, l.tc, wk, l.N, l.cin, l.kind == 0 ? l.k : 2));
+    B200_TRY(pack_tc(h, l.tc, wk));
     B200_CUDA(cudaDeviceSynchronize());
-    l.tc.kind = l.kind; l.tc.dil = l.kind == 0 ? l.dil : 1; l.tc.stride = l.kind == 0 ? l.stride : 1;
-    l.tc.bias_mod = l.cout;
   }
   const float* b = nullptr;
   B200_TRY(get_f32(h, l.key + ".bias", {l.cout}, &b));
@@ -308,11 +392,11 @@ int keep(b200_mimi* h, const std::string& name, std::vector<int64_t> shape, cons
   return B200_OK;
 }
 
-int keep_linear(b200_mimi* h, const std::string& name, int M, int K, mtc::TcLayer& L) {
+int keep_linear(b200_mimi* h, const std::string& name, const mtc::TcShape& s, mtc::TcLayer& L) {
   const float* src = nullptr;
-  B200_TRY(get_f32(h, name, {M, K}, &src));
-  B200_TRY(pack_tc(h, L, src, M, K, 1));       // nn.Linear weight [out][in] is already [N][K]
-  L.kind = 2; L.dil = 1; L.stride = 1; L.bias = nullptr; L.bias_mod = M;
+  B200_TRY(get_f32(h, name, {s.N, s.Cin}, &src));
+  L.s = s;
+  B200_TRY(pack_tc(h, L, src));                // nn.Linear weight [out][in] is already [N][K]
   B200_CUDA(cudaDeviceSynchronize());
   h->store.release(name);
   return B200_OK;
@@ -320,19 +404,19 @@ int keep_linear(b200_mimi* h, const std::string& name, int M, int K, mtc::TcLaye
 
 int pack_transformer(b200_mimi* h, const std::string& prefix, Transformer& tr) {
   const auto& c = h->cfg;
-  const int d = c.tr_d_model, ff = c.tr_dim_feedforward;
+  const int d = c.tr_d_model;
   tr.layers.resize(c.tr_num_layers);
   for (int li = 0; li < c.tr_num_layers; ++li) {
     const std::string p = prefix + ".transformer.layers." + std::to_string(li);
     TrLayer& L = tr.layers[li];
-    B200_TRY(keep_linear(h, p + ".self_attn.in_projs.0.weight", 3 * d, d, L.in_proj));
-    B200_TRY(keep_linear(h, p + ".self_attn.out_projs.0.weight", d, d, L.out_proj));
+    B200_TRY(keep_linear(h, p + ".self_attn.in_projs.0.weight", h->in_proj, L.in_proj));
+    B200_TRY(keep_linear(h, p + ".self_attn.out_projs.0.weight", h->out_proj, L.out_proj));
     B200_TRY(keep(h, p + ".norm1.weight", {d}, &L.n1w));
     B200_TRY(keep(h, p + ".norm1.bias", {d}, &L.n1b));
     B200_TRY(keep(h, p + ".norm2.weight", {d}, &L.n2w));
     B200_TRY(keep(h, p + ".norm2.bias", {d}, &L.n2b));
-    B200_TRY(keep_linear(h, p + ".linear1.weight", ff, d, L.l1));
-    B200_TRY(keep_linear(h, p + ".linear2.weight", d, ff, L.l2));
+    B200_TRY(keep_linear(h, p + ".linear1.weight", h->linear1, L.l1));
+    B200_TRY(keep_linear(h, p + ".linear2.weight", h->linear2, L.l2));
     B200_TRY(keep(h, p + ".layer_scale_1.scale", {d}, &L.ls1));
     B200_TRY(keep(h, p + ".layer_scale_2.scale", {d}, &L.ls2));
   }
@@ -480,7 +564,7 @@ int encode_body(b200_mimi* h) {
   {
     // deep and skinny (2048 reduction steps, N = sessions): the reduction cut over KS CTAs per 64 outputs, slices added in order
     const ConvSplitK p = down_conv(h);
-    const int KS = ceil_div(p.Kd, DS_KP);
+    const int KS = ds_splits(p.Kd);
     dim3 g1(ceil_div(p.M, DS_CO), KS);
     B200_LAUNCH(conv_splitk_kernel, g1, 256, 0, h->body, p, h->splitk_ws, KS);
     B200_LAUNCH(conv_splitk_reduce_kernel, (unsigned)ceil_div64((long long)p.N * p.M, 256), 256, 0, h->body, p, h->splitk_ws, KS);
@@ -566,17 +650,62 @@ int decode_latent_body(b200_mimi* h) {
 
 void register_tap(b200_mimi* h, const std::string& name, const float* p, int C, int T, bool transpose) { h->taps[name] = Tap{p, C, T, transpose}; }
 
-// Plans one tensor-core layer for B sessions of T GEMM rows: A maps over `in_hi / in_lo` ([B][rows][Cin]), epilogue pointers set
-// by the caller in L.p beforehand (y / res / act); this fills geometry, schedule and tensor maps.
-int plan_layer(b200_mimi* h, mtc::TcLayer& L, const float* in_hi, const float* in_lo, int rows_per_session, int row0, int T) {
-  const int B = h->batch;
-  int tt = 0, bb = 0;
-  if (mtc::tc_tile_shape(T, L.stride, &tt, &bb) != B200_OK) B200_FAIL(B200_ERR_INVALID, "mimi: %d steps per frame do not tile", T);
-  L.p.tt = tt; L.p.bb = bb; L.p.row0 = row0;
-  L.p.ws = h->splitk_ws;
-  B200_TRY(mtc::tc_make_map(&L.map_hi, in_hi, L.Cin, rows_per_session, (long long)rows_per_session * L.Cin, B, tt, bb, L.stride));
-  B200_TRY(mtc::tc_make_map(&L.map_lo, in_lo, L.Cin, rows_per_session, (long long)rows_per_session * L.Cin, B, tt, bb, L.stride));
-  return mtc::tc_plan(L, B, T, h->sms, kTcSplitBytes);
+// A SEANet's buffers for B sessions: every layer owns its extended input; raw outputs where something reads them
+int alloc_seanet(b200_mimi* h, std::vector<SeaLayer>& layers, int B, bool is_dec, std::vector<TmCommit>& commits, long long& max_rows) {
+  Arena& A = h->state;
+  for (size_t i = 0; i < layers.size(); ++i) {
+    SeaLayer& l = layers[i];
+    const size_t ext_n = (size_t)B * (l.P + l.t_in) * l.cin;
+    B200_TRY(A.alloc_t(&l.ext_hi, ext_n));
+    if (!l.simt_first && !l.simt_last) B200_TRY(A.alloc_t(&l.ext_lo, ext_n));
+    else l.ext_lo = nullptr;
+    if (l.P > 0) {
+      TmCommit cm;
+      cm.hi = l.ext_hi; cm.lo = l.ext_lo; cm.P = l.P; cm.T = l.t_in; cm.rowlen = l.cin; cm.sb = (long long)(l.P + l.t_in) * l.cin;
+      commits.push_back(cm);
+      if ((long long)B * l.cin > max_rows) max_rows = (long long)B * l.cin;
+    }
+    const int steps_out = l.kind == 1 ? l.t_out * l.stride : l.t_out;
+    const bool is_last = i + 1 == layers.size();
+    l.y = nullptr;
+    if (is_last && !is_dec) l.y = h->tok_in_enc;                       // transformer input
+    else if (is_last && is_dec) l.y = h->out_frame;
+    else if (!l.tap.empty()) B200_TRY(A.alloc_t(&l.y, (size_t)B * steps_out * l.cout));
+    if (!l.tap.empty() && l.y) register_tap(h, l.tap, l.y, l.cout, steps_out, !(is_last && !is_dec));
+  }
+  return B200_OK;
+}
+
+// the activation a tensor-core layer writes for its consumer nx (ELU applied where nx wants it) behind nx's carried rows;
+// a_row = the producer's N (= stride * nx.cin for a convtr: `stride` consumer rows per GEMM row)
+void feed(mtc::TcParams& e, const SeaLayer& nx, int a_row) {
+  e.act_mode = nx.simt_last ? mtc::TC_ACT_FULL : mtc::TC_ACT_SPLIT;
+  e.act_elu = nx.elu_in ? 1 : 0;
+  e.a_hi = nx.ext_hi + (long long)nx.P * nx.cin;
+  e.a_lo = nx.ext_lo ? nx.ext_lo + (long long)nx.P * nx.cin : nullptr;
+  e.a_sb = (long long)(nx.P + nx.t_in) * nx.cin;
+  e.a_row = a_row;
+}
+
+// Binds a SEANet's tensor-core layers to their schedules: layer i writes its raw output and the activation layer i + 1 reads.
+// conv: GEMM row t reads ext rows t * stride + tap * dil (ext row 0 = oldest carried sample)
+// convtr: GEMM row t reads ext rows t + slot, slot 0 = x[t-1] (ext row 0 = the carried previous step)
+int bind_seanet(b200_mimi* h, std::vector<SeaLayer>& layers, const std::vector<mtc::TcSchedule>& sched) {
+  for (size_t i = 0; i < layers.size(); ++i) {
+    SeaLayer& l = layers[i];
+    if (l.simt_first || l.simt_last) continue;
+    mtc::TcParams e{};
+    e.epi = mtc::TC_EPI_CONV;
+    e.y = l.y; e.y_sb = (long long)l.t_out * l.N; e.y_row = l.N;      // convtr: a GEMM row is `stride` consecutive output steps
+    if (l.res_from >= 0) {
+      const SeaLayer& r = layers[l.res_from];
+      if (!r.y) B200_FAIL(B200_ERR_INVALID, "bad residual plan");
+      e.res = r.y; e.r_sb = (long long)l.t_out * l.N; e.r_row = l.N;
+    }
+    if (i + 1 < layers.size()) feed(e, layers[i + 1], l.N);
+    B200_TRY(mtc::tc_bind(l.tc, sched[i], e, l.ext_hi, l.ext_lo, l.P + l.t_in, h->splitk_ws));
+  }
+  return B200_OK;
 }
 
 }  // namespace
@@ -594,29 +723,14 @@ extern "C" {
 
 int b200_mimi_create(const b200_mimi_config* cfg, b200_mimi** out) {
   if (!cfg || !out) B200_FAIL(B200_ERR_INVALID, "mimi_create: null argument");
-  if (cfg->n_ratios < 1 || cfg->n_ratios > 8) B200_FAIL(B200_ERR_INVALID, "mimi_create: n_ratios out of range");
-  if (cfg->channels != 1) B200_FAIL(B200_ERR_INVALID, "mimi_create: only mono audio is on the hot path");
-  if (cfg->q_dimension % 8) B200_FAIL(B200_ERR_INVALID, "mimi_create: codebook dimension must be a multiple of 8");
-  if (cfg->tr_d_model / cfg->tr_num_heads != 64) B200_FAIL(B200_ERR_INVALID, "mimi_create: head dim must be 64");
-  if (cfg->tr_d_model != cfg->dimension) B200_FAIL(B200_ERR_INVALID, "mimi_create: projected transformer unsupported");
-  if (cfg->n_filters % 32 || cfg->compress != 2 || cfg->n_filters / cfg->compress % 32)
-    B200_FAIL(B200_ERR_INVALID, "mimi_create: SEANet channel counts must be multiples of 32 (tensor-core k-blocks)");
+  MimiShape g;
+  B200_TRY(plan_seanet(*cfg, &g));
   b200_mimi* h = new b200_mimi();
-  h->cfg = *cfg;
+  static_cast<MimiShape&>(*h) = std::move(g);
   cudaGetDevice(&h->device);
   h->session_kind = SESSION_MIMI;
   h->fingerprint = config_fingerprint(&h->cfg, sizeof(h->cfg));
   h->num_codebooks = cfg->num_codebooks;
-  h->hop = 1;
-  for (int i = 0; i < cfg->n_ratios; ++i) h->hop *= cfg->ratios[i];
-  h->frame_size = (int)(cfg->sample_rate / cfg->frame_rate);
-  const double enc_rate = (double)cfg->sample_rate / h->hop;
-  h->rs = (int)(enc_rate / cfg->frame_rate);
-  if (h->rs < 1 || h->frame_size != h->hop * h->rs) {
-    delete h;
-    B200_FAIL(B200_ERR_INVALID, "mimi_create: frame size %d is not hop*stride", h->frame_size);
-  }
-  plan_seanet(h);
   *out = h;
   return B200_OK;
 }
@@ -634,7 +748,6 @@ int b200_mimi_finalize(b200_mimi* h) {
   if (h->finalized) return B200_OK;
   DeviceGuard g(h->device);
   B200_TRY(mtc::tc_init());
-  B200_CUDA(cudaDeviceGetAttribute(&h->sms, cudaDevAttrMultiProcessorCount, h->device));
   for (auto& l : h->enc) B200_TRY(pack_sea(h, l));
   for (auto& l : h->dec) B200_TRY(pack_sea(h, l));
   B200_TRY(pack_down(h, h->down));
@@ -680,16 +793,12 @@ int b200_mimi_streaming_begin(b200_mimi* h, int batch, void* stream) {
   h->taps.clear();
   Arena& A = h->state;
   struct Cleanup { b200_mimi* h; bool armed = true; ~Cleanup() { if (armed) b200_mimi_streaming_end(h); } } cleanup{h};
-  h->batch = B;                              // plan_layer reads it
+  MimiPlan plan;
+  B200_TRY(plan_mimi(*h, B, num_sms(), h->num_codebooks, &plan));
   B200_TRY(A.alloc_t(&h->exec_mask, B, false));
   B200_CUDA(cudaMemset(h->exec_mask, 1, B));
   B200_TRY(A.alloc_t(&h->err, 1));
-  {
-    // the tensor-core layers plan their splits within kTcSplitBytes; the down-sampling conv's partials outgrow it above 1024 sessions
-    const DownLayer& l = h->down;
-    const size_t down_bytes = (size_t)ceil_div(l.cin * l.k, DS_KP) * B * l.t_out * l.cout * 4;
-    B200_TRY(A.alloc(reinterpret_cast<void**>(&h->splitk_ws), down_bytes > kTcSplitBytes ? down_bytes : kTcSplitBytes, false));
-  }
+  B200_TRY(A.alloc(reinterpret_cast<void**>(&h->splitk_ws), plan.ws_bytes, false));
 
   const int T = h->rs;   // transformer tokens per frame on both sides
   B200_TRY(A.alloc_t(&h->tok_in_enc, (size_t)B * T * d));   // written by the last encoder conv
@@ -702,74 +811,10 @@ int b200_mimi_streaming_begin(b200_mimi* h, int batch, void* stream) {
 
   std::vector<TmCommit> enc_tm, dec_tm;
   h->max_enc_tm = h->max_dec_tm = 0;
-  // buffers of one SEANet: every layer owns its extended input; raw outputs where something reads them
-  auto setup = [&](std::vector<SeaLayer>& layers, int t0, bool is_dec, std::vector<TmCommit>& commits, long long& max_rows) -> int {
-    int t = t0;
-    for (size_t i = 0; i < layers.size(); ++i) {
-      SeaLayer& l = layers[i];
-      l.t_in = t;
-      if (l.kind == 0) {
-        if (t % l.stride) B200_FAIL(B200_ERR_INVALID, "%s: %d samples not divisible by stride %d", l.key.c_str(), t, l.stride);
-        l.t_out = t / l.stride;
-      } else {
-        l.t_out = t;                            // GEMM rows per session; each row holds `stride` output steps
-      }
-      const size_t ext_n = (size_t)B * (l.P + l.t_in) * l.cin;
-      B200_TRY(A.alloc_t(&l.ext_hi, ext_n));
-      if (!l.simt_first && !l.simt_last) B200_TRY(A.alloc_t(&l.ext_lo, ext_n));
-      else l.ext_lo = nullptr;
-      if (l.P > 0) {
-        TmCommit cm;
-        cm.hi = l.ext_hi; cm.lo = l.ext_lo; cm.P = l.P; cm.T = l.t_in; cm.rowlen = l.cin; cm.sb = (long long)(l.P + l.t_in) * l.cin;
-        commits.push_back(cm);
-        if ((long long)B * l.cin > max_rows) max_rows = (long long)B * l.cin;
-      }
-      const int steps_out = l.kind == 1 ? l.t_out * l.stride : l.t_out;
-      const bool is_last = i + 1 == layers.size();
-      l.y = nullptr;
-      if (is_last && !is_dec) l.y = h->tok_in_enc;                       // transformer input
-      else if (is_last && is_dec) l.y = h->out_frame;
-      else if (!l.tap.empty()) B200_TRY(A.alloc_t(&l.y, (size_t)B * steps_out * l.cout));
-      if (!l.tap.empty() && l.y) register_tap(h, l.tap, l.y, l.cout, steps_out, !(is_last && !is_dec));
-      t = steps_out;
-    }
-    return B200_OK;
-  };
-  B200_TRY(setup(h->enc, h->frame_size, false, enc_tm, h->max_enc_tm));
-  if (h->enc.back().t_out != T) B200_FAIL(B200_ERR_INVALID, "encoder yields %d tokens/frame, expected %d", h->enc.back().t_out, T);
-  B200_TRY(setup(h->dec, T, true, dec_tm, h->max_dec_tm));
-  if (h->dec.back().t_out != h->frame_size) B200_FAIL(B200_ERR_INVALID, "decoder yields %d samples/frame", h->dec.back().t_out);
-  // epilogues + plans: layer i writes its raw output and the activation its consumer i + 1 reads
-  auto wire = [&](std::vector<SeaLayer>& layers) -> int {
-    for (size_t i = 0; i < layers.size(); ++i) {
-      SeaLayer& l = layers[i];
-      if (l.simt_first || l.simt_last) continue;
-      mtc::TcParams& p = l.tc.p;
-      memset(&p, 0, sizeof(p));
-      p.epi = mtc::TC_EPI_CONV;
-      p.y = l.y; p.y_sb = (long long)l.t_out * l.N; p.y_row = l.N;      // convtr: a GEMM row is `stride` consecutive output steps
-      if (l.res_from >= 0) {
-        const SeaLayer& r = layers[l.res_from];
-        if (!r.y) B200_FAIL(B200_ERR_INVALID, "bad residual plan");
-        p.res = r.y; p.r_sb = (long long)l.t_out * l.N; p.r_row = l.N;
-      }
-      if (i + 1 < layers.size()) {
-        const SeaLayer& nx = layers[i + 1];
-        p.act_mode = nx.simt_last ? mtc::TC_ACT_FULL : mtc::TC_ACT_SPLIT;
-        p.act_elu = nx.elu_in ? 1 : 0;
-        p.a_hi = nx.ext_hi + (long long)nx.P * nx.cin;
-        p.a_lo = nx.ext_lo ? nx.ext_lo + (long long)nx.P * nx.cin : nullptr;
-        p.a_sb = (long long)(nx.P + nx.t_in) * nx.cin;
-        p.a_row = l.N;                         // = stride * nx.cin for a convtr: `stride` consumer rows per GEMM row
-      }
-      // conv: GEMM row t reads ext rows t * stride + tap * dil (ext row 0 = oldest carried sample)
-      // convtr: GEMM row t reads ext rows t + slot, slot 0 = x[t-1] (ext row 0 = the carried previous step)
-      B200_TRY(plan_layer(h, l.tc, l.ext_hi, l.ext_lo, l.P + l.t_in, 0, l.t_out));
-    }
-    return B200_OK;
-  };
-  B200_TRY(wire(h->enc));
-  B200_TRY(wire(h->dec));
+  B200_TRY(alloc_seanet(h, h->enc, B, false, enc_tm, h->max_enc_tm));
+  B200_TRY(alloc_seanet(h, h->dec, B, true, dec_tm, h->max_dec_tm));
+  B200_TRY(bind_seanet(h, h->enc, plan.enc));
+  B200_TRY(bind_seanet(h, h->dec, plan.dec));
   register_tap(h, "enc.tr", h->tok_enc, d, T, false);
   register_tap(h, "enc.latent", h->latent, d, 1, false);
   register_tap(h, "dec.latent", h->latent_q, d, 1, false);
@@ -810,34 +855,23 @@ int b200_mimi_streaming_begin(b200_mimi* h, int batch, void* stream) {
       B200_TRY(A.alloc_t(&L.kc, (size_t)B * H * c.tr_context * D));
       B200_TRY(A.alloc_t(&L.vc, (size_t)B * H * c.tr_context * D));
       const float* cur = li == 0 ? x_in : x;
-      auto lin = [&](mtc::TcLayer& G, float* y, int N) {
-        memset(&G.p, 0, sizeof(G.p));
-        G.p.epi = mtc::TC_EPI_CONV;
-        G.p.y = y; G.p.y_sb = (long long)T * N; G.p.y_row = N;
-      };
-      // in_proj: qkv = W_in xn
-      lin(L.in_proj, h->tr_qkv, 3 * d);
-      B200_TRY(plan_layer(h, L.in_proj, h->tr_xn_hi, h->tr_xn_lo, T, 0, T));
-      // out_proj: x = cur + layer_scale_1 * (W_out ao)   (transformer.py:769)
-      lin(L.out_proj, x, d);
-      L.out_proj.p.epi = mtc::TC_EPI_RES_SCALE; L.out_proj.p.res = cur; L.out_proj.p.r_sb = (long long)T * d; L.out_proj.p.r_row = d;
-      L.out_proj.p.scale = L.ls1;
-      B200_TRY(plan_layer(h, L.out_proj, h->tr_ao_hi, h->tr_ao_lo, T, 0, T));
-      // linear1 + GELU -> h as a hi / lo pair (never stored raw)
-      lin(L.l1, nullptr, ff);
-      L.l1.p.epi = mtc::TC_EPI_GELU; L.l1.p.act_mode = mtc::TC_ACT_SPLIT; L.l1.p.act_elu = 0;
-      L.l1.p.a_hi = h->tr_h_hi; L.l1.p.a_lo = h->tr_h_lo; L.l1.p.a_sb = (long long)T * ff; L.l1.p.a_row = ff;
-      B200_TRY(plan_layer(h, L.l1, h->tr_xn_hi, h->tr_xn_lo, T, 0, T));
+      const long long sb = (long long)T * d;
+      float* ws = h->splitk_ws;
+      mtc::TcParams e{};                      // in_proj: qkv = W_in xn
+      e.epi = mtc::TC_EPI_CONV; e.y = h->tr_qkv; e.y_sb = 3 * sb; e.y_row = 3 * d;
+      B200_TRY(mtc::tc_bind(L.in_proj, plan.in_proj, e, h->tr_xn_hi, h->tr_xn_lo, T, ws));
+      e = mtc::TcParams{};                    // out_proj: x = cur + layer_scale_1 * (W_out ao)   (transformer.py:769)
+      e.epi = mtc::TC_EPI_RES_SCALE; e.y = x; e.y_sb = sb; e.y_row = d; e.res = cur; e.r_sb = sb; e.r_row = d; e.scale = L.ls1;
+      B200_TRY(mtc::tc_bind(L.out_proj, plan.out_proj, e, h->tr_ao_hi, h->tr_ao_lo, T, ws));
+      e = mtc::TcParams{};                    // linear1 + GELU -> h as a hi / lo pair (never stored raw)
+      e.epi = mtc::TC_EPI_GELU; e.y_sb = (long long)T * ff; e.y_row = ff;
+      e.act_mode = mtc::TC_ACT_SPLIT; e.a_hi = h->tr_h_hi; e.a_lo = h->tr_h_lo; e.a_sb = (long long)T * ff; e.a_row = ff;
+      B200_TRY(mtc::tc_bind(L.l1, plan.linear1, e, h->tr_xn_hi, h->tr_xn_lo, T, ws));
       // linear2: x = x + layer_scale_2 * (W_2 h)   (transformer.py:777); the decoder's last layer also feeds dec[0]
-      lin(L.l2, x, d);
-      L.l2.p.epi = mtc::TC_EPI_RES_SCALE; L.l2.p.res = x; L.l2.p.r_sb = (long long)T * d; L.l2.p.r_row = d; L.l2.p.scale = L.ls2;
-      if (which == 1 && li + 1 == tr->layers.size()) {
-        const SeaLayer& nx = h->dec[0];
-        L.l2.p.act_mode = mtc::TC_ACT_SPLIT; L.l2.p.act_elu = nx.elu_in ? 1 : 0;
-        L.l2.p.a_hi = nx.ext_hi + (long long)nx.P * nx.cin; L.l2.p.a_lo = nx.ext_lo + (long long)nx.P * nx.cin;
-        L.l2.p.a_sb = (long long)(nx.P + nx.t_in) * nx.cin; L.l2.p.a_row = d;
-      }
-      B200_TRY(plan_layer(h, L.l2, h->tr_h_hi, h->tr_h_lo, T, 0, T));
+      e = mtc::TcParams{};
+      e.epi = mtc::TC_EPI_RES_SCALE; e.y = x; e.y_sb = sb; e.y_row = d; e.res = x; e.r_sb = sb; e.r_row = d; e.scale = L.ls2;
+      if (which == 1 && li + 1 == tr->layers.size()) feed(e, h->dec[0], d);
+      B200_TRY(mtc::tc_bind(L.l2, plan.linear2, e, h->tr_h_hi, h->tr_h_lo, T, ws));
     }
   }
   B200_TRY(A.alloc_t(&h->enc_codes, (size_t)B * c.q_n_q));
@@ -888,6 +922,7 @@ int b200_mimi_streaming_begin(b200_mimi* h, int batch, void* stream) {
     }
   }
   B200_CUDA(cudaDeviceSynchronize());
+  h->batch = B;
   cleanup.armed = false;
   return B200_OK;
 }
@@ -1145,6 +1180,40 @@ int64_t b200_mimi_algorithmic_bytes(b200_mimi* h) {
   st += (int64_t)h->down.cin * h->down.P + (int64_t)c.dimension * h->rs;
   per_row += 2 * st * 4 + (int64_t)2 * h->frame_size * 4 + h->num_codebooks * 8;
   return bytes + per_row * h->batch;
+}
+
+int b200_op_mimi_plan(const b200_mimi_config* cfg, int batch, int sms, int num_codebooks, int64_t* out, int capacity) {
+  constexpr int HEAD = 6, F = 21;
+  if (!cfg || !out) B200_FAIL(B200_ERR_INVALID, "op_mimi_plan: null argument");
+  MimiShape g;
+  B200_TRY(plan_seanet(*cfg, &g));
+  if (batch < 1 || sms < 1 || num_codebooks < cfg->q_n_semantic || num_codebooks > cfg->q_n_q)
+    B200_FAIL(B200_ERR_INVALID, "op_mimi_plan: batch %d, %d SMs, %d codebooks", batch, sms, num_codebooks);
+  MimiPlan P;
+  B200_TRY(plan_mimi(g, batch, sms, num_codebooks, &P));
+  int n_tc[2] = {0, 0};
+  for (int w = 0; w < 2; ++w)
+    for (const SeaLayer& l : w ? g.dec : g.enc) n_tc[w] += !l.simt_first && !l.simt_last;
+  const int n = n_tc[0] + n_tc[1] + 4;
+  if (capacity < HEAD + F * n) B200_FAIL(B200_ERR_INVALID, "op_mimi_plan: %d layers need %d slots", n, HEAD + F * n);
+  const long long head[HEAD] = {n_tc[0], n_tc[1], P.down_ksplit, (long long)P.ws_bytes, P.enc_launches, P.dec_launches};
+  int k = 0;
+  for (long long v : head) out[k++] = v;
+  auto put = [&](int layer, const mtc::TcShape& s, const mtc::TcSchedule& q) {
+    const long long v[F] = {layer, s.kind, s.Cin, s.N, s.n_taps, s.dil, s.stride, s.NT, s.n_tiles_n, s.num_kb, q.tt, q.bb, q.T,
+                            q.n_sessions, q.m_tiles, q.ksplit, q.kb_per_split, q.stages, q.stage_bytes, q.grid, (long long)q.smem};
+    for (long long x : v) out[k++] = x;
+  };
+  for (int w = 0; w < 2; ++w) {
+    const std::vector<SeaLayer>& ls = w ? g.dec : g.enc;
+    for (size_t i = 0; i < ls.size(); ++i)
+      if (!ls[i].simt_first && !ls[i].simt_last) put((int)i, ls[i].tc.s, (w ? P.dec : P.enc)[i]);
+  }
+  put(0, g.in_proj, P.in_proj);
+  put(1, g.out_proj, P.out_proj);
+  put(2, g.linear1, P.linear1);
+  put(3, g.linear2, P.linear2);
+  return B200_OK;
 }
 
 }  // extern "C"

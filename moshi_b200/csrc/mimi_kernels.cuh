@@ -47,6 +47,7 @@ struct ConvSplitK {
 // (deterministic).  The partials take KS * N * M floats.
 // ---------------------------------------------------------------------------------------------
 constexpr int DS_CO = 64, DS_KP = 64, DS_NC = 32;
+inline int ds_splits(int Kd) { return ceil_div(Kd, DS_KP); }     // KS for Kd = K * Cin reduction steps
 static __global__ void __launch_bounds__(256) conv_splitk_kernel(const ConvSplitK p, float* __restrict__ part, int KS) {
   __shared__ float ws[DS_KP][DS_CO + 1];
   __shared__ float xs[DS_KP][DS_NC + 1];

@@ -272,74 +272,82 @@ int tc_init() {
   return B200_OK;
 }
 
-void tc_set_shape(TcLayer& L, int N, int Cin, int n_taps) {
-  L.Cin = Cin; L.N = N; L.n_taps = n_taps;
-  L.NT = N >= TC_MAX_NT ? TC_MAX_NT : N;
-  L.n_tiles_n = (N + L.NT - 1) / L.NT;
-  L.num_kb = n_taps * (Cin / TC_KB);
+TcShape tc_shape(int kind, int N, int Cin, int n_taps, int dil, int stride, int bias_mod) {
+  TcShape s;
+  s.kind = kind; s.Cin = Cin; s.N = N; s.n_taps = n_taps; s.dil = dil; s.stride = stride;
+  s.bias_mod = bias_mod > 0 ? bias_mod : N;
+  s.NT = N >= TC_MAX_NT ? TC_MAX_NT : N;
+  s.n_tiles_n = (N + s.NT - 1) / s.NT;
+  s.num_kb = n_taps * (Cin / TC_KB);
+  return s;
 }
 
-int tc_tile_shape(int T, int stride, int* tt, int* bb) {
-  int t = TC_ROWS;
-  while (t > 1 && (T % t || t * stride > 256)) t >>= 1;
-  if (T % t) return B200_ERR_SHAPE;
-  *tt = t; *bb = TC_ROWS / t;
+int plan_tc(const TcShape& s, int n_sessions, int T, int sms, size_t ws_bytes, TcSchedule* out) {
+  if (n_sessions < 1 || T < 1 || sms < 1 || s.num_kb < 1 || s.NT < 1 || (s.kind == TC_LINEAR_ROWS && n_sessions != 1))
+    B200_FAIL(B200_ERR_INVALID, "plan_tc: %d sessions of %d rows, %d SMs, %d k-blocks, kind %d", n_sessions, T, sms, s.num_kb, s.kind);
+  TcSchedule q;
+  q.n_sessions = n_sessions; q.T = T;
+  q.tt = TC_ROWS;
+  if (s.kind != TC_LINEAR_ROWS)
+    while (q.tt > 1 && (T % q.tt || q.tt * s.stride > 256)) q.tt >>= 1;
+  q.bb = TC_ROWS / q.tt;
+  const int tpg = (T + q.tt - 1) / q.tt, groups = (n_sessions + q.bb - 1) / q.bb;
+  q.m_tiles = tpg * groups;
+  // deep-and-skinny layers: cut K so that the chip has a few hundred tiles, at least 4 k-blocks each
+  int ks = 1;
+  const long long mn = (long long)q.m_tiles * s.n_tiles_n;
+  if (mn < sms && s.num_kb >= 8) {
+    ks = (int)((2LL * sms + mn - 1) / mn);
+    if (ks > s.num_kb / 4) ks = s.num_kb / 4;
+    while (ks > 1 && (size_t)ks * q.m_tiles * TC_ROWS * (size_t)s.N * 4 > ws_bytes) --ks;
+    if (ks < 1) ks = 1;
+  }
+  q.kb_per_split = (s.num_kb + ks - 1) / ks;
+  q.ksplit = (s.num_kb + q.kb_per_split - 1) / q.kb_per_split;
+  q.stage_bytes = 2 * A_TILE_BYTES + 2 * (uint32_t)s.NT * 128u;
+  int stages = (200 * 1024) / (int)q.stage_bytes;
+  if (stages > TC_MAX_STAGES) stages = TC_MAX_STAGES;
+  q.stages = stages;
+  const long long tiles = mn * q.ksplit;
+  q.grid = (int)(tiles < sms ? tiles : sms);
+  q.smem = (size_t)stages * q.stage_bytes + 1024 + 16 * TC_MAX_STAGES + 64;
+  *out = q;
   return B200_OK;
 }
 
-size_t tc_packed_bytes(const TcLayer& L) { return (size_t)L.n_tiles_n * L.num_kb * 2 * L.NT * 128; }
+size_t tc_packed_bytes(const TcShape& s) { return (size_t)s.n_tiles_n * s.num_kb * 2 * s.NT * 128; }
 
-int tc_pack_weights(const float* w_dev, void* out_dev, const TcLayer& L, cudaStream_t st) {
-  if (L.Cin % TC_KB || L.N % 16 || (L.N > TC_MAX_NT && L.N % TC_MAX_NT))
-    B200_FAIL(B200_ERR_SHAPE, "tc_pack_weights: Cin %d must be a multiple of 32, N %d a multiple of 16 (of 128 above 128)", L.Cin, L.N);
-  const long long total = (long long)L.n_tiles_n * L.num_kb * L.NT * 8;
-  tc_pack_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(w_dev, static_cast<float4*>(out_dev), L.N, L.n_taps * L.Cin, L.NT,
-                                                                 L.n_tiles_n, L.num_kb);
+int tc_pack_weights(const float* w_dev, void* out_dev, const TcShape& s, cudaStream_t st) {
+  if (s.Cin % TC_KB || s.N % 16 || (s.N > TC_MAX_NT && s.N % TC_MAX_NT))
+    B200_FAIL(B200_ERR_SHAPE, "tc_pack_weights: Cin %d must be a multiple of 32, N %d a multiple of 16 (of 128 above 128)", s.Cin, s.N);
+  const long long total = (long long)s.n_tiles_n * s.num_kb * s.NT * 8;
+  tc_pack_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(w_dev, static_cast<float4*>(out_dev), s.N, s.n_taps * s.Cin, s.NT,
+                                                                 s.n_tiles_n, s.num_kb);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   return check_launch("tc_pack");
 }
 
-int tc_make_map(CUtensorMap* m, const float* base, int Cin, long long rows_per_session, long long sb_elems, int n_sessions, int tt,
-                int bb, int stride) {
+int tc_bind(TcLayer& L, const TcSchedule& q, const TcParams& epi, const float* in_hi, const float* in_lo, long long rows_per_session,
+            float* ws) {
   B200_TRY(tc_init());
-  cuuint64_t dims[3] = {(cuuint64_t)Cin, (cuuint64_t)rows_per_session, (cuuint64_t)n_sessions};
-  cuuint64_t strides[2] = {(cuuint64_t)Cin * 4, (cuuint64_t)sb_elems * 4};
-  cuuint32_t box[3] = {(cuuint32_t)TC_KB, (cuuint32_t)(tt * stride), (cuuint32_t)bb};
-  cuuint32_t estr[3] = {1, (cuuint32_t)stride, 1};
-  if (box[1] > 256 || box[2] > 256) B200_FAIL(B200_ERR_SHAPE, "tc_make_map: box %u x %u exceeds the TMA limit of 256", box[1], box[2]);
-  return encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, base, dims, strides, box, estr, "tc_make_map");
-}
-
-// Fills the launch plan of a layer for `n_sessions` sessions of T output steps each (linear: n_sessions = 1, T = tokens).
-// The caller has set the static fields, the tensor maps and the epilogue pointers of L.p.
-int tc_plan(TcLayer& L, int n_sessions, int T, int sms, size_t ws_bytes) {
+  const TcShape& s = L.s;
   TcParams& p = L.p;
-  p.n_sessions = n_sessions; p.T = T;
-  if (p.tt * p.bb != TC_ROWS) B200_FAIL(B200_ERR_INVALID, "tc_plan: tile %d x %d is not 128 rows", p.tt, p.bb);
-  const int tpg = (T + p.tt - 1) / p.tt, groups = (n_sessions + p.bb - 1) / p.bb;
-  p.m_tiles = tpg * groups;
-  p.n_taps = L.n_taps; p.dil = L.dil; p.stride = L.stride; p.Cin = L.Cin;
-  p.wt = L.wt; p.NT = L.NT; p.n_tiles_n = L.n_tiles_n; p.num_kb = L.num_kb; p.N = L.N;
-  p.bias = L.bias; p.bias_mod = L.bias_mod > 0 ? L.bias_mod : L.N;
-  // deep-and-skinny layers: cut K so that the chip has a few hundred tiles, at least 4 k-blocks each
-  int ks = 1;
-  const long long mn = (long long)p.m_tiles * p.n_tiles_n;
-  if (mn < sms && p.num_kb >= 8) {
-    ks = (int)((2LL * sms + mn - 1) / mn);
-    if (ks > p.num_kb / 4) ks = p.num_kb / 4;
-    while (ks > 1 && (size_t)ks * p.m_tiles * TC_ROWS * (size_t)p.N * 4 > ws_bytes) --ks;
-    if (ks < 1) ks = 1;
-  }
-  p.kb_per_split = (p.num_kb + ks - 1) / ks;
-  p.ksplit = (p.num_kb + p.kb_per_split - 1) / p.kb_per_split;
-  p.stage_bytes = 2 * A_TILE_BYTES + 2 * (uint32_t)p.NT * 128u;
-  int stages = (200 * 1024) / (int)p.stage_bytes;
-  if (stages > TC_MAX_STAGES) stages = TC_MAX_STAGES;
-  p.stages = stages;
-  const long long tiles = mn * p.ksplit;
-  L.grid = (int)(tiles < sms ? tiles : sms);
-  L.smem = (size_t)stages * p.stage_bytes + 1024 + 16 * TC_MAX_STAGES + 64;
-  return B200_OK;
+  p = epi;
+  p.tt = q.tt; p.bb = q.bb; p.T = q.T; p.n_sessions = q.n_sessions;
+  p.n_taps = s.n_taps; p.dil = s.dil; p.stride = s.stride; p.row0 = 0; p.Cin = s.Cin;
+  p.wt = L.wt; p.NT = s.NT; p.n_tiles_n = s.n_tiles_n; p.num_kb = s.num_kb; p.N = s.N;
+  p.m_tiles = q.m_tiles; p.ksplit = q.ksplit; p.kb_per_split = q.kb_per_split; p.ws = ws;
+  p.bias = L.bias; p.bias_mod = s.bias_mod;
+  p.stage_bytes = q.stage_bytes; p.stages = q.stages;
+  L.grid = q.grid; L.smem = q.smem;
+  // 3-D maps over base[b][row][Cin]: a box of 32 channels x tt rows (element stride = conv stride) x bb sessions
+  cuuint64_t dims[3] = {(cuuint64_t)s.Cin, (cuuint64_t)rows_per_session, (cuuint64_t)q.n_sessions};
+  cuuint64_t strides[2] = {(cuuint64_t)s.Cin * 4, (cuuint64_t)(rows_per_session * s.Cin) * 4};
+  cuuint32_t box[3] = {(cuuint32_t)TC_KB, (cuuint32_t)(q.tt * s.stride), (cuuint32_t)q.bb};
+  cuuint32_t estr[3] = {1, (cuuint32_t)s.stride, 1};
+  if (box[1] > 256 || box[2] > 256) B200_FAIL(B200_ERR_SHAPE, "tc_make_map: box %u x %u exceeds the TMA limit of 256", box[1], box[2]);
+  B200_TRY(encode_tiled(&L.map_hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, in_hi, dims, strides, box, estr, "tc_make_map"));
+  return encode_tiled(&L.map_lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, in_lo, dims, strides, box, estr, "tc_make_map");
 }
 
 int tc_launch(const TcLayer& L, cudaStream_t st) {

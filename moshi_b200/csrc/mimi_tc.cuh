@@ -76,33 +76,49 @@ __device__ __forceinline__ void split_tf32(float v, float& hi, float& lo) {
 }
 
 // ---- host side ---------------------------------------------------------------------------------------------------------
-struct TcLayer {
-  // static description
-  int kind = 0;               // 0 conv, 1 convtr, 2 linear
+enum { TC_CONV = 0, TC_CONVTR = 1, TC_LINEAR = 2, TC_LINEAR_ROWS = 3 };   // TC_LINEAR_ROWS: M flat rows as one session
+constexpr size_t TC_SPLIT_BYTES = (size_t)64 << 20;   // split-K partials budget of one layer
+
+// what the weights fix: N output features over n_taps * Cin inputs and their tiling NT / n_tiles_n / num_kb
+struct TcShape {
+  int kind = TC_CONV;
   int Cin = 0, N = 0, n_taps = 1, dil = 1, stride = 1;
-  int bias_mod = 0;
+  int bias_mod = 0;           // bias[n % bias_mod]
+  int NT = 0, n_tiles_n = 0, num_kb = 0;
+};
+
+// what one launch runs for n_sessions sessions of T GEMM rows each (plan_tc)
+struct TcSchedule {
+  int tt = 0, bb = 0, T = 0, n_sessions = 0;
+  int m_tiles = 0, ksplit = 0, kb_per_split = 0, stages = 0;
+  uint32_t stage_bytes = 0;
+  int grid = 0; size_t smem = 0;
+};
+
+// a layer bound to its weights, input and schedule: what tc_launch launches
+struct TcLayer {
+  TcShape s;
   uint8_t* wt = nullptr;      // packed hi/lo tiles
   const float* bias = nullptr;
-  int NT = 0, n_tiles_n = 0, num_kb = 0;
-  // per-session-batch plan (streaming_begin)
   CUtensorMap map_hi, map_lo;
   TcParams p;
   int grid = 0; size_t smem = 0;
 };
 
-// static shape of a layer of N output features over n_taps * Cin inputs: Cin, N, n_taps and the weight tiling NT / n_tiles_n / num_kb
-void tc_set_shape(TcLayer& L, int N, int Cin, int n_taps);
-// Tile shape of a layer whose sessions produce T GEMM rows: the largest power of two that divides T (<= 128) steps of
-// bb = 128 / tt sessions; strided convolutions also keep the TMA box (tt * stride rows) within 256.
-int tc_tile_shape(int T, int stride, int* tt, int* bb);
-size_t tc_packed_bytes(const TcLayer& L);
-// w: fp32 [N][n_taps * Cin] (k = tap * Cin + ci) -> tiles, for a layer whose shape tc_set_shape filled
-int tc_pack_weights(const float* w_dev, void* out_dev, const TcLayer& L, cudaStream_t st);
+// bias_mod 0: N
+TcShape tc_shape(int kind, int N, int Cin, int n_taps, int dil = 1, int stride = 1, int bias_mod = 0);
+// The schedule of a layer on a device of `sms` multiprocessors whose split-K partials fit ws_bytes; no CUDA call.  Tile:
+// bb = 128 / tt sessions of tt steps, tt the largest power of two (<= 128) that divides T and keeps the TMA box (tt * stride
+// rows) within 256; TC_LINEAR_ROWS: one session of T rows on 128 x 1 tiles, the last one partial.
+int plan_tc(const TcShape& s, int n_sessions, int T, int sms, size_t ws_bytes, TcSchedule* out);
+size_t tc_packed_bytes(const TcShape& s);
+// w: fp32 [N][n_taps * Cin] (k = tap * Cin + ci) -> tiles
+int tc_pack_weights(const float* w_dev, void* out_dev, const TcShape& s, cudaStream_t st);
 int tc_init();
-// 3-D tensor map over a token-major activation buffer base[b][row][Cin] (session stride sb elements, row stride = Cin)
-int tc_make_map(CUtensorMap* m, const float* base, int Cin, long long rows_per_session, long long sb_elems, int n_sessions, int tt,
-                int bb, int stride);
-int tc_plan(TcLayer& L, int n_sessions, int T, int sms, size_t ws_bytes);
+// Binds L (shape, weights and bias set) to schedule q: the launch parameters are `epi` (epilogue fields) completed from shape,
+// schedule and the split-K workspace ws; the A maps cover in_hi / in_lo, token-major [q.n_sessions][rows_per_session][Cin].
+int tc_bind(TcLayer& L, const TcSchedule& q, const TcParams& epi, const float* in_hi, const float* in_lo, long long rows_per_session,
+            float* ws);
 int tc_launch(const TcLayer& L, cudaStream_t st);
 
 }  // namespace mtc

@@ -354,7 +354,7 @@ int b200_op_conv1d(const float* x_dev, const float* w_dev, const float* bias_dev
   p.y = y_dev; p.yb = (long long)Cout * (T / stride); p.yc = T / stride; p.yt = 1;
   p.Cin = Cin; p.stride = stride; p.dil = dilation; p.Tout = T / stride; p.elu_in = elu_in;
   p.M = Cout; p.N = B * (T / stride); p.Kd = Cin * K;
-  const int KS = ceil_div(p.Kd, DS_KP);
+  const int KS = ds_splits(p.Kd);
   DevBufs d;
   float *wp, *part;
   B200_TRY(d.get(&wp, (size_t)Cout * Cin * K * 4));
@@ -375,28 +375,23 @@ int b200_op_tc_linear_f32(const float* x_dev, const float* w_dev, float* y_dev, 
   if (!x_dev || !w_dev || !y_dev || M < 1 || K % 32 || N % 16) B200_FAIL(B200_ERR_SHAPE, "op_tc_linear_f32: bad shape");
   B200_TRY(tc_init());
   TcLayer L;
-  tc_set_shape(L, N, K, 1);
-  L.kind = 2;
+  L.s = tc_shape(TC_LINEAR_ROWS, N, K, 1);
+  TcSchedule q;
+  B200_TRY(plan_tc(L.s, 1, M, num_sms(), TC_SPLIT_BYTES, &q));
   DevBufs d;
   float *hi, *lo, *ws; uint8_t* wt;
   B200_TRY(d.get(&hi, (size_t)M * K * 4));
   B200_TRY(d.get(&lo, (size_t)M * K * 4));
-  B200_TRY(d.get(&wt, tc_packed_bytes(L)));
-  const size_t ws_bytes = (size_t)64 << 20;
-  B200_TRY(d.get(&ws, ws_bytes));
+  B200_TRY(d.get(&wt, tc_packed_bytes(L.s)));
+  B200_TRY(d.get(&ws, TC_SPLIT_BYTES));
   const long long n = (long long)M * K;
   // x is already [M][K] token-major: a flat hi/lo split is tm_pack_in with B = M "sessions" of Cin = K, T = 1, P = 0
   B200_LAUNCH(tm_pack_in_kernel, (unsigned)ceil_div64(n, 256), 256, 0, st, x_dev, (const float*)nullptr, hi, lo, M, K, 1, 0, 0);
-  B200_TRY(tc_pack_weights(w_dev, wt, L, st));
+  B200_TRY(tc_pack_weights(w_dev, wt, L.s, st));
   L.wt = wt;
-  memset(&L.p, 0, sizeof(L.p));
-  L.p.tt = 128; L.p.bb = 1; L.p.row0 = 0;
-  L.p.epi = TC_EPI_CONV; L.p.y = y_dev; L.p.y_sb = 0; L.p.y_row = N; L.p.ws = ws;
-  B200_TRY(tc_make_map(&L.map_hi, hi, K, M, (long long)M * K, 1, 128, 1, 1));
-  B200_TRY(tc_make_map(&L.map_lo, lo, K, M, (long long)M * K, 1, 128, 1, 1));
-  int sms = 148;
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
-  B200_TRY(tc_plan(L, 1, M, sms, ws_bytes));
+  TcParams e{};
+  e.epi = TC_EPI_CONV; e.y = y_dev; e.y_sb = 0; e.y_row = N;
+  B200_TRY(tc_bind(L, q, e, hi, lo, M, ws));
   B200_TRY(tc_launch(L, st));
   B200_CUDA(cudaStreamSynchronize(st));
   return B200_OK;
@@ -416,34 +411,28 @@ int b200_op_tc_conv1d(const float* x_dev, const float* w_dev, const float* bias_
   if (Cin % 32 || N % 16 || (N > 128 && N % 128) || P < 0 || (!transposed && T % stride) || (transposed && K != 2 * S))
     B200_FAIL(B200_ERR_SHAPE, "op_tc_conv1d: unsupported shape");
   TcLayer L;
-  tc_set_shape(L, N, Cin, n_taps);
-  L.kind = transposed ? 1 : 0; L.dil = transposed ? 1 : dilation; L.stride = transposed ? 1 : stride;
-  L.bias = bias_dev; L.bias_mod = Cout;
+  L.s = transposed ? tc_shape(TC_CONVTR, N, Cin, 2, 1, 1, Cout) : tc_shape(TC_CONV, N, Cin, K, dilation, stride, Cout);
+  L.bias = bias_dev;
+  TcSchedule q;
+  B200_TRY(plan_tc(L.s, B, Tout, num_sms(), TC_SPLIT_BYTES, &q));
   DevBufs d;
   float *hi, *lo, *ws, *wk, *ytm; uint8_t* wt;
   const size_t E = (size_t)P + T;
   B200_TRY(d.get(&hi, (size_t)B * E * Cin * 4));
   B200_TRY(d.get(&lo, (size_t)B * E * Cin * 4));
   B200_TRY(d.get(&wk, (size_t)N * n_taps * Cin * 4));
-  B200_TRY(d.get(&wt, tc_packed_bytes(L)));
+  B200_TRY(d.get(&wt, tc_packed_bytes(L.s)));
   B200_TRY(d.get(&ytm, (size_t)B * Tout * N * 4));
-  const size_t ws_bytes = (size_t)64 << 20;
-  B200_TRY(d.get(&ws, ws_bytes));
+  B200_TRY(d.get(&ws, TC_SPLIT_BYTES));
   const long long n_in = (long long)B * E * Cin, n_w = (long long)N * n_taps * Cin;
   B200_LAUNCH(tm_pack_in_kernel, (unsigned)ceil_div64(n_in, 256), 256, 0, st, x_dev, (const float*)prev_dev, hi, lo, B, Cin, T, P, elu_in);
   if (transposed) B200_LAUNCH(mimi::tm_weight_convtr_kernel, (unsigned)ceil_div64(n_w, 256), 256, 0, st, w_dev, wk, Cin, Cout, S);
   else B200_LAUNCH(mimi::tm_weight_conv_kernel, (unsigned)ceil_div64(n_w, 256), 256, 0, st, w_dev, wk, Cout, Cin, K);
-  B200_TRY(tc_pack_weights(wk, wt, L, st));
+  B200_TRY(tc_pack_weights(wk, wt, L.s, st));
   L.wt = wt;
-  memset(&L.p, 0, sizeof(L.p));
-  if (tc_tile_shape(Tout, L.stride, &L.p.tt, &L.p.bb) != B200_OK) B200_FAIL(B200_ERR_SHAPE, "op_tc_conv1d: T");
-  L.p.row0 = 0;
-  L.p.epi = TC_EPI_CONV; L.p.y = ytm; L.p.y_sb = (long long)Tout * N; L.p.y_row = N; L.p.ws = ws;
-  B200_TRY(tc_make_map(&L.map_hi, hi, Cin, (long long)E, (long long)E * Cin, B, L.p.tt, L.p.bb, L.stride));
-  B200_TRY(tc_make_map(&L.map_lo, lo, Cin, (long long)E, (long long)E * Cin, B, L.p.tt, L.p.bb, L.stride));
-  int sms = 148;
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
-  B200_TRY(tc_plan(L, B, Tout, sms, ws_bytes));
+  TcParams e{};
+  e.epi = TC_EPI_CONV; e.y = ytm; e.y_sb = (long long)Tout * N; e.y_row = N;
+  B200_TRY(tc_bind(L, q, e, hi, lo, (long long)E, ws));
   B200_TRY(tc_launch(L, st));
   // token-major [B][Tout][N] -> the reference layout: conv [B][Cout][Tout]; convtr [B][Cout][Tout * S] (row t holds S steps of Cout)
   const int Tr = transposed ? Tout * S : Tout;
