@@ -184,7 +184,10 @@ typedef struct {
   int extra_heads_dim;        /* temporal output (lm.py:224-226), read by LMGen.step_with_extra_heads (lm.py:793-807)          */
 } b200_lm_config;
 /* Family limits: n_q <= 32, 0 <= dep_q <= 16 (dep_q = 0: no depformer, lm.py:219-222), temporal head dim 128, depformer head
- * dim 64, vocabularies < 65535: covers configs/moshi_7b_202409.json, configs/moshi_dev_2b.json and the STT checkpoints. */
+ * dim 64, vocabularies < 65535: covers configs/moshi_7b_202409.json, configs/moshi_dev_2b.json and the STT checkpoints.
+ * Depformer weight-sharing schedules and low-rank depformer embeddings are set by the two setters below.  Not supported:
+ * demux_second_text_stream, text_card_out, depformer_norm, norm_emb, and candle / GGUF-layout checkpoints of models with a
+ * schedule or low-rank embeddings (the Python loader refuses them: the candle layout unrolls a schedule into per-step slices). */
 
 /* loaders.get_moshi_lm (loaders.py:366-446). Tensors are bf16 with the reference's key names.  With cfg.quantize a linear may
  * instead arrive pre-quantised, the way `model.q8.safetensors` stores a QLinear (loaders.py:33; utils/quantize.py:16-21):
@@ -214,6 +217,20 @@ int b200_lm_set_condition_sum(b200_lm* h, const void* sum_bf16_dev, int rows);
  * .weight" [3*dim,dim], ".cross_attention.out_projs.0.weight" [dim,dim] and ".norm_cross.weight" / ".norm_cross.bias" [dim].
  * Not with quantize (B200_ERR_INVALID). */
 int b200_lm_set_cross_attention(b200_lm* h, int enable);
+/* LMModel(depformer_weights_per_step_schedule=...) (lm.py:125-127, 172-181; transformer.py:291-316, 399-401): depformer sub-step
+ * k runs weight set schedule[k] of "depformer_in.<j>", and of every layer's "self_attn.in_projs.<j>", "self_attn.out_projs.<j>"
+ * and "gating.<j>.*"; the checkpoint holds n_sets = max(schedule) + 1 of each, resident once.  n = dep_q entries in
+ * [0, dep_q); n = 0: no schedule (one set per sub-step).  After b200_lm_create and before the
+ * first b200_lm_load_tensor (B200_ERR_STATE after); B200_ERR_INVALID on a bad schedule. */
+int b200_lm_set_depformer_schedule(b200_lm* h, const int* schedule, int n);
+/* LMModel(depformer_low_rank_embeddings=rank) (lm.py:186-196; lm_utils.py:80-124): "depformer_text_emb.weight" [text_card+1,
+ * rank], "depformer_emb.<i>.weight" [card+1, rank], each with ".low_rank.weight" [depformer_dim, rank].  Finalize expands every
+ * table to the full-rank [V, depformer_dim] rows the step reads, row t = bf16(low_rank . e_t) with fp32 accumulation (under
+ * quantize the QLinear product: row-wise int8 of e_t and of low_rank, int32 sums), and releases the factors.  rank in
+ * [1, 4096]; 0 = full-rank tables; ignored on a model without a depformer (dep_q = 0).  The factors must be bf16: the
+ * pre-quantised form of a q8 checkpoint (int8 ".low_rank.weight" + "_scb") is refused at finalize (B200_ERR_INVALID).  Same
+ * timing and errors as b200_lm_set_depformer_schedule. */
+int b200_lm_set_depformer_low_rank(b200_lm* h, int rank);
 /* Keys T of every row's condition memory (k_cross / v_cross bf16 [MB,H,T,128] per layer, allocated at streaming_begin).
  * Before streaming_begin; a cross-attention handle cannot stream without it. */
 int b200_lm_set_cross_len(b200_lm* h, int keys);
@@ -259,8 +276,10 @@ int b200_lm_step_host(b200_lm* h, const int64_t* in_codes_host, int n_in, const 
  * "audio_tokens" i64 [dep_q,B], "noise" f32 [B,b200_lm_noise_per_row] (the Exp(1) draws the samplers read: the step's own
  * draws, or the caller's copy), "extra_heads" bf16 [n_heads,MB,extra_heads_dim] (softmax(extra_head(transformer_out)),
  * lm.py:803-806), "model_text_logits" bf16 [MB,text_card], "model_dep_logits" bf16 [dep_q,MB,card], "dep_in" bf16
- * [MB,dep_q,depformer_dim] (depformer_in[k](transformer_out) for every sub-step k), "depformer.layers.<l>.k" / ".v" bf16
- * [MB,depformer_heads,dep_q,64] (layer l's per-frame cache: every sub-step's key / value after the frame).  With the taps on
+ * [MB,n_sets,depformer_dim] (depformer_in[j](transformer_out) for every weight set j; n_sets = dep_q without a schedule, and
+ * sub-step k reads set schedule[k]), "depformer.layers.<l>.k" / ".v" bf16 [MB,depformer_heads,dep_q,64] (layer l's per-frame
+ * cache: every sub-step's key / value after the frame), "depformer.tables.<k>" bf16 [V,depformer_dim] (sub-step k's embedding
+ * table as the step reads it, V = text_card + 1 for k = 0 and card + 1 after: a low-rank table after its expansion).  With the taps on
  * (b200_lm_set_taps), the temporal transformer of the last step: "temporal.embed" bf16 [MB,dim] (the summed input embeddings
  * entering layer 0) and per layer l "temporal.layers.<l>.attn_out" bf16 [MB,dim] (the attention output, before out_proj),
  * ".x_attn" [MB,dim] (x after the attention residual), ".gated" [MB,ffn_hidden] (silu(gate) * value) and ".x_out" [MB,dim]

@@ -112,6 +112,8 @@ _PROTOTYPES: dict[str, tuple[tp.Any, list]] = {
     "b200_lm_set_cfg": (_I, [_P, C.c_float, _I, _P, _I]),
     "b200_lm_set_condition_sum": (_I, [_P, _P, _I]),
     "b200_lm_set_cross_attention": (_I, [_P, _I]),
+    "b200_lm_set_depformer_schedule": (_I, [_P, C.POINTER(_I), _I]),
+    "b200_lm_set_depformer_low_rank": (_I, [_P, _I]),
     "b200_lm_set_cross_len": (_I, [_P, _I]),
     "b200_lm_set_condition_cross": (_I, [_P, _P, _P, _I]),
     "b200_lm_seed_noise": (_I, [_P, C.c_uint64]),

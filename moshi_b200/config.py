@@ -162,6 +162,11 @@ class LMConfig:
     depformer_gating: str = "silu"
     depformer_pos_emb: str = "none"
     depformer_weights_per_step: bool = True
+    # lm.py:125-127, 172-181, transformer.py:291-316: sub-step k runs weight set schedule[k] of depformer_in and of every depformer
+    # layer's in_projs / out_projs / gating; max(schedule) + 1 sets are stored
+    depformer_weights_per_step_schedule: tp.Optional[tp.List[int]] = None
+    # lm.py:186-196, lm_utils.py:80-124: each depformer embedding is a [V, r] table followed by a bias-free nn.Linear(r, depformer_dim)
+    depformer_low_rank_embeddings: tp.Optional[int] = None
     quantize: bool = False       # LMModel(quantize=True), lm.py:107,242-243: every nn.Linear becomes an int8 QLinear
     extra_heads_num_heads: int = 0   # lm.py:108-109, 224-226: nn.Linear(dim, extra_heads_dim) heads on the temporal output (STT)
     extra_heads_dim: int = 6
@@ -190,6 +195,12 @@ class LMConfig:
     @property
     def depformer_ffn_hidden(self) -> int:
         return _gated_hidden(self.depformer_dim, self.depformer_dim_feedforward)
+
+    @property
+    def depformer_n_sets(self) -> int:
+        """Weight sets of the depformer's per-step linears (lm.py:177-178, transformer.py:399-401)."""
+        s = self.depformer_weights_per_step_schedule
+        return max(s) + 1 if s else self.dep_q
 
     @staticmethod
     def from_dict(d: dict) -> "LMConfig":
@@ -253,8 +264,29 @@ class LMConfig:
             bad.append("heads")
         if self.quantize and any(k % 16 for k in (self.dim, self.ffn_hidden, self.depformer_dim, self.depformer_ffn_hidden)):
             bad.append("quantize (int8 k-extents must be multiples of 16)")
+        bad += self._depformer_sharing_problems()
         if bad:
             raise ValueError(f"LM options outside the GPU hot path: {bad}")
+
+    def _depformer_sharing_problems(self) -> list[str]:
+        bad = []
+        s = self.depformer_weights_per_step_schedule
+        if s is not None:
+            if not (self.depformer_multi_linear and self.depformer_weights_per_step):
+                bad.append("depformer_weights_per_step_schedule without depformer_multi_linear and depformer_weights_per_step")
+            if len(s) != self.dep_q:
+                bad.append(f"depformer_weights_per_step_schedule of length {len(s)} (one entry per depformer step: {self.dep_q})")
+            if any(not isinstance(j, int) or not 0 <= j < self.dep_q for j in s):
+                bad.append(f"depformer_weights_per_step_schedule entries must be in [0, dep_q = {self.dep_q})")
+        r = self.depformer_low_rank_embeddings
+        if r is not None and (not isinstance(r, int) or not 1 <= r <= LOW_RANK_MAX):
+            bad.append(f"depformer_low_rank_embeddings = {r!r} (the rank must be in [1, {LOW_RANK_MAX}]: the load-time expansion "
+                       "holds one row of the factor table in shared memory)")
+        return bad
+
+
+# largest depformer_low_rank_embeddings the load-time table expansion takes (b200_lm_set_depformer_low_rank)
+LOW_RANK_MAX = 4096
 
 
 def _gated_hidden(dim: int, dim_feedforward: int) -> int:

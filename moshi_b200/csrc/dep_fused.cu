@@ -122,16 +122,17 @@ __device__ void row_phase(const P& p, int dd, int S, const float* part, int N, b
   }
 }
 
-// x = depformer_in[k](transformer_out) + emb_k(prev)   (lm.py:475-486; token -1 -> zero row, lm_utils.py:103-121)
+// x = depformer_in[schedule[k]](transformer_out) + emb_k(prev)   (lm.py:475-486; token -1 -> zero row, lm_utils.py:103-121)
 __device__ void input_rows(const DepParams& p, int k) {
   const long long* prev = k == 0 ? p.text_token : p.audio_tokens + (long long)(k - 1) * p.B;
   const bf16* table = p.tables[k];
+  const bf16* din = p.din + p.din_col[k];
   for (int m = blockIdx.x; m < p.B; m += gridDim.x) {
     const long long id = prev[m];
     const bool ok = lm::embed_id_ok(id, k == 0 ? p.text_card : p.card, p.err);
     for (int j = threadIdx.x; j < p.dd; j += THREADS) {
       const float e = ok ? bf2f(table[id * p.dd + j]) : 0.f;
-      p.x[(long long)m * p.dd + j] = f2bf(bf2f(p.din[(long long)m * p.din_ld + (long long)k * p.dd + j]) + e);
+      p.x[(long long)m * p.dd + j] = f2bf(bf2f(din[(long long)m * p.din_ld + j]) + e);
     }
   }
   __syncthreads();                                            // row_phase re-reads x written by other threads of this CTA
@@ -469,16 +470,16 @@ int dep_fused_create(const DepformerPlan& P, const DepParams& host, DepFused** o
   p.Mpad = ((p.B + 15) / 16) * 16;
   p.stages = P.stages; p.stage_bytes = (uint32_t)P.stage_bytes;
   p.g_in = P.g_in; p.g_out = P.g_out; p.g_lin_in = P.g_lin_in; p.g_lin_out = P.g_lin_out; p.g_head = P.g_head;
-  // pointer tables -> one device allocation
+  // pointer tables and the din columns -> one device allocation
   const size_t nq = (size_t)p.dep_q * 8, nl = (size_t)p.L * 8;
-  const void* src[7] = {host.w, host.heads, host.tables, host.n1, host.n2, host.kc, host.vc};
-  const size_t n[7] = {p.dep_q * p.L * sizeof(DepLayerW), nq, nq, nl, nl, nl, nl};
-  size_t off[8] = {0};
-  for (int i = 0; i < 7; ++i) off[i + 1] = off[i] + n[i];
-  std::vector<uint8_t> hp(off[7]);
-  for (int i = 0; i < 7; ++i) memcpy(hp.data() + off[i], src[i], n[i]);
-  if (cudaMalloc(&d->dev_tables, off[7]) != cudaSuccess) { delete d; B200_FAIL(B200_ERR_CUDA, "fused depformer: cudaMalloc failed"); }
-  B200_CUDA(cudaMemcpy(d->dev_tables, hp.data(), off[7], cudaMemcpyHostToDevice));
+  const void* src[8] = {host.w, host.heads, host.tables, host.n1, host.n2, host.kc, host.vc, host.din_col};
+  const size_t n[8] = {p.dep_q * p.L * sizeof(DepLayerW), nq, nq, nl, nl, nl, nl, (size_t)p.dep_q * sizeof(int)};
+  size_t off[9] = {0};
+  for (int i = 0; i < 8; ++i) off[i + 1] = off[i] + n[i];
+  std::vector<uint8_t> hp(off[8]);
+  for (int i = 0; i < 8; ++i) memcpy(hp.data() + off[i], src[i], n[i]);
+  if (cudaMalloc(&d->dev_tables, off[8]) != cudaSuccess) { delete d; B200_FAIL(B200_ERR_CUDA, "fused depformer: cudaMalloc failed"); }
+  B200_CUDA(cudaMemcpy(d->dev_tables, hp.data(), off[8], cudaMemcpyHostToDevice));
   uint8_t* dv = static_cast<uint8_t*>(d->dev_tables);
   p.w = reinterpret_cast<const DepLayerW*>(dv + off[0]);
   p.heads = reinterpret_cast<const uint8_t* const*>(dv + off[1]);
@@ -487,6 +488,7 @@ int dep_fused_create(const DepformerPlan& P, const DepParams& host, DepFused** o
   p.n2 = reinterpret_cast<const bf16* const*>(dv + off[4]);
   p.kc = reinterpret_cast<bf16* const*>(dv + off[5]);
   p.vc = reinterpret_cast<bf16* const*>(dv + off[6]);
+  p.din_col = reinterpret_cast<const int*>(dv + off[7]);
   B200_TRY(act_map(&d->map_xn, p.xn, p.dd, p.B, p.dd, MC, 2));
   B200_TRY(act_map(&d->map_ao, p.ao, p.dd, p.B, p.dd, MC, 2));
   B200_TRY(act_map(&d->map_h, p.hbuf, p.F, p.B, p.F, MC, 2));

@@ -137,7 +137,8 @@ struct DepParams {
   const uint8_t* const* heads;                               // [dep_q]
   const __nv_bfloat16* const* tables;                        // [dep_q] embedding tables ([0] = text)
   const __nv_bfloat16* const* n1; const __nv_bfloat16* const* n2;   // [L] RMSNorm alphas
-  const __nv_bfloat16* din; long long din_ld;                // depformer_in_all output [B][dep_q*dd]
+  const __nv_bfloat16* din; long long din_ld;                // depformer_in_all output [B][n_sets*dd]
+  const int* din_col;                                        // [dep_q] first column of sub-step k's block (its weight set * dd)
   const long long* text_token;                               // [B]
   __nv_bfloat16 *x, *xn, *ao, *hbuf;                         // [B][dd] x3, [B][F]
   __nv_bfloat16* const* kc; __nv_bfloat16* const* vc;        // [L] per-frame KV [B][H][dep_q][64]
@@ -151,7 +152,7 @@ struct DepParams {
 };
 constexpr int DEP_TRACE_SLOTS = 512;
 struct DepFused;
-// p: every field but the plan's, its pointer tables (w .. n2, kc, vc) on the host; they are copied to the device
+// p: every field but the plan's, its pointer tables (w .. n2, kc, vc) and din_col on the host; they are copied to the device
 int dep_fused_create(const DepformerPlan& plan, const DepParams& p, DepFused** out);
 void dep_fused_set_sampling(DepFused* d, int use_sampling, float temp, int top_k);
 void dep_fused_destroy(DepFused* d);

@@ -338,11 +338,15 @@ struct Depformer {
   // configuration
   int dep_q = 0, dd = 0, H = 0, F = 0, L = 0, card = 0, text_card = 0;
   int mode = B200_DEPFORMER_AUTO;              // b200_lm_set_depformer, before streaming_begin
+  // b200_lm_set_depformer_schedule / _low_rank, before the first tensor: sub-step k runs weight set sched[k] of n_sets
+  // (lm.py:172-181, transformer.py:399-401); low_rank > 0: the embedding tables arrive as [V][low_rank] factors
+  std::vector<int> sched;
+  int n_sets = 0, low_rank = 0;
   int kt = 0, ka = 0;                          // Exp(1) draws per noise row of the text sampler, and of each sub-step's
   // weights
-  const bf16* in_all = nullptr;                // depformer_in.{k} stacked: all dep_q projections of transformer_out are one GEMM
+  const bf16* in_all = nullptr;                // depformer_in.{j} stacked: all n_sets projections of transformer_out are one GEMM
   const float* in_s = nullptr;
-  std::vector<Step> w;                         // [dep_q][L]
+  std::vector<Step> w;                         // [dep_q][L], sub-step k pointing at the tiles of set sched[k]
   std::vector<const bf16*> n1, n2;             // [L]
   std::vector<const bf16*> tables;             // [0] = depformer_text_emb, [k] = depformer_emb[k-1]
   std::vector<const bf16*> heads; std::vector<const float*> heads_s;    // linears[k]
@@ -360,7 +364,20 @@ struct Depformer {
   void configure(const b200_lm_config& c) {
     dep_q = c.dep_q; dd = c.depformer_dim; H = c.depformer_num_heads; F = c.depformer_ffn_hidden;
     L = c.dep_q > 0 ? c.depformer_num_layers : 0; card = c.card; text_card = c.text_card;
+    set_schedule(nullptr, 0);
   }
+  // n = 0: one weight set per sub-step
+  void set_schedule(const int* s, int n) {
+    sched.resize(dep_q);
+    n_sets = n ? 0 : dep_q;
+    for (int k = 0; k < dep_q; ++k) {
+      sched[k] = n ? s[k] : k;
+      n_sets = std::max(n_sets, sched[k] + 1);
+    }
+  }
+  // the first column of sub-step k's block of din, and din's row stride
+  int din_col(int k) const { return sched[k] * dd; }
+  long long din_ld() const { return (long long)n_sets * dd; }
   // where sub-step k's draws start in a noise row (k = dep_q: the row's length)
   long long noise_at(int k) const { return kt + (long long)k * ka; }
   void set_sampling(int use_sampling, float temp, int top_k, int top_k_text) {
@@ -406,7 +423,15 @@ struct Depformer {
     if (n == "dep_logits") { *src = cfg ? logits_cfg : logits; *sz = (int64_t)dep_q * B * card * 2; }
     else if (n == "model_dep_logits") { *src = logits; *sz = (int64_t)dep_q * MB * card * 2; }
     else if (n == "dep_trace") { *src = trace; *sz = trace ? (int64_t)tc::DEP_TRACE_SLOTS * 8 : 0; }
-    else if (n == "dep_in" && dep_q > 0) { *src = din; *sz = (int64_t)MB * dep_q * dd * 2; }
+    else if (n == "dep_in" && dep_q > 0) { *src = din; *sz = (int64_t)MB * din_ld() * 2; }
+    else if (n.rfind("depformer.tables.", 0) == 0 && dep_q > 0) {
+      const std::string idx = n.substr(17);
+      const bool digits = !idx.empty() && idx.size() <= 2 && idx.find_first_not_of("0123456789") == std::string::npos;
+      const int k = digits ? atoi(idx.c_str()) : -1;
+      if (k < 0 || k >= dep_q) return false;
+      *src = tables[k];
+      *sz = (int64_t)((k == 0 ? text_card : card) + 1) * dd * 2;
+    }
     else if (n.rfind("depformer.layers.", 0) == 0 && dep_q > 0) {
       // the per-frame cache of one layer: after a frame it holds every sub-step's k / v
       const std::string rest = n.substr(17);
@@ -683,27 +708,54 @@ int tap(b200_lm* h, const bf16* src, int layer, int kind) {
 }
 
 // ---- depformer: loading and running ------------------------------------------------------------------------------------------
+// An embedding table of the depformer as the step reads it, [V][dd] bf16.  Low-rank (lm_utils.py:80-124): "<name>.weight" [V][r]
+// and "<name>.low_rank.weight" [dd][r] are expanded once into that table (lowrank_expand_kernel) and released.  The expansion
+// is exact per token, so the step reads one row per (row, sub-step) from the same layout as a full-rank table; token -1 reads no
+// row (embed_id_ok), as before.
+int get_dep_table(b200_lm* h, const std::string& name, int V, int dd, int r, const bf16** out) {
+  if (r == 0) return get_bf16(h, name + ".weight", {V, dd}, out);
+  const bf16 *e = nullptr, *low = nullptr;
+  const Tensor* lt = h->store.find(name + ".low_rank.weight");
+  if (lt && lt->dtype == B200_I8)
+    B200_FAIL(B200_ERR_INVALID, "lm tensor '%s.low_rank.weight' is pre-quantised (int8): low-rank factors are expanded from bf16 "
+              "only; load the bf16 checkpoint with quantize=True", name.c_str());
+  B200_TRY(get_bf16(h, name + ".weight", {V, r}, &e));
+  B200_TRY(get_bf16(h, name + ".low_rank.weight", {dd, r}, &low));
+  bf16* full = nullptr;
+  B200_TRY(h->weights.alloc_t(&full, (size_t)V * dd, false));
+  lowrank_expand_kernel<<<V, 256, (size_t)r * sizeof(float)>>>(e, low, full, r, dd, h->cfg.quantize);
+  B200_TRY(check_launch("lowrank_expand"));
+  B200_CUDA(cudaStreamSynchronize(nullptr));
+  h->store.release(name + ".weight");
+  h->store.release(name + ".low_rank.weight");
+  h->weight_bytes += ((int64_t)V * dd - (int64_t)V * r - (int64_t)dd * r) * 2;     // the table instead of its factors
+  *out = full;
+  return B200_OK;
+}
+
 int Depformer::load(b200_lm* h) {
   if (dep_q == 0) return B200_OK;
   std::vector<std::string> in_names;
-  for (int k = 0; k < dep_q; ++k) in_names.push_back("depformer_in." + std::to_string(k) + ".weight");
-  B200_TRY(get_linear(h, in_names, dep_q * dd, h->cfg.dim, LIN_STORE, 0, &in_all, &in_s));
+  for (int j = 0; j < n_sets; ++j) in_names.push_back("depformer_in." + std::to_string(j) + ".weight");
+  B200_TRY(get_linear(h, in_names, n_sets * dd, h->cfg.dim, LIN_STORE, 0, &in_all, &in_s));
   tables.resize(dep_q); heads.resize(dep_q); heads_s.resize(dep_q); w.resize((size_t)dep_q * L); n1.resize(L); n2.resize(L);
-  B200_TRY(get_bf16(h, "depformer_text_emb.weight", {text_card + 1, dd}, &tables[0]));
+  B200_TRY(get_dep_table(h, "depformer_text_emb", text_card + 1, dd, low_rank, &tables[0]));
   for (int k = 1; k < dep_q; ++k)
-    B200_TRY(get_bf16(h, "depformer_emb." + std::to_string(k - 1) + ".weight", {card + 1, dd}, &tables[k]));
+    B200_TRY(get_dep_table(h, "depformer_emb." + std::to_string(k - 1), card + 1, dd, low_rank, &tables[k]));
   for (int k = 0; k < dep_q; ++k)
     B200_TRY(get_linear(h, {"linears." + std::to_string(k) + ".weight"}, card, dd, LIN_STORE, 0, &heads[k], &heads_s[k]));
+  std::vector<Step> sets((size_t)n_sets);      // one layer's weight sets, each packed once
   for (int l = 0; l < L; ++l) {
     const std::string p = "depformer.layers." + std::to_string(l);
-    for (int k = 0; k < dep_q; ++k) {
-      const std::string ks = std::to_string(k);
-      Step& S = w[(size_t)k * L + l];
+    for (int j = 0; j < n_sets; ++j) {
+      const std::string ks = std::to_string(j);
+      Step& S = sets[j];
       B200_TRY(get_linear(h, {p + ".self_attn.in_projs." + ks + ".weight"}, 3 * dd, dd, LIN_STORE, 0, &S.in_w, &S.in_s));
       B200_TRY(get_linear(h, {p + ".self_attn.out_projs." + ks + ".weight"}, dd, dd, LIN_RESADD, 0, &S.out_w, &S.out_s));
       B200_TRY(get_linear(h, {p + ".gating." + ks + ".linear_in.weight"}, 2 * F, dd, LIN_GATE, F, &S.lin_in, &S.lin_in_s));
       B200_TRY(get_linear(h, {p + ".gating." + ks + ".linear_out.weight"}, dd, F, LIN_RESADD, 0, &S.lin_out, &S.lin_out_s));
     }
+    for (int k = 0; k < dep_q; ++k) w[(size_t)k * L + l] = sets[sched[k]];
     B200_TRY(get_bf16(h, p + ".norm1.alpha", {1, 1, dd}, &n1[l]));
     B200_TRY(get_bf16(h, p + ".norm2.alpha", {1, 1, dd}, &n2[l]));
   }
@@ -728,7 +780,9 @@ int Depformer::alloc_fused(b200_lm* h) {
   p.B = B; p.dd = dd; p.H = H; p.F = F; p.card = card; p.text_card = text_card; p.dep_q = dep_q; p.L = L; p.err = h->err;
   p.w = lw.data(); p.heads = reinterpret_cast<const uint8_t* const*>(heads.data()); p.tables = tables.data();
   p.n1 = n1.data(); p.n2 = n2.data(); p.kc = kc.data(); p.vc = vc.data();
-  p.din = din; p.din_ld = (long long)dep_q * dd; p.text_token = h->text_token;
+  std::vector<int> cols(dep_q);
+  for (int k = 0; k < dep_q; ++k) cols[k] = din_col(k);
+  p.din = din; p.din_ld = din_ld(); p.din_col = cols.data(); p.text_token = h->text_token;
   p.x = dx; p.xn = dxn; p.ao = dao; p.hbuf = dh; p.part0 = part0; p.part1 = part1;
   p.logits = logits; p.audio_tokens = h->audio_tokens;
   p.noise = h->noise; p.noise_ld = noise_at(dep_q); p.noise_off = (int)noise_at(0); p.ka = ka;
@@ -747,11 +801,11 @@ int Depformer::run(b200_lm* h, bool replace) {
     return B200_OK;
   }
   const int d = h->cfg.dim;
-  B200_TRY(linear(h, h->tout, d, in_all, din, (long long)dep_q * dd, nullptr, 0, MB, dep_q * dd, d, LIN_STORE, 0, in_s));
+  B200_TRY(linear(h, h->tout, d, in_all, din, din_ld(), nullptr, 0, MB, n_sets * dd, d, LIN_STORE, 0, in_s));
   if (plan.path == tc::DEP_FUSED) return tc::dep_fused_launch(fused, st);
   for (int k = 0; k < dep_q; ++k) {
     const long long* prev = k == 0 ? h->text_token : h->audio_tokens + (long long)(k - 1) * B;
-    B200_LAUNCH(dep_input_kernel, ceil_div(MB * dd, 256), 256, 0, st, din, (long long)dep_q * dd, k * dd, tables[k], prev, dx, MB, dd, B,
+    B200_LAUNCH(dep_input_kernel, ceil_div(MB * dd, 256), 256, 0, st, din, din_ld(), din_col(k), tables[k], prev, dx, MB, dd, B,
                 k == 0 ? text_card : card, h->err);
     for (int l = 0; l < L; ++l) {
       const Step& S = w[(size_t)k * L + l];
@@ -1339,6 +1393,31 @@ int b200_lm_set_cross_attention(b200_lm* h, int enable) {
   return B200_OK;
 }
 
+int b200_lm_set_depformer_schedule(b200_lm* h, const int* schedule, int n) {
+  if (!h) B200_FAIL(B200_ERR_INVALID, "lm_set_depformer_schedule: null handle");
+  if (h->finalized || !h->store.items.empty())
+    B200_FAIL(B200_ERR_STATE, "lm_set_depformer_schedule: the weight sets are named by the schedule; set it before the first tensor");
+  const int dep_q = h->cfg.dep_q;
+  if (n != 0 && (n != dep_q || !schedule))
+    B200_FAIL(B200_ERR_INVALID, "lm_set_depformer_schedule: %d entries, the depformer has %d steps", n, dep_q);
+  for (int k = 0; k < n; ++k)
+    if (schedule[k] < 0 || schedule[k] >= dep_q)
+      B200_FAIL(B200_ERR_INVALID, "lm_set_depformer_schedule: entry %d = %d outside [0, %d)", k, schedule[k], dep_q);
+  h->dep.set_schedule(schedule, n);
+  return B200_OK;
+}
+
+int b200_lm_set_depformer_low_rank(b200_lm* h, int rank) {
+  if (!h) B200_FAIL(B200_ERR_INVALID, "lm_set_depformer_low_rank: null handle");
+  if (h->finalized || !h->store.items.empty())
+    B200_FAIL(B200_ERR_STATE, "lm_set_depformer_low_rank: the tables' shapes follow the rank; set it before the first tensor");
+  // without a depformer (dep_q = 0) there are no tables to factor and the rank is ignored, as lm.py:186-196 does
+  if (rank < 0 || rank > DEP_LOW_RANK_MAX)
+    B200_FAIL(B200_ERR_INVALID, "lm_set_depformer_low_rank: rank %d (in [1, %d]; 0 = full rank)", rank, DEP_LOW_RANK_MAX);
+  h->dep.low_rank = rank;
+  return B200_OK;
+}
+
 int b200_lm_set_cross_len(b200_lm* h, int keys) {
   if (!h) B200_FAIL(B200_ERR_INVALID, "lm_set_cross_len: null handle");
   if (!h->cross_on) B200_FAIL(B200_ERR_INVALID, "lm_set_cross_len: the model has no cross-attention layers");
@@ -1617,7 +1696,7 @@ int64_t b200_lm_algorithmic_bytes(b200_lm* h, int kv_fill) {
   int64_t w = 0;
   w += (int64_t)c.num_layers * ((int64_t)3 * c.dim * c.dim + (int64_t)c.dim * c.dim + (int64_t)3 * c.ffn_hidden * c.dim) * 2;
   w += (int64_t)c.text_card * c.dim * 2;
-  w += (int64_t)c.dep_q * c.depformer_dim * c.dim * 2;
+  w += (int64_t)h->dep.n_sets * c.depformer_dim * c.dim * 2;      // depformer_in: one linear per weight set
   w += (int64_t)c.dep_q * c.depformer_num_layers *
        ((int64_t)4 * c.depformer_dim * c.depformer_dim + (int64_t)3 * c.depformer_ffn_hidden * c.depformer_dim) * 2;
   w += (int64_t)c.dep_q * c.card * c.depformer_dim * 2;

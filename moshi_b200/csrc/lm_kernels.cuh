@@ -169,6 +169,53 @@ static __global__ void dep_input_kernel(const bf16* __restrict__ din /*[B][ld]*/
   x[i] = f2bf(bf2f(din[(long long)b * ld + col0 + c]) + e);
 }
 
+// Load time, low-rank depformer embeddings (lm_utils.py:80-124): the full-rank table out[V][dd], row t = low[dd][r] . e_t for the
+// factor rows e[V][r].  One CTA per row.  bf16 weights: fp32 sums in k order.  quantize (QLinear, utils/quantize.py:13-40, restated
+// by oracle/quant.py): the row and each low-rank row are row-wise absmax int8 (the weight through fp16), summed in int32 and
+// dequantised as acc * (sa * sw / 127^2).  Dynamic shared memory: r floats.
+__device__ __forceinline__ int quant_i8_rn(float v, float inv) {       // round(v * 127 / absmax), ties to even, as the linears'
+  const int q = __float2int_rn(v * inv);
+  return q > 127 ? 127 : (q < -127 ? -127 : q);
+}
+static __global__ void lowrank_expand_kernel(const bf16* __restrict__ e, const bf16* __restrict__ low, bf16* __restrict__ out, int r,
+                                             int dd, int quantize) {
+  extern __shared__ float row[];
+  __shared__ float red[32];
+  const long long t = blockIdx.x;
+  float mx = 0.f;
+  for (int i = threadIdx.x; i < r; i += blockDim.x) {
+    row[i] = bf2f(e[t * r + i]);
+    mx = fmaxf(mx, fabsf(row[i]));
+  }
+  if (quantize) {
+    mx = warp_max(mx);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = mx;
+    __syncthreads();
+    float sa = 0.f;
+    for (int i = 0; i < (int)(blockDim.x + 31) / 32; ++i) sa = fmaxf(sa, red[i]);
+    const float inv = sa > 0.f ? 127.f / sa : 0.f;
+    for (int i = threadIdx.x; i < r; i += blockDim.x) row[i] = (float)quant_i8_rn(row[i], inv);
+    __syncthreads();
+    for (int j = threadIdx.x; j < dd; j += blockDim.x) {
+      const bf16* w = low + (long long)j * r;
+      float sw = 0.f;
+      for (int i = 0; i < r; ++i) sw = fmaxf(sw, fabsf(__half2float(__float2half_rn(bf2f(w[i])))));
+      const float winv = sw > 0.f ? 127.f / sw : 0.f;
+      int acc = 0;
+      for (int i = 0; i < r; ++i) acc += (int)row[i] * quant_i8_rn(__half2float(__float2half_rn(bf2f(w[i]))), winv);
+      out[t * dd + j] = f2bf((float)acc * (sa * sw * (1.f / 16129.f)));
+    }
+    return;
+  }
+  __syncthreads();
+  for (int j = threadIdx.x; j < dd; j += blockDim.x) {
+    const bf16* w = low + (long long)j * r;
+    float acc = 0.f;
+    for (int i = 0; i < r; ++i) acc = fmaf(row[i], bf2f(w[i]), acc);
+    out[t * dd + j] = f2bf(acc);
+  }
+}
+
 // classifier-free guidance on logits (lm.py:728-732, 828-833): out = null + (cond - null) * coef, every operation a bf16
 // tensor op like the reference's; rows [0, B) = conditioned, [B, 2B) = null
 static __global__ void cfg_combine_kernel(const bf16* __restrict__ logits /*[2B][card]*/, bf16* __restrict__ out /*[B][card]*/,
@@ -843,6 +890,7 @@ void cross_attn_launch(const bf16* q, long long ldq, const bf16* kc, const bf16*
                        int H, int T, int nsplit, cudaStream_t st);
 
 constexpr int DEP_MAX_Q = 16;              // dep_q of the largest family member (configs/moshi_dev_2b.json)
+constexpr int DEP_LOW_RANK_MAX = 4096;     // rank of low-rank depformer embeddings: lowrank_expand_kernel keeps a row in shared memory
 
 // Depformer attention step: the new key/value of sub-step `step` is appended to the per-frame cache and the query
 // attends over step + 1 keys; no positional embedding (depformer_pos_emb = "none").  One warp per (b, h), D = 64.

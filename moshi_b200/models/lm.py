@@ -24,7 +24,7 @@ import torch
 from .. import _lib
 from ..conditioners import ConditionFuser, ConditionProvider, ConditionTensors, build_conditioning
 from ..config import LMConfig
-from .state_dict import _CANDLE, normalize_lm_state_dict
+from .state_dict import candle_refusal, normalize_lm_state_dict
 
 _TORCH_DTYPES = {_lib.B200_F32: torch.float32, _lib.B200_BF16: torch.bfloat16, _lib.B200_F16: torch.float16,
                  _lib.B200_I64: torch.int64, _lib.B200_U8: torch.uint8}
@@ -78,12 +78,18 @@ class LMModel:
             _lib.check(self._lib.b200_lm_create(C.byref(_config_struct(cfg)), C.byref(self._h)))
             if cfg.cross_attention:
                 _lib.check(self._lib.b200_lm_set_cross_attention(self._h, 1))
+            if cfg.depformer_weights_per_step_schedule is not None:
+                sched = cfg.depformer_weights_per_step_schedule
+                _lib.check(self._lib.b200_lm_set_depformer_schedule(self._h, (C.c_int * len(sched))(*sched), len(sched)))
+            if cfg.depformer_low_rank_embeddings is not None:
+                _lib.check(self._lib.b200_lm_set_depformer_low_rank(self._h, cfg.depformer_low_rank_embeddings))
             for name, t in items:
                 if name.startswith("condition_provider."):
                     host_side[name] = t.detach()
                     continue
-                if cfg.cross_attention and _CANDLE.match(name):
-                    raise ValueError("candle-layout checkpoints of a cross-attention LM are not supported; load its safetensors checkpoint")
+                why = candle_refusal(cfg, name)
+                if why is not None:
+                    raise ValueError(why)
                 for n2, t2 in normalize_lm_state_dict({name: t}).items():
                     # a q8 checkpoint stores a QLinear as `weight` int8 + `weight_scb` float32, and the scale must stay float32
                     # (utils/quantize.py:13-35; the reference's loader casts it with the rest, loaders.py:415-421, and then fails)

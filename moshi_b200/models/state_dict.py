@@ -88,5 +88,23 @@ def _from_candle(sd: tp.Mapping[str, torch.Tensor]) -> dict[str, torch.Tensor]:
     return out
 
 
+def candle_refusal(cfg, key: str) -> str | None:
+    """Why the candle-layout tensor ``key`` cannot be loaded into an LM of configuration ``cfg`` (None: it can).
+    ``scripts/import_rust.py:69-110`` writes one slice per depformer step, a weight-sharing schedule unrolled into copies of
+    the shared sets: slice k holds set schedule[k], not set k, so a scheduled model would read the wrong weights from the
+    renamed slices.  Low-rank depformer embeddings have no candle form that this loader knows."""
+    if _CANDLE.match(key) is None:
+        return None
+    if cfg.cross_attention:
+        return "candle-layout checkpoints of a cross-attention LM are not supported; load its safetensors checkpoint"
+    if cfg.depformer_weights_per_step_schedule is not None:
+        return ("candle-layout checkpoints of an LM with depformer_weights_per_step_schedule are not supported (the layout unrolls "
+                "the schedule into one slice per step); load its safetensors checkpoint")
+    if cfg.depformer_low_rank_embeddings is not None:
+        return ("candle-layout checkpoints of an LM with depformer_low_rank_embeddings are not supported; load its safetensors "
+                "checkpoint")
+    return None
+
+
 def normalize_lm_state_dict(sd: tp.Mapping[str, torch.Tensor]) -> dict[str, torch.Tensor]:
     return _split_attention(_from_candle(sd))

@@ -196,14 +196,19 @@ def lm_tensor_specs(cfg: LMConfig) -> list[tuple[str, tuple[int, ...], float]]:
         specs.append((p + ".learnt_padding", (1, 1, d), 75.0))
     if cfg.dep_q == 0:                                               # lm.py:219-222: no depformer at all
         return specs
-    for k in range(cfg.dep_q):
+    n_sets, r = cfg.depformer_n_sets, cfg.depformer_low_rank_embeddings
+    for k in range(n_sets):
         specs.append((f"depformer_in.{k}.weight", (dd, d), d))
     for k in range(cfg.dep_q - 1):
-        specs.append((f"depformer_emb.{k}.weight", (cfg.card + 1, dd), dd))
-    specs.append(("depformer_text_emb.weight", (cfg.text_card + 1, dd), dd))
+        specs.append((f"depformer_emb.{k}.weight", (cfg.card + 1, r or dd), r or dd))
+        if r:                                                        # lm_utils.py:80-94: nn.Linear(r, dd, bias=False)
+            specs.append((f"depformer_emb.{k}.low_rank.weight", (dd, r), r))
+    specs.append(("depformer_text_emb.weight", (cfg.text_card + 1, r or dd), r or dd))
+    if r:
+        specs.append(("depformer_text_emb.low_rank.weight", (dd, r), r))
     for layer in range(cfg.depformer_num_layers):
         p = f"depformer.layers.{layer}"
-        for k in range(cfg.dep_q):
+        for k in range(n_sets):
             specs.append((f"{p}.self_attn.in_projs.{k}.weight", (3 * dd, dd), dd))
             specs.append((f"{p}.self_attn.out_projs.{k}.weight", (dd, dd), dd))
             specs.append((f"{p}.gating.{k}.linear_in.weight", (2 * hd, dd), dd))
