@@ -12,10 +12,6 @@ namespace {
 struct TLayer {
   const bf16 *in_w, *out_w, *n1, *n2, *lin_in, *lin_out;
   const float *in_s = nullptr, *out_s = nullptr, *lin_in_s = nullptr, *lin_out_s = nullptr;   // int8 path: weight-row scales
-  // cross-attention layers (b200_lm_set_cross_attention): norm_cross, the query / K|V / output linears, and the condition memory
-  // k_cross / v_cross [MB][H][cross_len][ATT_D] bf16
-  const bf16 *ncw = nullptr, *ncb = nullptr, *cq_w = nullptr, *ckv_w = nullptr, *co_w = nullptr;
-  bf16 *kx = nullptr, *vx = nullptr;
 };
 
 }  // namespace
@@ -451,6 +447,127 @@ struct Depformer {
 
 }  // namespace
 
+// ---- cross-attention conditioning ---------------------------------------------------------------------------------------------
+// The TTS models' conditioning (transformer.py:727-732, 779-798): every temporal layer attends to its row's condition memory
+// k_cross / v_cross [MB][H][T][ATT_D] bf16.  Only this unit knows the key count T, the layers' weights, the memory's size and
+// buffers, its fill, the step's block, the state entries and the record section; the handle asks only whether it is on (taps).
+namespace {
+
+// condition rows (x T keys) per K/V projection GEMM of the fill: the LM GEMMs take at most 256 rows
+constexpr int CROSS_CHUNK = 256;
+
+struct CrossAttention {
+  // configuration: b200_lm_set_cross_attention before finalize, b200_lm_set_cross_len before streaming_begin
+  bool on = false;
+  int T = 0;                                   // keys per condition memory
+  int d = 0, H = 0;                            // the model's
+  // per layer (when on): norm_cross weight and bias, the query / K|V / output linears in packed tiles, and the memory's K and V
+  struct Layer { const bf16 *nw = nullptr, *nb = nullptr, *q_w = nullptr, *kv_w = nullptr, *out_w = nullptr; bf16 *k = nullptr, *v = nullptr; };
+  std::vector<Layer> layers;
+  // per batch
+  int MB = 0, nsplit = 1;                      // model rows, splits of the attention
+  bf16 *chunk = nullptr, *chunk_kv = nullptr;  // fill staging: [CROSS_CHUNK][d] rows of the condition, their K|V
+  int* rows_dev = nullptr;                     // [MB] model rows of the condition rows being filled
+
+  int set(int enable, const b200_lm_config& c) {
+    if (enable && c.quantize)      // the reference's _compute_cross_attention asserts an nn.Linear in_proj
+      B200_FAIL(B200_ERR_INVALID, "lm_set_cross_attention: cross-attention layers with quantize=True (int8 linears) are not supported");
+    on = enable != 0;
+    d = c.dim; H = c.num_heads;
+    layers.assign(on ? c.num_layers : 0, Layer{});
+    return B200_OK;
+  }
+  int set_len(int keys, bool streaming) {
+    if (!on) B200_FAIL(B200_ERR_INVALID, "lm_set_cross_len: the model has no cross-attention layers");
+    if (streaming) B200_FAIL(B200_ERR_STATE, "lm_set_cross_len: the condition memory is allocated at streaming_begin; set it before");
+    if (keys < 1 || keys > (1 << 20)) B200_FAIL(B200_ERR_INVALID, "lm_set_cross_len: %d keys", keys);
+    T = keys;
+    return B200_OK;
+  }
+
+  // bytes of one model row's memory in one layer, K or V
+  int64_t row_bytes() const { return (int64_t)H * T * ATT_D * 2; }
+  // bytes of the memory of `rows` model rows, K and V of every layer (0 when off)
+  int64_t bytes(int64_t rows) const { return (int64_t)layers.size() * 2 * rows * row_bytes(); }
+  // the largest M of its linears (the fill's chunks; the step's run MB), 0 when off
+  int max_m() const { return on ? CROSS_CHUNK : 0; }
+
+  // streaming_begin, before it allocates: `rows` model rows, and the splits of the attention (its partials share attn_part)
+  int plan(int rows) {
+    if (on && T < 1) B200_FAIL(B200_ERR_STATE, "lm_streaming_begin: set the condition memory's length (b200_lm_set_cross_len) first");
+    MB = rows;
+    nsplit = on ? attn_pick_splits(MB, H, T) : 1;
+    return B200_OK;
+  }
+  // layer l's memory, where streaming_begin allocates that layer's state
+  int alloc_layer(Arena& A, int l) {
+    if (!on) return B200_OK;
+    B200_TRY(A.alloc_t(&layers[l].k, (size_t)MB * H * T * ATT_D));
+    return A.alloc_t(&layers[l].v, (size_t)MB * H * T * ATT_D);
+  }
+  int alloc_fill(Arena& A) {
+    if (!on) return B200_OK;
+    B200_TRY(A.alloc_t(&chunk, (size_t)CROSS_CHUNK * d, false));
+    B200_TRY(A.alloc_t(&chunk_kv, (size_t)CROSS_CHUNK * 2 * d, false));
+    return A.alloc_t(&rows_dev, MB, false);
+  }
+  // the state entries layers.<l>.k_cross / .v_cross (_MHAState, transformer.py:321-327)
+  void mark_state(Arena& A) const {
+    for (size_t l = 0; l < layers.size(); ++l) {
+      const std::string p = "layers." + std::to_string(l);
+      A.mark_state(layers[l].k, (size_t)(MB * row_bytes()), p + ".k_cross", B200_BF16, {MB, H, T, ATT_D});
+      A.mark_state(layers[l].v, (size_t)(MB * row_bytes()), p + ".v_cross", B200_BF16, {MB, H, T, ATT_D});
+    }
+  }
+  void end() {
+    MB = 0; nsplit = 1;
+    chunk = chunk_kv = nullptr; rows_dev = nullptr;
+    for (Layer& L : layers) L.k = L.v = nullptr;
+  }
+  int load(b200_lm* h, int l);
+  int fill(b200_lm* h, const void* src, const int32_t* rows_host, int n_rows) const;
+  int step(b200_lm* h, int l) const;
+
+  // The condition-memory section of a session record: from the first 256-byte boundary at or after `end` (*off), the memory of
+  // the session's `rows` model rows as [layer][k|v][model row][H][T][ATT_D] bf16.  Returns the record's end (`end` when off).
+  int64_t record_section(int64_t end, int rows, int64_t* off) const {
+    *off = (end + 255) / 256 * 256;
+    return on ? *off + bytes(rows) : end;
+  }
+  // model rows row + k * row_step (k < rows) to or from that section at `at`, each row's memory a contiguous [H][T][ATT_D]
+  int record(int row, int rows, int row_step, char* at, bool gather, cudaStream_t st) const {
+    const int64_t rb = row_bytes();
+    for (const Layer& L : layers)
+      for (bf16* m : {L.k, L.v})
+        for (int k = 0; k < rows; ++k, at += rb) {
+          char* mem = reinterpret_cast<char*>(m) + (int64_t)(row + k * row_step) * rb;
+          B200_CUDA(cudaMemcpyAsync(gather ? at : mem, gather ? mem : at, (size_t)rb, cudaMemcpyDeviceToDevice, st));
+        }
+    return B200_OK;
+  }
+  // export: SESSION_CROSS, and T in the header's first reserved bytes
+  void stamp(SessionHeader* s) const {
+    if (!on) return;
+    s->flags |= SESSION_CROSS;
+    memcpy(s->reserved, &T, sizeof(int32_t));
+  }
+  // import: a record whose flag or T differs from the handle's is refused
+  int check_record(const SessionHeader& s, const char* what) const {
+    if (((s.flags & SESSION_CROSS) != 0) != on) B200_FAIL(B200_ERR_INVALID, "%s: cross-attention conditioning on one side only", what);
+    int32_t keys = 0;
+    memcpy(&keys, s.reserved, sizeof(keys));
+    if (on && keys != T)
+      B200_FAIL(B200_ERR_INVALID, "%s: the record's condition memory has %d keys, the handle's %d", what, keys, T);
+    return B200_OK;
+  }
+
+  // its part of b200_lm_algorithmic_bytes for `rows` model rows: the query, K|V and output linears of every layer, once per step,
+  // and each row's read of its memory
+  int64_t algorithmic_bytes(int64_t rows) const { return on ? (int64_t)layers.size() * 4 * d * d * 2 + bytes(1) * rows : 0; }
+};
+
+}  // namespace
+
 struct b200_lm : StreamCore {       // batch: sessions (LMGen batch); graphs[0]: the step
   b200_lm_config cfg;
   TensorStore store;
@@ -493,6 +610,7 @@ struct b200_lm : StreamCore {       // batch: sessions (LMGen batch); graphs[0]:
   int* attn_counters = nullptr;                // split arrival counters [B*H]
   Depformer dep;                               // the depformer: weights, buffers and the path it runs on
   TemporalKv kv;                               // the temporal K/V: rings or pool, their state entries and record section
+  CrossAttention cross;                        // cross-attention conditioning: weights, condition memory, fill and record section
   // session records: the per-session slices of the small state entries; the condition_sum rows come last and travel while it is on
   RowSlice* slices_dev = nullptr;
   int n_slices = 0, n_slices_cond = 0;
@@ -501,12 +619,6 @@ struct b200_lm : StreamCore {       // batch: sessions (LMGen batch); graphs[0]:
   // b200_lm_set_taps: the step copies the temporal stack's activations into taps (see tap_slot), allocated on first enable
   int taps_on = 0;
   bf16* taps = nullptr;
-  // cross-attention conditioning (transformer.py:727-732, 779-798): every temporal layer attends to its row's condition memory
-  int cross_on = 0;                            // b200_lm_set_cross_attention, before finalize
-  int cross_len = 0;                           // b200_lm_set_cross_len: keys per condition memory, before streaming_begin
-  int cross_nsplit = 1;
-  bf16 *cross_src = nullptr, *cross_kv = nullptr;      // fill staging: [CROSS_CHUNK][dim] rows of the condition, their K|V
-  int* cross_rows = nullptr;                   // [MB] model rows of the condition rows being filled
   int n_in_static = 0;
   int noise_static = 0;                        // 1: the captured step draws its own noise
   int replace_static = 0;                      // 1: this step's audio tokens are given (depformer_replace_tokens, lm.py:751-755)
@@ -646,18 +758,6 @@ int get_linear(b200_lm* h, const std::vector<std::string>& names, int N, int K, 
   return B200_OK;
 }
 
-// A bf16 weight [N][K] already on the device (a slice of a loaded tensor) -> packed tiles; the caller releases the tensor
-int pack_bf16(b200_lm* h, const bf16* w, int N, int K, int epi, const bf16** out) {
-  void* packed = nullptr;
-  B200_TRY(h->weights.alloc(&packed, tc::sk_packed_bytes(N, K, epi, 0), false));
-  B200_TRY(tc::sk_pack_weights(w, packed, N, K, epi, 0, nullptr));
-  *out = static_cast<const bf16*>(packed);
-  return B200_OK;
-}
-
-// condition rows (x T keys) per K/V projection GEMM of b200_lm_set_condition_cross: the LM GEMMs take at most 256 rows
-constexpr int CROSS_CHUNK = 256;
-
 // logits [MB][card] of the model -> the [batch][card] rows the sampler reads: the conditioned rows themselves, or (CFG) the
 // guided combination written to `guided`
 const bf16* guide(b200_lm* h, const bf16* logits, bf16* guided, int card, bool combine) {
@@ -688,7 +788,7 @@ TokenRing ring(b200_lm* h) {
 enum TapKind { TAP_ATTN_OUT, TAP_X_ATTN, TAP_GATED, TAP_X_OUT, TAP_CROSS_OUT, TAP_X_CROSS };
 int64_t tap_elems(const b200_lm* h) {
   const int64_t MB = h->MB, d = h->cfg.dim;
-  return MB * d + (int64_t)h->layers.size() * MB * ((h->cross_on ? 5 : 3) * d + h->cfg.ffn_hidden);
+  return MB * d + (int64_t)h->layers.size() * MB * ((h->cross.on ? 5 : 3) * d + h->cfg.ffn_hidden);
 }
 // first element of a tap (layer -1: the embeddings) and its element count
 int64_t tap_slot(const b200_lm* h, int layer, int kind, int64_t* n) {
@@ -696,7 +796,7 @@ int64_t tap_slot(const b200_lm* h, int layer, int kind, int64_t* n) {
   *n = kind == TAP_GATED ? MB * F : MB * d;
   if (layer < 0) return 0;
   const int64_t at[6] = {0, MB * d, 2 * MB * d, 2 * MB * d + MB * F, 3 * MB * d + MB * F, 4 * MB * d + MB * F};
-  return MB * d + (int64_t)layer * MB * ((h->cross_on ? 5 : 3) * d + F) + at[kind];
+  return MB * d + (int64_t)layer * MB * ((h->cross.on ? 5 : 3) * d + F) + at[kind];
 }
 // device-to-device copy on the step's stream (a memcpy node of the captured graph); nothing when taps are off
 int tap(b200_lm* h, const bf16* src, int layer, int kind) {
@@ -823,6 +923,74 @@ int Depformer::run(b200_lm* h, bool replace) {
   return B200_OK;
 }
 
+// ---- cross-attention: loading, fill and step ----------------------------------------------------------------------------------
+// Layer l's weights (transformer.py:495-505, 727-732): in_projs.0 rows [0, d) packed as the query linear, rows [d, 3d) as one
+// [2d, d] K|V linear of the condition, out_projs.0 as a RESADD linear; norm_cross weight and bias.
+int CrossAttention::load(b200_lm* h, int l) {
+  if (!on) return B200_OK;
+  const std::string p = "transformer.layers." + std::to_string(l);
+  Layer& L = layers[l];
+  const std::string x = p + ".cross_attention.in_projs.0.weight";
+  const bf16* w = nullptr;
+  B200_TRY(get_bf16(h, x, {3 * d, d}, &w));
+  auto pack = [&](const bf16* rows, int N, const bf16** out) -> int {     // a slice of the loaded tensor -> packed tiles
+    void* packed = nullptr;
+    B200_TRY(h->weights.alloc(&packed, tc::sk_packed_bytes(N, d, LIN_STORE, 0), false));
+    B200_TRY(tc::sk_pack_weights(rows, packed, N, d, LIN_STORE, 0, nullptr));
+    *out = static_cast<const bf16*>(packed);
+    return B200_OK;
+  };
+  B200_TRY(pack(w, d, &L.q_w));
+  B200_TRY(pack(w + (size_t)d * d, 2 * d, &L.kv_w));
+  B200_CUDA(cudaStreamSynchronize(nullptr));
+  h->store.release(x);
+  const float* no_scales = nullptr;
+  B200_TRY(get_linear(h, {p + ".cross_attention.out_projs.0.weight"}, d, d, LIN_RESADD, 0, &L.out_w, &no_scales));
+  B200_TRY(get_bf16(h, p + ".norm_cross.weight", {d}, &L.nw));
+  return get_bf16(h, p + ".norm_cross.bias", {d}, &L.nb);
+}
+
+// b200_lm_set_condition_cross, outside the step (transformer.py:495-505 per layer): kv = src @ Wkv^T in chunks of rows, then
+// "b t (p h d) -> p b h t d" into the rows' memory.  The chunk is staged in a fixed buffer so that the GEMM's activation plan is
+// the same every call.
+int CrossAttention::fill(b200_lm* h, const void* src, const int32_t* rows_host, int n_rows) const {
+  if (!on) B200_FAIL(B200_ERR_INVALID, "lm_set_condition_cross: the model has no cross-attention layers");
+  if (!src || n_rows < 1 || n_rows > MB) B200_FAIL(B200_ERR_INVALID, "lm_set_condition_cross: %d condition rows", n_rows);
+  if (!rows_host && n_rows != MB)       // lm.py:650-651: "cfg requires 2x more conditions"
+    B200_FAIL(B200_ERR_SHAPE, "lm_set_condition_cross: %d rows given, the model runs on %d", n_rows, MB);
+  std::vector<int> rows(n_rows);
+  for (int k = 0; k < n_rows; ++k) {
+    rows[k] = rows_host ? rows_host[k] : k;
+    if (rows[k] < 0 || rows[k] >= MB) B200_FAIL(B200_ERR_INVALID, "lm_set_condition_cross: model row %d outside [0, %d)", rows[k], MB);
+  }
+  B200_CUDA(cudaMemcpyAsync(rows_dev, rows.data(), rows.size() * 4, cudaMemcpyHostToDevice, h->stream));
+  B200_TRY(tc::linear_prepare());
+  h->body = h->stream;
+  const long long total = (long long)n_rows * T;
+  for (long long i0 = 0; i0 < total; i0 += CROSS_CHUNK) {
+    const int n = (int)std::min<long long>(CROSS_CHUNK, total - i0);
+    B200_CUDA(cudaMemcpyAsync(chunk, static_cast<const bf16*>(src) + i0 * d, (size_t)n * d * 2, cudaMemcpyDeviceToDevice, h->stream));
+    for (const Layer& L : layers) {
+      B200_TRY(linear(h, chunk, d, L.kv_w, chunk_kv, 2 * d, nullptr, 0, n, 2 * d, d, LIN_STORE, 0));
+      B200_LAUNCH(cross_kv_scatter_kernel, (unsigned)ceil_div64((long long)n * 2 * H * (ATT_D / 8), 256), 256, 0, h->stream, chunk_kv,
+                  i0, n, rows_dev, L.k, L.v, H, T);
+    }
+  }
+  return check_launch("lm_set_condition_cross");
+}
+
+// Layer l's block between its self-attention and its MLP: x = x + cross_attention(norm_cross(x), memory) (transformer.py:779-798)
+int CrossAttention::step(b200_lm* h, int l) const {
+  if (!on) return B200_OK;
+  const Layer& L = layers[l];
+  B200_LAUNCH(layernorm_kernel, MB, 256, 0, h->body, h->x, L.nw, L.nb, h->xn, d, 1e-5f);
+  B200_TRY(linear(h, h->xn, d, L.q_w, h->qkv, d, nullptr, 0, MB, d, d, LIN_STORE, 0));
+  cross_attn_launch(h->qkv, d, L.k, L.v, h->ao, h->attn_part, h->attn_counters, MB, H, T, nsplit, h->body);
+  B200_TRY(tap(h, h->ao, l, TAP_CROSS_OUT));
+  B200_TRY(linear(h, h->ao, d, L.out_w, h->x, d, h->x, d, MB, d, d, LIN_RESADD, 0));
+  return tap(h, h->x, l, TAP_X_CROSS);
+}
+
 // The whole frame as a fixed launch sequence over static buffers (captured into one CUDA graph).
 int step_body(b200_lm* h) {
   const auto& c = h->cfg;
@@ -852,14 +1020,7 @@ int step_body(b200_lm* h) {
     B200_TRY(tap(h, h->ao, (int)l, TAP_ATTN_OUT));
     B200_TRY(linear(h, h->ao, d, L.out_w, h->x, d, h->x, d, MB, d, d, LIN_RESADD, 0, L.out_s));
     B200_TRY(tap(h, h->x, (int)l, TAP_X_ATTN));
-    if (h->cross_on) {     // x = x + cross_attention(norm_cross(x), condition memory) (transformer.py:779-798)
-      B200_LAUNCH(layernorm_kernel, MB, 256, 0, st, h->x, L.ncw, L.ncb, h->xn, d, 1e-5f);
-      B200_TRY(linear(h, h->xn, d, L.cq_w, h->qkv, d, nullptr, 0, MB, d, d, LIN_STORE, 0));
-      cross_attn_launch(h->qkv, d, L.kx, L.vx, h->ao, h->attn_part, h->attn_counters, MB, H, h->cross_len, h->cross_nsplit, st);
-      B200_TRY(tap(h, h->ao, (int)l, TAP_CROSS_OUT));
-      B200_TRY(linear(h, h->ao, d, L.co_w, h->x, d, h->x, d, MB, d, d, LIN_RESADD, 0));
-      B200_TRY(tap(h, h->x, (int)l, TAP_X_CROSS));
-    }
+    B200_TRY(h->cross.step(h, (int)l));
     B200_TRY(norm_linear(h, h->x, L.n2, h->xn, L.lin_in, h->hbuf, F, MB, F, d, LIN_GATE, F, L.lin_in_s));
     B200_TRY(tap(h, h->hbuf, (int)l, TAP_GATED));
     B200_TRY(linear(h, h->hbuf, F, L.lin_out, h->x, d, h->x, d, MB, d, F, LIN_RESADD, 0, L.lin_out_s));
@@ -884,9 +1045,8 @@ int step_body(b200_lm* h) {
 // After the 256-byte SessionHeader: the session's slices of exec_mask, cache, offsets, model.offset (1 or 2 rows), under CFG
 // model.exec_mask (2 rows) and cfg_is_masked_until, and while it is on the condition_sum rows, each 16-byte aligned (the
 // RowSlice table of streaming_begin).  From the next 256-byte boundary, the temporal K/V of slots [0, n), n = min(pos, ring
-// capacity), slot s being position s mod capacity (TemporalKv::record).  A cross-attention handle's record (SESSION_CROSS, the
-// memory's key count T in the header's first reserved bytes) ends, from the next 256-byte boundary, with the session's condition
-// memory [layer][k|v][model row][head][T][128] bf16.
+// capacity), slot s being position s mod capacity (TemporalKv::record).  A cross-attention handle's record ends with the session's
+// condition memory (CrossAttention::record_section).
 struct SessionPlan {
   int rows = 1;
   int64_t pos[2] = {0, 0};
@@ -894,17 +1054,10 @@ struct SessionPlan {
   bool cond = false;
 };
 
-// bytes of one model row's condition memory in one layer (K or V)
-int64_t cross_row_bytes(const b200_lm* h) { return (int64_t)h->cfg.num_heads * h->cross_len * ATT_D * 2; }
-
 void session_size(const b200_lm* h, SessionPlan* p) {
   const long long end = p->cond ? h->slices_end_cond : h->slices_end;
   p->kv_off = (end + 255) / 256 * 256;
-  p->bytes = p->kv_off + h->kv.record_bytes(p->rows, p->n);
-  if (h->cross_on) {
-    p->cross_off = (p->bytes + 255) / 256 * 256;
-    p->bytes = p->cross_off + (int64_t)h->cfg.num_layers * 2 * p->rows * cross_row_bytes(h);
-  }
+  p->bytes = h->cross.record_section(p->kv_off + h->kv.record_bytes(p->rows, p->n), p->rows, &p->cross_off);
 }
 
 // The record row `row` would export now (synchronises): B200_ERR_STATE for a short-ring row whose ring has already wrapped.
@@ -922,20 +1075,10 @@ int session_plan(b200_lm* h, int row, const char* what, SessionPlan* p) {
   return B200_OK;
 }
 
-// The session's K/V between the rings and the record
+// The session's temporal K/V and condition memory between the device and the record
 int session_kv(b200_lm* h, int row, const SessionPlan& p, char* rec, bool gather) {
   B200_TRY(h->kv.record(row, p.rows, h->batch, (int)p.n, rec + p.kv_off, gather, h->stream));
-  if (h->cross_on) {         // the condition memory of the session's model rows, each contiguous [H][T][128]
-    const int64_t rb = cross_row_bytes(h);
-    char* at = rec + p.cross_off;
-    for (auto& L : h->layers)
-      for (bf16* m : {L.kx, L.vx})
-        for (int k = 0; k < p.rows; ++k, at += rb) {
-          char* mem = reinterpret_cast<char*>(m) + (int64_t)(row + k * h->batch) * rb;
-          B200_CUDA(cudaMemcpyAsync(gather ? at : mem, gather ? mem : at, (size_t)rb, cudaMemcpyDeviceToDevice, h->stream));
-        }
-  }
-  return B200_OK;
+  return h->cross.record(row, p.rows, h->batch, rec + p.cross_off, gather, h->stream);
 }
 
 }  // namespace
@@ -1012,8 +1155,6 @@ int b200_lm_finalize(b200_lm* h) {
   if (h->finalized) return B200_OK;
   const auto& c = h->cfg;
   const int d = c.dim, F = c.ffn_hidden;
-  if (h->cross_on && c.quantize)      // the reference's _compute_cross_attention asserts an nn.Linear in_proj
-    B200_FAIL(B200_ERR_INVALID, "lm_finalize: cross-attention layers with quantize=True (int8 linears) are not supported");
   h->emb.n_q = c.n_q; h->emb.card = c.card; h->emb.text_card = c.text_card; h->emb.condition_sum = nullptr; h->emb.err = nullptr;
   DeviceGuard guard_dev(h->device);
   for (int k = 0; k < c.n_q; ++k)
@@ -1031,19 +1172,7 @@ int b200_lm_finalize(b200_lm* h) {
     B200_TRY(get_bf16(h, p + ".norm2.alpha", {1, 1, d}, &L.n2));
     B200_TRY(get_linear(h, {p + ".gating.linear_in.weight"}, 2 * F, d, LIN_GATE, F, &L.lin_in, &L.lin_in_s));
     B200_TRY(get_linear(h, {p + ".gating.linear_out.weight"}, d, F, LIN_RESADD, 0, &L.lin_out, &L.lin_out_s));
-    if (h->cross_on) {      // transformer.py:495-505, 727-732: in_projs.0 rows [0, d) the query, [d, 3d) K|V of the condition
-      const std::string x = p + ".cross_attention.in_projs.0.weight";
-      const bf16* w = nullptr;
-      const float* no_scales = nullptr;
-      B200_TRY(get_bf16(h, x, {3 * d, d}, &w));
-      B200_TRY(pack_bf16(h, w, d, d, LIN_STORE, &L.cq_w));
-      B200_TRY(pack_bf16(h, w + (size_t)d * d, 2 * d, d, LIN_STORE, &L.ckv_w));
-      B200_CUDA(cudaStreamSynchronize(nullptr));
-      h->store.release(x);
-      B200_TRY(get_linear(h, {p + ".cross_attention.out_projs.0.weight"}, d, d, LIN_RESADD, 0, &L.co_w, &no_scales));
-      B200_TRY(get_bf16(h, p + ".norm_cross.weight", {d}, &L.ncw));
-      B200_TRY(get_bf16(h, p + ".norm_cross.bias", {d}, &L.ncb));
-    }
+    B200_TRY(h->cross.load(h, l));
   }
   for (int i = 0; i < c.extra_heads_num_heads; ++i) {      // lm.py:224-226
     const bf16* w = nullptr;
@@ -1133,7 +1262,7 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
   DeviceGuard guard_dev(h->device);
   const auto& c = h->cfg;
   const bool cfg = cfg_on(h);
-  const int B = batch, MB = cfg ? 2 * batch : batch, d = c.dim, H = c.num_heads, D = d / H;
+  const int B = batch, MB = cfg ? 2 * batch : batch, d = c.dim, H = c.num_heads;
   if (MB > 256) B200_FAIL(B200_ERR_INVALID, "lm_streaming_begin: %d model rows (the linears take at most 256)", MB);
   if (cfg && !h->cfg_until_host.empty() && (int)h->cfg_until_host.size() != B)      // lm.py:717 view(-1, 1, 1) broadcast
     B200_FAIL(B200_ERR_SHAPE, "lm_streaming_begin: cfg_is_masked_until has %zu entries for %d sessions", h->cfg_until_host.size(), B);
@@ -1143,11 +1272,8 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
   size_t free_b = 0, total_b = 0;
   cudaMemGetInfo(&free_b, &total_b);
   B200_TRY(h->kv.plan(MB, c.num_layers));
-  if (h->cross_on && h->cross_len < 1)
-    B200_FAIL(B200_ERR_STATE, "lm_streaming_begin: set the condition memory's length (b200_lm_set_cross_len) first");
-  // the cross-attention handle's condition memory: K and V [MB][H][T][128] bf16 per layer
-  const size_t cross_bytes = h->cross_on ? (size_t)c.num_layers * 2 * MB * h->cross_len * d * 2 : 0;
-  const size_t kv_bytes = h->kv.bytes() + cross_bytes;
+  B200_TRY(h->cross.plan(MB));
+  const size_t kv_bytes = h->kv.bytes() + h->cross.bytes(MB);
   if (kv_bytes + (1ull << 30) > free_b)
     B200_FAIL(B200_ERR_INVALID, "lm_streaming_begin: %d sessions need %.1f GB of KV ring, %.1f GB free", B, kv_bytes / 1e9,
               free_b / 1e9);
@@ -1175,19 +1301,11 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
   B200_TRY(A.alloc_t(&h->pos, MB));
   h->kv.pos = h->pos;
   h->offset_cpu = 0;
-  for (size_t l = 0; l < h->layers.size(); ++l) {
-    TLayer& L = h->layers[l];
-    B200_TRY(h->kv.alloc_layer(A, (int)l));
-    if (h->cross_on) {
-      B200_TRY(A.alloc_t(&L.kx, (size_t)MB * H * h->cross_len * D));
-      B200_TRY(A.alloc_t(&L.vx, (size_t)MB * H * h->cross_len * D));
-    }
+  for (int l = 0; l < c.num_layers; ++l) {
+    B200_TRY(h->kv.alloc_layer(A, l));
+    B200_TRY(h->cross.alloc_layer(A, l));
   }
-  if (h->cross_on) {
-    B200_TRY(A.alloc_t(&h->cross_src, (size_t)CROSS_CHUNK * d, false));
-    B200_TRY(A.alloc_t(&h->cross_kv, (size_t)CROSS_CHUNK * 2 * d, false));
-    B200_TRY(A.alloc_t(&h->cross_rows, MB, false));
-  }
+  B200_TRY(h->cross.alloc_fill(A));
   B200_TRY(h->kv.alloc_pages(A));
   B200_TRY(h->dep.begin(A, B, cfg, c.quantize != 0));
   const int n_in_max = c.n_q;   // callers may pass more columns than needed (lm.py:688-689)
@@ -1218,13 +1336,11 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
   }
   if (!h->extra_w.empty()) B200_TRY(A.alloc_t(&h->extra_out, h->extra_w.size() * (size_t)MB * c.extra_heads_dim));
   B200_TRY(h->dep.alloc_activations(A));
-  // (the condition memory's K/V projection runs CROSS_CHUNK rows at a time)
-  B200_TRY(A.alloc(reinterpret_cast<void**>(&h->sk_ws), tc::sk_workspace_bytes(h->cross_on ? std::max(MB, CROSS_CHUNK) : MB), false));
+  B200_TRY(A.alloc(reinterpret_cast<void**>(&h->sk_ws), tc::sk_workspace_bytes(std::max(MB, h->cross.max_m())), false));
   B200_TRY(A.alloc_t(&h->sk_counters, tc::SK_MAX_TILES));
   const int ns = attn_pick_splits(MB, H, h->kv.cap);
   h->nsplit = ns;
-  h->cross_nsplit = h->cross_on ? attn_pick_splits(MB, H, h->cross_len) : 1;      // the cross step shares the partials
-  B200_TRY(A.alloc_t(&h->attn_part, (size_t)MB * H * (h->cross_on ? std::max(ns, h->cross_nsplit) : ns) * (ATT_D + 2)));
+  B200_TRY(A.alloc_t(&h->attn_part, (size_t)MB * H * std::max(ns, h->cross.nsplit) * (ATT_D + 2)));   // the cross step's too
   B200_TRY(A.alloc_t(&h->attn_counters, (size_t)MB * H));
   B200_TRY(h->open_streams());
   B200_TRY(A.alloc_host(&h->pin_in, (size_t)B * n_in_max));
@@ -1245,13 +1361,7 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
   A.mark_state(h->pos, (size_t)MB * 8, "model.offset", B200_I64, {MB});
   A.mark_state(h->noise_ctr, 8, "noise_counter", B200_I64, {1});
   B200_TRY(h->kv.mark_state(A));
-  for (size_t l = 0; h->cross_on && l < h->layers.size(); ++l) {     // _MHAState.k_cross / v_cross (transformer.py:321-327)
-    auto& L = h->layers[l];
-    const std::string p = "layers." + std::to_string(l);
-    const int T = h->cross_len;
-    A.mark_state(L.kx, (size_t)MB * H * T * D * 2, p + ".k_cross", B200_BF16, {MB, H, T, D});
-    A.mark_state(L.vx, (size_t)MB * H * T * D * 2, p + ".v_cross", B200_BF16, {MB, H, T, D});
-  }
+  h->cross.mark_state(A);
   {
     const int rows_add[2] = {0, B};
     std::vector<RowSlice> s;
@@ -1343,6 +1453,7 @@ int b200_lm_streaming_end(b200_lm* h) {
   h->dep.end();
   h->cfg_until = nullptr; h->noise_ctr = nullptr; h->cond_sum = nullptr; h->cond_on = 0;
   h->kv.end();
+  h->cross.end();
   h->taps = nullptr; h->taps_on = 0;
   h->pin_in = h->pin_out = nullptr;
   h->pin_noise = nullptr;
@@ -1387,10 +1498,7 @@ int b200_lm_set_condition_sum(b200_lm* h, const void* sum_bf16_dev, int rows) {
 int b200_lm_set_cross_attention(b200_lm* h, int enable) {
   if (!h) B200_FAIL(B200_ERR_INVALID, "lm_set_cross_attention: null handle");
   if (h->finalized) B200_FAIL(B200_ERR_STATE, "lm_set_cross_attention: the layers' weights are packed at finalize; set it before");
-  if (enable && h->cfg.quantize)
-    B200_FAIL(B200_ERR_INVALID, "lm_set_cross_attention: cross-attention layers with quantize=True (int8 linears) are not supported");
-  h->cross_on = enable ? 1 : 0;
-  return B200_OK;
+  return h->cross.set(enable, h->cfg);
 }
 
 int b200_lm_set_depformer_schedule(b200_lm* h, const int* schedule, int n) {
@@ -1420,42 +1528,12 @@ int b200_lm_set_depformer_low_rank(b200_lm* h, int rank) {
 
 int b200_lm_set_cross_len(b200_lm* h, int keys) {
   if (!h) B200_FAIL(B200_ERR_INVALID, "lm_set_cross_len: null handle");
-  if (!h->cross_on) B200_FAIL(B200_ERR_INVALID, "lm_set_cross_len: the model has no cross-attention layers");
-  if (h->batch > 0) B200_FAIL(B200_ERR_STATE, "lm_set_cross_len: the condition memory is allocated at streaming_begin; set it before");
-  if (keys < 1 || keys > (1 << 20)) B200_FAIL(B200_ERR_INVALID, "lm_set_cross_len: %d keys", keys);
-  h->cross_len = keys;
-  return B200_OK;
+  return h->cross.set_len(keys, h->batch > 0);
 }
 
 int b200_lm_set_condition_cross(b200_lm* h, const void* src_bf16_dev, const int32_t* rows_host, int n_rows) {
   B200_STREAMING_ENTRY(h, "lm_set_condition_cross");
-  if (!h->cross_on) B200_FAIL(B200_ERR_INVALID, "lm_set_condition_cross: the model has no cross-attention layers");
-  if (!src_bf16_dev || n_rows < 1 || n_rows > h->MB) B200_FAIL(B200_ERR_INVALID, "lm_set_condition_cross: %d condition rows", n_rows);
-  if (!rows_host && n_rows != h->MB)       // lm.py:650-651: "cfg requires 2x more conditions"
-    B200_FAIL(B200_ERR_SHAPE, "lm_set_condition_cross: %d rows given, the model runs on %d", n_rows, h->MB);
-  std::vector<int> rows(n_rows);
-  for (int k = 0; k < n_rows; ++k) {
-    rows[k] = rows_host ? rows_host[k] : k;
-    if (rows[k] < 0 || rows[k] >= h->MB) B200_FAIL(B200_ERR_INVALID, "lm_set_condition_cross: model row %d outside [0, %d)", rows[k], h->MB);
-  }
-  const int d = h->cfg.dim, H = h->cfg.num_heads, T = h->cross_len;
-  B200_CUDA(cudaMemcpyAsync(h->cross_rows, rows.data(), rows.size() * 4, cudaMemcpyHostToDevice, h->stream));
-  B200_TRY(tc::linear_prepare());
-  // transformer.py:495-505 per layer, outside the step: kv = src @ W[d:]^T in chunks of rows, then "b t (p h d) -> p b h t d"
-  // into the rows' memory.  The chunk is staged in a fixed buffer so that the GEMM's activation plan is the same every call.
-  h->body = h->stream;
-  const long long total = (long long)n_rows * T;
-  for (long long i0 = 0; i0 < total; i0 += CROSS_CHUNK) {
-    const int n = (int)std::min<long long>(CROSS_CHUNK, total - i0);
-    B200_CUDA(cudaMemcpyAsync(h->cross_src, static_cast<const bf16*>(src_bf16_dev) + i0 * d, (size_t)n * d * 2, cudaMemcpyDeviceToDevice,
-                              h->stream));
-    for (auto& L : h->layers) {
-      B200_TRY(linear(h, h->cross_src, d, L.ckv_w, h->cross_kv, 2 * d, nullptr, 0, n, 2 * d, d, LIN_STORE, 0));
-      B200_LAUNCH(cross_kv_scatter_kernel, (unsigned)ceil_div64((long long)n * 2 * H * (ATT_D / 8), 256), 256, 0, h->stream, h->cross_kv,
-                  i0, n, h->cross_rows, L.kx, L.vx, H, T);
-    }
-  }
-  return check_launch("lm_set_condition_cross");
+  return h->cross.fill(h, src_bf16_dev, rows_host, n_rows);
 }
 
 int b200_lm_set_taps(b200_lm* h, int enable) {
@@ -1506,8 +1584,8 @@ int b200_lm_session_export(b200_lm* h, int row, void* dst_dev, int64_t capacity)
   if (capacity < p.bytes) B200_FAIL(B200_ERR_SHAPE, "lm_session_export: the record takes %lld bytes, capacity %lld", (long long)p.bytes, (long long)capacity);
   SessionHeader s = h->session_header(p.bytes);
   s.kv_dtype = (uint32_t)h->kv.kind; s.rows = p.rows;
-  s.flags = (p.cond ? SESSION_COND : 0) | (h->cfg_until ? SESSION_CFG_UNTIL : 0) | (h->cross_on ? SESSION_CROSS : 0);
-  if (h->cross_on) memcpy(s.reserved, &h->cross_len, sizeof(int32_t));
+  s.flags = (p.cond ? SESSION_COND : 0) | (h->cfg_until ? SESSION_CFG_UNTIL : 0);
+  h->cross.stamp(&s);
   s.pos[0] = p.pos[0]; s.pos[1] = p.pos[1]; s.n = p.n;
   char* rec = static_cast<char*>(dst_dev);
   B200_CUDA(cudaMemcpyAsync(rec, &s, sizeof(s), cudaMemcpyHostToDevice, h->stream));
@@ -1530,14 +1608,7 @@ int b200_lm_session_import(b200_lm* h, int row, const void* src_dev, int64_t nby
     B200_FAIL(B200_ERR_INVALID, "lm_session_import: classifier-free guidance (or cfg_is_masked_until) on one side only");
   p.cond = (s.flags & SESSION_COND) != 0;
   if (p.cond != (h->cond_on != 0)) B200_FAIL(B200_ERR_INVALID, "lm_session_import: condition_sum on one side only");
-  if (((s.flags & SESSION_CROSS) != 0) != (h->cross_on != 0))
-    B200_FAIL(B200_ERR_INVALID, "lm_session_import: cross-attention conditioning on one side only");
-  if (h->cross_on) {
-    int32_t T = 0;
-    memcpy(&T, s.reserved, sizeof(T));
-    if (T != h->cross_len)
-      B200_FAIL(B200_ERR_INVALID, "lm_session_import: the record's condition memory has %d keys, the handle's %d", T, h->cross_len);
-  }
+  B200_TRY(h->cross.check_record(s, "lm_session_import"));
   p.pos[0] = s.pos[0]; p.pos[1] = p.rows > 1 ? s.pos[1] : 0;
   const int64_t top = std::max(p.pos[0], p.pos[1]);
   if (p.pos[0] < 0 || p.pos[1] < 0 || s.n != std::min<int64_t>(top, c.context))
@@ -1675,7 +1746,7 @@ int b200_lm_read_buffer(b200_lm* h, const char* name, void* dst_dev, int64_t cap
       const bool digits = !idx.empty() && idx.size() <= 4 && idx.find_first_not_of("0123456789") == std::string::npos;
       layer = digits ? atoi(idx.c_str()) : -1;
       kind = k == "attn_out" ? TAP_ATTN_OUT : k == "x_attn" ? TAP_X_ATTN : k == "gated" ? TAP_GATED : k == "x_out" ? TAP_X_OUT : -1;
-      if (h->cross_on && kind < 0) kind = k == "cross_out" ? TAP_CROSS_OUT : k == "x_cross" ? TAP_X_CROSS : -1;
+      if (h->cross.on && kind < 0) kind = k == "cross_out" ? TAP_CROSS_OUT : k == "x_cross" ? TAP_X_CROSS : -1;
       if (layer < 0 || layer >= (int)h->layers.size() || kind < 0)
         B200_FAIL(B200_ERR_INVALID, "lm_read_buffer: unknown buffer '%s'", n.c_str());
     }
@@ -1706,11 +1777,7 @@ int64_t b200_lm_algorithmic_bytes(b200_lm* h, int kv_fill) {
   int64_t per = (int64_t)c.num_layers * 2 * kv_fill * kv_row + (int64_t)c.num_layers * 2 * kv_row;
   per += (int64_t)(c.n_q + 1) * c.dim * 2 + (int64_t)c.dep_q * c.depformer_dim * 2;
   per += (int64_t)2 * (c.text_card + (int64_t)c.dep_q * c.card) * 2;
-  if (h->cross_on) {          // the query, K|V and output linears of every layer; each row reads its condition memory
-    w += (int64_t)c.num_layers * 4 * c.dim * c.dim * 2;
-    per += (int64_t)c.num_layers * 2 * h->cross_len * c.dim * 2;
-  }
-  return w + per * B;
+  return w + per * B + h->cross.algorithmic_bytes(B);
 }
 
 }  // extern "C"
