@@ -6,12 +6,14 @@ the dequantised and up-sampled latents and the PCM are judged against float64, t
 |got - want| <= 2^-20 |want| + c rms with the constants MIMI_C_TC of tests/util.py (the fp32 oracle's constants, widened for
 the 3xTF32 kernels where measured).  The reference uses the kernels' fp32 RoPE frequencies (device_rope_freqs).
 
-The reference runs on selected rows only: row 0, the last row and the rows on each side of every 64-session tile edge (the tile
+The reference runs on selected rows only: row 0, the last row, the rows on each side of every 64-session tile edge (the tile
 of the layers with two steps per session; the 4- and 8-session tiles of the deeper SEANet layers are covered at rows 3 / 4 and
-7 / 8), at most 12 rows per case.  Its host cost is a few hundredths of a second per row and frame for encode and decode
-together; the whole file ran in 32 s on one H100 80GB HBM3 (power limit 700 W), worst ratio 0.91 (encoder taps, B = 129).
+7 / 8) and the first row of the last 4-, 8- and 64-session group.  Its host cost is a few hundredths of a second per row and
+frame for encode and decode together.  On one H100 80GB HBM3 (power limit 700 W) the whole file ran in 149 s, 118 s of it
+the 61 batches of test_every_stage_matches_fp64_at_serving_batch; worst ratio 0.95 (encoder taps, B = 89).
 """
 import ctypes as C
+import time
 
 import pytest
 import torch
@@ -20,8 +22,8 @@ from moshi_b200 import _lib
 from moshi_b200.config import MimiConfig
 from moshi_b200.synth import synth_mimi_state_dict
 from oracle import scenarios
-from tests.util import (MIMI_C_TC, MimiRef64, attn_mask64, device_rope_freqs, cptr, mimi_checkpoints, mimi_kind, mimi_ratios, ring_attention64,
-                        rope64, rvq_unexcused, RVQ_GAP_BOUND)
+from tests.util import (MIMI_C_TC, MimiRef64, attn_mask64, device_rope_freqs, cptr, mimi_checkpoints, mimi_kind, mimi_plan_batches,
+                        mimi_ratios, mimi_tc_chain_factor, ring_attention64, rope64, rvq_unexcused, RVQ_GAP_BOUND)
 
 pytestmark = pytest.mark.gpu
 
@@ -132,8 +134,9 @@ def gpu(sd):
 
 
 def select_rows(B: int, extra: tuple[int, ...] = ()) -> list[int]:
-    """Row 0, the last row, the rows on each side of the 4-, 8- and 64-session tile edges, and ``extra`` (rows a case acts on)."""
-    rows = {0, B - 1} | {r for r in (3, 4, 7, 8) if r < B} | set(extra)
+    """Row 0, the last row, the rows on each side of the 4-, 8- and 64-session tile edges, the first row of the last 4-, 8- and
+    64-session group (it sits in the partial last tile), and ``extra`` (rows a case acts on)."""
+    rows = {0, B - 1} | {r for r in (3, 4, 7, 8) if r < B} | {(B - 1) // g * g for g in (4, 8, 64)} | set(extra)
     for m in range(64, B, 64):
         rows |= {m - 1, m}
     return sorted(rows)
@@ -235,6 +238,10 @@ def run_case(gpu, sd, B: int, frames: int, *, seed: int = 0, ncb: int = 8, wrap_
     v = Verdict(f"B={B} ncb={ncb}" + (" wrap" if wrap_at is not None else "") + (" events" if events else ""))
     g = torch.Generator().manual_seed(seed + 1)
     H, cap = CFG.tr_num_heads, CFG.tr_context
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    consts = dict(MIMI_C_TC)
+    for kind, side in (("enc", "encoder"), ("dec", "decoder")):
+        consts[kind] *= mimi_tc_chain_factor(_lib.lib(), sms, B, side)
     with gpu.streaming(B):
         gpu.set_num_codebooks(ncb)
         for f in range(frames):
@@ -282,7 +289,7 @@ def run_case(gpu, sd, B: int, frames: int, *, seed: int = 0, ncb: int = 8, wrap_
             want.update(ref.decode_frame(dev_codes, dtaps, dec_rings))
             after = _rings(gpu, B, rows)
             for name, got, w, per_head in mimi_checkpoints(want, {**taps, **dtaps}, after, off_before, executing, cap):
-                r = mimi_ratios(got, w, MIMI_C_TC[mimi_kind(name, LAST_DEC)], per_head)
+                r = mimi_ratios(got, w, consts[mimi_kind(name, LAST_DEC)], per_head)
                 v.add(f, rows, name, r, [rows[i] for i in executing.nonzero().flatten()] if per_head else None)
             un = rvq_unexcused(dev_codes, q, RVQ_GAP_BOUND)
             v.add(f, rows, "codes", un.any(dim=1).double() * 2)
@@ -300,8 +307,16 @@ BATCHES = [1, 3, 63, 64, 65, 129, 200, 256]
 
 
 def test_every_stage_matches_fp64_at_serving_batch(gpu, sd):
-    """Encode and decode at each batch, frames 0..2 (frame 0 takes the replicate-padding and zero-carry paths)."""
-    verdicts = [run_case(gpu, sd, B, 3, seed=B) for B in BATCHES]
+    """Encode and decode at each batch of BATCHES, frames 0..2, and at the first and last session count of every run of Mimi's
+    plan on this device (tests/util.py mimi_plan_batches) not among them, frames 0 and 1.  Frame 0 takes the replicate-padding
+    and zero-carry paths, frame 1 the carried ones.  This is where the fused epilogues the op-level tests cannot reach are
+    judged at every plan: GELU, the layer-scaled residual and the consumer's hi / lo split with ELU, in both the kernel's
+    2-wide fragment store and the split-K reduction's 4-wide store."""
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    runs = [(B, 3) for B in BATCHES] + [(B, 2) for B in mimi_plan_batches(_lib.lib(), sms) if B not in BATCHES]
+    t0 = time.time()
+    verdicts = [run_case(gpu, sd, B, frames, seed=B) for B, frames in runs]
+    print(f"{len(runs)} batches in {time.time() - t0:.1f} s")
     fails = [f"{v.case}: {v.first}" for v in verdicts if v.first]
     assert not fails, "\n".join(fails)
 

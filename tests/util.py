@@ -1299,6 +1299,19 @@ MIMI_C = {"enc": 4e-6, "dec": 7e-6, "pcm": 1.1e-6, "enc.tr": 1.7e-6, "dec.tr": 1
 # encoder taps, 4.5 times on the decoder taps, 3.7 times on the transformer outputs and 1.2 times on the PCM; the ring entries,
 # latents and the up-sampling stayed under 0.75 times MIMI_C.  Those four kinds get about twice the measured need; the rest keep the fp32 oracle's constants.
 MIMI_C_TC = {**MIMI_C, "enc": 6e-5, "dec": 6e-5, "enc.tr": 1.2e-5, "dec.tr": 1.2e-5, "pcm": 2.5e-6}
+# Those constants hold while no SEANet layer of the side accumulates more than MIMI_TC_CHAIN k-blocks in one chain (the longest
+# chain up to 256 sessions at 132 SMs: encoder.6's 40).  From 257 sessions the plan stops splitting encoder.9 (96 k-blocks)
+# and decoder.1 (64), whose tensor-core accumulation then errs more (tc_c); on one H100 80GB HBM3 (power limit 700 W) the
+# encoder taps needed 1.69 times MIMI_C_TC there and the decoder taps 1.21 times.  The "enc" / "dec" constants grow in
+# proportion to the side's longest chain beyond MIMI_TC_CHAIN (mimi_tc_chain_factor).
+MIMI_TC_CHAIN = 40
+
+
+def mimi_tc_chain_factor(lib, sms: int, B: int, side: str) -> float:
+    """max(1, longest k-blocks per split of the ``side`` ("encoder" / "decoder") SEANet layers at B sessions / MIMI_TC_CHAIN)."""
+    t = mimi_plan_runs(lib, sms)
+    chain = max(next(f[3] for b0, b1, f in runs if b0 <= B <= b1) for n, runs in t["runs"].items() if n.startswith(side + "."))
+    return max(1.0, chain / MIMI_TC_CHAIN)
 
 # A device code may differ from the fp64 code only where the fp64 gap between the best and the second-best squared distance
 # is at most RVQ_GAP_BOUND (|r|^2 + |c|^2): the fp32 search forms |c|^2 - 2 r.c over 256 products, whose rounding is below
@@ -1564,3 +1577,150 @@ def linear_rows(M: int, K: int, gen: torch.Generator, device: str = "cpu") -> to
             x[m] *= scale
             used.add(m)
     return x.bfloat16()
+
+
+# ---- Mimi's tensor-core layers: the plan runs, and one layer against fp64 ----------------------------------------------------
+def _gen_mimi_plans():
+    import sys
+    from pathlib import Path
+    tools = str(Path(__file__).resolve().parent.parent / "tools")
+    if tools not in sys.path:
+        sys.path.insert(0, tools)
+    import gen_mimi_plans
+    return gen_mimi_plans
+
+
+@functools.lru_cache(maxsize=4)
+def _mimi_plan_runs(lib, sms: int, max_b: int) -> dict:
+    shapes, runs, frame = _gen_mimi_plans().plan_runs(sms, max_b, lib)
+    return {"shapes": shapes, "runs": runs, "frame": frame}
+
+
+def mimi_plan_runs(lib, sms: int, max_b: int = 512) -> dict:
+    """b200_op_mimi_plan at 1..max_b sessions on ``sms`` SMs for the default MimiConfig, compressed as tools/gen_mimi_plans.py
+    writes tests/golden/mimi_plans.json: "shapes" {layer: SHAPE}, "runs" {layer: [[B_first, B_last, FIELDS]]} and "frame"
+    [[B_first, B_last, FRAME]] (the field lists of that tool)."""
+    return _mimi_plan_runs(lib, sms, max_b)
+
+
+def mimi_plan_batches(lib, sms: int, max_b: int = 512) -> list[int]:
+    """The first and last session count of every run of mimi_plan_runs (layers and frame), ascending."""
+    t = mimi_plan_runs(lib, sms, max_b)
+    return sorted({b for runs in [t["frame"], *t["runs"].values()] for r in runs for b in r[:2]})
+
+
+# Acceptance rule of one 3xTF32 layer (mimi_tc_kernel, with or without its split-K reduction): every output within
+# tc_c(chain) * 2^-24 * scale of the fp64 layer, scale = sum_k |a_k w_k| + |bias| over the products that make the output (a
+# the activated input).  TC_C covers, per product, the dropped a_lo * w_lo term and the tf32 rounding of the lo parts (about
+# 3 * 2^-22 together), fp32 accumulation in any order (k-blocks, splits, the split-order reduction), and fp32 expm1f in the
+# ELU, for accumulation chains of up to TC_CHAIN k-blocks.  The tensor cores' fp32 accumulation is not a rounded-to-nearest
+# chain: on one H100 80GB HBM3 (power limit 700 W) a layer's need grew as about 6.3 sqrt(k-blocks per split), from 9 at one
+# k-block to 61 at encoder.9's 96 unsplit k-blocks (257..512 sessions), while an fp32 emulation needs at most 5 at any
+# length.  Longer chains therefore get TC_C sqrt(chain / TC_CHAIN) (tc_c).  tests/test_mimi_plan_runs_cpu.py pins both,
+# shows that fp32 emulations pass in several orders at every plan run of the golden table and that the kernel bugs it lists
+# are rejected in every output row they touch.
+TC_C = 32.0
+TC_CHAIN = 8
+
+
+def tc_c(chain: int) -> float:
+    """The rule's constant for a layer whose k-blocks run in chains of ``chain`` (the plan's kb_per_split)."""
+    return TC_C * max(1.0, (chain / TC_CHAIN) ** 0.5)
+TC_CONV, TC_CONVTR, TC_LINEAR = 0, 1, 2
+
+
+def tc_ref64(kind: int, x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None = None, prev: torch.Tensor | None = None,
+             stride: int = 1, dil: int = 1, elu: bool = False) -> tuple[torch.Tensor, torch.Tensor]:
+    """(want, scale) of one tensor-core layer in float64, on x's device, as b200_op_tc_conv1d / b200_op_tc_linear_f32 state it:
+      conv:    y = conv1d(cat(prev, act(x)), w, bias, stride, dil), x [B, Cin, T], w [Cout, Cin, k], prev [B, Cin, P]
+               (P = (k - 1) dil + 1 - stride; absent: zeros) -> [B, Cout, T / stride];
+      convtr:  StreamingConvTranspose1d with k = 2 stride as two taps over [x[t-1], x[t]], x[-1] = prev [B, Cin, 1]:
+               y[b, co, t S + r] = bias[co] + x[t] . w[:, co, r] + x[t-1] . w[:, co, S + r], w [Cin, Cout, 2 S] -> [B, Cout, T S];
+      linear:  y = x . w^T, x [M, K], w [N, K] -> [M, N].
+    act is ELU with ``elu`` (fp64 here), identity otherwise; the carried context ``prev`` is already activated.  scale is the
+    same layer on |act|, |w| plus |bias|."""
+    f64 = torch.float64
+    if kind == TC_LINEAR:
+        xd, wd = x.to(f64), w.to(x.device, f64)
+        return xd @ wd.T, xd.abs() @ wd.abs().T
+    B, Cin, T = x.shape
+    a = x.to(f64)
+    a = F.elu(a) if elu else a
+    wd = w.to(x.device, f64)
+    bd = torch.zeros(wd.shape[1] if kind == TC_CONVTR else wd.shape[0], dtype=f64, device=x.device) if bias is None \
+        else bias.to(x.device, f64)
+    if kind == TC_CONVTR:
+        S = wd.shape[-1] // 2
+        ctx = torch.zeros(B, Cin, 1, dtype=f64, device=x.device) if prev is None else prev.to(x.device, f64)
+        ext = torch.cat([ctx, a], dim=-1)
+        # taps (x[t-1], x[t]) of phase r: [S, Cout, Cin, 2] -> [S Cout, Cin, 2]
+        taps = torch.stack([wd[:, :, S:], wd[:, :, :S]], dim=-1).permute(2, 1, 0, 3).reshape(S * wd.shape[1], Cin, 2)
+
+        def run(e, k, b):
+            y = F.conv1d(e, k, b.repeat(S))                                  # [B, S Cout, T]: channel r Cout + co
+            return y.view(B, S, -1, T).permute(0, 2, 3, 1).reshape(B, -1, T * S)
+        return run(ext, taps, bd), run(ext.abs(), taps.abs(), bd.abs())
+    k = wd.shape[-1]
+    P = (k - 1) * dil + 1 - stride
+    ctx = torch.zeros(B, Cin, P, dtype=f64, device=x.device) if prev is None else prev.to(x.device, f64)
+    ext = torch.cat([ctx, a], dim=-1)
+    return (F.conv1d(ext, wd, bd, stride=stride, dilation=dil),
+            F.conv1d(ext.abs(), wd.abs(), bd.abs(), stride=stride, dilation=dil))
+
+
+def tc_ratios(got: torch.Tensor, want: torch.Tensor, scale: torch.Tensor, c: float = TC_C) -> torch.Tensor:
+    """|got - want| / (c 2^-24 scale) per output (<= 1 passes).  Where scale is 0 only an exact 0 passes; a NaN never does."""
+    want = want.double()
+    got = got.detach().to(want.device, torch.float64).reshape(want.shape)
+    tol = c * 2.0 ** -24 * scale.double()
+    err = (got - want).abs()
+    r = torch.where(tol > 0, err / tol, torch.where(err == 0, torch.zeros_like(err), torch.full_like(err, math.inf)))
+    return torch.nan_to_num(r, nan=math.inf, posinf=math.inf)
+
+
+def tc_rows(r: torch.Tensor, kind: int, stride: int = 1) -> torch.Tensor:
+    """Per-output values of one layer [B, Cout, T'] (or [M, N]) regrouped by GEMM row: [B, T, outputs of the row] (a
+    transposed conv's GEMM row t holds its output steps t S .. t S + S - 1); a linear's [M, N] becomes [M, 1, N]."""
+    if kind == TC_LINEAR:
+        return r[:, None]
+    B, Co, Tr = r.shape
+    S = stride if kind == TC_CONVTR else 1
+    return r.view(B, Co, Tr // S, S).permute(0, 2, 1, 3).reshape(B, Tr // S, Co * S)
+
+
+def mimi_tc_layers(cfg) -> dict[str, dict]:
+    """The tensor-core layers of b200_op_mimi_plan by name ("encoder.<i>" / "decoder.<i>": position i in the handle's list of
+    SEANet convolutions, a resnet block giving two; "transformer.<linear>"), each with what b200_op_tc_conv1d takes: kind
+    (TC_CONV / TC_CONVTR; the transformer linears as 1-tap convs), cin, cout, k, stride, dil and elu (ELU on the input).
+    Restates the module order of synth.seanet_layout; the first encoder and the last decoder conv (one channel) are not
+    tensor-core layers."""
+    from moshi_b200.synth import seanet_layout
+    out = {}
+    for side, layout in zip(("encoder", "decoder"), seanet_layout(cfg)):
+        convs = []
+        for kind, _, cin, cout, k, stride, dil in layout:
+            if kind == "res":
+                hid = cin // cfg.compress
+                convs += [(TC_CONV, cin, hid, k, 1, dil), (TC_CONV, hid, cout, 1, 1, 1)]
+            else:
+                convs.append((TC_CONVTR if kind == "convtr" else TC_CONV, cin, cout, k, stride, dil))
+        for i, (kind, cin, cout, k, stride, dil) in enumerate(convs):
+            if cin == 1 or cout == 1:
+                continue
+            out[f"{side}.{i}"] = dict(kind=kind, cin=cin, cout=cout, k=k, stride=stride, dil=dil, elu=i > 0)
+    d, ff = cfg.tr_d_model, cfg.tr_dim_feedforward
+    for name, cin, cout in (("in_proj", d, 3 * d), ("out_proj", d, d), ("linear1", d, ff), ("linear2", ff, d)):
+        out[f"transformer.{name}"] = dict(kind=TC_CONV, cin=cin, cout=cout, k=1, stride=1, dil=1, elu=False)
+    return out
+
+
+def tc_op_shape(layer: dict, T_rows: int) -> list[int]:
+    """What b200_op_tc_conv1d plans for ``layer`` (mimi_tc_layers) at T_rows GEMM rows per session, in the order of
+    gen_mimi_plans.SHAPE without the kind: Cin, N, taps, dilation, stride, NT, feature tiles, k-blocks, T.  Its input has
+    T_rows * stride steps (T_rows for a transposed conv)."""
+    tr = layer["kind"] == TC_CONVTR
+    N = layer["stride"] * layer["cout"] if tr else layer["cout"]
+    taps = 2 if tr else layer["k"]
+    NT = min(N, 128)
+    return [layer["cin"], N, taps, 1 if tr else layer["dil"], 1 if tr else layer["stride"], NT, -(-N // NT),
+            taps * (layer["cin"] // 32), T_rows]

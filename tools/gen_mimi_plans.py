@@ -34,13 +34,13 @@ LINEARS = ["in_proj", "out_proj", "linear1", "linear2"]
 
 
 def plan(B: int, sms: int = SMS, num_codebooks: int | None = None, cfg: MimiConfig | None = None,
-         capacity: int = CAPACITY) -> tuple[int, dict, dict[str, dict]]:
-    """(return code, header by HEAD, {layer name: values by LAYER}) of b200_op_mimi_plan."""
+         capacity: int = CAPACITY, lib=None) -> tuple[int, dict, dict[str, dict]]:
+    """(return code, header by HEAD, {layer name: values by LAYER}) of b200_op_mimi_plan (``lib``: the loaded library)."""
     cfg = cfg or MimiConfig()
     buf = (C.c_int64 * capacity)()
     c = _config_struct(cfg)
     ncb = cfg.num_codebooks if num_codebooks is None else num_codebooks
-    rc = _lib.lib().b200_op_mimi_plan(C.byref(c), B, sms, ncb, buf, capacity)
+    rc = (lib or _lib.lib()).b200_op_mimi_plan(C.byref(c), B, sms, ncb, buf, capacity)
     if rc != _lib.B200_OK:
         return rc, {}, {}
     head = dict(zip(HEAD, buf[:len(HEAD)]))
@@ -61,18 +61,24 @@ def add_run(runs: list[list], B: int, value: list[int]) -> None:
         runs.append([B, B, value])
 
 
-def table() -> dict:
+def plan_runs(sms: int = SMS, max_b: int = MAX_B, lib=None) -> tuple[dict[str, list[int]], dict[str, list[list]], list[list]]:
+    """(SHAPE per layer, runs [B_first, B_last, FIELDS] per layer, runs [B_first, B_last, FRAME]) over 1..max_b sessions."""
     shapes: dict[str, list[int]] = {}
     runs: dict[str, list[list]] = {}
     frame: list[list] = []
-    for B in range(1, MAX_B + 1):
-        rc, head, layers = plan(B)
+    for B in range(1, max_b + 1):
+        rc, head, layers = plan(B, sms, lib=lib)
         assert rc == _lib.B200_OK, (B, rc)
         add_run(frame, B, [head[f] for f in FRAME])
         for name, v in layers.items():
             shape = [v[f] for f in SHAPE]
             assert shapes.setdefault(name, shape) == shape, (name, B)
             add_run(runs.setdefault(name, []), B, [v[f] for f in FIELDS])
+    return shapes, runs, frame
+
+
+def table() -> dict:
+    shapes, runs, frame = plan_runs()
     return {"sms": SMS, "max_b": MAX_B, "shape_fields": SHAPE, "fields": FIELDS, "frame_fields": FRAME, "frame": frame,
             "shapes": shapes, "runs": runs}
 
