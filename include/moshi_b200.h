@@ -41,7 +41,7 @@ enum {
   B200_ERR_MISSING = 5    /* finalize: a required tensor was never loaded                  */
 };
 
-enum { B200_F32 = 0, B200_BF16 = 1, B200_F16 = 2, B200_I64 = 3, B200_U8 = 4, B200_I8 = 5 };
+enum { B200_F32 = 0, B200_BF16 = 1, B200_F16 = 2, B200_I64 = 3, B200_U8 = 4, B200_I8 = 5, B200_I32 = 6 };
 
 const char* b200_last_error(void);
 int b200_abi_version(void);
@@ -202,6 +202,31 @@ int b200_lm_destroy(b200_lm* h);
 /* LMGen(...) sampling arguments (lm.py:556-571). */
 int b200_lm_set_sampling(b200_lm* h, int use_sampling, float temp, float temp_text, int top_k,
                          int top_k_text);
+/* Per-session sampling settings (the SessionConfigReq of Kyutai's Rust server).  b200_lm_set_session_sampling(h, history) turns
+ * them on before streaming_begin: history in [1, 1024] is the length of each session's text-history ring, 0 turns them off.
+ * While on, b200_lm_set_row_sampling gives rows rows[0..n) the settings p[0..n) (p NULL: those rows return to the handle-wide
+ * values), ordered on the handle's stream before the next step (and before the next b200_frame_step that drives the handle).
+ * A row that was never given settings follows b200_lm_set_sampling's values at every step, with pad_mult 0, no penalty.
+ * Text token of row b, after the classifier-free-guidance combination: l = float(bf16 logit); each distinct id among the newest
+ * repetition_context tokens of the row's history gets l = l >= 0 ? l / repetition_penalty : l * repetition_penalty; a sampling
+ * row (use_sampling and temp_text > 0) samples softmax(l / temp_text, with pad_mult added to the score of the padding token 3)
+ * over its top_k_text; a greedy row takes the first argmax of the penalised l and ignores pad_mult.  The history holds the
+ * row's sampled text tokens of the steps it executed, without 0, 3 and text_card; b200_lm_reset empties it and keeps the
+ * settings.  The audio tokens use temp and top_k, with no penalty and no pad bias.  Ranges (else B200_ERR_INVALID and nothing
+ * changes): temperatures >= 0 and finite; top_k in [1, handle top_k], top_k_text in [1, handle top_k_text] (the noise row is
+ * laid out by the handle's top-k; a row's top-k is also held to the handle's at every step, so settings that arrive through a
+ * session record or a state snapshot of a handle with larger values sample as if given the handle's); pad_mult finite;
+ * repetition_context in [0, 1024], the window holding at most the `history` tokens the row keeps; repetition_penalty in
+ * (0, 1000].  Int32 state entries (the histories) carry dtype B200_I32. */
+typedef struct {
+  float temp_text, temp;
+  int32_t top_k_text, top_k;
+  float pad_mult;
+  int32_t repetition_context;
+  float repetition_penalty;
+} b200_row_sampling;
+int b200_lm_set_session_sampling(b200_lm* h, int history);
+int b200_lm_set_row_sampling(b200_lm* h, const int32_t* rows, int n, const b200_row_sampling* p);
 /* LMGen(cfg_coef, cfg_is_masked_until, cfg_is_no_text) (lm.py:556-604): classifier-free guidance.  cfg_coef != 1 makes the
  * model run on 2 * batch rows (lm.py:646-647), the second half with the text stream zeroed (cfg_is_no_text) and / or every
  * stream zeroed until a per-session step (masked_until_host i64 [n = batch], NULL = not used) (lm.py:714-726); the logits
@@ -595,6 +620,13 @@ int b200_op_sample(const void* logits_bf16_dev, const float* noise_dev, int64_t*
  * i % 4 of Philox4x32-10 block i / 4 with counter (i / 4 low, high, ctr low, high) and key (seed low, high).  Nothing past n is
  * written.  The counter is staged in a device word shared by all calls: calls must not overlap. */
 int b200_op_lm_noise(float* out_dev, int64_t n, uint64_t seed, uint64_t ctr, void* stream);
+/* The per-session text sampler of the LM step (b200_lm_set_session_sampling) on B rows: logits bf16 [B,card], noise f32 rows of
+ * noise_ld floats, settings p[B] (host, every row with its own settings; NULL: every row follows use_sampling / temp / top_k),
+ * history int32 [B,history] and counts int32 [B] on the device, updated in place as the step updates them (every row executes)
+ * -> i64 [B]. */
+int b200_op_sample_text_rows(const void* logits_bf16_dev, const float* noise_dev, int64_t noise_ld, int64_t* out_dev, int B, int card,
+                             int use_sampling, float temp, int top_k, const b200_row_sampling* p, int32_t* history_dev,
+                             int32_t* count_dev, int history, void* stream);
 /* The step's bits -> Exp(1) transform on given 32-bit words: out[i] = -log(((words[i] >> 8) + 1) * 2^-24), and 2^-24 for the top
  * two 24-bit patterns (u >= 1 - 2^-24, as torch's exponential_ on CUDA); every output is finite and strictly positive. */
 int b200_op_exp1(const uint32_t* words_dev, float* out_dev, int64_t n, void* stream);

@@ -13,7 +13,7 @@ from pathlib import Path
 LIB_PATH = Path(__file__).resolve().parent / "_C" / "libmoshi_b200.so"
 
 B200_OK, B200_ERR_INVALID, B200_ERR_SHAPE, B200_ERR_STATE, B200_ERR_CUDA, B200_ERR_MISSING = range(6)
-B200_F32, B200_BF16, B200_F16, B200_I64, B200_U8, B200_I8 = range(6)
+B200_F32, B200_BF16, B200_F16, B200_I64, B200_U8, B200_I8, B200_I32 = range(7)
 B200_DEPFORMER_AUTO, B200_DEPFORMER_CHAIN, B200_DEPFORMER_FUSED = range(3)     # b200_lm_set_depformer
 ABI_VERSION = 2
 
@@ -30,6 +30,12 @@ class MimiConfigC(C.Structure):
         ("q_dimension", C.c_int), ("q_bins", C.c_int), ("q_n_q", C.c_int), ("q_n_semantic", C.c_int),
         ("num_codebooks", C.c_int),
     ]
+
+
+class RowSamplingC(C.Structure):
+    """``b200_row_sampling``: one session's sampling settings."""
+    _fields_ = [("temp_text", C.c_float), ("temp", C.c_float), ("top_k_text", C.c_int32), ("top_k", C.c_int32),
+                ("pad_mult", C.c_float), ("repetition_context", C.c_int32), ("repetition_penalty", C.c_float)]
 
 
 class LMConfigC(C.Structure):
@@ -85,6 +91,8 @@ _PROTOTYPES: dict[str, tuple[tp.Any, list]] = {
     "b200_lm_finalize": (_I, [_P]),
     "b200_lm_destroy": (_I, [_P]),
     "b200_lm_set_sampling": (_I, [_P, _I, C.c_float, C.c_float, _I, _I]),
+    "b200_lm_set_session_sampling": (_I, [_P, _I]),
+    "b200_lm_set_row_sampling": (_I, [_P, _P, _I, _P]),
     "b200_lm_streaming_begin": (_I, [_P, _I, _P]),
     "b200_lm_streaming_end": (_I, [_P]),
     "b200_lm_reset": (_I, [_P, _P]),
@@ -163,6 +171,7 @@ _PROTOTYPES: dict[str, tuple[tp.Any, list]] = {
     "b200_op_linear_sk_norm": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "b200_op_sample": (_I, [_P, _P, _P, _I, _I, _I, C.c_float, _I, _P]),
     "b200_op_lm_noise": (_I, [_P, C.c_int64, C.c_uint64, C.c_uint64, _P]),
+    "b200_op_sample_text_rows": (_I, [_P, _P, C.c_int64, _P, _I, _I, _I, C.c_float, _I, _P, _P, _P, _I, _P]),
     "b200_op_exp1": (_I, [_P, _P, C.c_int64, _P]),
 }
 
@@ -215,7 +224,8 @@ def dtype_code(t) -> int:
     if _DTYPES is None:
         import torch
         _DTYPES = {torch.float32: B200_F32, torch.bfloat16: B200_BF16, torch.float16: B200_F16,
-                   torch.int64: B200_I64, torch.uint8: B200_U8, torch.bool: B200_U8, torch.int8: B200_I8}
+                   torch.int64: B200_I64, torch.uint8: B200_U8, torch.bool: B200_U8, torch.int8: B200_I8,
+                   torch.int32: B200_I32}
     return _DTYPES[t]
 
 

@@ -83,6 +83,7 @@ inline size_t dtype_size(int dtype) {
     case B200_I64: return 8;
     case B200_U8: return 1;
     case B200_I8: return 1;
+    case B200_I32: return 4;
   }
   return 0;
 }
@@ -179,14 +180,15 @@ struct SessionHeader {
   uint32_t magic, version, kind, kv_dtype;   // kv_dtype: B200_KV_* of an LM record, 0 for Mimi
   uint64_t fingerprint;                      // config_fingerprint of the model configuration
   int32_t rows;                              // model rows per session (LM: 2 under classifier-free guidance, else 1)
-  int32_t flags;                             // LM: SESSION_COND / SESSION_CFG_UNTIL / SESSION_CROSS
+  int32_t flags;                             // LM: SESSION_COND / SESSION_CFG_UNTIL / SESSION_CROSS / SESSION_SAMPLING
   int64_t pos[2];                            // LM: model position of each row
   int64_t n;                                 // LM: temporal KV slots carried, min(pos, ring capacity)
   int64_t bytes;                             // size of the whole record
-  uint8_t reserved[256 - 64];                // LM with SESSION_CROSS: int32 keys of the condition memory first
+  uint8_t reserved[256 - 64];                // LM: int32 keys of the condition memory (SESSION_CROSS), then int32
+                                             // history length (SESSION_SAMPLING)
 };
 static_assert(sizeof(SessionHeader) == 256, "session header is 256 bytes");
-enum { SESSION_COND = 1, SESSION_CFG_UNTIL = 2, SESSION_CROSS = 4 };
+enum { SESSION_COND = 1, SESSION_CFG_UNTIL = 2, SESSION_CROSS = 4, SESSION_SAMPLING = 8 };
 
 // FNV-1a over a configuration struct: records only go into handles built from the same configuration
 inline uint64_t config_fingerprint(const void* p, size_t n) {

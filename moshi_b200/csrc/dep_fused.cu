@@ -205,8 +205,11 @@ __device__ void sample_phase(const DepParams& p, int S, int k) {
       lg[j] = f2bf(a);
     }
     __syncthreads();
+    float temp = p.temp;
+    int top_k = p.top_k;
+    lm::row_sampling(p.rows, m, false, &temp, &top_k);
     lm::sample_row(lg, p.noise + (long long)m * p.noise_ld + p.noise_off + (long long)k * p.ka, p.audio_tokens + (long long)k * p.B + m,
-                   p.card, p.use_sampling, p.temp, p.top_k);
+                   p.card, p.use_sampling, temp, top_k);
     __syncthreads();
   }
 }

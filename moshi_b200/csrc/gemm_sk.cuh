@@ -12,6 +12,7 @@
 #include "tc_host.cuh"
 
 namespace b200 {
+namespace lm { struct RowSampling; }
 namespace tc {
 
 struct MapKey {
@@ -147,6 +148,7 @@ struct DepParams {
   long long* audio_tokens;                                   // [dep_q][B]
   const float* noise; long long noise_ld; int noise_off, ka; // Exp(1) noise, row stride, offset of sub-step 0, per-step width
   int use_sampling, top_k; float temp;
+  const lm::RowSampling* rows;                               // [B] per-session settings (their temp / top_k), or null
   unsigned* bar;                                             // grid barrier counter (zero at launch)
   unsigned long long* trace;                                 // optional [DEP_TRACE_SLOTS]: %globaltimer of CTA 0 after every grid barrier
 };

@@ -568,6 +568,97 @@ struct CrossAttention {
 
 }  // namespace
 
+// ---- per-session sampling ----------------------------------------------------------------------------------------------------
+// Each session's own temperatures, top-k, pad bias and text repetition penalty (b200_lm_set_session_sampling / _row_sampling).
+// Only this unit knows whether it is on, the history length N, the device settings and history, the text path of the step
+// (text_adjust_kernel, then the fp32-score sampler that appends to the history), the clear on reset, the state entries and the
+// record section; the rest of the handle asks it whether it is on and for the per-row settings the audio samplers read.
+namespace {
+
+struct SessionSampling {
+  int N = 0;                                   // history ring length; 0 = off (before streaming_begin)
+  int B = 0, card = 0;
+  RowSampling* params = nullptr;               // [B] (own = 0: the row follows the handle-wide values)
+  int *ring = nullptr, *count = nullptr;       // [B][N], [B]
+  float* scores = nullptr;                     // [B][text_card] the adjusted text scores of the step
+
+  bool on() const { return N > 0; }
+  int set(int history, bool streaming) {
+    if (streaming) B200_FAIL(B200_ERR_STATE, "lm_set_session_sampling: the settings and histories are allocated at streaming_begin; set it before");
+    if (history < 0 || history > 1024) B200_FAIL(B200_ERR_INVALID, "lm_set_session_sampling: history %d outside [0, 1024]", history);
+    N = history;
+    return B200_OK;
+  }
+  int alloc(Arena& A, int batch, int text_card) {
+    if (!on()) return B200_OK;
+    B = batch; card = text_card;
+    B200_TRY(A.alloc_t(&params, B));
+    B200_TRY(A.alloc_t(&ring, (size_t)B * N));
+    B200_TRY(A.alloc_t(&count, B));
+    return A.alloc_t(&scores, (size_t)B * card, false);
+  }
+  // the state entries session_sampling.params [B][8] (RowSampling's fields), .history [B][N], .count [B]
+  void mark_state(Arena& A) const {
+    if (!on()) return;
+    A.mark_state(params, (size_t)B * sizeof(RowSampling), "session_sampling.params", B200_F32, {B, 8});
+    A.mark_state(ring, (size_t)B * N * 4, "session_sampling.history", B200_I32, {B, N});
+    A.mark_state(count, (size_t)B * 4, "session_sampling.count", B200_I32, {B});
+  }
+  void end() { B = card = 0; params = nullptr; ring = count = nullptr; scores = nullptr; }
+
+  const RowSampling* rows() const { return on() ? params : nullptr; }
+  TextHistory history() const { return TextHistory{ring, count, N}; }
+  // b200_lm_set_row_sampling: every row and setting checked before anything is written
+  int set_rows(const int32_t* rows, int n, const b200_row_sampling* p, int top_k, int top_k_text, cudaStream_t st) const {
+    const char* what = "lm_set_row_sampling";
+    if (!on()) B200_FAIL(B200_ERR_STATE, "%s: per-session sampling is off (b200_lm_set_session_sampling before streaming_begin)", what);
+    if (n < 0 || (n > 0 && !rows)) B200_FAIL(B200_ERR_INVALID, "%s: %d rows", what, n);
+    std::vector<RowSampling> v(n, RowSampling{});
+    for (int k = 0; k < n; ++k) {
+      if (rows[k] < 0 || rows[k] >= B) B200_FAIL(B200_ERR_INVALID, "%s: row %d outside [0, %d)", what, rows[k], B);
+      if (p) B200_TRY(row_sampling_check(p[k], top_k, top_k_text, &v[k], what));
+    }
+    for (int k = 0; k < n; ++k)
+      B200_CUDA(cudaMemcpyAsync(params + rows[k], &v[k], sizeof(RowSampling), cudaMemcpyHostToDevice, st));
+    return B200_OK;
+  }
+  // b200_lm_reset: the masked rows' histories (null: all)
+  void clear(const uint8_t* mask, cudaStream_t st) const {
+    if (on()) B200_LAUNCH(text_history_clear_kernel, ceil_div(B, 128), 128, 0, st, count, mask, B);
+  }
+
+  // The session-record section: from the first 256-byte boundary at or after `end` (*off), the row's settings (32 bytes), its
+  // count (4 bytes, then 12 of padding) and its history ring (N int32).  Returns the record's end (`end` when off).
+  int64_t record_section(int64_t end, int64_t* off) const {
+    *off = (end + 255) / 256 * 256;
+    return on() ? *off + 48 + (int64_t)N * 4 : end;
+  }
+  int record(int row, char* at, bool gather, cudaStream_t st) const {
+    if (!on()) return B200_OK;
+    const struct { void* dev; char* rec; size_t n; } part[3] = {{params + row, at, sizeof(RowSampling)}, {count + row, at + 32, 4},
+                                                              {ring + (size_t)row * N, at + 48, (size_t)N * 4}};
+    for (const auto& x : part)
+      B200_CUDA(cudaMemcpyAsync(gather ? x.rec : x.dev, gather ? x.dev : x.rec, x.n, cudaMemcpyDeviceToDevice, st));
+    return B200_OK;
+  }
+  // export: SESSION_SAMPLING, and N in the header's reserved bytes after the condition memory's keys
+  void stamp(SessionHeader* s) const {
+    if (!on()) return;
+    s->flags |= SESSION_SAMPLING;
+    memcpy(s->reserved + 4, &N, sizeof(int32_t));
+  }
+  // import: a record whose flag or N differs from the handle's is refused
+  int check_record(const SessionHeader& s, const char* what) const {
+    if (((s.flags & SESSION_SAMPLING) != 0) != on()) B200_FAIL(B200_ERR_INVALID, "%s: per-session sampling on one side only", what);
+    int32_t n = 0;
+    memcpy(&n, s.reserved + 4, sizeof(n));
+    if (on() && n != N) B200_FAIL(B200_ERR_INVALID, "%s: the record's text history holds %d tokens, the handle's %d", what, n, N);
+    return B200_OK;
+  }
+};
+
+}  // namespace
+
 struct b200_lm : StreamCore {       // batch: sessions (LMGen batch); graphs[0]: the step
   b200_lm_config cfg;
   TensorStore store;
@@ -611,6 +702,7 @@ struct b200_lm : StreamCore {       // batch: sessions (LMGen batch); graphs[0]:
   Depformer dep;                               // the depformer: weights, buffers and the path it runs on
   TemporalKv kv;                               // the temporal K/V: rings or pool, their state entries and record section
   CrossAttention cross;                        // cross-attention conditioning: weights, condition memory, fill and record section
+  SessionSampling ss;                          // per-session sampling settings, text histories and their record section
   // session records: the per-session slices of the small state entries; the condition_sum rows come last and travel while it is on
   RowSlice* slices_dev = nullptr;
   int n_slices = 0, n_slices_cond = 0;
@@ -767,10 +859,20 @@ const bf16* guide(b200_lm* h, const bf16* logits, bf16* guided, int card, bool c
   return guided;
 }
 
-int sample(b200_lm* h, const bf16* logits, int card, const float* noise, long long* out, float temp, int top_k) {
+// text: the text sampler (the rows' own temp_text / top_k_text where they have them), else an audio sub-step's (temp / top_k)
+int sample(b200_lm* h, const bf16* logits, int card, const float* noise, long long* out, float temp, int top_k, bool text) {
   B200_LAUNCH(sample_kernel, h->batch, SAMPLE_THREADS, 0, h->body, logits, (long long)card, noise,
-              (long long)noise_per_row(h), out, card, h->use_sampling, temp, top_k);
+              (long long)noise_per_row(h), out, card, h->use_sampling, temp, top_k, h->ss.rows(), text ? 1 : 0);
   return check_launch("sample");
+}
+
+// The step's text token from the sampler's logits [batch][text_card]: a session-sampling handle adjusts them per row and appends
+// the tokens to the rows' histories
+int sample_text(b200_lm* h, const bf16* logits) {
+  if (!h->ss.on()) return sample(h, logits, h->cfg.text_card, h->noise, h->text_token, h->temp_text, h->top_k_text, true);
+  text_rows_launch(logits, h->ss.scores, h->noise, noise_per_row(h), h->text_token, h->batch, h->cfg.text_card, h->use_sampling,
+                   h->temp_text, h->top_k_text, h->ss.params, h->ss.history(), h->exec_mask, h->body);
+  return check_launch("sample_text");
 }
 
 TokenRing ring(b200_lm* h) {
@@ -887,6 +989,7 @@ int Depformer::alloc_fused(b200_lm* h) {
   p.logits = logits; p.audio_tokens = h->audio_tokens;
   p.noise = h->noise; p.noise_ld = noise_at(dep_q); p.noise_off = (int)noise_at(0); p.ka = ka;
   p.use_sampling = h->use_sampling; p.top_k = h->top_k; p.temp = h->temp;
+  p.rows = h->ss.rows();
   p.bar = bar; p.trace = trace;
   return tc::dep_fused_create(plan, p, &fused);
 }
@@ -918,7 +1021,7 @@ int Depformer::run(b200_lm* h, bool replace) {
     bf16* lg = logits + (long long)k * MB * card;
     B200_TRY(linear(h, dx, dd, heads[k], lg, card, nullptr, 0, MB, card, dd, LIN_STORE, 0, heads_s[k]));
     const bf16* gl = guide(h, lg, cfg_on(h) ? logits_cfg + (long long)k * B * card : nullptr, card, true);   // lm.py:828-833
-    B200_TRY(sample(h, gl, card, h->noise + noise_at(k), h->audio_tokens + (long long)k * B, h->temp, h->top_k));
+    B200_TRY(sample(h, gl, card, h->noise + noise_at(k), h->audio_tokens + (long long)k * B, h->temp, h->top_k, false));
   }
   return B200_OK;
 }
@@ -1030,7 +1133,7 @@ int step_body(b200_lm* h) {
   B200_TRY(linear(h, h->tout, d, h->text_linear, h->text_logits, c.text_card, nullptr, 0, MB, c.text_card, d, LIN_STORE, 0, h->text_linear_s));
   // lm.py:728-732: with cfg_is_no_text the text logits are the conditioned rows, otherwise the guided combination
   const bf16* tl = guide(h, h->text_logits, h->text_logits_cfg, c.text_card, !h->cfg_is_no_text);
-  B200_TRY(sample(h, tl, c.text_card, h->noise, h->text_token, h->temp_text, h->top_k_text));
+  B200_TRY(sample_text(h, tl));
   if (!h->extra_w.empty())
     B200_LAUNCH(extra_heads_kernel, ceil_div((int)h->extra_w.size() * MB * 32, 128), 128, 0, st, h->tout, h->extra_w_dev, h->extra_out, MB, d,
                 c.extra_heads_dim, (int)h->extra_w.size());
@@ -1045,19 +1148,21 @@ int step_body(b200_lm* h) {
 // After the 256-byte SessionHeader: the session's slices of exec_mask, cache, offsets, model.offset (1 or 2 rows), under CFG
 // model.exec_mask (2 rows) and cfg_is_masked_until, and while it is on the condition_sum rows, each 16-byte aligned (the
 // RowSlice table of streaming_begin).  From the next 256-byte boundary, the temporal K/V of slots [0, n), n = min(pos, ring
-// capacity), slot s being position s mod capacity (TemporalKv::record).  A cross-attention handle's record ends with the session's
-// condition memory (CrossAttention::record_section).
+// capacity), slot s being position s mod capacity (TemporalKv::record).  A cross-attention handle's record continues with the
+// session's condition memory (CrossAttention::record_section), a session-sampling handle's ends with the session's settings and
+// text history (SessionSampling::record_section).
 struct SessionPlan {
   int rows = 1;
   int64_t pos[2] = {0, 0};
-  int64_t n = 0, kv_off = 0, cross_off = 0, bytes = 0;
+  int64_t n = 0, kv_off = 0, cross_off = 0, ss_off = 0, bytes = 0;
   bool cond = false;
 };
 
 void session_size(const b200_lm* h, SessionPlan* p) {
   const long long end = p->cond ? h->slices_end_cond : h->slices_end;
   p->kv_off = (end + 255) / 256 * 256;
-  p->bytes = h->cross.record_section(p->kv_off + h->kv.record_bytes(p->rows, p->n), p->rows, &p->cross_off);
+  p->bytes = h->ss.record_section(h->cross.record_section(p->kv_off + h->kv.record_bytes(p->rows, p->n), p->rows, &p->cross_off),
+                                  &p->ss_off);
 }
 
 // The record row `row` would export now (synchronises): B200_ERR_STATE for a short-ring row whose ring has already wrapped.
@@ -1078,7 +1183,8 @@ int session_plan(b200_lm* h, int row, const char* what, SessionPlan* p) {
 // The session's temporal K/V and condition memory between the device and the record
 int session_kv(b200_lm* h, int row, const SessionPlan& p, char* rec, bool gather) {
   B200_TRY(h->kv.record(row, p.rows, h->batch, (int)p.n, rec + p.kv_off, gather, h->stream));
-  return h->cross.record(row, p.rows, h->batch, rec + p.cross_off, gather, h->stream);
+  B200_TRY(h->cross.record(row, p.rows, h->batch, rec + p.cross_off, gather, h->stream));
+  return h->ss.record(row, rec + p.ss_off, gather, h->stream);
 }
 
 }  // namespace
@@ -1217,6 +1323,16 @@ int b200_lm_set_sampling(b200_lm* h, int use_sampling, float temp, float temp_te
 
 int b200_lm_noise_per_row(b200_lm* h) { return h ? noise_per_row(h) : 0; }
 
+int b200_lm_set_session_sampling(b200_lm* h, int history) {
+  if (!h) B200_FAIL(B200_ERR_INVALID, "lm_set_session_sampling: null handle");
+  return h->ss.set(history, h->batch > 0);
+}
+
+int b200_lm_set_row_sampling(b200_lm* h, const int32_t* rows, int n, const b200_row_sampling* p) {
+  B200_STREAMING_ENTRY(h, "lm_set_row_sampling");
+  return h->ss.set_rows(rows, n, p, h->top_k, h->top_k_text, h->stream);
+}
+
 int b200_lm_set_graph(b200_lm* h, int enable) {
   if (!h) B200_FAIL(B200_ERR_INVALID, "lm_set_graph: null handle");
   h->set_graph(enable);
@@ -1316,6 +1432,7 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
   B200_TRY(A.alloc_t(&h->audio_tokens, (size_t)B * dq1));
   B200_TRY(A.alloc_t(&h->replace_tokens, (size_t)B * dq1));
   B200_TRY(A.alloc_t(&h->out_tokens, (size_t)B * (c.dep_q + 1)));
+  B200_TRY(h->ss.alloc(A, B, c.text_card));
   B200_TRY(A.alloc_t(&h->noise, (size_t)B * noise_per_row(h), false));
   {
     std::vector<float> ones((size_t)B * noise_per_row(h), 1.f);
@@ -1362,6 +1479,7 @@ int b200_lm_streaming_begin(b200_lm* h, int batch, void* stream) {
   A.mark_state(h->noise_ctr, 8, "noise_counter", B200_I64, {1});
   B200_TRY(h->kv.mark_state(A));
   h->cross.mark_state(A);
+  h->ss.mark_state(A);
   {
     const int rows_add[2] = {0, B};
     std::vector<RowSlice> s;
@@ -1454,6 +1572,7 @@ int b200_lm_streaming_end(b200_lm* h) {
   h->cfg_until = nullptr; h->noise_ctr = nullptr; h->cond_sum = nullptr; h->cond_on = 0;
   h->kv.end();
   h->cross.end();
+  h->ss.end();
   h->taps = nullptr; h->taps_on = 0;
   h->pin_in = h->pin_out = nullptr;
   h->pin_noise = nullptr;
@@ -1468,6 +1587,7 @@ int b200_lm_reset(b200_lm* h, const uint8_t* reset_mask_dev) {
   // per-row device offsets (lm.py:539, transformer.py:229-234, 331-333) ...
   B200_LAUNCH(lm_reset_kernel, ceil_div(B, 128), 128, 0, h->stream, h->offsets, h->pos, h->exec_mask, h->exec_mask_m,
               reset_mask_dev, B, cfg_on(h) ? 1 : 0);
+  h->ss.clear(reset_mask_dev, h->stream);       // the rows' text histories; their settings stay
   // ... and the global host counter (lm.py:540): after any reset, step() reports "not ready" for max_delay calls
   h->offset_cpu = 0;
   return check_launch("lm_reset");
@@ -1586,6 +1706,7 @@ int b200_lm_session_export(b200_lm* h, int row, void* dst_dev, int64_t capacity)
   s.kv_dtype = (uint32_t)h->kv.kind; s.rows = p.rows;
   s.flags = (p.cond ? SESSION_COND : 0) | (h->cfg_until ? SESSION_CFG_UNTIL : 0);
   h->cross.stamp(&s);
+  h->ss.stamp(&s);
   s.pos[0] = p.pos[0]; s.pos[1] = p.pos[1]; s.n = p.n;
   char* rec = static_cast<char*>(dst_dev);
   B200_CUDA(cudaMemcpyAsync(rec, &s, sizeof(s), cudaMemcpyHostToDevice, h->stream));
@@ -1609,6 +1730,7 @@ int b200_lm_session_import(b200_lm* h, int row, const void* src_dev, int64_t nby
   p.cond = (s.flags & SESSION_COND) != 0;
   if (p.cond != (h->cond_on != 0)) B200_FAIL(B200_ERR_INVALID, "lm_session_import: condition_sum on one side only");
   B200_TRY(h->cross.check_record(s, "lm_session_import"));
+  B200_TRY(h->ss.check_record(s, "lm_session_import"));
   p.pos[0] = s.pos[0]; p.pos[1] = p.rows > 1 ? s.pos[1] : 0;
   const int64_t top = std::max(p.pos[0], p.pos[1]);
   if (p.pos[0] < 0 || p.pos[1] < 0 || s.n != std::min<int64_t>(top, c.context))

@@ -5,6 +5,8 @@
 // residual adds and the 17-way embedding sum are bf16 adds.
 #pragma once
 
+#include <cmath>
+
 #include <cuda_fp16.h>
 #include <cuda_fp8.h>
 
@@ -1093,6 +1095,44 @@ __device__ __forceinline__ unsigned sample_key(const bf16* logits, int i) {
   return ((unsigned)mono << 16) | (unsigned)(0xFFFFu - (unsigned)i);
 }
 
+// Per-session sampling settings of one row (b200_lm_set_row_sampling), all fp32 so that the row is one state entry row.
+// own = 0: the row follows the handle-wide temperatures and top-k, with no pad bias and no repetition penalty.
+struct RowSampling { float temp_text, temp, top_k_text, top_k, pad_mult, context, penalty, own; };
+constexpr int TEXT_PAD_ID = 3;               // existing_text_padding_id: the token pad_mult biases, skipped by the history
+
+// the temperature and top-k row b samples with: its own where it has them, else the handle's (*temp, *top_k on entry).  The own
+// top-k is clamped to [1, the handle's] here, at every step, and not only where the settings are set: settings that arrive
+// through a session record or a state snapshot of a handle with a larger top-k must still draw within the row's noise block.
+__device__ __forceinline__ void row_sampling(const RowSampling* rs, int b, bool text, float* temp, int* top_k) {
+  if (rs != nullptr && rs[b].own != 0.f) {
+    const float k = text ? rs[b].top_k_text : rs[b].top_k;
+    *temp = text ? rs[b].temp_text : rs[b].temp;
+    *top_k = k >= 1.f ? (int)fminf(k, (float)*top_k) : 1;
+  }
+}
+
+// Where the sampler's scores come from.  bf16 logits: the score is logit / temp, the key (monotone bf16 bits, 0xFFFF - index)
+// in 32 bits, four radix passes.  fp32 scores (text_adjust_kernel: penalised logits, already / temp with the pad bias on
+// sampling rows): the score as it is, the key (monotone fp32 bits, 0xFFFF - index) in the low 48 bits of a 64-bit word, six
+// passes.  On an unadjusted row the fp32 scores are the bf16 path's logit / temp, so both pick the same token.
+template <typename T> struct SampleSrc;
+template <> struct SampleSrc<bf16> {
+  typedef unsigned Key;
+  static constexpr int PASSES = 4;
+  static __device__ __forceinline__ float score(const bf16* p, int i, float temp) { return bf2f(p[i]) / temp; }
+  static __device__ __forceinline__ Key key(const bf16* p, int i) { return sample_key(p, i); }
+};
+template <> struct SampleSrc<float> {
+  typedef unsigned long long Key;
+  static constexpr int PASSES = 6;
+  static __device__ __forceinline__ float score(const float* p, int i, float) { return p[i]; }
+  static __device__ __forceinline__ Key key(const float* p, int i) {
+    const unsigned raw = __float_as_uint(p[i]);
+    const unsigned mono = (raw & 0x80000000u) ? ~raw : (raw | 0x80000000u);
+    return ((Key)mono << 16) | (Key)(0xFFFFu - (unsigned)i);
+  }
+};
+
 static __device__ float block_reduce(float v, bool is_max, float* red) {
   v = is_max ? warp_max(v) : warp_sum(v);
   __syncthreads();
@@ -1103,50 +1143,55 @@ static __device__ float block_reduce(float v, bool is_max, float* red) {
   return t;
 }
 
-// One row per call; every thread of a SAMPLE_THREADS-wide CTA must call it (block-wide barriers inside).
-static __device__ void sample_row(const bf16* __restrict__ logits, const float* __restrict__ noise, long long* __restrict__ out,
+// One row per call; every thread of a SAMPLE_THREADS-wide CTA must call it (block-wide barriers inside).  T: bf16 logits or
+// fp32 scores (SampleSrc).  Thread 0 writes *out.
+template <typename T>
+static __device__ void sample_row(const T* __restrict__ logits, const float* __restrict__ noise, long long* __restrict__ out,
                                   int card, int use_sampling, float temp, int top_k) {
+  typedef SampleSrc<T> S;
+  typedef typename S::Key Key;
   __shared__ float red[SAMPLE_THREADS / 32];
   __shared__ unsigned hist[256];
-  __shared__ unsigned s_prefix, s_remaining, s_count;
-  __shared__ unsigned sel[SAMPLE_MAX_K];
+  __shared__ Key s_prefix;
+  __shared__ unsigned s_remaining, s_count;
+  __shared__ Key sel[SAMPLE_MAX_K];
   __shared__ float s_best[SAMPLE_THREADS / 32];
   __shared__ int s_brank[SAMPLE_THREADS / 32];
   const int tid = threadIdx.x;
 
   if (!(use_sampling && temp > 0.f)) {        // greedy: argmax, first maximum (sampling.py:102-103)
-    unsigned best = 0;
-    for (int i = tid; i < card; i += SAMPLE_THREADS) best = max(best, sample_key(logits, i));
+    Key best = 0;
+    for (int i = tid; i < card; i += SAMPLE_THREADS) best = max(best, S::key(logits, i));
     for (int o = 16; o > 0; o >>= 1) best = max(best, __shfl_xor_sync(0xffffffffu, best, o));
-    if ((tid & 31) == 0) hist[tid >> 5] = best;
+    if ((tid & 31) == 0) sel[tid >> 5] = best;
     __syncthreads();
     if (tid == 0) {
-      unsigned bb = 0;
-      for (int w = 0; w < SAMPLE_THREADS / 32; ++w) bb = max(bb, hist[w]);
-      *out = 0xFFFFu - (bb & 0xFFFFu);
+      Key bb = 0;
+      for (int w = 0; w < SAMPLE_THREADS / 32; ++w) bb = max(bb, sel[w]);
+      *out = 0xFFFFu - (unsigned)(bb & 0xFFFFu);
     }
     return;
   }
   const int k = min(min(top_k, card), SAMPLE_MAX_K);
-  // softmax statistics in fp32 on logits / temp
+  // softmax statistics in fp32 on the scores (logits / temp)
   float mx = -INFINITY;
-  for (int i = tid; i < card; i += SAMPLE_THREADS) mx = fmaxf(mx, bf2f(logits[i]) / temp);
+  for (int i = tid; i < card; i += SAMPLE_THREADS) mx = fmaxf(mx, S::score(logits, i, temp));
   mx = block_reduce(mx, true, red);
   float sum = 0.f;
-  for (int i = tid; i < card; i += SAMPLE_THREADS) sum += expf(bf2f(logits[i]) / temp - mx);
+  for (int i = tid; i < card; i += SAMPLE_THREADS) sum += expf(S::score(logits, i, temp) - mx);
   sum = block_reduce(sum, false, red);
 
-  // radix select of the k-th largest 32-bit key (keys are unique)
+  // radix select of the k-th largest key (keys are unique)
   if (tid == 0) { s_prefix = 0; s_remaining = (unsigned)k; }
   __syncthreads();
-  for (int pass = 3; pass >= 0; --pass) {
+  for (int pass = S::PASSES - 1; pass >= 0; --pass) {
     hist[tid] = 0;
     __syncthreads();
-    const unsigned prefix = s_prefix;
-    const unsigned mask = pass == 3 ? 0u : (0xFFFFFFFFu << ((pass + 1) * 8));
+    const Key prefix = s_prefix;
+    const Key mask = pass == S::PASSES - 1 ? (Key)0 : (~(Key)0 << ((pass + 1) * 8));
     for (int i = tid; i < card; i += SAMPLE_THREADS) {
-      const unsigned key = sample_key(logits, i);
-      if ((key & mask) == prefix) atomicAdd(&hist[(key >> (pass * 8)) & 0xFFu], 1u);
+      const Key key = S::key(logits, i);
+      if ((key & mask) == prefix) atomicAdd(&hist[(unsigned)(key >> (pass * 8)) & 0xFFu], 1u);
     }
     __syncthreads();
     if (tid < 32) {
@@ -1171,20 +1216,20 @@ static __device__ void sample_row(const bf16* __restrict__ logits, const float* 
           cum += h8[i];
         }
         s_remaining = rem - cum;
-        s_prefix = prefix | ((unsigned)bin << (pass * 8));
+        s_prefix = prefix | ((Key)bin << (pass * 8));
       }
     }
     __syncthreads();
   }
-  const unsigned thr = s_prefix;               // exactly k keys are >= thr
+  const Key thr = s_prefix;                    // exactly k keys are >= thr
   if (tid == 0) s_count = 0;
   // pad the sort buffer
   int p2 = 1;
   while (p2 < k) p2 <<= 1;
-  for (int i = tid; i < p2; i += SAMPLE_THREADS) sel[i] = 0u;
+  for (int i = tid; i < p2; i += SAMPLE_THREADS) sel[i] = 0;
   __syncthreads();
   for (int i = tid; i < card; i += SAMPLE_THREADS) {
-    const unsigned key = sample_key(logits, i);
+    const Key key = S::key(logits, i);
     if (key >= thr) {
       const unsigned slot = atomicAdd(&s_count, 1u);
       if (slot < (unsigned)p2) sel[slot] = key;
@@ -1198,7 +1243,7 @@ static __device__ void sample_row(const bf16* __restrict__ logits, const float* 
         const int lo = 2 * i - (i & (stride - 1));
         const int hi = lo + stride;
         const bool desc = ((lo & size) == 0);
-        const unsigned a = sel[lo], b = sel[hi];
+        const Key a = sel[lo], b = sel[hi];
         if ((a < b) == desc) { sel[lo] = b; sel[hi] = a; }
       }
       __syncthreads();
@@ -1209,7 +1254,7 @@ static __device__ void sample_row(const bf16* __restrict__ logits, const float* 
   int brank = 0x7fffffff;
   for (int j = tid; j < k; j += SAMPLE_THREADS) {
     const int idx = 0xFFFF - (int)(sel[j] & 0xFFFFu);
-    const float p = expf(bf2f(logits[idx]) / temp - mx) / sum;
+    const float p = expf(S::score(logits, idx, temp) - mx) / sum;
     const float s = p / noise[j];
     if (s > best || (s == best && j < brank)) { best = s; brank = j; }
   }
@@ -1228,13 +1273,129 @@ static __device__ void sample_row(const bf16* __restrict__ logits, const float* 
   }
 }
 
+// rs: per-row settings (null, or rows without their own: temp / top_k); text: rs's text or audio fields
 static __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(const bf16* __restrict__ logits_all, long long ld,
                                                                 const float* __restrict__ noise, long long noise_ld,
                                                                 long long* __restrict__ out, int card, int use_sampling,
-                                                                float temp, int top_k) {
+                                                                float temp, int top_k, const RowSampling* rs, int text) {
   pdl_trigger();
   const int row = blockIdx.x;
+  row_sampling(rs, row, text != 0, &temp, &top_k);
   sample_row(logits_all + (long long)row * ld, noise + (long long)row * noise_ld, out + row, card, use_sampling, temp, top_k);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Per-session text sampling (lm_generate_multistream.rs:142-175, 247-255): repetition penalty over the row's recent text,
+// temperature and pad bias, into fp32 scores; then the shared sampler on them, and the row's history ring.
+// ---------------------------------------------------------------------------------------------
+struct TextHistory {
+  int* ring;                 // [B][N] the row's generated text tokens, the special ids left out; slot count % N is the next
+  int* count;                // [B] tokens appended since the last reset
+  int N;
+};
+
+__device__ __forceinline__ bool text_special(int t, int text_card) { return t == 0 || t == TEXT_PAD_ID || t == text_card; }
+
+// One CTA per row.  The penalty window: the newest `context` entries of the ring that are not special ids, each distinct id
+// penalised once (a bitmap of card bits in shared memory, 8 KB at 65 535 ids).  Greedy rows get the penalised logits.
+static __global__ void __launch_bounds__(SAMPLE_THREADS) text_adjust_kernel(const bf16* __restrict__ logits, float* __restrict__ scores,
+                                                                     int card, int use_sampling, float temp,
+                                                                     const RowSampling* __restrict__ rs, TextHistory th) {
+  __shared__ unsigned bits[2048];
+  __shared__ int s_warp[SAMPLE_THREADS / 32];
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const RowSampling r = rs[b];
+  float pen = 1.f, pad = 0.f;
+  int ctx = 0;
+  if (r.own != 0.f) { temp = r.temp_text; pen = r.penalty; pad = r.pad_mult; ctx = (int)r.context; }
+  const bool sampling = use_sampling && temp > 0.f;
+  const int cnt = th.count[b];
+  const int n = min(cnt, th.N);
+  const bool penal = pen != 1.f && ctx > 0 && n > 0;
+  if (penal) {
+    const int words = (card + 31) >> 5;
+    for (int i = tid; i < words; i += SAMPLE_THREADS) bits[i] = 0u;
+    __syncthreads();
+    int taken = 0;                                      // window entries before this chunk (same value in every thread)
+    for (int base = 0; base < n && taken < ctx; base += SAMPLE_THREADS) {
+      const int j = base + tid;                         // the j-th newest entry
+      int t = -1;
+      if (j < n) t = th.ring[(long long)b * th.N + ((cnt - 1 - j) % th.N + th.N) % th.N];
+      const bool keep = j < n && t >= 0 && t < card && !text_special(t, card);
+      const unsigned bal = __ballot_sync(0xffffffffu, keep);
+      if ((tid & 31) == 0) s_warp[tid >> 5] = __popc(bal);
+      __syncthreads();
+      int before = taken;
+      for (int w = 0; w < (tid >> 5); ++w) before += s_warp[w];
+      before += __popc(bal & ((1u << (tid & 31)) - 1u));
+      if (keep && before < ctx) atomicOr(&bits[t >> 5], 1u << (t & 31));
+      for (int w = 0; w < SAMPLE_THREADS / 32; ++w) taken += s_warp[w];
+      __syncthreads();
+    }
+  }
+  const bf16* lg = logits + (long long)b * card;
+  float* sc = scores + (long long)b * card;
+  for (int i = tid; i < card; i += SAMPLE_THREADS) {
+    float l = bf2f(lg[i]);
+    if (penal && (bits[i >> 5] >> (i & 31)) & 1u) l = l >= 0.f ? l / pen : l * pen;
+    if (sampling) {
+      l = l / temp;
+      if (i == TEXT_PAD_ID && pad != 0.f) l += pad;
+    }
+    sc[i] = l;
+  }
+}
+
+// The text sampler on the adjusted scores, then the row's history: the token is appended when the row executed this step
+// (exec_mask null: every row did) and it is not a special id.
+static __global__ void __launch_bounds__(SAMPLE_THREADS) sample_text_kernel(const float* __restrict__ scores, const float* __restrict__ noise,
+                                                                     long long noise_ld, long long* __restrict__ out, int card,
+                                                                     int use_sampling, float temp, int top_k, const RowSampling* rs,
+                                                                     TextHistory th, const uint8_t* exec_mask) {
+  const int row = blockIdx.x;
+  row_sampling(rs, row, true, &temp, &top_k);
+  sample_row(scores + (long long)row * card, noise + (long long)row * noise_ld, out + row, card, use_sampling, temp, top_k);
+  if (threadIdx.x == 0 && (exec_mask == nullptr || exec_mask[row])) {
+    const int t = (int)out[row];
+    if (!text_special(t, card)) {
+      const int c = max(th.count[row], 0);           // a count from a state snapshot is not trusted to be in range
+      th.ring[(long long)row * th.N + c % th.N] = t;
+      th.count[row] = c + 1;
+    }
+  }
+}
+
+// b200_lm_reset: the masked rows' histories are emptied (null mask: all); their settings stay
+static __global__ void text_history_clear_kernel(int* count, const uint8_t* mask, int B) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b < B && (mask == nullptr || mask[b])) count[b] = 0;
+}
+
+// Host: b200_row_sampling -> the row's device settings; B200_ERR_INVALID outside the ranges of moshi_b200.h (top-k capped by
+// the handle's, whose top-k lays out the noise rows)
+inline int row_sampling_check(const b200_row_sampling& p, int top_k, int top_k_text, RowSampling* out, const char* what) {
+  const bool temps = std::isfinite(p.temp) && std::isfinite(p.temp_text) && p.temp >= 0.f && p.temp_text >= 0.f;
+  if (!temps) B200_FAIL(B200_ERR_INVALID, "%s: temperatures %g / %g (finite, >= 0)", what, p.temp_text, p.temp);
+  if (p.top_k < 1 || p.top_k > top_k || p.top_k_text < 1 || p.top_k_text > top_k_text)
+    B200_FAIL(B200_ERR_INVALID, "%s: top_k %d / top_k_text %d outside [1, %d] / [1, %d] (the handle's)", what, p.top_k, p.top_k_text,
+              top_k, top_k_text);
+  if (!std::isfinite(p.pad_mult)) B200_FAIL(B200_ERR_INVALID, "%s: pad_mult %g", what, p.pad_mult);
+  if (p.repetition_context < 0 || p.repetition_context > 1024)
+    B200_FAIL(B200_ERR_INVALID, "%s: repetition_context %d outside [0, 1024]", what, p.repetition_context);
+  if (!(p.repetition_penalty > 0.f && p.repetition_penalty <= 1000.f))
+    B200_FAIL(B200_ERR_INVALID, "%s: repetition_penalty %g outside (0, 1000]", what, p.repetition_penalty);
+  *out = RowSampling{p.temp_text, p.temp, (float)p.top_k_text, (float)p.top_k, p.pad_mult, (float)p.repetition_context,
+                     p.repetition_penalty, 1.f};
+  return B200_OK;
+}
+
+// Host: the text path of a session-sampling step on B rows: adjusted scores, then the sampler and the history
+inline void text_rows_launch(const bf16* logits, float* scores, const float* noise, long long noise_ld, long long* out, int B, int card,
+                             int use_sampling, float temp, int top_k, const RowSampling* rs, const TextHistory& th,
+                             const uint8_t* exec_mask, cudaStream_t st) {
+  B200_LAUNCH(text_adjust_kernel, B, SAMPLE_THREADS, 0, st, logits, scores, card, use_sampling, temp, rs, th);
+  B200_LAUNCH(sample_text_kernel, B, SAMPLE_THREADS, 0, st, scores, noise, noise_ld, out, card, use_sampling, temp, top_k, rs, th,
+              exec_mask);
 }
 
 }  // namespace lm

@@ -471,8 +471,38 @@ int b200_op_sample(const void* logits_bf16_dev, const float* noise_dev, int64_t*
   if (card + 1 > 65535 || top_k < 1 || top_k > SAMPLE_MAX_K) B200_FAIL(B200_ERR_SHAPE, "op_sample: bad card/top_k");
   const int k = top_k < card ? top_k : card;
   B200_LAUNCH(sample_kernel, B, SAMPLE_THREADS, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(logits_bf16_dev),
-              (long long)card, noise_dev, (long long)k, reinterpret_cast<long long*>(out_dev), card, use_sampling, temp, top_k);
+              (long long)card, noise_dev, (long long)k, reinterpret_cast<long long*>(out_dev), card, use_sampling, temp, top_k,
+              nullptr, 0);
   return check_launch("op_sample");
+}
+
+int b200_op_sample_text_rows(const void* logits_bf16_dev, const float* noise_dev, int64_t noise_ld, int64_t* out_dev, int B, int card,
+                             int use_sampling, float temp, int top_k, const b200_row_sampling* p, int32_t* history_dev,
+                             int32_t* count_dev, int history, void* stream) {
+  using namespace b200::lm;
+  const char* what = "op_sample_text_rows";
+  if (!logits_bf16_dev || !noise_dev || !out_dev || !history_dev || !count_dev || B < 1)
+    B200_FAIL(B200_ERR_INVALID, "%s: null pointer or B < 1", what);
+  if (card < 4 || card + 1 > 65535 || top_k < 1 || top_k > SAMPLE_MAX_K || history < 1 || history > 1024 || noise_ld < 1)
+    B200_FAIL(B200_ERR_SHAPE, "%s: bad card / top_k / history / noise_ld", what);
+  std::vector<RowSampling> rs(B, RowSampling{});
+  for (int b = 0; p && b < B; ++b) B200_TRY(row_sampling_check(p[b], top_k, top_k, &rs[b], what));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  RowSampling* rs_dev = nullptr;
+  float* scores = nullptr;
+  B200_CUDA(cudaMalloc(&rs_dev, (size_t)B * sizeof(RowSampling)));
+  if (cudaMalloc(&scores, (size_t)B * card * 4) != cudaSuccess) {
+    cudaFree(rs_dev);
+    B200_FAIL(B200_ERR_CUDA, "%s: out of device memory", what);
+  }
+  cudaMemcpyAsync(rs_dev, rs.data(), rs.size() * sizeof(RowSampling), cudaMemcpyHostToDevice, st);
+  text_rows_launch(static_cast<const bf16*>(logits_bf16_dev), scores, noise_dev, noise_ld, reinterpret_cast<long long*>(out_dev), B, card,
+                   use_sampling, temp, top_k, rs_dev, TextHistory{history_dev, count_dev, history}, nullptr, st);
+  const int rc = check_launch(what);
+  cudaStreamSynchronize(st);
+  cudaFree(scores);
+  cudaFree(rs_dev);
+  return rc;
 }
 
 }  // extern "C"

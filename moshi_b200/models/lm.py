@@ -27,7 +27,7 @@ from ..config import LMConfig
 from .state_dict import candle_refusal, normalize_lm_state_dict
 
 _TORCH_DTYPES = {_lib.B200_F32: torch.float32, _lib.B200_BF16: torch.bfloat16, _lib.B200_F16: torch.float16,
-                 _lib.B200_I64: torch.int64, _lib.B200_U8: torch.uint8}
+                 _lib.B200_I64: torch.int64, _lib.B200_U8: torch.uint8, _lib.B200_I32: torch.int32}
 
 
 def _config_struct(cfg: LMConfig) -> _lib.LMConfigC:
@@ -194,6 +194,9 @@ class LMGen:
         # a row takes pages as its fill grows and returns them on reset (None = one full ring per row).  Same numerics, bit for bit
         self.kv_pool_frames: int | None = None
         self.kv_page_slots = 64
+        # per-session sampling settings (set_session_sampling): the length of each session's text-history ring in [1, 1024], or
+        # None = every session samples with the handle-wide values above
+        self.session_sampling: int | None = None
 
     # ---- plumbing ---------------------------------------------------------------------------------
     def _device(self):
@@ -250,6 +253,7 @@ class LMGen:
             _lib.check(self._lib.b200_lm_set_kv_dtype(self._h, kinds[self.kv_dtype]))
             _lib.check(self._lib.b200_lm_set_kv_capacity(self._h, int(self.kv_capacity or 0)))
             _lib.check(self._lib.b200_lm_set_kv_pool(self._h, int(self.kv_pool_frames or 0), int(self.kv_page_slots)))
+            _lib.check(self._lib.b200_lm_set_session_sampling(self._h, int(self.session_sampling or 0)))
             until = None
             if self.cfg_coef != 1. and self.cfg_is_masked_until is not None:
                 until = (C.c_int64 * len(self.cfg_is_masked_until))(*[int(v) for v in self.cfg_is_masked_until])
@@ -323,6 +327,42 @@ class LMGen:
             self._sync_stream()
             _lib.check(self._lib.b200_lm_set_condition_cross(self._h, _lib.ptr(src), rows_c, n))
 
+    _ROW_SAMPLING = ("temp_text", "temp", "top_k_text", "top_k", "pad_mult", "repetition_context", "repetition_penalty")
+
+    def set_session_sampling(self, rows: tp.Sequence[int] | torch.Tensor, temp_text: float | None = None, temp: float | None = None,
+                             top_k_text: int | None = None, top_k: int | None = None, pad_mult: float | None = None,
+                             repetition_context: int | None = None, repetition_penalty: float | None = None) -> None:
+        """Gives sessions ``rows`` their own sampling settings (``session_sampling`` must be set before streaming).  A setting
+        left at None takes the handle-wide value (``temp_text``, ``temp``, ``top_k_text``, ``top_k`` of this LMGen; pad_mult 0,
+        repetition_context 0, repetition_penalty 1); all of them None returns the rows to the handle-wide values, which they then
+        follow as they change.  Text tokens: the rows' recent text (the newest ``repetition_context`` tokens of their history,
+        padding and initial tokens left out) is penalised, l / penalty where l >= 0 and l * penalty below, then a sampling row
+        samples at ``temp_text`` with ``pad_mult`` added to the padding token's tempered score, over its ``top_k_text``; a
+        greedy row takes the argmax of the penalised logits.  Audio tokens use ``temp`` and ``top_k``.  Top-k values must lie in
+        [1, this LMGen's]; ValueError outside the ranges, and nothing changes.  Ordered before the next step."""
+        assert self._batch is not None, "lm_gen is not streaming"
+        if not self.session_sampling:
+            raise RuntimeError("per-session sampling is off: set lm_gen.session_sampling before streaming")
+        rows = [int(r) for r in (rows.tolist() if isinstance(rows, torch.Tensor) else rows)]
+        for r in rows:
+            if not 0 <= r < self._batch:
+                raise ValueError(f"row {r} outside [0, {self._batch})")
+        vals = dict(temp_text=temp_text, temp=temp, top_k_text=top_k_text, top_k=top_k, pad_mult=pad_mult,
+                    repetition_context=repetition_context, repetition_penalty=repetition_penalty)
+        p = None
+        if any(v is not None for v in vals.values()):
+            for k in ("top_k_text", "top_k", "repetition_context"):
+                if vals[k] is not None and (isinstance(vals[k], bool) or int(vals[k]) != vals[k]):
+                    raise ValueError(f"{k} must be an integer, got {vals[k]!r}")
+            base = dict(temp_text=self.temp_text, temp=self.temp, top_k_text=self.top_k_text, top_k=self.top_k, pad_mult=0.0,
+                        repetition_context=0, repetition_penalty=1.0)
+            one = _lib.RowSamplingC(**{k: (base[k] if vals[k] is None else vals[k]) for k in self._ROW_SAMPLING})
+            p = (_lib.RowSamplingC * max(len(rows), 1))(*([one] * len(rows)))
+        rows_c = (C.c_int32 * max(len(rows), 1))(*rows)
+        with self._device():
+            self._sync_stream()
+            _lib.check(self._lib.b200_lm_set_row_sampling(self._h, rows_c, len(rows), p))
+
     def _entry_shape(self, name: str) -> tuple[int, ...]:
         for n, _, shape, _ in self._state_entries():
             if n == name:
@@ -370,6 +410,9 @@ class LMGen:
         state[""] = SimpleNamespace(batch_size=self._batch, device=self.lm_model.device, cache=raw["cache"], offsets=raw["offsets"],
                                     offset_cpu=offset_cpu, exec_mask=raw["exec_mask"].bool(),
                                     noise_counter=raw["noise_counter"])
+        if "session_sampling.params" in raw:          # per-session settings [B, 8], text histories [B, N] and their counts [B]
+            state[""].session_sampling = SimpleNamespace(params=raw["session_sampling.params"], history=raw["session_sampling.history"],
+                                                         count=raw["session_sampling.count"])
         mexec = raw.get("model.exec_mask", raw["exec_mask"]).bool()
         state["lm_model"] = SimpleNamespace(batch_size=self._model_batch, exec_mask=mexec)
         state["lm_model.transformer"] = SimpleNamespace(batch_size=self._model_batch, exec_mask=mexec, offsets=raw["model.offset"])
@@ -409,6 +452,11 @@ class LMGen:
             self._write_state("exec_mask", root.exec_mask.to(torch.uint8))
             if hasattr(root, "noise_counter"):
                 self._write_state("noise_counter", root.noise_counter.long())
+            if self.session_sampling:
+                ss = root.session_sampling
+                self._write_state("session_sampling.params", ss.params.float())
+                self._write_state("session_sampling.history", ss.history.int())
+                self._write_state("session_sampling.count", ss.count.int())
             _lib.check(self._lib.b200_lm_set_offset_cpu(self._h, int(root.offset_cpu)))
             tr = state.pop("lm_model.transformer")
             state.pop("lm_model")

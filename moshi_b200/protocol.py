@@ -16,6 +16,7 @@ samples for the tests and for clients that skip opus.  ``serve_aiohttp`` binds i
 from __future__ import annotations
 
 import json
+import math
 import struct
 import typing as tp
 from dataclasses import dataclass, field
@@ -107,6 +108,58 @@ def opus_codec(sample_rate: int = 24000):
         return RawPcmCodec(sample_rate), RawPcmCodec(sample_rate)
 
 
+# SessionConfigReq (rust/moshi-backend/src/stream_both.rs) query parameters -> the service's per-session settings
+SESSION_CONFIG_KEYS = {"text_temperature": ("temp_text", float), "text_topk": ("top_k_text", int), "audio_temperature": ("temp", float),
+                       "audio_topk": ("top_k", int), "pad_mult": ("pad_mult", float),
+                       "repetition_penalty_context": ("repetition_context", int), "repetition_penalty": ("repetition_penalty", float)}
+# MetaData field of each setting (the JSON the Rust server sends after the handshake)
+_METADATA_NAMES = {v[0]: k for k, v in SESSION_CONFIG_KEYS.items()}
+
+
+class SessionConfigError(ValueError):
+    """A malformed or out-of-range session setting in a connection's query."""
+
+
+def session_settings(config: tp.Mapping[str, tp.Any], defaults: tp.Mapping[str, tp.Any], history: int) -> dict[str, tp.Any]:
+    """Every setting of a session from its ``SessionConfigReq`` (query strings or numbers): a missing key takes the handle-wide
+    value (``defaults``: temp_text, temp, top_k_text, top_k; pad_mult 0, repetition_context 0, repetition_penalty 1), top-k
+    values are clamped to the handle's and the repetition context to ``history`` (the tokens each session's history holds),
+    unknown keys are ignored (max_steps, the seeds, email, ...).  SessionConfigError for a malformed value, a negative
+    temperature or top-k below 1, a repetition context outside [0, 1024] or a penalty outside (0, 1000]."""
+    out = dict(temp_text=float(defaults["temp_text"]), temp=float(defaults["temp"]), top_k_text=int(defaults["top_k_text"]),
+               top_k=int(defaults["top_k"]), pad_mult=0.0, repetition_context=0, repetition_penalty=1.0)
+    for key, (name, kind) in SESSION_CONFIG_KEYS.items():
+        if key not in config or config[key] is None:
+            continue
+        raw = config[key]
+        try:
+            if isinstance(raw, bool) or (kind is int and isinstance(raw, float) and not raw.is_integer()):
+                raise ValueError
+            v = kind(raw.strip() if isinstance(raw, str) else raw)
+        except (TypeError, ValueError):
+            raise SessionConfigError(f"{key}: malformed value {raw!r}") from None
+        if kind is float and not math.isfinite(v):
+            raise SessionConfigError(f"{key}: {raw!r} is not finite")
+        out[name] = v
+    if out["temp_text"] < 0 or out["temp"] < 0:
+        raise SessionConfigError("temperatures must be >= 0")
+    if out["top_k_text"] < 1 or out["top_k"] < 1:
+        raise SessionConfigError("top-k values must be >= 1")
+    if not 0 <= out["repetition_context"] <= 1024:
+        raise SessionConfigError(f"repetition_penalty_context {out['repetition_context']} outside [0, 1024]")
+    if not 0 < out["repetition_penalty"] <= 1000:
+        raise SessionConfigError(f"repetition_penalty {out['repetition_penalty']} outside (0, 1000]")
+    out["top_k_text"] = min(out["top_k_text"], int(defaults["top_k_text"]))
+    out["top_k"] = min(out["top_k"], int(defaults["top_k"]))
+    out["repetition_context"] = min(out["repetition_context"], int(history))
+    return out
+
+
+def session_metadata(settings: tp.Mapping[str, tp.Any]) -> dict[str, tp.Any]:
+    """The effective settings under the Rust server's ``MetaData`` field names."""
+    return {_METADATA_NAMES[k]: v for k, v in settings.items()}
+
+
 @dataclass
 class Connection:
     slot: int
@@ -114,6 +167,7 @@ class Connection:
     writer: tp.Any
     outbox: list[bytes] = field(default_factory=list)
     frames_out: int = 0
+    settings: dict | None = None       # the session's own sampling settings (connect(config)), None = the service-wide values
 
 
 class FrontEnd:
@@ -128,6 +182,7 @@ class FrontEnd:
         self.model_version = model_version
         self.codec_factory = codec_factory or opus_codec
         self.connections: dict[int, Connection] = {}
+        self._own_settings: set[int] = set()     # slots the service samples with a connection's own settings
         B = batch_size
         self._pcm_in = np.zeros(B * frame_size, dtype=np.float32)
         self._updates = np.zeros(B, dtype=np.int32)
@@ -136,13 +191,38 @@ class FrontEnd:
         self._flags = np.zeros(B, dtype=np.uint8)
 
     # ---- connection lifecycle (server.py:154-190: handshake first, then the receive loop) --------------------------------------
-    def connect(self) -> Connection:
+    def connect(self, config: tp.Mapping[str, tp.Any] | None = None) -> Connection:
+        """A new connection on a free slot.  ``config``: the connection's ``SessionConfigReq`` (e.g. the websocket URL's query):
+        on a service with per-session sampling (``DialogueService(session_sampling=N)``) the slot samples with those settings
+        (``session_settings``) and the outbox gets an ``MT_METADATA`` message with the effective values after the handshake;
+        SessionConfigError for a bad value, with no slot taken.  A service without it ignores the config, as it always did.
+        Without a config a slot that a previous connection gave settings returns to the service-wide values."""
+        history = int(getattr(self.service, "session_sampling", None) or 0)
+        settings = None
+        if config is not None and history > 0:
+            settings = session_settings(config, self.service.sampling_defaults, history)
         slot = self.pool.open()            # raises RuntimeError when every slot is taken
         reader, writer = self.codec_factory()
-        conn = Connection(slot, reader, writer)
+        conn = Connection(slot, reader, writer, settings=settings)
+        try:
+            self._apply_settings(conn)
+        except BaseException:
+            self.pool.close(slot)          # a refused connection gives its slot back
+            raise
         conn.outbox.append(encode_message(Message(MT_HANDSHAKE, (PROTOCOL_VERSION, self.model_version))))   # server.py:167
+        if settings is not None:
+            conn.outbox.append(encode_message(Message(MT_METADATA, session_metadata(settings))))
         self.connections[slot] = conn
         return conn
+
+    def _apply_settings(self, conn: Connection) -> None:
+        """The connection's settings onto its slot, every field of them, so that a slot never keeps a previous session's."""
+        if conn.settings is not None:
+            self.service.set_session_sampling(conn.slot, **conn.settings)
+            self._own_settings.add(conn.slot)
+        elif conn.slot in self._own_settings:
+            self.service.set_session_sampling(conn.slot)
+            self._own_settings.discard(conn.slot)
 
     def disconnect(self, conn: Connection) -> None:
         if conn.slot in self.connections:
@@ -165,6 +245,7 @@ class FrontEnd:
             if slot != conn.slot:
                 self.connections[slot] = self.connections.pop(conn.slot)
                 conn.slot = slot
+                self._apply_settings(conn)          # the connection keeps its settings on its new slot
         # handshake / text / metadata / ping from the client carry nothing the model consumes
 
     # ---- one 80 ms tick --------------------------------------------------------------------------------------------------------
@@ -203,8 +284,10 @@ async def serve_aiohttp(front: FrontEnd, host: str = "localhost", port: int = 89
         ws = web.WebSocketResponse()
         await ws.prepare(request)
         try:
-            conn = front.connect()
-        except RuntimeError as e:
+            # SessionConfigReq in the query string (the web client's sliders): no setting key, no per-session settings
+            config = {k: v for k, v in request.query.items() if k in SESSION_CONFIG_KEYS}
+            conn = front.connect(config or None)
+        except (RuntimeError, SessionConfigError) as e:
             await ws.send_bytes(encode_message(Message(MT_ERROR, str(e))))
             await ws.close()
             return ws

@@ -85,18 +85,22 @@ class DialogueService:
 
     def __init__(self, batch_size: int, lm, mimi, use_sampling: bool = True, temp: float = 0.8, temp_text: float = 0.7,
                  top_k: int = 250, top_k_text: int = 25, kv_dtype: str = "bf16", kv_capacity: int | None = None,
-                 kv_pool_frames: int | None = None):
+                 kv_pool_frames: int | None = None, session_sampling: int | None = None):
         import ctypes as C
 
         from . import _lib
         from .models import LMGen
         self.batch_size = batch_size
+        # the handle-wide values a session's missing settings take (protocol.FrontEnd.connect)
+        self.sampling_defaults = dict(temp_text=temp_text, temp=temp, top_k_text=top_k_text, top_k=top_k)
+        self.session_sampling = session_sampling    # tokens of text history per session, or None: no per-session settings
         self.lm, self.mimi = lm, mimi
         self.lm_gen = LMGen(lm, use_sampling=use_sampling, temp=temp, temp_text=temp_text, top_k=top_k, top_k_text=top_k_text,
                             support_out_of_sync=True)
         self.lm_gen.kv_dtype = kv_dtype
         self.lm_gen.kv_capacity = kv_capacity
         self.lm_gen.kv_pool_frames = kv_pool_frames
+        self.lm_gen.session_sampling = session_sampling
         self.lm_gen.streaming_forever(batch_size)
         self.mimi.streaming_forever(batch_size)
         self._lib = _lib.lib()
@@ -125,6 +129,12 @@ class DialogueService:
         if mask.any():
             self.lm_gen.reset_streaming(mask)
             self.mimi.reset_streaming(mask)
+
+    def set_session_sampling(self, slot: int, **settings) -> None:
+        """Session ``slot``'s own sampling settings (``LMGen.set_session_sampling``; the service was built with
+        ``session_sampling``); none given returns it to the service-wide values.  They apply from the next ``step`` on and
+        stay across that slot's RESET frames until they are set again."""
+        self.lm_gen.set_session_sampling([slot], **settings)
 
     def export_session(self, slot: int) -> "SessionRecord":
         """The LM and Mimi state of session ``slot`` as device records (``LMGen.export_session``, ``MimiModel.export_session``).
